@@ -1,9 +1,10 @@
 #!/usr/bin/env python3
-"""Benchmark of the NR-NeRF render hot path on B200 (driver contract: see the task statement).
+"""Benchmark of the NR-NeRF render hot path on one or more H100s.
 
     python bench.py --gpus N --steps K --warmup W                  # this framework, BASELINE configs[1] per GPU
     python bench.py --impl reference --gpus N --steps K ...        # the reference's own CPU path on the host cores
     python bench.py --workload cfg4|render|sweep ...               # the other BASELINE configs (see below)
+    python bench.py ... --dump-outputs DIR                         # also write the last timed step's results as .npy
 
 Default workload (BASELINE.json configs[1]): one training step of configs/example_sequence.txt -- N_rand = 1024 rays per
 GPU, 64 coarse + 128 fine network evaluations per ray, 8x256 MLP, ray bending on, perturb = 1, raw_noise_std = 1,
@@ -25,6 +26,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import types
 
 import numpy as np
@@ -66,18 +68,31 @@ def synth_batch(rs, n, n_images=86):
 
 
 def read_peaks():
+    """Roofline denominators: NVIDIA's H100 SXM data sheet (dense fp16 tensor rate, HBM3 bandwidth, 700 W card; a ceiling,
+    not a measured rate), each replaced by the measured value where MEASURED_PEAKS.json provides one."""
+    peaks = {"tf_burst": 989.0, "tf_sustained": 989.0, "hbm_gbs": 3350.0}
+    measured = []
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
-        return {"tf_burst": float(d.get("bf16_tflops", 1590.0)), "tf_sustained": float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1400.0))),
-                "hbm_gbs": float(d.get("hbm_gbs", 6500.0)), "source": "measured (MEASURED_PEAKS.json: cuBLAS bf16 burst / sustained, copy bandwidth)"}
-    return {"tf_burst": 1590.0, "tf_sustained": 1400.0, "hbm_gbs": 6500.0, "source": "fallback (B200_PROFILING.md figures)"}
+        for key, names in (("tf_burst", ("bf16_tflops",)), ("tf_sustained", ("bf16_tflops_sustained", "bf16_tflops")),
+                           ("hbm_gbs", ("hbm_gbs",))):
+            for name in names:
+                if name in d:
+                    peaks[key] = float(d[name])
+                    measured.append(key)
+                    break
+    rest = [k for k in peaks if k not in measured]
+    peaks["source"] = "; ".join(x for x in (
+        f"measured (MEASURED_PEAKS.json): {', '.join(measured)}" if measured else "",
+        f"H100 SXM data sheet (not measured): {', '.join(rest)}" if rest else "") if x)
+    return peaks
 
 
 class ClockSampler:
     def __init__(self, dev_index):
-        self.path = f"/tmp/nrn_clocks_{os.getpid()}.csv"
+        self.path = os.path.join(tempfile.gettempdir(), f"nrn_clocks_{os.getpid()}.csv")
         q = "clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
         try:
@@ -146,7 +161,7 @@ def cpu_baseline(n_rays, steps, warmup):
 def run_reference_arm(args, rank):
     if rank != 0:
         return
-    steps = max(1, min(args.steps, 8))      # ~1.5 s per 1024-ray step on the box's cores: bounded to a few minutes
+    steps = max(1, args.steps)              # a 1024-ray step takes seconds on CPU cores: choose --steps accordingly
     cb = cpu_baseline(args.n_rand, steps, min(args.warmup, 2))
     line = {"impl": "reference", "metric": METRIC, "value": cb["value"], "unit": "rays/s", "n_gpus": args.gpus, "steps": steps,
             "warmup": min(args.warmup, 2), "ms_per_step": cb["seconds_per_step"] * 1e3, "higher_is_better": True, "scaling": "weak",
@@ -204,17 +219,6 @@ def roofline_block(per_step, n_rand, peaks, traffic):
     return roof
 
 
-def read_traffic():
-    for name in ("r02_traffic.json", "r01_traffic.json"):
-        p = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(p):
-            with open(p) as f:
-                d = json.load(f)
-            d["_source"] = "profiles/" + name
-            return d
-    return None
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -229,7 +233,12 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="run the step eagerly instead of replaying a CUDA graph")
     ap.add_argument("--no-breakdown", action="store_true", help="skip the instrumented per-kernel pass")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (its loss, the parameters and latent codes after its Adam "
+                         "update) to DIR/<name>.npy, float32, for comparing two builds on identical inputs")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or args.workload not in ("train", "cfg4")):
+        ap.error("--dump-outputs writes the outputs of the training-step workloads (train, cfg4) of this implementation only")
     args.warmup = max(args.warmup, 3)
     if args.n_rand is None:
         args.n_rand = 8192 if args.workload == "cfg4" else N_RAND
@@ -305,7 +314,7 @@ def main():
 
     def local_step(rays_o, rays_d, target, idx):
         """One iteration on this rank's rows: forward, per-ray loss, backward of the GLOBAL mean (train.py:1606-1607),
-        gradient reduction + Adam, and the per-ray losses of all ranks for the caller's log line."""
+        gradient reduction + Adam, and (their mean, the per-ray losses of all ranks) for the caller."""
         optimizer.zero_grad()                                    # one memset over the gradient arena
         losses = local_module(targs, rays_o, rays_d, 100, render_kwargs_train, target, global_step, 0, dataset_extras, idx)
         (losses.sum() / n_global).backward()
@@ -313,7 +322,7 @@ def main():
             optimizer.step()                                     # 1 GPU: Adam; N GPUs: peer reduce + Adam, same launch
             gathered = peer_red.gather_rows(losses) if peer_red is not None else losses.detach()
             global_step.add_(1.0)
-            return gathered.mean()
+            return gathered.mean(), gathered
         return losses.detach()
 
     graphed = None
@@ -335,13 +344,13 @@ def main():
         optimizer.set_lr(lrate * (0.1 ** (iteration[0] / (lrate_decay * 1000))))   # per-iteration decay of train.py:1631-1642
         out = graphed(*batch) if graphed is not None else local_step(*batch)
         if fused_collectives:
-            return out
+            return out      # (mean loss, per-ray losses)
         # NCCL reducer: collectives outside the graph -- in-place arena all-reduce + Adam, then the loss all-gather
         optimizer.step()
         global_step.add_(1.0)
         gathered = torch.empty(world * (hi - lo), dtype=out.dtype, device=dev)
         dist.all_gather_into_tensor(gathered, out.contiguous())
-        return gathered.mean()
+        return gathered.mean(), gathered
 
     def barrier():
         if world > 1:
@@ -349,30 +358,43 @@ def main():
         torch.cuda.synchronize()
 
     def timed(loop_steps, e2e):
+        """(elapsed ms, the last step's (mean loss, per-ray losses))"""
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
+        loss = None
         for i in range(loop_steps):
             if e2e:
                 # host -> device copy of this step's inputs from pinned memory (straight into the graph's input buffers)
                 loss = step(pinned[i % pool] if graphed is not None else upload(pinned[i % pool]))
-                loss.item()                              # device -> host read of the step's result
+                loss[0].item()                           # device -> host read of the step's result
             else:
-                step(resident[i % pool])
+                loss = step(resident[i % pool])
         e1.record()
         barrier()
         ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
         if world > 1:
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
-        return float(ms.item())
+        return float(ms.item()), loss
 
     for i in range(args.warmup):
         step(resident[i % pool])
     _lib.device_error_check()
 
     sampler = ClockSampler(local_rank) if rank == 0 else None
-    ms_total = timed(args.steps, e2e=False)      # headline: the plain step (no instrumentation inside the graph)
-    ms_e2e = timed(args.steps, e2e=True)
+    ms_total, last_loss = timed(args.steps, e2e=False)      # headline: the plain step (no instrumentation inside the graph)
+    dump = None
+    if args.dump_outputs:
+        # the caller of a training step receives its per-ray losses and the updated parameters: snapshot them before any
+        # further step
+        dump = {"loss": last_loss[0].detach().float().cpu().numpy(), "per_ray_loss": last_loss[1].detach().float().cpu().numpy()}
+        for prefix, mod in (("coarse", coarse), ("fine", fine), ("bender", bender)):
+            for name, prm in mod.named_parameters():
+                if prefix != "bender" and name.startswith("ray_bender."):
+                    continue      # the NeRF modules hold a reference to the shared bender
+                dump[f"{prefix}.{name}"] = prm.detach().float().cpu().numpy()
+        dump["latents"] = torch.stack([z.detach() for z in latents]).float().cpu().numpy()
+    ms_e2e, _ = timed(args.steps, e2e=True)
     clocks = sampler.stop() if sampler else None
     # per-kernel breakdown: the same K steps once more with CUDA event records around every launch of this repo's
     # kernels (external event-record nodes inside the re-captured graph; they cost a few us per step themselves)
@@ -381,13 +403,18 @@ def main():
     # graph with event-record nodes in between is not something this bench needs -- the per-kernel breakdown is a per-GPU
     # quantity, reported by the N = 1 and NCCL runs)
     if not args.no_breakdown and peer_red is None:
+        plain = graphed
         _lib.timing_enable(True)
         if graphed is not None:
             graphed = GraphedStep(local_step, resident[0], warmup=1)
             for i in range(3):
                 step(resident[i % pool])
-        ms_instrumented = timed(args.steps, e2e=False)
+        ms_instrumented, _ = timed(args.steps, e2e=False)
         kinds = _lib.timing_read()
+        # the instrumented graph's event-record nodes refer to the library's timing events: release the graph before the
+        # events, and take the final step with the plain graph
+        graphed = plain
+        torch.cuda.synchronize()
         _lib.timing_enable(False)
         # launches per step: forward / DGRAD / composite / composite backward 2 (coarse + fine), divergence 2 (fwd + bwd),
         # WGRAD 3 (fine, coarse, divergence; each followed by its split reduction, timed with it)
@@ -395,7 +422,11 @@ def main():
         per_step = {k: (kinds[k][0] / (kinds[k][1] / float(launches.get(k, 2))) if kinds[k][1] else 0.0) for k in kinds}
     _lib.device_error_check()
 
-    final_loss = float(step(resident[0]).item())
+    final_loss = float(step(resident[0])[0].item())
+    if dump is not None and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in dump.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), np.asarray(arr, dtype=np.float32))
     if peer_red is not None:
         peer_red.close()
     if world > 1:
@@ -407,10 +438,7 @@ def main():
     value = n_global * args.steps / (ms_total * 1e-3)
     e2e_value = n_global * args.steps / (ms_e2e * 1e-3)
     peaks = read_peaks()
-    traffic = read_traffic() if args.n_rand == N_RAND else None
-    roof = roofline_block(per_step, args.n_rand, peaks, traffic)
-    if traffic:
-        roof["traffic_source"] = traffic.get("_source")
+    roof = roofline_block(per_step, args.n_rand, peaks, None)
     step_tf = 3 * args.n_rand * POINTS_PER_RAY * FLOP_PER_POINT / (ms_total / args.steps * 1e-3) / 1e12
     line = {
         "metric": METRIC, "value": value, "unit": "rays/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
@@ -419,11 +447,10 @@ def main():
         "config": {"workload": workload_text(args.n_rand),
                    "parallelism": f"ray-sharded x{world}; gradient reduction: {reducer_note}",
                    "inputs": "every rank draws the global batch from the shared seed and uploads its own row block from pinned memory",
-                   "l2": "per-step working set (activation + gradient stash, ~1.9 GB at 1024 rays) exceeds the 126 MB L2; 8 rotating input batches"},
+                   "l2": "per-step working set (activation + gradient stash, ~1.9 GB at 1024 rays) exceeds the 50 MB L2; 8 rotating input batches"},
         "e2e": {"value": e2e_value, "unit": "rays/s", "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": 4},
         "gpu_launches": (32 if world == 1 else 36) * args.steps,
-        # this repo's kernels per step, counted in profiles/r02_launches_step.csv (32 of the step's 63 launches, 94 % of its GPU
-        # time): 3 weight packs, 1 coarse sampler, 2 field forwards, 2 composites, 1 ray loss + 4 scalings, 3 divergence, 2
+        # this repo's kernels per step: 3 weight packs, 1 coarse sampler, 2 field forwards, 2 composites, 1 ray loss + 4 scalings, 3 divergence, 2
         # composite backwards, 4 absmax, 2 field DGRADs, 3 WGRADs + 3 reductions, 2 optimizer (N GPUs: 3 peer reduce + Adam and
         # 3 loss-gather launches instead of the 2 optimizer launches)
         "kernel_ms_per_step": per_step, "ms_per_step_instrumented": (ms_instrumented / args.steps) if ms_instrumented else None,

@@ -1,4 +1,4 @@
-/* nrnerf_b200 -- C ABI of the B200-native NR-NeRF render hot path (libnrnerf_b200.so).
+/* nrnerf_b200 -- C ABI of the H100-native (sm_90a) NR-NeRF render hot path (libnrnerf_b200.so).
  *
  * Plain C: raw device pointers, sizes, a cudaStream_t passed as void*.  No torch types, no C++
  * types, no exceptions.  Every function returns 0 on success or a negative NRN_E_* code; the
@@ -34,7 +34,7 @@ const char* nrn_last_error(void);
 int nrn_device_error(int* code_out);
 
 /* ---- weight packing -------------------------------------------------------------------------
- * fp32 nn.Linear tensors in the reference's checkpoint layout ([out][in] row-major) -> fp16 UMMA
+ * fp32 nn.Linear tensors in the reference's checkpoint layout ([out][in] row-major) -> fp16 wgmma
  * operand images.  Replaces nothing in the reference (derived data); sources are
  * NeRF.pts_linears / output_linear (run_nerf_helpers.py:218-238) and ray_bending.network /
  * rigidity_network (run_nerf_helpers.py:411-482). */
@@ -299,7 +299,9 @@ int nrn_peer_gather_rows(const NrnPeerCtx* ctx, const float* local, int n_per_ra
 /* ---- optional per-kernel timing (measurement aid for bench.py) ---------------------------------
  * While enabled, every launch of the kernel kinds below is bracketed by CUDA events recorded on the
  * launch stream.  kinds: 0 field forward, 1 field DGRAD, 2 WGRAD (+reduce), 3 composite(+resample),
- * 4 composite backward, 5 divergence regulariser.  nrn_timing_read synchronises the recorded events and returns per-kind sums. */
+ * 4 composite backward, 5 divergence regulariser.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
+ * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);
 int nrn_timing_read(double* ms_sum, int* counts, int n_kinds);
 

@@ -1,4 +1,4 @@
-"""nonrigid_nerf_b200 -- B200-native (sm_100a) implementation of NR-NeRF's per-ray volumetric
+"""nonrigid_nerf_b200 -- H100-native (sm_90a) implementation of NR-NeRF's per-ray volumetric
 rendering hot path behind the reference's Python entry points.  See DESIGN.md / INTEGRATION.md."""
 from . import _lib  # noqa: F401
 

@@ -188,7 +188,7 @@ def load() -> C.CDLL:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"nonrigid_nerf_b200: CUDA extension not found at {LIB_PATH}. There is no CPU/PyTorch fallback; "
-                "build it with `make -C nonrigid_nerf_b200/csrc` (needs nvcc, sm_100a).")
+                "build it with `make -C nonrigid_nerf_b200/csrc` (needs nvcc, sm_90a).")
         lib = C.CDLL(LIB_PATH)
         for name, (res, args) in SYMBOLS.items():
             fn = getattr(lib, name)  # AttributeError => symbol missing => broken build

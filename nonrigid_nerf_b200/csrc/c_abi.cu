@@ -51,7 +51,8 @@ int device_state(DeviceState** out) {
     cudaDeviceProp prop;
     e = cudaGetDeviceProperties(&prop, dev);
     if (e != cudaSuccess) return cuda_fail(e, "cudaGetDeviceProperties");
-    if (prop.major != 10) return fail(NRN_E_INVALID, "nrnerf_b200 needs an sm_100 GPU, found sm_%d%d", prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)
+      return fail(NRN_E_INVALID, "nrnerf_b200 is built for sm_90a (H100) only, found sm_%d%d", prop.major, prop.minor);
     s.num_sms = prop.multiProcessorCount;
     if (const char* g = getenv("NRN_GRID")) { const int v = atoi(g); if (v > 0 && v < s.num_sms) s.num_sms = v; }   // developer experiments
     e = cudaMalloc(&s.err_word, 4 * sizeof(int));
@@ -230,7 +231,6 @@ int nrn_field_forward(const NrnFieldArgs* a) {
   p.raw = a->raw; p.d_init = a->initial_input_pts; p.d_bent = a->input_pts; p.d_unmasked = a->unmasked_offsets;
   p.d_masked = a->masked_offsets; p.d_rigid = a->rigidity_mask;
   p.stash = static_cast<uint8_t*>(a->stash);
-  { const char* dm = getenv("NRN_DEBUG_MODE"); p.debug_mode = dm ? atoi(dm) : 0; }
   if (a->stash && a->points) return fail(NRN_E_INVALID, "nrn_field_forward: the training stash needs ray mode");
   p.err = ds->err_word;
   cudaError_t e;
@@ -283,7 +283,7 @@ int nrn_composite_backward(const NrnCompositeBwdArgs* a) {
 static long long even_tiles(int n_rays, int n_samples) {
   const long long P = static_cast<long long>(n_rays) * n_samples;
   const long long tiles = (P + nrn::kTileM - 1) / nrn::kTileM;
-  return (tiles + 1) & ~1LL;   // the kernels work on tile pairs (two slots per CTA)
+  return (tiles + 1) & ~1LL;   // rounded up to an even count: the stash layout of ABI version 2
 }
 size_t nrn_stash_bytes(int n_rays, int n_samples) { return static_cast<size_t>(even_tiles(n_rays, n_samples)) * nrn::kStashTileBytes; }
 size_t nrn_grad_stash_bytes(int n_rays, int n_samples) { return static_cast<size_t>(even_tiles(n_rays, n_samples)) * nrn::kGradTileBytes; }
@@ -571,9 +571,13 @@ int nrn_peer_gather_rows(const NrnPeerCtx* c, const float* local, int n_per_rank
   return e == cudaSuccess ? NRN_OK : cuda_fail(e, "peer_collect_kernel");
 }
 
+// Turning timing off only stops recording: a CUDA graph captured while it was on keeps event-record nodes that refer to
+// these events and may still be replayed.  They are released when a new timing session starts.
 int nrn_timing_enable(int on) {
-  for (int i = 0; i < g_timed_n; ++i) { cudaEventDestroy(g_timed[i].a); cudaEventDestroy(g_timed[i].b); }
-  g_timed_n = 0;
+  if (on) {
+    for (int i = 0; i < g_timed_n; ++i) { cudaEventDestroy(g_timed[i].a); cudaEventDestroy(g_timed[i].b); }
+    g_timed_n = 0;
+  }
   g_timing = on != 0;
   return NRN_OK;
 }

@@ -5,8 +5,8 @@
 // layer's pre-activation ("dY_l"), the per-ray latent gradient, and -- through the gradient stash --
 // the inputs of the weight-gradient kernel (wgrad.cu).  SURVEY.md appendix C is the specification.
 //
-// Same machine as field_fwd.cu: persistent CTA, two 128-point slots ping-ponging between a
-// tcgen05.mma issuer and two epilogue warpgroups, weights (here W^T images) streamed by bulk TMA.
+// Same machine as field_fwd.cu (field_mma.cuh): persistent CTA over 128-point tiles, two consumer
+// warpgroups (wgmma + epilogue, 64 rows each), weights (here W^T images) streamed by bulk TMA.
 //   step  0      head^T   dh8 = d_raw . Wout          -> dY7 = dh8 * [h8 > 0]
 //   steps 1,2    L7^T,L6^T                            -> dY6, dY5
 //   step  3      L5e^T    dE  = dY5 . W5[:, :63]      -> PE backward -> d(bent xyz)
@@ -16,22 +16,17 @@
 //   step  14     B0^T     d(bender input)             -> per-ray latent gradient (fp32 atomics)
 // All gradients travel in fp16 scaled by a power-of-two loss scale derived on the device from
 // max|d_raw| (no host sync); WGRAD and the latent reduction divide it out again in fp32.
-#include "nrn_common.cuh"
-#include "sm100_ptx.cuh"
+#include "field_mma.cuh"
 
 namespace nrn {
 
 namespace {
 
-constexpr long long kWaitLimitCycles = 1ll << 28;
-constexpr int kBwdRingStages = 3;
+constexpr int kBwdStageLd = 66;   // floats per staged row (64 used)
 
 struct Shared {
-  uint64_t w_full[kBwdRingStages];
-  uint64_t w_empty[kBwdRingStages];
-  uint64_t a_ready[2];
-  uint64_t d_full[2];
-  uint32_t tmem_base;
+  uint64_t w_full[kRingStages];
+  uint64_t w_empty[kRingStages];
   int abort_flag;
 };
 
@@ -53,57 +48,34 @@ __device__ __forceinline__ StepShape step_shape(int step) {
   }
 }
 
-struct Waiter {
-  int* s_abort;
-  int* g_err;
-  __device__ __forceinline__ bool wait(uint64_t* bar, uint32_t parity, int code) const {
-    if (mbar_try_wait(bar, parity)) return true;
-    const long long t0 = clock64();
-    while (!mbar_try_wait(bar, parity)) {
-      if (*reinterpret_cast<volatile int*>(s_abort)) return false;
-      if (clock64() - t0 > kWaitLimitCycles) {
-        atomicExch(s_abort, code);
-        atomicCAS(g_err, 0, code);
-        return false;
-      }
-    }
-    return true;
-  }
-};
-
 __device__ __forceinline__ float clamp_h(float v) { return fminf(fmaxf(v, -65504.f), 65504.f); }
 
-// dY = dh * [h > 0]: drain NCOLS accumulator columns, mask with the forward activation stashed as
-// fp16 (row pointer `mask_row` into the stash tile), write fp16 to the next A operand (smem); the whole
-// image then goes to the gradient stash with a bulk TMA store (stash_store in the kernel body).
-template <int NCOLS>
-__device__ __forceinline__ void epi_mask_store(uint32_t taddr, const uint8_t* __restrict__ mask_row,
-                                               uint8_t* dst_row) {
-  // software pipeline: TMEM load of chunk c+1 and mask loads of chunk c overlap the processing
-  constexpr int NC = NCOLS / 32;
-  uint32_t v[2][32];
-  tmem_ld32(taddr, v[0]);
+// dY = dh * [h > 0]: accumulator columns [0, NCOLS), masked with the forward activation stashed as fp16 (`mask_img`:
+// the tile's stash image), written as fp16 to this warpgroup's rows of the next A operand `img`; the whole image then
+// goes to the gradient stash with bulk TMA stores.
+template <int NCOLS, int NR>
+__device__ __forceinline__ void epi_mask_store(const float (&acc)[NR], const uint8_t* __restrict__ mask_img, uint8_t* img, int g) {
+  const int r0 = g * kWgRows + acc_r0(), q = acc_q();
+  constexpr int kBlk = NCOLS / 8 < 8 ? NCOLS / 8 : 8;   // column groups whose mask loads are in flight together
 #pragma unroll
-  for (int c = 0; c < NC; ++c) {
-    uint4 m[4];
+  for (int j0 = 0; j0 < NCOLS / 8; j0 += kBlk) {
+    uint32_t m[kBlk][2];
 #pragma unroll
-    for (int q = 0; q < 4; ++q) m[q] = __ldg(reinterpret_cast<const uint4*>(mask_row + (c * 4 + q) * kChunkBytes));
-    tmem_ld_wait();
-    if (c + 1 < NC) tmem_ld32(taddr + (c + 1) * 32, v[(c + 1) & 1]);
-    const uint32_t(&w)[32] = v[c & 1];
+    for (int jj = 0; jj < kBlk; ++jj)
 #pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const uint32_t mw[4] = {m[q].x, m[q].y, m[q].z, m[q].w};
-      uint32_t o[4];
+      for (int i = 0; i < 2; ++i)
+        m[jj][i] = __ldg(reinterpret_cast<const unsigned int*>(mask_img + (j0 + jj) * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q));
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        // dY = dh * [h > 0] on packed halves: saturating convert, then multiply by the 0/1 mask of the stashed h
-        const uint32_t g2 = pack_h2_sat(__uint_as_float(w[q * 8 + 2 * j]), __uint_as_float(w[q * 8 + 2 * j + 1]));
-        const __half2 hm = __hgt2(*reinterpret_cast<const __half2*>(&mw[j]), __float2half2_rn(0.f));
+    for (int jj = 0; jj < kBlk; ++jj) {
+      const int j = j0 + jj;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        // saturating convert, then multiply by the 0/1 mask of the stashed h on packed halves
+        const uint32_t g2 = pack_h2_sat(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+        const __half2 hm = __hgt2(*reinterpret_cast<const __half2*>(&m[jj][i]), __float2half2_rn(0.f));
         const __half2 r2 = __hmul2(*reinterpret_cast<const __half2*>(&g2), hm);
-        o[j] = *reinterpret_cast<const uint32_t*>(&r2);
+        *reinterpret_cast<uint32_t*>(img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = *reinterpret_cast<const uint32_t*>(&r2);
       }
-      *reinterpret_cast<uint4*>(dst_row + (c * 4 + q) * kChunkBytes) = make_uint4(o[0], o[1], o[2], o[3]);
     }
   }
 }
@@ -112,20 +84,8 @@ __device__ __forceinline__ float h_lo(uint32_t w) { return __half2float(__ushort
 __device__ __forceinline__ float h_hi(uint32_t w) { return __half2float(__ushort_as_half(static_cast<unsigned short>(w >> 16))); }
 
 // Backward of the positional encoding: dx_d += dE[d] + sum_k 2^k (dE[sin_kd] cos_kd - dE[cos_kd] sin_kd)
-// dE: 64 accumulator columns of this row; sin/cos: the forward embedding stashed as fp16.
-__device__ __forceinline__ void pe_backward(uint32_t taddr, const uint8_t* __restrict__ e_row, float (&dx)[3]) {
-  float de[64];
-  {
-    uint32_t v[32];
-    tmem_ld32(taddr, v);
-    tmem_ld_wait();
-#pragma unroll
-    for (int i = 0; i < 32; ++i) de[i] = __uint_as_float(v[i]);
-    tmem_ld32(taddr + 32, v);
-    tmem_ld_wait();
-#pragma unroll
-    for (int i = 0; i < 32; ++i) de[32 + i] = __uint_as_float(v[i]);
-  }
+// de: this row's 64 staged accumulator columns; sin/cos: the forward embedding stashed as fp16.
+__device__ __forceinline__ void pe_backward(const float* de, const uint8_t* __restrict__ e_row, float (&dx)[3]) {
   float e[64];
 #pragma unroll
   for (int c = 0; c < 8; ++c) {
@@ -146,18 +106,25 @@ __device__ __forceinline__ void pe_backward(uint32_t taddr, const uint8_t* __res
   }
 }
 
-// Sum over the warp's 32 lanes of v[j] for each j; lane L returns the total of column L.
-__device__ __forceinline__ float warp_transpose_reduce(float (&v)[32], int lane) {
-#pragma unroll
-  for (int off = 16, n = 32; off >= 1; off >>= 1, n >>= 1) {
+// One halving step of warp_transpose_reduce on the first N entries (a compile-time N keeps every index static, so v
+// stays in registers).
+template <int N>
+__device__ __forceinline__ void transpose_reduce_step(float (&v)[32], int lane) {
+  if constexpr (N > 1) {
+    constexpr int off = N / 2;
     const bool upper = (lane & off) != 0;
 #pragma unroll
-    for (int i = 0; i < n / 2; ++i) {
-      const float send = upper ? v[i] : v[i + n / 2];
-      const float keep = upper ? v[i + n / 2] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
+    for (int i = 0; i < off; ++i) {
+      const float lo = v[i], hi = v[i + off];
+      v[i] = (upper ? hi : lo) + __shfl_xor_sync(0xffffffffu, upper ? lo : hi, off);
     }
+    transpose_reduce_step<off>(v, lane);
   }
+}
+
+// Sum over the warp's 32 lanes of v[j] for each j; lane L returns the total of column L.
+__device__ __forceinline__ float warp_transpose_reduce(float (&v)[32], int lane) {
+  transpose_reduce_step<32>(v, lane);
   return v[0];
 }
 
@@ -166,285 +133,226 @@ __device__ __forceinline__ float warp_transpose_reduce(float (&v)[32], int lane)
 template <bool HAS_BENDER>
 __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* act = smem;                       // 2 slots x 64 KB gradient operand
-  uint8_t* ring = smem + 2 * kHBytes;        // kBwdRingStages x 32 KB
-  Shared* sh = reinterpret_cast<Shared*>(ring + kBwdRingStages * kRingStageBytes);
+  uint8_t* act = smem;                               // 64 KB gradient operand, 128 rows
+  uint8_t* ring_buf = smem + kHBytes;                // kRingStages x 32 KB
+  float* stage_all = reinterpret_cast<float*>(ring_buf + kRingStages * kRingStageBytes);   // 2 x 64 rows x kBwdStageLd
+  Shared* sh = reinterpret_cast<Shared*>(stage_all + 2 * kWgRows * kBwdStageLd);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int n_pairs = (p.n_tiles + 1) >> 1;
   constexpr int kNumSteps = HAS_BENDER ? 15 : 10;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kBwdRingStages; ++i) {
+    for (int i = 0; i < kRingStages; ++i) {
       mbar_init(&sh->w_full[i], 1);
-      mbar_init(&sh->w_empty[i], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&sh->a_ready[s], 128);
-      mbar_init(&sh->d_full[s], 1);
+      mbar_init(&sh->w_empty[i], 8);
     }
     sh->abort_flag = 0;
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc(&sh->tmem_base, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = sh->tmem_base;
   const Waiter W{&sh->abort_flag, p.err};
+  Ring ring{ring_buf, sh->w_full, sh->w_empty};
 
-  if (warp == 0) {
+  if (warp >= 8) {
+    setmaxnreg_dec<kProducerRegs>();
     // ===================== weight producer (W^T images) =====================
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0;
-      for (int pair = blockIdx.x; pair < n_pairs; pair += gridDim.x) {
+    if (warp == 8 && lane == 0) {
+      for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
         uint32_t gn = 0, gb = 0;
 #pragma unroll 1
         for (int step = 0; step < kNumSteps; ++step) {
           const StepShape s = step_shape(step);
           const uint8_t* src = step < 10 ? p.nerf_wT + gn : p.bend_wT + gb;
-          for (int slot = 0; slot < 2; ++slot) {
-            for (uint32_t j = 0; j < s.nslabs; ++j) {
-              W.wait(&sh->w_empty[stage], phase ^ 1u, 101);
-              uint8_t* dst = ring + stage * kRingStageBytes;
-              mbar_arrive_expect_tx(&sh->w_full[stage], s.slab_bytes);
-              const uint8_t* g = src + j * s.slab_bytes;
-              for (uint32_t off = 0; off < s.slab_bytes; off += 16384u) {
-                const uint32_t n = s.slab_bytes - off < 16384u ? s.slab_bytes - off : 16384u;
-                tma_bulk_g2s(dst + off, g + off, n, &sh->w_full[stage]);
-              }
-              if (++stage == kBwdRingStages) { stage = 0; phase ^= 1u; }
-            }
-          }
+          for (uint32_t j = 0; j < s.nslabs; ++j) ring_put(ring, src + j * s.slab_bytes, s.slab_bytes, W);
           if (step < 10) gn += s.nslabs * s.slab_bytes; else gb += s.nslabs * s.slab_bytes;
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0;
-      uint32_t aph[2] = {0u, 0u};
-      for (int pair = blockIdx.x; pair < n_pairs; pair += gridDim.x) {
-#pragma unroll 1
-        for (int step = 0; step < kNumSteps; ++step) {
-          const StepShape s = step_shape(step);
-          const uint32_t idesc = umma_instr_desc(kTileM, s.N, UMMA_F16, UMMA_F16, UMMA_K_MAJOR, UMMA_K_MAJOR);
-          for (int slot = 0; slot < 2; ++slot) {
-            W.wait(&sh->a_ready[slot], aph[slot], 201);
-            aph[slot] ^= 1u;
-            tc_fence_after_sync();
-            const uint32_t d_tmem = tmem_base + slot * 256;
-            const uint32_t a_base = smem_u32(act + slot * kHBytes);
-            for (uint32_t j = 0; j < s.nslabs; ++j) {
-              W.wait(&sh->w_full[stage], phase, 202);
-              tc_fence_after_sync();
-              const uint64_t adesc = umma_smem_desc(a_base + j * 8 * kChunkBytes, kChunkBytes, 128);
-              const uint64_t bdesc = umma_smem_desc(smem_u32(ring + stage * kRingStageBytes), s.N * 16, 128);
-              for (uint32_t k = 0; k < s.k16; ++k) {
-                umma_f16_ss(d_tmem, umma_desc_advance(adesc, k * 2 * kChunkBytes),
-                            umma_desc_advance(bdesc, k * 2 * s.N * 16), idesc, (j | k) ? 1u : 0u);
-              }
-              umma_commit(&sh->w_empty[stage]);
-              if (++stage == kBwdRingStages) { stage = 0; phase ^= 1u; }
-            }
-            umma_commit(&sh->d_full[slot]);
-          }
-        }
-      }
+    return;
+  }
+
+  // ===================== consumer warpgroups =====================
+  setmaxnreg_inc<kConsumerRegs>();
+  const int g = warp >> 2;
+  const int tw = threadIdx.x & 127;
+  const bool row_thread = tw < kWgRows;   // threads 0-63 (warps 0, 1 of the warpgroup) each own one row
+  const int bar = 1 + g;
+  const bool wg_leader = tw == 0;
+  const int row = g * kWgRows + tw;       // tile row of a row thread
+  uint8_t* a_row = act + row * 16;
+  const uint32_t a_base = smem_u32(act) + g * kWgRows * 16;
+  auto a_slab = [&](uint32_t j) { return a_base + j * 8 * kChunkBytes; };
+  float* stg = stage_all + g * kWgRows * kBwdStageLd;
+  const float* my_stg = stg + tw * kBwdStageLd;
+
+  // power-of-two loss scale from max|d_raw| (written by the compositing backward kernel)
+  float scale = 1.0f;
+  {
+    const float amax = p.amax ? __ldg(p.amax) : 0.f;
+    if (amax > 0.f && amax < 3.0e38f) {
+      int e;
+      frexpf(amax, &e);                       // amax = m * 2^e, m in [0.5, 1)
+      scale = ldexpf(1.0f, min(max(10 - e, -60), 60));  // max|d_raw| * scale in [512, 1024)
     }
-  } else if (warp >= 4) {
-    // ===================== epilogue warpgroups =====================
-    const int slot = (warp - 4) >> 2;
-    const int row = ((warp & 3) << 5) | lane;
-    uint8_t* a_row = act + slot * kHBytes + row * 16;
-    const uint32_t taddr = tmem_base + ((static_cast<uint32_t>(warp & 3) * 32u) << 16) + slot * 256;
-    uint32_t dph = 0;
-    auto signal_ready = [&]() {
+  }
+  const float inv_scale = 1.0f / scale;
+
+  for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
+    const long long pt = static_cast<long long>(tile) * kTileM + row;
+    const bool valid = row_thread && pt < p.P;
+    const uint8_t* st_tile = p.stash + static_cast<long long>(tile) * kStashTileBytes;
+    const uint8_t* st = st_tile + row * 16;
+    uint8_t* gs = p.gstash + static_cast<long long>(tile) * kGradTileBytes;
+    // gradient stash: bulk TMA stores of finished images from shared memory (see field_fwd.cu)
+    auto stash_begin = [&]() {
+      if (wg_leader) tma_bulk_wait_read<0>();
+      wg_bar(bar);
+    };
+    auto ready = [&](uint32_t off, uint32_t chunks) {
       fence_proxy_async_smem();
-      tc_fence_before_sync();
-      mbar_arrive(&sh->a_ready[slot]);
+      wg_bar(bar);
+      if (wg_leader && chunks) store_rows(gs + off, act, g, chunks);
     };
-    auto wait_acc = [&](int code) {
-      W.wait(&sh->d_full[slot], dph, code);
-      dph ^= 1u;
-      tc_fence_after_sync();
-    };
-    // power-of-two loss scale from max|d_raw| (written by the compositing backward kernel)
-    float scale = 1.0f;
-    {
-      const float amax = p.amax ? __ldg(p.amax) : 0.f;
-      if (amax > 0.f && amax < 3.0e38f) {
-        int e;
-        frexpf(amax, &e);                       // amax = m * 2^e, m in [0.5, 1)
-        scale = ldexpf(1.0f, min(max(10 - e, -60), 60));  // max|d_raw| * scale in [512, 1024)
+    // The ReLU masks come from the forward stash (read once, straight from HBM).  One thread pulls the image the
+    // NEXT step will read into L2 while this step's epilogue runs, so the per-thread loads find it there.
+    auto prefetch = [&](uint32_t off, uint32_t bytes) {
+      if (wg_leader) {
+        for (uint32_t o = 0; o < bytes; o += 16384u) tma_prefetch_l2(st_tile + off + o, bytes - o < 16384u ? bytes - o : 16384u);
       }
+    };
+    prefetch(kStH + 7 * kHBytes, kHBytes);
+    // ---- d_raw image: [g_r g_g g_b g_sigma 0 ...] (K = 16) ----
+    stash_begin();
+    if (row_thread) {
+      float gr[4] = {0.f, 0.f, 0.f, 0.f};
+      if (valid) {
+        const float* q = p.d_raw + pt * p.out_ch;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) gr[c] = clamp_h(__ldg(q + c) * scale);
+      }
+      *reinterpret_cast<uint4*>(a_row) = make_uint4(pack_h2(gr[0], gr[1]), pack_h2(gr[2], gr[3]), 0u, 0u);
+      *reinterpret_cast<uint4*>(a_row + kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
     }
-    const float inv_scale = 1.0f / scale;
-
-    for (int pair = blockIdx.x; pair < n_pairs; pair += gridDim.x) {
-      const long long tile = static_cast<long long>(pair) * 2 + slot;
-      const long long pt = tile * kTileM + row;
-      const bool valid = pt < p.P;
-      const uint8_t* st = p.stash + tile * kStashTileBytes + row * 16;
-      uint8_t* gs = p.gstash + tile * kGradTileBytes;
-      uint8_t* a_img = act + slot * kHBytes;
-      const bool wg_leader = (threadIdx.x & 127) == 0;
-      // gradient stash: bulk TMA stores of finished images from shared memory (see field_fwd.cu)
-      auto stash_begin = [&]() {
-        if (wg_leader) tma_bulk_wait_read<0>();
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + slot) : "memory");
-      };
-      auto stash_store = [&](uint32_t off, uint32_t bytes) {
-        fence_proxy_async_smem();
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + slot) : "memory");
-        if (wg_leader) {
-          for (uint32_t o = 0; o < bytes; o += 16384u) tma_bulk_s2g(gs + off + o, a_img + o, bytes - o < 16384u ? bytes - o : 16384u);
-          tma_bulk_commit();
-        }
-      };
-
-      // The ReLU masks come from the forward stash (read once, straight from HBM).  One thread pulls the image the
-      // NEXT step will read into L2 while this step's epilogue runs, so the per-thread loads find it there.
-      const uint8_t* st_tile = p.stash + tile * kStashTileBytes;
-      auto prefetch = [&](uint32_t off, uint32_t bytes) {
-        if (wg_leader) {
-          for (uint32_t o = 0; o < bytes; o += 16384u) tma_prefetch_l2(st_tile + off + o, bytes - o < 16384u ? bytes - o : 16384u);
-        }
-      };
-      prefetch(kStH + 7 * kHBytes, kHBytes);
-      // ---- d_raw image: [g_r g_g g_b g_sigma 0 ...] (K = 16) ----
-      {
-        float g[4] = {0.f, 0.f, 0.f, 0.f};
-        if (valid) {
-          const float* q = p.d_raw + pt * p.out_ch;
-#pragma unroll
-          for (int c = 0; c < 4; ++c) g[c] = clamp_h(__ldg(q + c) * scale);
-        }
-        const uint4 c0 = make_uint4(pack_h2(g[0], g[1]), pack_h2(g[2], g[3]), 0u, 0u);
-        const uint4 zz = make_uint4(0u, 0u, 0u, 0u);
-        stash_begin();
-        *reinterpret_cast<uint4*>(a_row) = c0;
-        *reinterpret_cast<uint4*>(a_row + kChunkBytes) = zz;
-        stash_store(kGsRaw, 2 * kChunkBytes);
-      }
-      signal_ready();
-      float dx[3] = {0.f, 0.f, 0.f};
-      // ---- head^T, L7^T, L6^T : dY7, dY6, dY5 ----
+    ready(kGsRaw, 2);
+    float dx[3] = {0.f, 0.f, 0.f};
+    // ---- head^T, L7^T, L6^T : dY7, dY6, dY5 ----
 #pragma unroll 1
-      for (int s = 0; s < 3; ++s) {
-        wait_acc(300 + s);
-        if (s < 2) prefetch(kStH + (6 - s) * kHBytes, kHBytes); else prefetch(kStE, kEBytes);
-        stash_begin();
-        epi_mask_store<256>(taddr, st + kStH + (7 - s) * kHBytes, a_row);
-        stash_store(kGsY + (7 - s) * kHBytes, kHBytes);
-        signal_ready();
-      }
-      // ---- L5e^T: gradient into the skip-connected embedding ----
-      wait_acc(303);
+    for (int s = 0; s < 3; ++s) {
+      const StepShape sh_ = step_shape(s);
+      float acc[128];
+      wg_gemm<256>(acc, ring, sh_.nslabs, sh_.k16, a_slab, W, 300 + s);
+      if (s < 2) prefetch(kStH + (6 - s) * kHBytes, kHBytes); else prefetch(kStE, kEBytes);
+      stash_begin();
+      epi_mask_store<256>(acc, st_tile + kStH + (7 - s) * kHBytes, act, g);
+      ready(kGsY + (7 - s) * kHBytes, 32);
+    }
+    // ---- L5e^T: gradient into the skip-connected embedding ----
+    {
+      float acc[32];
+      wg_gemm<64>(acc, ring, 1, 16, a_slab, W, 303);
       prefetch(kStH + 4 * kHBytes, kHBytes);
-      pe_backward(taddr, st + kStE, dx);
-      signal_ready();   // A operand (dY5) untouched; accumulator drained
-      // ---- L5h^T, L4^T .. L1^T : dY4 .. dY0 ----
+      stage_cols<0, 8>(acc, stg, kBwdStageLd);
+      wg_bar(bar);
+      if (row_thread) pe_backward(my_stg, st + kStE, dx);
+      // A operand (dY5) untouched; the staging rows are rewritten only after the barriers of the next steps
+    }
+    // ---- L5h^T, L4^T .. L1^T : dY4 .. dY0 ----
 #pragma unroll 1
-      for (int s = 0; s < 5; ++s) {
-        wait_acc(304 + s);
-        if (s < 4) prefetch(kStH + (3 - s) * kHBytes, kHBytes); else prefetch(kStE, kEBytes);
-        stash_begin();
-        epi_mask_store<256>(taddr, st + kStH + (4 - s) * kHBytes, a_row);
-        stash_store(kGsY + (4 - s) * kHBytes, kHBytes);
-        signal_ready();
-      }
-      // ---- L0^T: gradient into the embedding; then through the bend ----
-      wait_acc(309);
+    for (int s = 0; s < 5; ++s) {
+      float acc[128];
+      wg_gemm<256>(acc, ring, 4, 4, a_slab, W, 304 + s);
+      if (s < 4) prefetch(kStH + (3 - s) * kHBytes, kHBytes); else prefetch(kStE, kEBytes);
+      stash_begin();
+      epi_mask_store<256>(acc, st_tile + kStH + (4 - s) * kHBytes, act, g);
+      ready(kGsY + (4 - s) * kHBytes, 32);
+    }
+    // ---- L0^T: gradient into the embedding; then through the bend ----
+    {
+      float acc[32];
+      wg_gemm<64>(acc, ring, 1, 16, a_slab, W, 309);
       if (HAS_BENDER) prefetch(kStHb4, 8 * kChunkBytes);
-      pe_backward(taddr, st + kStE, dx);
-      if (!HAS_BENDER) continue;   // xyz has no learnable upstream without a bender (appendix C)
+      stage_cols<0, 8>(acc, stg, kBwdStageLd);
+      wg_bar(bar);
+      if (row_thread) pe_backward(my_stg, st + kStE, dx);
+    }
+    if (!HAS_BENDER) continue;   // xyz has no learnable upstream without a bender (appendix C)
 
-      float rig = 0.f, drpre = 0.f;
-      {
-        float un[3] = {0.f, 0.f, 0.f}, dun[3], dm[3];
-        float up_r = 0.f, up_u[3] = {0.f, 0.f, 0.f};
-        if (valid) {
-          rig = __ldg(p.rigidity + pt);
+    float drpre = 0.f;
+    stash_begin();
+    if (row_thread) {
+      float rig = 0.f, un[3] = {0.f, 0.f, 0.f}, dun[3], dm[3];
+      float up_r = 0.f, up_u[3] = {0.f, 0.f, 0.f};
+      if (valid) {
+        rig = __ldg(p.rigidity + pt);
 #pragma unroll
-          for (int d = 0; d < 3; ++d) un[d] = __ldg(p.unmasked + pt * 3 + d);
-          if (p.d_rigid_up) up_r = __ldg(p.d_rigid_up + pt) * scale;
-          if (p.d_unmasked_up) {
+        for (int d = 0; d < 3; ++d) un[d] = __ldg(p.unmasked + pt * 3 + d);
+        if (p.d_rigid_up) up_r = __ldg(p.d_rigid_up + pt) * scale;
+        if (p.d_unmasked_up) {
 #pragma unroll
-            for (int d = 0; d < 3; ++d) up_u[d] = __ldg(p.d_unmasked_up + pt * 3 + d) * scale;
-          }
+          for (int d = 0; d < 3; ++d) up_u[d] = __ldg(p.d_unmasked_up + pt * 3 + d) * scale;
         }
-        float dr = up_r;
-#pragma unroll
-        for (int d = 0; d < 3; ++d) {
-          dm[d] = p.use_scaling ? dx[d] * p.scaling : dx[d];   // masked = rig * un (* scaling); bent = xyz + masked
-          dun[d] = rig * dm[d] + up_u[d];
-          dr += un[d] * dm[d];
-        }
-        // rigidity = (tanh(pre) + 1) / 2  =>  d/dpre = (1 - tanh^2) / 2 = 2 r (1 - r); cut-off entries carry no gradient
-        drpre = dr * 2.0f * rig * (1.0f - rig);
-        if (p.use_cutoff && rig <= p.cutoff) drpre = 0.f;
-        if (!valid) { dun[0] = dun[1] = dun[2] = 0.f; drpre = 0.f; }
-        const uint4 c0 = make_uint4(pack_h2(clamp_h(dun[0]), clamp_h(dun[1])), pack_h2(clamp_h(dun[2]), 0.f), 0u, 0u);
-        const uint4 zz = make_uint4(0u, 0u, 0u, 0u);
-        stash_begin();
-        *reinterpret_cast<uint4*>(a_row) = c0;
-        *reinterpret_cast<uint4*>(a_row + kChunkBytes) = zz;
-        stash_store(kGsYb4, 2 * kChunkBytes);
       }
-      signal_ready();
-      // ---- B4^T -> dYb3 ----
-      wait_acc(310);
+      float dr = up_r;
+#pragma unroll
+      for (int d = 0; d < 3; ++d) {
+        dm[d] = p.use_scaling ? dx[d] * p.scaling : dx[d];   // masked = rig * un (* scaling); bent = xyz + masked
+        dun[d] = rig * dm[d] + up_u[d];
+        dr += un[d] * dm[d];
+      }
+      // rigidity = (tanh(pre) + 1) / 2  =>  d/dpre = (1 - tanh^2) / 2 = 2 r (1 - r); cut-off entries carry no gradient
+      drpre = dr * 2.0f * rig * (1.0f - rig);
+      if (p.use_cutoff && rig <= p.cutoff) drpre = 0.f;
+      if (!valid) { dun[0] = dun[1] = dun[2] = 0.f; drpre = 0.f; }
+      *reinterpret_cast<uint4*>(a_row) = make_uint4(pack_h2(clamp_h(dun[0]), clamp_h(dun[1])), pack_h2(clamp_h(dun[2]), 0.f), 0u, 0u);
+      *reinterpret_cast<uint4*>(a_row + kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
+    }
+    ready(kGsYb4, 2);
+    // ---- B4^T -> dYb3 ----
+    {
+      float acc[32];
+      wg_gemm<64>(acc, ring, 1, 1, a_slab, W, 310);
       prefetch(kStHb3, 8 * kChunkBytes);
       stash_begin();
-      epi_mask_store<64>(taddr, st + kStHb4, a_row);
-      stash_store(kGsYb3, 8 * kChunkBytes);
-      signal_ready();
-      // ---- B3^T -> dYb2 = [dh * mask (64) | d rigidity pre-activation | 0 (15)] ----
-      wait_acc(311);
+      epi_mask_store<64>(acc, st_tile + kStHb4, act, g);
+      ready(kGsYb3, 8);
+    }
+    // ---- B3^T -> dYb2 = [dh * mask (64) | d rigidity pre-activation | 0 (15)] ----
+    {
+      float acc[32];
+      wg_gemm<64>(acc, ring, 1, 4, a_slab, W, 311);
       prefetch(kStHb2, 12 * kChunkBytes);
       stash_begin();
-      epi_mask_store<64>(taddr, st + kStHb3, a_row);
-      {
-        const uint4 c8 = make_uint4(pack_h2(clamp_h(drpre), 0.f), 0u, 0u, 0u);
-        const uint4 zz = make_uint4(0u, 0u, 0u, 0u);
-        *reinterpret_cast<uint4*>(a_row + 8 * kChunkBytes) = c8;
-        *reinterpret_cast<uint4*>(a_row + 9 * kChunkBytes) = zz;
+      epi_mask_store<64>(acc, st_tile + kStHb3, act, g);
+      if (row_thread) {
+        *reinterpret_cast<uint4*>(a_row + 8 * kChunkBytes) = make_uint4(pack_h2(clamp_h(drpre), 0.f), 0u, 0u, 0u);
+        *reinterpret_cast<uint4*>(a_row + 9 * kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
       }
-      stash_store(kGsYb2, 10 * kChunkBytes);
-      signal_ready();
-      // ---- B2^T -> dYb1, B1^T -> dYb0 ----
-      wait_acc(312);
+      ready(kGsYb2, 10);
+    }
+    // ---- B2^T -> dYb1, B1^T -> dYb0 ----
+    {
+      float acc[48];
+      wg_gemm<96>(acc, ring, 1, 5, a_slab, W, 312);
       prefetch(kStHb1, 12 * kChunkBytes);
       stash_begin();
-      epi_mask_store<96>(taddr, st + kStHb2, a_row);
-      stash_store(kGsYb1, 12 * kChunkBytes);
-      signal_ready();
-      wait_acc(313);
+      epi_mask_store<96>(acc, st_tile + kStHb2, act, g);
+      ready(kGsYb1, 12);
+      wg_gemm<96>(acc, ring, 1, 6, a_slab, W, 313);
       stash_begin();
-      epi_mask_store<96>(taddr, st + kStHb1, a_row);
-      stash_store(kGsYb0, 12 * kChunkBytes);
-      signal_ready();
-      // ---- B0^T: d(bender input); columns 6..37 are the latent code -> per-ray reduction ----
-      wait_acc(314);
-      {
+      epi_mask_store<96>(acc, st_tile + kStHb1, act, g);
+      ready(kGsYb0, 12);
+    }
+    // ---- B0^T: d(bender input); columns 6..37 are the latent code -> per-ray reduction ----
+    {
+      float acc[24];
+      wg_gemm<48>(acc, ring, 1, 6, a_slab, W, 314);
+      stage_cols<0, 5>(acc, stg, kBwdStageLd);
+      wg_bar(bar);
+      if (row_thread) {   // warps 0 and 1 of the warpgroup: 32 consecutive rows each
         float dl[32];
-        {
-          uint32_t v[32];
-          tmem_ld32(taddr, v);
-          uint32_t w[16];
-          tmem_ld16(taddr + 32, w);
-          tmem_ld_wait();
 #pragma unroll
-          for (int i = 0; i < 26; ++i) dl[i] = __uint_as_float(v[6 + i]) * inv_scale;
-#pragma unroll
-          for (int i = 0; i < 6; ++i) dl[26 + i] = __uint_as_float(w[i]) * inv_scale;
-        }
+        for (int i = 0; i < 32; ++i) dl[i] = my_stg[6 + i] * inv_scale;
         const long long ray = valid ? pt / p.S : -1;
         const long long ray0 = __shfl_sync(0xffffffffu, ray, 0);
         if (__all_sync(0xffffffffu, ray == ray0 && valid)) {
@@ -455,22 +363,17 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
           for (int i = 0; i < 32; ++i) atomicAdd(p.d_latents + ray * kLatent + i, dl[i]);
         }
       }
-      // next a_ready arrival: the next pair's d_raw image
     }
-    if ((threadIdx.x & 127) == 0) tma_bulk_wait<0>();   // all gradient-stash stores complete before the CTA exits
+    // next: the next tile's d_raw image (after stash_begin's barrier)
   }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, 512);
+  if (wg_leader) tma_bulk_wait<0>();   // all gradient-stash stores complete before the CTA exits
 }
 
 // ------------------------------------------------------------------------------------------------
 cudaError_t launch_field_bwd(const FieldBwdParams& p, bool has_bender, int num_sms, cudaStream_t stream) {
-  const size_t smem = 2 * kHBytes + kBwdRingStages * kRingStageBytes + sizeof(Shared) + 64;
-  const int n_pairs = (p.n_tiles + 1) / 2;
-  if (n_pairs <= 0) return cudaSuccess;
-  const int grid = n_pairs < num_sms ? n_pairs : num_sms;
+  const size_t smem = kHBytes + kRingStages * kRingStageBytes + 2 * kWgRows * kBwdStageLd * sizeof(float) + sizeof(Shared) + 64;
+  if (p.n_tiles <= 0) return cudaSuccess;
+  const int grid = p.n_tiles < num_sms ? p.n_tiles : num_sms;
   cudaError_t e;
   if (has_bender) {
     e = cudaFuncSetAttribute(field_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

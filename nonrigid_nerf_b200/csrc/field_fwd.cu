@@ -4,36 +4,28 @@
 //   run_network (train.py:57-105) -> batchify (train.py:27-54) -> NeRF.forward
 //   (run_nerf_helpers.py:240-314) -> ray_bending.forward (run_nerf_helpers.py:507-584)
 //   -> Embedder.embed (run_nerf_helpers.py:149-150)
-// with ONE persistent sm_100a kernel.  No [P,95] / [P,256] tensor ever touches HBM.
+// with ONE persistent sm_90a kernel.  No [P,95] / [P,256] tensor ever touches HBM.
 //
-// Work decomposition
-//   tile   = 128 consecutive sample points (= 128 TMEM lanes = UMMA M)
-//   CTA    = 1 per SM, persistent; processes tile PAIRS (slot 0 / slot 1) so that the epilogue of
-//            one slot overlaps the tensor-core work of the other
-//   warps  : 0 weight producer (bulk TMA ring), 1 MMA issuer (tcgen05.mma, one lane),
-//            2 TMEM allocator, 3 idle, 4-7 epilogue warpgroup of slot 0, 8-11 of slot 1
-//   a "step" = one dense layer for one slot:  D[128 x N] (TMEM, fp32) = A[128 x K] (smem, fp16)
-//            . W[N x K]^T (smem ring, fp16); the epilogue warpgroup drains D, applies
-//            bias/ReLU/(bend + positional encoding), and writes the next A operand in place.
+// Work decomposition (field_mma.cuh)
+//   tile   = 128 consecutive sample points; CTA = 1 per SM, persistent over tiles
+//   warps  : 0-3 / 4-7 consumer warpgroups (rows 0-63 / 64-127 of the tile), 8 weight producer (bulk TMA ring)
+//   a "step" = one dense layer:  D[64 x N] (registers, fp32) = A[64 x K] (smem, fp16) . W[N x K]^T (smem ring,
+//            fp16) with wgmma; the same warpgroup then applies bias/ReLU/(bend + positional encoding) and writes
+//            the next A operand in place.
 //   steps  : B0..B4 (ray bender, offset + rigidity MLPs fused block-diagonally), L0..L7, head
 //
-// Shared memory (per CTA): 2 x (H 64 KB + E 16 KB) activations + 2 x 32 KB weight ring + barriers.
-// Tensor memory: 512 columns, 256 per slot.
-#include "nrn_common.cuh"
-#include "sm100_ptx.cuh"
+// Shared memory (per CTA): H 64 KB + E 16 KB activations, 4 x 32 KB weight ring, per-row staging, barriers.
+#include "field_mma.cuh"
 
 namespace nrn {
 
 namespace {
 
-constexpr long long kWaitLimitCycles = 1ll << 28;  // ~0.14 s: protocol bug => error flag, not a hang
+constexpr int kFwdStageLd = 12;   // floats per staged row (8 used)
 
 struct Shared {
   uint64_t w_full[kRingStages];
   uint64_t w_empty[kRingStages];
-  uint64_t a_ready[2];
-  uint64_t d_full[2];
-  uint32_t tmem_base;
   int abort_flag;
 };
 
@@ -55,7 +47,7 @@ __device__ __forceinline__ StepShape step_shape(int step) {
     default: return {256u, 4u, 32768u, 4u};
   }
 }
-// byte offset (inside a slot's activation region: H at 0, E at kHBytes) of the A operand of slab j
+// byte offset (inside the activation region: H at 0, E at kHBytes) of the A operand of slab j
 __device__ __forceinline__ uint32_t a_operand_offset(int step, uint32_t j) {
   if (step == 0 || step == 5) return kHBytes;                       // bender input / embedding live in E
   if (step == 10) return j == 0 ? kHBytes : (j - 1) * 8 * kChunkBytes;  // skip: [embedding | h]
@@ -63,60 +55,18 @@ __device__ __forceinline__ uint32_t a_operand_offset(int step, uint32_t j) {
   return j * 8 * kChunkBytes;
 }
 
-// Developer profile (NRN_DEBUG_MODE=9): cycles CTA 0's roles spend waiting, read with nrn_debug_profile_fwd1().
-//   [0] issuer total  [1] issuer: a_ready  [3] issuer: w_full  [4] producer: w_empty  [5] epilogue WG (slot 0) total
-//   [6] epilogue: d_full  [10] slabs issued  [11] tile pairs
-__device__ unsigned long long g_fwd1_prof[16];
-
-struct Waiter {
-  int* s_abort;
-  int* g_err;
-  __device__ __forceinline__ bool wait(uint64_t* bar, uint32_t parity, int code, unsigned long long* acc = nullptr) const {
-    if (mbar_try_wait(bar, parity)) return true;
-    const long long t0 = clock64();
-    while (!mbar_try_wait(bar, parity)) {
-      if (*reinterpret_cast<volatile int*>(s_abort)) return false;
-      if (clock64() - t0 > kWaitLimitCycles) {
-        atomicExch(s_abort, code);
-        atomicCAS(g_err, 0, code);
-        return false;
-      }
-    }
-    if (acc) *acc += static_cast<unsigned long long>(clock64() - t0);
-    return true;
-  }
-};
-
-__device__ __forceinline__ float relu_h(float v) { return fminf(fmaxf(v, 0.f), 65504.f); }
-
-// Drain NCOLS accumulator columns (multiple of 32), add bias, ReLU, convert to fp16 and store them
-// as chunks [chunk0, chunk0 + NCOLS/8) of this thread's row in a chunk-major activation image.
-template <int NCOLS>
-__device__ __forceinline__ void epi_bias_relu_store(uint32_t taddr, const float* __restrict__ bias,
-                                                    uint8_t* dst_row) {
-  // software pipeline: the TMEM load of chunk c+1 and the bias loads of chunk c are in flight while
-  // chunk c-1 / c is being processed (tcgen05.wait::ld only ever waits for a load issued a block ago)
-  constexpr int NC = NCOLS / 32;
-  uint32_t v[2][32];
-  tmem_ld32(taddr, v[0]);
+// Accumulator columns [0, NCOLS) + bias, ReLU, fp16 -> this warpgroup's rows of the chunk-major image `img`.
+template <int NCOLS, int NR>
+__device__ __forceinline__ void epi_bias_relu_store(const float (&acc)[NR], const float* __restrict__ bias, uint8_t* img, int g) {
+  const int r0 = g * kWgRows + acc_r0(), q = acc_q();
 #pragma unroll
-  for (int c = 0; c < NC; ++c) {
-    float4 b[8];
+  for (int j = 0; j < NCOLS / 8; ++j) {
+    const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * q));
 #pragma unroll
-    for (int i = 0; i < 8; ++i) b[i] = __ldg(reinterpret_cast<const float4*>(bias + c * 32 + i * 4));
-    tmem_ld_wait();
-    if (c + 1 < NC) tmem_ld32(taddr + (c + 1) * 32, v[(c + 1) & 1]);
-    const uint32_t(&w)[32] = v[c & 1];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const float4 b0 = b[2 * q], b1 = b[2 * q + 1];
-      uint4 pk;
+    for (int i = 0; i < 2; ++i) {
       // one cvt.rn.relu.satfinite.f16x2 per two outputs: ReLU, clamp to fp16 range and pack in a single instruction
-      pk.x = pack_h2_relu_sat(__uint_as_float(w[q * 8 + 0]) + b0.x, __uint_as_float(w[q * 8 + 1]) + b0.y);
-      pk.y = pack_h2_relu_sat(__uint_as_float(w[q * 8 + 2]) + b0.z, __uint_as_float(w[q * 8 + 3]) + b0.w);
-      pk.z = pack_h2_relu_sat(__uint_as_float(w[q * 8 + 4]) + b1.x, __uint_as_float(w[q * 8 + 5]) + b1.y);
-      pk.w = pack_h2_relu_sat(__uint_as_float(w[q * 8 + 6]) + b1.z, __uint_as_float(w[q * 8 + 7]) + b1.w);
-      *reinterpret_cast<uint4*>(dst_row + (c * 4 + q) * kChunkBytes) = pk;
+      *reinterpret_cast<uint32_t*>(img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) =
+          pack_h2_relu_sat(acc[4 * j + 2 * i] + b.x, acc[4 * j + 2 * i + 1] + b.y);
     }
   }
 }
@@ -162,180 +112,102 @@ __device__ __forceinline__ void write_pe(const float (&x)[3], uint8_t* dst_row) 
 template <bool HAS_BENDER>
 __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* act = smem;                                  // 2 slots x (H | E)
-  uint8_t* ring = smem + 2 * kSlotBytes;                // kRingStages x 32 KB
-  Shared* sh = reinterpret_cast<Shared*>(ring + kRingStages * kRingStageBytes);
+  uint8_t* act = smem;                                  // H | E, 128 rows
+  uint8_t* ring_buf = smem + kSlotBytes;                // kRingStages x 32 KB
+  float* stage_all = reinterpret_cast<float*>(ring_buf + kRingStages * kRingStageBytes);   // 2 x 64 rows x kFwdStageLd
+  Shared* sh = reinterpret_cast<Shared*>(stage_all + 2 * kWgRows * kFwdStageLd);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int n_pairs = (p.n_tiles + 1) >> 1;
   constexpr int kFirstStep = HAS_BENDER ? 0 : 5;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kRingStages; ++i) {
       mbar_init(&sh->w_full[i], 1);
-      mbar_init(&sh->w_empty[i], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&sh->a_ready[s], 128);
-      mbar_init(&sh->d_full[s], 1);
+      mbar_init(&sh->w_empty[i], 8);
     }
     sh->abort_flag = 0;
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc(&sh->tmem_base, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = sh->tmem_base;
   const Waiter W{&sh->abort_flag, p.err};
-  const bool prof = p.debug_mode == 9 && blockIdx.x == 0;
+  Ring ring{ring_buf, sh->w_full, sh->w_empty};
 
-  if (warp == 0) {
+  if (warp >= 8) {
+    setmaxnreg_dec<kProducerRegs>();
     // ===================== weight producer: global -> smem ring (bulk TMA) =====================
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0;
-      unsigned long long pw = 0;
-      for (int pair = blockIdx.x; pair < n_pairs; pair += gridDim.x) {
+    if (warp == 8 && lane == 0) {
+      for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
         uint32_t gb = 0, gn = 0;
 #pragma unroll 1
         for (int step = kFirstStep; step < 14; ++step) {
           const StepShape s = step_shape(step);
           const uint8_t* src = step < 5 ? p.bend_w + gb : p.nerf_w + gn;
-          for (int slot = 0; slot < 2; ++slot) {
-            for (uint32_t j = 0; j < s.nslabs; ++j) {
-              W.wait(&sh->w_empty[stage], phase ^ 1u, 101, prof ? &pw : nullptr);
-              uint8_t* dst = ring + stage * kRingStageBytes;
-              mbar_arrive_expect_tx(&sh->w_full[stage], s.slab_bytes);
-              const uint8_t* g = src + j * s.slab_bytes;
-              for (uint32_t off = 0; off < s.slab_bytes; off += 16384u) {
-                const uint32_t n = s.slab_bytes - off < 16384u ? s.slab_bytes - off : 16384u;
-                tma_bulk_g2s(dst + off, g + off, n, &sh->w_full[stage]);
-              }
-              if (++stage == kRingStages) { stage = 0; phase ^= 1u; }
-            }
-          }
+          for (uint32_t j = 0; j < s.nslabs; ++j) ring_put(ring, src + j * s.slab_bytes, s.slab_bytes, W);
           if (step < 5) gb += s.nslabs * s.slab_bytes; else gn += s.nslabs * s.slab_bytes;
         }
       }
-      if (prof) g_fwd1_prof[4] = pw;
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0;
-      uint32_t aph[2] = {0u, 0u};
-      unsigned long long w_a = 0, w_w = 0, n_slabs = 0, n_done = 0;
-      const long long t_start = clock64();
-      for (int pair = blockIdx.x; pair < n_pairs; pair += gridDim.x) {
-        ++n_done;
-#pragma unroll 1
-        for (int step = kFirstStep; step < 14; ++step) {
-          const StepShape s = step_shape(step);
-          const uint32_t idesc = umma_instr_desc(kTileM, s.N, UMMA_F16, UMMA_F16, UMMA_K_MAJOR, UMMA_K_MAJOR);
-          for (int slot = 0; slot < 2; ++slot) {
-            W.wait(&sh->a_ready[slot], aph[slot], 201, prof ? &w_a : nullptr);
-            aph[slot] ^= 1u;
-            tc_fence_after_sync();
-            const uint32_t d_tmem = tmem_base + slot * 256;
-            const uint32_t a_base = smem_u32(act + slot * kSlotBytes);
-            for (uint32_t j = 0; j < s.nslabs; ++j) {
-              ++n_slabs;
-              W.wait(&sh->w_full[stage], phase, 202, prof ? &w_w : nullptr);
-              tc_fence_after_sync();
-              const uint64_t adesc = umma_smem_desc(a_base + a_operand_offset(step, j), kChunkBytes, 128);
-              const uint64_t bdesc = umma_smem_desc(smem_u32(ring + stage * kRingStageBytes), s.N * 16, 128);
-              for (uint32_t k = 0; k < s.k16 && p.debug_mode != 2; ++k) {
-                umma_f16_ss(d_tmem, umma_desc_advance(adesc, k * 2 * kChunkBytes),
-                            umma_desc_advance(bdesc, k * 2 * s.N * 16), idesc, (j | k) ? 1u : 0u);
-              }
-              umma_commit(&sh->w_empty[stage]);  // slab free once these MMAs retire
-              if (++stage == kRingStages) { stage = 0; phase ^= 1u; }
-            }
-            umma_commit(&sh->d_full[slot]);      // accumulator complete
-          }
-        }
-      }
-      if (prof) {
-        g_fwd1_prof[0] = static_cast<unsigned long long>(clock64() - t_start);
-        g_fwd1_prof[1] = w_a; g_fwd1_prof[3] = w_w; g_fwd1_prof[10] = n_slabs; g_fwd1_prof[11] = n_done;
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue warpgroups =====================
-    const int slot = (warp - 4) >> 2;
-    const int row = ((warp & 3) << 5) | lane;
-    uint8_t* Hs = act + slot * kSlotBytes;
-    uint8_t* Es = Hs + kHBytes;
-    uint8_t* h_row = Hs + row * 16;
-    uint8_t* e_row = Es + row * 16;
-    const uint32_t taddr = tmem_base + ((static_cast<uint32_t>(warp & 3) * 32u) << 16) + slot * 256;
-    uint32_t dph = 0;
-    unsigned long long w_d = 0;
-    const bool tprof = prof && slot == 0 && (threadIdx.x & 127) == 0;
-    const long long t_start = clock64();
-    auto signal_ready = [&]() {
-      fence_proxy_async_smem();
-      tc_fence_before_sync();
-      mbar_arrive(&sh->a_ready[slot]);
-    };
-    auto wait_acc = [&](int code) {
-      W.wait(&sh->d_full[slot], dph, code, tprof ? &w_d : nullptr);
-      dph ^= 1u;
-      tc_fence_after_sync();
-    };
+    return;
+  }
 
-    for (int pair = blockIdx.x; pair < n_pairs; pair += gridDim.x) {
-      const long long pt = (static_cast<long long>(pair) * 2 + slot) * kTileM + row;
-      const bool valid = pt < p.P;
-      // Training stash: every finished activation image (a contiguous chunk-major block of shared memory) is
-      // written to this tile's stash block with bulk TMA stores issued by one thread of the warpgroup; the
-      // epilogue threads spend no load/store slots on it.  stash_begin(): the previous store must have finished
-      // READING shared memory before any image is overwritten.
-      uint8_t* st = p.stash ? p.stash + (static_cast<long long>(pair) * 2 + slot) * kStashTileBytes : nullptr;
-      const bool wg_leader = (threadIdx.x & 127) == 0;
-      auto stash_begin = [&]() {
-        if (st) {
-          if (wg_leader) tma_bulk_wait_read<0>();
-          asm volatile("bar.sync %0, 128;" ::"r"(1 + slot) : "memory");
-        }
-      };
-      auto stash_store = [&](uint32_t stash_off, const uint8_t* img, uint32_t bytes) {
-        if (st) {
-          fence_proxy_async_smem();
-          asm volatile("bar.sync %0, 128;" ::"r"(1 + slot) : "memory");
-          if (wg_leader) {
-            for (uint32_t o = 0; o < bytes; o += 16384u) tma_bulk_s2g(st + stash_off + o, img + o, bytes - o < 16384u ? bytes - o : 16384u);
-            tma_bulk_commit();
-          }
-        }
-      };
-      float x[3] = {0.f, 0.f, 0.f};
-      long long ray = 0;
-      if (valid) {
-        ray = pt / p.S;
-        if (p.pts) {
-          const float* q = p.pts + pt * p.pts_stride;  // point mode: NeRF.forward(x) reads x[:, :3]
-          x[0] = __ldg(q + 0); x[1] = __ldg(q + 1); x[2] = __ldg(q + 2);
-        } else {
-          const float z = __ldg(p.z_vals + pt);
-          const float* r = p.rays + ray * 8;
-          // pts = rays_o + rays_d * z  (train.py:871-873), multiply then add like the reference
-          x[0] = __fadd_rn(__ldg(r + 0), __fmul_rn(__ldg(r + 3), z));
-          x[1] = __fadd_rn(__ldg(r + 1), __fmul_rn(__ldg(r + 4), z));
-          x[2] = __fadd_rn(__ldg(r + 2), __fmul_rn(__ldg(r + 5), z));
-        }
-        if (p.d_init) {
-          p.d_init[pt * 3 + 0] = x[0]; p.d_init[pt * 3 + 1] = x[1]; p.d_init[pt * 3 + 2] = x[2];
-        }
+  // ===================== consumer warpgroups =====================
+  setmaxnreg_inc<kConsumerRegs>();
+  const int g = warp >> 2;
+  const int tw = threadIdx.x & 127;
+  const bool row_thread = tw < kWgRows;   // threads 0-63 of the warpgroup each own one row for the per-point work
+  const int bar = 1 + g;
+  const bool wg_leader = tw == 0;
+  uint8_t* Hs = act;
+  uint8_t* Es = act + kHBytes;
+  uint8_t* e_row = Es + (g * kWgRows + tw) * 16;
+  const uint32_t a_h = smem_u32(Hs) + g * kWgRows * 16;
+  const uint32_t a_e = smem_u32(Es) + g * kWgRows * 16;
+  float* stg = stage_all + g * kWgRows * kFwdStageLd;
+  float* my_stg = stg + tw * kFwdStageLd;
+
+  for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
+    const long long pt = static_cast<long long>(tile) * kTileM + g * kWgRows + tw;
+    const bool valid = row_thread && pt < p.P;
+    // Training stash: every finished activation image is written to this tile's stash block with bulk TMA stores
+    // issued by one thread of the warpgroup (its 64 rows of each chunk); the epilogue threads spend no load/store
+    // slots on it.  stash_begin(): the previous stores must have finished READING shared memory before any image is
+    // overwritten; it also orders every warp's wgmma reads of an operand before any warp rewrites it in place.
+    // ready(): the image is complete and visible to the async proxy (wgmma operand, TMA store).
+    uint8_t* st = p.stash ? p.stash + static_cast<long long>(tile) * kStashTileBytes : nullptr;
+    auto stash_begin = [&]() {
+      if (st && wg_leader) tma_bulk_wait_read<0>();
+      wg_bar(bar);
+    };
+    auto ready = [&](uint32_t stash_off, const uint8_t* img, uint32_t chunks) {
+      fence_proxy_async_smem();
+      wg_bar(bar);
+      if (st && wg_leader && chunks) store_rows(st + stash_off, img, g, chunks);
+    };
+    float x[3] = {0.f, 0.f, 0.f};
+    long long ray = 0;
+    if (valid) {
+      ray = pt / p.S;
+      if (p.pts) {
+        const float* q = p.pts + pt * p.pts_stride;  // point mode: NeRF.forward(x) reads x[:, :3]
+        x[0] = __ldg(q + 0); x[1] = __ldg(q + 1); x[2] = __ldg(q + 2);
+      } else {
+        const float z = __ldg(p.z_vals + pt);
+        const float* r = p.rays + ray * 8;
+        // pts = rays_o + rays_d * z  (train.py:871-873), multiply then add like the reference
+        x[0] = __fadd_rn(__ldg(r + 0), __fmul_rn(__ldg(r + 3), z));
+        x[1] = __fadd_rn(__ldg(r + 1), __fmul_rn(__ldg(r + 4), z));
+        x[2] = __fadd_rn(__ldg(r + 2), __fmul_rn(__ldg(r + 5), z));
       }
-      float rigidity = 0.f;
-      if (HAS_BENDER) {
-        // ---- bender input row: [xyz_hi(3) xyz_lo(3) latent(32) 0(10)] fp16, chunks 0..5 of E ----
-        stash_begin();
+      if (p.d_init) {
+        p.d_init[pt * 3 + 0] = x[0]; p.d_init[pt * 3 + 1] = x[1]; p.d_init[pt * 3 + 2] = x[2];
+      }
+    }
+    float rigidity = 0.f;
+    if (HAS_BENDER) {
+      // ---- bender input row: [xyz_hi(3) xyz_lo(3) latent(32) 0(10)] fp16, chunks 0..5 of E ----
+      stash_begin();
+      if (row_thread) {
         float in[48];
 #pragma unroll
         for (int d = 0; d < 3; ++d) {
@@ -357,49 +229,56 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
           pk.w = pack_h2(in[c * 8 + 6], in[c * 8 + 7]);
           *reinterpret_cast<uint4*>(e_row + c * kChunkBytes) = pk;
         }
-        stash_store(kStBin, Es, 6 * kChunkBytes);
-        signal_ready();
-        // ---- B0, B1: 96 hidden units (64 offset | 32 rigidity) ----
-        wait_acc(301);
+      }
+      ready(kStBin, Es, 6);
+      // ---- B0, B1: 96 hidden units (64 offset | 32 rigidity) ----
+      {
+        float acc[48];
+        wg_gemm<96>(acc, ring, 1, 3, [&](uint32_t) { return a_e; }, W, 301);
         stash_begin();
-        epi_bias_relu_store<96>(taddr, p.bend_bias, h_row);
-        stash_store(kStHb1, Hs, 12 * kChunkBytes);
-        signal_ready();
-        wait_acc(302);
+        epi_bias_relu_store<96>(acc, p.bend_bias, Hs, g);
+        ready(kStHb1, Hs, 12);
+        wg_gemm<96>(acc, ring, 1, 6, [&](uint32_t) { return a_h; }, W, 302);
         stash_begin();
-        epi_bias_relu_store<96>(taddr, p.bend_bias + 96, h_row);
-        stash_store(kStHb2, Hs, 12 * kChunkBytes);
-        signal_ready();
-        // ---- B2: 64 offset hidden + rigidity output (column 64) ----
-        wait_acc(303);
+        epi_bias_relu_store<96>(acc, p.bend_bias + 96, Hs, g);
+        ready(kStHb2, Hs, 12);
+      }
+      // ---- B2: 64 offset hidden + rigidity output (column 64) ----
+      {
+        float acc[40];
+        wg_gemm<80>(acc, ring, 1, 6, [&](uint32_t) { return a_h; }, W, 303);
         stash_begin();
-        epi_bias_relu_store<64>(taddr, p.bend_bias + 192, h_row);
-        stash_store(kStHb3, Hs, 8 * kChunkBytes);
-        {
-          uint32_t v[16];
-          tmem_ld16(taddr + 64, v);
-          tmem_ld_wait();
-          const float rr = __uint_as_float(v[0]) + __ldg(p.bend_bias + 192 + 64);
+        epi_bias_relu_store<64>(acc, p.bend_bias + 192, Hs, g);
+        if (acc_q() == 0) {
+          stg[acc_r0() * kFwdStageLd] = acc[32];
+          stg[(acc_r0() + 8) * kFwdStageLd] = acc[34];
+        }
+        ready(kStHb3, Hs, 8);
+        if (row_thread) {
+          const float rr = my_stg[0] + __ldg(p.bend_bias + 192 + 64);
           rigidity = (tanhf(rr) + 1.0f) * 0.5f;   // run_nerf_helpers.py:559-561
           if (p.use_cutoff && rigidity <= p.cutoff) rigidity = 0.f;  // :563-564
         }
-        signal_ready();
-        // ---- B3 ----
-        wait_acc(304);
+      }
+      // ---- B3 ----
+      {
+        float acc[32];
+        wg_gemm<64>(acc, ring, 1, 4, [&](uint32_t) { return a_h; }, W, 304);
         stash_begin();
-        epi_bias_relu_store<64>(taddr, p.bend_bias + 272, h_row);
-        stash_store(kStHb4, Hs, 8 * kChunkBytes);
-        signal_ready();
-        // ---- B4: offsets; bend; positional encoding of the bent point -> E ----
-        wait_acc(305);
-        {
-          uint32_t v[16];
-          tmem_ld16(taddr, v);
-          tmem_ld_wait();
+        epi_bias_relu_store<64>(acc, p.bend_bias + 272, Hs, g);
+        ready(kStHb4, Hs, 8);
+      }
+      // ---- B4: offsets; bend ----
+      {
+        float acc[8];
+        wg_gemm<16>(acc, ring, 1, 4, [&](uint32_t) { return a_h; }, W, 305);
+        stage_cols<0, 1>(acc, stg, kFwdStageLd);
+        wg_bar(bar);
+        if (row_thread) {
           float un[3], ma[3];
 #pragma unroll
           for (int d = 0; d < 3; ++d) {
-            un[d] = __uint_as_float(v[d]);
+            un[d] = my_stg[d];
             ma[d] = __fmul_rn(rigidity, un[d]);              // :567
             if (p.use_scaling) ma[d] = __fmul_rn(ma[d], p.scaling);  // :568-569
           }
@@ -412,61 +291,55 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
           for (int d = 0; d < 3; ++d) x[d] = __fadd_rn(x[d], ma[d]);  // :570
         }
       }
-      if (valid && p.d_bent) {
-        p.d_bent[pt * 3 + 0] = x[0]; p.d_bent[pt * 3 + 1] = x[1]; p.d_bent[pt * 3 + 2] = x[2];
-      }
-      stash_begin();
-      write_pe(x, e_row);
-      stash_store(kStE, Es, kEBytes);
-      signal_ready();
-      // ---- L0 .. L7 ----
-#pragma unroll 1
-      for (int L = 0; L < 8; ++L) {
-        wait_acc(310 + L);
-        stash_begin();
-        if (p.debug_mode != 1) epi_bias_relu_store<256>(taddr, p.nerf_bias + L * 256, h_row);
-        stash_store(kStH + L * kHBytes, Hs, kHBytes);
-        signal_ready();
-      }
-      // ---- head: raw = output_linear(h) (run_nerf_helpers.py:306) ----
-      wait_acc(320);
-      {
-        uint32_t v[16];
-        tmem_ld16(taddr, v);
-        tmem_ld_wait();
-        if (valid) {
-          float o[5];
-#pragma unroll
-          for (int c = 0; c < 5; ++c) o[c] = __uint_as_float(v[c]) + __ldg(p.nerf_bias + 2048 + c);
-          // test-time non-rigid object removal (run_nerf_helpers.py:309-310)
-          if (HAS_BENDER && p.use_removal && rigidity >= p.removal) o[3] *= 0.f;
-          float* dst = p.raw + pt * p.out_ch;
-          for (int c = 0; c < p.out_ch; ++c) dst[c] = o[c];
-        }
-      }
-      // the next a_ready arrival is the next pair's prologue (which also means TMEM is drained)
     }
-    if (p.stash && (threadIdx.x & 127) == 0) tma_bulk_wait<0>();   // all stash stores complete before the CTA exits
-    if (tprof) { g_fwd1_prof[5] = static_cast<unsigned long long>(clock64() - t_start); g_fwd1_prof[6] = w_d; }
+    if (valid && p.d_bent) {
+      p.d_bent[pt * 3 + 0] = x[0]; p.d_bent[pt * 3 + 1] = x[1]; p.d_bent[pt * 3 + 2] = x[2];
+    }
+    // ---- positional encoding of the (bent) point -> E ----
+    stash_begin();
+    if (row_thread) write_pe(x, e_row);
+    ready(kStE, Es, 8);
+    // ---- L0 .. L7 ----
+#pragma unroll 1
+    for (int L = 0; L < 8; ++L) {
+      const int step = 5 + L;
+      const StepShape s = step_shape(step);
+      float acc[128];
+      wg_gemm<256>(acc, ring, s.nslabs, s.k16, [&](uint32_t j) { return a_h + a_operand_offset(step, j); }, W, 310 + L);
+      stash_begin();
+      epi_bias_relu_store<256>(acc, p.nerf_bias + L * 256, Hs, g);
+      ready(kStH + L * kHBytes, Hs, 32);
+    }
+    // ---- head: raw = output_linear(h) (run_nerf_helpers.py:306) ----
+    {
+      float acc[8];
+      wg_gemm<16>(acc, ring, 1, 16, [&](uint32_t) { return a_h; }, W, 320);
+      stage_cols<0, 1>(acc, stg, kFwdStageLd);
+      wg_bar(bar);
+      if (valid) {
+        float o[5];
+#pragma unroll
+        for (int c = 0; c < 5; ++c) o[c] = my_stg[c] + __ldg(p.nerf_bias + 2048 + c);
+        // test-time non-rigid object removal (run_nerf_helpers.py:309-310)
+        if (HAS_BENDER && p.use_removal && rigidity >= p.removal) o[3] *= 0.f;
+        float* dst = p.raw + pt * p.out_ch;
+        for (int c = 0; c < p.out_ch; ++c) dst[c] = o[c];
+      }
+    }
+    // the staging rows are rewritten only after further warpgroup barriers (next tile's B2 / head)
   }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, 512);
+  if (p.stash && wg_leader) tma_bulk_wait<0>();   // all stash stores complete before the CTA exits
 }
 
 // ------------------------------------------------------------------------------------------------
-extern "C" int nrn_debug_profile_fwd1(unsigned long long* out16) {
-  return cudaMemcpyFromSymbol(out16, g_fwd1_prof, sizeof(unsigned long long) * 16) == cudaSuccess ? 0 : -2;
+size_t field_fwd_smem_bytes() {
+  return kSlotBytes + kRingStages * kRingStageBytes + 2 * kWgRows * kFwdStageLd * sizeof(float) + sizeof(Shared) + 64;
 }
-
-size_t field_fwd_smem_bytes() { return 2 * kSlotBytes + kRingStages * kRingStageBytes + sizeof(Shared) + 64; }
 
 cudaError_t launch_field_fwd(const FieldFwdParams& p, bool has_bender, int num_sms, cudaStream_t stream) {
   const size_t smem = field_fwd_smem_bytes();
-  const int n_pairs = (p.n_tiles + 1) / 2;
-  if (n_pairs <= 0) return cudaSuccess;
-  const int grid = n_pairs < num_sms ? n_pairs : num_sms;
+  if (p.n_tiles <= 0) return cudaSuccess;
+  const int grid = p.n_tiles < num_sms ? p.n_tiles : num_sms;
   cudaError_t e;
   if (has_bender) {
     e = cudaFuncSetAttribute(field_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -8,14 +8,15 @@ namespace nrn {
 // ------------------------------------------------------------------------------------------
 // Geometry of the fused field kernels
 // ------------------------------------------------------------------------------------------
-constexpr int kTileM = 128;                 // points per tile = TMEM lanes = UMMA M
+constexpr int kTileM = 128;                 // points per tile = 2 warpgroups x wgmma M (64)
 constexpr int kChunkBytes = kTileM * 16;    // one 8-column chunk of a 128-row activation image
 constexpr int kHBytes = 32 * kChunkBytes;   // 256-wide hidden activations, 64 KB
 constexpr int kEBytes = 8 * kChunkBytes;    // 64-wide positional embedding, 16 KB
 constexpr int kSlotBytes = kHBytes + kEBytes;
 constexpr int kRingStageBytes = 32768;      // one weight slab: 256 rows x 64 K-columns fp16
-constexpr int kRingStages = 2;
-constexpr int kFwdThreads = 384;            // 12 warps: producer, mma, tmem, spare, 2 x 4 epilogue
+constexpr int kRingStages = 4;
+constexpr int kFwdThreads = 384;            // 2 consumer warpgroups (MMA + epilogue), 1 producer warpgroup (one thread streams)
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // setmaxnreg budgets: 128 x (40 + 2 x 232) <= 64K
 
 // ------------------------------------------------------------------------------------------
 // Packed NeRF weights (fp16, chunk-major images in streaming order), see pack.cu
@@ -143,7 +144,6 @@ struct FieldFwdParams {
   float* d_masked;        // [P][3] or null
   float* d_rigid;         // [P]    or null
   uint8_t* stash;         // training stash [n_tiles rounded up to even][kStashTileBytes] or null
-  int debug_mode;         // developer experiments (NRN_DEBUG_MODE): 1 = epilogues skip their work, 2 = no MMAs issued, 3 = 1 + no weight streaming
   int* err;               // device error word (0 = ok)
 };
 

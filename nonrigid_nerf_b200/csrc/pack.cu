@@ -1,5 +1,5 @@
 // Weight packing: fp32 nn.Linear tensors ([out][in] row-major, the reference's checkpoint layout,
-// run_nerf_helpers.py:218-238 and :411-482) -> fp16 "chunk-major" UMMA operand images laid out in the
+// run_nerf_helpers.py:218-238 and :411-482) -> fp16 "chunk-major" wgmma operand images laid out in the
 // exact order the fused kernels stream them (layout table in nrn_common.cuh).
 // Re-run after every optimizer step / load_state_dict (1.07 M parameters: a few microseconds); forward and
 // transposed (DGRAD) images of a module are written by ONE launch.

@@ -6,7 +6,7 @@
 
 namespace nrn {
 
-constexpr int kPeerMaxRanks = 8;       // one NVSwitch domain of a B200 node
+constexpr int kPeerMaxRanks = 8;       // one NVSwitch domain of an 8-GPU H100 node
 constexpr int kPeerArrive = 0;         // flag rows inside a window: [3][kPeerMaxRanks] u32, then padding to kPeerFlagBytes
 constexpr int kPeerDone = 1;
 constexpr int kPeerGather = 2;

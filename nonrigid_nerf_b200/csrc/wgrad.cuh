@@ -11,14 +11,15 @@ constexpr int kWgMaxCtas = 192;
 struct WgradParams {
   const uint8_t* stash;    // forward activation stash
   const uint8_t* gstash;   // gradient stash written by DGRAD
-  float* scratch;          // [kWgMaxCtas][kWgScratchFloats]
+  float* scratch;          // [kWgMaxCtas][kWgScratchFloats]: one partial per (job, split)
   const float* amax;       // loss-scale source (see field_bwd.cu) or null
   int n_tiles;
   int compact;             // 1: stashes hold only the bender images (divergence regulariser), bender jobs only
   long long stash_tile_bytes, gstash_tile_bytes;   // filled in by launch_wgrad
   int n_jobs;
   int job_ids[16];
-  int splits[16];
+  int splits[16];          // scratch partials (tile ranges) per job
+  int halves[16];          // CTAs per split: 2 for a NeRF layer's 256-row dW, else 1
   int* err;
 };
 

@@ -3,7 +3,7 @@
 At N_rand = 1024 the fused kernels need ~2 ms per step, but an iteration also launches several hundred
 tiny PyTorch kernels (loss arithmetic, the double-backward divergence regulariser, per-latent gradient
 accumulation, Adam): launch-bound.  Capturing forward + backward + optimizer step once and replaying the
-graph removes the host from the loop (the B200 way: "CUDA streams and graphs instead of a tracing compiler").
+graph removes the host from the loop ("CUDA streams and graphs instead of a tracing compiler").
 Everything the eager step does is still executed by every replay, including the weight re-packing kernels.
 """
 from __future__ import annotations

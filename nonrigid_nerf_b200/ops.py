@@ -70,7 +70,7 @@ def bender_param_list(bender):
 
 
 def pack_nerf(net) -> torch.Tensor:
-    """fp16 UMMA image of a NeRF module's weights (see csrc/nrn_common.cuh)."""
+    """fp16 wgmma operand image of a NeRF module's weights (see csrc/nrn_common.cuh)."""
     ws, bs = nerf_param_list(net)
     key = _versions(ws + bs)
     cache = getattr(net, "_nrn_pack", None)

@@ -1,4 +1,4 @@
-"""Peer-memory gradient reduction (csrc/peer.cu): the B200-native replacement of DataParallel's gradient reduce + Adam.
+"""Peer-memory gradient reduction (csrc/peer.cu): the H100-native replacement of DataParallel's gradient reduce + Adam.
 
 One process per GPU on one NVSwitch node.  Every rank's gradient arena lives in a CUDA-IPC window the other ranks map;
 `optimizer.step()` becomes ONE fused sequence of plain kernels that reads the peers' arenas over NVLink while summing them

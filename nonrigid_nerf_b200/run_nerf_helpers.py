@@ -3,7 +3,7 @@
 Same names, constructor/forward signatures, attribute names and state_dict keys as the reference
 (so `logs/*.tar` checkpoints interchange: pts_linears.N.{weight,bias}, views_linears.0.*,
 output_linear.*, network.N.*, rigidity_network.N.*), but every forward dispatches to the fused
-sm_100a kernels through the C ABI.  There is no PyTorch fallback: unsupported configurations raise.
+sm_90a kernels through the C ABI.  There is no PyTorch fallback: unsupported configurations raise.
 
 Reference: run_nerf_helpers.py:10-19 (misc), :120-168 (Embedder), :172-385 (NeRF), :388-584
 (ray_bending), :651-698 (sample_pdf).

@@ -2,7 +2,7 @@
 
 render / batchify_rays / render_rays / run_network / batchify / raw2outputs keep the reference's
 names, argument meaning, return structure and error behaviour (train.py:27-137, :326-416,
-:724-980), but run on the fused sm_100a kernels.  torch.nn.DataParallel (train.py:290-323) is
+:724-980), but run on the fused sm_90a kernels.  torch.nn.DataParallel (train.py:290-323) is
 replaced by ray sharding over torch.distributed/NCCL (parallel.py).
 
 Randomness (t_rand, sigma noise coarse, u, sigma noise fine; train.py:861, :753, run_nerf_helpers.py:666) comes from the

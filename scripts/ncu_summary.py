@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
-"""Summarise an `ncu --page raw --csv` export of one training step into profiles/:
-    python scripts/ncu_summary.py gpurun_out/r02_ncu_full_step_raw.csv profiles/r02
-writes <prefix>_traffic.json (DRAM bytes per step and kernel kind, read by bench.py for roofline.traffic) and
+"""Summarise an `ncu --page raw --csv` export of one training step:
+    python scripts/ncu_summary.py ncu_out/h100_ncu_full_step_raw.csv ncu_out/h100
+writes <prefix>_traffic.json (DRAM bytes per step and kernel kind) and
 <prefix>_ncu_summary.md (one row per launch: duration, DRAM read / write, achieved DRAM GB/s, tensor-pipe and SM activity)."""
 import csv
 import json

@@ -1,35 +1,33 @@
 #!/bin/bash
-# SASS opcode summary per kernel of libnrnerf_b200.so: proves the tcgen05 / TMEM / bulk-TMA instructions are in the binary.
-#   scripts/sass_summary.sh > profiles/r02_sass_summary.txt
+# SASS opcode summary per kernel of libnrnerf_b200.so: proves the wgmma / bulk-TMA / mbarrier instructions are in the binary.
+#   scripts/sass_summary.sh > sass_summary.txt
 set -e
 SO=${1:-nonrigid_nerf_b200/libnrnerf_b200.so}
-echo "# cuobjdump -sass $SO  (sm_100a) -- instruction counts per kernel"
-echo "# UTCHMMA = tcgen05.mma, LDTM = tcgen05.ld, UTCBAR = tcgen05.commit, UBLKCP = cp.async.bulk (G.S load / S.G store), UBLKPF = bulk L2 prefetch, SYNCS = mbarrier"
+echo "# cuobjdump -sass $SO  (sm_90a) -- instruction counts per kernel"
+echo "# HGMMA = wgmma.mma_async, UBLKCP = cp.async.bulk (G.S load / S.G store), UBLKPF = bulk L2 prefetch, SYNCS = mbarrier"
 cuobjdump -sass "$SO" | awk '
 /Function :/ { fn=$3; next }
 {
   if (fn == "") next;
   n[fn]++;
-  if ($0 ~ /UTCHMMA\.2CTA/) c[fn,"UTCHMMA.2CTA"]++; else if ($0 ~ /UTCHMMA/) c[fn,"UTCHMMA"]++;
-  if ($0 ~ /LDTM/) c[fn,"LDTM"]++;
-  if ($0 ~ /UTCBAR/) c[fn,"UTCBAR"]++;
+  if ($0 ~ /HGMMA/) c[fn,"HGMMA"]++;
   if ($0 ~ /UBLKCP\.S\.G|UBLKCP.*\.S\.G/) c[fn,"UBLKCP.S.G"]++; else if ($0 ~ /UBLKCP/) c[fn,"UBLKCP.G.S"]++;
   if ($0 ~ /UBLKPF/) c[fn,"UBLKPF"]++;
   if ($0 ~ /SYNCS/) c[fn,"SYNCS"]++;
-  if ($0 ~ /HMMA|IMMA/ && $0 !~ /UTCHMMA/) c[fn,"legacy-MMA"]++;
+  if ($0 ~ /HMMA|IMMA/ && $0 !~ /HGMMA/) c[fn,"legacy-MMA"]++;
   if ($0 ~ /MUFU/) c[fn,"MUFU"]++;
   if ($0 ~ /ATOM|RED\./) c[fn,"ATOM/RED"]++;
   if ($0 ~ /LD\.E.*SYS|ST\.E.*SYS|\.STRONG\.SYS/) c[fn,"sys-scope ld/st"]++;
 }
 END {
-  split("UTCHMMA UTCHMMA.2CTA LDTM UTCBAR UBLKCP.G.S UBLKCP.S.G UBLKPF SYNCS MUFU ATOM/RED sys-scope_ld/st legacy-MMA", cols, " ");
+  split("HGMMA UBLKCP.G.S UBLKCP.S.G UBLKPF SYNCS MUFU ATOM/RED sys-scope_ld/st legacy-MMA", cols, " ");
   printf "%-62s %8s", "kernel", "instrs";
-  for (i = 1; i <= 12; i++) printf " %12s", cols[i];
+  for (i = 1; i <= 9; i++) printf " %12s", cols[i];
   printf "\n";
   for (f in n) {
     g = f; gsub(/^_ZN3nrn[0-9]*/, "", g); gsub(/_GLOBAL__N__[0-9a-f_]*/, "", g);
     printf "%-62s %8d", substr(g, 1, 62), n[f];
-    for (i = 1; i <= 12; i++) { k = cols[i]; gsub(/_/, " ", k); printf " %12d", c[f,k] + 0; }
+    for (i = 1; i <= 9; i++) { k = cols[i]; gsub(/_/, " ", k); printf " %12d", c[f,k] + 0; }
     printf "\n";
   }
 }' | (read -r hdr; echo "$hdr"; sort)

@@ -11,7 +11,7 @@ on a synthetic non-rigid scene (analytic density / colour blobs that move with t
 regularisers on, then renders held-out pixels of every frame with each trained model (deterministic sampling) and
 reports the loss curves and the PSNR against the ground truth.  Writes one JSON document (stdout or --out).
 
-    python scripts/train_ab.py --iters 1000 --out profiles/r02_train_ab.json
+    python scripts/train_ab.py --iters 1000 --out train_ab.json
 """
 import argparse
 import json

@@ -9,7 +9,7 @@
   * full gradient parity at the benchmark batch (N_rand = 1024, 64c + 128f): WGRAD split-K over 1,536 tiles;
   * the default-config regulariser weights with a vanishing data term (shared fp16 loss scale).
 
-Tolerances are ~10x the errors measured on B200 (printed by the tests; fp16 tensor-core operands vs the fp32 reference).
+Tolerances are ~10x the errors measured on the GPU (printed by the tests; fp16 tensor-core operands vs the fp32 reference).
 """
 import os
 
@@ -214,7 +214,7 @@ def test_public_sample_pdf_and_raw2outputs_wrappers_match_golden_caseE():
 
 
 def test_gradient_parity_at_the_benchmark_batch_1024_rays():
-    """N_rand = 1024, 64c + 128f: WGRAD split-K over 1,536 tiles / 148 CTAs against the oracle's autograd."""
+    """N_rand = 1024, 64c + 128f: WGRAD split-K over 1,536 tiles / one CTA per SM against the oracle's autograd."""
     from nonrigid_nerf_b200 import _lib, train as T
     seed, n = 1024, 1024
     coarse, fine, bender, (cp, fp, bp) = helpers.build_models(O, seed, DEV)
