@@ -50,6 +50,34 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 
+// ----------------------------------------------------------------------------------------------
+// thread-block clusters: rank, cluster-wide barrier, shared memory of another CTA of the cluster
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster arrives and waits (also a full CTA barrier)
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;\n" ::: "memory");
+}
+// shared::cluster address of the variable at p's offset in the shared memory of CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa_shared(const void* p, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(r) : "r"(smem_u32(p)), "r"(rank));
+  return r;
+}
+// arrive on an mbarrier given by its shared::cluster address (possibly in another CTA of the cluster).  Default
+// (.release.cta) semantics: meant for releasing a stage whose reads have completed (wgmma.wait_group, loads whose
+// values were used).  A .release.cluster arrive compiles to a GPU-wide MEMBAR on every call.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];\n" ::"r"(cluster_addr) : "memory");
+}
+__device__ __forceinline__ void st_shared_cluster(uint32_t cluster_addr, int v) {
+  asm volatile("st.relaxed.cluster.shared::cluster.u32 [%0], %1;\n" ::"r"(cluster_addr), "r"(v) : "memory");
+}
+
 // generic-proxy smem writes -> visible to the async proxy (TMA stores / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
@@ -67,6 +95,16 @@ __device__ __forceinline__ void tma_bulk_g2s(void* smem_dst, const void* gmem_sr
       "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(
           smem_u32(smem_dst)),
       "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
+      : "memory");
+}
+// the same, delivered to the same shared-memory offset of every CTA of the cluster in cta_mask, each completing on its
+// own mbarrier at bar's offset
+__device__ __forceinline__ void tma_bulk_g2s_multicast(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar,
+                                                       uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;\n" ::"r"(
+          smem_u32(smem_dst)),
+      "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "h"(cta_mask)
       : "memory");
 }
 // contiguous shared -> global (bulk_group completion)

@@ -11,9 +11,13 @@
 // and one activation image block (B) per tile (jobs 0-9: one NeRF layer; jobs 10-11: the five small ray-bender
 // layers, grouped so that their images are one contiguous range of each stash).  The fp32 accumulators live in
 // registers: a consumer warpgroup holds at most 64 x 256 of them, so a CTA (two consumer warpgroups) covers 128 rows
-// of dW and a NeRF layer's 256-row dW is split over two CTAs ("halves") that stream the same activation blocks at
-// the same time (adjacent CTAs: the second read of a block is an L2 hit).  A pipeline stage holds ONE whole 128-point
-// block, A and B alternating through a 3 x 64 KB ring, fetched with a handful of 16 KB bulk copies.  Every job is
+// of dW and a NeRF layer's 256-row dW is split over two CTAs ("halves").  The two halves of a split are the two CTAs
+// of one cluster: each fetches its own A block (different gradient columns) and half of the shared B block, which TMA
+// multicasts into both CTAs, so every activation block leaves L2 once per cluster.  A pipeline stage holds one
+// tile's A block followed by its B block (at most 48 chunks, 96 KB); the 192 KB ring has 2 such stages, or 4 for
+// the 48 KB tiles of the L5e / L0 jobs, so the next tile's operands are in flight while the current tile's MMAs and
+// bias sums run.  A stage that received multicast data is refilled only after the consumers of BOTH CTAs released
+// it (each consumer warp arrives on its own and on the partner's empty barrier).  Every job is
 // split over contiguous tile ranges ("split-K") proportionally to its bytes; partial sums go to a scratch buffer
 // and a second kernel reduces them in a fixed order (deterministic) while un-padding / un-permuting
 // into the reference's parameter layout and dividing out the loss scale.
@@ -31,8 +35,9 @@ namespace nrn {
 namespace {
 
 constexpr long long kWaitLimitCycles = 1ll << 28;
-constexpr int kWgStages = 3;
-constexpr int kStageBytes = 32 * kChunkBytes;      // one block of up to 32 chunk images (128 points x 8 features each)
+constexpr int kRingBytes = 96 * kChunkBytes;       // operand ring: 96 chunk images (128 points x 8 features each)
+constexpr int kMaxStages = 4;
+constexpr uint32_t kPieceBytes = 16384;            // size of one bulk copy
 constexpr int kWgThreads = 384;                    // 2 consumer warpgroups (MMA, bias sums, drain), producer warpgroup
 
 // One 64-row M tile of a sub-MMA, issued by one warpgroup: dW rows [m0, m0 + 64) of the sub.
@@ -99,14 +104,16 @@ __device__ __forceinline__ Job job_desc(int j, int half, int g, int compact) {
 }
 
 struct Shared {
-  uint64_t full[kWgStages];
-  uint64_t empty[kWgStages];
+  uint64_t full[kMaxStages];
+  uint64_t empty[kMaxStages];
   int abort_flag;
 };
 
 struct Waiter {
   int* s_abort;
   int* g_err;
+  bool paired;
+  uint32_t partner_abort;   // shared::cluster address of the partner CTA's abort_flag (paired CTAs)
   __device__ __forceinline__ bool wait(uint64_t* bar, uint32_t parity, int code) const {
     if (mbar_try_wait(bar, parity)) return true;
     const long long t0 = clock64();
@@ -114,12 +121,21 @@ struct Waiter {
       if (*reinterpret_cast<volatile int*>(s_abort)) return false;
       if (clock64() - t0 > kWaitLimitCycles) {
         atomicExch(s_abort, code);
+        if (paired) st_shared_cluster(partner_abort, code);   // the partner stops waiting for this CTA's releases
         atomicCAS(g_err, 0, code);
         return false;
       }
     }
     return true;
   }
+};
+
+// Operand ring: stage s holds one tile's A block at smem + s * stage_bytes and its B block right behind it.
+struct Ring {
+  uint8_t* smem;
+  int stage_bytes, n_stages;
+  bool paired;
+  uint32_t partner_empty;   // shared::cluster address of the partner CTA's empty[0] (paired CTAs)
 };
 
 // One halving step of warp_transpose_reduce on the first N entries (a compile-time N keeps every index static, so v
@@ -145,13 +161,15 @@ __device__ __forceinline__ float warp_transpose_reduce(float (&v)[32], int lane)
 }
 
 // which (job, split, half) does this CTA own, and which scratch partial is the split's?  job_ids[] / splits[] /
-// halves[] come from the host (WgradParams); the halves of one split are adjacent CTAs.
-__device__ __forceinline__ bool locate(const WgradParams& p, int cta, int& job, int& split, int& nsplit, int& half, int& part) {
+// halves[] come from the host (WgradParams); the halves of one split are the two CTAs of one cluster.
+__device__ __forceinline__ bool locate(const WgradParams& p, int cta, int& job, int& split, int& nsplit, int& half, int& halves,
+                                       int& part) {
   int base = 0, pbase = 0;
   for (int j = 0; j < p.n_jobs; ++j) {
     const int n = p.splits[j] * p.halves[j];
     if (cta < base + n) {
       job = p.job_ids[j]; split = (cta - base) / p.halves[j]; half = (cta - base) % p.halves[j]; nsplit = p.splits[j];
+      halves = p.halves[j];
       part = pbase + split;
       return true;
     }
@@ -186,7 +204,7 @@ __device__ __forceinline__ void unit_drain(const float (&acc)[NR], const Unit& u
 // One consumer warpgroup: its units' MMAs over every tile of the split (accumulators in registers), the bias column
 // sums of its warps' A chunks, then the drain into the scratch partial.  N0 / N1 = 0: no such unit.
 template <int N0, int N1>
-__device__ __forceinline__ void consume(const Job& jb, const Unit& u0, const Unit& u1, uint8_t* smem, Shared* sh, const Waiter& W,
+__device__ __forceinline__ void consume(const Job& jb, const Unit& u0, const Unit& u1, const Ring& R, Shared* sh, const Waiter& W,
                                         int n_tiles_local, float* part, bool have) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float acc0[N0 > 0 ? N0 / 2 : 1];
@@ -199,13 +217,9 @@ __device__ __forceinline__ void consume(const Job& jb, const Unit& u0, const Uni
   float bias_acc = 0.f;
   uint32_t stage = 0, phase = 0;
   for (int it = 0; it < n_tiles_local; ++it) {
-    const uint32_t sa = stage;
-    W.wait(&sh->full[sa], phase, 201);
-    if (++stage == kWgStages) { stage = 0; phase ^= 1u; }
-    const uint32_t sb = stage;
-    W.wait(&sh->full[sb], phase, 202);
-    if (++stage == kWgStages) { stage = 0; phase ^= 1u; }
-    const uint32_t a0 = smem_u32(smem + sa * kStageBytes), b0 = smem_u32(smem + sb * kStageBytes);
+    W.wait(&sh->full[stage], phase, 201);
+    const uint8_t* st_a = R.smem + stage * R.stage_bytes;
+    const uint32_t a0 = smem_u32(st_a), b0 = a0 + jb.a_chunks * kChunkBytes;
     if constexpr (N0 > 0) {
       acc_fence(acc0);
       acc_fence(acc1);
@@ -222,9 +236,9 @@ __device__ __forceinline__ void consume(const Job& jb, const Unit& u0, const Uni
 #pragma unroll
       for (int cc = 0; cc < 4; ++cc) {
         const int c = warp * 4 + cc;
-        const uint8_t* src = smem + sa * kStageBytes + c * kChunkBytes + lane * 16;
+        const uint8_t* src = st_a + c * kChunkBytes + lane * 16;
         float t8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        if (c < jb.a_chunks) {        // chunks beyond the block hold stale data
+        if (c < jb.a_chunks) {        // chunks beyond the A block belong to the B block
 #pragma unroll
           for (int r = 0; r < 4; ++r) {
             const uint4 w = *reinterpret_cast<const uint4*>(src + r * 512);
@@ -248,9 +262,10 @@ __device__ __forceinline__ void consume(const Job& jb, const Unit& u0, const Uni
     }
     __syncwarp();
     if (lane == 0) {
-      mbar_arrive(&sh->empty[sa]);
-      mbar_arrive(&sh->empty[sb]);
+      mbar_arrive(&sh->empty[stage]);
+      if (R.paired) mbar_arrive_cluster(R.partner_empty + stage * static_cast<uint32_t>(sizeof(uint64_t)));
     }
+    if (++stage == R.n_stages) { stage = 0; phase ^= 1u; }
   }
   if (!have || n_tiles_local == 0) return;
   if (jb.bias && (warp * 4 + (lane >> 3)) < jb.a_chunks) part[65536 + jb.bias_off + warp * 32 + lane] = bias_acc;
@@ -262,70 +277,92 @@ __device__ __forceinline__ void consume(const Job& jb, const Unit& u0, const Uni
 
 __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  Shared* sh = reinterpret_cast<Shared*>(smem + kWgStages * kStageBytes);
+  Shared* sh = reinterpret_cast<Shared*>(smem + kRingBytes);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  int job_id = 0, split = 0, nsplit = 1, half = 0, part_idx = 0;
-  const bool have = locate(p, blockIdx.x, job_id, split, nsplit, half, part_idx);
+  int job_id = 0, split = 0, nsplit = 1, half = 0, halves = 1, part_idx = 0;
+  const bool have = locate(p, blockIdx.x, job_id, split, nsplit, half, halves, part_idx);
   const Job jb = job_desc(job_id, half, (warp >> 2) & 1, p.compact);
   // contiguous tile range of this split
   const int per = (p.n_tiles + nsplit - 1) / nsplit;
   const int t_begin = have ? min(split * per, p.n_tiles) : 0;
   const int t_end = have ? min(t_begin + per, p.n_tiles) : 0;
   const int n_local = t_end - t_begin;
+  // the two halves of a NeRF-layer split share their B blocks with the other CTA of the cluster; every other CTA
+  // (head, bender jobs, an idle CTA) works alone and shares only the cluster barriers with its neighbour
+  const bool paired = have && halves == 2;
+  const uint32_t rank = cluster_ctarank(), partner = rank ^ 1u;
+  // both halves of a split have the same A and B block sizes, hence the same stage layout
+  const int stage_bytes = (jb.a_chunks + jb.b_chunks) * kChunkBytes;
+  const int n_stages = min(kMaxStages, kRingBytes / stage_bytes);
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kWgStages; ++i) {
+    for (int i = 0; i < n_stages; ++i) {
       mbar_init(&sh->full[i], 1);
-      mbar_init(&sh->empty[i], 8);   // one arrival per consumer warp
+      mbar_init(&sh->empty[i], paired ? 16 : 8);   // one arrival per consumer warp of every CTA that reads the stage
     }
     sh->abort_flag = 0;
     fence_mbar_init();
   }
-  __syncthreads();
-  const Waiter W{&sh->abort_flag, p.err};
+  // the partner's barriers are initialised before any multicast data or remote arrival can reach them
+  cluster_sync();
+  const Waiter W{&sh->abort_flag, p.err, paired, paired ? mapa_shared(&sh->abort_flag, partner) : 0u};
+  const Ring R{smem, stage_bytes, n_stages, paired, paired ? mapa_shared(&sh->empty[0], partner) : 0u};
 
   if (warp >= 8) {
     setmaxnreg_dec<kProducerRegs>();
-    // ===================== producer: whole image blocks, 16 KB bulk copies =====================
+    // ===================== producer: one tile's A and B blocks per stage, 16 KB bulk copies =====================
     if (warp == 8 && lane == 0) {
+      const uint32_t a_bytes = static_cast<uint32_t>(jb.a_chunks) * kChunkBytes, b_bytes = static_cast<uint32_t>(jb.b_chunks) * kChunkBytes;
+      // paired: this CTA fetches its own A block and its half of the B block, the latter multicast into both CTAs
+      const uint32_t b_begin = paired ? rank * (b_bytes / 2) : 0u, b_end = paired ? b_begin + b_bytes / 2 : b_bytes;
       uint32_t stage = 0, phase = 0;
-      for (int it = 0; it < 2 * n_local; ++it) {   // per tile: the A block, then the B block
-        const long long tile = t_begin + (it >> 1);
-        const bool is_b = (it & 1) != 0;
-        const uint8_t* src = is_b ? p.stash + tile * p.stash_tile_bytes + jb.b_off : p.gstash + tile * p.gstash_tile_bytes + jb.a_off;
-        const uint32_t bytes = static_cast<uint32_t>(is_b ? jb.b_chunks : jb.a_chunks) * kChunkBytes;
+      for (int it = 0; it < n_local; ++it) {
+        const long long tile = t_begin + it;
+        const uint8_t* a_src = p.gstash + tile * p.gstash_tile_bytes + jb.a_off;
+        const uint8_t* b_src = p.stash + tile * p.stash_tile_bytes + jb.b_off;
         W.wait(&sh->empty[stage], phase ^ 1u, 101);
-        mbar_arrive_expect_tx(&sh->full[stage], bytes);
-        uint8_t* dst = smem + stage * kStageBytes;
-        for (uint32_t o = 0; o < bytes; o += 16384u) tma_bulk_g2s(dst + o, src + o, bytes - o < 16384u ? bytes - o : 16384u, &sh->full[stage]);
-        if (++stage == kWgStages) { stage = 0; phase ^= 1u; }
+        mbar_arrive_expect_tx(&sh->full[stage], a_bytes + b_bytes);   // the partner delivers the other half of B
+        uint8_t* dst = smem + stage * stage_bytes;
+        for (uint32_t o = 0; o < a_bytes; o += kPieceBytes)
+          tma_bulk_g2s(dst + o, a_src + o, a_bytes - o < kPieceBytes ? a_bytes - o : kPieceBytes, &sh->full[stage]);
+        dst += a_bytes;
+        for (uint32_t o = b_begin; o < b_end; o += kPieceBytes) {
+          const uint32_t n = b_end - o < kPieceBytes ? b_end - o : kPieceBytes;
+          if (paired) tma_bulk_g2s_multicast(dst + o, b_src + o, n, &sh->full[stage], 0x3);
+          else tma_bulk_g2s(dst + o, b_src + o, n, &sh->full[stage]);
+        }
+        if (++stage == n_stages) { stage = 0; phase ^= 1u; }
       }
     }
-    return;
-  }
-
-  setmaxnreg_inc<kConsumerRegs>();
-  const int g = warp >> 2;
-  float* part = p.scratch + static_cast<size_t>(part_idx) * kWgScratchFloats;
-  const Unit& u0 = jb.u[0];
-  const Unit& u1 = jb.u[1];
-  if (job_id <= 9) {
-    const bool mine = u0.rows > 0;
-    if (job_id == 8 || job_id == 9) {
-      if (mine) consume<64, 0>(jb, u0, u1, smem, sh, W, n_local, part, have);
-      else consume<0, 0>(jb, u0, u1, smem, sh, W, n_local, part, have);
-    } else {
-      if (mine) consume<256, 0>(jb, u0, u1, smem, sh, W, n_local, part, have);
-      else consume<0, 0>(jb, u0, u1, smem, sh, W, n_local, part, have);
-    }
-  } else if (job_id == 10) {
-    if (g == 0) consume<64, 64>(jb, u0, u1, smem, sh, W, n_local, part, have);
-    else consume<96, 96>(jb, u0, u1, smem, sh, W, n_local, part, have);
   } else {
-    if (g == 0) consume<96, 96>(jb, u0, u1, smem, sh, W, n_local, part, have);
-    else consume<48, 48>(jb, u0, u1, smem, sh, W, n_local, part, have);
+    setmaxnreg_inc<kConsumerRegs>();
+    const int g = warp >> 2;
+    float* part = p.scratch + static_cast<size_t>(part_idx) * kWgScratchFloats;
+    const Unit& u0 = jb.u[0];
+    const Unit& u1 = jb.u[1];
+    if (job_id <= 9) {
+      const bool mine = u0.rows > 0;
+      if (job_id == 8 || job_id == 9) {
+        if (mine) consume<64, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
+        else consume<0, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
+      } else {
+        if (mine) consume<256, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
+        else consume<0, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
+      }
+    } else if (job_id == 10) {
+      if (g == 0) consume<64, 64>(jb, u0, u1, R, sh, W, n_local, part, have);
+      else consume<96, 96>(jb, u0, u1, R, sh, W, n_local, part, have);
+    } else {
+      if (g == 0) consume<96, 96>(jb, u0, u1, R, sh, W, n_local, part, have);
+      else consume<48, 48>(jb, u0, u1, R, sh, W, n_local, part, have);
+    }
   }
+  // No CTA leaves while its partner may still arrive on its barriers or write its abort flag.  Multicast data has
+  // landed: each CTA's consumers waited for every tile's full barrier.  Every thread gets here after a finite number of
+  // bounded waits (an abort reaches the partner through its abort flag), so this barrier cannot hang.
+  __syncwarp();
+  cluster_sync();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -491,43 +528,71 @@ __global__ void wgrad_reduce_kernel(const WgradParams p, const WgradDst dst, int
 
 // ------------------------------------------------------------------------------------------------
 cudaError_t launch_wgrad(WgradParams p, bool has_bender, int num_sms, const WgradDst& dst, int out_ch, cudaStream_t st) {
-  // relative cost of one tile of every job's CTAs = 2 KB chunks a CTA moves (a NeRF layer's half: 16 gradient chunks +
-  // the activation block); the head job (a 4 KB gradient block alternating with a 64 KB activation block keeps fewer
-  // bytes in flight) and the three-MMA bender job stream a little slower per byte, hence their surcharge
+  // relative cost of one tile of every job's CTAs = 2 KB chunks a CTA receives (a NeRF layer's half: 16 gradient
+  // chunks + the activation block); the head job and the three-MMA bender job stream a little slower per byte, hence
+  // their surcharge.  The plan decides how the fp32 partial sums associate: changing a weight changes the gradients'
+  // last bits.
   static const int kJobChunks[12] = {46, 48, 48, 48, 48, 48, 48, 48, 16 + 8 + 8, 16 + 8 + 8, 54, 24 + 18};
   int first = 0, last = has_bender ? 12 : 10;
   if (p.compact) { first = 10; last = 12; p.stash_tile_bytes = kTanTileBytes; p.gstash_tile_bytes = kAdjTileBytes; }
   else { p.stash_tile_bytes = kStashTileBytes; p.gstash_tile_bytes = kGradTileBytes; }
-  p.n_jobs = last - first;
+
+  // Launched in clusters of 2 CTAs (the two halves of a NeRF-layer split).  A cluster lives inside one GPC, so the
+  // CTAs that can run at once are the resident clusters x 2, which can be fewer than the SMs.
+  const size_t smem = kRingBytes + sizeof(Shared) + 64;
+  cudaError_t e = cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  cudaLaunchAttribute cluster{};
+  cluster.id = cudaLaunchAttributeClusterDimension;
+  cluster.val.clusterDim.x = 2; cluster.val.clusterDim.y = 1; cluster.val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(2); cfg.blockDim = dim3(kWgThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cfg.attrs = &cluster; cfg.numAttrs = 1;
+  static int s_max_clusters[64];   // per device
+  int dev = 0;
+  e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
+  if (s_max_clusters[dev] <= 0) {
+    e = cudaOccupancyMaxActiveClusters(&s_max_clusters[dev], wgrad_kernel, &cfg);
+    if (e != cudaSuccess) return e;
+    if (s_max_clusters[dev] <= 0) return cudaErrorInvalidConfiguration;
+  }
+  const int max_ctas = min(num_sms, 2 * s_max_clusters[dev]) & ~1;
+
   // Every CTA streams at about the same bytes/clk (the kernel is HBM-bound), so the launch ends when the CTA with the
   // most bytes ends: start with one split per job and hand each further split (its halves' CTAs) to the job whose CTAs
   // currently carry the most (chunks per tile x tiles per CTA).
-  int used = 0;
+  int splits[12], halves[12], used = 0;
   for (int j = first; j < last; ++j) {
-    p.job_ids[j - first] = j; p.splits[j - first] = 1;
-    p.halves[j - first] = (j >= 1 && j <= 9) ? 2 : 1;   // the head's 16-row dW and the bender jobs fit one CTA
-    used += p.halves[j - first];
+    splits[j] = 1;
+    halves[j] = (j >= 1 && j <= 9) ? 2 : 1;   // the head's 16-row dW and the bender jobs fit one CTA
+    used += halves[j];
   }
   const int tiles = p.n_tiles > 0 ? p.n_tiles : 1;
   for (;;) {
     int best = -1;
     long long best_load = -1;
     for (int j = first; j < last; ++j) {
-      const int sp = p.splits[j - first];
-      if (sp >= tiles || used + p.halves[j - first] > num_sms) continue;   // a CTA needs at least one tile
+      const int sp = splits[j];
+      if (sp >= tiles || used + halves[j] > max_ctas) continue;   // a CTA needs at least one tile
       const long long load = static_cast<long long>(kJobChunks[j]) * ((tiles + sp - 1) / sp);
       if (load > best_load) { best_load = load; best = j; }
     }
     if (best < 0) break;
-    ++p.splits[best - first];
-    used += p.halves[best - first];
+    ++splits[best];
+    used += halves[best];
   }
+  // CTA order: the two-half jobs first, so that the halves of every split are the two CTAs of one cluster; then the
+  // one-CTA jobs (head, bender; all jobs of the compact launch), two splits to a cluster without multicast, and one
+  // idle CTA when their count is odd.  The scratch partials follow the same order (wgrad_reduce_kernel looks jobs up).
+  p.n_jobs = 0;
+  for (int h = 2; h >= 1; --h)
+    for (int j = first; j < last; ++j)
+      if (halves[j] == h) { p.job_ids[p.n_jobs] = j; p.splits[p.n_jobs] = splits[j]; p.halves[p.n_jobs] = h; ++p.n_jobs; }
   if (p.n_tiles > 0) {
-    const size_t smem = kWgStages * kStageBytes + sizeof(Shared) + 64;
-    cudaError_t e = cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    wgrad_kernel<<<used, kWgThreads, smem, st>>>(p);
-    e = cudaGetLastError();
+    cfg.gridDim = dim3((used + 1) & ~1);
+    e = cudaLaunchKernelEx(&cfg, wgrad_kernel, p);
     if (e != cudaSuccess) return e;
   }
   const int n = dst.nerf_n + dst.bend_n;
