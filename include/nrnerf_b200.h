@@ -19,7 +19,7 @@
 extern "C" {
 #endif
 
-#define NRN_ABI_VERSION 2
+#define NRN_ABI_VERSION 3
 
 #define NRN_OK 0
 #define NRN_E_INVALID (-1)   /* bad argument / unsupported configuration */
@@ -94,6 +94,8 @@ typedef struct NrnFieldArgs {
   float* rigidity_mask;       /* out [P]    or NULL */
   void* stash;                /* training only: activation stash of nrn_stash_bytes() bytes, else NULL */
   void* stream;
+  void* relu_mask;            /* training only (given with stash, else NULL): ReLU masks for the backward pass,
+                                 nrn_relu_mask_bytes() bytes */
 } NrnFieldArgs;
 int nrn_field_forward(const NrnFieldArgs* args);
 
@@ -141,6 +143,7 @@ int nrn_composite_backward(const NrnCompositeBwdArgs* args);
  * nrn_field_forward (ray mode) and, with a bender, that call's unmasked_offsets / rigidity_mask. */
 size_t nrn_stash_bytes(int n_rays, int n_samples);
 size_t nrn_grad_stash_bytes(int n_rays, int n_samples);
+size_t nrn_relu_mask_bytes(int n_rays, int n_samples);   /* 1 bit per hidden activation: 40 KB per 128-point tile */
 size_t nrn_wgrad_scratch_bytes(void);
 int nrn_nerf_grad_floats(int out_ch);   /* flat order: W0 b0 W1 b1 ... W7 b7 Wout bout (reference shapes) */
 int nrn_bender_grad_floats(void);       /* flat order: network.0.w .0.b .1.w .1.b .2.w .2.b .3.w .3.b .4.w,
@@ -169,6 +172,7 @@ typedef struct NrnFieldBwdArgs {
    * adds to the destination instead of overwriting it (what autograd's AccumulateGrad would do). */
   float* nerf_grad_head;
   int32_t accumulate_nerf, accumulate_bender;
+  const void* relu_mask;          /* from the forward call (nrn_relu_mask_bytes()) */
 } NrnFieldBwdArgs;
 int nrn_field_backward(const NrnFieldBwdArgs* args);
 

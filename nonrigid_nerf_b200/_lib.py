@@ -11,7 +11,7 @@ import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libnrnerf_b200.so")
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 _f32p = C.POINTER(C.c_float)
 _vp = C.c_void_p
@@ -31,6 +31,7 @@ class NrnFieldArgs(C.Structure):
         ("masked_offsets", _vp), ("rigidity_mask", _vp),
         ("stash", _vp),
         ("stream", _vp),
+        ("relu_mask", _vp),
     ]
 
 
@@ -45,6 +46,7 @@ class NrnFieldBwdArgs(C.Structure):
         ("nerf_grad", _vp), ("bender_grad", _vp), ("d_latents", _vp),
         ("stream", _vp),
         ("nerf_grad_head", _vp), ("accumulate_nerf", C.c_int32), ("accumulate_bender", C.c_int32),
+        ("relu_mask", _vp),
     ]
 
 
@@ -135,6 +137,7 @@ SYMBOLS = {
     "nrn_composite_backward": (C.c_int, [C.POINTER(NrnCompositeBwdArgs)]),
     "nrn_stash_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "nrn_grad_stash_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "nrn_relu_mask_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "nrn_wgrad_scratch_bytes": (C.c_size_t, []),
     "nrn_nerf_grad_floats": (C.c_int, [C.c_int]),
     "nrn_bender_grad_floats": (C.c_int, []),

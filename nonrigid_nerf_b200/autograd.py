@@ -75,12 +75,15 @@ class _FieldTrainFn(torch.autograd.Function):
         n, s = z_vals.shape
         lib = _lib.load()
         stash = torch.empty(lib.nrn_stash_bytes(n, s), dtype=torch.uint8, device=z_vals.device)
-        raw, det = ops.field_forward(rays, z_vals, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, None, True, stash)
+        relu_mask = torch.empty(lib.nrn_relu_mask_bytes(n, s), dtype=torch.uint8, device=z_vals.device)
+        raw, det = ops.field_forward(rays, z_vals, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, None, True, stash,
+                                     relu_mask)
         ctx.net, ctx.n_nerf = net, n_nerf
         ctx.shape = (n, s, out_ch)
         ctx.knobs = (cutoff, scaling)
         ctx.packs = (nerf_pack, bender_pack)
         ctx.stash = stash
+        ctx.relu_mask = relu_mask
         ctx.params = params
         ctx.set_materialize_grads(False)
         if bender is not None:
@@ -112,7 +115,7 @@ class _FieldTrainFn(torch.autograd.Function):
         a.n_rays, a.n_samples, a.out_ch = n, s, out_ch
         d_raw = d_raw.contiguous().float()
         a.d_raw = d_raw.data_ptr()
-        a.stash = ctx.stash.data_ptr()
+        a.stash, a.relu_mask = ctx.stash.data_ptr(), ctx.relu_mask.data_ptr()
         gstash = torch.empty(lib.nrn_grad_stash_bytes(n, s), dtype=torch.uint8, device=dev)
         scratch = torch.empty(lib.nrn_wgrad_scratch_bytes(), dtype=torch.uint8, device=dev)
         a.grad_stash, a.wgrad_scratch = gstash.data_ptr(), scratch.data_ptr()
@@ -161,7 +164,7 @@ class _FieldTrainFn(torch.autograd.Function):
         a.stream = torch.cuda.current_stream().cuda_stream
         with torch.cuda.device(dev):
             _lib.check(lib.nrn_field_backward(C.byref(a)), "field_backward")
-        # the stash lives as long as the autograd node: backward(retain_graph=True) followed by a second backward()
+        # the stash and the ReLU masks live as long as the autograd node: backward(retain_graph=True) followed by a second backward()
         # over the same graph (test-latent pass of the reference loop, train.py:1595-1606) reads it again
         if nerf_grad is None:
             grads = [None] * len(nerf_p)

@@ -208,6 +208,8 @@ int nrn_field_forward(const NrnFieldArgs* a) {
   if (a->out_ch < 4 || a->out_ch > 5) return fail(NRN_E_INVALID, "nrn_field_forward: out_ch=%d unsupported (4 or 5)", a->out_ch);
   if (!aligned16(a->nerf_packed) || (a->bender_packed && !aligned16(a->bender_packed)))
     return fail(NRN_E_INVALID, "nrn_field_forward: packed weights must be 16-byte aligned");
+  if ((a->stash != nullptr) != (a->relu_mask != nullptr))
+    return fail(NRN_E_INVALID, "nrn_field_forward: training needs both the stash and the ReLU mask buffer (relu_mask)");
   DeviceState* ds;
   int rc = device_state(&ds);
   if (rc) return rc;
@@ -231,6 +233,7 @@ int nrn_field_forward(const NrnFieldArgs* a) {
   p.raw = a->raw; p.d_init = a->initial_input_pts; p.d_bent = a->input_pts; p.d_unmasked = a->unmasked_offsets;
   p.d_masked = a->masked_offsets; p.d_rigid = a->rigidity_mask;
   p.stash = static_cast<uint8_t*>(a->stash);
+  p.relu_mask = static_cast<uint8_t*>(a->relu_mask);
   if (a->stash && a->points) return fail(NRN_E_INVALID, "nrn_field_forward: the training stash needs ray mode");
   p.err = ds->err_word;
   cudaError_t e;
@@ -287,6 +290,7 @@ static long long even_tiles(int n_rays, int n_samples) {
 }
 size_t nrn_stash_bytes(int n_rays, int n_samples) { return static_cast<size_t>(even_tiles(n_rays, n_samples)) * nrn::kStashTileBytes; }
 size_t nrn_grad_stash_bytes(int n_rays, int n_samples) { return static_cast<size_t>(even_tiles(n_rays, n_samples)) * nrn::kGradTileBytes; }
+size_t nrn_relu_mask_bytes(int n_rays, int n_samples) { return static_cast<size_t>(even_tiles(n_rays, n_samples)) * nrn::kMaskTileBytes; }
 size_t nrn_wgrad_scratch_bytes(void) { return static_cast<size_t>(nrn::kWgMaxCtas) * nrn::kWgScratchFloats * sizeof(float); }
 int nrn_nerf_grad_floats(int out_ch) { return 256 * 63 + 256 + 6 * (65536 + 256) + 256 * 319 + 256 + out_ch * 257; }
 int nrn_bender_grad_floats(void) { return 16193; }
@@ -299,6 +303,7 @@ int nrn_field_backward(const NrnFieldBwdArgs* a) {
   const bool bend = a->bender_packed != nullptr;
   if (bend && (!a->unmasked_offsets || !a->rigidity_mask || !a->bender_grad || !a->d_latents))
     return fail(NRN_E_INVALID, "nrn_field_backward: bender needs unmasked_offsets, rigidity_mask, bender_grad, d_latents");
+  if (a->n_rays > 0 && !a->relu_mask) return fail(NRN_E_INVALID, "nrn_field_backward: null relu_mask (the ReLU masks of the forward call)");
   DeviceState* ds;
   int rc = device_state(&ds);
   if (rc) return rc;
@@ -335,6 +340,7 @@ int nrn_field_backward(const NrnFieldBwdArgs* a) {
   p.d_unmasked_up = a->d_unmasked_offsets; p.d_rigid_up = a->d_rigidity_mask;
   p.cutoff = a->rigidity_cutoff; p.use_cutoff = a->use_cutoff; p.scaling = a->scaling; p.use_scaling = a->use_scaling;
   p.d_latents = a->d_latents; p.err = ds->err_word;
+  p.relu_mask = static_cast<const uint8_t*>(a->relu_mask);
   e = nrn::launch_absmax(a->d_raw, p.P * a->out_ch, amax, st);
   // the regularisers' upstream gradients share the fp16 loss scale: they take part in the maximum, otherwise a large
   // offsets_loss_weight saturates them (or, with a vanishing data term, lets them underflow)

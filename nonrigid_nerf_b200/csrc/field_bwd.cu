@@ -50,32 +50,19 @@ __device__ __forceinline__ StepShape step_shape(int step) {
 
 __device__ __forceinline__ float clamp_h(float v) { return fminf(fmaxf(v, -65504.f), 65504.f); }
 
-// dY = dh * [h > 0]: accumulator columns [0, NCOLS), masked with the forward activation stashed as fp16 (`mask_img`:
-// the tile's stash image), written as fp16 to this warpgroup's rows of the next A operand `img`; the whole image then
-// goes to the gradient stash with bulk TMA stores.
+// dY = dh * [h > 0]: accumulator columns [0, NCOLS), masked with the forward's ReLU mask bits `m` (loaded before the
+// step's MMAs), written as fp16 to this warpgroup's rows of the next A operand `img`; the whole image then goes to the
+// gradient stash with bulk TMA stores.
 template <int NCOLS, int NR>
-__device__ __forceinline__ void epi_mask_store(const float (&acc)[NR], const uint8_t* __restrict__ mask_img, uint8_t* img, int g) {
+__device__ __forceinline__ void epi_mask_store(const float (&acc)[NR], const ReluMask<NCOLS>& m, uint8_t* img, int g) {
   const int r0 = g * kWgRows + acc_r0(), q = acc_q();
-  constexpr int kBlk = NCOLS / 8 < 8 ? NCOLS / 8 : 8;   // column groups whose mask loads are in flight together
 #pragma unroll
-  for (int j0 = 0; j0 < NCOLS / 8; j0 += kBlk) {
-    uint32_t m[kBlk][2];
+  for (int j = 0; j < NCOLS / 8; ++j) {
 #pragma unroll
-    for (int jj = 0; jj < kBlk; ++jj)
-#pragma unroll
-      for (int i = 0; i < 2; ++i)
-        m[jj][i] = __ldg(reinterpret_cast<const unsigned int*>(mask_img + (j0 + jj) * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q));
-#pragma unroll
-    for (int jj = 0; jj < kBlk; ++jj) {
-      const int j = j0 + jj;
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        // saturating convert, then multiply by the 0/1 mask of the stashed h on packed halves
-        const uint32_t g2 = pack_h2_sat(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-        const __half2 hm = __hgt2(*reinterpret_cast<const __half2*>(&m[jj][i]), __float2half2_rn(0.f));
-        const __half2 r2 = __hmul2(*reinterpret_cast<const __half2*>(&g2), hm);
-        *reinterpret_cast<uint32_t*>(img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = *reinterpret_cast<const uint32_t*>(&r2);
-      }
+    for (int i = 0; i < 2; ++i) {
+      // saturating convert, then multiply by the 0/1 mask on packed halves
+      const uint32_t g2 = pack_h2_sat(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+      *reinterpret_cast<uint32_t*>(img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = m.apply(i, j, g2);
     }
   }
 }
@@ -214,14 +201,13 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
       wg_bar(bar);
       if (wg_leader && chunks) store_rows(gs + off, act, g, chunks);
     };
-    // The ReLU masks come from the forward stash (read once, straight from HBM).  One thread pulls the image the
-    // NEXT step will read into L2 while this step's epilogue runs, so the per-thread loads find it there.
-    auto prefetch = [&](uint32_t off, uint32_t bytes) {
-      if (wg_leader) {
-        for (uint32_t o = 0; o < bytes; o += 16384u) tma_prefetch_l2(st_tile + off + o, bytes - o < 16384u ? bytes - o : 16384u);
-      }
+    // The ReLU masks are bits the forward kernel wrote (ReluMask): each thread loads its few words of a step's mask
+    // before that step's MMAs, which hide the latency.  The embedding pe_backward reads from the forward stash is pulled
+    // into L2 by one thread while the epilogue of the step before runs.
+    const uint8_t* mk = p.relu_mask + static_cast<long long>(tile) * kMaskTileBytes;
+    auto prefetch_e = [&]() {
+      if (wg_leader) tma_prefetch_l2(st_tile + kStE, kEBytes);
     };
-    prefetch(kStH + 7 * kHBytes, kHBytes);
     // ---- d_raw image: [g_r g_g g_b g_sigma 0 ...] (K = 16) ----
     stash_begin();
     if (row_thread) {
@@ -241,17 +227,18 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
     for (int s = 0; s < 3; ++s) {
       const StepShape sh_ = step_shape(s);
       float acc[128];
+      ReluMask<256> m;
+      m.load(mk + kMkH + (7 - s) * kMaskHBytes, g);
       wg_gemm<256>(acc, ring, sh_.nslabs, sh_.k16, a_slab, W, 300 + s);
-      if (s < 2) prefetch(kStH + (6 - s) * kHBytes, kHBytes); else prefetch(kStE, kEBytes);
+      if (s == 2) prefetch_e();
       stash_begin();
-      epi_mask_store<256>(acc, st_tile + kStH + (7 - s) * kHBytes, act, g);
+      epi_mask_store<256>(acc, m, act, g);
       ready(kGsY + (7 - s) * kHBytes, 32);
     }
     // ---- L5e^T: gradient into the skip-connected embedding ----
     {
       float acc[32];
       wg_gemm<64>(acc, ring, 1, 16, a_slab, W, 303);
-      prefetch(kStH + 4 * kHBytes, kHBytes);
       stage_cols<0, 8>(acc, stg, kBwdStageLd);
       wg_bar(bar);
       if (row_thread) pe_backward(my_stg, st + kStE, dx);
@@ -261,17 +248,18 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
 #pragma unroll 1
     for (int s = 0; s < 5; ++s) {
       float acc[128];
+      ReluMask<256> m;
+      m.load(mk + kMkH + (4 - s) * kMaskHBytes, g);
       wg_gemm<256>(acc, ring, 4, 4, a_slab, W, 304 + s);
-      if (s < 4) prefetch(kStH + (3 - s) * kHBytes, kHBytes); else prefetch(kStE, kEBytes);
+      if (s == 4) prefetch_e();
       stash_begin();
-      epi_mask_store<256>(acc, st_tile + kStH + (4 - s) * kHBytes, act, g);
+      epi_mask_store<256>(acc, m, act, g);
       ready(kGsY + (4 - s) * kHBytes, 32);
     }
     // ---- L0^T: gradient into the embedding; then through the bend ----
     {
       float acc[32];
       wg_gemm<64>(acc, ring, 1, 16, a_slab, W, 309);
-      if (HAS_BENDER) prefetch(kStHb4, 8 * kChunkBytes);
       stage_cols<0, 8>(acc, stg, kBwdStageLd);
       wg_bar(bar);
       if (row_thread) pe_backward(my_stg, st + kStE, dx);
@@ -311,19 +299,21 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
     // ---- B4^T -> dYb3 ----
     {
       float acc[32];
+      ReluMask<64> m;
+      m.load(mk + kMkHb4, g);
       wg_gemm<64>(acc, ring, 1, 1, a_slab, W, 310);
-      prefetch(kStHb3, 8 * kChunkBytes);
       stash_begin();
-      epi_mask_store<64>(acc, st_tile + kStHb4, act, g);
+      epi_mask_store<64>(acc, m, act, g);
       ready(kGsYb3, 8);
     }
     // ---- B3^T -> dYb2 = [dh * mask (64) | d rigidity pre-activation | 0 (15)] ----
     {
       float acc[32];
+      ReluMask<64> m;
+      m.load(mk + kMkHb3, g);
       wg_gemm<64>(acc, ring, 1, 4, a_slab, W, 311);
-      prefetch(kStHb2, 12 * kChunkBytes);
       stash_begin();
-      epi_mask_store<64>(acc, st_tile + kStHb3, act, g);
+      epi_mask_store<64>(acc, m, act, g);
       if (row_thread) {
         *reinterpret_cast<uint4*>(a_row + 8 * kChunkBytes) = make_uint4(pack_h2(clamp_h(drpre), 0.f), 0u, 0u, 0u);
         *reinterpret_cast<uint4*>(a_row + 9 * kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
@@ -333,14 +323,16 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
     // ---- B2^T -> dYb1, B1^T -> dYb0 ----
     {
       float acc[48];
+      ReluMask<96> m;
+      m.load(mk + kMkHb2, g);
       wg_gemm<96>(acc, ring, 1, 5, a_slab, W, 312);
-      prefetch(kStHb1, 12 * kChunkBytes);
       stash_begin();
-      epi_mask_store<96>(acc, st_tile + kStHb2, act, g);
+      epi_mask_store<96>(acc, m, act, g);
       ready(kGsYb1, 12);
+      m.load(mk + kMkHb1, g);
       wg_gemm<96>(acc, ring, 1, 6, a_slab, W, 313);
       stash_begin();
-      epi_mask_store<96>(acc, st_tile + kStHb1, act, g);
+      epi_mask_store<96>(acc, m, act, g);
       ready(kGsYb0, 12);
     }
     // ---- B0^T: d(bender input); columns 6..37 are the latent code -> per-ray reduction ----

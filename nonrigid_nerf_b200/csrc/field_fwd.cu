@@ -55,20 +55,27 @@ __device__ __forceinline__ uint32_t a_operand_offset(int step, uint32_t j) {
   return j * 8 * kChunkBytes;
 }
 
-// Accumulator columns [0, NCOLS) + bias, ReLU, fp16 -> this warpgroup's rows of the chunk-major image `img`.
-template <int NCOLS, int NR>
-__device__ __forceinline__ void epi_bias_relu_store(const float (&acc)[NR], const float* __restrict__ bias, uint8_t* img, int g) {
+// Accumulator columns [0, NCOLS) + bias, ReLU, fp16 -> this warpgroup's rows of the chunk-major image `img`.  MASK
+// (training kernel): also the ReLU mask bits of those elements -> this thread's words of the tile's mask image at
+// byte `mask_off` of `mask_tile`.
+template <int NCOLS, bool MASK, int NR>
+__device__ __forceinline__ void epi_bias_relu_store(const float (&acc)[NR], const float* __restrict__ bias, uint8_t* img, int g,
+                                                    uint8_t* mask_tile, int mask_off) {
   const int r0 = g * kWgRows + acc_r0(), q = acc_q();
+  ReluMask<NCOLS> m;
+  if constexpr (MASK) m.clear();
 #pragma unroll
   for (int j = 0; j < NCOLS / 8; ++j) {
     const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * q));
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       // one cvt.rn.relu.satfinite.f16x2 per two outputs: ReLU, clamp to fp16 range and pack in a single instruction
-      *reinterpret_cast<uint32_t*>(img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) =
-          pack_h2_relu_sat(acc[4 * j + 2 * i] + b.x, acc[4 * j + 2 * i + 1] + b.y);
+      const uint32_t h2 = pack_h2_relu_sat(acc[4 * j + 2 * i] + b.x, acc[4 * j + 2 * i + 1] + b.y);
+      *reinterpret_cast<uint32_t*>(img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = h2;
+      if constexpr (MASK) m.pack(i, j, h2);
     }
   }
+  if constexpr (MASK) m.store(mask_tile + mask_off, g);
 }
 
 // Positional encoding of one point (Embedder.embed, run_nerf_helpers.py:149-150 with the settings of
@@ -109,7 +116,8 @@ __device__ __forceinline__ void write_pe(const float (&x)[3], uint8_t* dst_row) 
 
 }  // namespace
 
-template <bool HAS_BENDER>
+// TRAIN: p.stash and p.relu_mask are given (the inference kernel carries none of the mask code)
+template <bool HAS_BENDER, bool TRAIN>
 __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* act = smem;                                  // H | E, 128 rows
@@ -175,6 +183,8 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
     // overwritten; it also orders every warp's wgmma reads of an operand before any warp rewrites it in place.
     // ready(): the image is complete and visible to the async proxy (wgmma operand, TMA store).
     uint8_t* st = p.stash ? p.stash + static_cast<long long>(tile) * kStashTileBytes : nullptr;
+    // ReLU masks for DGRAD (training): every row of the tile is written, those past P of a ragged last tile included
+    uint8_t* mk = TRAIN ? p.relu_mask + static_cast<long long>(tile) * kMaskTileBytes : nullptr;
     auto stash_begin = [&]() {
       if (st && wg_leader) tma_bulk_wait_read<0>();
       wg_bar(bar);
@@ -236,11 +246,11 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
         float acc[48];
         wg_gemm<96>(acc, ring, 1, 3, [&](uint32_t) { return a_e; }, W, 301);
         stash_begin();
-        epi_bias_relu_store<96>(acc, p.bend_bias, Hs, g);
+        epi_bias_relu_store<96, TRAIN>(acc, p.bend_bias, Hs, g, mk, kMkHb1);
         ready(kStHb1, Hs, 12);
         wg_gemm<96>(acc, ring, 1, 6, [&](uint32_t) { return a_h; }, W, 302);
         stash_begin();
-        epi_bias_relu_store<96>(acc, p.bend_bias + 96, Hs, g);
+        epi_bias_relu_store<96, TRAIN>(acc, p.bend_bias + 96, Hs, g, mk, kMkHb2);
         ready(kStHb2, Hs, 12);
       }
       // ---- B2: 64 offset hidden + rigidity output (column 64) ----
@@ -248,7 +258,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
         float acc[40];
         wg_gemm<80>(acc, ring, 1, 6, [&](uint32_t) { return a_h; }, W, 303);
         stash_begin();
-        epi_bias_relu_store<64>(acc, p.bend_bias + 192, Hs, g);
+        epi_bias_relu_store<64, TRAIN>(acc, p.bend_bias + 192, Hs, g, mk, kMkHb3);
         if (acc_q() == 0) {
           stg[acc_r0() * kFwdStageLd] = acc[32];
           stg[(acc_r0() + 8) * kFwdStageLd] = acc[34];
@@ -265,7 +275,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
         float acc[32];
         wg_gemm<64>(acc, ring, 1, 4, [&](uint32_t) { return a_h; }, W, 304);
         stash_begin();
-        epi_bias_relu_store<64>(acc, p.bend_bias + 272, Hs, g);
+        epi_bias_relu_store<64, TRAIN>(acc, p.bend_bias + 272, Hs, g, mk, kMkHb4);
         ready(kStHb4, Hs, 8);
       }
       // ---- B4: offsets; bend ----
@@ -307,7 +317,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
       float acc[128];
       wg_gemm<256>(acc, ring, s.nslabs, s.k16, [&](uint32_t j) { return a_h + a_operand_offset(step, j); }, W, 310 + L);
       stash_begin();
-      epi_bias_relu_store<256>(acc, p.nerf_bias + L * 256, Hs, g);
+      epi_bias_relu_store<256, TRAIN>(acc, p.nerf_bias + L * 256, Hs, g, mk, kMkH + L * kMaskHBytes);
       ready(kStH + L * kHBytes, Hs, 32);
     }
     // ---- head: raw = output_linear(h) (run_nerf_helpers.py:306) ----
@@ -336,21 +346,21 @@ size_t field_fwd_smem_bytes() {
   return kSlotBytes + kRingStages * kRingStageBytes + 2 * kWgRows * kFwdStageLd * sizeof(float) + sizeof(Shared) + 64;
 }
 
+template <bool HAS_BENDER, bool TRAIN>
+static cudaError_t launch_field_fwd_t(const FieldFwdParams& p, int grid, size_t smem, cudaStream_t stream) {
+  const cudaError_t e = cudaFuncSetAttribute(field_fwd_kernel<HAS_BENDER, TRAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  field_fwd_kernel<HAS_BENDER, TRAIN><<<grid, kFwdThreads, smem, stream>>>(p);
+  return cudaGetLastError();
+}
+
 cudaError_t launch_field_fwd(const FieldFwdParams& p, bool has_bender, int num_sms, cudaStream_t stream) {
   const size_t smem = field_fwd_smem_bytes();
   if (p.n_tiles <= 0) return cudaSuccess;
   const int grid = p.n_tiles < num_sms ? p.n_tiles : num_sms;
-  cudaError_t e;
-  if (has_bender) {
-    e = cudaFuncSetAttribute(field_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    field_fwd_kernel<true><<<grid, kFwdThreads, smem, stream>>>(p);
-  } else {
-    e = cudaFuncSetAttribute(field_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    field_fwd_kernel<false><<<grid, kFwdThreads, smem, stream>>>(p);
-  }
-  return cudaGetLastError();
+  const bool train = p.relu_mask != nullptr;   // the C ABI passes the ReLU masks exactly when it passes the stash
+  if (has_bender) return train ? launch_field_fwd_t<true, true>(p, grid, smem, stream) : launch_field_fwd_t<true, false>(p, grid, smem, stream);
+  return train ? launch_field_fwd_t<false, true>(p, grid, smem, stream) : launch_field_fwd_t<false, false>(p, grid, smem, stream);
 }
 
 }  // namespace nrn

@@ -94,6 +94,57 @@ __device__ __forceinline__ void wg_gemm(float (&acc)[N / 2], Ring& r, uint32_t n
 __device__ __forceinline__ int acc_r0() { return ((threadIdx.x >> 5) & 3) * 16 + ((threadIdx.x & 31) >> 2); }
 __device__ __forceinline__ int acc_q() { return threadIdx.x & 3; }
 
+// ReLU masks (layout in nrn_common.cuh), stored in the order of the accumulator so that the forward epilogue writes and
+// the DGRAD epilogue reads only its own words.  A row holds one 32-bit word per (q, h) with h < kH (h = 0 only for images
+// of at most 128 columns): bit k is [h > 0] of column 8 (16 h + k) + 2 q and bit 16 + k that of column
+// 8 (16 h + k) + 2 q + 1, k = 0..15.  A thread's kH words of row r0 + 8 i are contiguous, so a warp's words of one i
+// are 128 kH contiguous bytes.
+template <int NCOLS>
+struct ReluMask {
+  static constexpr int kH = NCOLS > 128 ? 2 : 1;
+  uint32_t w[2][kH];
+  // this thread's words of row r0 + 8 i in the mask image `img` of tile rows [64 g, 64 g + 64)
+  static __device__ __forceinline__ size_t offset(int g, int i) {
+    return static_cast<size_t>(g * kWgRows + acc_r0() + 8 * i) * (16 * kH) + acc_q() * (4 * kH);
+  }
+  __device__ __forceinline__ void clear() {
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int h = 0; h < kH; ++h) w[i][h] = 0u;
+  }
+  // forward: add column group j of row r0 + 8 i from the packed fp16 pair `h2` the epilogue stores (the same half > 0
+  // test DGRAD applied to the stashed fp16 activation, so an fp32 value that rounds to fp16 zero stays masked)
+  __device__ __forceinline__ void pack(int i, int j, uint32_t h2) {
+    w[i][j >> 4] |= __hgt2_mask(*reinterpret_cast<const __half2*>(&h2), __float2half2_rn(0.f)) & (0x00010001u << (j & 15));
+  }
+  __device__ __forceinline__ void store(uint8_t* img, int g) const {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      if constexpr (kH == 2) *reinterpret_cast<uint2*>(img + offset(g, i)) = make_uint2(w[i][0], w[i][1]);
+      else *reinterpret_cast<uint32_t*>(img + offset(g, i)) = w[i][0];
+    }
+  }
+  __device__ __forceinline__ void load(const uint8_t* __restrict__ img, int g) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      if constexpr (kH == 2) {
+        const uint2 v = __ldg(reinterpret_cast<const uint2*>(img + offset(g, i)));
+        w[i][0] = v.x; w[i][1] = v.y;
+      } else {
+        w[i][0] = __ldg(reinterpret_cast<const unsigned int*>(img + offset(g, i)));
+      }
+    }
+  }
+  // DGRAD: fp16 pair g2 of column group j, row r0 + 8 i, times the 0/1 mask: the same __hmul2 as with the stashed
+  // activation, so -0 for a masked negative gradient and NaN propagation are unchanged
+  __device__ __forceinline__ uint32_t apply(int i, int j, uint32_t g2) const {
+    const uint32_t one = ((w[i][j >> 4] >> (j & 15)) & 0x00010001u) * 0x3c00u;   // fp16 1.0 where the bit is set
+    const __half2 r2 = __hmul2(*reinterpret_cast<const __half2*>(&g2), *reinterpret_cast<const __half2*>(&one));
+    return *reinterpret_cast<const uint32_t*>(&r2);
+  }
+};
+
 // Column groups [J0, J0 + NJ) of the accumulator -> stage[row][8 (j - J0) + col % 8] (row = warpgroup-local, fp32),
 // for the per-row work of one thread per row.
 template <int J0, int NJ, int NR>

@@ -76,6 +76,17 @@ constexpr int kGsYb2 = kGsYb3 + 8 * kChunkBytes;           // 10 chunks (64 + ri
 constexpr int kGsYb1 = kGsYb2 + 10 * kChunkBytes;          // 12 chunks
 constexpr int kGsYb0 = kGsYb1 + 12 * kChunkBytes;          // 12 chunks
 constexpr int kGradTileBytes = kGsYb0 + 12 * kChunkBytes;  // 618,496
+// ReLU masks (forward -> DGRAD), per tile: one bit per element of H1..H8 and Hb1..Hb4 (the 64 ReLU columns of Hb3),
+// in the wgmma accumulator's own order (field_mma.cuh: relu_mask_*).  256-column images take 32 B per row, bender
+// images (<= 128 columns) 16 B per row.
+constexpr int kMaskHBytes = kTileM * 32;                   // 4 KB
+constexpr int kMaskBBytes = kTileM * 16;                   // 2 KB
+constexpr int kMkH = 0;                                    // H_l at kMkH + (l-1)*kMaskHBytes, l = 1..8
+constexpr int kMkHb1 = kMkH + 8 * kMaskHBytes;
+constexpr int kMkHb2 = kMkHb1 + kMaskBBytes;
+constexpr int kMkHb3 = kMkHb2 + kMaskBBytes;
+constexpr int kMkHb4 = kMkHb3 + kMaskBBytes;
+constexpr int kMaskTileBytes = kMkHb4 + kMaskBBytes;       // 40,960
 // compact stashes of the divergence regulariser (div.cu): only the bender images, same relative order
 constexpr int kTanTileBytes = kStashTileBytes - kStBin;    // 94,208: [e | t1 s1 | t2 s2 | t3 | t4]
 constexpr int kAdjTileBytes = kGradTileBytes - kGsYb4;     // 90,112: adjoints of the tangent chain
@@ -115,6 +126,7 @@ struct FieldBwdParams {
   int use_cutoff, use_scaling;
   float* d_latents;            // [n_rays][32] fp32, zero-initialised, accumulated with atomics
   int* err;
+  const uint8_t* relu_mask;    // ReLU masks of the forward call [n_tiles even][kMaskTileBytes]
 };
 
 // ------------------------------------------------------------------------------------------
@@ -145,6 +157,7 @@ struct FieldFwdParams {
   float* d_rigid;         // [P]    or null
   uint8_t* stash;         // training stash [n_tiles rounded up to even][kStashTileBytes] or null
   int* err;               // device error word (0 = ok)
+  uint8_t* relu_mask;     // training only (with stash): ReLU masks [n_tiles rounded up to even][kMaskTileBytes]
 };
 
 }  // namespace nrn

@@ -130,7 +130,7 @@ def sample_coarse(rays: torch.Tensor, n_samples: int, t_rand: Optional[torch.Ten
     return z
 
 
-def _field(rays, z_vals, points, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details, stash=None):
+def _field(rays, z_vals, points, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details, stash=None, relu_mask=None):
     a = _lib.NrnFieldArgs()
     keep = []
     if points is None:
@@ -188,6 +188,8 @@ def _field(rays, z_vals, points, latents, nerf_pack, bender_pack, out_ch, cutoff
             a.rigidity_mask = details["rigidity_mask"].data_ptr()
     if stash is not None:
         a.stash = stash.data_ptr()
+    if relu_mask is not None:
+        a.relu_mask = relu_mask.data_ptr()
     a.stream = torch.cuda.current_stream().cuda_stream
     with torch.cuda.device(dev):
         _lib.check(_lib.load().nrn_field_forward(C.byref(a)), "field_forward")
@@ -197,10 +199,13 @@ def _field(rays, z_vals, points, latents, nerf_pack, bender_pack, out_ch, cutoff
 def field_forward(rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[torch.Tensor], nerf_pack: torch.Tensor,
                   bender_pack: Optional[torch.Tensor], out_ch: int, cutoff: Optional[float] = None,
                   scaling: Optional[float] = None, removal: Optional[float] = None,
-                  want_details: bool = False, stash: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
+                  want_details: bool = False, stash: Optional[torch.Tensor] = None,
+                  relu_mask: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
     """One fused pass over rays x samples: raw [N, S, out_ch] (+ the reference's per-point `details`).
-    `stash` (uint8, nrn_stash_bytes) switches the kernel to training mode (activations kept for backward)."""
-    return _field(rays, z_vals, None, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details, stash)
+    `stash` (uint8, nrn_stash_bytes) with `relu_mask` (uint8, nrn_relu_mask_bytes) switches the kernel to training mode
+    (activations and ReLU masks kept for backward)."""
+    return _field(rays, z_vals, None, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details, stash,
+                  relu_mask)
 
 
 def field_forward_points(points: torch.Tensor, latents: Optional[torch.Tensor], nerf_pack: torch.Tensor,
