@@ -19,7 +19,7 @@
 extern "C" {
 #endif
 
-#define NRN_ABI_VERSION 3
+#define NRN_ABI_VERSION 4
 
 #define NRN_OK 0
 #define NRN_E_INVALID (-1)   /* bad argument / unsupported configuration */
@@ -178,19 +178,19 @@ int nrn_field_backward(const NrnFieldBwdArgs* args);
 
 /* ---- divergence regulariser of the offset field on the coarse samples: compute_divergence_loss /
  * divergence_approx (run_nerf_helpers.py:22-116) as driven by train.py:245-286, forward and backward
- * in closed form (no double backward).  Needs the coarse pass's activation stash. ---------------- */
+ * in closed form (no double backward), on tensor cores with the fp16 bender weights the coarse pass ran with.
+ * Needs that pass's ReLU masks (relu_mask of the training nrn_field_forward call) and its packed bender. ------ */
 size_t nrn_div_stash_bytes(int n_rays, int n_samples);
 size_t nrn_div_grad_stash_bytes(int n_rays, int n_samples);
 typedef struct NrnDivArgs {
   int32_t n_rays, n_samples;
-  const void* stash;               /* activation stash of the coarse nrn_field_forward call */
+  const void* relu_mask;           /* ReLU masks written by the coarse nrn_field_forward call (nrn_relu_mask_bytes()) */
   const float* e;                  /* [P][3] probe vectors ~ N(0, I) (torch.randn_like, run_nerf_helpers.py:110) */
   const float* unmasked_offsets;   /* [P][3] coarse pass output */
   const float* rigidity_mask;      /* [P]    coarse pass output */
   const float* weights;            /* [P]    1 - exp(-relu(opacity_alpha)), detached (train.py:267) ... */
   int32_t weights_are_opacity_alpha; /* ... or, if 1, opacity_alpha itself: the kernels apply 1 - exp(-relu(.)) */
-  const float* const* net_w;       /* 5: ray_bending.network.i.weight (fp32, reference layout) */
-  const float* const* rig_w;       /* 3: ray_bending.rigidity_network.i.weight */
+  const void* bender_packed;       /* nrn_pack_bender output the coarse pass ran with (16-byte aligned) */
   void* tangent_stash;             /* nrn_div_stash_bytes(): written by forward, read by backward */
   float* d; float* alpha; float* beta; float* tau_c;   /* [P] each: written by forward, read by backward */
   float* loss;                     /* forward out [n_rays]: mean over the ray's samples of weights * d^2 */

@@ -11,7 +11,7 @@ import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libnrnerf_b200.so")
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 _f32p = C.POINTER(C.c_float)
 _vp = C.c_void_p
@@ -53,9 +53,9 @@ class NrnFieldBwdArgs(C.Structure):
 class NrnDivArgs(C.Structure):
     _fields_ = [
         ("n_rays", C.c_int32), ("n_samples", C.c_int32),
-        ("stash", _vp), ("e", _vp), ("unmasked_offsets", _vp), ("rigidity_mask", _vp), ("weights", _vp),
+        ("relu_mask", _vp), ("e", _vp), ("unmasked_offsets", _vp), ("rigidity_mask", _vp), ("weights", _vp),
         ("weights_are_opacity_alpha", C.c_int32),
-        ("net_w", C.POINTER(_vp)), ("rig_w", C.POINTER(_vp)),
+        ("bender_packed", _vp),
         ("tangent_stash", _vp), ("d", _vp), ("alpha", _vp), ("beta", _vp), ("tau_c", _vp), ("loss", _vp),
         ("G", _vp), ("g_ray", _vp), ("G_workspace", _vp), ("adjoint_stash", _vp), ("wgrad_scratch", _vp), ("d_unmasked_offsets", _vp),
         ("d_rigidity_mask", _vp), ("bender_grad", _vp),

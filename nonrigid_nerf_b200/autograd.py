@@ -87,7 +87,7 @@ class _FieldTrainFn(torch.autograd.Function):
         ctx.params = params
         ctx.set_materialize_grads(False)
         if bender is not None:
-            _register_stash(det["unmasked_offsets"], stash)
+            _register_relu_mask(det["unmasked_offsets"], relu_mask)
             ctx.save_for_backward(det["unmasked_offsets"], det["rigidity_mask"])
             outs = (raw, det["unmasked_offsets"], det["rigidity_mask"], det["initial_input_pts"], det["input_pts"],
                     det["masked_offsets"])
@@ -238,30 +238,30 @@ def gather_latents(latents, timestep: torch.Tensor) -> torch.Tensor:
 # ---------------------------------------------------------------------------------------------
 # divergence regulariser (fused; SURVEY.md section 8f row f2)
 # ---------------------------------------------------------------------------------------------
-_STASH_BY_PTR = {}   # data_ptr of a coarse pass's unmasked_offsets -> weakref to that pass's activation stash
+_MASK_BY_PTR = {}   # data_ptr of a coarse pass's unmasked_offsets -> weakref to that pass's ReLU masks
 
 
-def _register_stash(unmasked: torch.Tensor, stash: torch.Tensor) -> None:
+def _register_relu_mask(unmasked: torch.Tensor, relu_mask: torch.Tensor) -> None:
     import weakref
-    for k in [k for k, v in _STASH_BY_PTR.items() if v() is None]:
-        del _STASH_BY_PTR[k]
-    _STASH_BY_PTR[unmasked.data_ptr()] = weakref.ref(stash)
+    for k in [k for k, v in _MASK_BY_PTR.items() if v() is None]:
+        del _MASK_BY_PTR[k]
+    _MASK_BY_PTR[unmasked.data_ptr()] = weakref.ref(relu_mask)
 
 
-def lookup_stash(unmasked: torch.Tensor) -> Optional[torch.Tensor]:
-    """The activation stash of the coarse pass that produced `unmasked`: found by walking the tensor's autograd history
-    (through the reshapes of render()) to the _FieldTrainFn node, which owns the stash; the address table is only the
+def lookup_relu_mask(unmasked: torch.Tensor) -> Optional[torch.Tensor]:
+    """The ReLU masks of the coarse pass that produced `unmasked`: found by walking the tensor's autograd history
+    (through the reshapes of render()) to the _FieldTrainFn node, which owns them; the address table is only the
     fallback for detached tensors."""
     fn = unmasked.grad_fn
     for _ in range(8):
         if fn is None:
             break
-        stash = getattr(fn, "stash", None)
-        if isinstance(stash, torch.Tensor):
-            return stash
+        relu_mask = getattr(fn, "relu_mask", None)
+        if isinstance(relu_mask, torch.Tensor):
+            return relu_mask
         nxt = [f for f, _ in fn.next_functions if f is not None]
         fn = nxt[0] if len(nxt) == 1 else None
-    ref = _STASH_BY_PTR.get(unmasked.data_ptr())
+    ref = _MASK_BY_PTR.get(unmasked.data_ptr())
     return ref() if ref is not None else None
 
 
@@ -269,7 +269,7 @@ class _DivergenceFn(torch.autograd.Function):
     """per-ray mean_s(w * (e^T J e)^2) of the offset field, closed-form forward and backward (csrc/div.cu)."""
 
     @staticmethod
-    def forward(ctx, unmasked, rigidity, weights, e, stash, bender, w_is_alpha, *bend_p):
+    def forward(ctx, unmasked, rigidity, weights, e, relu_mask, bender, w_is_alpha, *bend_p):
         n, s = unmasked.shape[0], unmasked.shape[1]
         dev = unmasked.device
         lib = _lib.load()
@@ -279,22 +279,20 @@ class _DivergenceFn(torch.autograd.Function):
         rg = rigidity.detach().contiguous().float()
         w = weights.detach().contiguous().float()
         e = e.contiguous().float()
-        net_w, _, rig_w, _ = ops.bender_param_list(bender)
-        net_arr = ops._ptr_array([t.detach() for t in net_w])
-        rig_arr = ops._ptr_array([t.detach() for t in rig_w])
+        bender_pack = ops.pack_bender(bender)   # the cached fp16 images the coarse pass ran with
         tan = torch.empty(lib.nrn_div_stash_bytes(n, s), dtype=torch.uint8, device=dev)
         scal = torch.empty(4, n * s, dtype=torch.float32, device=dev)
         loss = torch.empty(n, dtype=torch.float32, device=dev)
-        a.stash, a.e, a.unmasked_offsets, a.rigidity_mask, a.weights = stash.data_ptr(), e.data_ptr(), un.data_ptr(), rg.data_ptr(), w.data_ptr()
+        a.relu_mask, a.e, a.unmasked_offsets, a.rigidity_mask, a.weights = relu_mask.data_ptr(), e.data_ptr(), un.data_ptr(), rg.data_ptr(), w.data_ptr()
         a.weights_are_opacity_alpha = 1 if w_is_alpha else 0
-        a.net_w, a.rig_w = net_arr, rig_arr
+        a.bender_packed = bender_pack.data_ptr()
         a.tangent_stash = tan.data_ptr()
         a.d, a.alpha, a.beta, a.tau_c = (scal[i].data_ptr() for i in range(4))
         a.loss = loss.data_ptr()
         a.stream = torch.cuda.current_stream().cuda_stream
         with torch.cuda.device(dev):
             _lib.check(lib.nrn_divergence_forward(C.byref(a)), "divergence_forward")
-        ctx.keep = (un, rg, w, e, stash, tan, scal, bender)
+        ctx.keep = (un, rg, w, e, relu_mask, bender_pack, tan, scal, bender)
         ctx.bend_p = bend_p
         ctx.w_is_alpha = bool(w_is_alpha)
         ctx.shape = (n, s)
@@ -303,7 +301,7 @@ class _DivergenceFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g):
-        un, rg, w, e, stash, tan, scal, bender = ctx.keep
+        un, rg, w, e, relu_mask, bender_pack, tan, scal, bender = ctx.keep
         n, s = ctx.shape
         dev = un.device
         lib = _lib.load()
@@ -312,12 +310,9 @@ class _DivergenceFn(torch.autograd.Function):
         G = torch.empty(n * s, dtype=torch.float32, device=dev)
         a = _lib.NrnDivArgs()
         a.n_rays, a.n_samples = n, s
-        net_w, _, rig_w, _ = ops.bender_param_list(bender)
-        net_arr = ops._ptr_array([t.detach() for t in net_w])
-        rig_arr = ops._ptr_array([t.detach() for t in rig_w])
-        a.stash, a.e, a.unmasked_offsets, a.rigidity_mask, a.weights = stash.data_ptr(), e.data_ptr(), un.data_ptr(), rg.data_ptr(), w.data_ptr()
+        a.relu_mask, a.e, a.unmasked_offsets, a.rigidity_mask, a.weights = relu_mask.data_ptr(), e.data_ptr(), un.data_ptr(), rg.data_ptr(), w.data_ptr()
         a.weights_are_opacity_alpha = 1 if ctx.w_is_alpha else 0
-        a.net_w, a.rig_w = net_arr, rig_arr
+        a.bender_packed = bender_pack.data_ptr()
         a.tangent_stash = tan.data_ptr()
         a.d, a.alpha, a.beta, a.tau_c = (scal[i].data_ptr() for i in range(4))
         a.g_ray, a.G_workspace = g.data_ptr(), G.data_ptr()
@@ -348,22 +343,22 @@ class _DivergenceFn(torch.autograd.Function):
 def divergence_loss(unmasked: torch.Tensor, rigidity: torch.Tensor, weights: Optional[torch.Tensor], bender,
                     e: Optional[torch.Tensor] = None, opacity_alpha: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Fused divergence regulariser on the coarse samples of the LAST differentiable coarse pass.
-    unmasked [N,S,3], rigidity [N,S,1] must be that pass's outputs (they locate its activation stash and
+    unmasked [N,S,3], rigidity [N,S,1] must be that pass's outputs (they locate its ReLU masks and
     carry the gradient w.r.t. the primal bender evaluation); weights [N,S] are used detached; `e` [N*S,3]
     are the Hutchinson probes (drawn with torch.randn like run_nerf_helpers.py:110 when None).
     Instead of `weights`, `opacity_alpha` [N,S] may be given: the kernels then apply the reference's
     1 - exp(-relu(opacity_alpha)) (train.py:267) themselves."""
-    stash = lookup_stash(unmasked)
-    if stash is None:
-        raise RuntimeError("nonrigid_nerf_b200: no activation stash for these offsets -- the fused divergence term needs the "
+    relu_mask = lookup_relu_mask(unmasked)
+    if relu_mask is None:
+        raise RuntimeError("nonrigid_nerf_b200: no ReLU masks for these offsets -- the fused divergence term needs the "
                            "un-chunked coarse pass of the current differentiable render() call (N_rand <= chunk)")
     n, s = unmasked.shape[0], unmasked.shape[1]
     if e is None:
         e = torch.randn(n * s, 3, device=unmasked.device)
     _, bend_p = _flat_params_bender(bender)
     if opacity_alpha is not None:
-        return _DivergenceFn.apply(unmasked, rigidity, opacity_alpha, e, stash, bender, True, *bend_p)
-    return _DivergenceFn.apply(unmasked, rigidity, weights, e, stash, bender, False, *bend_p)
+        return _DivergenceFn.apply(unmasked, rigidity, opacity_alpha, e, relu_mask, bender, True, *bend_p)
+    return _DivergenceFn.apply(unmasked, rigidity, weights, e, relu_mask, bender, False, *bend_p)
 
 
 def _flat_params_bender(bender):

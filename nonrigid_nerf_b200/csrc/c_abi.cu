@@ -365,15 +365,17 @@ size_t nrn_div_grad_stash_bytes(int n_rays, int n_samples) { return static_cast<
 static int fill_div(const NrnDivArgs* a, nrn::DivParams& p, const char* who) {
   if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
   if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "%s: bad sizes", who);
-  if (!a->stash || !a->e || !a->unmasked_offsets || !a->rigidity_mask || !a->weights || !a->net_w || !a->rig_w || !a->tangent_stash ||
-      !a->d || !a->alpha || !a->beta || !a->tau_c)
+  if (!a->relu_mask) return fail(NRN_E_INVALID, "%s: null relu_mask (the ReLU masks of the coarse nrn_field_forward call)", who);
+  if (!a->bender_packed) return fail(NRN_E_INVALID, "%s: null bender_packed (the nrn_pack_bender output the coarse pass ran with)", who);
+  if (!aligned16(a->bender_packed)) return fail(NRN_E_INVALID, "%s: bender_packed must be 16-byte aligned", who);
+  if (!a->e || !a->unmasked_offsets || !a->rigidity_mask || !a->weights || !a->tangent_stash || !a->d || !a->alpha || !a->beta ||
+      !a->tau_c)
     return fail(NRN_E_INVALID, "%s: null argument", who);
   p.P = static_cast<long long>(a->n_rays) * a->n_samples;
   p.S = a->n_samples; p.n_rays = a->n_rays;
-  p.stash = static_cast<const uint8_t*>(a->stash);
+  p.relu_mask = static_cast<const uint8_t*>(a->relu_mask);
+  p.bender = static_cast<const uint8_t*>(a->bender_packed);
   p.e = a->e; p.unmasked = a->unmasked_offsets; p.rigidity = a->rigidity_mask; p.w = a->weights; p.w_is_alpha = a->weights_are_opacity_alpha != 0;
-  for (int i = 0; i < 5; ++i) { if (!a->net_w[i]) return fail(NRN_E_INVALID, "%s: null weight", who); p.net_w[i] = a->net_w[i]; }
-  for (int i = 0; i < 3; ++i) { if (!a->rig_w[i]) return fail(NRN_E_INVALID, "%s: null weight", who); p.rig_w[i] = a->rig_w[i]; }
   p.tan = static_cast<uint8_t*>(a->tangent_stash);
   p.d = a->d; p.adot = a->alpha; p.beta = a->beta; p.tauc = a->tau_c;
   return NRN_OK;
@@ -384,11 +386,15 @@ int nrn_divergence_forward(const NrnDivArgs* a) {
   int rc = fill_div(a, p, "nrn_divergence_forward");
   if (rc) return rc;
   if (!a->loss) return fail(NRN_E_INVALID, "nrn_divergence_forward: null loss");
+  DeviceState* ds;
+  rc = device_state(&ds);
+  if (rc) return rc;
+  p.err = ds->err_word;
   cudaStream_t st = static_cast<cudaStream_t>(a->stream);
   cudaError_t e = cudaMemsetAsync(a->loss, 0, sizeof(float) * static_cast<size_t>(a->n_rays), st);
   if (e != cudaSuccess) return cuda_fail(e, "memset loss");
   p.loss = a->loss;
-  { ScopedTimer tm(5, st); e = nrn::launch_div_fwd(p, st); }
+  { ScopedTimer tm(5, st); e = nrn::launch_div_fwd(p, ds->num_sms, st); }
   return e == cudaSuccess ? NRN_OK : cuda_fail(e, "div_fwd_kernel");
 }
 
@@ -405,10 +411,10 @@ int nrn_divergence_backward(const NrnDivArgs* a) {
   cudaStream_t st = static_cast<cudaStream_t>(a->stream);
   float* amax = reinterpret_cast<float*>(ds->err_word + 2);
   p.G = a->G ? a->G : a->G_workspace; p.amax = amax; p.adj = static_cast<uint8_t*>(a->adjoint_stash);
-  p.d_unmasked = a->d_unmasked_offsets; p.d_rigid = a->d_rigidity_mask;
+  p.d_unmasked = a->d_unmasked_offsets; p.d_rigid = a->d_rigidity_mask; p.err = ds->err_word;
   cudaError_t e = a->G ? nrn::launch_absmax(a->G, p.P, amax, st) : nrn::launch_div_G(p, a->g_ray, a->G_workspace, amax, st);
   if (e != cudaSuccess) return cuda_fail(e, "absmax_kernel");
-  { ScopedTimer tm(5, st); e = nrn::launch_div_bwd(p, st); }
+  { ScopedTimer tm(5, st); e = nrn::launch_div_bwd(p, ds->num_sms, st); }
   if (e != cudaSuccess) return cuda_fail(e, "div_bwd_kernel");
   nrn::WgradParams w{};
   w.stash = p.tan; w.gstash = p.adj; w.scratch = a->wgrad_scratch; w.amax = amax; w.compact = 1;

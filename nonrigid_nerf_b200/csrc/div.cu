@@ -11,210 +11,310 @@
 //          = r * tau_off + off * tau_r                       (D_i, E_i: ReLU masks of the primal pass)
 //   d      = r * alpha + beta * tau_r,   alpha = e . tau_off,  beta = e . off,  tau_r = 2 r (1 - r) tau_c
 //
-// Forward kernel: the tangent chain t_i = D_i (W_{i-1} t_{i-1}) (no bias), per point, fp32 SIMT with
-// the weights in shared memory; masks come from the coarse pass's activation stash; the tangent
-// activations are written as fp16 chunk-major images (same layout as the bender part of the stash).
-// Backward kernel: given G = dL/dd per point, the adjoint chain of the tangent pass -> fp16 adjoint
-// images; the weight gradients  sum_p abar_i t_{i-1}^T  are then formed by the WGRAD kernel (compact
-// mode) exactly like the primal bender layers.  ReLU masks are piecewise constant, so no gradient
-// flows into them (autograd's double backward gives the same zeros).  The dependence on the PRIMAL
-// quantities r and off is returned as gradients w.r.t. the coarse pass's `rigidity_mask` and
-// `unmasked_offsets` outputs and continues through the ordinary field backward:
+// Both chains run on tensor cores as the bender steps of the field kernels (field_mma.cuh), with the ReLU mask bits the
+// primal pass wrote (ReluMask), at fp32 accuracy: every operand x is carried as x_hi = fp16(x) plus a residual
+// x_lo = fp16((x - x_hi) * 2048), weights included (ops.pack_bender writes the residual images), and a step is
+//   acc = (A_lo . W_hi + A_hi . W_lo) / 2048 + A_hi . W_hi       (fp32 accumulators; the A_lo . W_lo term is below fp32)
+// so the tangent is the derivative of the fp32 network, as an fp32 SIMT evaluation would give it.  The images stored for
+// WGRAD are the x_hi parts, i.e. the fp16 roundings of those fp32 values.
+//   forward  = the field forward's B0..B4 on the input row [e_hi e_lo | 0] (no bias; the epilogue multiplies by the
+//              primal mask instead of applying bias + ReLU).  tau_c is column 64 of B2, tau_off columns 0-2 of B4.
+//              The tangent images [e | t1 s1 | t2 s2 | t3 | t4] go to the tangent stash (layout of the forward stash's
+//              bender section).
+//   backward = DGRAD's B4^T..B1^T on [taubar_off | 0], with taubar_c in column 64 of the B3^T output (where DGRAD puts
+//              the rigidity pre-activation gradient), under the power-of-two loss scale of max|dL/dd|.  The adjoint
+//              images go to the adjoint stash (layout of the gradient stash's bender section).
+// The weight gradients  sum_p abar_i t_{i-1}^T  are then formed by the WGRAD kernel (compact mode) exactly like the
+// primal bender layers.  ReLU masks are piecewise constant, so no gradient flows into them (autograd's double backward
+// gives the same zeros).  The dependence on the PRIMAL quantities r and off is returned as gradients w.r.t. the coarse
+// pass's `rigidity_mask` and `unmasked_offsets` outputs and continues through the ordinary field backward:
 //   dL/d off = G tau_r e,     dL/d r = G (alpha + 2 beta tau_c (1 - 2 r))
-#include <cuda_fp16.h>
-#include "nrn_common.cuh"
+//
+// CTA: four consumer warpgroups, persistent over tiles; warpgroups 2p and 2p + 1 work on one tile (rows 0-63 / 64-127), so
+// two tiles are in flight per SM.  The weight images and their residuals (104 KB forward, 86 KB backward) are loaded once
+// per CTA by bulk TMA and stay resident, so there is no producer warp and no ring.
+#include "field_mma.cuh"
 #include "div.cuh"
 
 namespace nrn {
 
 namespace {
 
-constexpr int kDivThreads = 128;   // one tile per block
-// shared-memory weight table (fp32)
-constexpr int kW0x = 0;                   // [64][4]  (3 used)
-constexpr int kW1 = kW0x + 64 * 4;        // [64][64]
-constexpr int kW2 = kW1 + 4096;
-constexpr int kW3 = kW2 + 4096;
-constexpr int kW4 = kW3 + 4096;           // [3][64]
-constexpr int kR0 = kW4 + 192;            // [32][4]
-constexpr int kR1 = kR0 + 128;            // [32][32]
-constexpr int kR2 = kR1 + 1024;           // [32]
-constexpr int kWTotal = kR2 + 32;         // 13,920 floats
-constexpr int kActFloats = 64 * kDivThreads;   // per-thread activation column [k][thread]
+constexpr int kDivTilesPerCta = 2;                       // tiles in flight per CTA, two warpgroups each
+constexpr int kDivWgs = 2 * kDivTilesPerCta;
+constexpr int kDivThreads = 128 * kDivWgs;
+constexpr int kDivStageLd = 12;                          // floats per staged row: B4 columns 0-7, tau_c at 8
+constexpr int kDivImgBytes = 12 * kChunkBytes;           // widest image of either chain: 96 columns
+constexpr float kLoInv = 1.0f / kBendLoScale;
 
-// compact tile layouts (bytes): tangent stash and adjoint stash
+// tile layouts of the tangent stash and the adjoint stash (bytes)
 constexpr int kTE = 0, kT1 = 6 * kChunkBytes, kT2 = 18 * kChunkBytes, kT3 = 30 * kChunkBytes, kT4 = 38 * kChunkBytes;
 constexpr int kA4 = 0, kA3 = 2 * kChunkBytes, kA2 = 10 * kChunkBytes, kA1 = 20 * kChunkBytes, kA0 = 32 * kChunkBytes;
 
-__device__ __forceinline__ void load_weights(float* sw, const DivParams& p) {
-  for (int i = threadIdx.x; i < 64 * 4; i += blockDim.x) sw[kW0x + i] = (i & 3) < 3 ? p.net_w[0][(i >> 2) * 35 + (i & 3)] : 0.f;
-  for (int i = threadIdx.x; i < 4096; i += blockDim.x) {
-    sw[kW1 + i] = p.net_w[1][i];
-    sw[kW2 + i] = p.net_w[2][i];
-    sw[kW3 + i] = p.net_w[3][i];
-  }
-  for (int i = threadIdx.x; i < 192; i += blockDim.x) sw[kW4 + i] = p.net_w[4][i];
-  for (int i = threadIdx.x; i < 32 * 4; i += blockDim.x) sw[kR0 + i] = (i & 3) < 3 ? p.rig_w[0][(i >> 2) * 3 + (i & 3)] : 0.f;
-  for (int i = threadIdx.x; i < 1024; i += blockDim.x) sw[kR1 + i] = p.rig_w[1][i];
-  for (int i = threadIdx.x; i < 32; i += blockDim.x) sw[kR2 + i] = p.rig_w[2][i];
+// resident weights (each with its residual image): B0..B4 (forward); B4^T..B1^T (backward: the probe e is not
+// differentiated)
+constexpr int kDivFwdWBytes = kBendWBytes;
+constexpr int kDivBwdWBytes = kBendTB4Bytes + kBendTB3Bytes + kBendTB2Bytes + kBendTB1Bytes;
+
+struct DivShared {
+  uint64_t w_full;
+  int abort_flag;
+};
+
+// shared memory: [per tile in flight: A image hi | A image lo] [weights hi | weights lo] [per-row staging] [barrier]
+constexpr size_t div_smem_bytes(int wbytes) {
+  return 2 * kDivTilesPerCta * kDivImgBytes + 2 * wbytes + kDivWgs * kWgRows * kDivStageLd * sizeof(float) + sizeof(DivShared);
+}
+static_assert(div_smem_bytes(kDivFwdWBytes) <= 227 * 1024, "div kernels: shared memory of one CTA per SM");
+
+struct DivSmem {
+  uint8_t* img_hi;   // this warpgroup's tile: fp16 parts (the images stored for WGRAD)
+  uint8_t* img_lo;   //                        scaled residuals
+  uint8_t* w_hi;
+  uint8_t* w_lo;
+  float* stage;      // this warpgroup's 64 rows
+  DivShared* sh;
+};
+__device__ __forceinline__ DivSmem div_smem(uint8_t* smem, int wbytes, int wg) {
+  DivSmem s;
+  s.img_hi = smem + (wg >> 1) * 2 * kDivImgBytes;
+  s.img_lo = s.img_hi + kDivImgBytes;
+  s.w_hi = smem + 2 * kDivTilesPerCta * kDivImgBytes;
+  s.w_lo = s.w_hi + wbytes;
+  float* stage_all = reinterpret_cast<float*>(s.w_lo + wbytes);
+  s.stage = stage_all + wg * kWgRows * kDivStageLd;
+  s.sh = reinterpret_cast<DivShared*>(stage_all + kDivWgs * kWgRows * kDivStageLd);
+  return s;
 }
 
-// bit j = (stashed fp16 activation j > 0), over `nchunks` consecutive chunks of this thread's row
-__device__ __forceinline__ unsigned long long read_mask(const uint8_t* row, int nchunks) {
-  unsigned long long m = 0ull;
-  for (int c = 0; c < nchunks; ++c) {
-    const uint4 w = __ldg(reinterpret_cast<const uint4*>(row + c * kChunkBytes));
-    const uint32_t ww[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      if (ww[q] & 0x7fffu) m |= 1ull << (c * 8 + 2 * q);
-      if (ww[q] & 0x7fff0000u) m |= 1ull << (c * 8 + 2 * q + 1);
+// one thread starts the bulk copies of the weight images and their residuals; every consumer waits on sh->w_full
+// (phase 0) before its first MMA
+__device__ __forceinline__ void load_resident_weights(const DivSmem& s, const uint8_t* hi, const uint8_t* lo, uint32_t bytes) {
+  if (threadIdx.x == 0) {
+    mbar_init(&s.sh->w_full, 1);
+    s.sh->abort_flag = 0;
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(&s.sh->w_full, 2 * bytes);
+    for (uint32_t off = 0; off < bytes; off += 16384u) {
+      tma_bulk_g2s(s.w_hi + off, hi + off, min(bytes - off, 16384u), &s.sh->w_full);
+      tma_bulk_g2s(s.w_lo + off, lo + off, min(bytes - off, 16384u), &s.sh->w_full);
     }
   }
-  return m;
 }
 
-__device__ __forceinline__ uint32_t pk(float a, float b) {
-  __half2 h = __floats2half2_rn(fminf(fmaxf(a, -65504.f), 65504.f), fminf(fmaxf(b, -65504.f), 65504.f));
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-
-// out[j] = sum_k W[j][k] in[k]  (W row-major [OUT][IN] in smem, `in` in registers), out -> act column
-template <int IN>
-__device__ __forceinline__ void matvec(const float* W, const float (&in)[IN], float* act, int OUT) {
+// acc[64 x N] = (A_lo . W_hi + A_hi . W_lo) / kBendLoScale + A_hi . W_hi over k16 steps of 16 columns, all operands in
+// shared memory: A = this warpgroup's rows of chunk-major images of kTileM rows (fenced for the async proxy, warpgroup
+// synced), W = resident N-row weight images at byte `w_off`.  A_LO = false: the A residual is zero (the probe input, whose
+// hi / lo split lives in its columns).  The small terms are summed first, scaled exactly, then the main products added.
+template <int N, bool A_LO>
+__device__ __forceinline__ void wg_mma_split(float (&acc)[N / 2], uint32_t a_hi, uint32_t a_lo, const DivSmem& s, uint32_t w_off,
+                                             uint32_t k16) {
+  const uint64_t ahi = gmma_desc(a_hi, kChunkBytes, 128), alo = gmma_desc(a_lo, kChunkBytes, 128);
+  const uint64_t whi = gmma_desc(smem_u32(s.w_hi) + w_off, N * 16, 128), wlo = gmma_desc(smem_u32(s.w_lo) + w_off, N * 16, 128);
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  acc_fence(acc);
+  wgmma_fence();
 #pragma unroll 1
-  for (int j0 = 0; j0 < OUT; j0 += 4) {
-    float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-#pragma unroll
-    for (int k = 0; k < IN; k += 4) {
-      const float4 w0 = *reinterpret_cast<const float4*>(W + (j0 + 0) * IN + k);
-      const float4 w1 = *reinterpret_cast<const float4*>(W + (j0 + 1) * IN + k);
-      const float4 w2 = *reinterpret_cast<const float4*>(W + (j0 + 2) * IN + k);
-      const float4 w3 = *reinterpret_cast<const float4*>(W + (j0 + 3) * IN + k);
-      a0 += w0.x * in[k] + w0.y * in[k + 1] + w0.z * in[k + 2] + w0.w * in[k + 3];
-      a1 += w1.x * in[k] + w1.y * in[k + 1] + w1.z * in[k + 2] + w1.w * in[k + 3];
-      a2 += w2.x * in[k] + w2.y * in[k + 1] + w2.z * in[k + 2] + w2.w * in[k + 3];
-      a3 += w3.x * in[k] + w3.y * in[k + 1] + w3.z * in[k + 2] + w3.w * in[k + 3];
-    }
-    act[(j0 + 0) * kDivThreads] = a0; act[(j0 + 1) * kDivThreads] = a1;
-    act[(j0 + 2) * kDivThreads] = a2; act[(j0 + 3) * kDivThreads] = a3;
+  for (uint32_t k = 0; k < k16; ++k) {
+    if (A_LO) wgmma<N, 0, 0>(acc, gmma_desc_advance(alo, k * 2 * kChunkBytes), gmma_desc_advance(whi, k * 2 * N * 16), 1u);
+    wgmma<N, 0, 0>(acc, gmma_desc_advance(ahi, k * 2 * kChunkBytes), gmma_desc_advance(wlo, k * 2 * N * 16), 1u);
   }
-}
-// out[k] = sum_j W[j][k] in[j]  (transposed product; W row-major [NJ][NK] in smem)
-template <int NJ>
-__device__ __forceinline__ void matvec_t(const float* W, const float (&in)[NJ], float* act, int NK) {
+  wgmma_commit();
+  wgmma_wait<0>();
+  acc_fence(acc);
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] *= kLoInv;
+  acc_fence(acc);
+  wgmma_fence();
 #pragma unroll 1
-  for (int k0 = 0; k0 < NK; k0 += 4) {
-    float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-#pragma unroll
-    for (int j = 0; j < NJ; ++j) {
-      const float4 w = *reinterpret_cast<const float4*>(W + j * NK + k0);
-      a0 += w.x * in[j]; a1 += w.y * in[j]; a2 += w.z * in[j]; a3 += w.w * in[j];
-    }
-    act[(k0 + 0) * kDivThreads] = a0; act[(k0 + 1) * kDivThreads] = a1;
-    act[(k0 + 2) * kDivThreads] = a2; act[(k0 + 3) * kDivThreads] = a3;
-  }
+  for (uint32_t k = 0; k < k16; ++k)
+    wgmma<N, 0, 0>(acc, gmma_desc_advance(ahi, k * 2 * kChunkBytes), gmma_desc_advance(whi, k * 2 * N * 16), 1u);
+  wgmma_commit();
+  wgmma_wait<0>();
+  acc_fence(acc);
 }
-// masked copy act column -> registers, and fp16 image chunks [chunk0, chunk0 + N/8) of this row
-template <int N>
-__device__ __forceinline__ void take(const float* act, unsigned long long mask, float scale, float (&out)[N], uint8_t* img_row) {
+
+// fp32 pair -> {fp16 part, scaled fp16 residual}, each packed as fp16x2 (saturating)
+__device__ __forceinline__ uint2 split_h2(float a, float b) {
+  const uint32_t hi = pack_h2_sat(a, b);
+  const float2 h = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+  return make_uint2(hi, pack_h2_sat((a - h.x) * kBendLoScale, (b - h.y) * kBendLoScale));
+}
+
+// Accumulator columns [0, NCOLS) times the primal ReLU mask bits -> this warpgroup's rows (half `h` of the tile) of the
+// next A operand, as fp16 parts (img_hi) and residuals (img_lo)
+template <int NCOLS, int NR>
+__device__ __forceinline__ void epi_mask_split(const float (&acc)[NR], const ReluMask<NCOLS>& m, const DivSmem& s, int h) {
+  const int r0 = h * kWgRows + acc_r0(), q = acc_q();
 #pragma unroll
-  for (int j = 0; j < N; ++j) out[j] = ((mask >> j) & 1ull) ? act[j * kDivThreads] * scale : 0.f;
+  for (int j = 0; j < NCOLS / 8; ++j) {
 #pragma unroll
-  for (int c = 0; c < N / 8; ++c) {
-    const uint4 v = make_uint4(pk(out[c * 8], out[c * 8 + 1]), pk(out[c * 8 + 2], out[c * 8 + 3]), pk(out[c * 8 + 4], out[c * 8 + 5]),
-                               pk(out[c * 8 + 6], out[c * 8 + 7]));
-    *reinterpret_cast<uint4*>(img_row + c * kChunkBytes) = v;
+    for (int i = 0; i < 2; ++i) {
+      const uint2 v = split_h2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+      const int off = j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q;
+      *reinterpret_cast<uint32_t*>(s.img_hi + off) = m.apply(i, j, v.x);
+      *reinterpret_cast<uint32_t*>(s.img_lo + off) = m.apply(i, j, v.y);
+    }
   }
 }
 
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kDivThreads) div_fwd_kernel(const DivParams p) {
-  extern __shared__ __align__(16) float sm[];
-  float* sw = sm;
-  float* act = sm + kWTotal + threadIdx.x;   // column of this thread: act[k * 128]
-  load_weights(sw, p);
-  __syncthreads();
-  const long long tile = blockIdx.x;
-  const int row = threadIdx.x;
-  const long long pt = tile * kTileM + row;
-  const bool valid = pt < p.P;
-  const uint8_t* st = p.stash + tile * kStashTileBytes + row * 16;
-  uint8_t* tn = p.tan + tile * kTanTileBytes + row * 16;
+__global__ void __launch_bounds__(kDivThreads, 1) div_fwd_kernel(const DivParams p) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  const int wg = threadIdx.x >> 7;
+  const int h = wg & 1;                   // half of the tile: rows [64 h, 64 h + 64)
+  const DivSmem s = div_smem(smem, kDivFwdWBytes, wg);
+  load_resident_weights(s, p.bender, p.bender + kBendLoOffset, kDivFwdWBytes);
+  const Waiter W{&s.sh->abort_flag, p.err};
 
-  float e[4] = {0.f, 0.f, 0.f, 0.f}, off[3] = {0.f, 0.f, 0.f};
-  float r = 0.f, w = 0.f;
-  if (valid) {
-#pragma unroll
-    for (int d = 0; d < 3; ++d) { e[d] = p.e[pt * 3 + d]; off[d] = p.unmasked[pt * 3 + d]; }
-    r = p.rigidity[pt];
-    w = p.w[pt];
-    if (p.w_is_alpha) w = 1.0f - expf(-fmaxf(w, 0.f));
-  }
-  // e image (bender-input layout: hi columns 0-2, lo columns 3-5)
-  {
-    float hi[3], lo[3];
-#pragma unroll
-    for (int d = 0; d < 3; ++d) { hi[d] = __half2float(__float2half_rn(e[d])); lo[d] = e[d] - hi[d]; }
-    *reinterpret_cast<uint4*>(tn + kTE) = make_uint4(pk(hi[0], hi[1]), pk(hi[2], lo[0]), pk(lo[1], lo[2]), 0u);
-    const uint4 zz = make_uint4(0u, 0u, 0u, 0u);
-#pragma unroll
-    for (int c = 1; c < 6; ++c) *reinterpret_cast<uint4*>(tn + kTE + c * kChunkBytes) = zz;
-  }
-  const unsigned long long m1 = read_mask(st + kStHb1, 8), e1 = read_mask(st + kStHb1 + 8 * kChunkBytes, 4);
-  const unsigned long long m2 = read_mask(st + kStHb2, 8), e2 = read_mask(st + kStHb2 + 8 * kChunkBytes, 4);
-  const unsigned long long m3 = read_mask(st + kStHb3, 8), m4 = read_mask(st + kStHb4, 8);
+  const int tw = threadIdx.x & 127;
+  const int lane = threadIdx.x & 31;
+  const bool row_thread = tw < kWgRows;   // threads 0-63 (warps 0, 1) of the warpgroup each own one row
+  const int bar = 1 + wg;
+  const bool wg_leader = tw == 0;
+  const int row_off = (h * kWgRows + tw) * 16;
+  const uint32_t a_hi = smem_u32(s.img_hi) + h * kWgRows * 16, a_lo = smem_u32(s.img_lo) + h * kWgRows * 16;
+  constexpr uint32_t w_b0 = 0, w_b1 = w_b0 + kBendB0Bytes, w_b2 = w_b1 + kBendB1Bytes, w_b3 = w_b2 + kBendB2Bytes,
+                     w_b4 = w_b3 + kBendB3Bytes;
+  const float* my_stg = s.stage + tw * kDivStageLd;
+  const long long n_tiles = (p.P + kTileM - 1) / kTileM;
 
-  float t[64], s[32];
-  // layer 0: t1 = D1 (W0[:, :3] e), s1 = E1 (R0 e)
-  matvec<4>(sw + kW0x, e, act, 64);
-  take<64>(act, m1, 1.0f, t, tn + kT1);
-  matvec<4>(sw + kR0, e, act, 32);
-  take<32>(act, e1, 1.0f, s, tn + kT1 + 8 * kChunkBytes);
-  // layer 1
-  matvec<64>(sw + kW1, t, act, 64);
-  take<64>(act, m2, 1.0f, t, tn + kT2);
-  matvec<32>(sw + kR1, s, act, 32);
-  take<32>(act, e2, 1.0f, s, tn + kT2 + 8 * kChunkBytes);
-  // layers 2, 3
-  matvec<64>(sw + kW2, t, act, 64);
-  take<64>(act, m3, 1.0f, t, tn + kT3);
-  matvec<64>(sw + kW3, t, act, 64);
-  take<64>(act, m4, 1.0f, t, tn + kT4);
-  // outputs
-  float tau_off[3] = {0.f, 0.f, 0.f}, tau_c = 0.f;
+  for (long long tile = static_cast<long long>(blockIdx.x) * kDivTilesPerCta + (wg >> 1); tile < n_tiles;
+       tile += static_cast<long long>(gridDim.x) * kDivTilesPerCta) {
+    const long long pt = tile * kTileM + h * kWgRows + tw;
+    const bool valid = row_thread && pt < p.P;
+    uint8_t* tn = p.tan + tile * kTanTileBytes;
+    const uint8_t* mk = p.relu_mask + tile * kMaskTileBytes;
+    // every finished fp16 image goes to the tangent stash by bulk TMA stores of one thread (see field_fwd.cu)
+    auto stash_begin = [&]() {
+      if (wg_leader) tma_bulk_wait_read<0>();
+      wg_bar(bar);
+    };
+    auto ready = [&](uint32_t off, uint32_t chunks) {
+      fence_proxy_async_smem();
+      wg_bar(bar);
+      if (wg_leader) store_rows(tn + off, s.img_hi, h, chunks);
+    };
+
+    float e[3] = {0.f, 0.f, 0.f}, off[3] = {0.f, 0.f, 0.f};
+    float r = 0.f, w = 0.f;
+    if (valid) {
 #pragma unroll
-  for (int k = 0; k < 64; ++k) {
-    tau_off[0] += sw[kW4 + k] * t[k]; tau_off[1] += sw[kW4 + 64 + k] * t[k]; tau_off[2] += sw[kW4 + 128 + k] * t[k];
-  }
+      for (int d = 0; d < 3; ++d) { e[d] = __ldg(p.e + pt * 3 + d); off[d] = __ldg(p.unmasked + pt * 3 + d); }
+      r = __ldg(p.rigidity + pt);
+      w = __ldg(p.w + pt);
+      if (p.w_is_alpha) w = 1.0f - expf(-fmaxf(w, 0.f));
+    }
+    // ---- tangent input row: [e_hi(3) e_lo(3) 0(42)], the bender-input layout (B0 applies W0[:, :3] to hi and lo) ----
+    stash_begin();
+    if (row_thread) {
+      float hi[3], lo[3];
 #pragma unroll
-  for (int k = 0; k < 32; ++k) tau_c += sw[kR2 + k] * s[k];
-  const float alpha = e[0] * tau_off[0] + e[1] * tau_off[1] + e[2] * tau_off[2];
-  const float beta = e[0] * off[0] + e[1] * off[1] + e[2] * off[2];
-  const float tau_r = 2.0f * r * (1.0f - r) * tau_c;
-  const float d = r * alpha + beta * tau_r;
-  if (valid) {
-    p.d[pt] = d; p.adot[pt] = alpha; p.beta[pt] = beta; p.tauc[pt] = tau_c;
-    atomicAdd(p.loss + pt / p.S, w * d * d / static_cast<float>(p.S));   // mean over the ray's samples of w |d|^2
+      for (int d = 0; d < 3; ++d) { hi[d] = __half2float(__float2half_rn(e[d])); lo[d] = e[d] - hi[d]; }
+      uint8_t* a_row = s.img_hi + row_off;
+      *reinterpret_cast<uint4*>(a_row) = make_uint4(pack_h2(hi[0], hi[1]), pack_h2(hi[2], lo[0]), pack_h2(lo[1], lo[2]), 0u);
+#pragma unroll
+      for (int c = 1; c < 6; ++c) *reinterpret_cast<uint4*>(a_row + c * kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
+    }
+    ready(kTE, 6);
+    // ---- B0, B1: [t1 | s1] = D1/E1 (B0 [e]), [t2 | s2] = D2/E2 (B1 [t1 | s1]) ----
+    {
+      float acc[48];
+      ReluMask<96> m;
+      m.load(mk + kMkHb1, h);
+      W.wait(&s.sh->w_full, 0, 330);
+      wg_mma_split<96, false>(acc, a_hi, a_lo, s, w_b0, 3);
+      stash_begin();
+      epi_mask_split<96>(acc, m, s, h);
+      ready(kT1, 12);
+      m.load(mk + kMkHb2, h);
+      wg_mma_split<96, true>(acc, a_hi, a_lo, s, w_b1, 6);
+      stash_begin();
+      epi_mask_split<96>(acc, m, s, h);
+      ready(kT2, 12);
+    }
+    // ---- B2: t3 = D3 (W2 t2); column 64 = tau_c = R2 s2 ----
+    {
+      float acc[40];
+      ReluMask<64> m;
+      m.load(mk + kMkHb3, h);
+      wg_mma_split<80, true>(acc, a_hi, a_lo, s, w_b2, 6);
+      stash_begin();
+      epi_mask_split<64>(acc, m, s, h);
+      if (acc_q() == 0) {
+        s.stage[acc_r0() * kDivStageLd + 8] = acc[32];
+        s.stage[(acc_r0() + 8) * kDivStageLd + 8] = acc[34];
+      }
+      ready(kT3, 8);
+    }
+    // ---- B3: t4 = D4 (W3 t3) ----
+    {
+      float acc[32];
+      ReluMask<64> m;
+      m.load(mk + kMkHb4, h);
+      wg_mma_split<64, true>(acc, a_hi, a_lo, s, w_b3, 4);
+      stash_begin();
+      epi_mask_split<64>(acc, m, s, h);
+      ready(kT4, 8);
+    }
+    // ---- B4: tau_off = W4 t4; per-point scalars and the per-ray loss ----
+    {
+      float acc[8];
+      wg_mma_split<16, true>(acc, a_hi, a_lo, s, w_b4, 4);
+      stage_cols<0, 1>(acc, s.stage, kDivStageLd);
+      wg_bar(bar);
+      if (row_thread) {   // warps 0 and 1 of the warpgroup: 32 consecutive rows each
+        const float tau_c = my_stg[8];
+        const float alpha = e[0] * my_stg[0] + e[1] * my_stg[1] + e[2] * my_stg[2];
+        const float beta = e[0] * off[0] + e[1] * off[1] + e[2] * off[2];
+        const float tau_r = 2.0f * r * (1.0f - r) * tau_c;
+        const float d = r * alpha + beta * tau_r;
+        float part = 0.f;   // this point's share of mean over the ray's samples of w |d|^2
+        if (valid) {
+          p.d[pt] = d; p.adot[pt] = alpha; p.beta[pt] = beta; p.tauc[pt] = tau_c;
+          part = w * d * d / static_cast<float>(p.S);
+        }
+        const long long ray = valid ? pt / p.S : -1;
+        const long long ray0 = __shfl_sync(0xffffffffu, ray, 0);
+        if (__all_sync(0xffffffffu, valid && ray == ray0)) {
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+          if (lane == 0) atomicAdd(p.loss + ray0, part);
+        } else if (valid) {
+          atomicAdd(p.loss + ray, part);
+        }
+      }
+    }
+    // the staging rows are rewritten only after the next tile's warpgroup barriers
   }
+  if (wg_leader) tma_bulk_wait<0>();   // all tangent-stash stores complete before the CTA exits
 }
 
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kDivThreads) div_bwd_kernel(const DivParams p) {
-  extern __shared__ __align__(16) float sm[];
-  float* sw = sm;
-  float* act = sm + kWTotal + threadIdx.x;
-  load_weights(sw, p);
-  __syncthreads();
-  const long long tile = blockIdx.x;
-  const int row = threadIdx.x;
-  const long long pt = tile * kTileM + row;
-  const bool valid = pt < p.P;
-  const uint8_t* st = p.stash + tile * kStashTileBytes + row * 16;
-  uint8_t* ad = p.adj + tile * kAdjTileBytes + row * 16;
+__global__ void __launch_bounds__(kDivThreads, 1) div_bwd_kernel(const DivParams p) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  const int wg = threadIdx.x >> 7;
+  const int h = wg & 1;
+  const DivSmem s = div_smem(smem, kDivBwdWBytes, wg);
+  load_resident_weights(s, p.bender + kBendTOffset, p.bender + kBendTLoOffset, kDivBwdWBytes);
+  const Waiter W{&s.sh->abort_flag, p.err};
 
+  const int tw = threadIdx.x & 127;
+  const bool row_thread = tw < kWgRows;
+  const int bar = 1 + wg;
+  const bool wg_leader = tw == 0;
+  const int row_off = (h * kWgRows + tw) * 16;
+  const uint32_t a_hi = smem_u32(s.img_hi) + h * kWgRows * 16, a_lo = smem_u32(s.img_lo) + h * kWgRows * 16;
+  constexpr uint32_t w_t4 = 0, w_t3 = w_t4 + kBendTB4Bytes, w_t2 = w_t3 + kBendTB3Bytes, w_t1 = w_t2 + kBendTB2Bytes;
+  const long long n_tiles = (p.P + kTileM - 1) / kTileM;
+
+  // power-of-two loss scale from max|G| (written by div_G_kernel / absmax), as in DGRAD
   float scale = 1.0f;
   {
     const float amax = p.amax ? __ldg(p.amax) : 0.f;
@@ -224,57 +324,91 @@ __global__ void __launch_bounds__(kDivThreads) div_bwd_kernel(const DivParams p)
       scale = ldexpf(1.0f, min(max(10 - ex, -60), 60));
     }
   }
-  float e[3] = {0.f, 0.f, 0.f};
-  float r = 0.f, G = 0.f, alpha = 0.f, beta = 0.f, tau_c = 0.f;
-  if (valid) {
+
+  for (long long tile = static_cast<long long>(blockIdx.x) * kDivTilesPerCta + (wg >> 1); tile < n_tiles;
+       tile += static_cast<long long>(gridDim.x) * kDivTilesPerCta) {
+    const long long pt = tile * kTileM + h * kWgRows + tw;
+    const bool valid = row_thread && pt < p.P;
+    uint8_t* ad = p.adj + tile * kAdjTileBytes;
+    const uint8_t* mk = p.relu_mask + tile * kMaskTileBytes;
+    auto stash_begin = [&]() {
+      if (wg_leader) tma_bulk_wait_read<0>();
+      wg_bar(bar);
+    };
+    auto ready = [&](uint32_t off, uint32_t chunks) {
+      fence_proxy_async_smem();
+      wg_bar(bar);
+      if (wg_leader) store_rows(ad + off, s.img_hi, h, chunks);
+    };
+
+    float e[3] = {0.f, 0.f, 0.f};
+    float r = 0.f, G = 0.f, beta = 0.f;
+    if (valid) {
 #pragma unroll
-    for (int d = 0; d < 3; ++d) e[d] = p.e[pt * 3 + d];
-    r = p.rigidity[pt]; G = p.G[pt]; alpha = p.adot[pt]; beta = p.beta[pt]; tau_c = p.tauc[pt];
+      for (int d = 0; d < 3; ++d) e[d] = __ldg(p.e + pt * 3 + d);
+      r = __ldg(p.rigidity + pt); G = __ldg(p.G + pt); beta = __ldg(p.beta + pt);
+      const float alpha = __ldg(p.adot + pt), tau_c = __ldg(p.tauc + pt);
+      const float tau_r = 2.0f * r * (1.0f - r) * tau_c;
+#pragma unroll
+      for (int d = 0; d < 3; ++d) p.d_unmasked[pt * 3 + d] = G * tau_r * e[d];
+      p.d_rigid[pt] = G * (alpha + 2.0f * beta * tau_c * (1.0f - 2.0f * r));
+    }
+    const float Gs = G * scale;
     const float rp = 2.0f * r * (1.0f - r);
-    const float tau_r = rp * tau_c;
-#pragma unroll
-    for (int d = 0; d < 3; ++d) p.d_unmasked[pt * 3 + d] = G * tau_r * e[d];
-    p.d_rigid[pt] = G * (alpha + 2.0f * beta * tau_c * (1.0f - 2.0f * r));
+    const float tb_c = Gs * beta * rp;   // adjoint of tau_c
+    // ---- [taubar_off (3) | 0], taubar_off = G r e ----
+    stash_begin();
+    if (row_thread) {
+      const uint2 t01 = split_h2(Gs * r * e[0], Gs * r * e[1]), t2 = split_h2(Gs * r * e[2], 0.f);
+      *reinterpret_cast<uint4*>(s.img_hi + row_off) = make_uint4(t01.x, t2.x, 0u, 0u);
+      *reinterpret_cast<uint4*>(s.img_lo + row_off) = make_uint4(t01.y, t2.y, 0u, 0u);
+      *reinterpret_cast<uint4*>(s.img_hi + row_off + kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
+      *reinterpret_cast<uint4*>(s.img_lo + row_off + kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
+    }
+    ready(kA4, 2);
+    // ---- B4^T -> abar4 = D4 (W4^T taubar_off); B3^T -> [abar3 = D3 (W3^T abar4) | taubar_c | 0] ----
+    {
+      float acc[32];
+      ReluMask<64> m;
+      m.load(mk + kMkHb4, h);
+      W.wait(&s.sh->w_full, 0, 340);
+      wg_mma_split<64, true>(acc, a_hi, a_lo, s, w_t4, 1);
+      stash_begin();
+      epi_mask_split<64>(acc, m, s, h);
+      ready(kA3, 8);
+      m.load(mk + kMkHb3, h);
+      wg_mma_split<64, true>(acc, a_hi, a_lo, s, w_t3, 4);
+      stash_begin();
+      epi_mask_split<64>(acc, m, s, h);
+      if (row_thread) {
+        const uint2 t = split_h2(tb_c, 0.f);
+        *reinterpret_cast<uint4*>(s.img_hi + row_off + 8 * kChunkBytes) = make_uint4(t.x, 0u, 0u, 0u);
+        *reinterpret_cast<uint4*>(s.img_lo + row_off + 8 * kChunkBytes) = make_uint4(t.y, 0u, 0u, 0u);
+        *reinterpret_cast<uint4*>(s.img_hi + row_off + 9 * kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
+        *reinterpret_cast<uint4*>(s.img_lo + row_off + 9 * kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
+      }
+      ready(kA2, 10);
+    }
+    // ---- B2^T -> [abar2 | qbar2] = D2/E2 [W2^T abar3 | R2^T taubar_c];  B1^T -> [abar1 | qbar1] ----
+    {
+      float acc[48];
+      ReluMask<96> m;
+      m.load(mk + kMkHb2, h);
+      wg_mma_split<96, true>(acc, a_hi, a_lo, s, w_t2, 5);
+      stash_begin();
+      epi_mask_split<96>(acc, m, s, h);
+      ready(kA1, 12);
+      m.load(mk + kMkHb1, h);
+      wg_mma_split<96, true>(acc, a_hi, a_lo, s, w_t1, 6);
+      stash_begin();
+      epi_mask_split<96>(acc, m, s, h);
+      ready(kA0, 12);
+    }
   }
-  const float Gs = G * scale;
-  const float rp = 2.0f * r * (1.0f - r);
-  float tb_off[4] = {Gs * r * e[0], Gs * r * e[1], Gs * r * e[2], 0.f};   // adjoint of tau_off
-  const float tb_c = Gs * beta * rp;                                      // adjoint of tau_c
-  const uint4 zz = make_uint4(0u, 0u, 0u, 0u);
-  *reinterpret_cast<uint4*>(ad + kA4) = make_uint4(pk(tb_off[0], tb_off[1]), pk(tb_off[2], 0.f), 0u, 0u);
-  *reinterpret_cast<uint4*>(ad + kA4 + kChunkBytes) = zz;
-
-  const unsigned long long m1 = read_mask(st + kStHb1, 8), e1 = read_mask(st + kStHb1 + 8 * kChunkBytes, 4);
-  const unsigned long long m2 = read_mask(st + kStHb2, 8), e2 = read_mask(st + kStHb2 + 8 * kChunkBytes, 4);
-  const unsigned long long m3 = read_mask(st + kStHb3, 8), m4 = read_mask(st + kStHb4, 8);
-
-  float a[64], q[32];
-  // tbar4 = W4^T taubar_off ; abar4 = D4 tbar4
-#pragma unroll 1
-  for (int k = 0; k < 64; ++k)
-    act[k * kDivThreads] = sw[kW4 + k] * tb_off[0] + sw[kW4 + 64 + k] * tb_off[1] + sw[kW4 + 128 + k] * tb_off[2];
-  take<64>(act, m4, 1.0f, a, ad + kA3);
-  // abar3 = D3 (W3^T abar4); rigidity output adjoint rides in column 64 of the same image
-  matvec_t<64>(sw + kW3, a, act, 64);
-  take<64>(act, m3, 1.0f, a, ad + kA2);
-  *reinterpret_cast<uint4*>(ad + kA2 + 8 * kChunkBytes) = make_uint4(pk(tb_c, 0.f), 0u, 0u, 0u);
-  *reinterpret_cast<uint4*>(ad + kA2 + 9 * kChunkBytes) = zz;
-  // abar2 = D2 (W2^T abar3), qbar2 = E2 (R2^T taubar_c)
-  matvec_t<64>(sw + kW2, a, act, 64);
-  take<64>(act, m2, 1.0f, a, ad + kA1);
-#pragma unroll 1
-  for (int k = 0; k < 32; ++k) act[k * kDivThreads] = sw[kR2 + k] * tb_c;
-  take<32>(act, e2, 1.0f, q, ad + kA1 + 8 * kChunkBytes);
-  // abar1 = D1 (W1^T abar2), qbar1 = E1 (R1^T qbar2)
-  matvec_t<64>(sw + kW1, a, act, 64);
-  take<64>(act, m1, 1.0f, a, ad + kA0);
-  matvec_t<32>(sw + kR1, q, act, 32);
-  take<32>(act, e1, 1.0f, q, ad + kA0 + 8 * kChunkBytes);
+  if (wg_leader) tma_bulk_wait<0>();   // all adjoint-stash stores complete before the CTA exits
 }
 
 // ------------------------------------------------------------------------------------------------
-static size_t div_smem() { return sizeof(float) * (kWTotal + kActFloats); }
-
 namespace {
 __global__ void div_G_kernel(const DivParams p, const float* __restrict__ g_ray, float* __restrict__ G, float* __restrict__ amax) {
   const long long pt = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
@@ -291,6 +425,18 @@ __global__ void div_G_kernel(const DivParams p, const float* __restrict__ g_ray,
   for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
   if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(reinterpret_cast<int*>(amax), __float_as_int(m));   // non-negative floats order like ints
 }
+
+template <typename Kernel>
+cudaError_t launch_div(Kernel kernel, int wbytes, const DivParams& p, int num_sms, cudaStream_t st) {
+  const long long tiles = (p.P + kTileM - 1) / kTileM;
+  if (tiles <= 0) return cudaSuccess;
+  const int smem = static_cast<int>(div_smem_bytes(wbytes));
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e != cudaSuccess) return e;
+  const long long pairs = (tiles + kDivTilesPerCta - 1) / kDivTilesPerCta;
+  kernel<<<static_cast<unsigned>(pairs < num_sms ? pairs : num_sms), kDivThreads, smem, st>>>(p);
+  return cudaGetLastError();
+}
 }  // namespace
 
 cudaError_t launch_div_G(const DivParams& p, const float* g_ray, float* G, float* amax, cudaStream_t st) {
@@ -300,21 +446,11 @@ cudaError_t launch_div_G(const DivParams& p, const float* g_ray, float* G, float
   return cudaGetLastError();
 }
 
-cudaError_t launch_div_fwd(const DivParams& p, cudaStream_t st) {
-  const long long tiles = (p.P + kTileM - 1) / kTileM;
-  if (tiles <= 0) return cudaSuccess;
-  cudaError_t e = cudaFuncSetAttribute(div_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)div_smem());
-  if (e != cudaSuccess) return e;
-  div_fwd_kernel<<<static_cast<unsigned>(tiles), kDivThreads, div_smem(), st>>>(p);
-  return cudaGetLastError();
+cudaError_t launch_div_fwd(const DivParams& p, int num_sms, cudaStream_t st) {
+  return launch_div(div_fwd_kernel, kDivFwdWBytes, p, num_sms, st);
 }
-cudaError_t launch_div_bwd(const DivParams& p, cudaStream_t st) {
-  const long long tiles = (p.P + kTileM - 1) / kTileM;
-  if (tiles <= 0) return cudaSuccess;
-  cudaError_t e = cudaFuncSetAttribute(div_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)div_smem());
-  if (e != cudaSuccess) return e;
-  div_bwd_kernel<<<static_cast<unsigned>(tiles), kDivThreads, div_smem(), st>>>(p);
-  return cudaGetLastError();
+cudaError_t launch_div_bwd(const DivParams& p, int num_sms, cudaStream_t st) {
+  return launch_div(div_bwd_kernel, kDivBwdWBytes, p, num_sms, st);
 }
 
 }  // namespace nrn

@@ -76,7 +76,7 @@ constexpr int kGsYb2 = kGsYb3 + 8 * kChunkBytes;           // 10 chunks (64 + ri
 constexpr int kGsYb1 = kGsYb2 + 10 * kChunkBytes;          // 12 chunks
 constexpr int kGsYb0 = kGsYb1 + 12 * kChunkBytes;          // 12 chunks
 constexpr int kGradTileBytes = kGsYb0 + 12 * kChunkBytes;  // 618,496
-// ReLU masks (forward -> DGRAD), per tile: one bit per element of H1..H8 and Hb1..Hb4 (the 64 ReLU columns of Hb3),
+// ReLU masks (forward -> DGRAD and the divergence kernels), per tile: one bit per element of H1..H8 and Hb1..Hb4 (the 64 ReLU columns of Hb3),
 // in the wgmma accumulator's own order (field_mma.cuh: relu_mask_*).  256-column images take 32 B per row, bender
 // images (<= 128 columns) 16 B per row.
 constexpr int kMaskHBytes = kTileM * 32;                   // 4 KB
@@ -107,7 +107,13 @@ constexpr int kBendTB1Bytes = 12 * 96 * 16;
 constexpr int kBendTB0Bytes = 12 * 48 * 16;
 constexpr int kBendTWBytes = kBendTB4Bytes + kBendTB3Bytes + kBendTB2Bytes + kBendTB1Bytes + kBendTB0Bytes;
 constexpr int kNerfPackedBytes = kNerfTOffset + kNerfTWBytes;
-constexpr int kBendPackedBytes = kBendTOffset + kBendTWBytes;
+// Bender residual images for the divergence kernels (div.cu), after the transposed images: for every weight w of the
+// forward and transposed images above, fp16((w - fp16(w)) * kBendLoScale), so that fp16(w) + lo / kBendLoScale carries
+// w to about 22 bits and the tangent / adjoint chains can run at fp32 accuracy on fp16 tensor cores.
+constexpr float kBendLoScale = 2048.f;
+constexpr int kBendLoOffset = kBendTOffset + kBendTWBytes;   // residuals of B0..B4
+constexpr int kBendTLoOffset = kBendLoOffset + kBendWBytes;  // residuals of B4^T..B0^T
+constexpr int kBendPackedBytes = kBendTLoOffset + kBendTWBytes;
 
 struct FieldBwdParams {
   long long P;

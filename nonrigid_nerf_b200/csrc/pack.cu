@@ -56,7 +56,11 @@ __device__ __forceinline__ void pack_nerf_elem(const int idx, const NerfSrc& src
   (void)nh;
 }
 
-__device__ __forceinline__ void pack_bender_elem(const int idx, const BenderSrc& src, __half* __restrict__ w, float* __restrict__ bias) {
+// fp16 residual of a weight, scaled into fp16's normal range (nrn_common.cuh: kBendLoScale)
+__device__ __forceinline__ __half lo_half(float v) { return __float2half_rn((v - __half2float(__float2half_rn(v))) * kBendLoScale); }
+
+__device__ __forceinline__ void pack_bender_elem(const int idx, const BenderSrc& src, __half* __restrict__ w, float* __restrict__ bias,
+                                                 __half* __restrict__ wlo) {
   constexpr int n0 = kBendB0Bytes / 2, n1 = kBendB1Bytes / 2, n2 = kBendB2Bytes / 2, n3 = kBendB3Bytes / 2;
   constexpr int ld0 = 3 + kLatent;
   if (idx < kBendWBytes / 2) {
@@ -89,6 +93,7 @@ __device__ __forceinline__ void pack_bender_elem(const int idx, const BenderSrc&
       if (r < 3) v = src.net_w[4][r * 64 + k];
     }
     w[idx] = __float2half_rn(v);
+    wlo[idx] = lo_half(v);
   }
   if (idx < kBendBiasFloats) {
     float b = 0.f;
@@ -133,7 +138,7 @@ __device__ __forceinline__ void pack_nerf_t_elem(const int idx, const NerfSrc& s
   w[idx] = __float2half_rn(v);
 }
 
-__device__ __forceinline__ void pack_bender_t_elem(const int idx, const BenderSrc& src, __half* __restrict__ w) {
+__device__ __forceinline__ void pack_bender_t_elem(const int idx, const BenderSrc& src, __half* __restrict__ w, __half* __restrict__ wlo) {
   if (idx >= kBendTWBytes / 2) return;
   constexpr int n4 = kBendTB4Bytes / 2, n3 = kBendTB3Bytes / 2, n2 = kBendTB2Bytes / 2, n1 = kBendTB1Bytes / 2;
   constexpr int ld0 = 3 + kLatent;
@@ -160,6 +165,7 @@ __device__ __forceinline__ void pack_bender_t_elem(const int idx, const BenderSr
     else if (r < 3) v = k < 64 ? src.net_w[0][k * ld0 + r] : src.rig_w[0][(k - 64) * 3 + r];
   }
   w[idx] = __float2half_rn(v);
+  wlo[idx] = lo_half(v);
 }
 
 
@@ -172,15 +178,16 @@ __global__ void __launch_bounds__(kPackThreads) pack_nerf_kernel(NerfSrc src, in
   else pack_nerf_t_elem((blockIdx.x - nb_fwd) * kPackThreads + threadIdx.x, src, in_ch, out_ch, wt);
 }
 __global__ void __launch_bounds__(kPackThreads) pack_bender_kernel(BenderSrc src, __half* __restrict__ w, float* __restrict__ bias,
-                                                                   __half* __restrict__ wt) {
+                                                                   __half* __restrict__ wt, __half* __restrict__ wlo,
+                                                                   __half* __restrict__ wtlo) {
   constexpr int nb_fwd = (kBendWBytes / 2 + kPackThreads - 1) / kPackThreads;
-  if (blockIdx.x < nb_fwd) pack_bender_elem(blockIdx.x * kPackThreads + threadIdx.x, src, w, bias);
-  else pack_bender_t_elem((blockIdx.x - nb_fwd) * kPackThreads + threadIdx.x, src, wt);
+  if (blockIdx.x < nb_fwd) pack_bender_elem(blockIdx.x * kPackThreads + threadIdx.x, src, w, bias, wlo);
+  else pack_bender_t_elem((blockIdx.x - nb_fwd) * kPackThreads + threadIdx.x, src, wt, wtlo);
 }
 
 }  // namespace
 
-// packed = [forward images | biases | transposed images] (offsets in nrn_common.cuh)
+// packed = [forward images | biases | transposed images] (+ the bender's residual images; offsets in nrn_common.cuh)
 cudaError_t launch_pack_nerf(const NerfSrc& src, int in_ch, int out_ch, void* packed, cudaStream_t st) {
   uint8_t* base = reinterpret_cast<uint8_t*>(packed);
   const int nb = (kNerfWBytes / 2 + kPackThreads - 1) / kPackThreads + (kNerfTWBytes / 2 + kPackThreads - 1) / kPackThreads;
@@ -192,7 +199,8 @@ cudaError_t launch_pack_bender(const BenderSrc& src, void* packed, cudaStream_t 
   uint8_t* base = reinterpret_cast<uint8_t*>(packed);
   const int nb = (kBendWBytes / 2 + kPackThreads - 1) / kPackThreads + (kBendTWBytes / 2 + kPackThreads - 1) / kPackThreads;
   pack_bender_kernel<<<nb, kPackThreads, 0, st>>>(src, reinterpret_cast<__half*>(base), reinterpret_cast<float*>(base + kBendWBytes),
-                                                 reinterpret_cast<__half*>(base + kBendTOffset));
+                                                 reinterpret_cast<__half*>(base + kBendTOffset), reinterpret_cast<__half*>(base + kBendLoOffset),
+                                                 reinterpret_cast<__half*>(base + kBendTLoOffset));
   return cudaGetLastError();
 }
 
