@@ -341,7 +341,8 @@ int nrn_field_backward(const NrnFieldBwdArgs* a) {
   p.cutoff = a->rigidity_cutoff; p.use_cutoff = a->use_cutoff; p.scaling = a->scaling; p.use_scaling = a->use_scaling;
   p.d_latents = a->d_latents; p.err = ds->err_word;
   p.relu_mask = static_cast<const uint8_t*>(a->relu_mask);
-  e = nrn::launch_absmax(a->d_raw, p.P * a->out_ch, amax, st);
+  // DGRAD reads channels 0-3 of d_raw; channel 4 never reaches the loss and must not set the scale
+  e = nrn::launch_absmax(a->d_raw, p.P * a->out_ch, amax, st, false, a->out_ch, 4);
   // the regularisers' upstream gradients share the fp16 loss scale: they take part in the maximum, otherwise a large
   // offsets_loss_weight saturates them (or, with a vanishing data term, lets them underflow)
   if (e == cudaSuccess && bend && p.d_unmasked_up) e = nrn::launch_absmax(p.d_unmasked_up, p.P * 3, amax, st, true);

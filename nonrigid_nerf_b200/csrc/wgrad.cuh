@@ -33,7 +33,9 @@ struct WgradDst {
   int acc_nerf, acc_bend;
 };
 cudaError_t launch_wgrad(WgradParams p, bool has_bender, int num_sms, const WgradDst& dst, int out_ch, cudaStream_t st);
-// amax[0] = max |x[i]| over n floats (device scalar, overwritten)
-cudaError_t launch_absmax(const float* x, long long n, float* amax, cudaStream_t st, bool accumulate = false);
+// amax[0] = max |x[i]| over n floats (device scalar, overwritten; accumulate: max with its value).  x as rows of
+// `row_len` floats: only the first `cols` of every row take part.
+cudaError_t launch_absmax(const float* x, long long n, float* amax, cudaStream_t st, bool accumulate = false, int row_len = 1,
+                          int cols = 1);
 
 }  // namespace nrn

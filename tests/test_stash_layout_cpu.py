@@ -1,0 +1,101 @@
+"""The stash, mask and gradient layouts that tests/stash_layout.py mirrors, pinned to the library's own sizes, and a round
+trip of the documented ReLU mask bit layout.  No kernel is launched here."""
+import math
+
+import pytest
+import torch
+
+from tests import stash_layout as SL
+
+
+def _contiguous(images, tile_bytes, unit):
+    o = 0
+    for off, n in images:
+        assert off == o, (off, o)
+        o += n * unit
+    assert o == tile_bytes
+
+
+def test_image_offsets_tile_the_library_buffers():
+    from nonrigid_nerf_b200 import _lib
+    lib = _lib.load()
+    _contiguous(SL.STASH_IMAGES, SL.STASH_TILE, SL.CHUNK)
+    _contiguous(SL.GRAD_IMAGES, SL.GRAD_TILE, SL.CHUNK)
+    o = 0
+    for off, ncols in SL.MASK_IMAGES:
+        assert off == o
+        o += SL.TILE_M * (32 if ncols > 128 else 16)
+    assert o == SL.MASK_TILE
+    _contiguous([SL.T_E, SL.T_1, SL.T_2, SL.T_3, SL.T_4], SL.TAN_TILE, SL.CHUNK)
+    _contiguous([SL.A_4, SL.A_3, SL.A_2, SL.A_1, SL.A_0], SL.ADJ_TILE, SL.CHUNK)
+    # the compact divergence stashes are the bender sections of the field stashes, in the same order
+    assert SL.TAN_TILE == SL.STASH_TILE - SL.ST_BIN[0] and SL.ADJ_TILE == SL.GRAD_TILE - SL.GS_YB4[0]
+    # the field stashes and masks hold an even number of tiles, the divergence stashes exactly the point tiles
+    for n, s in ((1, 7), (2, 64), (3, 100), (11, 100), (1023, 64), (1024, 128)):
+        tiles = -(-n * s // SL.TILE_M)
+        even = tiles + (tiles & 1)
+        assert lib.nrn_stash_bytes(n, s) == even * SL.STASH_TILE
+        assert lib.nrn_grad_stash_bytes(n, s) == even * SL.GRAD_TILE
+        assert lib.nrn_relu_mask_bytes(n, s) == even * SL.MASK_TILE
+        assert lib.nrn_div_stash_bytes(n, s) == tiles * SL.TAN_TILE
+        assert lib.nrn_div_grad_stash_bytes(n, s) == tiles * SL.ADJ_TILE
+
+
+@pytest.mark.parametrize("out_ch", [4, 5])
+def test_gradient_parameter_maps_match_the_library(out_ch):
+    from nonrigid_nerf_b200 import _lib
+    lib = _lib.load()
+    assert sum(math.prod(s) for _, s in SL.nerf_param_shapes(out_ch)) == lib.nrn_nerf_grad_floats(out_ch)
+    assert sum(math.prod(s) for _, s in SL.bender_param_shapes()) == lib.nrn_bender_grad_floats()
+
+
+def _encode_reference(bits):
+    """The documented layout written out element by element (independent of stash_layout's vectorised code)."""
+    rows, ncols = bits.shape
+    kh = 2 if ncols > 128 else 1
+    words = [[0] * (4 * kh) for _ in range(rows)]
+    for r in range(rows):
+        for c in range(ncols):
+            if bits[r, c]:
+                j, q = c // 8, (c % 8) // 2
+                h, k = j // 16, j % 16
+                words[r][q * kh + h] |= 1 << (k + 16 * (c % 2))
+    out = bytearray()
+    for r in range(rows):
+        for w in words[r]:
+            out += w.to_bytes(4, "little")
+    return torch.frombuffer(out, dtype=torch.uint8).reshape(rows // SL.TILE_M, -1)
+
+
+@pytest.mark.parametrize("ncols", [256, 96, 64])
+def test_relu_mask_round_trip(ncols):
+    g = torch.Generator().manual_seed(ncols)
+    bits = torch.rand(2 * SL.TILE_M, ncols, generator=g) > 0.5
+    ref = _encode_reference(bits)
+    enc = SL.encode_relu_bits(bits)
+    assert torch.equal(enc, ref)
+    kh = 2 if ncols > 128 else 1
+    assert enc.shape == (2, SL.TILE_M * 16 * kh)
+    # decode from a mask buffer: the image sits at its offset inside each tile
+    off = 8 * SL.MASK_H_BYTES if ncols < 128 else 3 * SL.MASK_H_BYTES
+    buf = torch.zeros(2 * SL.MASK_TILE, dtype=torch.uint8)
+    buf.view(2, SL.MASK_TILE)[:, off:off + enc.shape[1]] = enc
+    assert torch.equal(SL.relu_bits(buf, off, ncols, 2), bits)
+    # a single bit lands at the documented byte and bit: column 8 (16 h + k) + 2 q + 1 of row r
+    one = torch.zeros(SL.TILE_M, ncols, dtype=torch.bool)
+    r, c = 37, ncols - 5
+    one[r, c] = True
+    j, q = c // 8, (c % 8) // 2
+    word = int.from_bytes(bytes(SL.encode_relu_bits(one)[0, r * 16 * kh + q * 4 * kh + 4 * (j // 16):][:4].tolist()), "little")
+    assert word == 1 << (j % 16 + 16 * (c % 2))
+
+
+def test_loss_scale_matches_the_kernels_rule():
+    assert SL.loss_scale(0.0) == 1.0 and SL.loss_scale(float("inf")) == 1.0 and SL.loss_scale(float("nan")) == 1.0
+    assert SL.loss_scale(3.1e38) == 1.0
+    for amax in (1.0, 0.75, 1023.9, 1024.0, 3e-15, 2.5e10, 1e-30, 1e30):
+        s = SL.loss_scale(amax)
+        assert s == 2.0 ** round(math.log2(s))
+        if 2.0 ** -60 <= s <= 2.0 ** 60 and 1e-17 < amax < 1e17:
+            assert 512.0 <= amax * s < 1024.0, (amax, s)
+    assert SL.loss_scale(1e-30) == 2.0 ** 60 and SL.loss_scale(1e30) == 2.0 ** -60
