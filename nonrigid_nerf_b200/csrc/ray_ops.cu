@@ -454,6 +454,10 @@ cudaError_t launch_sample_pdf(const float* bins, const float* weights, const flo
                               float* out, cudaStream_t st) {
   if (n == 0) return cudaSuccess;
   const size_t smem = sizeof(float) * kWarpsPerBlock * 3 * nb;
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(sample_pdf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+  }
   sample_pdf_kernel<<<(n + kWarpsPerBlock - 1) / kWarpsPerBlock, kWarpsPerBlock * 32, smem, st>>>(bins, weights, u, n, nb,
                                                                                                 n_samp, out);
   return cudaGetLastError();
@@ -461,6 +465,10 @@ cudaError_t launch_sample_pdf(const float* bins, const float* weights, const flo
 cudaError_t launch_composite_bwd(const CompositeBwdParams& p, cudaStream_t st) {
   if (p.n == 0) return cudaSuccess;
   const size_t smem = sizeof(float) * kWarpsPerBlock * p.S;
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(composite_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+  }
   composite_bwd_kernel<<<(p.n + kWarpsPerBlock - 1) / kWarpsPerBlock, kWarpsPerBlock * 32, smem, st>>>(p);
   return cudaGetLastError();
 }
