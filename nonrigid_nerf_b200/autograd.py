@@ -30,11 +30,13 @@ def _knobs(net):
 
 
 def _flat_params(net, bender):
-    """Parameters in the flat order of the WGRAD output buffers (csrc/wgrad.cu)."""
-    ws, bs = ops.nerf_param_list(net)
+    """Parameters in the flat order of the WGRAD output buffers (csrc/wgrad.cu); `net` may be None for the bender's
+    alone."""
     nerf = []
-    for w, b in zip(ws, bs):
-        nerf += [w, b]
+    if net is not None:
+        ws, bs = ops.nerf_param_list(net)
+        for w, b in zip(ws, bs):
+            nerf += [w, b]
     bend = []
     if bender is not None:
         net_w, net_b, rig_w, rig_b = ops.bender_param_list(bender)
@@ -188,7 +190,7 @@ def _arena_destination(params):
 
 
 def _bender_arena(bender):
-    _, bend_p = _flat_params_bender(bender)
+    _, bend_p = _flat_params(None, bender)
     if not all(p.requires_grad for p in bend_p):
         return None
     return _arena_destination(bend_p)
@@ -355,21 +357,10 @@ def divergence_loss(unmasked: torch.Tensor, rigidity: torch.Tensor, weights: Opt
     n, s = unmasked.shape[0], unmasked.shape[1]
     if e is None:
         e = torch.randn(n * s, 3, device=unmasked.device)
-    _, bend_p = _flat_params_bender(bender)
+    _, bend_p = _flat_params(None, bender)
     if opacity_alpha is not None:
         return _DivergenceFn.apply(unmasked, rigidity, opacity_alpha, e, relu_mask, bender, True, *bend_p)
     return _DivergenceFn.apply(unmasked, rigidity, weights, e, relu_mask, bender, False, *bend_p)
-
-
-def _flat_params_bender(bender):
-    net_w, net_b, rig_w, rig_b = ops.bender_param_list(bender)
-    bend = []
-    for i in range(4):
-        bend += [net_w[i], net_b[i]]
-    bend.append(net_w[4])
-    for i in range(3):
-        bend += [rig_w[i], rig_b[i]]
-    return None, bend
 
 
 class _RayLossFn(torch.autograd.Function):

@@ -292,8 +292,8 @@ size_t nrn_stash_bytes(int n_rays, int n_samples) { return static_cast<size_t>(e
 size_t nrn_grad_stash_bytes(int n_rays, int n_samples) { return static_cast<size_t>(even_tiles(n_rays, n_samples)) * nrn::kGradTileBytes; }
 size_t nrn_relu_mask_bytes(int n_rays, int n_samples) { return static_cast<size_t>(even_tiles(n_rays, n_samples)) * nrn::kMaskTileBytes; }
 size_t nrn_wgrad_scratch_bytes(void) { return static_cast<size_t>(nrn::kWgMaxCtas) * nrn::kWgScratchFloats * sizeof(float); }
-int nrn_nerf_grad_floats(int out_ch) { return 256 * 63 + 256 + 6 * (65536 + 256) + 256 * 319 + 256 + out_ch * 257; }
-int nrn_bender_grad_floats(void) { return 16193; }
+int nrn_nerf_grad_floats(int out_ch) { return nrn::nerf_grad_floats(out_ch); }
+int nrn_bender_grad_floats(void) { return nrn::bparam::total(); }
 
 int nrn_field_backward(const NrnFieldBwdArgs* a) {
   if (!a) return fail(NRN_E_INVALID, "nrn_field_backward: null args");

@@ -44,17 +44,13 @@ constexpr int kDivTilesPerCta = 2;                       // tiles in flight per 
 constexpr int kDivWgs = 2 * kDivTilesPerCta;
 constexpr int kDivThreads = 128 * kDivWgs;
 constexpr int kDivStageLd = 12;                          // floats per staged row: B4 columns 0-7, tau_c at 8
-constexpr int kDivImgBytes = 12 * kChunkBytes;           // widest image of either chain: 96 columns
+constexpr int kDivImgBytes = kStHb1.chunks * kChunkBytes;  // widest image of either chain: 96 columns
 constexpr float kLoInv = 1.0f / kBendLoScale;
-
-// tile layouts of the tangent stash and the adjoint stash (bytes)
-constexpr int kTE = 0, kT1 = 6 * kChunkBytes, kT2 = 18 * kChunkBytes, kT3 = 30 * kChunkBytes, kT4 = 38 * kChunkBytes;
-constexpr int kA4 = 0, kA3 = 2 * kChunkBytes, kA2 = 10 * kChunkBytes, kA1 = 20 * kChunkBytes, kA0 = 32 * kChunkBytes;
 
 // resident weights (each with its residual image): B0..B4 (forward); B4^T..B1^T (backward: the probe e is not
 // differentiated)
 constexpr int kDivFwdWBytes = kBendWBytes;
-constexpr int kDivBwdWBytes = kBendTB4Bytes + kBendTB3Bytes + kBendTB2Bytes + kBendTB1Bytes;
+constexpr int kDivBwdWBytes = dgrad::w_off(dgrad::B0T);
 
 struct DivShared {
   uint64_t w_full;
@@ -105,15 +101,17 @@ __device__ __forceinline__ void load_resident_weights(const DivSmem& s, const ui
   }
 }
 
-// acc[64 x N] = (A_lo . W_hi + A_hi . W_lo) / kBendLoScale + A_hi . W_hi over k16 steps of 16 columns, all operands in
-// shared memory: A = this warpgroup's rows of chunk-major images of kTileM rows (fenced for the async proxy, warpgroup
-// synced), W = resident N-row weight images at byte `w_off`.  A_LO = false: the A residual is zero (the probe input, whose
-// hi / lo split lives in its columns).  The small terms are summed first, scaled exactly, then the main products added.
-template <int N, bool A_LO>
-__device__ __forceinline__ void wg_mma_split(float (&acc)[N / 2], uint32_t a_hi, uint32_t a_lo, const DivSmem& s, uint32_t w_off,
-                                             uint32_t k16) {
+// acc[64 x N] = (A_lo . W_hi + A_hi . W_lo) / kBendLoScale + A_hi . W_hi over the k16 steps of 16 columns of bender step S
+// (fwd:: or dgrad::), all operands in shared memory: A = this warpgroup's rows of chunk-major images of kTileM rows (fenced
+// for the async proxy, warpgroup synced), W = the step's resident N-row weight images.  A_LO = false: the A residual is
+// zero (the probe input, whose hi / lo split lives in its columns).  The small terms are summed first, scaled exactly,
+// then the main products added.
+template <auto S, bool A_LO>
+__device__ __forceinline__ void wg_mma_split(Acc<S>& acc, uint32_t a_hi, uint32_t a_lo, const DivSmem& s) {
+  constexpr int N = step(S).N;
+  constexpr uint32_t w0 = w_off(S), k16 = step(S).k16;
   const uint64_t ahi = gmma_desc(a_hi, kChunkBytes, 128), alo = gmma_desc(a_lo, kChunkBytes, 128);
-  const uint64_t whi = gmma_desc(smem_u32(s.w_hi) + w_off, N * 16, 128), wlo = gmma_desc(smem_u32(s.w_lo) + w_off, N * 16, 128);
+  const uint64_t whi = gmma_desc(smem_u32(s.w_hi) + w0, N * 16, 128), wlo = gmma_desc(smem_u32(s.w_lo) + w0, N * 16, 128);
 #pragma unroll
   for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
   acc_fence(acc);
@@ -180,8 +178,6 @@ __global__ void __launch_bounds__(kDivThreads, 1) div_fwd_kernel(const DivParams
   const bool wg_leader = tw == 0;
   const int row_off = (h * kWgRows + tw) * 16;
   const uint32_t a_hi = smem_u32(s.img_hi) + h * kWgRows * 16, a_lo = smem_u32(s.img_lo) + h * kWgRows * 16;
-  constexpr uint32_t w_b0 = 0, w_b1 = w_b0 + kBendB0Bytes, w_b2 = w_b1 + kBendB1Bytes, w_b3 = w_b2 + kBendB2Bytes,
-                     w_b4 = w_b3 + kBendB3Bytes;
   const float* my_stg = s.stage + tw * kDivStageLd;
   const long long n_tiles = (p.P + kTileM - 1) / kTileM;
 
@@ -191,16 +187,7 @@ __global__ void __launch_bounds__(kDivThreads, 1) div_fwd_kernel(const DivParams
     const bool valid = row_thread && pt < p.P;
     uint8_t* tn = p.tan + tile * kTanTileBytes;
     const uint8_t* mk = p.relu_mask + tile * kMaskTileBytes;
-    // every finished fp16 image goes to the tangent stash by bulk TMA stores of one thread (see field_fwd.cu)
-    auto stash_begin = [&]() {
-      if (wg_leader) tma_bulk_wait_read<0>();
-      wg_bar(bar);
-    };
-    auto ready = [&](uint32_t off, uint32_t chunks) {
-      fence_proxy_async_smem();
-      wg_bar(bar);
-      if (wg_leader) store_rows(tn + off, s.img_hi, h, chunks);
-    };
+    const StashWriter<false> sw{tn, wg_leader, bar, h};   // every finished fp16 image goes to the tangent stash
 
     float e[3] = {0.f, 0.f, 0.f}, off[3] = {0.f, 0.f, 0.f};
     float r = 0.f, w = 0.f;
@@ -212,7 +199,7 @@ __global__ void __launch_bounds__(kDivThreads, 1) div_fwd_kernel(const DivParams
       if (p.w_is_alpha) w = 1.0f - expf(-fmaxf(w, 0.f));
     }
     // ---- tangent input row: [e_hi(3) e_lo(3) 0(42)], the bender-input layout (B0 applies W0[:, :3] to hi and lo) ----
-    stash_begin();
+    sw.begin();
     if (row_thread) {
       float hi[3], lo[3];
 #pragma unroll
@@ -222,51 +209,51 @@ __global__ void __launch_bounds__(kDivThreads, 1) div_fwd_kernel(const DivParams
 #pragma unroll
       for (int c = 1; c < 6; ++c) *reinterpret_cast<uint4*>(a_row + c * kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
     }
-    ready(kTE, 6);
+    sw.ready(tan_image(kStBin), s.img_hi);
     // ---- B0, B1: [t1 | s1] = D1/E1 (B0 [e]), [t2 | s2] = D2/E2 (B1 [t1 | s1]) ----
     {
-      float acc[48];
-      ReluMask<96> m;
-      m.load(mk + kMkHb1, h);
+      Acc<fwd::B0> acc;
+      ReluMask<kMkHb1.cols> m;
+      m.load(mk + kMkHb1.off, h);
       W.wait(&s.sh->w_full, 0, 330);
-      wg_mma_split<96, false>(acc, a_hi, a_lo, s, w_b0, 3);
-      stash_begin();
-      epi_mask_split<96>(acc, m, s, h);
-      ready(kT1, 12);
-      m.load(mk + kMkHb2, h);
-      wg_mma_split<96, true>(acc, a_hi, a_lo, s, w_b1, 6);
-      stash_begin();
-      epi_mask_split<96>(acc, m, s, h);
-      ready(kT2, 12);
+      wg_mma_split<fwd::B0, false>(acc, a_hi, a_lo, s);
+      sw.begin();
+      epi_mask_split<kMkHb1.cols>(acc, m, s, h);
+      sw.ready(tan_image(kStHb1), s.img_hi);
+      m.load(mk + kMkHb2.off, h);
+      wg_mma_split<fwd::B1, true>(acc, a_hi, a_lo, s);
+      sw.begin();
+      epi_mask_split<kMkHb2.cols>(acc, m, s, h);
+      sw.ready(tan_image(kStHb2), s.img_hi);
     }
     // ---- B2: t3 = D3 (W2 t2); column 64 = tau_c = R2 s2 ----
     {
-      float acc[40];
-      ReluMask<64> m;
-      m.load(mk + kMkHb3, h);
-      wg_mma_split<80, true>(acc, a_hi, a_lo, s, w_b2, 6);
-      stash_begin();
-      epi_mask_split<64>(acc, m, s, h);
+      Acc<fwd::B2> acc;
+      ReluMask<kMkHb3.cols> m;
+      m.load(mk + kMkHb3.off, h);
+      wg_mma_split<fwd::B2, true>(acc, a_hi, a_lo, s);
+      sw.begin();
+      epi_mask_split<kMkHb3.cols>(acc, m, s, h);
       if (acc_q() == 0) {
         s.stage[acc_r0() * kDivStageLd + 8] = acc[32];
         s.stage[(acc_r0() + 8) * kDivStageLd + 8] = acc[34];
       }
-      ready(kT3, 8);
+      sw.ready(tan_image(kStHb3), s.img_hi);
     }
     // ---- B3: t4 = D4 (W3 t3) ----
     {
-      float acc[32];
-      ReluMask<64> m;
-      m.load(mk + kMkHb4, h);
-      wg_mma_split<64, true>(acc, a_hi, a_lo, s, w_b3, 4);
-      stash_begin();
-      epi_mask_split<64>(acc, m, s, h);
-      ready(kT4, 8);
+      Acc<fwd::B3> acc;
+      ReluMask<kMkHb4.cols> m;
+      m.load(mk + kMkHb4.off, h);
+      wg_mma_split<fwd::B3, true>(acc, a_hi, a_lo, s);
+      sw.begin();
+      epi_mask_split<kMkHb4.cols>(acc, m, s, h);
+      sw.ready(tan_image(kStHb4), s.img_hi);
     }
     // ---- B4: tau_off = W4 t4; per-point scalars and the per-ray loss ----
     {
-      float acc[8];
-      wg_mma_split<16, true>(acc, a_hi, a_lo, s, w_b4, 4);
+      Acc<fwd::B4> acc;
+      wg_mma_split<fwd::B4, true>(acc, a_hi, a_lo, s);
       stage_cols<0, 1>(acc, s.stage, kDivStageLd);
       wg_bar(bar);
       if (row_thread) {   // warps 0 and 1 of the warpgroup: 32 consecutive rows each
@@ -311,19 +298,9 @@ __global__ void __launch_bounds__(kDivThreads, 1) div_bwd_kernel(const DivParams
   const bool wg_leader = tw == 0;
   const int row_off = (h * kWgRows + tw) * 16;
   const uint32_t a_hi = smem_u32(s.img_hi) + h * kWgRows * 16, a_lo = smem_u32(s.img_lo) + h * kWgRows * 16;
-  constexpr uint32_t w_t4 = 0, w_t3 = w_t4 + kBendTB4Bytes, w_t2 = w_t3 + kBendTB3Bytes, w_t1 = w_t2 + kBendTB2Bytes;
   const long long n_tiles = (p.P + kTileM - 1) / kTileM;
 
-  // power-of-two loss scale from max|G| (written by div_G_kernel / absmax), as in DGRAD
-  float scale = 1.0f;
-  {
-    const float amax = p.amax ? __ldg(p.amax) : 0.f;
-    if (amax > 0.f && amax < 3.0e38f) {
-      int ex;
-      frexpf(amax, &ex);
-      scale = ldexpf(1.0f, min(max(10 - ex, -60), 60));
-    }
-  }
+  const float scale = loss_scale(p.amax);   // max|G| is written by div_G_kernel / absmax
 
   for (long long tile = static_cast<long long>(blockIdx.x) * kDivTilesPerCta + (wg >> 1); tile < n_tiles;
        tile += static_cast<long long>(gridDim.x) * kDivTilesPerCta) {
@@ -331,15 +308,7 @@ __global__ void __launch_bounds__(kDivThreads, 1) div_bwd_kernel(const DivParams
     const bool valid = row_thread && pt < p.P;
     uint8_t* ad = p.adj + tile * kAdjTileBytes;
     const uint8_t* mk = p.relu_mask + tile * kMaskTileBytes;
-    auto stash_begin = [&]() {
-      if (wg_leader) tma_bulk_wait_read<0>();
-      wg_bar(bar);
-    };
-    auto ready = [&](uint32_t off, uint32_t chunks) {
-      fence_proxy_async_smem();
-      wg_bar(bar);
-      if (wg_leader) store_rows(ad + off, s.img_hi, h, chunks);
-    };
+    const StashWriter<false> sw{ad, wg_leader, bar, h};   // every finished fp16 image goes to the adjoint stash
 
     float e[3] = {0.f, 0.f, 0.f};
     float r = 0.f, G = 0.f, beta = 0.f;
@@ -357,7 +326,7 @@ __global__ void __launch_bounds__(kDivThreads, 1) div_bwd_kernel(const DivParams
     const float rp = 2.0f * r * (1.0f - r);
     const float tb_c = Gs * beta * rp;   // adjoint of tau_c
     // ---- [taubar_off (3) | 0], taubar_off = G r e ----
-    stash_begin();
+    sw.begin();
     if (row_thread) {
       const uint2 t01 = split_h2(Gs * r * e[0], Gs * r * e[1]), t2 = split_h2(Gs * r * e[2], 0.f);
       *reinterpret_cast<uint4*>(s.img_hi + row_off) = make_uint4(t01.x, t2.x, 0u, 0u);
@@ -365,21 +334,21 @@ __global__ void __launch_bounds__(kDivThreads, 1) div_bwd_kernel(const DivParams
       *reinterpret_cast<uint4*>(s.img_hi + row_off + kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
       *reinterpret_cast<uint4*>(s.img_lo + row_off + kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
     }
-    ready(kA4, 2);
+    sw.ready(adj_image(kGsYb4), s.img_hi);
     // ---- B4^T -> abar4 = D4 (W4^T taubar_off); B3^T -> [abar3 = D3 (W3^T abar4) | taubar_c | 0] ----
     {
-      float acc[32];
-      ReluMask<64> m;
-      m.load(mk + kMkHb4, h);
+      Acc<dgrad::B4T> acc;
+      ReluMask<kMkHb4.cols> m;
+      m.load(mk + kMkHb4.off, h);
       W.wait(&s.sh->w_full, 0, 340);
-      wg_mma_split<64, true>(acc, a_hi, a_lo, s, w_t4, 1);
-      stash_begin();
-      epi_mask_split<64>(acc, m, s, h);
-      ready(kA3, 8);
-      m.load(mk + kMkHb3, h);
-      wg_mma_split<64, true>(acc, a_hi, a_lo, s, w_t3, 4);
-      stash_begin();
-      epi_mask_split<64>(acc, m, s, h);
+      wg_mma_split<dgrad::B4T, true>(acc, a_hi, a_lo, s);
+      sw.begin();
+      epi_mask_split<kMkHb4.cols>(acc, m, s, h);
+      sw.ready(adj_image(kGsYb3), s.img_hi);
+      m.load(mk + kMkHb3.off, h);
+      wg_mma_split<dgrad::B3T, true>(acc, a_hi, a_lo, s);
+      sw.begin();
+      epi_mask_split<kMkHb3.cols>(acc, m, s, h);
       if (row_thread) {
         const uint2 t = split_h2(tb_c, 0.f);
         *reinterpret_cast<uint4*>(s.img_hi + row_off + 8 * kChunkBytes) = make_uint4(t.x, 0u, 0u, 0u);
@@ -387,22 +356,22 @@ __global__ void __launch_bounds__(kDivThreads, 1) div_bwd_kernel(const DivParams
         *reinterpret_cast<uint4*>(s.img_hi + row_off + 9 * kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
         *reinterpret_cast<uint4*>(s.img_lo + row_off + 9 * kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
       }
-      ready(kA2, 10);
+      sw.ready(adj_image(kGsYb2), s.img_hi);
     }
     // ---- B2^T -> [abar2 | qbar2] = D2/E2 [W2^T abar3 | R2^T taubar_c];  B1^T -> [abar1 | qbar1] ----
     {
-      float acc[48];
-      ReluMask<96> m;
-      m.load(mk + kMkHb2, h);
-      wg_mma_split<96, true>(acc, a_hi, a_lo, s, w_t2, 5);
-      stash_begin();
-      epi_mask_split<96>(acc, m, s, h);
-      ready(kA1, 12);
-      m.load(mk + kMkHb1, h);
-      wg_mma_split<96, true>(acc, a_hi, a_lo, s, w_t1, 6);
-      stash_begin();
-      epi_mask_split<96>(acc, m, s, h);
-      ready(kA0, 12);
+      Acc<dgrad::B2T> acc;
+      ReluMask<kMkHb2.cols> m;
+      m.load(mk + kMkHb2.off, h);
+      wg_mma_split<dgrad::B2T, true>(acc, a_hi, a_lo, s);
+      sw.begin();
+      epi_mask_split<kMkHb2.cols>(acc, m, s, h);
+      sw.ready(adj_image(kGsYb1), s.img_hi);
+      m.load(mk + kMkHb1.off, h);
+      wg_mma_split<dgrad::B1T, true>(acc, a_hi, a_lo, s);
+      sw.begin();
+      epi_mask_split<kMkHb1.cols>(acc, m, s, h);
+      sw.ready(adj_image(kGsYb0), s.img_hi);
     }
   }
   if (wg_leader) tma_bulk_wait<0>();   // all adjoint-stash stores complete before the CTA exits

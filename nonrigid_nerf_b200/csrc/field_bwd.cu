@@ -24,27 +24,24 @@ namespace {
 
 constexpr int kBwdStageLd = 66;   // floats per staged row (64 used)
 
-struct Shared {
-  uint64_t w_full[kRingStages];
-  uint64_t w_empty[kRingStages];
-  int abort_flag;
-};
+static_assert(dgrad::step(dgrad::L6T) == dgrad::step(dgrad::L7T) && dgrad::step(dgrad::L5hT) == dgrad::step(dgrad::L7T) &&
+              dgrad::step(dgrad::L4T) == dgrad::step(dgrad::L7T) && dgrad::step(dgrad::L3T) == dgrad::step(dgrad::L7T) &&
+              dgrad::step(dgrad::L2T) == dgrad::step(dgrad::L7T) && dgrad::step(dgrad::L1T) == dgrad::step(dgrad::L7T),
+              "step_at: one default shape; the consumers run L5h^T .. L1^T as one loop");
+constexpr uint32_t kSlabA = 2 * dgrad::step(dgrad::L4T).k16 * kChunkBytes;   // A operand bytes of one weight slab
 
-struct StepShape {
-  uint32_t N, nslabs, slab_bytes, k16;
-};
-
-__device__ __forceinline__ StepShape step_shape(int step) {
+// step -> shape for a run-time step index: a switch over immediate table entries (no table in memory)
+__device__ __forceinline__ Step step_at(int step) {
   switch (step) {
-    case 0: return {256u, 1u, (uint32_t)kNerfTHeadBytes, 1u};
-    case 3: return {64u, 1u, 32768u, 16u};
-    case 9: return {64u, 1u, 32768u, 16u};
-    case 10: return {64u, 1u, (uint32_t)kBendTB4Bytes, 1u};
-    case 11: return {64u, 1u, (uint32_t)kBendTB3Bytes, 4u};
-    case 12: return {96u, 1u, (uint32_t)kBendTB2Bytes, 5u};
-    case 13: return {96u, 1u, (uint32_t)kBendTB1Bytes, 6u};
-    case 14: return {48u, 1u, (uint32_t)kBendTB0Bytes, 6u};
-    default: return {256u, 4u, 32768u, 4u};
+    case dgrad::HeadT: return step_imm<dgrad::HeadT>();
+    case dgrad::L5eT: return step_imm<dgrad::L5eT>();
+    case dgrad::L0T: return step_imm<dgrad::L0T>();
+    case dgrad::B4T: return step_imm<dgrad::B4T>();
+    case dgrad::B3T: return step_imm<dgrad::B3T>();
+    case dgrad::B2T: return step_imm<dgrad::B2T>();
+    case dgrad::B1T: return step_imm<dgrad::B1T>();
+    case dgrad::B0T: return step_imm<dgrad::B0T>();
+    default: return step_imm<dgrad::L7T>();   // L7^T, L6^T, L5h^T, L4^T .. L1^T
   }
 }
 
@@ -93,28 +90,6 @@ __device__ __forceinline__ void pe_backward(const float* de, const uint8_t* __re
   }
 }
 
-// One halving step of warp_transpose_reduce on the first N entries (a compile-time N keeps every index static, so v
-// stays in registers).
-template <int N>
-__device__ __forceinline__ void transpose_reduce_step(float (&v)[32], int lane) {
-  if constexpr (N > 1) {
-    constexpr int off = N / 2;
-    const bool upper = (lane & off) != 0;
-#pragma unroll
-    for (int i = 0; i < off; ++i) {
-      const float lo = v[i], hi = v[i + off];
-      v[i] = (upper ? hi : lo) + __shfl_xor_sync(0xffffffffu, upper ? lo : hi, off);
-    }
-    transpose_reduce_step<off>(v, lane);
-  }
-}
-
-// Sum over the warp's 32 lanes of v[j] for each j; lane L returns the total of column L.
-__device__ __forceinline__ float warp_transpose_reduce(float (&v)[32], int lane) {
-  transpose_reduce_step<32>(v, lane);
-  return v[0];
-}
-
 }  // namespace
 
 template <bool HAS_BENDER>
@@ -123,20 +98,12 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
   uint8_t* act = smem;                               // 64 KB gradient operand, 128 rows
   uint8_t* ring_buf = smem + kHBytes;                // kRingStages x 32 KB
   float* stage_all = reinterpret_cast<float*>(ring_buf + kRingStages * kRingStageBytes);   // 2 x 64 rows x kBwdStageLd
-  Shared* sh = reinterpret_cast<Shared*>(stage_all + 2 * kWgRows * kBwdStageLd);
+  RingShared* sh = reinterpret_cast<RingShared*>(stage_all + 2 * kWgRows * kBwdStageLd);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  constexpr int kNumSteps = HAS_BENDER ? 15 : 10;
 
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < kRingStages; ++i) {
-      mbar_init(&sh->w_full[i], 1);
-      mbar_init(&sh->w_empty[i], 8);
-    }
-    sh->abort_flag = 0;
-    fence_mbar_init();
-  }
+  if (threadIdx.x == 0) sh->init();
   __syncthreads();
   const Waiter W{&sh->abort_flag, p.err};
   Ring ring{ring_buf, sh->w_full, sh->w_empty};
@@ -144,18 +111,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
   if (warp >= 8) {
     setmaxnreg_dec<kProducerRegs>();
     // ===================== weight producer (W^T images) =====================
-    if (warp == 8 && lane == 0) {
-      for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
-        uint32_t gn = 0, gb = 0;
-#pragma unroll 1
-        for (int step = 0; step < kNumSteps; ++step) {
-          const StepShape s = step_shape(step);
-          const uint8_t* src = step < 10 ? p.nerf_wT + gn : p.bend_wT + gb;
-          for (uint32_t j = 0; j < s.nslabs; ++j) ring_put(ring, src + j * s.slab_bytes, s.slab_bytes, W);
-          if (step < 10) gn += s.nslabs * s.slab_bytes; else gb += s.nslabs * s.slab_bytes;
-        }
-      }
-    }
+    if (warp == 8 && lane == 0) produce(p.nerf_wT, p.bend_wT, p.n_tiles, 0, HAS_BENDER ? dgrad::kCount : dgrad::B4T, dgrad::B4T, step_at, ring, W);
     return;
   }
 
@@ -169,20 +125,11 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
   const int row = g * kWgRows + tw;       // tile row of a row thread
   uint8_t* a_row = act + row * 16;
   const uint32_t a_base = smem_u32(act) + g * kWgRows * 16;
-  auto a_slab = [&](uint32_t j) { return a_base + j * 8 * kChunkBytes; };
+  auto a_slab = [&](uint32_t j) { return a_base + j * kSlabA; };
   float* stg = stage_all + g * kWgRows * kBwdStageLd;
   const float* my_stg = stg + tw * kBwdStageLd;
 
-  // power-of-two loss scale from max|d_raw| (written by the compositing backward kernel)
-  float scale = 1.0f;
-  {
-    const float amax = p.amax ? __ldg(p.amax) : 0.f;
-    if (amax > 0.f && amax < 3.0e38f) {
-      int e;
-      frexpf(amax, &e);                       // amax = m * 2^e, m in [0.5, 1)
-      scale = ldexpf(1.0f, min(max(10 - e, -60), 60));  // max|d_raw| * scale in [512, 1024)
-    }
-  }
+  const float scale = loss_scale(p.amax);   // max|d_raw| is written by the compositing backward kernel
   const float inv_scale = 1.0f / scale;
 
   for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
@@ -191,25 +138,16 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
     const uint8_t* st_tile = p.stash + static_cast<long long>(tile) * kStashTileBytes;
     const uint8_t* st = st_tile + row * 16;
     uint8_t* gs = p.gstash + static_cast<long long>(tile) * kGradTileBytes;
-    // gradient stash: bulk TMA stores of finished images from shared memory (see field_fwd.cu)
-    auto stash_begin = [&]() {
-      if (wg_leader) tma_bulk_wait_read<0>();
-      wg_bar(bar);
-    };
-    auto ready = [&](uint32_t off, uint32_t chunks) {
-      fence_proxy_async_smem();
-      wg_bar(bar);
-      if (wg_leader && chunks) store_rows(gs + off, act, g, chunks);
-    };
+    const StashWriter<false> sw{gs, wg_leader, bar, g};
     // The ReLU masks are bits the forward kernel wrote (ReluMask): each thread loads its few words of a step's mask
     // before that step's MMAs, which hide the latency.  The embedding pe_backward reads from the forward stash is pulled
     // into L2 by one thread while the epilogue of the step before runs.
     const uint8_t* mk = p.relu_mask + static_cast<long long>(tile) * kMaskTileBytes;
     auto prefetch_e = [&]() {
-      if (wg_leader) tma_prefetch_l2(st_tile + kStE, kEBytes);
+      if (wg_leader) tma_prefetch_l2(st_tile + kStE.off, kEBytes);
     };
     // ---- d_raw image: [g_r g_g g_b g_sigma 0 ...] (K = 16) ----
-    stash_begin();
+    sw.begin();
     if (row_thread) {
       float gr[4] = {0.f, 0.f, 0.f, 0.f};
       if (valid) {
@@ -220,54 +158,54 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
       *reinterpret_cast<uint4*>(a_row) = make_uint4(pack_h2(gr[0], gr[1]), pack_h2(gr[2], gr[3]), 0u, 0u);
       *reinterpret_cast<uint4*>(a_row + kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
     }
-    ready(kGsRaw, 2);
+    sw.ready(kGsRaw, act);
     float dx[3] = {0.f, 0.f, 0.f};
-    // ---- head^T, L7^T, L6^T : dY7, dY6, dY5 ----
+    // ---- head^T, L7^T, L6^T : dY7, dY6, dY5 (every one 256 wide) ----
 #pragma unroll 1
     for (int s = 0; s < 3; ++s) {
-      const StepShape sh_ = step_shape(s);
-      float acc[128];
-      ReluMask<256> m;
+      const Step st = step_at(dgrad::HeadT + s);
+      Acc<dgrad::L7T> acc;
+      ReluMask<kMaskHCols> m;
       m.load(mk + kMkH + (7 - s) * kMaskHBytes, g);
-      wg_gemm<256>(acc, ring, sh_.nslabs, sh_.k16, a_slab, W, 300 + s);
+      wg_gemm<dgrad::step(dgrad::L7T).N>(acc, ring, st.nslabs, st.k16, a_slab, W, 300 + s);
       if (s == 2) prefetch_e();
-      stash_begin();
-      epi_mask_store<256>(acc, m, act, g);
-      ready(kGsY + (7 - s) * kHBytes, 32);
+      sw.begin();
+      epi_mask_store<kMaskHCols>(acc, m, act, g);
+      sw.ready({kGsY + (7 - s) * kHBytes, kHChunks}, act);
     }
     // ---- L5e^T: gradient into the skip-connected embedding ----
     {
-      float acc[32];
-      wg_gemm<64>(acc, ring, 1, 16, a_slab, W, 303);
+      Acc<dgrad::L5eT> acc;
+      wg_gemm_step<dgrad::L5eT>(acc, ring, a_slab, W, 303);
       stage_cols<0, 8>(acc, stg, kBwdStageLd);
       wg_bar(bar);
-      if (row_thread) pe_backward(my_stg, st + kStE, dx);
+      if (row_thread) pe_backward(my_stg, st + kStE.off, dx);
       // A operand (dY5) untouched; the staging rows are rewritten only after the barriers of the next steps
     }
-    // ---- L5h^T, L4^T .. L1^T : dY4 .. dY0 ----
+    // ---- L5h^T, L4^T .. L1^T : dY4 .. dY0 (one shape) ----
 #pragma unroll 1
     for (int s = 0; s < 5; ++s) {
-      float acc[128];
-      ReluMask<256> m;
+      Acc<dgrad::L4T> acc;
+      ReluMask<kMaskHCols> m;
       m.load(mk + kMkH + (4 - s) * kMaskHBytes, g);
-      wg_gemm<256>(acc, ring, 4, 4, a_slab, W, 304 + s);
+      wg_gemm_step<dgrad::L4T>(acc, ring, a_slab, W, 304 + s);
       if (s == 4) prefetch_e();
-      stash_begin();
-      epi_mask_store<256>(acc, m, act, g);
-      ready(kGsY + (4 - s) * kHBytes, 32);
+      sw.begin();
+      epi_mask_store<kMaskHCols>(acc, m, act, g);
+      sw.ready({kGsY + (4 - s) * kHBytes, kHChunks}, act);
     }
     // ---- L0^T: gradient into the embedding; then through the bend ----
     {
-      float acc[32];
-      wg_gemm<64>(acc, ring, 1, 16, a_slab, W, 309);
+      Acc<dgrad::L0T> acc;
+      wg_gemm_step<dgrad::L0T>(acc, ring, a_slab, W, 309);
       stage_cols<0, 8>(acc, stg, kBwdStageLd);
       wg_bar(bar);
-      if (row_thread) pe_backward(my_stg, st + kStE, dx);
+      if (row_thread) pe_backward(my_stg, st + kStE.off, dx);
     }
     if (!HAS_BENDER) continue;   // xyz has no learnable upstream without a bender (appendix C)
 
     float drpre = 0.f;
-    stash_begin();
+    sw.begin();
     if (row_thread) {
       float rig = 0.f, un[3] = {0.f, 0.f, 0.f}, dun[3], dm[3];
       float up_r = 0.f, up_u[3] = {0.f, 0.f, 0.f};
@@ -295,50 +233,50 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
       *reinterpret_cast<uint4*>(a_row) = make_uint4(pack_h2(clamp_h(dun[0]), clamp_h(dun[1])), pack_h2(clamp_h(dun[2]), 0.f), 0u, 0u);
       *reinterpret_cast<uint4*>(a_row + kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
     }
-    ready(kGsYb4, 2);
+    sw.ready(kGsYb4, act);
     // ---- B4^T -> dYb3 ----
     {
-      float acc[32];
-      ReluMask<64> m;
-      m.load(mk + kMkHb4, g);
-      wg_gemm<64>(acc, ring, 1, 1, a_slab, W, 310);
-      stash_begin();
-      epi_mask_store<64>(acc, m, act, g);
-      ready(kGsYb3, 8);
+      Acc<dgrad::B4T> acc;
+      ReluMask<kMkHb4.cols> m;
+      m.load(mk + kMkHb4.off, g);
+      wg_gemm_step<dgrad::B4T>(acc, ring, a_slab, W, 310);
+      sw.begin();
+      epi_mask_store<kMkHb4.cols>(acc, m, act, g);
+      sw.ready(kGsYb3, act);
     }
     // ---- B3^T -> dYb2 = [dh * mask (64) | d rigidity pre-activation | 0 (15)] ----
     {
-      float acc[32];
-      ReluMask<64> m;
-      m.load(mk + kMkHb3, g);
-      wg_gemm<64>(acc, ring, 1, 4, a_slab, W, 311);
-      stash_begin();
-      epi_mask_store<64>(acc, m, act, g);
+      Acc<dgrad::B3T> acc;
+      ReluMask<kMkHb3.cols> m;
+      m.load(mk + kMkHb3.off, g);
+      wg_gemm_step<dgrad::B3T>(acc, ring, a_slab, W, 311);
+      sw.begin();
+      epi_mask_store<kMkHb3.cols>(acc, m, act, g);
       if (row_thread) {
         *reinterpret_cast<uint4*>(a_row + 8 * kChunkBytes) = make_uint4(pack_h2(clamp_h(drpre), 0.f), 0u, 0u, 0u);
         *reinterpret_cast<uint4*>(a_row + 9 * kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
       }
-      ready(kGsYb2, 10);
+      sw.ready(kGsYb2, act);
     }
     // ---- B2^T -> dYb1, B1^T -> dYb0 ----
     {
-      float acc[48];
-      ReluMask<96> m;
-      m.load(mk + kMkHb2, g);
-      wg_gemm<96>(acc, ring, 1, 5, a_slab, W, 312);
-      stash_begin();
-      epi_mask_store<96>(acc, m, act, g);
-      ready(kGsYb1, 12);
-      m.load(mk + kMkHb1, g);
-      wg_gemm<96>(acc, ring, 1, 6, a_slab, W, 313);
-      stash_begin();
-      epi_mask_store<96>(acc, m, act, g);
-      ready(kGsYb0, 12);
+      Acc<dgrad::B2T> acc;
+      ReluMask<kMkHb2.cols> m;
+      m.load(mk + kMkHb2.off, g);
+      wg_gemm_step<dgrad::B2T>(acc, ring, a_slab, W, 312);
+      sw.begin();
+      epi_mask_store<kMkHb2.cols>(acc, m, act, g);
+      sw.ready(kGsYb1, act);
+      m.load(mk + kMkHb1.off, g);
+      wg_gemm_step<dgrad::B1T>(acc, ring, a_slab, W, 313);
+      sw.begin();
+      epi_mask_store<kMkHb1.cols>(acc, m, act, g);
+      sw.ready(kGsYb0, act);
     }
     // ---- B0^T: d(bender input); columns 6..37 are the latent code -> per-ray reduction ----
     {
-      float acc[24];
-      wg_gemm<48>(acc, ring, 1, 6, a_slab, W, 314);
+      Acc<dgrad::B0T> acc;
+      wg_gemm_step<dgrad::B0T>(acc, ring, a_slab, W, 314);
       stage_cols<0, 5>(acc, stg, kBwdStageLd);
       wg_bar(bar);
       if (row_thread) {   // warps 0 and 1 of the warpgroup: 32 consecutive rows each
@@ -356,27 +294,15 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
         }
       }
     }
-    // next: the next tile's d_raw image (after stash_begin's barrier)
+    // next: the next tile's d_raw image (after sw.begin()'s barrier)
   }
   if (wg_leader) tma_bulk_wait<0>();   // all gradient-stash stores complete before the CTA exits
 }
 
 // ------------------------------------------------------------------------------------------------
 cudaError_t launch_field_bwd(const FieldBwdParams& p, bool has_bender, int num_sms, cudaStream_t stream) {
-  const size_t smem = kHBytes + kRingStages * kRingStageBytes + 2 * kWgRows * kBwdStageLd * sizeof(float) + sizeof(Shared) + 64;
-  if (p.n_tiles <= 0) return cudaSuccess;
-  const int grid = p.n_tiles < num_sms ? p.n_tiles : num_sms;
-  cudaError_t e;
-  if (has_bender) {
-    e = cudaFuncSetAttribute(field_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    field_bwd_kernel<true><<<grid, kFwdThreads, smem, stream>>>(p);
-  } else {
-    e = cudaFuncSetAttribute(field_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    field_bwd_kernel<false><<<grid, kFwdThreads, smem, stream>>>(p);
-  }
-  return cudaGetLastError();
+  const size_t smem = kHBytes + kRingStages * kRingStageBytes + 2 * kWgRows * kBwdStageLd * sizeof(float) + sizeof(RingShared) + 64;
+  return launch_field(has_bender ? field_bwd_kernel<true> : field_bwd_kernel<false>, p, num_sms, smem, stream);
 }
 
 }  // namespace nrn

@@ -23,36 +23,30 @@ namespace {
 
 constexpr int kFwdStageLd = 12;   // floats per staged row (8 used)
 
-struct Shared {
-  uint64_t w_full[kRingStages];
-  uint64_t w_empty[kRingStages];
-  int abort_flag;
-};
-
-struct StepShape {
-  uint32_t N, nslabs, slab_bytes, k16;
-};
-
-// step index: 0-4 bender B0..B4, 5-12 NeRF L0..L7, 13 head
-__device__ __forceinline__ StepShape step_shape(int step) {
+static_assert(fwd::step(fwd::L2) == fwd::step(fwd::L1) && fwd::step(fwd::L3) == fwd::step(fwd::L1) &&
+              fwd::step(fwd::L4) == fwd::step(fwd::L1) && fwd::step(fwd::L6) == fwd::step(fwd::L1) &&
+              fwd::step(fwd::L7) == fwd::step(fwd::L1), "step_at: one default shape");
+// step -> shape for a run-time step index: a switch over immediate table entries (no table in memory)
+__device__ __forceinline__ Step step_at(int step) {
   switch (step) {
-    case 0: return {96u, 1u, (uint32_t)kBendB0Bytes, 3u};
-    case 1: return {96u, 1u, (uint32_t)kBendB1Bytes, 6u};
-    case 2: return {80u, 1u, (uint32_t)kBendB2Bytes, 6u};
-    case 3: return {64u, 1u, (uint32_t)kBendB3Bytes, 4u};
-    case 4: return {16u, 1u, (uint32_t)kBendB4Bytes, 4u};
-    case 5: return {256u, 1u, 32768u, 4u};
-    case 10: return {256u, 5u, 32768u, 4u};
-    case 13: return {16u, 1u, (uint32_t)kNerfHeadBytes, 16u};
-    default: return {256u, 4u, 32768u, 4u};
+    case fwd::B0: return step_imm<fwd::B0>();
+    case fwd::B1: return step_imm<fwd::B1>();
+    case fwd::B2: return step_imm<fwd::B2>();
+    case fwd::B3: return step_imm<fwd::B3>();
+    case fwd::B4: return step_imm<fwd::B4>();
+    case fwd::L0: return step_imm<fwd::L0>();
+    case fwd::L5: return step_imm<fwd::L5>();
+    case fwd::Head: return step_imm<fwd::Head>();
+    default: return step_imm<fwd::L1>();   // L1-L4, L6, L7: one shape
   }
 }
 // byte offset (inside the activation region: H at 0, E at kHBytes) of the A operand of slab j
 __device__ __forceinline__ uint32_t a_operand_offset(int step, uint32_t j) {
-  if (step == 0 || step == 5) return kHBytes;                       // bender input / embedding live in E
-  if (step == 10) return j == 0 ? kHBytes : (j - 1) * 8 * kChunkBytes;  // skip: [embedding | h]
-  if (step < 5 || step == 13) return 0;
-  return j * 8 * kChunkBytes;
+  if (step == fwd::B0 || step == fwd::L0) return kHBytes;                          // bender input / embedding live in E
+  constexpr uint32_t kSlabA = 2 * fwd::step(fwd::L1).k16 * kChunkBytes;   // A operand bytes of one slab of the hidden layers
+  if (step == fwd::L5) return j == 0 ? kHBytes : (j - 1) * kSlabA;      // skip: [embedding | h]
+  if (step < fwd::L0 || step == fwd::Head) return 0;
+  return j * kSlabA;
 }
 
 // Accumulator columns [0, NCOLS) + bias, ReLU, fp16 -> this warpgroup's rows of the chunk-major image `img`.  MASK
@@ -123,20 +117,12 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
   uint8_t* act = smem;                                  // H | E, 128 rows
   uint8_t* ring_buf = smem + kSlotBytes;                // kRingStages x 32 KB
   float* stage_all = reinterpret_cast<float*>(ring_buf + kRingStages * kRingStageBytes);   // 2 x 64 rows x kFwdStageLd
-  Shared* sh = reinterpret_cast<Shared*>(stage_all + 2 * kWgRows * kFwdStageLd);
+  RingShared* sh = reinterpret_cast<RingShared*>(stage_all + 2 * kWgRows * kFwdStageLd);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  constexpr int kFirstStep = HAS_BENDER ? 0 : 5;
 
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < kRingStages; ++i) {
-      mbar_init(&sh->w_full[i], 1);
-      mbar_init(&sh->w_empty[i], 8);
-    }
-    sh->abort_flag = 0;
-    fence_mbar_init();
-  }
+  if (threadIdx.x == 0) sh->init();
   __syncthreads();
   const Waiter W{&sh->abort_flag, p.err};
   Ring ring{ring_buf, sh->w_full, sh->w_empty};
@@ -144,18 +130,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
   if (warp >= 8) {
     setmaxnreg_dec<kProducerRegs>();
     // ===================== weight producer: global -> smem ring (bulk TMA) =====================
-    if (warp == 8 && lane == 0) {
-      for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
-        uint32_t gb = 0, gn = 0;
-#pragma unroll 1
-        for (int step = kFirstStep; step < 14; ++step) {
-          const StepShape s = step_shape(step);
-          const uint8_t* src = step < 5 ? p.bend_w + gb : p.nerf_w + gn;
-          for (uint32_t j = 0; j < s.nslabs; ++j) ring_put(ring, src + j * s.slab_bytes, s.slab_bytes, W);
-          if (step < 5) gb += s.nslabs * s.slab_bytes; else gn += s.nslabs * s.slab_bytes;
-        }
-      }
-    }
+    if (warp == 8 && lane == 0) produce(p.bend_w, p.nerf_w, p.n_tiles, HAS_BENDER ? fwd::B0 : fwd::L0, fwd::kCount, fwd::L0, step_at, ring, W);
     return;
   }
 
@@ -177,23 +152,11 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
   for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
     const long long pt = static_cast<long long>(tile) * kTileM + g * kWgRows + tw;
     const bool valid = row_thread && pt < p.P;
-    // Training stash: every finished activation image is written to this tile's stash block with bulk TMA stores
-    // issued by one thread of the warpgroup (its 64 rows of each chunk); the epilogue threads spend no load/store
-    // slots on it.  stash_begin(): the previous stores must have finished READING shared memory before any image is
-    // overwritten; it also orders every warp's wgmma reads of an operand before any warp rewrites it in place.
-    // ready(): the image is complete and visible to the async proxy (wgmma operand, TMA store).
+    // Training stash: every finished activation image goes to this tile's stash block
     uint8_t* st = p.stash ? p.stash + static_cast<long long>(tile) * kStashTileBytes : nullptr;
+    const StashWriter<true> sw{st, wg_leader, bar, g};
     // ReLU masks for DGRAD (training): every row of the tile is written, those past P of a ragged last tile included
     uint8_t* mk = TRAIN ? p.relu_mask + static_cast<long long>(tile) * kMaskTileBytes : nullptr;
-    auto stash_begin = [&]() {
-      if (st && wg_leader) tma_bulk_wait_read<0>();
-      wg_bar(bar);
-    };
-    auto ready = [&](uint32_t stash_off, const uint8_t* img, uint32_t chunks) {
-      fence_proxy_async_smem();
-      wg_bar(bar);
-      if (st && wg_leader && chunks) store_rows(st + stash_off, img, g, chunks);
-    };
     float x[3] = {0.f, 0.f, 0.f};
     long long ray = 0;
     if (valid) {
@@ -216,7 +179,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
     float rigidity = 0.f;
     if (HAS_BENDER) {
       // ---- bender input row: [xyz_hi(3) xyz_lo(3) latent(32) 0(10)] fp16, chunks 0..5 of E ----
-      stash_begin();
+      sw.begin();
       if (row_thread) {
         float in[48];
 #pragma unroll
@@ -240,48 +203,48 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
           *reinterpret_cast<uint4*>(e_row + c * kChunkBytes) = pk;
         }
       }
-      ready(kStBin, Es, 6);
+      sw.ready(kStBin, Es);
       // ---- B0, B1: 96 hidden units (64 offset | 32 rigidity) ----
       {
-        float acc[48];
-        wg_gemm<96>(acc, ring, 1, 3, [&](uint32_t) { return a_e; }, W, 301);
-        stash_begin();
-        epi_bias_relu_store<96, TRAIN>(acc, p.bend_bias, Hs, g, mk, kMkHb1);
-        ready(kStHb1, Hs, 12);
-        wg_gemm<96>(acc, ring, 1, 6, [&](uint32_t) { return a_h; }, W, 302);
-        stash_begin();
-        epi_bias_relu_store<96, TRAIN>(acc, p.bend_bias + 96, Hs, g, mk, kMkHb2);
-        ready(kStHb2, Hs, 12);
+        Acc<fwd::B0> acc;
+        wg_gemm_step<fwd::B0>(acc, ring, [&](uint32_t) { return a_e; }, W, 301);
+        sw.begin();
+        epi_bias_relu_store<kMkHb1.cols, TRAIN>(acc, p.bend_bias + fwd::b_off(fwd::B0), Hs, g, mk, kMkHb1.off);
+        sw.ready(kStHb1, Hs);
+        wg_gemm_step<fwd::B1>(acc, ring, [&](uint32_t) { return a_h; }, W, 302);
+        sw.begin();
+        epi_bias_relu_store<kMkHb2.cols, TRAIN>(acc, p.bend_bias + fwd::b_off(fwd::B1), Hs, g, mk, kMkHb2.off);
+        sw.ready(kStHb2, Hs);
       }
       // ---- B2: 64 offset hidden + rigidity output (column 64) ----
       {
-        float acc[40];
-        wg_gemm<80>(acc, ring, 1, 6, [&](uint32_t) { return a_h; }, W, 303);
-        stash_begin();
-        epi_bias_relu_store<64, TRAIN>(acc, p.bend_bias + 192, Hs, g, mk, kMkHb3);
+        Acc<fwd::B2> acc;
+        wg_gemm_step<fwd::B2>(acc, ring, [&](uint32_t) { return a_h; }, W, 303);
+        sw.begin();
+        epi_bias_relu_store<kMkHb3.cols, TRAIN>(acc, p.bend_bias + fwd::b_off(fwd::B2), Hs, g, mk, kMkHb3.off);
         if (acc_q() == 0) {
           stg[acc_r0() * kFwdStageLd] = acc[32];
           stg[(acc_r0() + 8) * kFwdStageLd] = acc[34];
         }
-        ready(kStHb3, Hs, 8);
+        sw.ready(kStHb3, Hs);
         if (row_thread) {
-          const float rr = my_stg[0] + __ldg(p.bend_bias + 192 + 64);
+          const float rr = my_stg[0] + __ldg(p.bend_bias + fwd::b_off(fwd::B2) + 64);
           rigidity = (tanhf(rr) + 1.0f) * 0.5f;   // run_nerf_helpers.py:559-561
           if (p.use_cutoff && rigidity <= p.cutoff) rigidity = 0.f;  // :563-564
         }
       }
       // ---- B3 ----
       {
-        float acc[32];
-        wg_gemm<64>(acc, ring, 1, 4, [&](uint32_t) { return a_h; }, W, 304);
-        stash_begin();
-        epi_bias_relu_store<64, TRAIN>(acc, p.bend_bias + 272, Hs, g, mk, kMkHb4);
-        ready(kStHb4, Hs, 8);
+        Acc<fwd::B3> acc;
+        wg_gemm_step<fwd::B3>(acc, ring, [&](uint32_t) { return a_h; }, W, 304);
+        sw.begin();
+        epi_bias_relu_store<kMkHb4.cols, TRAIN>(acc, p.bend_bias + fwd::b_off(fwd::B3), Hs, g, mk, kMkHb4.off);
+        sw.ready(kStHb4, Hs);
       }
       // ---- B4: offsets; bend ----
       {
-        float acc[8];
-        wg_gemm<16>(acc, ring, 1, 4, [&](uint32_t) { return a_h; }, W, 305);
+        Acc<fwd::B4> acc;
+        wg_gemm_step<fwd::B4>(acc, ring, [&](uint32_t) { return a_h; }, W, 305);
         stage_cols<0, 1>(acc, stg, kFwdStageLd);
         wg_bar(bar);
         if (row_thread) {
@@ -306,30 +269,30 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
       p.d_bent[pt * 3 + 0] = x[0]; p.d_bent[pt * 3 + 1] = x[1]; p.d_bent[pt * 3 + 2] = x[2];
     }
     // ---- positional encoding of the (bent) point -> E ----
-    stash_begin();
+    sw.begin();
     if (row_thread) write_pe(x, e_row);
-    ready(kStE, Es, 8);
-    // ---- L0 .. L7 ----
+    sw.ready(kStE, Es);
+    // ---- L0 .. L7 (every one 256 wide) ----
 #pragma unroll 1
     for (int L = 0; L < 8; ++L) {
-      const int step = 5 + L;
-      const StepShape s = step_shape(step);
-      float acc[128];
-      wg_gemm<256>(acc, ring, s.nslabs, s.k16, [&](uint32_t j) { return a_h + a_operand_offset(step, j); }, W, 310 + L);
-      stash_begin();
-      epi_bias_relu_store<256, TRAIN>(acc, p.nerf_bias + L * 256, Hs, g, mk, kMkH + L * kMaskHBytes);
-      ready(kStH + L * kHBytes, Hs, 32);
+      const int step = fwd::L0 + L;
+      Acc<fwd::L1> acc;
+      const Step s = step_at(step);
+      wg_gemm<fwd::step(fwd::L1).N>(acc, ring, s.nslabs, s.k16, [&](uint32_t j) { return a_h + a_operand_offset(step, j); }, W, 310 + L);
+      sw.begin();
+      epi_bias_relu_store<kMaskHCols, TRAIN>(acc, p.nerf_bias + L * fwd::b_off(fwd::L1), Hs, g, mk, kMkH + L * kMaskHBytes);
+      sw.ready(st_h(L + 1), Hs);
     }
     // ---- head: raw = output_linear(h) (run_nerf_helpers.py:306) ----
     {
-      float acc[8];
-      wg_gemm<16>(acc, ring, 1, 16, [&](uint32_t) { return a_h; }, W, 320);
+      Acc<fwd::Head> acc;
+      wg_gemm_step<fwd::Head>(acc, ring, [&](uint32_t) { return a_h; }, W, 320);
       stage_cols<0, 1>(acc, stg, kFwdStageLd);
       wg_bar(bar);
       if (valid) {
         float o[5];
 #pragma unroll
-        for (int c = 0; c < 5; ++c) o[c] = my_stg[c] + __ldg(p.nerf_bias + 2048 + c);
+        for (int c = 0; c < 5; ++c) o[c] = my_stg[c] + __ldg(p.nerf_bias + fwd::b_off(fwd::Head) + c);
         // test-time non-rigid object removal (run_nerf_helpers.py:309-310)
         if (HAS_BENDER && p.use_removal && rigidity >= p.removal) o[3] *= 0.f;
         float* dst = p.raw + pt * p.out_ch;
@@ -343,24 +306,14 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
 
 // ------------------------------------------------------------------------------------------------
 size_t field_fwd_smem_bytes() {
-  return kSlotBytes + kRingStages * kRingStageBytes + 2 * kWgRows * kFwdStageLd * sizeof(float) + sizeof(Shared) + 64;
-}
-
-template <bool HAS_BENDER, bool TRAIN>
-static cudaError_t launch_field_fwd_t(const FieldFwdParams& p, int grid, size_t smem, cudaStream_t stream) {
-  const cudaError_t e = cudaFuncSetAttribute(field_fwd_kernel<HAS_BENDER, TRAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  field_fwd_kernel<HAS_BENDER, TRAIN><<<grid, kFwdThreads, smem, stream>>>(p);
-  return cudaGetLastError();
+  return kSlotBytes + kRingStages * kRingStageBytes + 2 * kWgRows * kFwdStageLd * sizeof(float) + sizeof(RingShared) + 64;
 }
 
 cudaError_t launch_field_fwd(const FieldFwdParams& p, bool has_bender, int num_sms, cudaStream_t stream) {
   const size_t smem = field_fwd_smem_bytes();
-  if (p.n_tiles <= 0) return cudaSuccess;
-  const int grid = p.n_tiles < num_sms ? p.n_tiles : num_sms;
   const bool train = p.relu_mask != nullptr;   // the C ABI passes the ReLU masks exactly when it passes the stash
-  if (has_bender) return train ? launch_field_fwd_t<true, true>(p, grid, smem, stream) : launch_field_fwd_t<true, false>(p, grid, smem, stream);
-  return train ? launch_field_fwd_t<false, true>(p, grid, smem, stream) : launch_field_fwd_t<false, false>(p, grid, smem, stream);
+  if (has_bender) return launch_field(train ? field_fwd_kernel<true, true> : field_fwd_kernel<true, false>, p, num_sms, smem, stream);
+  return launch_field(train ? field_fwd_kernel<false, true> : field_fwd_kernel<false, false>, p, num_sms, smem, stream);
 }
 
 }  // namespace nrn

@@ -13,24 +13,20 @@ namespace nrn {
 
 namespace {
 
-constexpr long long kWaitLimitCycles = 1ll << 28;  // ~0.15 s: protocol bug => error flag, not a hang
 constexpr int kWgRows = kTileM / 2;                 // rows of a tile owned by one consumer warpgroup
 
-struct Waiter {
-  int* s_abort;
-  int* g_err;
-  __device__ __forceinline__ bool wait(uint64_t* bar, uint32_t parity, int code) const {
-    if (mbar_try_wait(bar, parity)) return true;
-    const long long t0 = clock64();
-    while (!mbar_try_wait(bar, parity)) {
-      if (*reinterpret_cast<volatile int*>(s_abort)) return false;
-      if (clock64() - t0 > kWaitLimitCycles) {
-        atomicExch(s_abort, code);
-        atomicCAS(g_err, 0, code);
-        return false;
-      }
+// Weight ring barriers; one thread initialises them before the CTA's first barrier
+struct RingShared {
+  uint64_t w_full[kRingStages];
+  uint64_t w_empty[kRingStages];
+  int abort_flag;
+  __device__ __forceinline__ void init() {
+    for (int i = 0; i < kRingStages; ++i) {
+      mbar_init(&w_full[i], 1);
+      mbar_init(&w_empty[i], 8);
     }
-    return true;
+    abort_flag = 0;
+    fence_mbar_init();
   }
 };
 
@@ -51,6 +47,23 @@ __device__ __forceinline__ void ring_put(Ring& r, const uint8_t* src, uint32_t b
   mbar_arrive_expect_tx(&r.full[r.stage], bytes);
   for (uint32_t off = 0; off < bytes; off += 16384u) tma_bulk_g2s(dst + off, src + off, min(bytes - off, 16384u), &r.full[r.stage]);
   r.next();
+}
+
+// Producer thread: for every tile of this CTA, the weight images of steps [first, last) through the ring (shapes from
+// step_at(step)), those of steps before `split` from `w_lo`, the others from `w_hi`.
+template <typename StepAt>
+__device__ __forceinline__ void produce(const uint8_t* w_lo, const uint8_t* w_hi, int n_tiles, int first, int last, int split,
+                                        StepAt step_at, Ring& ring, const Waiter& W) {
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    uint32_t glo = 0, ghi = 0;
+#pragma unroll 1
+    for (int step = first; step < last; ++step) {
+      const Step s = step_at(step);
+      const uint8_t* src = step < split ? w_lo + glo : w_hi + ghi;
+      for (uint32_t j = 0; j < s.nslabs; ++j) ring_put(ring, src + j * s.slab_bytes, s.slab_bytes, W);
+      if (step < split) glo += s.nslabs * s.slab_bytes; else ghi += s.nslabs * s.slab_bytes;
+    }
+  }
 }
 
 // consumer warpgroup: acc[64 x N] = A . W^T accumulated over `nslabs` weight slabs of the ring (slab j: N rows x 16 k16
@@ -87,6 +100,22 @@ __device__ __forceinline__ void wg_gemm(float (&acc)[N / 2], Ring& r, uint32_t n
   acc_fence(acc);
   __syncwarp();
   if (lane == 0) mbar_arrive(&r.empty[prev]);
+}
+
+// Accumulators and wg_gemm of a step known at compile time (fwd:: or dgrad:: id): N, slabs and k16 from its table entry
+template <auto S>
+using Acc = float[step(S).N / 2];
+template <auto S, typename AAddr>
+__device__ __forceinline__ void wg_gemm_step(Acc<S>& acc, Ring& r, AAddr a_addr, const Waiter& W, int code) {
+  constexpr Step s = step(S);
+  wg_gemm<s.N>(acc, r, s.nslabs, s.k16, a_addr, W, code);
+}
+
+// A step's shape as immediates, for run-time step switches (a copied constexpr Step would be read from memory)
+template <auto S>
+__device__ __forceinline__ Step step_imm() {
+  constexpr Step s = step(S);
+  return {s.N, s.nslabs, s.slab_bytes, s.k16};
 }
 
 // Coordinates of this thread's accumulator elements (sm90_ptx.cuh): rows r0 and r0 + 8 of the warpgroup's 64,
@@ -166,6 +195,36 @@ __device__ __forceinline__ void store_rows(uint8_t* gdst, const uint8_t* img, in
   for (uint32_t c = 0; c < chunks; ++c)
     tma_bulk_s2g(gdst + c * kChunkBytes + g * kWgRows * 16, img + c * kChunkBytes + g * kWgRows * 16, kWgRows * 16);
   tma_bulk_commit();
+}
+
+// A warpgroup's writer of finished images to a tile's stash block by bulk TMA stores of one thread (`leader`), so the
+// epilogue threads spend no load/store slots on it (OPTIONAL: a null `tile` stores nothing).  begin(): the previous stores
+// have finished READING shared memory, and every warp's wgmma reads of an operand are done, before any image is rewritten.
+// ready(): the image `img` is complete and visible to the async proxy (wgmma operand, TMA store); it goes to `im`.
+template <bool OPTIONAL>
+struct StashWriter {
+  uint8_t* tile;
+  bool leader;
+  int bar, g;
+  __device__ __forceinline__ void begin() const {
+    if ((!OPTIONAL || tile) && leader) tma_bulk_wait_read<0>();
+    wg_bar(bar);
+  }
+  __device__ __forceinline__ void ready(Image im, const uint8_t* img) const {
+    fence_proxy_async_smem();
+    wg_bar(bar);
+    if ((!OPTIONAL || tile) && leader && im.chunks) store_rows(tile + static_cast<uint32_t>(im.off), img, g, im.chunks);
+  }
+};
+
+// Launch of a persistent field kernel: one CTA per SM at most, `smem` bytes of dynamic shared memory
+template <typename Kernel, typename Params>
+cudaError_t launch_field(Kernel kernel, const Params& p, int num_sms, size_t smem, cudaStream_t stream) {
+  if (p.n_tiles <= 0) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  kernel<<<p.n_tiles < num_sms ? p.n_tiles : num_sms, kFwdThreads, smem, stream>>>(p);
+  return cudaGetLastError();
 }
 
 }  // namespace

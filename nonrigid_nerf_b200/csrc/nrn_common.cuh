@@ -1,4 +1,4 @@
-// Shared definitions: packed-weight layout, kernel parameter blocks, launch helpers.
+// Shared definitions: the layout of the fused field path, kernel parameter blocks.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -6,114 +6,176 @@
 namespace nrn {
 
 // ------------------------------------------------------------------------------------------
-// Geometry of the fused field kernels
+// Layout of the fused field path: the shapes of the weight images (pack.cu), the GEMM steps of the forward, DGRAD and
+// divergence kernels, the stash, gradient-stash and ReLU-mask images of a tile, and the flat gradient buffers.  Every
+// kernel, the packer and the C ABI read these; a new layer is one entry here.
 // ------------------------------------------------------------------------------------------
 constexpr int kTileM = 128;                 // points per tile = 2 warpgroups x wgmma M (64)
 constexpr int kChunkBytes = kTileM * 16;    // one 8-column chunk of a 128-row activation image
-constexpr int kHBytes = 32 * kChunkBytes;   // 256-wide hidden activations, 64 KB
-constexpr int kEBytes = 8 * kChunkBytes;    // 64-wide positional embedding, 16 KB
-constexpr int kSlotBytes = kHBytes + kEBytes;
 constexpr int kRingStageBytes = 32768;      // one weight slab: 256 rows x 64 K-columns fp16
 constexpr int kRingStages = 4;
 constexpr int kFwdThreads = 384;            // 2 consumer warpgroups (MMA + epilogue), 1 producer warpgroup (one thread streams)
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // setmaxnreg budgets: 128 x (40 + 2 x 232) <= 64K
-
-// ------------------------------------------------------------------------------------------
-// Packed NeRF weights (fp16, chunk-major images in streaming order), see pack.cu
-//   L0   : [ 8 chunks][256 rows][8]  K = 63 (+1 zero pad)                 32 KB   (1 slab)
-//   L1-4 : [32 chunks][256 rows][8]                                       128 KB  (4 slabs each)
-//   L5   : [40 chunks][256 rows][8]  K = 64 (embedding, padded) + 256     160 KB  (5 slabs)
-//   L6-7 : [32 chunks][256 rows][8]                                       128 KB  (4 slabs each)
-//   head : [32 chunks][ 16 rows][8]  N = out_ch (<= 16, zero padded)      8 KB    (1 slab)
-// followed by fp32 biases: [8][256] + [16]
-// ------------------------------------------------------------------------------------------
-constexpr int kNerfL0Bytes = 8 * 256 * 16;
-constexpr int kNerfLBytes = 32 * 256 * 16;
-constexpr int kNerfL5Bytes = 40 * 256 * 16;
-constexpr int kNerfHeadBytes = 32 * 16 * 16;
-constexpr int kNerfWBytes = kNerfL0Bytes + 6 * kNerfLBytes + kNerfL5Bytes + kNerfHeadBytes;  // 991,232
-constexpr int kNerfBiasFloats = 8 * 256 + 16;
-constexpr int kNerfTOffset = kNerfWBytes + kNerfBiasFloats * 4;   // transposed images (DGRAD) follow the biases
-
-// Packed ray-bender weights (fp16): offset MLP and rigidity MLP fused block-diagonally.
-//   B0: N=96 K=48  rows 0-63 offset L0 (cols: xyz_hi 0-2, xyz_lo 3-5, latent 6-37), rows 64-95 rigidity L0
-//   B1: N=96 K=96  rows 0-63 offset L1 (cols 0-63),   rows 64-95 rigidity L1 (cols 64-95)
-//   B2: N=80 K=96  rows 0-63 offset L2 (cols 0-63),   row 64 rigidity L2 (cols 64-95)
-//   B3: N=64 K=64  offset L3
-//   B4: N=16 K=64  rows 0-2 offset L4 (no bias)
-// followed by fp32 biases: [96] [96] [80] [64]
-constexpr int kBendB0Bytes = 6 * 96 * 16;
-constexpr int kBendB1Bytes = 12 * 96 * 16;
-constexpr int kBendB2Bytes = 12 * 80 * 16;
-constexpr int kBendB3Bytes = 8 * 64 * 16;
-constexpr int kBendB4Bytes = 8 * 16 * 16;
-constexpr int kBendWBytes = kBendB0Bytes + kBendB1Bytes + kBendB2Bytes + kBendB3Bytes + kBendB4Bytes;  // 53,248
-constexpr int kBendBiasFloats = 96 + 96 + 80 + 64;
-constexpr int kBendTOffset = kBendWBytes + kBendBiasFloats * 4;
 constexpr int kLatent = 32;
 
-// ------------------------------------------------------------------------------------------
-// Training stash (forward -> backward), per 128-point tile, fp16 chunk-major tile images:
-//   E  (positional encoding of the bent point, 64 cols; the pad column 63 holds 1.0 so that the
-//       WGRAD of L0 / L5 yields the bias gradient in that column)
-//   H1..H8 (post-ReLU activations), bender input and hidden activations.
-// Gradient stash (DGRAD -> WGRAD), same format: d_raw, dY7..dY0, bender dY's.
-// ------------------------------------------------------------------------------------------
-constexpr int kStE = 0;
-constexpr int kStH = kStE + kEBytes;                       // H_l at kStH + (l-1)*kHBytes, l = 1..8
-constexpr int kStBin = kStH + 8 * kHBytes;                 // bender input, 6 chunks
-constexpr int kStHb1 = kStBin + 6 * kChunkBytes;           // 12 chunks
-constexpr int kStHb2 = kStHb1 + 12 * kChunkBytes;          // 12 chunks
-constexpr int kStHb3 = kStHb2 + 12 * kChunkBytes;          // 8 chunks
-constexpr int kStHb4 = kStHb3 + 8 * kChunkBytes;           // 8 chunks
-constexpr int kStashTileBytes = kStHb4 + 8 * kChunkBytes;  // 634,880
+// A packed weight image: `rows` output features (the MMA's N) x `chunks` 8-column K chunks, fp16, chunk-major
+// ([chunk][row][8]); t(): its transpose W^T (DGRAD).
+struct WImage {
+  int rows, chunks;
+  __host__ __device__ constexpr int bytes() const { return rows * chunks * 16; }
+  __host__ __device__ constexpr WImage t() const { return {8 * chunks, rows / 8}; }
+};
 
-constexpr int kGsRaw = 0;                                  // d_raw, 2 chunks (16 cols)
-constexpr int kGsY = kGsRaw + 2 * kChunkBytes;             // dY_l at kGsY + l*kHBytes, l = 0..7
-constexpr int kGsYb4 = kGsY + 8 * kHBytes;                 // 2 chunks (d unmasked offsets)
-constexpr int kGsYb3 = kGsYb4 + 2 * kChunkBytes;           // 8 chunks
-constexpr int kGsYb2 = kGsYb3 + 8 * kChunkBytes;           // 10 chunks (64 + rigidity pre-activation + pad)
-constexpr int kGsYb1 = kGsYb2 + 10 * kChunkBytes;          // 12 chunks
-constexpr int kGsYb0 = kGsYb1 + 12 * kChunkBytes;          // 12 chunks
-constexpr int kGradTileBytes = kGsYb0 + 12 * kChunkBytes;  // 618,496
-// ReLU masks (forward -> DGRAD and the divergence kernels), per tile: one bit per element of H1..H8 and Hb1..Hb4 (the 64 ReLU columns of Hb3),
-// in the wgmma accumulator's own order (field_mma.cuh: relu_mask_*).  256-column images take 32 B per row, bender
-// images (<= 128 columns) 16 B per row.
-constexpr int kMaskHBytes = kTileM * 32;                   // 4 KB
-constexpr int kMaskBBytes = kTileM * 16;                   // 2 KB
-constexpr int kMkH = 0;                                    // H_l at kMkH + (l-1)*kMaskHBytes, l = 1..8
-constexpr int kMkHb1 = kMkH + 8 * kMaskHBytes;
-constexpr int kMkHb2 = kMkHb1 + kMaskBBytes;
-constexpr int kMkHb3 = kMkHb2 + kMaskBBytes;
-constexpr int kMkHb4 = kMkHb3 + kMaskBBytes;
-constexpr int kMaskTileBytes = kMkHb4 + kMaskBBytes;       // 40,960
-// compact stashes of the divergence regulariser (div.cu): only the bender images, same relative order
-constexpr int kTanTileBytes = kStashTileBytes - kStBin;    // 94,208: [e | t1 s1 | t2 s2 | t3 | t4]
-constexpr int kAdjTileBytes = kGradTileBytes - kGsYb4;     // 90,112: adjoints of the tangent chain
+// Forward steps in streaming order: the ray bender's B0..B4 (offset and rigidity MLPs fused block-diagonally, its own
+// packed block), then NeRF L0..L7 and the head.  The A operand of a step is the image the step before wrote.
+namespace fwd {
+enum Id : int { B0, B1, B2, B3, B4, L0, L1, L2, L3, L4, L5, L6, L7, Head, kCount };
+__host__ __device__ constexpr WImage image(int s) {
+  switch (s) {
+    case B0: return {96, 6};      // rows 0-63 offset L0, 64-95 rigidity L0; K = xyz_hi(3) xyz_lo(3) latent(32) 0(10)
+    case B1: return {96, 12};     // offset L1 (64 x 64) | rigidity L1 (32 x 32)
+    case B2: return {80, 12};     // offset L2 (64 x 64) | rigidity output (row 64, cols 64-95)
+    case B3: return {64, 8};
+    case B4: return {16, 8};      // offsets: rows 0-2, no bias
+    case L0: return {256, 8};     // K = 63 (+1 zero pad column)
+    case L5: return {256, 40};    // skip connection: K = embedding (64) + 256
+    case Head: return {16, 32};   // N = out_ch (<= 16, zero padded)
+    default: return {256, 32};    // L1-L4, L6, L7
+  }
+}
+}  // namespace fwd
 
-// ------------------------------------------------------------------------------------------
-// Transposed weight images for DGRAD (dX = dY . W: B operand = W^T, rows = input features,
-// K = output features), fp16, in the order field_bwd.cu streams them (pack.cu):
-//   head^T [2 chunks][256][8] | L7^T L6^T [32][256][8] | L5e^T [32][64][8] | L5h^T L4^T..L1^T | L0^T [32][64][8]
-//   bender: B4^T [2][64][8] | B3^T [8][64][8] | B2^T [10][96][8] | B1^T [12][96][8] | B0^T [12][48][8]
-// ------------------------------------------------------------------------------------------
-constexpr int kNerfTHeadBytes = 2 * 256 * 16;
-constexpr int kNerfTEBytes = 32 * 64 * 16;
-constexpr int kNerfTWBytes = kNerfTHeadBytes + 7 * kNerfLBytes + 2 * kNerfTEBytes;
-constexpr int kBendTB4Bytes = 2 * 64 * 16;
-constexpr int kBendTB3Bytes = 8 * 64 * 16;
-constexpr int kBendTB2Bytes = 10 * 96 * 16;
-constexpr int kBendTB1Bytes = 12 * 96 * 16;
-constexpr int kBendTB0Bytes = 12 * 48 * 16;
-constexpr int kBendTWBytes = kBendTB4Bytes + kBendTB3Bytes + kBendTB2Bytes + kBendTB1Bytes + kBendTB0Bytes;
+// DGRAD steps in streaming order; step X^T's image is the transpose of forward step X's (L5 in two parts).
+namespace dgrad {
+enum Id : int { HeadT, L7T, L6T, L5eT, L5hT, L4T, L3T, L2T, L1T, L0T, B4T, B3T, B2T, B1T, B0T, kCount };
+// the forward step whose weights step s applies transposed
+__host__ __device__ constexpr int forward_of(int s) {
+  const int f[kCount] = {fwd::Head, fwd::L7, fwd::L6, fwd::L5, fwd::L5, fwd::L4, fwd::L3, fwd::L2, fwd::L1, fwd::L0,
+                         fwd::B4, fwd::B3, fwd::B2, fwd::B1, fwd::B0};
+  return f[s];
+}
+__host__ __device__ constexpr WImage image(int s) {
+  const WImage w = fwd::image(forward_of(s));
+  const int e = fwd::image(fwd::L0).chunks;   // L5's first chunks multiply the embedding (L5e^T), the rest h (L5h^T)
+  return s == L5eT ? WImage{w.rows, e}.t() : s == L5hT ? WImage{w.rows, w.chunks - e}.t() : w.t();
+}
+}  // namespace dgrad
+
+// Shape of one GEMM step of the field kernels: its weight image goes through the ring in `nslabs` slabs of `slab_bytes`
+// (as many chunks as fit one ring stage), k16 MMAs of K = 16 per slab.
+struct Step { uint32_t N, nslabs, slab_bytes, k16; };
+__host__ __device__ constexpr Step make_step(WImage w) {
+  const int per_slab = w.chunks < kRingStageBytes / (16 * w.rows) ? w.chunks : kRingStageBytes / (16 * w.rows);
+  return {(uint32_t)w.rows, (uint32_t)(w.chunks / per_slab), (uint32_t)(per_slab * w.rows * 16), (uint32_t)(per_slab / 2)};
+}
+__host__ __device__ constexpr bool operator==(Step a, Step b) {
+  return a.N == b.N && a.nslabs == b.nslabs && a.slab_bytes == b.slab_bytes && a.k16 == b.k16;
+}
+// w_off: byte offset of a step's weight image in its module's packed block (bender: B*, NeRF: the rest); b_off: float
+// offset of its bias (one per image row) in the module's biases.
+namespace fwd {
+__host__ __device__ constexpr Step step(int s) { return make_step(image(s)); }
+__host__ __device__ constexpr int w_off(int s) { int o = 0; for (int i = s < L0 ? B0 : L0; i < s; ++i) o += image(i).bytes(); return o; }
+__host__ __device__ constexpr int b_off(int s) { int o = 0; for (int i = s < L0 ? B0 : L0; i < s; ++i) o += image(i).rows; return o; }
+}  // namespace fwd
+namespace dgrad {
+__host__ __device__ constexpr Step step(int s) { return make_step(image(s)); }
+__host__ __device__ constexpr int w_off(int s) { int o = 0; for (int i = s < B4T ? HeadT : B4T; i < s; ++i) o += image(i).bytes(); return o; }
+}  // namespace dgrad
+
+// Packed NeRF weights: forward images L0..head | fp32 biases (one per image row) | transposed images head^T..L0^T
+constexpr int kNerfWBytes = fwd::w_off(fwd::Head) + fwd::image(fwd::Head).bytes();
+constexpr int kNerfBiasFloats = fwd::b_off(fwd::Head) + fwd::image(fwd::Head).rows;
+constexpr int kNerfTOffset = kNerfWBytes + kNerfBiasFloats * 4;
+constexpr int kNerfTWBytes = dgrad::w_off(dgrad::L0T) + dgrad::image(dgrad::L0T).bytes();
 constexpr int kNerfPackedBytes = kNerfTOffset + kNerfTWBytes;
-// Bender residual images for the divergence kernels (div.cu), after the transposed images: for every weight w of the
-// forward and transposed images above, fp16((w - fp16(w)) * kBendLoScale), so that fp16(w) + lo / kBendLoScale carries
-// w to about 22 bits and the tangent / adjoint chains can run at fp32 accuracy on fp16 tensor cores.
+// Packed ray-bender weights: forward images B0..B4 | fp32 biases of B0..B3 | transposed images B4^T..B0^T | residuals
+// for the divergence kernels (div.cu): fp16((w - fp16(w)) * kBendLoScale) of every weight w of those images, so that
+// fp16(w) + lo / kBendLoScale carries w to about 22 bits and the tangent / adjoint chains run at fp32 accuracy on fp16.
+constexpr int kBendWBytes = fwd::w_off(fwd::B4) + fwd::image(fwd::B4).bytes();
+constexpr int kBendBiasFloats = fwd::b_off(fwd::B4);
+constexpr int kBendTOffset = kBendWBytes + kBendBiasFloats * 4;
+constexpr int kBendTWBytes = dgrad::w_off(dgrad::B0T) + dgrad::image(dgrad::B0T).bytes();
 constexpr float kBendLoScale = 2048.f;
 constexpr int kBendLoOffset = kBendTOffset + kBendTWBytes;   // residuals of B0..B4
 constexpr int kBendTLoOffset = kBendLoOffset + kBendWBytes;  // residuals of B4^T..B0^T
 constexpr int kBendPackedBytes = kBendTLoOffset + kBendTWBytes;
+static_assert(kNerfWBytes == 991232 && kNerfTWBytes == 991232 && kBendWBytes == 53248 && kBendTWBytes == 53248, "weight images");
+static_assert(kNerfBiasFloats == 8 * 256 + 16 && kBendBiasFloats == 96 + 96 + 80 + 64, "biases");
+
+// A tile image of the stashes: `chunks` 8-column chunks of 128 rows (fp16, chunk-major) at byte `off` of the tile.
+struct Image {
+  int off, chunks;
+  __host__ __device__ constexpr int end() const { return off + chunks * kChunkBytes; }
+  __host__ __device__ constexpr Image next(int c) const { return {end(), c}; }   // the image behind this one
+};
+constexpr int kHChunks = fwd::image(fwd::L1).chunks;                 // 256-wide hidden activations
+constexpr int kHBytes = kHChunks * kChunkBytes;                         // 64 KB
+constexpr int kEBytes = fwd::image(fwd::L0).chunks * kChunkBytes;   // 64-wide positional embedding, 16 KB
+constexpr int kSlotBytes = kHBytes + kEBytes;
+
+// Training stash (forward -> DGRAD, WGRAD), per tile: every image is the A operand of the forward step it feeds.
+//   E: positional encoding of the bent point; the pad column 63 holds 1.0, so that the WGRAD of L0 / L5 yields the bias
+//   gradient in that column.  H_l: post-ReLU activations (l = 1..8).  Bin: bender input.  Hb1..Hb4: bender hidden.
+constexpr Image kStE{0, fwd::image(fwd::L0).chunks};
+constexpr int kStH = kStE.end();                           // H_l at kStH + (l - 1) * kHBytes
+__host__ __device__ constexpr Image st_h(int l) { return {kStH + (l - 1) * kHBytes, kHChunks}; }
+constexpr Image kStBin{kStH + 8 * kHBytes, fwd::image(fwd::B0).chunks};
+constexpr Image kStHb1 = kStBin.next(fwd::image(fwd::B1).chunks);
+constexpr Image kStHb2 = kStHb1.next(fwd::image(fwd::B2).chunks);
+constexpr Image kStHb3 = kStHb2.next(fwd::image(fwd::B3).chunks);
+constexpr Image kStHb4 = kStHb3.next(fwd::image(fwd::B4).chunks);
+constexpr int kStashTileBytes = kStHb4.end();
+// Gradient stash (DGRAD -> WGRAD), per tile: every image is the A operand of the DGRAD step it feeds.  d_raw, dY_l
+// (pre-activation gradient of L_l), dYb4 (d unmasked offsets) .. dYb0; dYb2 = [64 offset | rigidity pre-activation | pad].
+constexpr Image kGsRaw{0, dgrad::image(dgrad::HeadT).chunks};
+constexpr int kGsY = kGsRaw.end();                         // dY_l at kGsY + l * kHBytes, kHChunks each
+constexpr Image kGsYb4{kGsY + 8 * kHBytes, dgrad::image(dgrad::B4T).chunks};
+constexpr Image kGsYb3 = kGsYb4.next(dgrad::image(dgrad::B3T).chunks);
+constexpr Image kGsYb2 = kGsYb3.next(dgrad::image(dgrad::B2T).chunks);
+constexpr Image kGsYb1 = kGsYb2.next(dgrad::image(dgrad::B1T).chunks);
+constexpr Image kGsYb0 = kGsYb1.next(dgrad::image(dgrad::B0T).chunks);
+constexpr int kGradTileBytes = kGsYb0.end();
+// Compact stashes of the divergence regulariser (div.cu): only the bender images, in the same order.  Tangent stash
+// [e | t1 s1 | t2 s2 | t3 | t4] = the forward stash from kStBin on; adjoint stash = the gradient stash from kGsYb4 on.
+constexpr int kTanTileBytes = kStashTileBytes - kStBin.off;
+constexpr int kAdjTileBytes = kGradTileBytes - kGsYb4.off;
+__host__ __device__ constexpr Image tan_image(Image st) { return {st.off - kStBin.off, st.chunks}; }
+__host__ __device__ constexpr Image adj_image(Image gs) { return {gs.off - kGsYb4.off, gs.chunks}; }
+
+// ReLU masks (forward -> DGRAD and the divergence kernels), per tile: one bit per element of H1..H8 and Hb1..Hb4, in the
+// wgmma accumulator's order (field_mma.cuh: ReluMask); images of more than 128 columns take 32 B per row, others 16 B.
+struct MaskImage {
+  int off, cols;
+  __host__ __device__ constexpr int end() const { return off + kTileM * (cols > 128 ? 32 : 16); }
+  __host__ __device__ constexpr MaskImage next(int c) const { return {end(), c}; }
+};
+constexpr int kMaskHCols = 8 * kHChunks;
+constexpr int kMaskHBytes = MaskImage{0, kMaskHCols}.end();  // 4 KB
+constexpr int kMkH = 0;                                      // H_l at kMkH + (l - 1) * kMaskHBytes
+constexpr MaskImage kMkHb1 = MaskImage{kMkH + 7 * kMaskHBytes, kMaskHCols}.next(8 * kStHb1.chunks);
+constexpr MaskImage kMkHb2 = kMkHb1.next(8 * kStHb2.chunks);
+constexpr MaskImage kMkHb3 = kMkHb2.next(8 * kStHb3.chunks);
+constexpr MaskImage kMkHb4 = kMkHb3.next(8 * kStHb4.chunks);
+constexpr int kMaskTileBytes = kMkHb4.end();
+static_assert(kStashTileBytes == 634880 && kGradTileBytes == 618496 && kMaskTileBytes == 40960, "stash tiles");
+static_assert(kTanTileBytes == 94208 && kAdjTileBytes == 90112, "divergence stash tiles");
+
+// Flat gradient buffers, in the reference's parameter order and shapes ([out][in] weights, then the bias):
+//   NeRF   : W0[256][63] b0 W1[256][256] b1 ... W5[256][63 + 256] b5 ... W7 b7 Wout[out_ch][256] bout
+//   bender : net_w0[64][35] net_b0 net_w1 net_b1 net_w2 net_b2 net_w3 net_b3 net_w4[3][64]
+//            rig_w0[32][3] rig_b0 rig_w1[32][32] rig_b1 rig_w2[1][32] rig_b2
+constexpr int kPeCols = 63;   // positional encoding of xyz, 10 octaves
+__host__ __device__ constexpr int nerf_in(int l) { return l == 0 ? kPeCols : l == 5 ? kPeCols + 256 : 256; }
+__host__ __device__ constexpr int nerf_grad_floats(int out_ch) { int n = out_ch * 257; for (int l = 0; l < 8; ++l) n += 256 * (nerf_in(l) + 1); return n; }
+namespace bparam {
+enum Id : int { NetW0, NetB0, NetW1, NetB1, NetW2, NetB2, NetW3, NetB3, NetW4, RigW0, RigB0, RigW1, RigB1, RigW2, RigB2, kCount };
+constexpr int kShape[kCount][2] = {{64, 3 + kLatent}, {64, 1}, {64, 64}, {64, 1}, {64, 64}, {64, 1}, {64, 64}, {64, 1}, {3, 64},
+                                   {32, 3}, {32, 1}, {32, 32}, {32, 1}, {1, 32}, {1, 1}};   // [rows, cols]
+__host__ __device__ constexpr int floats(int i) { return kShape[i][0] * kShape[i][1]; }
+__host__ __device__ constexpr int total() { int n = 0; for (int i = 0; i < kCount; ++i) n += floats(i); return n; }
+}  // namespace bparam
+static_assert(nerf_grad_floats(4) == 494084 && nerf_grad_floats(5) == 494341 && bparam::total() == 16193, "gradient buffers");
 
 struct FieldBwdParams {
   long long P;

@@ -278,4 +278,66 @@ __device__ __forceinline__ uint32_t pack_bf2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
+// ---- helpers shared by the tensor-core kernels ----
+constexpr long long kWaitLimitCycles = 1ll << 28;  // ~0.15 s: protocol bug => error flag, not a hang
+
+// Bounded mbarrier wait: past kWaitLimitCycles it raises the CTA's abort flag (every waiter of the CTA stops) and the device
+// error word.  paired (WGRAD's 2-CTA clusters): the abort also reaches the partner CTA's flag at shared::cluster address
+// partner_abort.
+struct Waiter {
+  int* s_abort;
+  int* g_err;
+  bool paired = false;
+  uint32_t partner_abort = 0;
+  __device__ __forceinline__ bool wait(uint64_t* bar, uint32_t parity, int code) const {
+    if (mbar_try_wait(bar, parity)) return true;
+    const long long t0 = clock64();
+    while (!mbar_try_wait(bar, parity)) {
+      if (*reinterpret_cast<volatile int*>(s_abort)) return false;
+      if (clock64() - t0 > kWaitLimitCycles) {
+        atomicExch(s_abort, code);
+        if (paired) st_shared_cluster(partner_abort, code);   // the partner stops waiting for this CTA's releases
+        atomicCAS(g_err, 0, code);
+        return false;
+      }
+    }
+    return true;
+  }
+};
+
+// One halving step of warp_transpose_reduce on the first N entries (a compile-time N keeps every index static, so v
+// stays in registers).
+template <int N>
+__device__ __forceinline__ void transpose_reduce_step(float (&v)[32], int lane) {
+  if constexpr (N > 1) {
+    constexpr int off = N / 2;
+    const bool upper = (lane & off) != 0;
+#pragma unroll
+    for (int i = 0; i < off; ++i) {
+      const float lo = v[i], hi = v[i + off];
+      v[i] = (upper ? hi : lo) + __shfl_xor_sync(0xffffffffu, upper ? lo : hi, off);
+    }
+    transpose_reduce_step<off>(v, lane);
+  }
+}
+
+// Sum over the warp's 32 lanes of v[j] for each j; lane L returns the total of column L.
+__device__ __forceinline__ float warp_transpose_reduce(float (&v)[32], int lane) {
+  transpose_reduce_step<32>(v, lane);
+  return v[0];
+}
+
+// Power-of-two loss scale of the backward chains from the device scalar *amax (max |upstream gradient|; null: 1), so that
+// max * scale lands in [512, 1024).  Gradients travel in fp16 times this scale; WGRAD divides it out in fp32.
+__device__ __forceinline__ float loss_scale(const float* amax_ptr) {
+  float scale = 1.0f;
+  const float amax = amax_ptr ? __ldg(amax_ptr) : 0.f;
+  if (amax > 0.f && amax < 3.0e38f) {
+    int e;
+    frexpf(amax, &e);                                   // amax = m * 2^e, m in [0.5, 1)
+    scale = ldexpf(1.0f, min(max(10 - e, -60), 60));
+  }
+  return scale;
+}
+
 }  // namespace nrn

@@ -34,7 +34,6 @@ namespace nrn {
 
 namespace {
 
-constexpr long long kWaitLimitCycles = 1ll << 28;
 constexpr int kRingBytes = 96 * kChunkBytes;       // operand ring: 96 chunk images (128 points x 8 features each)
 constexpr int kMaxStages = 4;
 constexpr uint32_t kPieceBytes = 16384;            // size of one bulk copy
@@ -58,14 +57,20 @@ struct Job {
 // of a NeRF layer's dW; g: the calling consumer warpgroup (0 or 1; the producer passes 0).  Built per warpgroup so that
 // the units are selected by branches, not by a runtime array index, and the Job stays in registers.
 // Scratch partial layout: NeRF jobs [256 rows][256]; bender jobs [sub][128 rows][128].
+// The bender jobs read adjacent images of both stashes: A = dYb4 dYb3 dYb2 (job 10), dYb1 dYb0 (job 11); B = Hb2 Hb3
+// Hb4 (job 10), bender input and Hb1 (job 11).
+__host__ __device__ constexpr Image span(Image first, Image last) { return {first.off, (last.end() - first.off) / kChunkBytes}; }
+__host__ __device__ constexpr int chunk_in(Image im, Image first) { return (im.off - first.off) / kChunkBytes; }
+constexpr Image kJ10A = span(kGsYb4, kGsYb2), kJ10B = span(kStHb2, kStHb4), kJ11A = span(kGsYb1, kGsYb0), kJ11B = span(kStBin, kStHb1);
+
 __device__ __forceinline__ Job job_desc(int j, int half, int g, int compact) {
   Job jb{};
   if (j <= 9) {
     int a_off, a_cols, b_off, b_cols, bias = 1;
-    if (j == 0) { a_off = kGsRaw; a_cols = 16; b_off = kStH + 7 * kHBytes; b_cols = 256; }
-    else if (j == 8) { a_off = kGsY + 5 * kHBytes; a_cols = 256; b_off = kStE; b_cols = 64; bias = 0; }
-    else if (j == 9) { a_off = kGsY; a_cols = 256; b_off = kStE; b_cols = 64; }
-    else { a_off = kGsY + j * kHBytes; a_cols = 256; b_off = kStH + (j - 1) * kHBytes; b_cols = 256; }
+    if (j == 0) { a_off = kGsRaw.off; a_cols = 8 * kGsRaw.chunks; b_off = kStH + 7 * kHBytes; b_cols = 8 * kHChunks; }
+    else if (j == 8) { a_off = kGsY + 5 * kHBytes; a_cols = 8 * kHChunks; b_off = kStE.off; b_cols = 8 * kStE.chunks; bias = 0; }
+    else if (j == 9) { a_off = kGsY; a_cols = 8 * kHChunks; b_off = kStE.off; b_cols = 8 * kStE.chunks; }
+    else { a_off = kGsY + j * kHBytes; a_cols = 8 * kHChunks; b_off = kStH + (j - 1) * kHBytes; b_cols = 8 * kHChunks; }
     jb.a_off = a_off + half * 16 * kChunkBytes; jb.a_chunks = min(a_cols / 8 - 16 * half, 16);
     jb.b_off = b_off; jb.b_chunks = b_cols / 8;
     jb.bias = bias; jb.bias_off = half * 128;
@@ -73,30 +78,27 @@ __device__ __forceinline__ Job job_desc(int j, int half, int g, int compact) {
     jb.u[0] = {8 * g, 0, m0 * 256, 256, max(min(a_cols - m0, 64), 0)};
     return jb;
   }
-  // bender jobs: the images of a job are adjacent in both stashes (nrn_common.cuh); in compact mode the stashes hold
-  // only the bender images
-  const int ga = compact ? kGsYb4 : 0, sa = compact ? kStBin : 0;
+  // in compact mode the stashes hold only the bender images
+  const int ga = compact ? kGsYb4.off : 0, sa = compact ? kStBin.off : 0;
   if (j == 10) {
-    // A: Yb4 (2 chunks) Yb3 (8) Yb2 (10)      B: Hb2 (12) Hb3 (8) Hb4 (8)
-    jb.a_off = kGsYb4 - ga; jb.a_chunks = 20;
-    jb.b_off = kStHb2 - sa; jb.b_chunks = 28;
+    jb.a_off = kJ10A.off - ga; jb.a_chunks = kJ10A.chunks;
+    jb.b_off = kJ10B.off - sa; jb.b_chunks = kJ10B.chunks;
     if (g == 0) {
-      jb.u[0] = {0, 20, 0, 128, 16};                  // dYb4 x Hb4      (N = 64)
-      jb.u[1] = {2, 12, 16384, 128, 64};              // dYb3 x Hb3      (N = 64)
+      jb.u[0] = {chunk_in(kGsYb4, kJ10A), chunk_in(kStHb4, kJ10B), 0, 128, 8 * kGsYb4.chunks};           // dYb4 x Hb4
+      jb.u[1] = {chunk_in(kGsYb3, kJ10A), chunk_in(kStHb3, kJ10B), 16384, 128, 8 * kGsYb3.chunks};       // dYb3 x Hb3
     } else {
-      jb.u[0] = {10, 0, 2 * 16384, 128, 64};          // dYb2 x Hb2      (N = 96), rows 0-63
-      jb.u[1] = {18, 0, 2 * 16384 + 64 * 128, 128, 16};  //               rows 64-79
+      jb.u[0] = {chunk_in(kGsYb2, kJ10A), chunk_in(kStHb2, kJ10B), 2 * 16384, 128, 64};                  // dYb2 x Hb2, rows 0-63
+      jb.u[1] = {chunk_in(kGsYb2, kJ10A) + 8, chunk_in(kStHb2, kJ10B), 2 * 16384 + 64 * 128, 128, 8 * kGsYb2.chunks - 64};  // rows 64-
     }
   } else {
-    // A: Yb1 (12) Yb0 (12)                    B: bender input (6) Hb1 (12)
-    jb.a_off = kGsYb1 - ga; jb.a_chunks = 24;
-    jb.b_off = kStBin - sa; jb.b_chunks = 18;
+    jb.a_off = kJ11A.off - ga; jb.a_chunks = kJ11A.chunks;
+    jb.b_off = kJ11B.off - sa; jb.b_chunks = kJ11B.chunks;
     if (g == 0) {
-      jb.u[0] = {0, 6, 0, 128, 64};                   // dYb1 x Hb1      (N = 96), rows 0-63
-      jb.u[1] = {8, 6, 64 * 128, 128, 32};            //                 rows 64-95
+      jb.u[0] = {chunk_in(kGsYb1, kJ11A), chunk_in(kStHb1, kJ11B), 0, 128, 64};                          // dYb1 x Hb1, rows 0-63
+      jb.u[1] = {chunk_in(kGsYb1, kJ11A) + 8, chunk_in(kStHb1, kJ11B), 64 * 128, 128, 8 * kGsYb1.chunks - 64};  // rows 64-
     } else {
-      jb.u[0] = {12, 0, 16384, 128, 64};              // dYb0 x input    (N = 48), rows 0-63
-      jb.u[1] = {20, 0, 16384 + 64 * 128, 128, 32};   //                 rows 64-95
+      jb.u[0] = {chunk_in(kGsYb0, kJ11A), chunk_in(kStBin, kJ11B), 16384, 128, 64};                      // dYb0 x input, rows 0-63
+      jb.u[1] = {chunk_in(kGsYb0, kJ11A) + 8, chunk_in(kStBin, kJ11B), 16384 + 64 * 128, 128, 8 * kGsYb0.chunks - 64};  // rows 64-
     }
   }
   jb.bias = compact ? 0 : 1;   // the tangent chain of the divergence term has no bias
@@ -109,27 +111,6 @@ struct Shared {
   int abort_flag;
 };
 
-struct Waiter {
-  int* s_abort;
-  int* g_err;
-  bool paired;
-  uint32_t partner_abort;   // shared::cluster address of the partner CTA's abort_flag (paired CTAs)
-  __device__ __forceinline__ bool wait(uint64_t* bar, uint32_t parity, int code) const {
-    if (mbar_try_wait(bar, parity)) return true;
-    const long long t0 = clock64();
-    while (!mbar_try_wait(bar, parity)) {
-      if (*reinterpret_cast<volatile int*>(s_abort)) return false;
-      if (clock64() - t0 > kWaitLimitCycles) {
-        atomicExch(s_abort, code);
-        if (paired) st_shared_cluster(partner_abort, code);   // the partner stops waiting for this CTA's releases
-        atomicCAS(g_err, 0, code);
-        return false;
-      }
-    }
-    return true;
-  }
-};
-
 // Operand ring: stage s holds one tile's A block at smem + s * stage_bytes and its B block right behind it.
 struct Ring {
   uint8_t* smem;
@@ -137,28 +118,6 @@ struct Ring {
   bool paired;
   uint32_t partner_empty;   // shared::cluster address of the partner CTA's empty[0] (paired CTAs)
 };
-
-// One halving step of warp_transpose_reduce on the first N entries (a compile-time N keeps every index static, so v
-// stays in registers).
-template <int N>
-__device__ __forceinline__ void transpose_reduce_step(float (&v)[32], int lane) {
-  if constexpr (N > 1) {
-    constexpr int off = N / 2;
-    const bool upper = (lane & off) != 0;
-#pragma unroll
-    for (int i = 0; i < off; ++i) {
-      const float lo = v[i], hi = v[i + off];
-      v[i] = (upper ? hi : lo) + __shfl_xor_sync(0xffffffffu, upper ? lo : hi, off);
-    }
-    transpose_reduce_step<off>(v, lane);
-  }
-}
-
-// Sum over the warp's 32 lanes of v[j] for each j; lane L returns the total of column L.
-__device__ __forceinline__ float warp_transpose_reduce(float (&v)[32], int lane) {
-  transpose_reduce_step<32>(v, lane);
-  return v[0];
-}
 
 // which (job, split, half) does this CTA own, and which scratch partial is the split's?  job_ids[] / splits[] /
 // halves[] come from the host (WgradParams); the halves of one split are the two CTAs of one cluster.
@@ -343,19 +302,20 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradParams 
     const Unit& u1 = jb.u[1];
     if (job_id <= 9) {
       const bool mine = u0.rows > 0;
+      // N = columns of the job's activation image
       if (job_id == 8 || job_id == 9) {
-        if (mine) consume<64, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
+        if (mine) consume<8 * kStE.chunks, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
         else consume<0, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
       } else {
-        if (mine) consume<256, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
+        if (mine) consume<8 * kHChunks, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
         else consume<0, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
       }
     } else if (job_id == 10) {
-      if (g == 0) consume<64, 64>(jb, u0, u1, R, sh, W, n_local, part, have);
-      else consume<96, 96>(jb, u0, u1, R, sh, W, n_local, part, have);
+      if (g == 0) consume<8 * kStHb4.chunks, 8 * kStHb3.chunks>(jb, u0, u1, R, sh, W, n_local, part, have);
+      else consume<8 * kStHb2.chunks, 8 * kStHb2.chunks>(jb, u0, u1, R, sh, W, n_local, part, have);
     } else {
-      if (g == 0) consume<96, 96>(jb, u0, u1, R, sh, W, n_local, part, have);
-      else consume<48, 48>(jb, u0, u1, R, sh, W, n_local, part, have);
+      if (g == 0) consume<8 * kStHb1.chunks, 8 * kStHb1.chunks>(jb, u0, u1, R, sh, W, n_local, part, have);
+      else consume<8 * kStBin.chunks, 8 * kStBin.chunks>(jb, u0, u1, R, sh, W, n_local, part, have);
     }
   }
   // No CTA leaves while its partner may still arrive on its barriers or write its abort flag.  Multicast data has
@@ -367,10 +327,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradParams 
 
 // ------------------------------------------------------------------------------------------------
 // Deterministic reduction of the split partials into the reference's parameter layout.
-// One thread per destination element of the flat gradient buffers:
-//   NeRF   : W0[256x63] b0 W1 b1 ... W7 b7 Wout[out_ch x 256] bout
-//   bender : net_w0[64x35] net_b0 net_w1 net_b1 net_w2 net_b2 net_w3 net_b3 net_w4[3x64]
-//            rig_w0[32x3] rig_b0 rig_w1[32x32] rig_b1 rig_w2[1x32] rig_b2
+// One thread per destination element of the flat gradient buffers (their shapes: nrn_common.cuh).
 // ------------------------------------------------------------------------------------------------
 namespace {
 
@@ -389,21 +346,22 @@ __device__ __forceinline__ Src bend_w(int job, int sub, int m, int n, int n2 = -
 
 __device__ __forceinline__ Src nerf_src(int idx, int out_ch, bool& ok) {
   ok = true;
-  const int sz0 = 256 * 63 + 256, szl = 256 * 256 + 256, sz5 = 256 * 319 + 256;
+  constexpr int in0 = nerf_in(0), in5 = nerf_in(5);   // L0: the embedding; L5: [embedding | h]
+  const int sz0 = 256 * in0 + 256, szl = 256 * 256 + 256, sz5 = 256 * in5 + 256;
   if (idx < sz0) {
-    if (idx < 256 * 63) return nerf_w(9, idx / 63, idx % 63);
-    return nerf_b(9, idx - 256 * 63);
+    if (idx < 256 * in0) return nerf_w(9, idx / in0, idx % in0);
+    return nerf_b(9, idx - 256 * in0);
   }
   idx -= sz0;
   for (int l = 1; l < 8; ++l) {
     const int sz = l == 5 ? sz5 : szl;
     if (idx < sz) {
       if (l == 5) {
-        if (idx < 256 * 319) {
-          const int m = idx / 319, k = idx % 319;
-          return k < 63 ? nerf_w(8, m, k) : nerf_w(5, m, k - 63);
+        if (idx < 256 * in5) {
+          const int m = idx / in5, k = idx % in5;
+          return k < in0 ? nerf_w(8, m, k) : nerf_w(5, m, k - in0);
         }
-        return nerf_b(5, idx - 256 * 319);
+        return nerf_b(5, idx - 256 * in5);
       }
       if (idx < 65536) return nerf_w(l, idx >> 8, idx & 255);
       return nerf_b(l, idx - 65536);
@@ -420,42 +378,47 @@ __device__ __forceinline__ Src nerf_src(int idx, int out_ch, bool& ok) {
   return nerf_b(0, idx);
 }
 
-// A-chunk layout of the bender jobs (bias index = column inside the concatenated A images):
-//   job 10: Yb4 cols 0-15 | Yb3 cols 16-79 | Yb2 cols 80-159      job 11: Yb1 cols 0-95 | Yb0 cols 96-191
+// Bias index of the bender jobs = column inside the job's concatenated A images: job 10 dYb4 | dYb3 | dYb2, job 11
+// dYb1 | dYb0 (rigidity columns from 64 on).  Sub-MMAs: job 10 0 = B4, 1 = B3, 2 = B2; job 11 0 = B1, 1 = B0.
 __device__ __forceinline__ Src bender_src(int idx, bool& ok) {
+  using namespace bparam;
+  constexpr int c_yb3 = 8 * chunk_in(kGsYb3, kJ10A), c_yb2 = 8 * chunk_in(kGsYb2, kJ10A), c_yb1 = 8 * chunk_in(kGsYb1, kJ11A),
+                c_yb0 = 8 * chunk_in(kGsYb0, kJ11A);
+  constexpr int n_w0 = floats(NetW0), n_b = floats(NetB0), n_w = floats(NetW1), n_w4 = floats(NetW4), n_rw0 = floats(RigW0),
+                n_rb = floats(RigB0), n_rw1 = floats(RigW1), n_rw2 = floats(RigW2), k0 = kShape[NetW0][1];
   ok = true;
-  if (idx < 64 * 35) {  // net_w0: xyz columns collect the hi and lo operand columns
-    const int m = idx / 35, k = idx % 35;
+  if (idx < n_w0) {  // net_w0: xyz columns collect the hi and lo operand columns
+    const int m = idx / k0, k = idx % k0;
     return k < 3 ? bend_w(11, 1, m, k, k + 3) : bend_w(11, 1, m, 6 + (k - 3));
   }
-  idx -= 64 * 35;
-  if (idx < 64) return {11, 96 + idx, -1, 1};                                    // net_b0
-  idx -= 64;
-  if (idx < 4096) return bend_w(11, 0, idx >> 6, idx & 63);                      // net_w1
-  idx -= 4096;
-  if (idx < 64) return {11, idx, -1, 1};                                         // net_b1
-  idx -= 64;
-  if (idx < 4096) return bend_w(10, 2, idx >> 6, idx & 63);                      // net_w2
-  idx -= 4096;
-  if (idx < 64) return {10, 80 + idx, -1, 1};                                    // net_b2
-  idx -= 64;
-  if (idx < 4096) return bend_w(10, 1, idx >> 6, idx & 63);                      // net_w3
-  idx -= 4096;
-  if (idx < 64) return {10, 16 + idx, -1, 1};                                    // net_b3
-  idx -= 64;
-  if (idx < 192) return bend_w(10, 0, idx >> 6, idx & 63);                       // net_w4
-  idx -= 192;
-  if (idx < 96) return bend_w(11, 1, 64 + idx / 3, idx % 3, idx % 3 + 3);        // rig_w0
-  idx -= 96;
-  if (idx < 32) return {11, 96 + 64 + idx, -1, 1};                               // rig_b0
-  idx -= 32;
-  if (idx < 1024) return bend_w(11, 0, 64 + (idx >> 5), 64 + (idx & 31));        // rig_w1
-  idx -= 1024;
-  if (idx < 32) return {11, 64 + idx, -1, 1};                                    // rig_b1
-  idx -= 32;
-  if (idx < 32) return bend_w(10, 2, 64, 64 + idx);                              // rig_w2
-  idx -= 32;
-  return {10, 80 + 64, -1, 1};                                                   // rig_b2
+  idx -= n_w0;
+  if (idx < n_b) return {11, c_yb0 + idx, -1, 1};                                 // net_b0
+  idx -= n_b;
+  if (idx < n_w) return bend_w(11, 0, idx >> 6, idx & 63);                        // net_w1
+  idx -= n_w;
+  if (idx < n_b) return {11, c_yb1 + idx, -1, 1};                                 // net_b1
+  idx -= n_b;
+  if (idx < n_w) return bend_w(10, 2, idx >> 6, idx & 63);                        // net_w2
+  idx -= n_w;
+  if (idx < n_b) return {10, c_yb2 + idx, -1, 1};                                 // net_b2
+  idx -= n_b;
+  if (idx < n_w) return bend_w(10, 1, idx >> 6, idx & 63);                        // net_w3
+  idx -= n_w;
+  if (idx < n_b) return {10, c_yb3 + idx, -1, 1};                                 // net_b3
+  idx -= n_b;
+  if (idx < n_w4) return bend_w(10, 0, idx >> 6, idx & 63);                       // net_w4
+  idx -= n_w4;
+  if (idx < n_rw0) return bend_w(11, 1, 64 + idx / 3, idx % 3, idx % 3 + 3);      // rig_w0
+  idx -= n_rw0;
+  if (idx < n_rb) return {11, c_yb0 + 64 + idx, -1, 1};                           // rig_b0
+  idx -= n_rb;
+  if (idx < n_rw1) return bend_w(11, 0, 64 + (idx >> 5), 64 + (idx & 31));        // rig_w1
+  idx -= n_rw1;
+  if (idx < n_rb) return {11, c_yb1 + 64 + idx, -1, 1};                           // rig_b1
+  idx -= n_rb;
+  if (idx < n_rw2) return bend_w(10, 2, 64, 64 + idx);                            // rig_w2
+  idx -= n_rw2;
+  return {10, c_yb2 + 64, -1, 1};                                                 // rig_b2
 }
 
 }  // namespace
@@ -466,15 +429,7 @@ __global__ void wgrad_reduce_kernel(const WgradParams p, const WgradDst dst, int
   if (idx >= nerf_n + bend_n) return;
   bool ok;
   const Src s = idx < nerf_n ? nerf_src(idx, out_ch, ok) : bender_src(idx - nerf_n, ok);
-  float scale = 1.0f;
-  {
-    const float amax = p.amax ? __ldg(p.amax) : 0.f;
-    if (amax > 0.f && amax < 3.0e38f) {
-      int e;
-      frexpf(amax, &e);
-      scale = ldexpf(1.0f, min(max(10 - e, -60), 60));
-    }
-  }
+  const float scale = loss_scale(p.amax);
   float sum = 0.f;
   if (ok && !(s.bias && p.compact)) {
     int base = 0, slot = -1;
