@@ -23,6 +23,10 @@ namespace nrn {
 namespace {
 
 constexpr int kBwdStageLd = 66;   // floats per staged row (64 used)
+constexpr int kBwdRingStages = 4;
+constexpr size_t kBwdSmemBytes = kHBytes + kBwdRingStages * kRingStageBytes + 2 * kWgRows * kBwdStageLd * sizeof(float) +
+                                 sizeof(RingShared<kBwdRingStages>) + 64;
+static_assert(kBwdSmemBytes <= 227 * 1024, "DGRAD kernel: dynamic shared memory per block");
 
 static_assert(dgrad::step(dgrad::L6T) == dgrad::step(dgrad::L7T) && dgrad::step(dgrad::L5hT) == dgrad::step(dgrad::L7T) &&
               dgrad::step(dgrad::L4T) == dgrad::step(dgrad::L7T) && dgrad::step(dgrad::L3T) == dgrad::step(dgrad::L7T) &&
@@ -96,9 +100,9 @@ template <bool HAS_BENDER>
 __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* act = smem;                               // 64 KB gradient operand, 128 rows
-  uint8_t* ring_buf = smem + kHBytes;                // kRingStages x 32 KB
-  float* stage_all = reinterpret_cast<float*>(ring_buf + kRingStages * kRingStageBytes);   // 2 x 64 rows x kBwdStageLd
-  RingShared* sh = reinterpret_cast<RingShared*>(stage_all + 2 * kWgRows * kBwdStageLd);
+  uint8_t* ring_buf = smem + kHBytes;                // kBwdRingStages x 32 KB
+  float* stage_all = reinterpret_cast<float*>(ring_buf + kBwdRingStages * kRingStageBytes);   // 2 x 64 rows x kBwdStageLd
+  auto* sh = reinterpret_cast<RingShared<kBwdRingStages>*>(stage_all + 2 * kWgRows * kBwdStageLd);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -106,7 +110,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
   if (threadIdx.x == 0) sh->init();
   __syncthreads();
   const Waiter W{&sh->abort_flag, p.err};
-  Ring ring{ring_buf, sh->w_full, sh->w_empty};
+  Ring<kBwdRingStages> ring{ring_buf, sh->w_full, sh->w_empty};
 
   if (warp >= 8) {
     setmaxnreg_dec<kProducerRegs>();
@@ -301,8 +305,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
 
 // ------------------------------------------------------------------------------------------------
 cudaError_t launch_field_bwd(const FieldBwdParams& p, bool has_bender, int num_sms, cudaStream_t stream) {
-  const size_t smem = kHBytes + kRingStages * kRingStageBytes + 2 * kWgRows * kBwdStageLd * sizeof(float) + sizeof(RingShared) + 64;
-  return launch_field(has_bender ? field_bwd_kernel<true> : field_bwd_kernel<false>, p, num_sms, smem, stream);
+  return launch_field(has_bender ? field_bwd_kernel<true> : field_bwd_kernel<false>, p, num_sms, kBwdSmemBytes, stream);
 }
 
 }  // namespace nrn

@@ -9,12 +9,14 @@
 // Work decomposition (field_mma.cuh)
 //   tile   = 128 consecutive sample points; CTA = 1 per SM, persistent over tiles
 //   warps  : 0-3 / 4-7 consumer warpgroups (rows 0-63 / 64-127 of the tile), 8 weight producer (bulk TMA ring)
-//   a "step" = one dense layer:  D[64 x N] (registers, fp32) = A[64 x K] (smem, fp16) . W[N x K]^T (smem ring,
+//   a "step" = one dense layer:  D[64 x N] (registers, fp32) = A[64 x K] (fp16) . W[N x K]^T (smem ring,
 //            fp16) with wgmma; the same warpgroup then applies bias/ReLU/(bend + positional encoding) and writes
-//            the next A operand in place.
+//            the next A operand.  B0..B4, L0 and the embedding slab of L5 read A from shared memory; L1..L7 and the
+//            head take it from registers: the fp16 fragments the previous trunk epilogue packed (wg_gemm_rs), which
+//            the training kernel also stores to the stash from registers.
 //   steps  : B0..B4 (ray bender, offset + rigidity MLPs fused block-diagonally), L0..L7, head
 //
-// Shared memory (per CTA): H 64 KB + E 16 KB activations, 4 x 32 KB weight ring, per-row staging, barriers.
+// Shared memory (per CTA): bender H 24 KB + E 16 KB activations, 5 x 32 KB weight ring, per-row staging, barriers.
 #include "field_mma.cuh"
 
 namespace nrn {
@@ -22,6 +24,14 @@ namespace nrn {
 namespace {
 
 constexpr int kFwdStageLd = 12;   // floats per staged row (8 used)
+// Activations in shared memory: the bender's hidden images (A operands of B1..B4, at most 96 columns) and E.  The trunk's
+// 256-wide activations stay in registers (epi_bias_relu_frag), so the rest of shared memory goes to the weight ring.
+constexpr int kFwdHBytes = kStHb1.chunks * kChunkBytes;   // 24 KB
+static_assert(kStHb2.chunks <= kStHb1.chunks && kStHb3.chunks <= kStHb1.chunks && kStHb4.chunks <= kStHb1.chunks, "bender images fit H");
+constexpr int kFwdRingStages = 5;
+constexpr size_t kFwdSmemBytes = kFwdHBytes + kEBytes + kFwdRingStages * kRingStageBytes + 2 * kWgRows * kFwdStageLd * sizeof(float) +
+                                 sizeof(RingShared<kFwdRingStages>) + 64;
+static_assert(kFwdSmemBytes <= 227 * 1024, "forward kernel: dynamic shared memory per block");
 
 static_assert(fwd::step(fwd::L2) == fwd::step(fwd::L1) && fwd::step(fwd::L3) == fwd::step(fwd::L1) &&
               fwd::step(fwd::L4) == fwd::step(fwd::L1) && fwd::step(fwd::L6) == fwd::step(fwd::L1) &&
@@ -40,15 +50,6 @@ __device__ __forceinline__ Step step_at(int step) {
     default: return step_imm<fwd::L1>();   // L1-L4, L6, L7: one shape
   }
 }
-// byte offset (inside the activation region: H at 0, E at kHBytes) of the A operand of slab j
-__device__ __forceinline__ uint32_t a_operand_offset(int step, uint32_t j) {
-  if (step == fwd::B0 || step == fwd::L0) return kHBytes;                          // bender input / embedding live in E
-  constexpr uint32_t kSlabA = 2 * fwd::step(fwd::L1).k16 * kChunkBytes;   // A operand bytes of one slab of the hidden layers
-  if (step == fwd::L5) return j == 0 ? kHBytes : (j - 1) * kSlabA;      // skip: [embedding | h]
-  if (step < fwd::L0 || step == fwd::Head) return 0;
-  return j * kSlabA;
-}
-
 // Accumulator columns [0, NCOLS) + bias, ReLU, fp16 -> this warpgroup's rows of the chunk-major image `img`.  MASK
 // (training kernel): also the ReLU mask bits of those elements -> this thread's words of the tile's mask image at
 // byte `mask_off` of `mask_tile`.
@@ -70,6 +71,32 @@ __device__ __forceinline__ void epi_bias_relu_store(const float (&acc)[NR], cons
     }
   }
   if constexpr (MASK) m.store(mask_tile + mask_off, g);
+}
+
+// The same for a 256-wide trunk layer whose output stays in registers: bias, ReLU, fp16 -> the next step's A fragments
+// `a`.  TRAIN: also the mask bits, and the fp16 pairs straight to this warpgroup's rows of the tile's stash image `st_img`
+// (a warp's 32 words of one column group and row half are one contiguous 128-byte line of the chunk-major image).
+template <bool TRAIN>
+__device__ __forceinline__ void epi_bias_relu_frag(const float (&acc)[kMaskHCols / 2], const float* __restrict__ bias,
+                                                   uint32_t (&a)[kMaskHCols / 16][4], uint8_t* st_img, int g,
+                                                   uint8_t* mask_tile, int mask_off) {
+  const int r0 = g * kWgRows + acc_r0(), q = acc_q();
+  ReluMask<kMaskHCols> m;
+  if constexpr (TRAIN) m.clear();
+#pragma unroll
+  for (int j = 0; j < kMaskHCols / 8; ++j) {
+    const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * q));
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const uint32_t h2 = pack_h2_relu_sat(acc[4 * j + 2 * i] + b.x, acc[4 * j + 2 * i + 1] + b.y);
+      frag_pair(a, j, i) = h2;
+      if constexpr (TRAIN) {
+        m.pack(i, j, h2);
+        *reinterpret_cast<uint32_t*>(st_img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = h2;
+      }
+    }
+  }
+  if constexpr (TRAIN) m.store(mask_tile + mask_off, g);
 }
 
 // Positional encoding of one point (Embedder.embed, run_nerf_helpers.py:149-150 with the settings of
@@ -114,10 +141,10 @@ __device__ __forceinline__ void write_pe(const float (&x)[3], uint8_t* dst_row) 
 template <bool HAS_BENDER, bool TRAIN>
 __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* act = smem;                                  // H | E, 128 rows
-  uint8_t* ring_buf = smem + kSlotBytes;                // kRingStages x 32 KB
-  float* stage_all = reinterpret_cast<float*>(ring_buf + kRingStages * kRingStageBytes);   // 2 x 64 rows x kFwdStageLd
-  RingShared* sh = reinterpret_cast<RingShared*>(stage_all + 2 * kWgRows * kFwdStageLd);
+  uint8_t* act = smem;                                  // H (bender) | E, 128 rows
+  uint8_t* ring_buf = smem + kFwdHBytes + kEBytes;      // kFwdRingStages x 32 KB
+  float* stage_all = reinterpret_cast<float*>(ring_buf + kFwdRingStages * kRingStageBytes);   // 2 x 64 rows x kFwdStageLd
+  auto* sh = reinterpret_cast<RingShared<kFwdRingStages>*>(stage_all + 2 * kWgRows * kFwdStageLd);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -125,7 +152,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
   if (threadIdx.x == 0) sh->init();
   __syncthreads();
   const Waiter W{&sh->abort_flag, p.err};
-  Ring ring{ring_buf, sh->w_full, sh->w_empty};
+  Ring<kFwdRingStages> ring{ring_buf, sh->w_full, sh->w_empty};
 
   if (warp >= 8) {
     setmaxnreg_dec<kProducerRegs>();
@@ -142,7 +169,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
   const int bar = 1 + g;
   const bool wg_leader = tw == 0;
   uint8_t* Hs = act;
-  uint8_t* Es = act + kHBytes;
+  uint8_t* Es = act + kFwdHBytes;
   uint8_t* e_row = Es + (g * kWgRows + tw) * 16;
   const uint32_t a_h = smem_u32(Hs) + g * kWgRows * 16;
   const uint32_t a_e = smem_u32(Es) + g * kWgRows * 16;
@@ -272,21 +299,19 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
     sw.begin();
     if (row_thread) write_pe(x, e_row);
     sw.ready(kStE, Es);
-    // ---- L0 .. L7 (every one 256 wide) ----
+    // ---- L0 .. L7 (every one 256 wide): L0 reads E, every later step its A fragments h (L5: E first, then h) ----
+    uint32_t h[kMaskHCols / 16][4];
 #pragma unroll 1
     for (int L = 0; L < 8; ++L) {
-      const int step = fwd::L0 + L;
       Acc<fwd::L1> acc;
-      const Step s = step_at(step);
-      wg_gemm<fwd::step(fwd::L1).N>(acc, ring, s.nslabs, s.k16, [&](uint32_t j) { return a_h + a_operand_offset(step, j); }, W, 310 + L);
-      sw.begin();
-      epi_bias_relu_store<kMaskHCols, TRAIN>(acc, p.nerf_bias + L * fwd::b_off(fwd::L1), Hs, g, mk, kMkH + L * kMaskHBytes);
-      sw.ready(st_h(L + 1), Hs);
+      if (L == 0) wg_gemm_step<fwd::L0>(acc, ring, [&](uint32_t) { return a_e; }, W, 310);
+      else wg_gemm_rs<fwd::step(fwd::L1).N, fwd::step(fwd::L1).k16>(acc, h, ring, L == 5, a_e, W, 310 + L);
+      epi_bias_relu_frag<TRAIN>(acc, p.nerf_bias + L * fwd::b_off(fwd::L1), h, st + st_h(L + 1).off, g, mk, kMkH + L * kMaskHBytes);
     }
     // ---- head: raw = output_linear(h) (run_nerf_helpers.py:306) ----
     {
       Acc<fwd::Head> acc;
-      wg_gemm_step<fwd::Head>(acc, ring, [&](uint32_t) { return a_h; }, W, 320);
+      wg_gemm_rs<fwd::step(fwd::Head).N, fwd::step(fwd::Head).k16>(acc, h, ring, false, 0u, W, 320);
       stage_cols<0, 1>(acc, stg, kFwdStageLd);
       wg_bar(bar);
       if (valid) {
@@ -305,9 +330,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
 }
 
 // ------------------------------------------------------------------------------------------------
-size_t field_fwd_smem_bytes() {
-  return kSlotBytes + kRingStages * kRingStageBytes + 2 * kWgRows * kFwdStageLd * sizeof(float) + sizeof(RingShared) + 64;
-}
+size_t field_fwd_smem_bytes() { return kFwdSmemBytes; }
 
 cudaError_t launch_field_fwd(const FieldFwdParams& p, bool has_bender, int num_sms, cudaStream_t stream) {
   const size_t smem = field_fwd_smem_bytes();

@@ -15,13 +15,15 @@ namespace {
 
 constexpr int kWgRows = kTileM / 2;                 // rows of a tile owned by one consumer warpgroup
 
-// Weight ring barriers; one thread initialises them before the CTA's first barrier
+// Weight ring of S stages of kRingStageBytes (a per-kernel depth: what the kernel's activation images leave of shared
+// memory).  Barriers; one thread initialises them before the CTA's first barrier.
+template <int S>
 struct RingShared {
-  uint64_t w_full[kRingStages];
-  uint64_t w_empty[kRingStages];
+  uint64_t w_full[S];
+  uint64_t w_empty[S];
   int abort_flag;
   __device__ __forceinline__ void init() {
-    for (int i = 0; i < kRingStages; ++i) {
+    for (int i = 0; i < S; ++i) {
       mbar_init(&w_full[i], 1);
       mbar_init(&w_empty[i], 8);
     }
@@ -30,18 +32,20 @@ struct RingShared {
   }
 };
 
+template <int S>
 struct Ring {
-  uint8_t* buf;      // kRingStages x kRingStageBytes
+  uint8_t* buf;      // S x kRingStageBytes
   uint64_t* full;    // TMA bytes landed (count 1 + tx)
   uint64_t* empty;   // slab consumed: one arrival per consumer warp (count 8)
   uint32_t stage = 0, phase = 0;
   __device__ __forceinline__ void next() {
-    if (++stage == kRingStages) { stage = 0; phase ^= 1u; }
+    if (++stage == S) { stage = 0; phase ^= 1u; }
   }
 };
 
 // producer (one thread): one weight slab global -> ring
-__device__ __forceinline__ void ring_put(Ring& r, const uint8_t* src, uint32_t bytes, const Waiter& W) {
+template <int S>
+__device__ __forceinline__ void ring_put(Ring<S>& r, const uint8_t* src, uint32_t bytes, const Waiter& W) {
   W.wait(&r.empty[r.stage], r.phase ^ 1u, 101);
   uint8_t* dst = r.buf + r.stage * kRingStageBytes;
   mbar_arrive_expect_tx(&r.full[r.stage], bytes);
@@ -51,9 +55,9 @@ __device__ __forceinline__ void ring_put(Ring& r, const uint8_t* src, uint32_t b
 
 // Producer thread: for every tile of this CTA, the weight images of steps [first, last) through the ring (shapes from
 // step_at(step)), those of steps before `split` from `w_lo`, the others from `w_hi`.
-template <typename StepAt>
+template <typename StepAt, int S>
 __device__ __forceinline__ void produce(const uint8_t* w_lo, const uint8_t* w_hi, int n_tiles, int first, int last, int split,
-                                        StepAt step_at, Ring& ring, const Waiter& W) {
+                                        StepAt step_at, Ring<S>& ring, const Waiter& W) {
   for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     uint32_t glo = 0, ghi = 0;
 #pragma unroll 1
@@ -69,8 +73,8 @@ __device__ __forceinline__ void produce(const uint8_t* w_lo, const uint8_t* w_hi
 // consumer warpgroup: acc[64 x N] = A . W^T accumulated over `nslabs` weight slabs of the ring (slab j: N rows x 16 k16
 // column chunks of W, K-major).  a_addr(j): shared address of this warpgroup's first row of slab j's A operand, a
 // K-major image with kTileM rows.  The A operand must have been fenced for the async proxy and the warpgroup synced.
-template <int N, typename AAddr>
-__device__ __forceinline__ void wg_gemm(float (&acc)[N / 2], Ring& r, uint32_t nslabs, uint32_t k16, AAddr a_addr,
+template <int N, typename AAddr, int S>
+__device__ __forceinline__ void wg_gemm(float (&acc)[N / 2], Ring<S>& r, uint32_t nslabs, uint32_t k16, AAddr a_addr,
                                         const Waiter& W, int code) {
   const int lane = threadIdx.x & 31;
   uint32_t prev = 0;
@@ -102,12 +106,62 @@ __device__ __forceinline__ void wg_gemm(float (&acc)[N / 2], Ring& r, uint32_t n
   if (lane == 0) mbar_arrive(&r.empty[prev]);
 }
 
+// wg_gemm with the A operand in registers: slab j (K16 MMAs) takes the A fragments K16 j .. K16 j + K16 - 1 of `a`, the
+// fragments of this warpgroup's 64 rows x 16 KF columns (sm90_ptx.cuh: wgmma_rs).  lead: one slab of K16 MMAs with A from
+// shared memory at a_lead (as in wg_gemm) comes first (the embedding columns of the skip layer).
+template <int N, int K16, int KF, int S>
+__device__ __forceinline__ void wg_gemm_rs(float (&acc)[N / 2], uint32_t (&a)[KF][4], Ring<S>& r, bool lead, uint32_t a_lead,
+                                           const Waiter& W, int code) {
+  static_assert(KF % K16 == 0, "whole slabs of A fragments");
+  const int lane = threadIdx.x & 31;
+  uint32_t prev = 0;
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  if (lead) {
+    W.wait(&r.full[r.stage], r.phase, code);
+    const uint64_t adesc = gmma_desc(a_lead, kChunkBytes, 128);
+    const uint64_t bdesc = gmma_desc(smem_u32(r.buf + r.stage * kRingStageBytes), N * 16, 128);
+    acc_fence(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < K16; ++k)
+      wgmma<N, 0, 0>(acc, gmma_desc_advance(adesc, k * 2 * kChunkBytes), gmma_desc_advance(bdesc, k * 2 * N * 16), k ? 1u : 0u);
+    wgmma_commit();
+    prev = r.stage;
+    r.next();
+  }
+#pragma unroll
+  for (int j = 0; j < KF / K16; ++j) {
+    W.wait(&r.full[r.stage], r.phase, code);
+    const uint64_t bdesc = gmma_desc(smem_u32(r.buf + r.stage * kRingStageBytes), N * 16, 128);
+    acc_fence(acc);
+    frag_fence(a);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < K16; ++k)
+      wgmma_rs<N, 0>(acc, a[j * K16 + k], gmma_desc_advance(bdesc, k * 2 * N * 16), (lead || j || k) ? 1u : 0u);
+    wgmma_commit();
+    if (lead || j > 0) {   // the previous slab's MMAs have retired: hand its stage back while this slab's run
+      wgmma_wait<1>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&r.empty[prev]);
+    }
+    prev = r.stage;
+    r.next();
+  }
+  wgmma_wait<0>();
+  acc_fence(acc);
+  frag_fence(a);
+  __syncwarp();
+  if (lane == 0) mbar_arrive(&r.empty[prev]);
+}
+
 // Accumulators and wg_gemm of a step known at compile time (fwd:: or dgrad:: id): N, slabs and k16 from its table entry
 template <auto S>
 using Acc = float[step(S).N / 2];
-template <auto S, typename AAddr>
-__device__ __forceinline__ void wg_gemm_step(Acc<S>& acc, Ring& r, AAddr a_addr, const Waiter& W, int code) {
-  constexpr Step s = step(S);
+template <auto ID, typename AAddr, int S>
+__device__ __forceinline__ void wg_gemm_step(Acc<ID>& acc, Ring<S>& r, AAddr a_addr, const Waiter& W, int code) {
+  constexpr Step s = step(ID);
   wg_gemm<s.N>(acc, r, s.nslabs, s.k16, a_addr, W, code);
 }
 

@@ -13,7 +13,6 @@ namespace nrn {
 constexpr int kTileM = 128;                 // points per tile = 2 warpgroups x wgmma M (64)
 constexpr int kChunkBytes = kTileM * 16;    // one 8-column chunk of a 128-row activation image
 constexpr int kRingStageBytes = 32768;      // one weight slab: 256 rows x 64 K-columns fp16
-constexpr int kRingStages = 4;
 constexpr int kFwdThreads = 384;            // 2 consumer warpgroups (MMA + epilogue), 1 producer warpgroup (one thread streams)
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // setmaxnreg budgets: 128 x (40 + 2 x 232) <= 64K
 constexpr int kLatent = 32;
@@ -112,7 +111,6 @@ struct Image {
 constexpr int kHChunks = fwd::image(fwd::L1).chunks;                 // 256-wide hidden activations
 constexpr int kHBytes = kHChunks * kChunkBytes;                         // 64 KB
 constexpr int kEBytes = fwd::image(fwd::L0).chunks * kChunkBytes;   // 64-wide positional embedding, 16 KB
-constexpr int kSlotBytes = kHBytes + kEBytes;
 
 // Training stash (forward -> DGRAD, WGRAD), per tile: every image is the A operand of the forward step it feeds.
 //   E: positional encoding of the bent point; the pad column 63 holds 1.0, so that the WGRAD of L0 / L5 yields the bias
