@@ -23,8 +23,13 @@ namespace nrn {
 namespace {
 
 constexpr int kBwdStageLd = 66;   // floats per staged row (64 used)
-constexpr int kBwdRingStages = 4;
-constexpr size_t kBwdSmemBytes = kHBytes + kBwdRingStages * kRingStageBytes + 2 * kWgRows * kBwdStageLd * sizeof(float) +
+// Gradient images in shared memory: only the bender chain's (A operands of B4^T..B0^T, at most 96 columns).  The trunk's
+// 256-wide gradients stay in registers (epi_mask_frag), so the rest of shared memory goes to the weight ring.
+constexpr int kBwdActBytes = kGsYb1.chunks * kChunkBytes;   // 24 KB
+static_assert(kGsYb4.chunks <= kGsYb1.chunks && kGsYb3.chunks <= kGsYb1.chunks && kGsYb2.chunks <= kGsYb1.chunks &&
+              kGsYb0.chunks <= kGsYb1.chunks, "bender gradient images fit act");
+constexpr int kBwdRingStages = 5;
+constexpr size_t kBwdSmemBytes = kBwdActBytes + kBwdRingStages * kRingStageBytes + 2 * kWgRows * kBwdStageLd * sizeof(float) +
                                  sizeof(RingShared<kBwdRingStages>) + 64;
 static_assert(kBwdSmemBytes <= 227 * 1024, "DGRAD kernel: dynamic shared memory per block");
 
@@ -68,6 +73,23 @@ __device__ __forceinline__ void epi_mask_store(const float (&acc)[NR], const Rel
   }
 }
 
+// The same for a 256-wide trunk gradient that stays in registers: dY = dh * [h > 0] as fp16 -> the next step's A fragments
+// `a`, and the same fp16 pairs straight to this warpgroup's rows of the tile's gradient-stash image `gs_img` (a warp's 32
+// words of one column group and row half are one contiguous 128-byte line of the chunk-major image).
+__device__ __forceinline__ void epi_mask_frag(const float (&acc)[kMaskHCols / 2], const ReluMask<kMaskHCols>& m,
+                                              uint32_t (&a)[kMaskHCols / 16][4], uint8_t* gs_img, int g) {
+  const int r0 = g * kWgRows + acc_r0(), q = acc_q();
+#pragma unroll
+  for (int j = 0; j < kMaskHCols / 8; ++j) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const uint32_t g2 = m.apply(i, j, pack_h2_sat(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]));
+      frag_pair(a, j, i) = g2;
+      *reinterpret_cast<uint32_t*>(gs_img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = g2;
+    }
+  }
+}
+
 __device__ __forceinline__ float h_lo(uint32_t w) { return __half2float(__ushort_as_half(static_cast<unsigned short>(w & 0xffffu))); }
 __device__ __forceinline__ float h_hi(uint32_t w) { return __half2float(__ushort_as_half(static_cast<unsigned short>(w >> 16))); }
 
@@ -99,8 +121,8 @@ __device__ __forceinline__ void pe_backward(const float* de, const uint8_t* __re
 template <bool HAS_BENDER>
 __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* act = smem;                               // 64 KB gradient operand, 128 rows
-  uint8_t* ring_buf = smem + kHBytes;                // kBwdRingStages x 32 KB
+  uint8_t* act = smem;                               // bender gradient operand (24 KB), 128 rows
+  uint8_t* ring_buf = smem + kBwdActBytes;           // kBwdRingStages x 32 KB
   float* stage_all = reinterpret_cast<float*>(ring_buf + kBwdRingStages * kRingStageBytes);   // 2 x 64 rows x kBwdStageLd
   auto* sh = reinterpret_cast<RingShared<kBwdRingStages>*>(stage_all + 2 * kWgRows * kBwdStageLd);
 
@@ -150,41 +172,62 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
     auto prefetch_e = [&]() {
       if (wg_leader) tma_prefetch_l2(st_tile + kStE.off, kEBytes);
     };
-    // ---- d_raw image: [g_r g_g g_b g_sigma 0 ...] (K = 16) ----
-    sw.begin();
-    if (row_thread) {
-      float gr[4] = {0.f, 0.f, 0.f, 0.f};
-      if (valid) {
-        const float* q = p.d_raw + pt * p.out_ch;
+    // The trunk's gradients dY7 .. dY0 stay in registers: each epilogue packs them into the A fragments h of the next step
+    // (wg_gemm_rs) and stores them to the gradient stash from there.  Only the staging rows stg are shared, and each of
+    // their rewrites is ordered after the reads before it by an explicit warpgroup barrier (L5e^T, L0^T).
+    constexpr Step kTrunk = dgrad::step(dgrad::L7T), kEmb = dgrad::step(dgrad::L5eT);
+    static_assert(dgrad::step(dgrad::L0T) == kEmb && kEmb.nslabs == 1 && kEmb.k16 == kMaskHCols / 16, "L5e^T, L0^T: one slab, K = 256");
+    uint32_t h[kMaskHCols / 16][4];
+    // ---- head^T: A = d_raw [g_r g_g g_b g_sigma 0 ...] (K = 16), one fragment built from global memory ----
+    {
+      static_assert(dgrad::step(dgrad::HeadT).N == kTrunk.N && dgrad::step(dgrad::HeadT).nslabs == 1 &&
+                    dgrad::step(dgrad::HeadT).k16 == 1 && kGsRaw.chunks == 2, "head^T: one K = 16 MMA");
+      const int r0 = g * kWgRows + acc_r0(), q = acc_q();
+      uint32_t a[1][4];
 #pragma unroll
-        for (int c = 0; c < 4; ++c) gr[c] = clamp_h(__ldg(q + c) * scale);
+      for (int i = 0; i < 2; ++i) {
+        // lanes q < 2 hold columns 2q, 2q + 1 of rows r0, r0 + 8; every other word is zero (rows past P too)
+        const long long pti = static_cast<long long>(tile) * kTileM + r0 + 8 * i;
+        float g0 = 0.f, g1 = 0.f;
+        if (q < 2 && pti < p.P) {
+          const float* src = p.d_raw + pti * p.out_ch + 2 * q;
+          g0 = clamp_h(__ldg(src) * scale);
+          g1 = clamp_h(__ldg(src + 1) * scale);
+        }
+        a[0][i] = q < 2 ? pack_h2(g0, g1) : 0u;
+        a[0][2 + i] = 0u;
       }
-      *reinterpret_cast<uint4*>(a_row) = make_uint4(pack_h2(gr[0], gr[1]), pack_h2(gr[2], gr[3]), 0u, 0u);
-      *reinterpret_cast<uint4*>(a_row + kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
+      // the same words -> the kGsRaw image (its zero columns and zero second chunk included)
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+          *reinterpret_cast<uint32_t*>(gs + kGsRaw.off + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = frag_pair(a, j, i);
+      Acc<dgrad::HeadT> acc;
+      ReluMask<kMaskHCols> m;
+      m.load(mk + kMkH + 7 * kMaskHBytes, g);
+      wg_gemm_rs<kTrunk.N, 1>(acc, a, ring, false, 0u, W, 300);
+      epi_mask_frag(acc, m, h, gs + kGsY + 7 * kHBytes, g);
     }
-    sw.ready(kGsRaw, act);
     float dx[3] = {0.f, 0.f, 0.f};
-    // ---- head^T, L7^T, L6^T : dY7, dY6, dY5 (every one 256 wide) ----
+    // ---- L7^T, L6^T : dY6, dY5 ----
 #pragma unroll 1
-    for (int s = 0; s < 3; ++s) {
-      const Step st = step_at(dgrad::HeadT + s);
+    for (int s = 0; s < 2; ++s) {
       Acc<dgrad::L7T> acc;
       ReluMask<kMaskHCols> m;
-      m.load(mk + kMkH + (7 - s) * kMaskHBytes, g);
-      wg_gemm<dgrad::step(dgrad::L7T).N>(acc, ring, st.nslabs, st.k16, a_slab, W, 300 + s);
-      if (s == 2) prefetch_e();
-      sw.begin();
-      epi_mask_store<kMaskHCols>(acc, m, act, g);
-      sw.ready({kGsY + (7 - s) * kHBytes, kHChunks}, act);
+      m.load(mk + kMkH + (6 - s) * kMaskHBytes, g);
+      wg_gemm_rs<kTrunk.N, kTrunk.k16>(acc, h, ring, false, 0u, W, 301 + s);
+      if (s == 1) prefetch_e();
+      epi_mask_frag(acc, m, h, gs + kGsY + (6 - s) * kHBytes, g);
     }
-    // ---- L5e^T: gradient into the skip-connected embedding ----
+    // ---- L5e^T: gradient into the skip-connected embedding; h (dY5) stays as it is for L5h^T ----
     {
       Acc<dgrad::L5eT> acc;
-      wg_gemm_step<dgrad::L5eT>(acc, ring, a_slab, W, 303);
+      wg_gemm_rs<kEmb.N, kEmb.k16>(acc, h, ring, false, 0u, W, 303);
+      wg_bar(bar);   // stg: every read of the previous tile (L0^T's pe_backward / B0^T's latent rows) is done
       stage_cols<0, 8>(acc, stg, kBwdStageLd);
       wg_bar(bar);
       if (row_thread) pe_backward(my_stg, st + kStE.off, dx);
-      // A operand (dY5) untouched; the staging rows are rewritten only after the barriers of the next steps
     }
     // ---- L5h^T, L4^T .. L1^T : dY4 .. dY0 (one shape) ----
 #pragma unroll 1
@@ -192,16 +235,15 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
       Acc<dgrad::L4T> acc;
       ReluMask<kMaskHCols> m;
       m.load(mk + kMkH + (4 - s) * kMaskHBytes, g);
-      wg_gemm_step<dgrad::L4T>(acc, ring, a_slab, W, 304 + s);
+      wg_gemm_rs<kTrunk.N, kTrunk.k16>(acc, h, ring, false, 0u, W, 304 + s);
       if (s == 4) prefetch_e();
-      sw.begin();
-      epi_mask_store<kMaskHCols>(acc, m, act, g);
-      sw.ready({kGsY + (4 - s) * kHBytes, kHChunks}, act);
+      epi_mask_frag(acc, m, h, gs + kGsY + (4 - s) * kHBytes, g);
     }
     // ---- L0^T: gradient into the embedding; then through the bend ----
     {
       Acc<dgrad::L0T> acc;
-      wg_gemm_step<dgrad::L0T>(acc, ring, a_slab, W, 309);
+      wg_gemm_rs<kEmb.N, kEmb.k16>(acc, h, ring, false, 0u, W, 309);
+      wg_bar(bar);   // stg: L5e^T's pe_backward reads are done
       stage_cols<0, 8>(acc, stg, kBwdStageLd);
       wg_bar(bar);
       if (row_thread) pe_backward(my_stg, st + kStE.off, dx);
@@ -298,7 +340,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
         }
       }
     }
-    // next: the next tile's d_raw image (after sw.begin()'s barrier)
+    // next: the next tile's L5e^T rewrites stg only after its own barrier; act only after the bender's sw.begin()
   }
   if (wg_leader) tma_bulk_wait<0>();   // all gradient-stash stores complete before the CTA exits
 }

@@ -272,6 +272,18 @@ __device__ __forceinline__ void wgmma_m64n16_rs(float (&d)[8], const uint32_t (&
 }
 
 template <int TB>
+__device__ __forceinline__ void wgmma_m64n64_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate), "n"(TB));
+}
+
+template <int TB>
 __device__ __forceinline__ void wgmma_m64n256_rs(float (&d)[128], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
@@ -285,8 +297,9 @@ __device__ __forceinline__ void wgmma_m64n256_rs(float (&d)[128], const uint32_t
 
 template <int N, int TB>
 __device__ __forceinline__ void wgmma_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
-  static_assert(N == 16 || N == 256, "wgmma_rs: N without a wrapper");
+  static_assert(N == 16 || N == 64 || N == 256, "wgmma_rs: N without a wrapper");
   if constexpr (N == 16) wgmma_m64n16_rs<TB>(d, a, bdesc, accumulate);
+  else if constexpr (N == 64) wgmma_m64n64_rs<TB>(d, a, bdesc, accumulate);
   else wgmma_m64n256_rs<TB>(d, a, bdesc, accumulate);
 }
 // The A-fragment word of a[KF][4] that holds the packed pair (column group j, row r0 + 8 i) of a 16-bit accumulator
