@@ -40,7 +40,7 @@ int nrn_device_error(int* code_out);
  * rigidity_network (run_nerf_helpers.py:411-482). */
 size_t nrn_packed_nerf_bytes(void);
 size_t nrn_packed_bender_bytes(void);
-/* w[0..7] = pts_linears.i.weight, w[8] = output_linear.weight; b likewise. input_ch = 63. */
+/* w[0..7] = pts_linears.i.weight, w[8] = output_linear.weight; b likewise. input_ch = 63 (95: time-conditioned baseline). */
 int nrn_pack_nerf(const float* const* w, const float* const* b, int input_ch, int out_ch, void* packed,
                   void* stream);
 int nrn_pack_bender(const float* const* net_w /*5*/, const float* const* net_b /*4*/,
@@ -176,6 +176,32 @@ typedef struct NrnFieldBwdArgs {
 } NrnFieldBwdArgs;
 int nrn_field_backward(const NrnFieldBwdArgs* args);
 
+/* ---- time-conditioned baseline (NeRF(time_conditioned_baseline=True), run_nerf_helpers.py:206-209, 273-282; no bender,
+ * train.py:574-578): the per-ray latent z is concatenated to the embedding at L0 ([PE(63) | z(32)], W0 [256][95]) and at
+ * the skip layer L5 ([PE | z | h], W5 [256][351]).  z is the same for every sample of a ray, so W_l[:, 63:95] . z + b_l is
+ * one fp32 bias row per ray and layer ("ray bias" [n][2][256], L0 then L5) and the fused kernels run the geometry of
+ * the 63-input NeRF.  nrn_pack_nerf with input_ch = 95 packs such weights (the latent columns are skipped). */
+/* ray_bias[n][l][o] = b_l[o] + sum_k W_l[o][63 + k] latents[n * latent_stride + k]  (fp32; w0 [256][95], w5 [256][351]) */
+int nrn_tc_latent_bias(const float* latents, int64_t latent_stride, int n_rays, const float* w0, const float* b0, const float* w5,
+                       const float* b5, float* ray_bias, void* stream);
+/* nrn_field_forward with the L0 / L5 biases taken from ray_bias: one row per ray (row stride 512 floats), or, when
+ * args->latent_stride == 0, one row for every ray.  args->bender_packed must be NULL; args->latents is not read. */
+int nrn_field_forward_tc(const NrnFieldArgs* args, const float* ray_bias);
+int nrn_nerf_tc_grad_floats(int out_ch);   /* flat order as nrn_nerf_grad_floats, with W0 [256][95] and W5 [256][351] */
+size_t nrn_tc_workspace_bytes(int n_rays);   /* per-ray sums [n][2][256] + latent columns of dW0 / dW5 [2][256][32] */
+typedef struct NrnTcBwdArgs {
+  const float* latents;           /* [n_rays][32] the forward call's latents ... */
+  int64_t latent_stride;          /* ... row stride in floats (0 = one row for every ray) */
+  const float* w0;                /* fp32 pts_linears.0.weight [256][95] */
+  const float* w5;                /* fp32 pts_linears.5.weight [256][351] */
+  float* d_latents;               /* out [n_rays][32], overwritten */
+  float* workspace;               /* nrn_tc_workspace_bytes(n_rays) */
+} NrnTcBwdArgs;
+/* nrn_field_backward of a nrn_field_forward_tc call (args->bender_packed NULL): nerf_grad (and nerf_grad_head) in the
+ * time-conditioned flat layout of nrn_nerf_tc_grad_floats, the latent columns of W0 / W5 included, and d_latents.
+ * Deterministic: every sum runs in a fixed order. */
+int nrn_field_backward_tc(const NrnFieldBwdArgs* args, const NrnTcBwdArgs* tc);
+
 /* ---- divergence regulariser of the offset field on the coarse samples: compute_divergence_loss /
  * divergence_approx (run_nerf_helpers.py:22-116) as driven by train.py:245-286, forward and backward
  * in closed form (no double backward), on tensor cores with the fp16 bender weights the coarse pass ran with.
@@ -303,7 +329,8 @@ int nrn_peer_gather_rows(const NrnPeerCtx* ctx, const float* local, int n_per_ra
 /* ---- optional per-kernel timing (measurement aid for bench.py) ---------------------------------
  * While enabled, every launch of the kernel kinds below is bracketed by CUDA events recorded on the
  * launch stream.  kinds: 0 field forward, 1 field DGRAD, 2 WGRAD (+reduce), 3 composite(+resample),
- * 4 composite backward, 5 divergence regulariser.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * 4 composite backward, 5 divergence regulariser, 6 time-conditioned ray bias (nrn_tc_latent_bias), 7 time-conditioned
+ * latent gradients (per-ray sums, d z, latent columns of dW0 / dW5).  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

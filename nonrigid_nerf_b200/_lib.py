@@ -50,6 +50,12 @@ class NrnFieldBwdArgs(C.Structure):
     ]
 
 
+class NrnTcBwdArgs(C.Structure):
+    _fields_ = [
+        ("latents", _vp), ("latent_stride", C.c_int64), ("w0", _vp), ("w5", _vp), ("d_latents", _vp), ("workspace", _vp),
+    ]
+
+
 class NrnDivArgs(C.Structure):
     _fields_ = [
         ("n_rays", C.c_int32), ("n_samples", C.c_int32),
@@ -142,6 +148,11 @@ SYMBOLS = {
     "nrn_nerf_grad_floats": (C.c_int, [C.c_int]),
     "nrn_bender_grad_floats": (C.c_int, []),
     "nrn_field_backward": (C.c_int, [C.POINTER(NrnFieldBwdArgs)]),
+    "nrn_tc_latent_bias": (C.c_int, [_vp, C.c_int64, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nrn_field_forward_tc": (C.c_int, [C.POINTER(NrnFieldArgs), _vp]),
+    "nrn_nerf_tc_grad_floats": (C.c_int, [C.c_int]),
+    "nrn_tc_workspace_bytes": (C.c_size_t, [C.c_int]),
+    "nrn_field_backward_tc": (C.c_int, [C.POINTER(NrnFieldBwdArgs), C.POINTER(NrnTcBwdArgs)]),
     "nrn_div_stash_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "nrn_div_grad_stash_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "nrn_divergence_forward": (C.c_int, [C.POINTER(NrnDivArgs)]),
@@ -162,19 +173,22 @@ SYMBOLS = {
 }
 
 KERNEL_KINDS = ("field_fwd", "field_dgrad", "wgrad", "composite", "composite_bwd", "divergence")
+# the time-conditioned baseline's own kernels (ray bias; per-ray sums, d z and latent weight columns), timing kinds 6 and 7
+TC_KERNEL_KINDS = ("tc_latent_bias", "tc_latent_bwd")
 
 
 def timing_enable(on: bool) -> None:
     check(load().nrn_timing_enable(1 if on else 0), "timing_enable")
 
 
-def timing_read():
-    """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True)."""
-    n = len(KERNEL_KINDS)
+def timing_read(kinds=KERNEL_KINDS):
+    """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True); `kinds` is KERNEL_KINDS or
+    KERNEL_KINDS + TC_KERNEL_KINDS."""
+    n = len(kinds)
     ms = (C.c_double * n)()
     cnt = (C.c_int * n)()
     check(load().nrn_timing_read(ms, cnt, n), "timing_read")
-    return {k: (ms[i], cnt[i]) for i, k in enumerate(KERNEL_KINDS)}
+    return {k: (ms[i], cnt[i]) for i, k in enumerate(kinds)}
 
 _lib = None
 _lock = threading.Lock()

@@ -29,6 +29,17 @@ def _knobs(net):
     return cutoff, scaling, removal
 
 
+def _tc_net(net):
+    """The NeRF itself when it is a time-conditioned baseline (its latents enter L0 / L5 as per-ray biases), else None.
+    Like train.py:574-576 the baseline runs without ray bending."""
+    if not getattr(net, "time_conditioned_baseline", False):
+        return None
+    if net.ray_bender[0] is not None:
+        raise RuntimeError("nonrigid_nerf_b200: the time_conditioned_baseline NeRF requires ray bending to be turned off "
+                           "(ray_bender must be None)")
+    return net
+
+
 def _flat_params(net, bender):
     """Parameters in the flat order of the WGRAD output buffers (csrc/wgrad.cu); `net` may be None for the bender's
     alone."""
@@ -78,8 +89,13 @@ class _FieldTrainFn(torch.autograd.Function):
         lib = _lib.load()
         stash = torch.empty(lib.nrn_stash_bytes(n, s), dtype=torch.uint8, device=z_vals.device)
         relu_mask = torch.empty(lib.nrn_relu_mask_bytes(n, s), dtype=torch.uint8, device=z_vals.device)
+        tc = _tc_net(net)
+        ctx.tc_latents = None
+        if tc is not None:   # the latents as the forward read them: the backward forms their gradient and dW0 / dW5's latent columns
+            ctx.tc_latents = ops.latent_rows(latents.detach(), n, z_vals.device)
+            latents = ctx.tc_latents[0]
         raw, det = ops.field_forward(rays, z_vals, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, None, True, stash,
-                                     relu_mask)
+                                     relu_mask, tc)
         ctx.net, ctx.n_nerf = net, n_nerf
         ctx.shape = (n, s, out_ch)
         ctx.knobs = (cutoff, scaling)
@@ -134,7 +150,8 @@ class _FieldTrainFn(torch.autograd.Function):
         if head_dst is not None:
             a.nerf_grad, a.nerf_grad_head, a.accumulate_nerf = pts_dst, head_dst, 1
         else:
-            nerf_grad = torch.empty(lib.nrn_nerf_grad_floats(out_ch), dtype=torch.float32, device=dev)
+            n_floats = lib.nrn_nerf_tc_grad_floats(out_ch) if ctx.tc_latents is not None else lib.nrn_nerf_grad_floats(out_ch)
+            nerf_grad = torch.empty(n_floats, dtype=torch.float32, device=dev)
             a.nerf_grad = nerf_grad.data_ptr()
         bend_grad = d_lat = None
         bend_in_place = False
@@ -164,8 +181,19 @@ class _FieldTrainFn(torch.autograd.Function):
             d_lat = torch.empty(n, ops.LATENT, dtype=torch.float32, device=dev)
             a.d_latents = d_lat.data_ptr()
         a.stream = torch.cuda.current_stream().cuda_stream
-        with torch.cuda.device(dev):
-            _lib.check(lib.nrn_field_backward(C.byref(a)), "field_backward")
+        if ctx.tc_latents is not None:
+            lat, stride = ctx.tc_latents
+            t = _lib.NrnTcBwdArgs()
+            t.latents, t.latent_stride = lat.data_ptr(), stride
+            t.w0, t.w5 = net.pts_linears[0].weight.data_ptr(), net.pts_linears[5].weight.data_ptr()
+            d_lat = torch.empty(n, ops.LATENT, dtype=torch.float32, device=dev)
+            workspace = torch.empty(lib.nrn_tc_workspace_bytes(n), dtype=torch.uint8, device=dev)
+            t.d_latents, t.workspace = d_lat.data_ptr(), workspace.data_ptr()
+            with torch.cuda.device(dev):
+                _lib.check(lib.nrn_field_backward_tc(C.byref(a), C.byref(t)), "field_backward_tc")
+        else:
+            with torch.cuda.device(dev):
+                _lib.check(lib.nrn_field_backward(C.byref(a)), "field_backward")
         # the stash and the ReLU masks live as long as the autograd node: backward(retain_graph=True) followed by a second backward()
         # over the same graph (test-latent pass of the reference loop, train.py:1595-1606) reads it again
         if nerf_grad is None:
@@ -483,6 +511,7 @@ def field(net, rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[torch
           want_details: bool) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
     """Fused field evaluation for rays x samples; differentiable when autograd is recording."""
     bender = net.ray_bender[0]
+    _tc_net(net)
     if not _needs_grad(net, latents):
         return field_rays(net, rays, z_vals, latents, want_details)
     nerf_p, bend_p = _flat_params(net, bender)
@@ -504,11 +533,13 @@ def field_rays(net, rays, z_vals, latents, want_details):
     nerf_pack = ops.pack_nerf(net)
     bender_pack = ops.pack_bender(bender) if bender is not None else None
     out_ch = net.output_linear.weight.shape[0]
-    return ops.field_forward(rays, z_vals, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details)
+    return ops.field_forward(rays, z_vals, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details,
+                             tc_net=_tc_net(net))
 
 
 def field_points(net, pts, latents, want_details):
     """NeRF.forward(x) semantics: one xyz (+ latent) per row.  Inference only."""
+    _tc_net(net)
     if _needs_grad(net, latents):
         raise RuntimeError("nonrigid_nerf_b200: the point-wise NeRF.forward / run_network entry is inference-only; "
                            "differentiable rendering goes through render() / render_rays()")
@@ -517,7 +548,8 @@ def field_points(net, pts, latents, want_details):
     nerf_pack = ops.pack_nerf(net)
     bender_pack = ops.pack_bender(bender) if bender is not None else None
     out_ch = net.output_linear.weight.shape[0]
-    return ops.field_forward_points(pts, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details)
+    return ops.field_forward_points(pts, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details,
+                                    tc_net=_tc_net(net))
 
 
 def composite(raw, z_vals, rays_d, noise=None, white_bkgd=False, n_importance=0, u=None) -> Dict[str, torch.Tensor]:

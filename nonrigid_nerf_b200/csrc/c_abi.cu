@@ -17,6 +17,10 @@
 namespace nrn {
 cudaError_t launch_field_fwd(const FieldFwdParams& p, bool has_bender, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_bwd(const FieldBwdParams& p, bool has_bender, int num_sms, cudaStream_t stream);
+cudaError_t launch_field_fwd_tc(const FieldFwdParams& p, int num_sms, cudaStream_t stream);
+cudaError_t launch_tc_latent_bias(const float* lat, long long lat_stride, int n_rays, const float* w0, const float* b0, const float* w5,
+                                  const float* b5, float* rb, cudaStream_t stream);
+cudaError_t launch_tc_latent_bwd(const TcBwdParams& p, cudaStream_t stream);
 }
 
 namespace {
@@ -124,7 +128,8 @@ size_t nrn_packed_bender_bytes(void) { return nrn::kBendPackedBytes; }
 
 int nrn_pack_nerf(const float* const* w, const float* const* b, int input_ch, int out_ch, void* packed, void* stream) {
   if (!w || !b || !packed) return fail(NRN_E_INVALID, "nrn_pack_nerf: null argument");
-  if (input_ch < 1 || input_ch > 63) return fail(NRN_E_INVALID, "nrn_pack_nerf: input_ch=%d unsupported (1..63; multires=10 gives 63)", input_ch);
+  if ((input_ch < 1 || input_ch > 63) && input_ch != nrn::kPeCols + nrn::kLatent)
+    return fail(NRN_E_INVALID, "nrn_pack_nerf: input_ch=%d unsupported (1..63; multires=10 gives 63; 95 = 63 + 32: time-conditioned baseline)", input_ch);
   if (out_ch < 4 || out_ch > 16) return fail(NRN_E_INVALID, "nrn_pack_nerf: out_ch=%d unsupported", out_ch);
   if (!aligned16(packed)) return fail(NRN_E_INVALID, "nrn_pack_nerf: packed buffer must be 16-byte aligned");
   nrn::NerfSrc src;
@@ -194,22 +199,23 @@ int nrn_median_visibility_index(const float* weights, int n_rays, int n_samples,
   return e == cudaSuccess ? NRN_OK : cuda_fail(e, "median_index_kernel");
 }
 
-int nrn_field_forward(const NrnFieldArgs* a) {
-  if (!a) return fail(NRN_E_INVALID, "nrn_field_forward: null args");
-  if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "nrn_field_forward: bad sizes n=%d S=%d", a->n_rays, a->n_samples);
+// nrn_field_forward, or with ray_bias (time-conditioned baseline, no bender) nrn_field_forward_tc
+static int field_forward(const NrnFieldArgs* a, const float* ray_bias, const char* who) {
+  if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
+  if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "%s: bad sizes n=%d S=%d", who, a->n_rays, a->n_samples);
   if (a->n_rays == 0) return NRN_OK;
-  if (!a->nerf_packed || !a->raw) return fail(NRN_E_INVALID, "nrn_field_forward: null argument");
+  if (!a->nerf_packed || !a->raw) return fail(NRN_E_INVALID, "%s: null argument", who);
   if (a->points) {
-    if (a->n_samples != 1 || a->points_stride < 3) return fail(NRN_E_INVALID, "nrn_field_forward: point mode needs n_samples=1, stride>=3");
+    if (a->n_samples != 1 || a->points_stride < 3) return fail(NRN_E_INVALID, "%s: point mode needs n_samples=1, stride>=3", who);
   } else if (!a->rays || !a->z_vals) {
-    return fail(NRN_E_INVALID, "nrn_field_forward: null rays / z_vals");
+    return fail(NRN_E_INVALID, "%s: null rays / z_vals", who);
   }
-  if (a->bender_packed && !a->latents) return fail(NRN_E_INVALID, "nrn_field_forward: bender given without latents");
-  if (a->out_ch < 4 || a->out_ch > 5) return fail(NRN_E_INVALID, "nrn_field_forward: out_ch=%d unsupported (4 or 5)", a->out_ch);
+  if (a->bender_packed && !a->latents) return fail(NRN_E_INVALID, "%s: bender given without latents", who);
+  if (a->out_ch < 4 || a->out_ch > 5) return fail(NRN_E_INVALID, "%s: out_ch=%d unsupported (4 or 5)", who, a->out_ch);
   if (!aligned16(a->nerf_packed) || (a->bender_packed && !aligned16(a->bender_packed)))
-    return fail(NRN_E_INVALID, "nrn_field_forward: packed weights must be 16-byte aligned");
+    return fail(NRN_E_INVALID, "%s: packed weights must be 16-byte aligned", who);
   if ((a->stash != nullptr) != (a->relu_mask != nullptr))
-    return fail(NRN_E_INVALID, "nrn_field_forward: training needs both the stash and the ReLU mask buffer (relu_mask)");
+    return fail(NRN_E_INVALID, "%s: training needs both the stash and the ReLU mask buffer (relu_mask)", who);
   DeviceState* ds;
   int rc = device_state(&ds);
   if (rc) return rc;
@@ -234,14 +240,37 @@ int nrn_field_forward(const NrnFieldArgs* a) {
   p.d_masked = a->masked_offsets; p.d_rigid = a->rigidity_mask;
   p.stash = static_cast<uint8_t*>(a->stash);
   p.relu_mask = static_cast<uint8_t*>(a->relu_mask);
-  if (a->stash && a->points) return fail(NRN_E_INVALID, "nrn_field_forward: the training stash needs ray mode");
+  if (a->stash && a->points) return fail(NRN_E_INVALID, "%s: the training stash needs ray mode", who);
   p.err = ds->err_word;
+  p.ray_bias = ray_bias; p.ray_bias_stride = a->latent_stride == 0 ? 0 : 2 * 256;
   cudaError_t e;
   {
     ScopedTimer tm(0, static_cast<cudaStream_t>(a->stream));
-    e = nrn::launch_field_fwd(p, a->bender_packed != nullptr, ds->num_sms, static_cast<cudaStream_t>(a->stream));
+    e = ray_bias ? nrn::launch_field_fwd_tc(p, ds->num_sms, static_cast<cudaStream_t>(a->stream))
+                 : nrn::launch_field_fwd(p, a->bender_packed != nullptr, ds->num_sms, static_cast<cudaStream_t>(a->stream));
   }
-  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "field_fwd_kernel");
+  return e == cudaSuccess ? NRN_OK : cuda_fail(e, ray_bias ? "field_fwd_tc_kernel" : "field_fwd_kernel");
+}
+
+int nrn_field_forward(const NrnFieldArgs* a) { return field_forward(a, nullptr, "nrn_field_forward"); }
+
+int nrn_field_forward_tc(const NrnFieldArgs* a, const float* ray_bias) {
+  if (!a) return fail(NRN_E_INVALID, "nrn_field_forward_tc: null args");
+  if (a->bender_packed) return fail(NRN_E_INVALID, "nrn_field_forward_tc: the time-conditioned baseline has no bender (bender_packed must be NULL)");
+  if (a->latent_stride < 0) return fail(NRN_E_INVALID, "nrn_field_forward_tc: latent_stride < 0");
+  if (a->n_rays > 0 && !ray_bias) return fail(NRN_E_INVALID, "nrn_field_forward_tc: null ray_bias (nrn_tc_latent_bias output)");
+  return field_forward(a, ray_bias, "nrn_field_forward_tc");
+}
+
+int nrn_tc_latent_bias(const float* latents, int64_t latent_stride, int n_rays, const float* w0, const float* b0, const float* w5,
+                       const float* b5, float* ray_bias, void* stream) {
+  if (n_rays < 0 || latent_stride < 0) return fail(NRN_E_INVALID, "nrn_tc_latent_bias: bad sizes n=%d stride=%lld", n_rays, (long long)latent_stride);
+  if (n_rays == 0) return NRN_OK;
+  if (!latents || !w0 || !b0 || !w5 || !b5 || !ray_bias) return fail(NRN_E_INVALID, "nrn_tc_latent_bias: null argument");
+  cudaError_t e;
+  { ScopedTimer tm(6, static_cast<cudaStream_t>(stream));
+    e = nrn::launch_tc_latent_bias(latents, latent_stride, n_rays, w0, b0, w5, b5, ray_bias, static_cast<cudaStream_t>(stream)); }
+  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "tc_latent_bias_kernel");
 }
 
 int nrn_composite(const NrnCompositeArgs* a) {
@@ -294,22 +323,25 @@ size_t nrn_relu_mask_bytes(int n_rays, int n_samples) { return static_cast<size_
 size_t nrn_wgrad_scratch_bytes(void) { return static_cast<size_t>(nrn::kWgMaxCtas) * nrn::kWgScratchFloats * sizeof(float); }
 int nrn_nerf_grad_floats(int out_ch) { return nrn::nerf_grad_floats(out_ch); }
 int nrn_bender_grad_floats(void) { return nrn::bparam::total(); }
+int nrn_nerf_tc_grad_floats(int out_ch) { return nrn::nerf_tc_grad_floats(out_ch); }
+size_t nrn_tc_workspace_bytes(int n_rays) { return n_rays < 0 ? 0 : (static_cast<size_t>(n_rays) * 2 * 256 + 2 * 256 * nrn::kLatent) * sizeof(float); }
 
-int nrn_field_backward(const NrnFieldBwdArgs* a) {
-  if (!a) return fail(NRN_E_INVALID, "nrn_field_backward: null args");
-  if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "nrn_field_backward: bad sizes");
-  if (a->out_ch < 4 || a->out_ch > 5) return fail(NRN_E_INVALID, "nrn_field_backward: out_ch=%d unsupported", a->out_ch);
-  if (!a->nerf_packed || !a->nerf_grad) return fail(NRN_E_INVALID, "nrn_field_backward: null argument");
+// nrn_field_backward, or with t (time-conditioned baseline, no bender) nrn_field_backward_tc
+static int field_backward(const NrnFieldBwdArgs* a, const NrnTcBwdArgs* t, const char* who) {
+  if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
+  if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "%s: bad sizes", who);
+  if (a->out_ch < 4 || a->out_ch > 5) return fail(NRN_E_INVALID, "%s: out_ch=%d unsupported", who, a->out_ch);
+  if (!a->nerf_packed || !a->nerf_grad) return fail(NRN_E_INVALID, "%s: null argument", who);
   const bool bend = a->bender_packed != nullptr;
   if (bend && (!a->unmasked_offsets || !a->rigidity_mask || !a->bender_grad || !a->d_latents))
-    return fail(NRN_E_INVALID, "nrn_field_backward: bender needs unmasked_offsets, rigidity_mask, bender_grad, d_latents");
-  if (a->n_rays > 0 && !a->relu_mask) return fail(NRN_E_INVALID, "nrn_field_backward: null relu_mask (the ReLU masks of the forward call)");
+    return fail(NRN_E_INVALID, "%s: bender needs unmasked_offsets, rigidity_mask, bender_grad, d_latents", who);
+  if (a->n_rays > 0 && !a->relu_mask) return fail(NRN_E_INVALID, "%s: null relu_mask (the ReLU masks of the forward call)", who);
   DeviceState* ds;
   int rc = device_state(&ds);
   if (rc) return rc;
-  if (ds->num_sms + 16 > nrn::kWgMaxCtas) return fail(NRN_E_INVALID, "nrn_field_backward: %d SMs exceed the scratch layout", ds->num_sms);
+  if (ds->num_sms + 16 > nrn::kWgMaxCtas) return fail(NRN_E_INVALID, "%s: %d SMs exceed the scratch layout", who, ds->num_sms);
   cudaStream_t st = static_cast<cudaStream_t>(a->stream);
-  const int nerf_n = nrn_nerf_grad_floats(a->out_ch);
+  const int nerf_n = t ? nrn_nerf_tc_grad_floats(a->out_ch) : nrn_nerf_grad_floats(a->out_ch);
   const int bend_n = bend ? nrn_bender_grad_floats() : 0;
   cudaError_t e;
   if (bend) {
@@ -326,7 +358,7 @@ int nrn_field_backward(const NrnFieldBwdArgs* a) {
     if (e == cudaSuccess && bend && !a->accumulate_bender) e = cudaMemsetAsync(a->bender_grad, 0, sizeof(float) * bend_n, st);
     return e == cudaSuccess ? NRN_OK : cuda_fail(e, "memset grads");
   }
-  if (!a->d_raw || !a->stash || !a->grad_stash || !a->wgrad_scratch) return fail(NRN_E_INVALID, "nrn_field_backward: null argument");
+  if (!a->d_raw || !a->stash || !a->grad_stash || !a->wgrad_scratch) return fail(NRN_E_INVALID, "%s: null argument", who);
   float* amax = reinterpret_cast<float*>(ds->err_word + 1);
   nrn::FieldBwdParams p{};
   p.P = static_cast<long long>(a->n_rays) * a->n_samples;
@@ -350,11 +382,31 @@ int nrn_field_backward(const NrnFieldBwdArgs* a) {
   if (e != cudaSuccess) return cuda_fail(e, "absmax_kernel");
   { ScopedTimer tm(1, st); e = nrn::launch_field_bwd(p, bend, ds->num_sms, st); }
   if (e != cudaSuccess) return cuda_fail(e, "field_bwd_kernel");
+  float* dw_lat = nullptr;
+  if (t) {   // per-ray sums of dY0 / dY5 -> d z and the latent columns of dW0 / dW5 (before WGRAD's reduction reads them)
+    nrn::TcBwdParams q{};
+    q.gstash = p.gstash; q.amax = amax; q.P = p.P; q.S = p.S; q.n_rays = a->n_rays;
+    q.latents = t->latents; q.latent_stride = t->latent_stride; q.w0 = t->w0; q.w5 = t->w5;
+    q.sums = t->workspace; q.dw_lat = dw_lat = t->workspace + static_cast<size_t>(a->n_rays) * 2 * 256; q.d_latents = t->d_latents;
+    { ScopedTimer tm(7, st); e = nrn::launch_tc_latent_bwd(q, st); }
+    if (e != cudaSuccess) return cuda_fail(e, "tc_ray_sums_kernel");
+  }
   nrn::WgradParams w{};
   w.stash = p.stash; w.gstash = p.gstash; w.scratch = a->wgrad_scratch; w.amax = amax; w.n_tiles = p.n_tiles; w.err = ds->err_word;
   const nrn::WgradDst dst{a->nerf_grad, a->nerf_grad_head, a->bender_grad, nerf_n, bend_n, a->accumulate_nerf, a->accumulate_bender};
-  { ScopedTimer tm(2, st); e = nrn::launch_wgrad(w, bend, ds->num_sms, dst, a->out_ch, st); }
+  { ScopedTimer tm(2, st); e = nrn::launch_wgrad(w, bend, ds->num_sms, dst, a->out_ch, st, dw_lat); }
   return e == cudaSuccess ? NRN_OK : cuda_fail(e, "wgrad_kernel");
+}
+
+int nrn_field_backward(const NrnFieldBwdArgs* a) { return field_backward(a, nullptr, "nrn_field_backward"); }
+
+int nrn_field_backward_tc(const NrnFieldBwdArgs* a, const NrnTcBwdArgs* t) {
+  if (!a || !t) return fail(NRN_E_INVALID, "nrn_field_backward_tc: null args");
+  if (a->bender_packed) return fail(NRN_E_INVALID, "nrn_field_backward_tc: the time-conditioned baseline has no bender (bender_packed must be NULL)");
+  if (t->latent_stride < 0) return fail(NRN_E_INVALID, "nrn_field_backward_tc: latent_stride < 0");
+  if (a->n_rays > 0 && (!t->latents || !t->w0 || !t->w5 || !t->d_latents || !t->workspace))
+    return fail(NRN_E_INVALID, "nrn_field_backward_tc: null latents, w0, w5, d_latents or workspace");
+  return field_backward(a, t, "nrn_field_backward_tc");
 }
 
 static long long point_tiles(int n_rays, int n_samples) {

@@ -346,8 +346,76 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
 }
 
 // ------------------------------------------------------------------------------------------------
+// Time-conditioned baseline: the latent enters L0 and L5 as a per-ray bias (field_fwd.cu), so its gradients are per-ray
+// sums of those layers' pre-activation gradients dY0, dY5 (gradient stash):
+//   s_l[ray] = sum over the ray's samples of dY_l,   d z[ray] = W0[:, 63:95]^T s_0 + W5[:, 63:95]^T s_5,
+//   dW_l[:, 63:95] = sum over rays of s_l[ray] (x) z[ray].
+// Every sum runs in a fixed order (samples, output features, rays), so the results are bit-reproducible.
+namespace {
+constexpr int kTcSumRays = 4;   // rays per block of tc_ray_sums_kernel: 64 threads = 2 layers x 32 column chunks each
+constexpr int kTcDzRays = 8;    // rays per block of tc_dz_kernel: 32 threads (latent dims) each
+
+// thread = (ray, layer, 8-column chunk): one 16-byte row piece of the chunk-major dY image per sample
+__global__ void __launch_bounds__(256) tc_ray_sums_kernel(const TcBwdParams p) {
+  const int ray = blockIdx.x * kTcSumRays + threadIdx.x / 64;
+  const int l = (threadIdx.x / 32) & 1, c = threadIdx.x & 31;
+  if (ray >= p.n_rays) return;
+  const float inv_scale = 1.0f / loss_scale(p.amax);
+  float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  const uint8_t* base = p.gstash + kGsY + (l ? 5 : 0) * kHBytes + c * kChunkBytes;
+  for (int s = 0; s < p.S; ++s) {
+    const long long pt = static_cast<long long>(ray) * p.S + s;
+    const uint4 w = __ldg(reinterpret_cast<const uint4*>(base + (pt / kTileM) * kGradTileBytes + (pt % kTileM) * 16));
+    const uint32_t wv[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      acc[2 * q] += __half2float(__ushort_as_half(static_cast<unsigned short>(wv[q] & 0xffffu)));
+      acc[2 * q + 1] += __half2float(__ushort_as_half(static_cast<unsigned short>(wv[q] >> 16)));
+    }
+  }
+  float* dst = p.sums + static_cast<long long>(ray) * 512 + l * 256 + c * 8;
+#pragma unroll
+  for (int e = 0; e < 8; ++e) dst[e] = acc[e] * inv_scale;
+}
+
+// thread = (ray, latent dim k): d z[ray][k] over the 256 outputs of both layers
+__global__ void __launch_bounds__(256) tc_dz_kernel(const TcBwdParams p) {
+  const int ray = blockIdx.x * kTcDzRays + threadIdx.x / 32, k = threadIdx.x & 31;
+  if (ray >= p.n_rays) return;
+  const float* s = p.sums + static_cast<long long>(ray) * 512;
+  float d = 0.f;
+#pragma unroll 4
+  for (int o = 0; o < 256; ++o) {
+    d = fmaf(__ldg(p.w0 + o * (kPeCols + kLatent) + kPeCols + k), __ldg(s + o), d);
+    d = fmaf(__ldg(p.w5 + o * (kPeCols + kLatent + 256) + kPeCols + k), __ldg(s + 256 + o), d);
+  }
+  p.d_latents[static_cast<long long>(ray) * kLatent + k] = d;
+}
+
+// thread = (layer, latent dim k, output o): dW_l[o][63 + k] over the rays (o fastest: coalesced reads of the sums)
+__global__ void __launch_bounds__(256) tc_dw_lat_kernel(const TcBwdParams p) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= 2 * kLatent * 256) return;
+  const int o = idx & 255, k = (idx >> 8) & (kLatent - 1), l = idx >> 13;
+  const float* s = p.sums + l * 256 + o;
+  const float* z = p.latents + k;
+  float a = 0.f;
+#pragma unroll 8
+  for (int r = 0; r < p.n_rays; ++r) a = fmaf(__ldg(s + static_cast<long long>(r) * 512), __ldg(z + r * p.latent_stride), a);
+  p.dw_lat[(l * 256 + o) * kLatent + k] = a;
+}
+}  // namespace
+
 cudaError_t launch_field_bwd(const FieldBwdParams& p, bool has_bender, int num_sms, cudaStream_t stream) {
   return launch_field(has_bender ? field_bwd_kernel<true> : field_bwd_kernel<false>, p, num_sms, kBwdSmemBytes, stream);
+}
+
+cudaError_t launch_tc_latent_bwd(const TcBwdParams& p, cudaStream_t stream) {
+  if (p.n_rays <= 0) return cudaSuccess;
+  tc_ray_sums_kernel<<<(p.n_rays + kTcSumRays - 1) / kTcSumRays, 64 * kTcSumRays, 0, stream>>>(p);
+  tc_dz_kernel<<<(p.n_rays + kTcDzRays - 1) / kTcDzRays, 32 * kTcDzRays, 0, stream>>>(p);
+  tc_dw_lat_kernel<<<2 * kLatent * 256 / 256, 256, 0, stream>>>(p);
+  return cudaGetLastError();
 }
 
 }  // namespace nrn

@@ -76,19 +76,24 @@ __device__ __forceinline__ void epi_bias_relu_store(const float (&acc)[NR], cons
 // The same for a 256-wide trunk layer whose output stays in registers: bias, ReLU, fp16 -> the next step's A fragments
 // `a`.  TRAIN: also the mask bits, and the fp16 pairs straight to this warpgroup's rows of the tile's stash image `st_img`
 // (a warp's 32 words of one column group and row half are one contiguous 128-byte line of the chunk-major image).
-template <bool TRAIN>
+// ROW_BIAS (time-conditioned L0 / L5): accumulator rows r0 and r0 + 8 take their biases from their own rows `bias` and
+// `bias8` (their rays' ray-bias rows) instead of one vector.
+template <bool TRAIN, bool ROW_BIAS = false>
 __device__ __forceinline__ void epi_bias_relu_frag(const float (&acc)[kMaskHCols / 2], const float* __restrict__ bias,
                                                    uint32_t (&a)[kMaskHCols / 16][4], uint8_t* st_img, int g,
-                                                   uint8_t* mask_tile, int mask_off) {
+                                                   uint8_t* mask_tile, int mask_off, const float* __restrict__ bias8 = nullptr) {
   const int r0 = g * kWgRows + acc_r0(), q = acc_q();
   ReluMask<kMaskHCols> m;
   if constexpr (TRAIN) m.clear();
 #pragma unroll
   for (int j = 0; j < kMaskHCols / 8; ++j) {
     const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * q));
+    float2 b8 = b;
+    if constexpr (ROW_BIAS) b8 = __ldg(reinterpret_cast<const float2*>(bias8 + 8 * j + 2 * q));
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-      const uint32_t h2 = pack_h2_relu_sat(acc[4 * j + 2 * i] + b.x, acc[4 * j + 2 * i + 1] + b.y);
+      const float2 bi = i ? b8 : b;
+      const uint32_t h2 = pack_h2_relu_sat(acc[4 * j + 2 * i] + bi.x, acc[4 * j + 2 * i + 1] + bi.y);
       frag_pair(a, j, i) = h2;
       if constexpr (TRAIN) {
         m.pack(i, j, h2);
@@ -137,9 +142,12 @@ __device__ __forceinline__ void write_pe(const float (&x)[3], uint8_t* dst_row) 
 
 }  // namespace
 
-// TRAIN: p.stash and p.relu_mask are given (the inference kernel carries none of the mask code)
-template <bool HAS_BENDER, bool TRAIN>
-__global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFwdParams p) {
+// TRAIN: p.stash and p.relu_mask are given (the inference kernel carries none of the mask code).
+// LATENT_BIAS (time-conditioned baseline, no bender): the L0 and L5 epilogues add the ray-bias rows p.ray_bias of their
+// rows' rays instead of the layers' bias vectors.
+template <bool HAS_BENDER, bool TRAIN, bool LATENT_BIAS>
+__device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p) {
+  static_assert(!(HAS_BENDER && LATENT_BIAS), "the time-conditioned baseline has no bender");
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* act = smem;                                  // H (bender) | E, 128 rows
   uint8_t* ring_buf = smem + kFwdHBytes + kEBytes;      // kFwdRingStages x 32 KB
@@ -301,12 +309,25 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
     sw.ready(kStE, Es);
     // ---- L0 .. L7 (every one 256 wide): L0 reads E, every later step its A fragments h (L5: E first, then h) ----
     uint32_t h[kMaskHCols / 16][4];
+    // LATENT_BIAS: the rays of this thread's accumulator rows r0 and r0 + 8 (rows past P take the last point's)
+    int ray_r0 = 0, ray_r8 = 0;
+    if constexpr (LATENT_BIAS) {
+      const long long r0 = static_cast<long long>(tile) * kTileM + g * kWgRows + acc_r0();
+      ray_r0 = static_cast<int>(min(r0, p.P - 1) / p.S);
+      ray_r8 = static_cast<int>(min(r0 + 8, p.P - 1) / p.S);
+    }
 #pragma unroll 1
     for (int L = 0; L < 8; ++L) {
       Acc<fwd::L1> acc;
       if (L == 0) wg_gemm_step<fwd::L0>(acc, ring, [&](uint32_t) { return a_e; }, W, 310);
       else wg_gemm_rs<fwd::step(fwd::L1).N, fwd::step(fwd::L1).k16>(acc, h, ring, L == 5, a_e, W, 310 + L);
-      epi_bias_relu_frag<TRAIN>(acc, p.nerf_bias + L * fwd::b_off(fwd::L1), h, st + st_h(L + 1).off, g, mk, kMkH + L * kMaskHBytes);
+      if (LATENT_BIAS && (L == 0 || L == 5)) {
+        const float* rb = p.ray_bias + (L == 5 ? fwd::b_off(fwd::L1) : 0);
+        epi_bias_relu_frag<TRAIN, true>(acc, rb + ray_r0 * p.ray_bias_stride, h, st + st_h(L + 1).off, g, mk, kMkH + L * kMaskHBytes,
+                                        rb + ray_r8 * p.ray_bias_stride);
+      } else {
+        epi_bias_relu_frag<TRAIN>(acc, p.nerf_bias + L * fwd::b_off(fwd::L1), h, st + st_h(L + 1).off, g, mk, kMkH + L * kMaskHBytes);
+      }
     }
     // ---- head: raw = output_linear(h) (run_nerf_helpers.py:306) ----
     {
@@ -329,6 +350,47 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFw
   if (p.stash && wg_leader) tma_bulk_wait<0>();   // all stash stores complete before the CTA exits
 }
 
+template <bool HAS_BENDER, bool TRAIN>
+__global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFwdParams p) { field_fwd_body<HAS_BENDER, TRAIN, false>(p); }
+template <bool TRAIN>
+__global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_tc_kernel(const FieldFwdParams p) { field_fwd_body<false, TRAIN, true>(p); }
+
+// Ray bias of the time-conditioned baseline: rb[n][l][o] = b_l[o] + sum_k W_l[o][63 + k] z[n][k] for l = L0, L5, in fp32
+// from the nn.Linear weights (W0 [256][95], W5 [256][351]).  Thread o of a block keeps both layers' 32 latent weights
+// of row o in registers and walks kTcRaysPerBlock rays.
+constexpr int kTcRaysPerBlock = 16;
+__global__ void __launch_bounds__(256) tc_latent_bias_kernel(const float* __restrict__ lat, long long lat_stride, int n_rays,
+                                                             const float* __restrict__ w0, const float* __restrict__ b0,
+                                                             const float* __restrict__ w5, const float* __restrict__ b5,
+                                                             float* __restrict__ rb) {
+  __shared__ float zs[kTcRaysPerBlock][kLatent];
+  const int o = threadIdx.x;
+  const int n0 = blockIdx.x * kTcRaysPerBlock;
+  for (int i = threadIdx.x; i < kTcRaysPerBlock * kLatent; i += blockDim.x) {
+    const int r = n0 + i / kLatent;
+    zs[i / kLatent][i % kLatent] = r < n_rays ? __ldg(lat + r * lat_stride + i % kLatent) : 0.f;
+  }
+  float wa[kLatent], wb[kLatent];
+#pragma unroll
+  for (int k = 0; k < kLatent; ++k) {
+    wa[k] = __ldg(w0 + o * (kPeCols + kLatent) + kPeCols + k);
+    wb[k] = __ldg(w5 + o * (kPeCols + kLatent + 256) + kPeCols + k);
+  }
+  const float ba = __ldg(b0 + o), bb = __ldg(b5 + o);
+  __syncthreads();
+  for (int i = 0; i < kTcRaysPerBlock && n0 + i < n_rays; ++i) {
+    float sa = 0.f, sb = 0.f;
+#pragma unroll
+    for (int k = 0; k < kLatent; ++k) {
+      sa = fmaf(wa[k], zs[i][k], sa);
+      sb = fmaf(wb[k], zs[i][k], sb);
+    }
+    float* dst = rb + static_cast<long long>(n0 + i) * 512;
+    dst[o] = ba + sa;
+    dst[256 + o] = bb + sb;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 size_t field_fwd_smem_bytes() { return kFwdSmemBytes; }
 
@@ -337,6 +399,17 @@ cudaError_t launch_field_fwd(const FieldFwdParams& p, bool has_bender, int num_s
   const bool train = p.relu_mask != nullptr;   // the C ABI passes the ReLU masks exactly when it passes the stash
   if (has_bender) return launch_field(train ? field_fwd_kernel<true, true> : field_fwd_kernel<true, false>, p, num_sms, smem, stream);
   return launch_field(train ? field_fwd_kernel<false, true> : field_fwd_kernel<false, false>, p, num_sms, smem, stream);
+}
+
+cudaError_t launch_field_fwd_tc(const FieldFwdParams& p, int num_sms, cudaStream_t stream) {
+  const bool train = p.relu_mask != nullptr;
+  return launch_field(train ? field_fwd_tc_kernel<true> : field_fwd_tc_kernel<false>, p, num_sms, field_fwd_smem_bytes(), stream);
+}
+
+cudaError_t launch_tc_latent_bias(const float* lat, long long lat_stride, int n_rays, const float* w0, const float* b0, const float* w5,
+                                  const float* b5, float* rb, cudaStream_t stream) {
+  tc_latent_bias_kernel<<<(n_rays + kTcRaysPerBlock - 1) / kTcRaysPerBlock, 256, 0, stream>>>(lat, lat_stride, n_rays, w0, b0, w5, b5, rb);
+  return cudaGetLastError();
 }
 
 }  // namespace nrn

@@ -174,6 +174,12 @@ __host__ __device__ constexpr int floats(int i) { return kShape[i][0] * kShape[i
 __host__ __device__ constexpr int total() { int n = 0; for (int i = 0; i < kCount; ++i) n += floats(i); return n; }
 }  // namespace bparam
 static_assert(nerf_grad_floats(4) == 494084 && nerf_grad_floats(5) == 494341 && bparam::total() == 16193, "gradient buffers");
+// Time-conditioned baseline (NeRF(time_conditioned_baseline=True), no bender): L0 reads [PE(63) | z(32)] and L5
+// [PE(63) | z(32) | h(256)], so its flat buffer has W0[256][95] and W5[256][351].  The latent z is the same for every
+// sample of a ray, so the kernels keep the geometry above and fold W_l[:, 63:95] . z + b_l into one fp32 bias row per ray
+// and layer (L0, L5): the "ray bias" [rays][2][256].
+__host__ __device__ constexpr int nerf_tc_grad_floats(int out_ch) { return nerf_grad_floats(out_ch) + 2 * 256 * kLatent; }
+static_assert(nerf_tc_grad_floats(5) == 510725, "time-conditioned gradient buffer");
 
 struct FieldBwdParams {
   long long P;
@@ -224,6 +230,24 @@ struct FieldFwdParams {
   uint8_t* stash;         // training stash [n_tiles rounded up to even][kStashTileBytes] or null
   int* err;               // device error word (0 = ok)
   uint8_t* relu_mask;     // training only (with stash): ReLU masks [n_tiles rounded up to even][kMaskTileBytes]
+  const float* ray_bias;  // time-conditioned kernels only: [ray][2][256] biases of L0 / L5 (stride ray_bias_stride floats,
+  long long ray_bias_stride;   // 0 = one row for every ray); the other kernels ignore both
+};
+
+// Time-conditioned backward: the per-ray sums s_l[ray] = sum over the ray's samples of dY_l (l = L0, L5), d z and the
+// latent columns of dW0 / dW5 (field_bwd.cu).
+struct TcBwdParams {
+  const uint8_t* gstash;       // gradient stash written by DGRAD
+  const float* amax;           // loss-scale source of that DGRAD run
+  long long P;
+  int S, n_rays;
+  const float* latents;        // [n_rays][32], row stride latent_stride floats (0 = one row for all)
+  long long latent_stride;
+  const float* w0;             // fp32 W0 [256][95]
+  const float* w5;             // fp32 W5 [256][351]
+  float* sums;                 // workspace [n_rays][2][256]
+  float* d_latents;            // out [n_rays][32]
+  float* dw_lat;               // out [2][256][32]: dW0[:, 63:95], dW5[:, 63:95]
 };
 
 }  // namespace nrn

@@ -19,7 +19,11 @@ __device__ __forceinline__ void decode(int idx, int R, int& k, int& r) {
   k = c * 8 + (rem & 7);
 }
 
+// TC (time-conditioned baseline, in_ch = 63 + 32): W0 / W5 carry the latent columns 63-94 behind the embedding; they are
+// skipped (they enter the kernels as a per-ray bias), so the images are the same as for in_ch = 63.
+template <bool TC>
 __device__ __forceinline__ void pack_nerf_elem(const int idx, const NerfSrc& src, int in_ch, int out_ch, __half* __restrict__ w, float* __restrict__ bias) {
+  const int pe = TC ? kPeCols : in_ch;   // embedding columns
   constexpr WImage w0 = fwd::image(fwd::L0), wl = fwd::image(fwd::L1), w5 = fwd::image(fwd::L5), wh = fwd::image(fwd::Head);
   constexpr int n0 = w0.bytes() / 2, nl = wl.bytes() / 2, n5 = w5.bytes() / 2;
   if (idx < kNerfWBytes / 2) {
@@ -27,7 +31,7 @@ __device__ __forceinline__ void pack_nerf_elem(const int idx, const NerfSrc& src
     float v = 0.f;
     if (i < n0) {  // L0: K = in_ch (63) padded to 64
       decode(i, w0.rows, k, r);
-      v = k < in_ch ? src.w[0][r * in_ch + k] : 0.f;
+      v = k < pe ? src.w[0][r * in_ch + k] : 0.f;
     } else if ((i -= n0) < 4 * nl) {  // L1..L4
       const int L = 1 + i / nl;
       decode(i % nl, wl.rows, k, r);
@@ -35,7 +39,7 @@ __device__ __forceinline__ void pack_nerf_elem(const int idx, const NerfSrc& src
     } else if ((i -= 4 * nl) < n5) {  // L5: [embedding(in_ch) pad | h(256)]
       decode(i, w5.rows, k, r);
       const int ld = in_ch + 256;
-      if (k < 8 * w0.chunks) v = k < in_ch ? src.w[5][r * ld + k] : 0.f;
+      if (k < 8 * w0.chunks) v = k < pe ? src.w[5][r * ld + k] : 0.f;
       else v = src.w[5][r * ld + in_ch + (k - 8 * w0.chunks)];
     } else if ((i -= n5) < 2 * nl) {  // L6, L7
       const int L = 6 + i / nl;
@@ -110,8 +114,10 @@ __device__ __forceinline__ void pack_bender_elem(const int idx, const BenderSrc&
 
 // ---- transposed images for DGRAD: W^T (rows = input features, K = output features), layout in nrn_common.cuh ----
 // r = input feature, k = output feature
+template <bool TC>
 __device__ __forceinline__ void pack_nerf_t_elem(const int idx, const NerfSrc& src, int in_ch, int out_ch, __half* __restrict__ w) {
   if (idx >= kNerfTWBytes / 2) return;
+  const int pe = TC ? kPeCols : in_ch;
   constexpr WImage wh = dgrad::image(dgrad::HeadT), wl = dgrad::image(dgrad::L7T), we = dgrad::image(dgrad::L5eT), w0 = dgrad::image(dgrad::L0T);
   constexpr int nh = wh.bytes() / 2, nl = wl.bytes() / 2, ne = we.bytes() / 2;
   int i = idx, k, r;
@@ -126,7 +132,7 @@ __device__ __forceinline__ void pack_nerf_t_elem(const int idx, const NerfSrc& s
     v = src.w[L][k * 256 + r];
   } else if ((i -= 2 * nl) < ne) {        // L5e^T: rows = embedding inputs (in_ch, padded to 64)
     decode(i, we.rows, k, r);
-    v = r < in_ch ? src.w[5][k * ld5 + r] : 0.f;
+    v = r < pe ? src.w[5][k * ld5 + r] : 0.f;
   } else if ((i -= ne) < nl) {            // L5h^T
     decode(i, wl.rows, k, r);
     v = src.w[5][k * ld5 + in_ch + r];
@@ -137,7 +143,7 @@ __device__ __forceinline__ void pack_nerf_t_elem(const int idx, const NerfSrc& s
   } else {                                // L0^T
     i -= 4 * nl;
     decode(i, w0.rows, k, r);
-    v = r < in_ch ? src.w[0][k * in_ch + r] : 0.f;
+    v = r < pe ? src.w[0][k * in_ch + r] : 0.f;
   }
   w[idx] = __float2half_rn(v);
 }
@@ -180,8 +186,15 @@ constexpr int kPackThreads = 256;
 __global__ void __launch_bounds__(kPackThreads) pack_nerf_kernel(NerfSrc src, int in_ch, int out_ch, __half* __restrict__ w,
                                                                  float* __restrict__ bias, __half* __restrict__ wt) {
   constexpr int nb_fwd = (kNerfWBytes / 2 + kPackThreads - 1) / kPackThreads;
-  if (blockIdx.x < nb_fwd) pack_nerf_elem(blockIdx.x * kPackThreads + threadIdx.x, src, in_ch, out_ch, w, bias);
-  else pack_nerf_t_elem((blockIdx.x - nb_fwd) * kPackThreads + threadIdx.x, src, in_ch, out_ch, wt);
+  if (blockIdx.x < nb_fwd) pack_nerf_elem<false>(blockIdx.x * kPackThreads + threadIdx.x, src, in_ch, out_ch, w, bias);
+  else pack_nerf_t_elem<false>((blockIdx.x - nb_fwd) * kPackThreads + threadIdx.x, src, in_ch, out_ch, wt);
+}
+__global__ void __launch_bounds__(kPackThreads) pack_nerf_tc_kernel(NerfSrc src, int out_ch, __half* __restrict__ w,
+                                                                    float* __restrict__ bias, __half* __restrict__ wt) {
+  constexpr int nb_fwd = (kNerfWBytes / 2 + kPackThreads - 1) / kPackThreads;
+  constexpr int in_ch = kPeCols + kLatent;
+  if (blockIdx.x < nb_fwd) pack_nerf_elem<true>(blockIdx.x * kPackThreads + threadIdx.x, src, in_ch, out_ch, w, bias);
+  else pack_nerf_t_elem<true>((blockIdx.x - nb_fwd) * kPackThreads + threadIdx.x, src, in_ch, out_ch, wt);
 }
 __global__ void __launch_bounds__(kPackThreads) pack_bender_kernel(BenderSrc src, __half* __restrict__ w, float* __restrict__ bias,
                                                                    __half* __restrict__ wt, __half* __restrict__ wlo,
@@ -197,8 +210,12 @@ __global__ void __launch_bounds__(kPackThreads) pack_bender_kernel(BenderSrc src
 cudaError_t launch_pack_nerf(const NerfSrc& src, int in_ch, int out_ch, void* packed, cudaStream_t st) {
   uint8_t* base = reinterpret_cast<uint8_t*>(packed);
   const int nb = (kNerfWBytes / 2 + kPackThreads - 1) / kPackThreads + (kNerfTWBytes / 2 + kPackThreads - 1) / kPackThreads;
-  pack_nerf_kernel<<<nb, kPackThreads, 0, st>>>(src, in_ch, out_ch, reinterpret_cast<__half*>(base),
-                                               reinterpret_cast<float*>(base + kNerfWBytes), reinterpret_cast<__half*>(base + kNerfTOffset));
+  if (in_ch == kPeCols + kLatent)   // time-conditioned baseline: [embedding | latent] inputs
+    pack_nerf_tc_kernel<<<nb, kPackThreads, 0, st>>>(src, out_ch, reinterpret_cast<__half*>(base), reinterpret_cast<float*>(base + kNerfWBytes),
+                                                     reinterpret_cast<__half*>(base + kNerfTOffset));
+  else
+    pack_nerf_kernel<<<nb, kPackThreads, 0, st>>>(src, in_ch, out_ch, reinterpret_cast<__half*>(base),
+                                                 reinterpret_cast<float*>(base + kNerfWBytes), reinterpret_cast<__half*>(base + kNerfTOffset));
   return cudaGetLastError();
 }
 cudaError_t launch_pack_bender(const BenderSrc& src, void* packed, cudaStream_t st) {

@@ -344,12 +344,24 @@ __device__ __forceinline__ Src bend_w(int job, int sub, int m, int n, int n2 = -
   return {job, sub * 16384 + m * 128 + n, n2 >= 0 ? sub * 16384 + m * 128 + n2 : -1, 0};
 }
 
+// TC (time-conditioned baseline): W0 [256][63 + 32], W5 [256][63 + 32 + 256]; the latent columns come from
+// tc_dw_lat_kernel (field_bwd.cu) as Src{kLatJob, index into its [2][256][32] output}.
+constexpr int kLatJob = -1;
+template <bool TC = false>
 __device__ __forceinline__ Src nerf_src(int idx, int out_ch, bool& ok) {
   ok = true;
-  constexpr int in0 = nerf_in(0), in5 = nerf_in(5);   // L0: the embedding; L5: [embedding | h]
+  constexpr int lat = TC ? kLatent : 0;
+  constexpr int in0 = nerf_in(0) + lat, in5 = nerf_in(5) + lat;   // L0: the embedding (| z); L5: [embedding (| z) | h]
+  constexpr int pe = nerf_in(0);
   const int sz0 = 256 * in0 + 256, szl = 256 * 256 + 256, sz5 = 256 * in5 + 256;
   if (idx < sz0) {
-    if (idx < 256 * in0) return nerf_w(9, idx / in0, idx % in0);
+    if (idx < 256 * in0) {
+      if constexpr (TC) {
+        const int m = idx / in0, k = idx % in0;
+        if (k >= pe) return {kLatJob, m * kLatent + (k - pe), -1, 0};
+      }
+      return nerf_w(9, idx / in0, idx % in0);
+    }
     return nerf_b(9, idx - 256 * in0);
   }
   idx -= sz0;
@@ -359,7 +371,10 @@ __device__ __forceinline__ Src nerf_src(int idx, int out_ch, bool& ok) {
       if (l == 5) {
         if (idx < 256 * in5) {
           const int m = idx / in5, k = idx % in5;
-          return k < in0 ? nerf_w(8, m, k) : nerf_w(5, m, k - in0);
+          if constexpr (TC) {
+            if (k >= pe && k < pe + lat) return {kLatJob, (256 + m) * kLatent + (k - pe), -1, 0};
+          }
+          return k < pe ? nerf_w(8, m, k) : nerf_w(5, m, k - (pe + lat));
         }
         return nerf_b(5, idx - 256 * in5);
       }
@@ -423,15 +438,17 @@ __device__ __forceinline__ Src bender_src(int idx, bool& ok) {
 
 }  // namespace
 
-__global__ void wgrad_reduce_kernel(const WgradParams p, const WgradDst dst, int out_ch) {
+template <bool TC>
+__device__ __forceinline__ void wgrad_reduce(const WgradParams p, const WgradDst dst, int out_ch, const float* dw_lat) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   const int nerf_n = dst.nerf_n, bend_n = dst.bend_n;
   if (idx >= nerf_n + bend_n) return;
   bool ok;
-  const Src s = idx < nerf_n ? nerf_src(idx, out_ch, ok) : bender_src(idx - nerf_n, ok);
+  const Src s = idx < nerf_n ? nerf_src<TC>(idx, out_ch, ok) : bender_src(idx - nerf_n, ok);
   const float scale = loss_scale(p.amax);
   float sum = 0.f;
-  if (ok && !(s.bias && p.compact)) {
+  const bool lat = TC && s.job == kLatJob;   // tc_dw_lat_kernel's sums: already divided by the loss scale
+  if (ok && !lat && !(s.bias && p.compact)) {
     int base = 0, slot = -1;
     for (int j = 0; j < p.n_jobs; ++j) {
       if (p.job_ids[j] == s.job) { slot = j; break; }
@@ -467,7 +484,7 @@ __global__ void wgrad_reduce_kernel(const WgradParams p, const WgradDst dst, int
       }
     }
   }
-  const float v = sum / scale;
+  const float v = lat ? __ldg(dw_lat + s.off) : sum / scale;
   float* out;
   bool acc;
   if (idx < nerf_n) {
@@ -481,8 +498,14 @@ __global__ void wgrad_reduce_kernel(const WgradParams p, const WgradDst dst, int
   *out = acc ? *out + v : v;
 }
 
+__global__ void wgrad_reduce_kernel(const WgradParams p, const WgradDst dst, int out_ch) { wgrad_reduce<false>(p, dst, out_ch, nullptr); }
+__global__ void wgrad_reduce_tc_kernel(const WgradParams p, const WgradDst dst, int out_ch, const float* dw_lat) {
+  wgrad_reduce<true>(p, dst, out_ch, dw_lat);
+}
+
 // ------------------------------------------------------------------------------------------------
-cudaError_t launch_wgrad(WgradParams p, bool has_bender, int num_sms, const WgradDst& dst, int out_ch, cudaStream_t st) {
+cudaError_t launch_wgrad(WgradParams p, bool has_bender, int num_sms, const WgradDst& dst, int out_ch, cudaStream_t st,
+                         const float* tc_dw_lat) {
   // relative cost of one tile of every job's CTAs = 2 KB chunks a CTA receives (a NeRF layer's half: 16 gradient
   // chunks + the activation block); the head job and the three-MMA bender job stream a little slower per byte, hence
   // their surcharge.  The plan decides how the fp32 partial sums associate: changing a weight changes the gradients'
@@ -551,7 +574,8 @@ cudaError_t launch_wgrad(WgradParams p, bool has_bender, int num_sms, const Wgra
     if (e != cudaSuccess) return e;
   }
   const int n = dst.nerf_n + dst.bend_n;
-  if (n > 0) wgrad_reduce_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, dst, out_ch);
+  if (n > 0 && tc_dw_lat) wgrad_reduce_tc_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, dst, out_ch, tc_dw_lat);
+  else if (n > 0) wgrad_reduce_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, dst, out_ch);
   return cudaGetLastError();
 }
 

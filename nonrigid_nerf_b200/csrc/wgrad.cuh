@@ -32,7 +32,10 @@ struct WgradDst {
   int nerf_n, bend_n;
   int acc_nerf, acc_bend;
 };
-cudaError_t launch_wgrad(WgradParams p, bool has_bender, int num_sms, const WgradDst& dst, int out_ch, cudaStream_t st);
+// tc_dw_lat: time-conditioned layout (nerf_tc_grad_floats), the latent columns of W0 / W5 read from this [2][256][32]
+// buffer (tc_dw_lat_kernel, field_bwd.cu)
+cudaError_t launch_wgrad(WgradParams p, bool has_bender, int num_sms, const WgradDst& dst, int out_ch, cudaStream_t st,
+                         const float* tc_dw_lat = nullptr);
 // amax[0] = max |x[i]| over n floats (device scalar, overwritten; accumulate: max with its value).  x as rows of
 // `row_len` floats: only the first `cols` of every row take part.
 cudaError_t launch_absmax(const float* x, long long n, float* amax, cudaStream_t st, bool accumulate = false, int row_len = 1,

@@ -80,13 +80,14 @@ def pack_nerf(net) -> torch.Tensor:
     for t in ws + bs:
         if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
             raise RuntimeError("nonrigid_nerf_b200: NeRF parameters must be contiguous fp32 CUDA tensors")
-    if ws[0].shape != (256, 63) or ws[5].shape != (256, 319) or ws[8].shape[1] != 256:
+    in_ch = 63 + (LATENT if getattr(net, "time_conditioned_baseline", False) else 0)   # [embedding (| latent)]
+    if ws[0].shape != (256, in_ch) or ws[5].shape != (256, in_ch + 256) or ws[8].shape[1] != 256:
         raise RuntimeError("nonrigid_nerf_b200: only D=8, W=256, skips=[4], multires=10, use_viewdirs=False is implemented "
                            f"(got layer shapes {[tuple(w.shape) for w in ws]})")
     buf = cache[1] if cache is not None else torch.empty(lib.nrn_packed_nerf_bytes(), dtype=torch.uint8, device=ws[0].device)
     out_ch = ws[8].shape[0]
     with torch.cuda.device(ws[0].device):
-        _lib.check(lib.nrn_pack_nerf(_ptr_array([w.detach() for w in ws]), _ptr_array([b.detach() for b in bs]), 63, out_ch,
+        _lib.check(lib.nrn_pack_nerf(_ptr_array([w.detach() for w in ws]), _ptr_array([b.detach() for b in bs]), in_ch, out_ch,
                                      _ptr(buf), _stream()), "pack_nerf")
     net._nrn_pack = (key, buf)
     return buf
@@ -130,7 +131,37 @@ def sample_coarse(rays: torch.Tensor, n_samples: int, t_rand: Optional[torch.Ten
     return z
 
 
-def _field(rays, z_vals, points, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details, stash=None, relu_mask=None):
+def latent_rows(latents: torch.Tensor, n: int, dev) -> Tuple[torch.Tensor, int]:
+    """The [n, 32] fp32 latents as the kernels read them, and their row stride in floats (0: one row for every ray).
+    An expanded (stride-0) latent row is passed as a broadcast instead of being materialised; a column slice of a wider
+    row-major matrix (run_network's [P, 95] input) is read in place."""
+    if latents.dtype != torch.float32 or not latents.is_cuda:
+        latents = latents.float().to(dev)
+    if not (latents.dim() == 2 and latents.shape[0] == n and latents.stride(1) == 1):
+        latents = latents.reshape(n, -1).contiguous()
+    if latents.shape[-1] != LATENT:
+        raise RuntimeError(f"nonrigid_nerf_b200: latent size {latents.shape[-1]} unsupported (32)")
+    return latents, (latents.stride(0) if n > 1 else 0)
+
+
+def tc_ray_bias(net, latents: torch.Tensor, stride: int) -> torch.Tensor:
+    """Time-conditioned baseline: the per-ray biases of L0 and L5, rb[n][l] = b_l + W_l[:, 63:95] . z[n] (fp32, from the
+    nn.Linear weights); one row when stride == 0."""
+    w0, b0 = net.pts_linears[0].weight, net.pts_linears[0].bias
+    w5, b5 = net.pts_linears[5].weight, net.pts_linears[5].bias
+    for t in (w0, b0, w5, b5):
+        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
+            raise RuntimeError("nonrigid_nerf_b200: NeRF parameters must be contiguous fp32 CUDA tensors")
+    rows = 1 if stride == 0 else latents.shape[0]
+    rb = torch.empty(rows, 2, 256, dtype=torch.float32, device=latents.device)
+    with torch.cuda.device(latents.device):
+        _lib.check(_lib.load().nrn_tc_latent_bias(_ptr(latents), stride, rows, _ptr(w0.detach()), _ptr(b0.detach()), _ptr(w5.detach()),
+                                                  _ptr(b5.detach()), _ptr(rb), _stream()), "tc_latent_bias")
+    return rb
+
+
+def _field(rays, z_vals, points, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details, stash=None, relu_mask=None,
+           tc_net=None):
     a = _lib.NrnFieldArgs()
     keep = []
     if points is None:
@@ -151,20 +182,21 @@ def _field(rays, z_vals, points, latents, nerf_pack, bender_pack, out_ch, cutoff
         keep.append(points)
     a.n_rays, a.n_samples = n, s
     a.nerf_packed = nerf_pack.data_ptr()
+    ray_bias = None
     if bender_pack is not None:
         if latents is None:
             raise RuntimeError("nonrigid_nerf_b200: ray bending needs latents")
-        if latents.dtype != torch.float32 or not latents.is_cuda:
-            latents = latents.float().to(dev)
-        # an expanded (stride-0) latent row is passed as a broadcast instead of being materialised;
-        # a column slice of a wider row-major matrix (run_network's [P, 95] input) is read in place
-        if not (latents.dim() == 2 and latents.shape[0] == n and latents.stride(1) == 1):
-            latents = latents.reshape(n, -1).contiguous()
-        if latents.shape[-1] != LATENT:
-            raise RuntimeError(f"nonrigid_nerf_b200: latent size {latents.shape[-1]} unsupported (32)")
-        a.latents, a.latent_stride = latents.data_ptr(), (latents.stride(0) if n > 1 else 0)
+        latents, stride = latent_rows(latents, n, dev)
+        a.latents, a.latent_stride = latents.data_ptr(), stride
         a.bender_packed = bender_pack.data_ptr()
         keep.append(latents)
+    elif tc_net is not None:   # time-conditioned baseline: the latents enter as per-ray biases of L0 and L5
+        if latents is None:
+            raise RuntimeError("nonrigid_nerf_b200: time_conditioned_baseline needs latents")
+        latents, stride = latent_rows(latents, n, dev)
+        a.latents, a.latent_stride = latents.data_ptr(), stride
+        ray_bias = tc_ray_bias(tc_net, latents, stride)
+        keep += [latents, ray_bias]
     a.out_ch = out_ch
     if cutoff is not None:
         a.use_cutoff, a.rigidity_cutoff = 1, float(cutoff)
@@ -192,7 +224,10 @@ def _field(rays, z_vals, points, latents, nerf_pack, bender_pack, out_ch, cutoff
         a.relu_mask = relu_mask.data_ptr()
     a.stream = torch.cuda.current_stream().cuda_stream
     with torch.cuda.device(dev):
-        _lib.check(_lib.load().nrn_field_forward(C.byref(a)), "field_forward")
+        if ray_bias is not None:
+            _lib.check(_lib.load().nrn_field_forward_tc(C.byref(a), _ptr(ray_bias)), "field_forward_tc")
+        else:
+            _lib.check(_lib.load().nrn_field_forward(C.byref(a)), "field_forward")
     return raw, details
 
 
@@ -200,19 +235,21 @@ def field_forward(rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[to
                   bender_pack: Optional[torch.Tensor], out_ch: int, cutoff: Optional[float] = None,
                   scaling: Optional[float] = None, removal: Optional[float] = None,
                   want_details: bool = False, stash: Optional[torch.Tensor] = None,
-                  relu_mask: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
+                  relu_mask: Optional[torch.Tensor] = None, tc_net=None) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
     """One fused pass over rays x samples: raw [N, S, out_ch] (+ the reference's per-point `details`).
     `stash` (uint8, nrn_stash_bytes) with `relu_mask` (uint8, nrn_relu_mask_bytes) switches the kernel to training mode
-    (activations and ReLU masks kept for backward)."""
+    (activations and ReLU masks kept for backward).  `tc_net`: the time-conditioned NeRF whose L0 / L5 weights turn
+    `latents` into per-ray biases (no bender)."""
     return _field(rays, z_vals, None, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details, stash,
-                  relu_mask)
+                  relu_mask, tc_net)
 
 
 def field_forward_points(points: torch.Tensor, latents: Optional[torch.Tensor], nerf_pack: torch.Tensor,
                          bender_pack: Optional[torch.Tensor], out_ch: int, cutoff=None, scaling=None, removal=None,
-                         want_details: bool = False) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
+                         want_details: bool = False, tc_net=None) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
     """Point mode (NeRF.forward(x)): one xyz (+ one latent) per row; returns raw [P, 1, out_ch]."""
-    return _field(None, None, points, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details)
+    return _field(None, None, points, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details,
+                  tc_net=tc_net)
 
 
 def composite(raw: torch.Tensor, z_vals: torch.Tensor, rays_d: torch.Tensor, noise: Optional[torch.Tensor] = None,

@@ -138,8 +138,9 @@ class NeRF(nn.Module):
         super().__init__()
         if use_viewdirs:
             raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True is not implemented yet (SURVEY.md 8f row f1)")
-        if time_conditioned_baseline:
-            raise RuntimeError("nonrigid_nerf_b200: time_conditioned_baseline is not implemented")
+        if time_conditioned_baseline and ray_bending_latent_size != ops.LATENT:
+            raise RuntimeError("nonrigid_nerf_b200: time_conditioned_baseline needs ray_bending_latent_size=32 "
+                               f"(got {ray_bending_latent_size})")
         if D != 8 or W != 256 or list(skips) != [4] or input_ch != 63:
             raise RuntimeError("nonrigid_nerf_b200: only netdepth=8, netwidth=256, skips=[4], multires=10 is implemented")
         self.D, self.W = D, W
@@ -153,8 +154,12 @@ class NeRF(nn.Module):
         self.time_conditioned_baseline = time_conditioned_baseline
         self.ray_bending_latent_size = ray_bending_latent_size
         self.ray_bender = (ray_bender,)  # 1-tuple: keeps the bender out of NeRF.parameters() (run_nerf_helpers.py:213-215)
-        self.pts_linears = nn.ModuleList([nn.Linear(input_ch, W)] + [nn.Linear(W, W) if i not in skips else nn.Linear(W + input_ch, W)
-                                                                      for i in range(D - 1)])
+        # naive NR-NeRF baseline (run_nerf_helpers.py:206-209): the per-frame latent joins the embedding at layer 0 and at the
+        # skip layer, so those layers take 63 + 32 and 63 + 32 + 256 inputs.  The kernels fold the latent columns into a
+        # per-ray bias of both layers (csrc/field_fwd.cu).
+        lin_in = input_ch + (ray_bending_latent_size if time_conditioned_baseline else 0)
+        self.pts_linears = nn.ModuleList([nn.Linear(lin_in, W)] + [nn.Linear(W, W) if i not in skips else nn.Linear(W + lin_in, W)
+                                                                    for i in range(D - 1)])
         self.views_linears = nn.ModuleList([nn.Linear(input_ch_views + W, W // 2)])  # dead weight, kept for checkpoints
         self.output_linear = nn.Linear(W, output_ch)
 

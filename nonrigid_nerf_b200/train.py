@@ -89,7 +89,7 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     rays = ray_batch if (ray_batch.dtype == torch.float32 and ray_batch.is_contiguous()) else ray_batch.float().contiguous()
     rays_d = rays[:, 3:6]
     latents = None
-    if network_fn.ray_bender[0] is not None:
+    if network_fn.ray_bender[0] is not None or getattr(network_fn, "time_conditioned_baseline", False):
         latents = additional_pixel_information["ray_bending_latents"]
 
     rnd = dummy_kwargs.get("randomness", None)
