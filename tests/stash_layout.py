@@ -100,10 +100,12 @@ def loss_scale(amax):
 
 
 # Flat parameter maps of the weight-gradient buffers (wgrad.cu, wgrad_reduce_kernel): (name, shape) in order
-def nerf_param_shapes(out_ch):
-    shapes = [("w0", (256, 63)), ("b0", (256,))]
+def nerf_param_shapes(out_ch, tc=False):
+    """tc: the time-conditioned layout (nrn_nerf_tc_grad_floats), W0 [256][63 + 32] and W5 [256][63 + 32 + 256]."""
+    in_ch = 63 + (32 if tc else 0)
+    shapes = [("w0", (256, in_ch)), ("b0", (256,))]
     for l in range(1, 8):
-        shapes += [(f"w{l}", (256, 319 if l == 5 else 256)), (f"b{l}", (256,))]
+        shapes += [(f"w{l}", (256, in_ch + 256 if l == 5 else 256)), (f"b{l}", (256,))]
     return shapes + [("w_out", (out_ch, 256)), ("b_out", (out_ch,))]
 
 

@@ -16,8 +16,19 @@ The divergence kernels are checked against the full tangent / adjoint chains in 
 weights at c = 64 (eta = 2^-18): their hi/lo split is meant to be fp32-accurate, and plain fp16 operands (about 4e-4)
 fail this by orders of magnitude.
 
-Measured on one H100 80GB HBM3: the worst observed ratio of each stage (|kernel - exact| - rounding) / (2^-24 |A||W|)
-is printed with `pytest -s` ("c_obs"); every c above has at least 4x margin over the largest c_obs of its stage.
+The time-conditioned baseline (TC: no bender, the latent z enters L0 and L5 as a per-ray bias) adds these checks:
+  ray bias rb[ray][l] = b_l + W_l[:, 63:95] z    fp32 weights and latents, c = 34 on |b| + |W||z|
+  H1, H6 (L0, L5)      each accumulator row adds rb of its own ray, min(row, P - 1) // S; c_mma(K) on |A||W| + |rb|
+  per-ray sums         sum of the decoded dY0 / dY5 over the ray's samples / loss scale, c = S + 2
+  d z                  from the kernel's own sums and the fp32 W0 / W5 latent columns, c = 514
+  dW0 / dW5[:, 63:95]  from the kernel's own sums, c = 4 (n + 2): n fp32 FMAs, whose worst case few rays nearly reach
+and WGRAD checks the whole TC gradient layout (W0 [256][95], W5 [256][351]) as above.
+
+Measured on one H100 80GB HBM3 (700 W power limit): the worst observed ratio of each stage (|kernel - exact| - rounding)
+/ (2^-24 |A||W|) is printed with `pytest -s` ("c_obs"); every c above has at least 4x margin over the largest c_obs of its
+stage.  The worst TC c_obs: ray bias 4.48 (1023 x 64), H1 1.55 and H6 8.30 (1024 x 128), per-ray sums 0.69 (37 x 3),
+d z 6.49 (1024 x 128), latent columns 2.24 of c = 20 (3 x 100); H2 .. H8, raw and dY0 .. dY6 at most 3.70 of c = 258,
+dY7 1.99 of 18, the other weight gradients 5.43 of 80 (37 x 3).
 
 Every caller-owned buffer (stashes, masks, scratch, outputs) is filled with 0xFF (fp16 / fp32 NaN) before the calls, so a
 read of memory no kernel wrote shows up as a NaN in a checked value.
@@ -30,6 +41,7 @@ import torch
 import oracle.nrnerf_oracle as O
 from tests import helpers
 from tests import stash_layout as SL
+from tests import tc_reference as TR
 from tests.parity import DEV, F64, U, Report, half_ulp, poison_bytes, poison_f32, ptr
 
 pytestmark = pytest.mark.gpu
@@ -42,6 +54,8 @@ WGRAD_REL_L2 = 1.5e-4      # weight gradients, relative L2 per tensor
 # fp16's normal range; below that (|x - fp16(x)| * 2048 < 2^-14) it carries x to 2^-36 absolute.  The divergence checks
 # therefore add that floor, propagated through one or two rows of at most 128 weights |w| < 1: 2^-36 * 128.
 DIV_FLOOR = 2.0 ** -29
+C_RAY_BIAS = 34            # time-conditioned ray bias: 32 fp32 FMAs, the bias add and the rounding
+C_DZ = 514                 # time-conditioned d z: 512 fp32 FMAs over both layers' per-ray sums
 
 
 def c_mma(k):
@@ -50,6 +64,12 @@ def c_mma(k):
 
 def c_wgrad(n_tiles):
     return 16 * n_tiles + 64
+
+
+def c_latent_columns(n_rays):
+    """The n + 2 of an n-ray fp32 FMA chain with the 4x margin applied up front: with few rays that worst case is nearly
+    reached (c_obs 2.24 at n = 3)."""
+    return 4 * (n_rays + 2)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -81,30 +101,41 @@ def _lib():
 _MODELS = {}
 
 
-def models(bender):
-    if bender not in _MODELS:
-        coarse, _, bend, _ = helpers.build_models(O, SEED, DEV, with_bender=bender)
-        _MODELS[bender] = (coarse, bend)
-    return _MODELS[bender]
+def models(bender, tc=False):
+    """(coarse NeRF, bender); tc: the time-conditioned baseline's NeRF (W0 [256][95], W5 [256][351]), no bender."""
+    key = "tc" if tc else bender
+    if key not in _MODELS:
+        if tc:
+            from nonrigid_nerf_b200 import run_nerf_helpers as H
+            cp, _ = TR.make_params(SEED)
+            kw = dict(D=8, W=256, input_ch=63, output_ch=5, skips=[4], input_ch_views=0, use_viewdirs=False, ray_bender=None,
+                      ray_bending_latent_size=32, time_conditioned_baseline=True)
+            _MODELS[key] = (helpers.load_nerf_module(H.NeRF(num_ray_samples=64, **kw), cp).to(DEV), None)
+        else:
+            coarse, _, bend, _ = helpers.build_models(O, SEED, DEV, with_bender=bender)
+            _MODELS[key] = (coarse, bend)
+    return _MODELS[key]
 
 
-def pack_nerf(ws, bs, out_ch):
+def pack_nerf(ws, bs, out_ch, input_ch=63):
     from nonrigid_nerf_b200 import ops
     L = _lib()
     lib = L.load()
     ws = [w.detach().contiguous() for w in ws[:8]] + [ws[8][:out_ch].detach().contiguous()]
     bs = [b.detach().contiguous() for b in bs[:8]] + [bs[8][:out_ch].detach().contiguous()]
     buf = torch.empty(lib.nrn_packed_nerf_bytes(), dtype=torch.uint8, device=DEV)
-    L.check(lib.nrn_pack_nerf(ops._ptr_array(ws), ops._ptr_array(bs), 63, out_ch, C.c_void_p(buf.data_ptr()),
+    L.check(lib.nrn_pack_nerf(ops._ptr_array(ws), ops._ptr_array(bs), input_ch, out_ch, C.c_void_p(buf.data_ptr()),
                               C.c_void_p(torch.cuda.current_stream().cuda_stream)), "pack_nerf")
     torch.cuda.synchronize()
     return buf, ws, bs
 
 
 class Case:
+    """tc: the time-conditioned baseline (no bender); lat_stride0: one latent row for every ray (latent_stride 0)."""
     def __init__(self, n, s, bender=True, out_ch=5, cutoff=None, scaling=None, draw_mag=1.0, reg_mag=0.05, ch4=0.0,
-                 seed=0):
-        self.n, self.s, self.bender, self.out_ch = n, s, bender, out_ch
+                 seed=0, tc=False, lat_stride0=False):
+        assert not (tc and bender), "the time-conditioned baseline has no bender"
+        self.n, self.s, self.bender, self.out_ch, self.tc = n, s, bender, out_ch, tc
         self.cutoff, self.scaling = cutoff, scaling
         self.P = n * s
         self.T = -(-self.P // SL.TILE_M)
@@ -115,6 +146,8 @@ class Case:
         u = (torch.arange(s, dtype=torch.float32) + torch.rand(n, s, generator=g)) / s
         self.z = (r["near"] + (r["far"] - r["near"]) * u).to(DEV).contiguous()
         self.lat = r["latents"].to(DEV).contiguous()
+        if lat_stride0:
+            self.lat = self.lat[:1].expand(n, 32)
         mags = torch.tensor([0.3, 0.3, 0.3, 2.0, 0.0][:out_ch])
         d = torch.randn(self.P, out_ch, generator=g) * mags * draw_mag
         if out_ch == 5:
@@ -129,17 +162,23 @@ class Case:
         self.g_ray = (torch.randn(n, generator=g) * 3.0).to(DEV).contiguous()
 
 
-def run_forward(cs):
+def run_forward(cs, train=True, removal=None, points=None):
+    """The training kernel (stash and ReLU masks), or with train=False the inference kernel render() runs; `removal`: its
+    object-removal threshold; `points` [P, stride >= 3]: point mode (NeRF.forward(x)) instead of cs.rays / cs.z."""
     from nonrigid_nerf_b200 import ops
     L = _lib()
     lib = L.load()
-    coarse, bend = models(cs.bender)
+    coarse, bend = models(cs.bender, cs.tc)
     ws, bs = ops.nerf_param_list(coarse)
-    npk, ws, bs = pack_nerf(ws, bs, cs.out_ch)
+    npk, ws, bs = pack_nerf(ws, bs, cs.out_ch, 95 if cs.tc else 63)
     bpk = ops.pack_bender(bend) if cs.bender else None
     o = {"npk": npk, "bpk": bpk, "ws": ws, "bs": bs, "bend": bend}
     a = L.NrnFieldArgs()
-    a.rays, a.z_vals, a.n_rays, a.n_samples = cs.rays.data_ptr(), cs.z.data_ptr(), cs.n, cs.s
+    if points is None:
+        a.rays, a.z_vals = cs.rays.data_ptr(), cs.z.data_ptr()
+    else:
+        a.points, a.points_stride = points.data_ptr(), points.stride(0)
+    a.n_rays, a.n_samples = cs.n, cs.s
     a.nerf_packed, a.out_ch = npk.data_ptr(), cs.out_ch
     o["raw"] = poison_f32(cs.P, cs.out_ch)
     o["init"], o["bent"] = poison_f32(cs.P, 3), poison_f32(cs.P, 3)
@@ -152,11 +191,24 @@ def run_forward(cs):
         a.use_cutoff, a.rigidity_cutoff = 1, cs.cutoff
     if cs.scaling is not None:
         a.use_scaling, a.scaling = 1, cs.scaling
-    o["stash"] = poison_bytes(lib.nrn_stash_bytes(cs.n, cs.s))
-    o["mask"] = poison_bytes(lib.nrn_relu_mask_bytes(cs.n, cs.s))
-    a.stash, a.relu_mask = o["stash"].data_ptr(), o["mask"].data_ptr()
+    if removal is not None:
+        a.use_removal, a.removal_threshold = 1, removal
+    if train:
+        o["stash"] = poison_bytes(lib.nrn_stash_bytes(cs.n, cs.s))
+        o["mask"] = poison_bytes(lib.nrn_relu_mask_bytes(cs.n, cs.s))
+        a.stash, a.relu_mask = o["stash"].data_ptr(), o["mask"].data_ptr()
     a.stream = torch.cuda.current_stream().cuda_stream
-    L.check(lib.nrn_field_forward(C.byref(a)), "field_forward")
+    if cs.tc:
+        # the ray bias [rows][L0, L5][256] from the fp32 weights; one row when the latent stride is 0
+        stride = cs.lat.stride(0)
+        rows = cs.n if stride else 1
+        o["rb"] = poison_f32(rows, 2, 256)
+        L.check(lib.nrn_tc_latent_bias(cs.lat.data_ptr(), stride, rows, ws[0].data_ptr(), bs[0].data_ptr(), ws[5].data_ptr(),
+                                       bs[5].data_ptr(), o["rb"].data_ptr(), a.stream), "tc_latent_bias")
+        a.latents, a.latent_stride = cs.lat.data_ptr(), stride
+        L.check(lib.nrn_field_forward_tc(C.byref(a), o["rb"].data_ptr()), "field_forward_tc")
+    else:
+        L.check(lib.nrn_field_forward(C.byref(a)), "field_forward")
     L.device_error_check()
     return o
 
@@ -169,7 +221,8 @@ def run_backward(cs, o, d_raw=None, nerf_grad=None, nerf_head=None, bender_grad=
     a.n_rays, a.n_samples, a.out_ch = cs.n, cs.s, cs.out_ch
     a.d_raw, a.stash, a.relu_mask, a.nerf_packed = d_raw.data_ptr(), o["stash"].data_ptr(), o["mask"].data_ptr(), o["npk"].data_ptr()
     b = {"gstash": poison_bytes(lib.nrn_grad_stash_bytes(cs.n, cs.s)), "scratch": poison_bytes(lib.nrn_wgrad_scratch_bytes())}
-    b["nerf_grad"] = poison_f32(lib.nrn_nerf_grad_floats(cs.out_ch)) if nerf_grad is None else nerf_grad
+    n_nerf = lib.nrn_nerf_tc_grad_floats(cs.out_ch) if cs.tc else lib.nrn_nerf_grad_floats(cs.out_ch)
+    b["nerf_grad"] = poison_f32(n_nerf) if nerf_grad is None else nerf_grad
     b["nerf_head"] = nerf_head
     a.grad_stash, a.wgrad_scratch, a.nerf_grad = b["gstash"].data_ptr(), b["scratch"].data_ptr(), b["nerf_grad"].data_ptr()
     if nerf_head is not None:
@@ -187,7 +240,16 @@ def run_backward(cs, o, d_raw=None, nerf_grad=None, nerf_head=None, bender_grad=
             a.use_scaling, a.scaling = 1, cs.scaling
     a.accumulate_nerf = a.accumulate_bender = 1 if accumulate else 0
     a.stream = torch.cuda.current_stream().cuda_stream
-    L.check(lib.nrn_field_backward(C.byref(a)), "field_backward")
+    if cs.tc:
+        t = L.NrnTcBwdArgs()
+        b["d_lat"] = poison_f32(cs.n, 32)
+        b["tc_ws"] = poison_f32(lib.nrn_tc_workspace_bytes(cs.n) // 4)   # per-ray sums [n][2][256] | latent columns [2][256][32]
+        t.latents, t.latent_stride = cs.lat.data_ptr(), cs.lat.stride(0)
+        t.w0, t.w5 = o["ws"][0].data_ptr(), o["ws"][5].data_ptr()
+        t.d_latents, t.workspace = b["d_lat"].data_ptr(), b["tc_ws"].data_ptr()
+        L.check(lib.nrn_field_backward_tc(C.byref(a), C.byref(t)), "field_backward_tc")
+    else:
+        L.check(lib.nrn_field_backward(C.byref(a)), "field_backward")
     L.device_error_check()
     return b
 
@@ -327,9 +389,22 @@ def check_forward(cs, o, rep):
     # L0 .. L7 from their own input images
     W = [h16(w) for w in o["ws"]]
     b = [x.detach().to(F64) for x in o["bs"]]
+    if cs.tc:
+        # the ray bias rb[ray][l] = b_l + W_l[:, 63:95] z[ray] from the fp32 weights; then L0 / L5 add, per row, the kernel's
+        # own row of the row's ray (rows past P: the last point's ray)
+        z = cs.lat[:o["rb"].shape[0]].to(F64)
+        ref, ref_a = [], []
+        for l in (0, 5):
+            wl = o["ws"][l][:, 63:95].to(F64)
+            ref.append(b[l] + z @ wl.T)
+            ref_a.append(b[l].abs() + z.abs() @ wl.abs().T)
+        rep.check("ray bias", o["rb"], torch.stack(ref, 1), torch.stack(ref_a, 1), C_RAY_BIAS)
+        ray = torch.arange(R, device=DEV).clamp(max=P - 1) // cs.s
+        rb = o["rb"].to(F64)[ray if o["rb"].shape[0] > 1 else torch.zeros_like(ray)]
+        b[0], b[5] = rb[:, 0], rb[:, 1]
     zc = torch.zeros(256, 1, dtype=F64, device=DEV)
-    W0p = torch.cat([W[0], zc], 1)
-    W5p = torch.cat([W[5][:, :63], zc, W[5][:, 63:]], 1)
+    W0p = torch.cat([W[0][:, :63], zc], 1)
+    W5p = torch.cat([W[5][:, :63], zc, W[5][:, -256:]], 1)
     for l in range(8):
         inp = E if l == 0 else (torch.cat([E, H[4]], 1) if l == 5 else H[l - 1])
         Wl = W0p if l == 0 else (W5p if l == 5 else W[l])
@@ -370,18 +445,29 @@ def dgrad_reference(cs, o, b, rep, scale):
         v, a = dmm(dY[l + 1], W[l + 1])
         rep.check(f"dY{l}", dY[l], v * m[l], a * m[l], c_mma(256), True)
     dE5, dE5a = dmm(dY[5], W[5][:, :63])
-    v, a = dmm(dY[5], W[5][:, 63:])
+    v, a = dmm(dY[5], W[5][:, -256:])   # W5 = [embedding (| latent) | h]
     rep.check("dY4", dY[4], v * m[4], a * m[4], c_mma(256), True)
     for l in (3, 2, 1, 0):
         v, a = dmm(dY[l + 1], W[l + 1])
         rep.check(f"dY{l}", dY[l], v * m[l], a * m[l], c_mma(256), True)
-    dE0, dE0a = dmm(dY[0], W[0])
+    dE0, dE0a = dmm(dY[0], W[0][:, :63])
     pad = lambda t: torch.cat([t, torch.zeros(R, 1, dtype=F64, device=DEV)], 1)
     dx5, ax5 = pe_backward(pad(dE5), pad(dE5a), E)
     dx0, ax0 = pe_backward(pad(dE0), pad(dE0a), E)
     dx, adx = dx5 + dx0, ax5 + ax0
     c_dx = c_mma(256) + C_PE
     out = {"E": E, "H": H, "Draw": Draw, "dY": dY}
+    if cs.tc:
+        # per-ray sums of the stashed dY0 / dY5 over the ray's samples, in fp32 and divided by the loss scale
+        ds = [dY[l][:P].view(cs.n, cs.s, 256) for l in (0, 5)]
+        sums = b["tc_ws"][:cs.n * 512].view(cs.n, 2, 256)
+        rep.check("tc per-ray sums", sums, torch.stack([d.sum(1) for d in ds], 1) / scale,
+                  torch.stack([d.abs().sum(1) for d in ds], 1) / scale, cs.s + 2)
+        # d z from the kernel's own sums and the fp32 latent columns of W0 / W5
+        s = sums.to(F64)
+        w0, w5 = o["ws"][0][:, 63:95].to(F64), o["ws"][5][:, 63:95].to(F64)
+        rep.check("tc d_latents", b["d_lat"], s[:, 0] @ w0 + s[:, 1] @ w5, s[:, 0].abs() @ w0.abs() + s[:, 1].abs() @ w5.abs(),
+                  C_DZ)
     if not cs.bender:
         return out
     Bin, Hb = img(SL.ST_BIN), [img(SL.ST_HB1), img(SL.ST_HB2), img(SL.ST_HB3), img(SL.ST_HB4)]
@@ -454,11 +540,17 @@ def bender_wgrad_reference(Yb, X):
 def check_wgrad(cs, b, imgs, rep, scale, nerf_flat=None, bend_flat=None, base_nerf=None, base_bend=None):
     E, H, Draw, dY = imgs["E"], imgs["H"], imgs["Draw"], imgs["dY"]
     c = c_wgrad(cs.T)
+    # the inputs of W0 and of W5's first columns: [E[:, :63] | the row's latent (time-conditioned; 0 past P)]
+    X = E[:, :63]
+    if cs.tc:
+        Z = torch.zeros(cs.R, 32, dtype=F64, device=DEV)
+        Z[:cs.P] = cs.lat.to(F64).repeat_interleave(cs.s, 0)
+        X = torch.cat([X, Z], 1)
     ref = {}
-    ref["w0"], ref["b0"] = wsum(dY[0], E[:, :63]), (dY[0].sum(0), dY[0].abs().sum(0))
+    ref["w0"], ref["b0"] = wsum(dY[0], X), (dY[0].sum(0), dY[0].abs().sum(0))
     for l in range(1, 8):
         if l == 5:
-            v1, a1 = wsum(dY[5], E[:, :63])
+            v1, a1 = wsum(dY[5], X)
             v2, a2 = wsum(dY[5], H[4])
             ref["w5"] = (torch.cat([v1, v2], 1), torch.cat([a1, a2], 1))
         else:
@@ -469,15 +561,26 @@ def check_wgrad(cs, b, imgs, rep, scale, nerf_flat=None, bend_flat=None, base_ne
     ref["w_out"] = (torch.cat([v, z]), torch.cat([a, z]))
     zb = torch.zeros(cs.out_ch - 4, dtype=F64, device=DEV)
     ref["b_out"] = (torch.cat([Draw[:, :4].sum(0), zb]), torch.cat([Draw[:, :4].abs().sum(0), zb]))
-    got = SL.split_flat(b["nerf_grad"] if nerf_flat is None else nerf_flat, SL.nerf_param_shapes(cs.out_ch))
+    shapes = SL.nerf_param_shapes(cs.out_ch, cs.tc)
+    got = SL.split_flat(b["nerf_grad"] if nerf_flat is None else nerf_flat, shapes)
     if b["nerf_head"] is not None:
-        got.update(SL.split_flat(b["nerf_head"], SL.nerf_param_shapes(cs.out_ch)[-2:]))
-    base = SL.split_flat(base_nerf, SL.nerf_param_shapes(cs.out_ch)) if base_nerf is not None else None
+        got.update(SL.split_flat(b["nerf_head"], shapes[-2:]))
+    base = SL.split_flat(base_nerf, shapes) if base_nerf is not None else None
     for name, (v, a) in ref.items():
         g = got[name].to(F64) - (base[name].to(F64) if base is not None else 0.0)
         rep.check(f"WGRAD {name}", g, v / scale, a / scale + (base[name].to(F64).abs() if base is not None else 0.0), c)
         if base is None:
             rep.rel_l2(f"WGRAD {name}", g, v / scale, WGRAD_REL_L2)
+    if cs.tc:
+        # the latent columns of W0 / W5 from the kernel's own per-ray sums: one fp32 FMA per ray, c_latent_columns(n)
+        s = b["tc_ws"][:cs.n * 512].view(cs.n, 2, 256).to(F64)
+        z = cs.lat.to(F64)
+        for l, name in ((0, "w0"), (1, "w5")):
+            g = got[name][:, 63:95].to(F64)
+            a = s[:, l].abs().T @ z.abs()
+            if base is not None:
+                g, a = g - base[name][:, 63:95].to(F64), a + base[name][:, 63:95].to(F64).abs()
+            rep.check(f"WGRAD {name}[:, 63:95]", g, s[:, l].T @ z, a, c_latent_columns(cs.n))
     if cs.out_ch == 5 and base is None:
         assert bool((got["w_out"][4] == 0).all()) and float(got["b_out"][4]) == 0.0, "head row 4 gradient is not exactly 0"
     if not cs.bender:
@@ -584,6 +687,11 @@ def check_divergence(cs, o, d, rep):
         rep.check(f"div WGRAD {name}", got[name], v / scale, a / scale, c_wgrad(T))
 
 
+def grad_stash_images(cs, b):
+    """Every gradient-stash image DGRAD writes, side by side: d_raw and dY0..dY7, and with a bender its dYb images."""
+    return SL.image(b["gstash"], SL.GRAD_TILE, 0, (SL.GRAD_TILE if cs.bender else SL.GS_YB4[0]) // SL.CHUNK, cs.T)
+
+
 def run_all(cs, tag, divergence=True):
     rep = Report(tag)
     o = run_forward(cs)
@@ -613,6 +721,16 @@ SHAPES = {
     "2x64_out4": dict(n=2, s=64, out_ch=4),
     "3x100_out4_nobender": dict(n=3, s=100, out_ch=4, bender=False),
     "3x100_cutoff_scaling": dict(n=3, s=100, cutoff="median", scaling=0.7),
+    # time-conditioned baseline: L0 / L5 take each accumulator row's bias from its own ray
+    "37x3_tc": dict(n=37, s=3, bender=False, tc=True),          # rows r0 and r0 + 8 on different rays; one ragged tile
+    "5x1_tc": dict(n=5, s=1, bender=False, tc=True),            # every row its own ray
+    "1x7_tc": dict(n=1, s=7, bender=False, tc=True),            # one ray, rows past P
+    "3x100_tc": dict(n=3, s=100, bender=False, tc=True),        # rays straddle tiles
+    "3x100_tc_stride0": dict(n=3, s=100, bender=False, tc=True, lat_stride0=True),   # one latent row for every ray
+    "3x100_out4_tc": dict(n=3, s=100, out_ch=4, bender=False, tc=True),
+    "11x100_tc": dict(n=11, s=100, bender=False, tc=True),      # 9 tiles: empty trailing WGRAD splits without a bender
+    "1023x64_tc": dict(n=1023, s=64, bender=False, tc=True),
+    "1024x128_tc": dict(n=1024, s=128, bender=False, tc=True),
 }
 
 
@@ -624,9 +742,16 @@ def test_every_stage_matches_its_fp64_reference(name):
         kw["cutoff"] = float(run_forward(Case(**dict(kw, cutoff=None)))["rig"].median())
     cs = Case(**kw)
     o, b, _ = run_all(cs, name)
+    if kw.get("lat_stride0"):
+        # a broadcast latent row computes exactly what the same row repeated for every ray does
+        ex = Case(**kw)
+        ex.lat = cs.lat.contiguous()
+        oe = run_forward(ex)
+        for k in ("stash", "mask", "raw"):
+            assert torch.equal(o[k], oe[k]), f"latent stride 0 vs repeated rows: {k} differs"
     if cs.T >= 500:
         # the fp16 gradient chain must not saturate at the benchmark's shapes
-        g = SL.image(b["gstash"], SL.GRAD_TILE, 0, SL.GRAD_TILE // SL.CHUNK, cs.T).float().abs()
+        g = grad_stash_images(cs, b).float().abs()
         assert float(g.max()) < 65504.0, f"gradient stash saturates: max {float(g.max())}"
         print(f"  [{name}] max |gradient stash| {float(g.max()):.1f}")
 
@@ -667,29 +792,39 @@ def empty_splits(n_tiles, splits):
 def test_the_9_tile_shape_has_an_empty_trailing_wgrad_split():
     """wgrad_reduce_kernel skips splits that own no tiles (n_valid).  The 11 x 100 shape above covers that path only if
     the plan for this device leaves such a split; a cluster-limited device can run fewer CTAs than SMs, so every even
-    CTA budget down to 3/4 of the SMs is checked."""
+    CTA budget down to 3/4 of the SMs is checked.  The same holds for the bender-less plan of 11 x 100_tc."""
     sms = torch.cuda.get_device_properties(DEV).multi_processor_count
-    n_tiles = SHAPES["11x100"]["n"] * SHAPES["11x100"]["s"] // SL.TILE_M + 1
-    assert n_tiles == 9
-    for max_ctas in range(sms & ~1, (3 * sms // 4) & ~1, -2):
-        assert empty_splits(n_tiles, wgrad_plan(n_tiles, max_ctas)), max_ctas
+    for name, has_bender in (("11x100", True), ("11x100_tc", False)):
+        n_tiles = SHAPES[name]["n"] * SHAPES[name]["s"] // SL.TILE_M + 1
+        assert n_tiles == 9
+        for max_ctas in range(sms & ~1, (3 * sms // 4) & ~1, -2):
+            assert empty_splits(n_tiles, wgrad_plan(n_tiles, max_ctas, has_bender)), (name, max_ctas)
 
 
-# ---- loss-scale edges ----
+# ---- loss-scale edges: the bending model and the time-conditioned baseline (TC) ----
+def edge_case(mode, **kw):
+    return Case(3, 100, bender=False, tc=True, **kw) if mode == "tc" else Case(3, 100, **kw)
+
+
+MODES = ["bender", "tc"]
+
+
 def test_zero_upstream_gives_exactly_zero_gradients():
-    cs = Case(3, 100, draw_mag=0.0, reg_mag=0.0)
-    o = run_forward(cs)
-    b = run_backward(cs, o)
-    for k in ("nerf_grad", "bender_grad", "d_lat"):
-        assert bool((b[k] == 0).all()), k
-    g = SL.image(b["gstash"], SL.GRAD_TILE, 0, SL.GRAD_TILE // SL.CHUNK, cs.T)
-    assert bool((g == 0).all())
+    for mode in MODES:
+        cs = edge_case(mode, draw_mag=0.0, reg_mag=0.0)
+        o = run_forward(cs)
+        b = run_backward(cs, o)
+        # every float of each buffer (nerf_grad: the TC layout's full length), the TC per-ray sums and latent columns included
+        for k in ("nerf_grad", "d_lat") + (("tc_ws",) if cs.tc else ("bender_grad",)):
+            assert bool((b[k] == 0).all()), (mode, k)
+        assert bool((grad_stash_images(cs, b) == 0).all()), (mode, "gradient stash")
 
 
 @pytest.mark.parametrize("mag", [1e-15, 1e10])
 def test_extreme_upstream_magnitudes_keep_every_stage_bound(mag):
-    cs = Case(3, 100, draw_mag=mag, reg_mag=0.05 * mag)
-    run_all(cs, f"|d_raw| x {mag:g}", divergence=False)
+    for mode in MODES:
+        cs = edge_case(mode, draw_mag=mag, reg_mag=0.05 * mag)
+        run_all(cs, f"{mode} |d_raw| x {mag:g}", divergence=False)
 
 
 def test_regulariser_upstream_sets_the_loss_scale():
@@ -700,42 +835,74 @@ def test_regulariser_upstream_sets_the_loss_scale():
 
 def test_channel_4_of_d_raw_changes_nothing():
     """Channel 4 never reaches the loss (the head's row 4 gets a zero gradient), so a large d_raw[..., 4] must not move
-    the loss scale: every gradient equals the channel-4-zero run bit for bit (the latent gradient up to the order of its
-    fp32 atomics)."""
-    cs = Case(3, 100)
-    o = run_forward(cs)
-    b0 = run_backward(cs, o)
-    d4 = cs.d_raw.clone()
-    d4[:, 4] = 3.0e4 * torch.sign(torch.randn(cs.P, device=DEV))
-    b4 = run_backward(cs, o, d_raw=d4)
-    assert torch.equal(b0["gstash"], b4["gstash"]), "gradient stash differs"
-    assert torch.equal(b0["nerf_grad"], b4["nerf_grad"]), "NeRF weight gradients differ"
-    assert torch.equal(b0["bender_grad"], b4["bender_grad"]), "bender weight gradients differ"
-    # the latent gradient's fp32 atomics add in no fixed order: equal up to that rounding
-    torch.testing.assert_close(b0["d_lat"], b4["d_lat"], rtol=0.0, atol=1e-5 * float(b0["d_lat"].abs().max()))
+    the loss scale: every gradient equals the channel-4-zero run bit for bit (the bender's latent gradient up to the order
+    of its fp32 atomics; the TC latent sums run in a fixed order, so there the latent gradient too)."""
+    for mode in MODES:
+        cs = edge_case(mode)
+        o = run_forward(cs)
+        b0 = run_backward(cs, o)
+        d4 = cs.d_raw.clone()
+        d4[:, 4] = 3.0e4 * torch.sign(torch.randn(cs.P, device=DEV))
+        b4 = run_backward(cs, o, d_raw=d4)
+        assert torch.equal(b0["gstash"], b4["gstash"]), f"{mode}: gradient stash differs"
+        assert torch.equal(b0["nerf_grad"], b4["nerf_grad"]), f"{mode}: NeRF weight gradients differ"
+        if cs.tc:
+            assert torch.equal(b0["tc_ws"], b4["tc_ws"]), "tc: per-ray sums or latent weight columns differ"
+            assert torch.equal(b0["d_lat"], b4["d_lat"]), "tc: latent gradients differ"
+        else:
+            assert torch.equal(b0["bender_grad"], b4["bender_grad"]), "bender weight gradients differ"
+            # the latent gradient's fp32 atomics add in no fixed order: equal up to that rounding
+            torch.testing.assert_close(b0["d_lat"], b4["d_lat"], rtol=0.0, atol=1e-5 * float(b0["d_lat"].abs().max()))
 
 
 def test_head_redirection_and_accumulation():
     """nerf_grad_head puts the output layer's gradient in its own buffer; accumulate_nerf / accumulate_bender add the
-    gradients onto what the destination holds."""
-    cs = Case(3, 100)
-    rep = Report("accumulate + head redirect")
-    o = run_forward(cs)
+    gradients onto what the destination holds (optim.Adam's gradient arena)."""
     lib = _lib().load()
-    g = torch.Generator(device=DEV).manual_seed(3)
-    n_head = cs.out_ch * 257
-    pre_n = torch.randn(lib.nrn_nerf_grad_floats(cs.out_ch), generator=g, device=DEV)
-    pre_n[-n_head:] = float("nan")        # the head part lives elsewhere: this tail must stay untouched
-    pre_h = torch.randn(n_head, generator=g, device=DEV)
-    pre_b = torch.randn(lib.nrn_bender_grad_floats(), generator=g, device=DEV)
-    nerf, head, bend = pre_n.clone(), pre_h.clone(), pre_b.clone()
-    b = run_backward(cs, o, nerf_grad=nerf, nerf_head=head, bender_grad=bend, accumulate=True)
-    assert bool(torch.isnan(nerf[-n_head:]).all()), "the head's slot of nerf_grad was written despite nerf_grad_head"
-    imgs = dgrad_reference(cs, o, b, rep, expected_scale(cs))
-    full = torch.cat([nerf[:-n_head], head])
-    base = torch.cat([pre_n[:-n_head], pre_h])
-    b["nerf_head"] = None
-    check_wgrad(cs, b, imgs, rep, expected_scale(cs), nerf_flat=full, bend_flat=bend, base_nerf=base, base_bend=pre_b)
+    for mode in MODES:
+        cs = edge_case(mode)
+        rep = Report(f"{mode} accumulate + head redirect")
+        o = run_forward(cs)
+        g = torch.Generator(device=DEV).manual_seed(3)
+        n_head = cs.out_ch * 257
+        pre_n = torch.randn(lib.nrn_nerf_tc_grad_floats(cs.out_ch) if cs.tc else lib.nrn_nerf_grad_floats(cs.out_ch),
+                            generator=g, device=DEV)
+        pre_n[-n_head:] = float("nan")        # the head part lives elsewhere: this tail must stay untouched
+        pre_h = torch.randn(n_head, generator=g, device=DEV)
+        pre_b = torch.randn(lib.nrn_bender_grad_floats(), generator=g, device=DEV)
+        nerf, head, bend = pre_n.clone(), pre_h.clone(), pre_b.clone()
+        b = run_backward(cs, o, nerf_grad=nerf, nerf_head=head, bender_grad=bend, accumulate=True)
+        assert bool(torch.isnan(nerf[-n_head:]).all()), f"{mode}: the head's slot of nerf_grad was written despite nerf_grad_head"
+        imgs = dgrad_reference(cs, o, b, rep, expected_scale(cs))
+        full = torch.cat([nerf[:-n_head], head])
+        base = torch.cat([pre_n[:-n_head], pre_h])
+        b["nerf_head"] = None
+        check_wgrad(cs, b, imgs, rep, expected_scale(cs), nerf_flat=full, bend_flat=bend, base_nerf=base, base_bend=pre_b)
+
+
+@pytest.mark.parametrize("head", [False, True])
+def test_empty_tc_batch_zeroes_the_whole_gradient_layout(head):
+    """n_rays = 0 (an empty shard) contributes zero gradients: every float of the time-conditioned layout, the latent
+    columns of W0 / W5 included, is overwritten with 0; with nerf_grad_head the head's slot of nerf_grad stays untouched."""
+    from nonrigid_nerf_b200 import ops
+    L = _lib()
+    lib = L.load()
+    npk, _, _ = pack_nerf(*ops.nerf_param_list(models(False, tc=True)[0]), 5, 95)
+    n_nerf, n_head = lib.nrn_nerf_tc_grad_floats(5), 5 * 257
+    grad, head_buf = poison_f32(n_nerf), poison_f32(n_head)
+    a, t = L.NrnFieldBwdArgs(), L.NrnTcBwdArgs()
+    a.n_rays, a.n_samples, a.out_ch = 0, 64, 5
+    a.nerf_packed, a.nerf_grad = npk.data_ptr(), grad.data_ptr()
+    if head:
+        a.nerf_grad_head = head_buf.data_ptr()
+    a.stream = torch.cuda.current_stream().cuda_stream
+    L.check(lib.nrn_field_backward_tc(C.byref(a), C.byref(t)), "field_backward_tc")
+    L.device_error_check()
+    if head:
+        assert bool((grad[:-n_head] == 0).all()) and bool((head_buf == 0).all())
+        assert bool(torch.isnan(grad[-n_head:]).all()), "the head's slot of nerf_grad was written despite nerf_grad_head"
+    else:
+        assert bool((grad == 0).all())
 
 
 def test_forward_is_deterministic_past_p():

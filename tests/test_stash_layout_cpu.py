@@ -46,6 +46,7 @@ def test_gradient_parameter_maps_match_the_library(out_ch):
     from nonrigid_nerf_b200 import _lib
     lib = _lib.load()
     assert sum(math.prod(s) for _, s in SL.nerf_param_shapes(out_ch)) == lib.nrn_nerf_grad_floats(out_ch)
+    assert sum(math.prod(s) for _, s in SL.nerf_param_shapes(out_ch, tc=True)) == lib.nrn_nerf_tc_grad_floats(out_ch)
     assert sum(math.prod(s) for _, s in SL.bender_param_shapes()) == lib.nrn_bender_grad_floats()
 
 

@@ -166,8 +166,7 @@ def test_per_ray_sums_latent_gradient_and_latent_columns_match_fp64():
     dz_ref = ref[:, 0] @ w0[:, 63:95] + ref[:, 1] @ w5[:, 63:95]
     e_z = R.rel(d_lat.double().cpu(), dz_ref.cpu())
     dw_ref = torch.stack([ref[:, 0].T @ lat.double(), ref[:, 1].T @ lat.double()])       # [2][256][32]
-    flat = SL.split_flat(grad.cpu(), [("w0", (256, 95)), ("b0", (256,))] + sum(
-        [[(f"w{l}", (256, 351 if l == 5 else 256)), (f"b{l}", (256,))] for l in range(1, 8)], []) + [("w_out", (5, 256)), ("b_out", (5,))])
+    flat = SL.split_flat(grad.cpu(), SL.nerf_param_shapes(out_ch, tc=True))
     e_w0 = R.rel(flat["w0"][:, 63:95].double(), dw_ref[0].cpu())
     e_w5 = R.rel(flat["w5"][:, 63:95].double(), dw_ref[1].cpu())
     print(f"d z vs fp64 {e_z:.3e}; dW0[:, 63:95] {e_w0:.3e}, dW5[:, 63:95] {e_w5:.3e}")
