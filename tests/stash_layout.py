@@ -116,6 +116,19 @@ def bender_param_shapes():
                      ("rig_b2", (1,))]
 
 
+# Peer-memory window (c_abi.cu fill_peer, peer.py): [flags: ARRIVE / DONE / GATHER x 8 u32, padded | 2 row slots | arena]
+PEER_FLAG_BYTES = 1024
+PEER_MAX_RANKS = 8
+PEER_ARRIVE, PEER_DONE, PEER_GATHER = 0, 1, 2
+
+
+def peer_window_layout(arena_floats, slot_floats):
+    """(slot_off, slot_bytes, arena_off, window_bytes); slots and arena each rounded up to 256 bytes."""
+    slot_bytes = (4 * slot_floats + 255) // 256 * 256
+    arena_off = PEER_FLAG_BYTES + 2 * slot_bytes
+    return PEER_FLAG_BYTES, slot_bytes, arena_off, arena_off + (4 * arena_floats + 255) // 256 * 256
+
+
 def split_flat(flat, shapes):
     out, o = {}, 0
     for name, shape in shapes:

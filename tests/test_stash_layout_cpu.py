@@ -50,6 +50,18 @@ def test_gradient_parameter_maps_match_the_library(out_ch):
     assert sum(math.prod(s) for _, s in SL.bender_param_shapes()) == lib.nrn_bender_grad_floats()
 
 
+def test_peer_window_layout_matches_the_library():
+    from nonrigid_nerf_b200 import _lib
+    lib = _lib.load()
+    assert SL.PEER_FLAG_BYTES >= 4 * 3 * SL.PEER_MAX_RANKS
+    for arena, slot in ((0, 0), (1, 1), (63, 64), (64, 65), (1_143_357, 1 << 16), (1_143_357, 65537), (2049, 8192)):
+        slot_off, slot_bytes, arena_off, nbytes = SL.peer_window_layout(arena, slot)
+        assert lib.nrn_peer_window_bytes(arena, slot) == nbytes, (arena, slot)
+        assert slot_bytes % 256 == 0 and slot_bytes >= 4 * slot and arena_off % 256 == 0
+        assert nbytes - arena_off >= 4 * arena
+    assert SL.peer_window_layout(0, 65537)[1] == 262400     # 65537 floats round up: the arena moves by 2 x 252 bytes
+
+
 def _encode_reference(bits):
     """The documented layout written out element by element (independent of stash_layout's vectorised code)."""
     rows, ncols = bits.shape
