@@ -188,6 +188,29 @@ int nrn_tc_latent_bias(const float* latents, int64_t latent_stride, int n_rays, 
  * args->latent_stride == 0, one row for every ray.  args->bender_packed must be NULL; args->latents is not read. */
 int nrn_field_forward_tc(const NrnFieldArgs* args, const float* ray_bias);
 int nrn_nerf_tc_grad_floats(int out_ch);   /* flat order as nrn_nerf_grad_floats, with W0 [256][95] and W5 [256][351] */
+
+/* ---- view-dependent head, inference only: NeRF(use_viewdirs=True, approx_nonrigid_viewdirs=True)
+ * (run_nerf_helpers.py:233-236, 284-304, 316-356; train.py:364-399).  raw = [rgb_linear(relu(views_linears.0(
+ * cat[feature_linear(h8), dir_enc]))), alpha_linear(h8)], dir_enc = [d, sin(2^k d), cos(2^k d)], k = 0..3 (27 columns).
+ * With a bender d is the normalised backward difference of the BENT points of the ray, (p_i - p_{i-1}) / (|.| + 1e-6),
+ * and d_0 = d_1; without one it is the given viewdirs row.  The trunk is packed by nrn_pack_nerf with out_ch = 4 and a
+ * head of zeros in rows 0-2 and alpha_linear in row 3; feature_linear, views_linears.0 and rgb_linear by nrn_pack_views. */
+size_t nrn_packed_views_bytes(void);
+/* w / b [0] = feature_linear [256][256], [1] = views_linears.0 [128][256 + 27], [2] = rgb_linear [3][128] */
+int nrn_pack_views(const float* const* w, const float* const* b, void* packed, void* stream);
+size_t nrn_views_workspace_bytes(int n_rays, int n_samples);   /* bend workspace: 16 bytes per point */
+typedef struct NrnViewArgs {
+  const void* views_packed;   /* nrn_pack_views output (16-byte aligned); may be NULL when args->raw is NULL */
+  const float* viewdirs;      /* no bender: normalised view directions, one row per ray (ray mode) or per point (point
+                                 mode); not read with a bender */
+  int64_t viewdirs_stride;    /* floats between rows, >= 3 */
+  void* workspace;            /* with a bender: nrn_views_workspace_bytes(n_rays, n_samples), 16-byte aligned */
+} NrnViewArgs;
+/* args as for nrn_field_forward, with out_ch = 4 and no stash / relu_mask (training is not implemented).  With a bender
+ * n_samples >= 2: the finite differences run over each ray's n_samples consecutive points.  Point mode takes
+ * n_rays * n_samples points, n_samples consecutive ones forming a ray; latents (and viewdirs) are read per point.  With a
+ * bender, raw = NULL runs the bend pass alone (the details: bent points, offsets, rigidity). */
+int nrn_field_forward_views(const NrnFieldArgs* args, const NrnViewArgs* views);
 size_t nrn_tc_workspace_bytes(int n_rays);   /* per-ray sums [n][2][256] + latent columns of dW0 / dW5 [2][256][32] */
 typedef struct NrnTcBwdArgs {
   const float* latents;           /* [n_rays][32] the forward call's latents ... */
@@ -330,7 +353,8 @@ int nrn_peer_gather_rows(const NrnPeerCtx* ctx, const float* local, int n_per_ra
  * While enabled, every launch of the kernel kinds below is bracketed by CUDA events recorded on the
  * launch stream.  kinds: 0 field forward, 1 field DGRAD, 2 WGRAD (+reduce), 3 composite(+resample),
  * 4 composite backward, 5 divergence regulariser, 6 time-conditioned ray bias (nrn_tc_latent_bias), 7 time-conditioned
- * latent gradients (per-ray sums, d z, latent columns of dW0 / dW5).  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * latent gradients (per-ray sums, d z, latent columns of dW0 / dW5), 8 bend pass of the view-dependent head, 9 its
+ * view-head field kernel (nrn_field_forward_views).  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

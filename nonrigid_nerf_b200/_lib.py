@@ -35,6 +35,12 @@ class NrnFieldArgs(C.Structure):
     ]
 
 
+class NrnViewArgs(C.Structure):
+    _fields_ = [
+        ("views_packed", _vp), ("viewdirs", _vp), ("viewdirs_stride", C.c_int64), ("workspace", _vp),
+    ]
+
+
 class NrnFieldBwdArgs(C.Structure):
     _fields_ = [
         ("n_rays", C.c_int32), ("n_samples", C.c_int32), ("out_ch", C.c_int32),
@@ -152,6 +158,10 @@ SYMBOLS = {
     "nrn_field_forward_tc": (C.c_int, [C.POINTER(NrnFieldArgs), _vp]),
     "nrn_nerf_tc_grad_floats": (C.c_int, [C.c_int]),
     "nrn_tc_workspace_bytes": (C.c_size_t, [C.c_int]),
+    "nrn_packed_views_bytes": (C.c_size_t, []),
+    "nrn_pack_views": (C.c_int, [C.POINTER(_vp), C.POINTER(_vp), _vp, _vp]),
+    "nrn_views_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "nrn_field_forward_views": (C.c_int, [C.POINTER(NrnFieldArgs), C.POINTER(NrnViewArgs)]),
     "nrn_field_backward_tc": (C.c_int, [C.POINTER(NrnFieldBwdArgs), C.POINTER(NrnTcBwdArgs)]),
     "nrn_div_stash_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "nrn_div_grad_stash_bytes": (C.c_size_t, [C.c_int, C.c_int]),
@@ -175,6 +185,8 @@ SYMBOLS = {
 KERNEL_KINDS = ("field_fwd", "field_dgrad", "wgrad", "composite", "composite_bwd", "divergence")
 # the time-conditioned baseline's own kernels (ray bias; per-ray sums, d z and latent weight columns), timing kinds 6 and 7
 TC_KERNEL_KINDS = ("tc_latent_bias", "tc_latent_bwd")
+# the view-dependent head's kernels (bend pass, view-head field kernel), timing kinds 8 and 9
+VIEW_KERNEL_KINDS = ("views_bend", "views_field")
 
 
 def timing_enable(on: bool) -> None:
@@ -182,8 +194,8 @@ def timing_enable(on: bool) -> None:
 
 
 def timing_read(kinds=KERNEL_KINDS):
-    """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True); `kinds` is KERNEL_KINDS or
-    KERNEL_KINDS + TC_KERNEL_KINDS."""
+    """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True); `kinds` is KERNEL_KINDS,
+    KERNEL_KINDS + TC_KERNEL_KINDS or KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS."""
     n = len(kinds)
     ms = (C.c_double * n)()
     cnt = (C.c_int * n)()

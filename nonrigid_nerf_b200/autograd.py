@@ -507,10 +507,46 @@ def _needs_grad(net, latents) -> bool:
     return bender is not None and any(p.requires_grad for p in bender.parameters())
 
 
-def field(net, rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[torch.Tensor],
-          want_details: bool) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
-    """Fused field evaluation for rays x samples; differentiable when autograd is recording."""
+def views_check(net, latents=None) -> None:
+    """Raise for what the view-dependent head (use_viewdirs=True) does not support: a seated bender with exact view
+    directions or without rays of at least two samples, and any differentiable call (training is not implemented)."""
+    if not getattr(net, "use_viewdirs", False):
+        return
+    if net.ray_bender[0] is not None:
+        if not net.approx_nonrigid_viewdirs:
+            raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True with approx_nonrigid_viewdirs=False (exact view directions "
+                               "through the ray bender) is not implemented")
+        if net.num_ray_samples is None or net.num_ray_samples < 2:
+            raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True with a ray bender needs num_ray_samples >= 2 (the view "
+                               f"directions are finite differences along each ray; got {net.num_ray_samples})")
+    if _needs_grad(net, latents):
+        raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True: training with the view-dependent head is not implemented yet; "
+                           "rendering works under torch.no_grad()")
+
+
+def field_views(net, rays, z_vals, points, latents, viewdirs, want_details, bend_only=False):
+    """The view-dependent head (inference): ray mode (rays, z_vals) or point mode (points grouped into rays of
+    net.num_ray_samples).  bend_only: the bend pass alone (details only, raw is None)."""
+    views_check(net, latents)
     bender = net.ray_bender[0]
+    cutoff, scaling, removal = _knobs(net)
+    nerf_pack = ops.pack_nerf(net)
+    bender_pack = ops.pack_bender(bender) if bender is not None else None
+    views_pack = None if bend_only else ops.pack_views(net)
+    s = net.num_ray_samples if (points is not None and bender is not None and not bend_only) else 1
+    return ops.field_forward_views(rays, z_vals, points, s, latents, viewdirs, nerf_pack, bender_pack, views_pack, cutoff,
+                                   scaling, removal, want_details)
+
+
+def field(net, rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[torch.Tensor],
+          want_details: bool, viewdirs: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
+    """Fused field evaluation for rays x samples; differentiable when autograd is recording.  viewdirs [N, 3]: the
+    normalised ray directions a use_viewdirs=True model takes."""
+    bender = net.ray_bender[0]
+    if getattr(net, "use_viewdirs", False):
+        if viewdirs is None:
+            raise RuntimeError("nonrigid_nerf_b200: a use_viewdirs=True model needs ray batches with view directions (11 columns)")
+        return field_views(net, rays, z_vals, None, latents, viewdirs, want_details)
     _tc_net(net)
     if not _needs_grad(net, latents):
         return field_rays(net, rays, z_vals, latents, want_details)
@@ -539,6 +575,8 @@ def field_rays(net, rays, z_vals, latents, want_details):
 
 def field_points(net, pts, latents, want_details):
     """NeRF.forward(x) semantics: one xyz (+ latent) per row.  Inference only."""
+    if getattr(net, "use_viewdirs", False):
+        raise RuntimeError("nonrigid_nerf_b200: a use_viewdirs=True model is evaluated point-wise by field_views")
     _tc_net(net)
     if _needs_grad(net, latents):
         raise RuntimeError("nonrigid_nerf_b200: the point-wise NeRF.forward / run_network entry is inference-only; "

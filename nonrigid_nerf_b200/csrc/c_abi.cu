@@ -21,6 +21,8 @@ cudaError_t launch_field_fwd_tc(const FieldFwdParams& p, int num_sms, cudaStream
 cudaError_t launch_tc_latent_bias(const float* lat, long long lat_stride, int n_rays, const float* w0, const float* b0, const float* w5,
                                   const float* b5, float* rb, cudaStream_t stream);
 cudaError_t launch_tc_latent_bwd(const TcBwdParams& p, cudaStream_t stream);
+cudaError_t launch_field_bend(const FieldFwdParams& p, const ViewParams& v, int num_sms, cudaStream_t stream);
+cudaError_t launch_field_views(const FieldFwdParams& p, const ViewParams& v, int num_sms, cudaStream_t stream);
 }
 
 namespace {
@@ -260,6 +262,94 @@ int nrn_field_forward_tc(const NrnFieldArgs* a, const float* ray_bias) {
   if (a->latent_stride < 0) return fail(NRN_E_INVALID, "nrn_field_forward_tc: latent_stride < 0");
   if (a->n_rays > 0 && !ray_bias) return fail(NRN_E_INVALID, "nrn_field_forward_tc: null ray_bias (nrn_tc_latent_bias output)");
   return field_forward(a, ray_bias, "nrn_field_forward_tc");
+}
+
+size_t nrn_packed_views_bytes(void) { return nrn::kViewsPackedBytes; }
+
+int nrn_pack_views(const float* const* w, const float* const* b, void* packed, void* stream) {
+  if (!w || !b || !packed) return fail(NRN_E_INVALID, "nrn_pack_views: null argument");
+  if (!aligned16(packed)) return fail(NRN_E_INVALID, "nrn_pack_views: packed buffer must be 16-byte aligned");
+  nrn::ViewsSrc src;
+  for (int i = 0; i < 3; ++i) {
+    if (!w[i] || !b[i]) return fail(NRN_E_INVALID, "nrn_pack_views: null layer %d", i);
+    src.w[i] = w[i];
+    src.b[i] = b[i];
+  }
+  const cudaError_t e = nrn::launch_pack_views(src, packed, static_cast<cudaStream_t>(stream));
+  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "pack_views_kernel");
+}
+
+size_t nrn_views_workspace_bytes(int n_rays, int n_samples) {
+  if (n_rays < 0 || n_samples < 1) return 0;
+  return static_cast<size_t>(n_rays) * n_samples * sizeof(float4);
+}
+
+// The view-dependent head: with a bender the bend pass (bent points and rigidities -> workspace, and the details), then,
+// unless raw is NULL, the view-head kernel; without a bender the view-head kernel alone, on the given view directions.
+int nrn_field_forward_views(const NrnFieldArgs* a, const NrnViewArgs* v) {
+  const char* who = "nrn_field_forward_views";
+  if (!a || !v) return fail(NRN_E_INVALID, "%s: null args", who);
+  if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "%s: bad sizes n=%d S=%d", who, a->n_rays, a->n_samples);
+  if (a->stash || a->relu_mask)
+    return fail(NRN_E_INVALID, "%s: use_viewdirs=True is inference only (stash / relu_mask must be NULL; training is not implemented)", who);
+  if (a->out_ch != 4) return fail(NRN_E_INVALID, "%s: out_ch=%d unsupported (use_viewdirs=True: 4 = rgb + alpha)", who, a->out_ch);
+  const bool bend = a->bender_packed != nullptr;
+  if (bend && a->raw && a->n_samples < 2)
+    return fail(NRN_E_INVALID, "%s: use_viewdirs=True with a bender needs n_samples >= 2 (finite-difference view directions)", who);
+  if (!bend && !a->raw) return fail(NRN_E_INVALID, "%s: raw is NULL without a bender (the bend pass alone needs one)", who);
+  if (!bend && !v->viewdirs) return fail(NRN_E_INVALID, "%s: use_viewdirs=True without a bender needs viewdirs", who);
+  if (!bend && v->viewdirs_stride < 3) return fail(NRN_E_INVALID, "%s: viewdirs_stride=%lld < 3", who, (long long)v->viewdirs_stride);
+  if (a->n_rays == 0) return NRN_OK;
+  if (!a->nerf_packed || (a->raw && !v->views_packed)) return fail(NRN_E_INVALID, "%s: null nerf_packed / views_packed", who);
+  if (a->points) {
+    if (a->points_stride < 3) return fail(NRN_E_INVALID, "%s: point mode needs points_stride >= 3", who);
+  } else if (!a->rays || !a->z_vals) {
+    return fail(NRN_E_INVALID, "%s: null rays / z_vals", who);
+  }
+  if (bend && !a->latents) return fail(NRN_E_INVALID, "%s: bender given without latents", who);
+  if (bend && (!v->workspace || !aligned16(v->workspace)))
+    return fail(NRN_E_INVALID, "%s: a bender needs the workspace (nrn_views_workspace_bytes, 16-byte aligned)", who);
+  if (!aligned16(a->nerf_packed) || (bend && !aligned16(a->bender_packed)) || (v->views_packed && !aligned16(v->views_packed)))
+    return fail(NRN_E_INVALID, "%s: packed weights must be 16-byte aligned", who);
+  const long long P = static_cast<long long>(a->n_rays) * a->n_samples;
+  const long long tiles = (P + nrn::kTileM - 1) / nrn::kTileM;
+  if (tiles > 0x7fffffffLL) return fail(NRN_E_INVALID, "%s: too many points", who);
+  DeviceState* ds;
+  int rc = device_state(&ds);
+  if (rc) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  nrn::FieldFwdParams p{};
+  p.rays = a->rays; p.z_vals = a->z_vals; p.pts = a->points; p.pts_stride = a->points_stride;
+  p.latents = a->latents; p.latent_stride = a->latent_stride;
+  p.n_rays = a->n_rays; p.S = a->n_samples; p.P = P; p.n_tiles = static_cast<int>(tiles);
+  const uint8_t* np = static_cast<const uint8_t*>(a->nerf_packed);
+  p.nerf_w = np; p.nerf_bias = reinterpret_cast<const float*>(np + nrn::kNerfWBytes);
+  p.cutoff = a->rigidity_cutoff; p.use_cutoff = a->use_cutoff;
+  p.scaling = a->scaling; p.use_scaling = a->use_scaling;
+  p.removal = a->removal_threshold; p.use_removal = a->use_removal;
+  p.out_ch = 4; p.err = ds->err_word;
+  nrn::ViewParams vp{};
+  const uint8_t* vw = static_cast<const uint8_t*>(v->views_packed);
+  vp.w = vw; vp.bias = vw ? reinterpret_cast<const float*>(vw + nrn::kViewsWBytes) : nullptr;
+  vp.viewdirs = v->viewdirs; vp.viewdirs_stride = v->viewdirs_stride;
+  cudaError_t e;
+  if (bend) {
+    nrn::FieldFwdParams b = p;   // point mode: every point its own latent row
+    if (a->points) { b.n_rays = static_cast<int>(P); b.S = 1; }
+    const uint8_t* bp = static_cast<const uint8_t*>(a->bender_packed);
+    b.bend_w = bp; b.bend_bias = reinterpret_cast<const float*>(bp + nrn::kBendWBytes);
+    b.d_init = a->initial_input_pts; b.d_bent = a->input_pts; b.d_unmasked = a->unmasked_offsets;
+    b.d_masked = a->masked_offsets; b.d_rigid = a->rigidity_mask;
+    vp.ws = static_cast<float4*>(v->workspace);
+    { ScopedTimer tm(8, st); e = nrn::launch_field_bend(b, vp, ds->num_sms, st); }
+    if (e != cudaSuccess) return cuda_fail(e, "field_bend_kernel");
+    if (!a->raw) return NRN_OK;
+  } else {
+    p.d_init = a->initial_input_pts; p.d_bent = a->input_pts;
+  }
+  p.raw = a->raw;
+  { ScopedTimer tm(9, st); e = nrn::launch_field_views(p, vp, ds->num_sms, st); }
+  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "field_views_kernel");
 }
 
 int nrn_tc_latent_bias(const float* latents, int64_t latent_stride, int n_rays, const float* w0, const float* b0, const float* w5,

@@ -17,6 +17,14 @@
 //   steps  : B0..B4 (ray bender, offset + rigidity MLPs fused block-diagonally), L0..L7, head
 //
 // Shared memory (per CTA): bender H 24 KB + E 16 KB activations, 5 x 32 KB weight ring, per-row staging, barriers.
+//
+// View-dependent head (NeRF(use_viewdirs=True), inference only), two more instantiations of the same body:
+//   bend pass (with a bender): B0..B4 only; every point's bent xyz and rigidity -> the bend workspace (16 B / point)
+//   view-head kernel: points from the workspace (or, without a bender, from rays + z), L0..L7, Head (alpha in column 3),
+//            Feature, ViewsE + ViewsF (one N = 128 accumulator), Rgb.  The direction of point r is the normalised
+//            backward difference of the bent points r - 1 and r of its ray (r + 1 and r for sample 0), read from the
+//            workspace in global memory, so it does not matter which tile or CTA owns the neighbour.  No bender H
+//            buffer: 24 KB less shared memory than the other kernels.
 #include "field_mma.cuh"
 
 namespace nrn {
@@ -109,8 +117,9 @@ __device__ __forceinline__ void epi_bias_relu_frag(const float (&acc)[kMaskHCols
 // Written as fp16 chunks 0..7 of the row (63 features + one zero pad column).
 // sin/cos: the argument 2^k * x is reduced EXACTLY to [-0.5, 0.5) turns (x / 2pi carried as a
 // two-float value), then evaluated with MUFU (abs err ~4e-7), well below fp16 resolution.
-__device__ __forceinline__ void write_pe(const float (&x)[3], uint8_t* dst_row) {
-  float f[64];
+// The encoding of NF octaves, [x, sin(2^k x), cos(2^k x)] for k < NF, as floats f[0, 3 + 6 NF).
+template <int NF, int NR>
+__device__ __forceinline__ void encode_octaves(const float (&x)[3], float (&f)[NR]) {
   f[0] = x[0]; f[1] = x[1]; f[2] = x[2];
   const float kInv2PiHi = 0.15915494f;      // fl(1/2pi)
   const float kInv2PiLo = 6.4206199e-09f;   // 1/2pi - fl(1/2pi)
@@ -119,7 +128,7 @@ __device__ __forceinline__ void write_pe(const float (&x)[3], uint8_t* dst_row) 
     const float thi = x[d] * kInv2PiHi;
     const float tlo = fmaf(x[d], kInv2PiLo, fmaf(x[d], kInv2PiHi, -thi));
 #pragma unroll
-    for (int k = 0; k < 10; ++k) {
+    for (int k = 0; k < NF; ++k) {
       const float sc = static_cast<float>(1 << k);
       const float a = thi * sc;
       const float ph = (a - rintf(a)) + tlo * sc;
@@ -128,6 +137,11 @@ __device__ __forceinline__ void write_pe(const float (&x)[3], uint8_t* dst_row) 
       f[3 + 6 * k + 3 + d] = __cosf(ang);
     }
   }
+}
+
+__device__ __forceinline__ void write_pe(const float (&x)[3], uint8_t* dst_row) {
+  float f[64];
+  encode_octaves<10>(x, f);
   f[63] = 1.f;  // pad column: its weight column is zero (forward unaffected); WGRAD reads it as the bias input
 #pragma unroll
   for (int c = 0; c < 8; ++c) {
@@ -140,17 +154,71 @@ __device__ __forceinline__ void write_pe(const float (&x)[3], uint8_t* dst_row) 
   }
 }
 
+// Direction encoding of the view-dependent head (embeddirs_fn, get_embedder(multires_views = 4): d, then sin(2^k d),
+// cos(2^k d) for k = 0..3, the same turn reduction as write_pe) as fp16 chunks 0..3 of the row: 27 columns + 5 zero.
+__device__ __forceinline__ void write_dir_enc(const float (&d)[3], uint8_t* dst_row) {
+  float f[32];
+  encode_octaves<4>(d, f);
+#pragma unroll
+  for (int i = views::kDirCols; i < 32; ++i) f[i] = 0.f;
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    uint4 pk;
+    pk.x = pack_h2(f[c * 8 + 0], f[c * 8 + 1]);
+    pk.y = pack_h2(f[c * 8 + 2], f[c * 8 + 3]);
+    pk.z = pack_h2(f[c * 8 + 4], f[c * 8 + 5]);
+    pk.w = pack_h2(f[c * 8 + 6], f[c * 8 + 7]);
+    *reinterpret_cast<uint4*>(dst_row + c * kChunkBytes) = pk;
+  }
+}
+
+// View head: accumulator columns [0, NCOLS) + bias (RELU: then ReLU), fp16 with saturation -> the next step's A fragments
+template <int NCOLS, bool RELU>
+__device__ __forceinline__ void epi_bias_frag(const float (&acc)[NCOLS / 2], const float* __restrict__ bias, uint32_t (&a)[NCOLS / 16][4]) {
+  const int q = acc_q();
+#pragma unroll
+  for (int j = 0; j < NCOLS / 8; ++j) {
+    const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * q));
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const float u = acc[4 * j + 2 * i] + b.x, v = acc[4 * j + 2 * i + 1] + b.y;
+      frag_pair(a, j, i) = RELU ? pack_h2_relu_sat(u, v) : pack_h2_sat(u, v);
+    }
+  }
+}
+
+static_assert(views::step(views::Feature) == fwd::step(fwd::L1), "step_at_views: Feature has the trunk's shape");
+// step -> shape in the view-head kernel's streaming order L0..Head, Feature..Rgb
+__device__ __forceinline__ Step step_at_views(int step) {
+  switch (step) {
+    case fwd::L0: return step_imm<fwd::L0>();
+    case fwd::L5: return step_imm<fwd::L5>();
+    case fwd::Head: return step_imm<fwd::Head>();
+    case views::ViewsE: return step_imm<views::ViewsE>();
+    case views::ViewsF: return step_imm<views::ViewsF>();
+    case views::Rgb: return step_imm<views::Rgb>();
+    default: return step_imm<fwd::L1>();   // L1-L4, L6, L7, Feature
+  }
+}
+
+// Which part of the forward a kernel runs: all of it, the bend pass of the view-dependent head, or its view-head kernel
+enum Part : int { kFull, kBend, kViews };
+
 }  // namespace
 
 // TRAIN: p.stash and p.relu_mask are given (the inference kernel carries none of the mask code).
 // LATENT_BIAS (time-conditioned baseline, no bender): the L0 and L5 epilogues add the ray-bias rows p.ray_bias of their
 // rows' rays instead of the layers' bias vectors.
-template <bool HAS_BENDER, bool TRAIN, bool LATENT_BIAS>
-__device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p) {
+// PART (view-dependent head, inference): kBend runs B0..B4 and writes v.ws; kViews (HAS_BENDER false) runs the trunk
+// and the view head, reading its points and rigidities from v.ws when that is given.
+template <bool HAS_BENDER, bool TRAIN, bool LATENT_BIAS, int PART = kFull>
+__device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p, const ViewParams& v = ViewParams{}) {
   static_assert(!(HAS_BENDER && LATENT_BIAS), "the time-conditioned baseline has no bender");
+  static_assert(PART == kFull || (!TRAIN && !LATENT_BIAS && (PART == kBend) == HAS_BENDER), "view-head parts: inference only");
+  constexpr int kHBytes = PART == kViews ? 0 : kFwdHBytes;   // the view-head kernel has no bender images
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* act = smem;                                  // H (bender) | E, 128 rows
-  uint8_t* ring_buf = smem + kFwdHBytes + kEBytes;      // kFwdRingStages x 32 KB
+  uint8_t* ring_buf = smem + kHBytes + kEBytes;         // kFwdRingStages x 32 KB
   float* stage_all = reinterpret_cast<float*>(ring_buf + kFwdRingStages * kRingStageBytes);   // 2 x 64 rows x kFwdStageLd
   auto* sh = reinterpret_cast<RingShared<kFwdRingStages>*>(stage_all + 2 * kWgRows * kFwdStageLd);
 
@@ -165,7 +233,10 @@ __device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p) {
   if (warp >= 8) {
     setmaxnreg_dec<kProducerRegs>();
     // ===================== weight producer: global -> smem ring (bulk TMA) =====================
-    if (warp == 8 && lane == 0) produce(p.bend_w, p.nerf_w, p.n_tiles, HAS_BENDER ? fwd::B0 : fwd::L0, fwd::kCount, fwd::L0, step_at, ring, W);
+    if (warp == 8 && lane == 0) {
+      if constexpr (PART == kViews) produce(p.nerf_w, v.w, p.n_tiles, fwd::L0, views::kEnd, views::Feature, step_at_views, ring, W);
+      else produce(p.bend_w, p.nerf_w, p.n_tiles, HAS_BENDER ? fwd::B0 : fwd::L0, PART == kBend ? fwd::L0 : fwd::kCount, fwd::L0, step_at, ring, W);
+    }
     return;
   }
 
@@ -177,7 +248,7 @@ __device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p) {
   const int bar = 1 + g;
   const bool wg_leader = tw == 0;
   uint8_t* Hs = act;
-  uint8_t* Es = act + kFwdHBytes;
+  uint8_t* Es = act + kHBytes;
   uint8_t* e_row = Es + (g * kWgRows + tw) * 16;
   const uint32_t a_h = smem_u32(Hs) + g * kWgRows * 16;
   const uint32_t a_e = smem_u32(Es) + g * kWgRows * 16;
@@ -196,7 +267,18 @@ __device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p) {
     long long ray = 0;
     if (valid) {
       ray = pt / p.S;
-      if (p.pts) {
+      if (PART == kViews && v.ws) {
+        // bent point of the bend pass, and the view direction: the normalised backward difference along the ray
+        // (run_nerf_helpers.py:316-356, difference_type "backward"; sample 0 takes sample 1's)
+        const float4 q = __ldg(v.ws + pt);
+        const bool first = pt % p.S == 0;
+        const float4 o = __ldg(v.ws + (first ? pt + 1 : pt - 1));
+        x[0] = q.x; x[1] = q.y; x[2] = q.z;
+        const float dx = first ? o.x - q.x : q.x - o.x, dy = first ? o.y - q.y : q.y - o.y, dz = first ? o.z - q.z : q.z - o.z;
+        const float nrm = __fadd_rn(__fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz))), 1e-6f);
+        my_stg[8] = __fdiv_rn(dx, nrm); my_stg[9] = __fdiv_rn(dy, nrm); my_stg[10] = __fdiv_rn(dz, nrm);
+        my_stg[11] = q.w;   // rigidity, for the object removal
+      } else if (p.pts) {
         const float* q = p.pts + pt * p.pts_stride;  // point mode: NeRF.forward(x) reads x[:, :3]
         x[0] = __ldg(q + 0); x[1] = __ldg(q + 1); x[2] = __ldg(q + 2);
       } else {
@@ -206,6 +288,10 @@ __device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p) {
         x[0] = __fadd_rn(__ldg(r + 0), __fmul_rn(__ldg(r + 3), z));
         x[1] = __fadd_rn(__ldg(r + 1), __fmul_rn(__ldg(r + 4), z));
         x[2] = __fadd_rn(__ldg(r + 2), __fmul_rn(__ldg(r + 5), z));
+      }
+      if (PART == kViews && !v.ws) {   // no bender: the given direction (ray mode: the ray's, point mode: the point's)
+        const float* vd = v.viewdirs + (p.pts ? pt : ray) * v.viewdirs_stride;
+        my_stg[8] = __ldg(vd + 0); my_stg[9] = __ldg(vd + 1); my_stg[10] = __ldg(vd + 2);
       }
       if (p.d_init) {
         p.d_init[pt * 3 + 0] = x[0]; p.d_init[pt * 3 + 1] = x[1]; p.d_init[pt * 3 + 2] = x[2];
@@ -303,6 +389,10 @@ __device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p) {
     if (valid && p.d_bent) {
       p.d_bent[pt * 3 + 0] = x[0]; p.d_bent[pt * 3 + 1] = x[1]; p.d_bent[pt * 3 + 2] = x[2];
     }
+    if constexpr (PART == kBend) {   // the bend pass ends here: bent point and rigidity -> the workspace
+      if (valid) v.ws[pt] = make_float4(x[0], x[1], x[2], rigidity);
+      continue;
+    }
     // ---- positional encoding of the (bent) point -> E ----
     sw.begin();
     if (row_thread) write_pe(x, e_row);
@@ -329,6 +419,52 @@ __device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p) {
         epi_bias_relu_frag<TRAIN>(acc, p.nerf_bias + L * fwd::b_off(fwd::L1), h, st + st_h(L + 1).off, g, mk, kMkH + L * kMaskHBytes);
       }
     }
+    if constexpr (PART == kViews) {
+      // ---- Head: alpha = alpha_linear(h) in column 3 (run_nerf_helpers.py:285) ----
+      {
+        Acc<fwd::Head> acc;
+        wg_gemm_rs<fwd::step(fwd::Head).N, fwd::step(fwd::Head).k16>(acc, h, ring, false, 0u, W, 320);
+        stage_cols<0, 1>(acc, stg, kFwdStageLd);
+        wg_bar(bar);   // also: every warp of this warpgroup is past L5, the last reader of E
+        if (row_thread) {
+          float alpha = my_stg[3] + __ldg(p.nerf_bias + fwd::b_off(fwd::Head) + 3);
+          // test-time non-rigid object removal (run_nerf_helpers.py:309-310)
+          if (v.ws && p.use_removal && my_stg[11] >= p.removal) alpha *= 0.f;
+          const float d[3] = {my_stg[8], my_stg[9], my_stg[10]};
+          my_stg[11] = alpha;
+          write_dir_enc(d, e_row);   // the direction encoding -> E, the A operand of ViewsE
+        }
+      }
+      // ---- Feature: feature_linear(h), no ReLU (run_nerf_helpers.py:286); the result replaces h as the A fragments ----
+      {
+        Acc<views::Feature> acc;
+        wg_gemm_rs<views::step(views::Feature).N, views::step(views::Feature).k16>(acc, h, ring, false, 0u, W, 330);
+        epi_bias_frag<256, false>(acc, v.bias + views::b_off(views::Feature), h);
+      }
+      fence_proxy_async_smem();   // the direction encoding is visible to the tensor cores
+      wg_bar(bar);
+      // ---- views_linears.0 on cat[feature, dirs]: ViewsE (E) then ViewsF (feature fragments), bias + ReLU ----
+      uint32_t hv[8][4];
+      {
+        Acc<views::ViewsF> acc;
+        wg_gemm_rs<views::step(views::ViewsF).N, views::step(views::ViewsF).k16, views::step(views::ViewsE).k16>(acc, h, ring, true, a_e, W, 331);
+        epi_bias_frag<128, true>(acc, v.bias + views::b_off(views::ViewsF), hv);
+      }
+      // ---- Rgb: rgb_linear(hv); raw = [rgb, alpha] (run_nerf_helpers.py:303-304) ----
+      {
+        Acc<views::Rgb> acc;
+        wg_gemm_rs<views::step(views::Rgb).N, views::step(views::Rgb).k16>(acc, hv, ring, false, 0u, W, 332);
+        stage_cols<0, 1>(acc, stg, kFwdStageLd);
+        wg_bar(bar);
+        if (valid) {
+          float* dst = p.raw + pt * 4;
+#pragma unroll
+          for (int c = 0; c < 3; ++c) dst[c] = my_stg[c] + __ldg(v.bias + views::b_off(views::Rgb) + c);
+          dst[3] = my_stg[11];
+        }
+      }
+      continue;
+    }
     // ---- head: raw = output_linear(h) (run_nerf_helpers.py:306) ----
     {
       Acc<fwd::Head> acc;
@@ -354,6 +490,12 @@ template <bool HAS_BENDER, bool TRAIN>
 __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kernel(const FieldFwdParams p) { field_fwd_body<HAS_BENDER, TRAIN, false>(p); }
 template <bool TRAIN>
 __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_tc_kernel(const FieldFwdParams p) { field_fwd_body<false, TRAIN, true>(p); }
+__global__ void __launch_bounds__(kFwdThreads, 1) field_bend_kernel(const FieldFwdParams p, const ViewParams v) {
+  field_fwd_body<true, false, false, kBend>(p, v);
+}
+__global__ void __launch_bounds__(kFwdThreads, 1) field_views_kernel(const FieldFwdParams p, const ViewParams v) {
+  field_fwd_body<false, false, false, kViews>(p, v);
+}
 
 // Ray bias of the time-conditioned baseline: rb[n][l][o] = b_l[o] + sum_k W_l[o][63 + k] z[n][k] for l = L0, L5, in fp32
 // from the nn.Linear weights (W0 [256][95], W5 [256][351]).  Thread o of a block keeps both layers' 32 latent weights
@@ -399,6 +541,27 @@ cudaError_t launch_field_fwd(const FieldFwdParams& p, bool has_bender, int num_s
   const bool train = p.relu_mask != nullptr;   // the C ABI passes the ReLU masks exactly when it passes the stash
   if (has_bender) return launch_field(train ? field_fwd_kernel<true, true> : field_fwd_kernel<true, false>, p, num_sms, smem, stream);
   return launch_field(train ? field_fwd_kernel<false, true> : field_fwd_kernel<false, false>, p, num_sms, smem, stream);
+}
+
+// The view-dependent head: with a bender the bend pass (-> v.ws) runs first, then the view-head kernel (c_abi.cu)
+size_t field_views_smem_bytes() { return kFwdSmemBytes - kFwdHBytes; }
+
+cudaError_t launch_field_bend(const FieldFwdParams& p, const ViewParams& v, int num_sms, cudaStream_t stream) {
+  if (p.n_tiles <= 0) return cudaSuccess;
+  const size_t smem = field_fwd_smem_bytes();
+  cudaError_t e = cudaFuncSetAttribute(field_bend_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  field_bend_kernel<<<p.n_tiles < num_sms ? p.n_tiles : num_sms, kFwdThreads, smem, stream>>>(p, v);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_field_views(const FieldFwdParams& p, const ViewParams& v, int num_sms, cudaStream_t stream) {
+  if (p.n_tiles <= 0) return cudaSuccess;
+  const size_t smem = field_views_smem_bytes();
+  cudaError_t e = cudaFuncSetAttribute(field_views_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  field_views_kernel<<<p.n_tiles < num_sms ? p.n_tiles : num_sms, kFwdThreads, smem, stream>>>(p, v);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_field_fwd_tc(const FieldFwdParams& p, int num_sms, cudaStream_t stream) {

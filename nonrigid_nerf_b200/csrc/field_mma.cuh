@@ -108,8 +108,8 @@ __device__ __forceinline__ void wg_gemm(float (&acc)[N / 2], Ring<S>& r, uint32_
 
 // wg_gemm with the A operand in registers: slab j (K16 MMAs) takes the A fragments K16 j .. K16 j + K16 - 1 of `a`, the
 // fragments of this warpgroup's 64 rows x 16 KF columns (sm90_ptx.cuh: wgmma_rs).  lead: one slab of K16 MMAs with A from
-// shared memory at a_lead (as in wg_gemm) comes first (the embedding columns of the skip layer).
-template <int N, int K16, int KF, int S>
+// shared memory at a_lead (as in wg_gemm) comes first (the embedding columns of the skip layer); it has LEAD_K16 MMAs.
+template <int N, int K16, int LEAD_K16 = K16, int KF, int S>
 __device__ __forceinline__ void wg_gemm_rs(float (&acc)[N / 2], uint32_t (&a)[KF][4], Ring<S>& r, bool lead, uint32_t a_lead,
                                            const Waiter& W, int code) {
   static_assert(KF % K16 == 0, "whole slabs of A fragments");
@@ -124,7 +124,7 @@ __device__ __forceinline__ void wg_gemm_rs(float (&acc)[N / 2], uint32_t (&a)[KF
     acc_fence(acc);
     wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < K16; ++k)
+    for (int k = 0; k < LEAD_K16; ++k)
       wgmma<N, 0, 0>(acc, gmma_desc_advance(adesc, k * 2 * kChunkBytes), gmma_desc_advance(bdesc, k * 2 * N * 16), k ? 1u : 0u);
     wgmma_commit();
     prev = r.stage;

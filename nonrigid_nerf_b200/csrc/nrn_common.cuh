@@ -102,6 +102,34 @@ constexpr int kBendPackedBytes = kBendTLoOffset + kBendTWBytes;
 static_assert(kNerfWBytes == 991232 && kNerfTWBytes == 991232 && kBendWBytes == 53248 && kBendTWBytes == 53248, "weight images");
 static_assert(kNerfBiasFloats == 8 * 256 + 16 && kBendBiasFloats == 96 + 96 + 80 + 64, "biases");
 
+// View-dependent head of NeRF(use_viewdirs=True), forward only.  The trunk runs L0..L7 and the Head step unchanged, the
+// head image holding alpha_linear in row 3 (rows 0-2 zero), so the Head step yields alpha in column 3.  Then, in streaming
+// order after Head: feature_linear (no ReLU), views_linears.0 split at input column 256 into its direction-encoding columns
+// (ViewsE, K = 27 padded to 32, A from shared memory) and its feature columns (ViewsF, A = the feature fragments), both
+// into one N = 128 accumulator, and rgb_linear (N = 3 padded to 16).  Step ids continue the forward table; the images are
+// a packed block of their own: forward images Feature..Rgb | fp32 biases (feature 256 | views 128 | rgb 16).
+namespace views {
+enum Id : int { Feature = fwd::kCount, ViewsE, ViewsF, Rgb, kEnd };
+constexpr int kDirCols = 27;   // direction encoding: d, then sin(2^k d), cos(2^k d) for k = 0..3
+__host__ __device__ constexpr WImage image(int s) {
+  switch (s) {
+    case Feature: return {256, 32};
+    case ViewsE: return {128, 4};
+    case ViewsF: return {128, 32};
+    default: return {16, 16};     // Rgb
+  }
+}
+__host__ __device__ constexpr Step step(int s) { return make_step(image(s)); }
+__host__ __device__ constexpr int w_off(int s) { int o = 0; for (int i = Feature; i < s; ++i) o += image(i).bytes(); return o; }
+// ViewsE and ViewsF share the views layer's bias (stored once, at ViewsF's offset)
+__host__ __device__ constexpr int b_off(int s) { int o = 0; for (int i = Feature; i < s; ++i) o += i == ViewsE ? 0 : image(i).rows; return o; }
+}  // namespace views
+constexpr int kViewsWBytes = views::w_off(views::kEnd);
+constexpr int kViewsBiasFloats = views::b_off(views::kEnd);
+constexpr int kViewsPackedBytes = kViewsWBytes + kViewsBiasFloats * 4;
+static_assert(views::b_off(views::ViewsE) == 256 && views::b_off(views::ViewsF) == 256 && views::b_off(views::Rgb) == 384, "view biases");
+static_assert(kViewsWBytes == 208896 && kViewsPackedBytes == 210496, "view-head images");
+
 // A tile image of the stashes: `chunks` 8-column chunks of 128 rows (fp16, chunk-major) at byte `off` of the tile.
 struct Image {
   int off, chunks;
@@ -232,6 +260,15 @@ struct FieldFwdParams {
   uint8_t* relu_mask;     // training only (with stash): ReLU masks [n_tiles rounded up to even][kMaskTileBytes]
   const float* ray_bias;  // time-conditioned kernels only: [ray][2][256] biases of L0 / L5 (stride ray_bias_stride floats,
   long long ray_bias_stride;   // 0 = one row for every ray); the other kernels ignore both
+};
+
+// View-dependent head (field_fwd.cu: the bend pass and the view-head kernel), next to a FieldFwdParams
+struct ViewParams {
+  const uint8_t* w;            // nrn_pack_views images ...
+  const float* bias;           // ... and biases
+  const float* viewdirs;       // no bender: normalised view directions, one row per ray (ray mode) or point (point mode)
+  long long viewdirs_stride;   // floats between rows
+  float4* ws;                  // bend workspace [P]: bent xyz and rigidity of every point (bend pass out, view head in)
 };
 
 // Time-conditioned backward: the per-ray sums s_l[ray] = sum over the ray's samples of dY_l (l = L0, L5), d z and the

@@ -204,7 +204,48 @@ __global__ void __launch_bounds__(kPackThreads) pack_bender_kernel(BenderSrc src
   else pack_bender_t_elem((blockIdx.x - nb_fwd) * kPackThreads + threadIdx.x, src, wt, wtlo);
 }
 
+// View-dependent head (layout in nrn_common.cuh, views::): feature_linear; views_linears.0 split at input column 256
+// into its direction-encoding columns (ViewsE, K = 27 padded to 32) and its feature columns (ViewsF); rgb_linear (N = 3
+// padded to 16).  Forward images only.
+__global__ void __launch_bounds__(kPackThreads) pack_views_kernel(ViewsSrc src, __half* __restrict__ w, float* __restrict__ bias) {
+  using namespace views;
+  constexpr WImage wf = image(Feature), we = image(ViewsE), wv = image(ViewsF), wr = image(Rgb);
+  constexpr int nf = wf.bytes() / 2, ne = we.bytes() / 2, nv = wv.bytes() / 2;
+  constexpr int ldv = 256 + kDirCols;   // views_linears.0: [feature(256) | direction encoding(27)] inputs
+  const int idx = blockIdx.x * kPackThreads + threadIdx.x;
+  if (idx < kViewsWBytes / 2) {
+    int i = idx, k, r;
+    float v = 0.f;
+    if (i < nf) {                          // Feature
+      decode(i, wf.rows, k, r);
+      v = src.w[0][r * 256 + k];
+    } else if ((i -= nf) < ne) {           // ViewsE: K = direction encoding, padded to 32
+      decode(i, we.rows, k, r);
+      v = k < kDirCols ? src.w[1][r * ldv + 256 + k] : 0.f;
+    } else if ((i -= ne) < nv) {           // ViewsF: K = feature
+      decode(i, wv.rows, k, r);
+      v = src.w[1][r * ldv + k];
+    } else {                               // Rgb: N = 3 padded to 16
+      i -= nv;
+      decode(i, wr.rows, k, r);
+      v = r < 3 ? src.w[2][r * 128 + k] : 0.f;
+    }
+    w[idx] = __float2half_rn(v);
+  }
+  if (idx < kViewsBiasFloats) {
+    constexpr int bv = b_off(ViewsF), br = b_off(Rgb);
+    bias[idx] = idx < bv ? src.b[0][idx] : idx < br ? src.b[1][idx - bv] : (idx - br < 3 ? src.b[2][idx - br] : 0.f);
+  }
+}
+
 }  // namespace
+
+cudaError_t launch_pack_views(const ViewsSrc& src, void* packed, cudaStream_t st) {
+  uint8_t* base = reinterpret_cast<uint8_t*>(packed);
+  const int nb = (kViewsWBytes / 2 + kPackThreads - 1) / kPackThreads;
+  pack_views_kernel<<<nb, kPackThreads, 0, st>>>(src, reinterpret_cast<__half*>(base), reinterpret_cast<float*>(base + kViewsWBytes));
+  return cudaGetLastError();
+}
 
 // packed = [forward images | biases | transposed images] (+ the bender's residual images; offsets in nrn_common.cuh)
 cudaError_t launch_pack_nerf(const NerfSrc& src, int in_ch, int out_ch, void* packed, cudaStream_t st) {

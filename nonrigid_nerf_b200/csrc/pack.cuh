@@ -15,7 +15,13 @@ struct BenderSrc {
   const float* rig_b[3];  // ray_bending.rigidity_network.0-2.bias
 };
 
+struct ViewsSrc {
+  const float* w[3];  // feature_linear.weight [256][256], views_linears.0.weight [128][256 + 27], rgb_linear.weight [3][128]
+  const float* b[3];  // their biases
+};
+
 cudaError_t launch_pack_nerf(const NerfSrc& src, int in_ch, int out_ch, void* packed, cudaStream_t st);
 cudaError_t launch_pack_bender(const BenderSrc& src, void* packed, cudaStream_t st);
+cudaError_t launch_pack_views(const ViewsSrc& src, void* packed, cudaStream_t st);
 
 }  // namespace nrn

@@ -69,9 +69,17 @@ def bender_param_list(bender):
     return net_w, net_b, rig_w, rig_b
 
 
+def _views_trunk_params(net):
+    """The trunk and alpha_linear of a NeRF(use_viewdirs=True)"""
+    return ([net.pts_linears[i].weight for i in range(8)] + [net.alpha_linear.weight],
+            [net.pts_linears[i].bias for i in range(8)] + [net.alpha_linear.bias])
+
+
 def pack_nerf(net) -> torch.Tensor:
-    """fp16 wgmma operand image of a NeRF module's weights (see csrc/nrn_common.cuh)."""
-    ws, bs = nerf_param_list(net)
+    """fp16 wgmma operand image of a NeRF module's weights (see csrc/nrn_common.cuh).  With use_viewdirs=True the head
+    of the image is alpha_linear in row 3 under three zero rows, so the head step yields alpha in channel 3."""
+    views = getattr(net, "use_viewdirs", False)
+    ws, bs = _views_trunk_params(net) if views else nerf_param_list(net)
     key = _versions(ws + bs)
     cache = getattr(net, "_nrn_pack", None)
     if cache is not None and cache[0] == key and not FORCE_PACK:
@@ -85,11 +93,42 @@ def pack_nerf(net) -> torch.Tensor:
         raise RuntimeError("nonrigid_nerf_b200: only D=8, W=256, skips=[4], multires=10, use_viewdirs=False is implemented "
                            f"(got layer shapes {[tuple(w.shape) for w in ws]})")
     buf = cache[1] if cache is not None else torch.empty(lib.nrn_packed_nerf_bytes(), dtype=torch.uint8, device=ws[0].device)
+    if views:   # [0, 0, 0, alpha]: the head rows of rgb + alpha
+        ws = ws[:8] + [torch.cat([ws[8].new_zeros(3, ws[8].shape[1]), ws[8]], 0)]
+        bs = bs[:8] + [torch.cat([bs[8].new_zeros(3), bs[8]], 0)]
     out_ch = ws[8].shape[0]
     with torch.cuda.device(ws[0].device):
         _lib.check(lib.nrn_pack_nerf(_ptr_array([w.detach() for w in ws]), _ptr_array([b.detach() for b in bs]), in_ch, out_ch,
                                      _ptr(buf), _stream()), "pack_nerf")
     net._nrn_pack = (key, buf)
+    return buf
+
+
+def views_param_list(net):
+    ws = [net.feature_linear.weight, net.views_linears[0].weight, net.rgb_linear.weight]
+    bs = [net.feature_linear.bias, net.views_linears[0].bias, net.rgb_linear.bias]
+    return ws, bs
+
+
+def pack_views(net) -> torch.Tensor:
+    """fp16 wgmma operand images of the view-dependent head (feature_linear, views_linears.0, rgb_linear)."""
+    ws, bs = views_param_list(net)
+    key = _versions(ws + bs)
+    cache = getattr(net, "_nrn_pack_views", None)
+    if cache is not None and cache[0] == key and not FORCE_PACK:
+        return cache[1]
+    lib = _lib.load()
+    for t in ws + bs:
+        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
+            raise RuntimeError("nonrigid_nerf_b200: NeRF parameters must be contiguous fp32 CUDA tensors")
+    if ws[0].shape != (256, 256) or ws[1].shape != (128, 256 + 27) or ws[2].shape != (3, 128):
+        raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True needs W=256 and input_ch_views=27 "
+                           f"(got view-head shapes {[tuple(w.shape) for w in ws]})")
+    buf = cache[1] if cache is not None else torch.empty(lib.nrn_packed_views_bytes(), dtype=torch.uint8, device=ws[0].device)
+    with torch.cuda.device(ws[0].device):
+        _lib.check(lib.nrn_pack_views(_ptr_array([w.detach() for w in ws]), _ptr_array([b.detach() for b in bs]), _ptr(buf), _stream()),
+                   "pack_views")
+    net._nrn_pack_views = (key, buf)
     return buf
 
 
@@ -250,6 +289,90 @@ def field_forward_points(points: torch.Tensor, latents: Optional[torch.Tensor], 
     """Point mode (NeRF.forward(x)): one xyz (+ one latent) per row; returns raw [P, 1, out_ch]."""
     return _field(None, None, points, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details,
                   tc_net=tc_net)
+
+
+def field_forward_views(rays: Optional[torch.Tensor], z_vals: Optional[torch.Tensor], points: Optional[torch.Tensor], n_samples: int,
+                        latents: Optional[torch.Tensor], viewdirs: Optional[torch.Tensor], nerf_pack: torch.Tensor,
+                        bender_pack: Optional[torch.Tensor], views_pack: Optional[torch.Tensor], cutoff=None, scaling=None,
+                        removal=None, want_details: bool = False) -> Tuple[Optional[torch.Tensor], Dict[str, torch.Tensor]]:
+    """The view-dependent head (inference): raw [N, S, 4] = [rgb, alpha].  Ray mode: rays [N, 8+] and z_vals [N, S].
+    Point mode: points [P, 3+] with P = N * n_samples, n_samples consecutive points forming one ray (the finite
+    differences of the bent points run inside each), latents per point.  With a bender the view directions are those
+    differences; without one `viewdirs` (per ray, or per point in point mode) is used.  views_pack = None with a bender
+    runs the bend pass alone (raw is None; the details are filled)."""
+    a = _lib.NrnFieldArgs()
+    v = _lib.NrnViewArgs()
+    keep = []
+    if points is None:
+        rays = rays if (rays.dtype == torch.float32 and rays.stride(-1) == 1) else rays.float().contiguous()
+        if not rays.is_cuda:
+            raise RuntimeError("nonrigid_nerf_b200: rays must be a CUDA tensor (there is no CPU path)")
+        z_vals = _f32c(z_vals, "z_vals")
+        n, s = z_vals.shape
+        dev = rays.device
+        if rays.stride(0) != 8:
+            rays = rays[:, :8].contiguous()
+        a.rays, a.z_vals = rays.data_ptr(), z_vals.data_ptr()
+        keep += [rays, z_vals]
+    else:
+        if not points.is_cuda:
+            raise RuntimeError("nonrigid_nerf_b200: points must be a CUDA tensor (there is no CPU path)")
+        if points.dtype != torch.float32 or points.dim() != 2 or points.stride(1) != 1:
+            points = points.reshape(points.shape[0], -1).float().contiguous()
+        s = n_samples
+        if points.shape[0] % s:
+            raise RuntimeError(f"nonrigid_nerf_b200: use_viewdirs=True: {points.shape[0]} points do not form rays of num_ray_samples={s}")
+        n = points.shape[0] // s
+        dev = points.device
+        a.points, a.points_stride = points.data_ptr(), points.stride(0)
+        keep.append(points)
+    a.n_rays, a.n_samples = n, s
+    a.nerf_packed = nerf_pack.data_ptr()
+    lib = _lib.load()
+    if bender_pack is not None:
+        if latents is None:
+            raise RuntimeError("nonrigid_nerf_b200: ray bending needs latents")
+        latents, stride = latent_rows(latents, n * s if points is not None else n, dev)
+        a.latents, a.latent_stride = latents.data_ptr(), stride
+        a.bender_packed = bender_pack.data_ptr()
+        ws = torch.empty(lib.nrn_views_workspace_bytes(n, s), dtype=torch.uint8, device=dev)
+        v.workspace = ws.data_ptr()
+        keep += [latents, ws]
+    else:
+        if viewdirs is None:
+            raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True without a ray bender needs the view directions")
+        if viewdirs.dtype != torch.float32 or viewdirs.dim() != 2 or viewdirs.stride(1) != 1 or not viewdirs.is_cuda:
+            viewdirs = viewdirs.reshape(viewdirs.shape[0], -1).float().contiguous().to(dev)
+        v.viewdirs, v.viewdirs_stride = viewdirs.data_ptr(), viewdirs.stride(0) if viewdirs.shape[0] > 1 else 3
+        keep.append(viewdirs)
+    a.out_ch = 4
+    if cutoff is not None:
+        a.use_cutoff, a.rigidity_cutoff = 1, float(cutoff)
+    if scaling is not None:
+        a.use_scaling, a.scaling = 1, float(scaling)
+    if removal is not None:
+        a.use_removal, a.removal_threshold = 1, float(removal)
+    raw = None
+    if views_pack is not None:
+        raw = torch.empty(n, s, 4, dtype=torch.float32, device=dev)
+        a.raw = raw.data_ptr()
+        v.views_packed = views_pack.data_ptr()
+    details: Dict[str, torch.Tensor] = {}
+    if want_details:
+        details["initial_input_pts"] = torch.empty(n, s, 3, dtype=torch.float32, device=dev)
+        details["input_pts"] = torch.empty(n, s, 3, dtype=torch.float32, device=dev)
+        a.initial_input_pts, a.input_pts = details["initial_input_pts"].data_ptr(), details["input_pts"].data_ptr()
+        if bender_pack is not None:
+            details["unmasked_offsets"] = torch.empty(n, s, 3, dtype=torch.float32, device=dev)
+            details["masked_offsets"] = torch.empty(n, s, 3, dtype=torch.float32, device=dev)
+            details["rigidity_mask"] = torch.empty(n, s, 1, dtype=torch.float32, device=dev)
+            a.unmasked_offsets = details["unmasked_offsets"].data_ptr()
+            a.masked_offsets = details["masked_offsets"].data_ptr()
+            a.rigidity_mask = details["rigidity_mask"].data_ptr()
+    a.stream = torch.cuda.current_stream().cuda_stream
+    with torch.cuda.device(dev):
+        _lib.check(lib.nrn_field_forward_views(C.byref(a), C.byref(v)), "field_forward_views")
+    return raw, details
 
 
 def composite(raw: torch.Tensor, z_vals: torch.Tensor, rays_d: torch.Tensor, noise: Optional[torch.Tensor] = None,

@@ -261,6 +261,9 @@ class training_wrapper_class(torch.nn.Module):
 
     def forward(self, args, rays_o, rays_d, i, render_kwargs_train, target_s, global_step, start, dataset_extras,
                 batch_pixel_indices):
+        for net in (self.coarse_model, self.fine_model):   # the view-dependent head cannot be trained yet: raise before any launch
+            if net is not None:
+                _ag.views_check(net)
         self.coarse_model.ray_bender = (self.ray_bender,)
         render_kwargs_train["network_fn"] = self.coarse_model
         render_kwargs_train["ray_bender"] = self.ray_bender

@@ -137,7 +137,18 @@ class NeRF(nn.Module):
                  approx_nonrigid_viewdirs=True, time_conditioned_baseline=False):
         super().__init__()
         if use_viewdirs:
-            raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True is not implemented yet (SURVEY.md 8f row f1)")
+            # the view-dependent head (run_nerf_helpers.py:233-236, 284-304), inference only; training raises at call time
+            if input_ch_views != 27:
+                raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True needs input_ch_views=27 (multires_views=4), "
+                                   f"got {input_ch_views}")
+            if time_conditioned_baseline:
+                raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True together with time_conditioned_baseline is not implemented")
+            if ray_bender is not None and not approx_nonrigid_viewdirs:
+                raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True with approx_nonrigid_viewdirs=False (exact view "
+                                   "directions through the ray bender) is not implemented")
+            if ray_bender is not None and (num_ray_samples is None or num_ray_samples < 2):
+                raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True with a ray bender needs num_ray_samples >= 2 "
+                                   f"(finite-difference view directions), got {num_ray_samples}")
         if time_conditioned_baseline and ray_bending_latent_size != ops.LATENT:
             raise RuntimeError("nonrigid_nerf_b200: time_conditioned_baseline needs ray_bending_latent_size=32 "
                                f"(got {ray_bending_latent_size})")
@@ -160,8 +171,14 @@ class NeRF(nn.Module):
         lin_in = input_ch + (ray_bending_latent_size if time_conditioned_baseline else 0)
         self.pts_linears = nn.ModuleList([nn.Linear(lin_in, W)] + [nn.Linear(W, W) if i not in skips else nn.Linear(W + lin_in, W)
                                                                     for i in range(D - 1)])
-        self.views_linears = nn.ModuleList([nn.Linear(input_ch_views + W, W // 2)])  # dead weight, kept for checkpoints
-        self.output_linear = nn.Linear(W, output_ch)
+        # use_viewdirs=False: views_linears is dead weight, kept for checkpoints
+        self.views_linears = nn.ModuleList([nn.Linear(input_ch_views + W, W // 2)])
+        if use_viewdirs:
+            self.feature_linear = nn.Linear(W, W)
+            self.alpha_linear = nn.Linear(W, 1)
+            self.rgb_linear = nn.Linear(W // 2, 3)
+        else:
+            self.output_linear = nn.Linear(W, output_ch)
 
     def forward(self, x, detailed_output=False):
         """x: [P, input_ch + input_ch_views + latent] as built by run_network; only x[:, :3] (raw xyz)
@@ -169,7 +186,14 @@ class NeRF(nn.Module):
         p = x.shape[0]
         pts = x[:, :3]
         lat = x[:, self.input_ch + self.input_ch_views:] if self.ray_bending_latent_size > 0 else None
-        raw, details = _ag.field_points(self, pts, lat, detailed_output)
+        if self.use_viewdirs:
+            # with a bender the rows form rays of num_ray_samples points (their bent points give the view directions,
+            # run_nerf_helpers.py:316-356); without one the direction is the first three view columns (the raw d of the
+            # embedded directions)
+            vd = x[:, self.input_ch:self.input_ch + 3]
+            raw, details = _ag.field_views(self, None, None, pts, lat, vd, detailed_output)
+        else:
+            raw, details = _ag.field_points(self, pts, lat, detailed_output)
         raw = raw.reshape(p, -1)
         if detailed_output:
             return raw, {k: v.reshape(p, -1) for k, v in details.items()}

@@ -43,13 +43,19 @@ def batchify(fn, chunk, detailed_output=False):
 def run_network(inputs, viewdirs, additional_pixel_information, fn, embed_fn, embeddirs_fn, netchunk=1024 * 64,
                 detailed_output=False):
     """Prepares inputs and applies network `fn` (train.py:57-105).  inputs: [N_rays, N_samples, 3]."""
-    if viewdirs is not None:
-        raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True is not implemented yet (SURVEY.md 8f row f1)")
+    views = getattr(fn, "use_viewdirs", False)
+    if (viewdirs is not None) != views:
+        raise RuntimeError("nonrigid_nerf_b200: " + ("a use_viewdirs=True model needs viewdirs" if views else
+                                                     "viewdirs given to a model without the view-dependent head (use_viewdirs=False)"))
     n, s = inputs.shape[0], inputs.shape[1]
     latents = additional_pixel_information["ray_bending_latents"]
     pts = inputs.reshape(-1, 3)
     lat = latents[:, None].expand(n, s, latents.shape[-1]).reshape(n * s, latents.shape[-1])
-    raw, details = _ag.field_points(fn, pts, lat, detailed_output)
+    if views:   # the ray's direction for each of its samples (train.py:79-84); with a bender the kernels use the bent points'
+        vd = viewdirs[:, None].expand(n, s, 3).reshape(n * s, 3)
+        raw, details = _ag.field_views(fn, None, None, pts, lat, vd, detailed_output)
+    else:
+        raw, details = _ag.field_points(fn, pts, lat, detailed_output)
     outputs = raw.reshape(n, s, -1)
     if detailed_output:
         return outputs, {k: v.reshape(n, s, -1) for k, v in details.items()}
@@ -80,13 +86,16 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     re-seeds numpy instead, train.py:863-867)."""
     if pytest:
         raise RuntimeError("nonrigid_nerf_b200: the pytest= numpy-random hook is not supported")
-    if ray_batch.shape[-1] > 8:
-        raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True is not implemented yet (SURVEY.md 8f row f1)")
     if not isinstance(network_fn, NeRF) or (network_fine is not None and not isinstance(network_fine, NeRF)):
         raise RuntimeError("nonrigid_nerf_b200: render_rays needs nonrigid_nerf_b200.run_nerf_helpers.NeRF modules")
+    _check_views(ray_batch.shape[-1] > 8, network_fn, network_fine if N_importance > 0 else None, additional_pixel_information)
     n = ray_batch.shape[0]
     dev = ray_batch.device
     rays = ray_batch if (ray_batch.dtype == torch.float32 and ray_batch.is_contiguous()) else ray_batch.float().contiguous()
+    viewdirs = None
+    if rays.shape[-1] > 8:   # (o, d, near, far, viewdirs): train.py:843
+        viewdirs = rays[:, -3:]
+        rays = rays[:, :8].contiguous()
     rays_d = rays[:, 3:6]
     latents = None
     if network_fn.ray_bender[0] is not None or getattr(network_fn, "time_conditioned_baseline", False):
@@ -125,7 +134,7 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     # coarse depths (train.py:847-869); t_rand drawn first, like the reference
     t_rand = draw("t_rand", torch.rand, n, N_samples) if perturb > 0.0 else None
     z_vals = ops.sample_coarse(rays, N_samples, t_rand, lindisp)
-    raw, details = _ag.field(network_fn, rays, z_vals, latents, detailed_output)
+    raw, details = _ag.field(network_fn, rays, z_vals, latents, detailed_output, viewdirs)
     noise = draw("noise_c", torch.randn, n, N_samples) if raw_noise_std > 0.0 else None   # already scaled by raw_noise_std
 
     if N_importance > 0:
@@ -133,7 +142,7 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
         c0 = _ag.composite(raw, z_vals, rays_d, noise, white_bkgd, N_importance, u)
         z_fine = c0["z_vals_out"]   # sorted union, detached (train.py:918-920)
         run_fn = network_fn if network_fine is None else network_fine
-        raw, fine_details = _ag.field(run_fn, rays, z_fine, latents, detailed_output)
+        raw, fine_details = _ag.field(run_fn, rays, z_fine, latents, detailed_output, viewdirs)
         noise_f = draw("noise_f", torch.randn, n, n_fine) if raw_noise_std > 0.0 else None
         c1 = _ag.composite(raw, z_fine, rays_d, noise_f, white_bkgd)
     else:
@@ -150,7 +159,12 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
             idx = ops.median_visibility_index(c1["weights"])
             z_s = torch.gather(z_fine, 1, idx[:, None])
             pts = rays[:, 0:3] + rays[:, 3:6] * z_s          # multiply, then add: the same rounding as the field kernel
-            _, det = _ag.field_points(run_fn, pts, latents, True)
+            if not getattr(run_fn, "use_viewdirs", False):
+                _, det = _ag.field_points(run_fn, pts, latents, True)
+            elif run_fn.ray_bender[0] is not None:   # the surface point and rigidity do not depend on the head: bend pass alone
+                _, det = _ag.field_views(run_fn, None, None, pts, latents, None, True, bend_only=True)
+            else:                                     # no bender: the point itself
+                det = {"input_pts": pts}
         ret["median_indices"] = idx
         ret["surface_pts"] = det["input_pts"].reshape(n, 3)
         if "rigidity_mask" in det:
@@ -178,6 +192,21 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     return ret
 
 
+def _check_views(batch_has_viewdirs, network_fn, network_fine, additional_pixel_information):
+    """Before any launch: the ray batch carries view directions exactly when the models have the view-dependent head,
+    and that head is only evaluated without autograd (_ag.views_check)."""
+    for net in (network_fn, network_fine):
+        if net is None:
+            continue
+        if getattr(net, "use_viewdirs", False) != batch_has_viewdirs:
+            raise RuntimeError("nonrigid_nerf_b200: " + ("a use_viewdirs=True model needs ray batches with view directions "
+                                                         "(render(use_viewdirs=True), 11 columns)" if not batch_has_viewdirs else
+                                                         "ray batch with view directions (use_viewdirs=True) for a model "
+                                                         "without the view-dependent head"))
+        info = additional_pixel_information or {}
+        _ag.views_check(net, info.get("ray_bending_latents"))
+
+
 # ---- batchify_rays / render (train.py:108-137, :326-416) --------------------------------------------
 def batchify_rays(rays_flat, additional_pixel_information, chunk=1024 * 32, detailed_output=False, **kwargs):
     """Render rays in chunks (`chunk` only bounds the per-launch working set; results do not depend on it)."""
@@ -193,8 +222,15 @@ def batchify_rays(rays_flat, additional_pixel_information, chunk=1024 * 32, deta
 def render(rays_o, rays_d, chunk=1024 * 32, ndc=True, near=0.0, far=1.0, use_viewdirs=False, c2w_staticcam=None,
            additional_pixel_information=None, detailed_output=False, **kwargs):
     """Render rays.  Returns [rgb_map, disp_map, acc_map, extras] (train.py:326-416)."""
-    if use_viewdirs:
-        raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True is not implemented yet (SURVEY.md 8f row f1)")
+    if kwargs.get("network_fn") is not None:
+        _check_views(bool(use_viewdirs), kwargs["network_fn"], kwargs.get("network_fine") if kwargs.get("N_importance", 0) > 0 else None,
+                     additional_pixel_information)
+    viewdirs = None
+    if use_viewdirs:   # provide ray directions as input (train.py:364-381)
+        if c2w_staticcam is not None:
+            raise RuntimeError("need to pull this call to get_rays out to render_path() for gpu parallelization to work")
+        viewdirs = rays_d / torch.norm(rays_d, dim=-1, keepdim=True)
+        viewdirs = torch.reshape(viewdirs, [-1, 3]).float()
     sh = rays_d.shape
     if ndc:
         raise RuntimeError("not implemented. change H, W, focal to use ray_params instead")  # train.py:384-386
@@ -208,6 +244,8 @@ def render(rays_o, rays_d, chunk=1024 * 32, ndc=True, near=0.0, far=1.0, use_vie
         rays = torch.cat([rays_o, rays_d, near_t, far_t], -1)
     else:
         rays = ops.pack_rays(rays_o, rays_d, float(near), float(far))     # scalar bounds (train.py:1463-1468): one launch
+    if viewdirs is not None:
+        rays = torch.cat([rays, viewdirs], -1)                               # train.py:398-399
     all_ret = batchify_rays(rays, additional_pixel_information, chunk=chunk, detailed_output=detailed_output, **kwargs)
     for k in all_ret:
         all_ret[k] = torch.reshape(all_ret[k], list(sh[:-1]) + list(all_ret[k].shape[1:]))
