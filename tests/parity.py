@@ -23,8 +23,16 @@ def half_ulp(x):
 
 
 class Report:
-    def __init__(self, tag):
-        self.tag = tag
+    """quiet: print nothing per check; worst() prints the largest c_obs / relative L2 of each stage seen so far."""
+    def __init__(self, tag, quiet=False):
+        self.tag, self.quiet = tag, quiet
+        self.c_obs, self.l2 = {}, {}
+
+    def worst(self):
+        for stage, (obs, c) in self.c_obs.items():
+            print(f"  [{self.tag}] {stage:<24s} worst c_obs {obs:10.3f}   c {c}")
+        for stage, (d, tol) in self.l2.items():
+            print(f"  [{self.tag}] {stage:<24s} worst rel L2 {d:.3e}   bound {tol:.0e}")
 
     def check(self, stage, got, exact, absb, c, fp16=False, floor=0.0):
         got = got.to(F64)
@@ -38,7 +46,10 @@ class Report:
             err = (err - floor).clamp_min(0.0)
         ratio = torch.where(err == 0, torch.zeros_like(err), err / (U * absb))
         obs = float(ratio.max()) if ratio.numel() else 0.0
-        print(f"  [{self.tag}] {stage:<24s} c_obs {obs:10.3f}   c {c}")
+        if obs >= self.c_obs.get(stage, (-1.0, c))[0]:
+            self.c_obs[stage] = (obs, c)
+        if not self.quiet:
+            print(f"  [{self.tag}] {stage:<24s} c_obs {obs:10.3f}   c {c}")
         if not obs <= c:
             i = int(ratio.flatten().argmax())
             raise AssertionError(f"{self.tag} {stage}: |kernel - exact| exceeds the bound, c_obs {obs:.4g} > c {c}; worst element "
@@ -48,7 +59,10 @@ class Report:
 
     def rel_l2(self, stage, got, exact, tol):
         d = float((got.to(F64) - exact).norm() / (exact.norm() + 1e-300))
-        print(f"  [{self.tag}] {stage:<24s} rel L2 {d:.3e}   bound {tol:.0e}")
+        if d >= self.l2.get(stage, (-1.0, tol))[0]:
+            self.l2[stage] = (d, tol)
+        if not self.quiet:
+            print(f"  [{self.tag}] {stage:<24s} rel L2 {d:.3e}   bound {tol:.0e}")
         assert d <= tol, (self.tag, stage, d)
 
 

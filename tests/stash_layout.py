@@ -52,11 +52,32 @@ A_4, A_3, A_2, A_1, A_0 = (0, 2), (2 * CHUNK, 8), (10 * CHUNK, 10), (20 * CHUNK,
 ADJ_TILE = 44 * CHUNK
 
 
-def image(buf, tile_bytes, off, chunks, n_tiles):
-    """Chunk-major tile images [tile][chunk][128 rows][8] fp16 at byte `off` of every tile -> [n_tiles * 128, 8 * chunks]."""
-    t = buf[:n_tiles * tile_bytes].view(n_tiles, tile_bytes)[:, off:off + chunks * CHUNK]
-    t = t.contiguous().view(torch.float16).view(n_tiles, chunks, TILE_M, 8)
-    return t.permute(0, 2, 1, 3).reshape(n_tiles * TILE_M, chunks * 8)
+def tile_slices(buf, tile_bytes, off, nbytes, n_tiles, tiles):
+    """[tiles, nbytes] at byte `off` of every tile, or of the listed tiles only (a long tensor on buf's device)."""
+    t = buf[:n_tiles * tile_bytes].view(n_tiles, tile_bytes)
+    if tiles is not None:
+        t = t.index_select(0, tiles)
+    return t[:, off:off + nbytes]
+
+
+def image(buf, tile_bytes, off, chunks, n_tiles, tiles=None):
+    """Chunk-major tile images [tile][chunk][128 rows][8] fp16 at byte `off` of every tile -> [n_tiles * 128, 8 * chunks];
+    with `tiles` only those tiles, in that order -> [len(tiles) * 128, 8 * chunks]."""
+    t = tile_slices(buf, tile_bytes, off, chunks * CHUNK, n_tiles, tiles)
+    n = t.shape[0]
+    t = t.contiguous().view(torch.float16).view(n, chunks, TILE_M, 8)
+    return t.permute(0, 2, 1, 3).reshape(n * TILE_M, chunks * 8)
+
+
+def boundary_tiles(tile_bytes, n_tiles, limits=(2 ** 31, 2 ** 32)):
+    """The tiles of a buffer of n_tiles x tile_bytes whose byte range holds byte `limit` (the first byte a 32-bit signed /
+    unsigned offset cannot address), and their neighbours, for every limit the buffer reaches; sorted."""
+    out = set()
+    for lim in limits:
+        t = lim // tile_bytes
+        if t < n_tiles:
+            out.update(x for x in (t - 1, t, t + 1) if 0 <= x < n_tiles)
+    return sorted(out)
 
 
 def _mask_geometry(ncols):
@@ -68,13 +89,13 @@ def _mask_geometry(ncols):
     return kh, word, bit
 
 
-def relu_bits(buf, off, ncols, n_tiles, tile_bytes=MASK_TILE):
+def relu_bits(buf, off, ncols, n_tiles, tile_bytes=MASK_TILE, tiles=None):
     """ReluMask image (field_mma.cuh) at byte `off` of every tile -> bool [n_tiles * 128, ncols].  Row r holds one 32-bit
     word per (q, h) at byte r * 16 kH + q * 4 kH + 4 h; bit k is column 8 (16 h + k) + 2 q, bit 16 + k that column + 1;
-    kH = 2 for 256 columns, else 1."""
+    kH = 2 for 256 columns, else 1.  With `tiles` only those tiles, as image() does."""
     kh, word, bit = _mask_geometry(ncols)
-    t = buf[:n_tiles * tile_bytes].view(n_tiles, tile_bytes)[:, off:off + TILE_M * 16 * kh]
-    w = t.contiguous().view(torch.int32).reshape(n_tiles * TILE_M, 4 * kh).long() & 0xFFFFFFFF
+    t = tile_slices(buf, tile_bytes, off, TILE_M * 16 * kh, n_tiles, tiles)
+    w = t.contiguous().view(torch.int32).reshape(t.shape[0] * TILE_M, 4 * kh).long() & 0xFFFFFFFF
     return ((w[:, word.to(w.device)] >> bit.to(w.device)) & 1).bool()
 
 

@@ -1,6 +1,8 @@
 """The stash, mask and gradient layouts that tests/stash_layout.py mirrors, pinned to the library's own sizes, and a round
 trip of the documented ReLU mask bit layout.  No kernel is launched here."""
 import math
+import os
+import re
 
 import pytest
 import torch
@@ -112,3 +114,53 @@ def test_loss_scale_matches_the_kernels_rule():
         if 2.0 ** -60 <= s <= 2.0 ** 60 and 1e-17 < amax < 1e17:
             assert 512.0 <= amax * s < 1024.0, (amax, s)
     assert SL.loss_scale(1e-30) == 2.0 ** 60 and SL.loss_scale(1e30) == 2.0 ** -60
+
+
+def test_boundary_tiles_hold_the_32_bit_limits_of_the_library_buffers():
+    """The tiles tests/test_scale_gpu.py samples: per-tile sizes from the library, and the tile that holds byte 2^31 /
+    2^32 of each buffer (the first byte a 32-bit signed / unsigned offset cannot address) with its neighbours."""
+    from nonrigid_nerf_b200 import _lib
+    lib = _lib.load()
+    for (n, s), name, nbytes, expect in (
+            ((8192, 128), "stash", lib.nrn_stash_bytes, [3381, 3382, 3383, 6764, 6765, 6766]),
+            ((8192, 128), "grad stash", lib.nrn_grad_stash_bytes, [3471, 3472, 3473, 6943, 6944, 6945]),
+            ((8192, 64), "stash", lib.nrn_stash_bytes, [3381, 3382, 3383]),
+            ((53248, 128), "masks", lib.nrn_relu_mask_bytes, [52427, 52428, 52429]),
+            ((53248, 128), "tangent", lib.nrn_div_stash_bytes, [22794, 22795, 22796, 45589, 45590, 45591]),
+            ((53248, 128), "adjoint", lib.nrn_div_grad_stash_bytes, [23830, 23831, 23832, 47661, 47662, 47663])):
+        T = -(-n * s // SL.TILE_M)
+        n_buf = T + (T & 1) if name in ("stash", "grad stash", "masks") else T
+        total = nbytes(n, s)
+        tb = total // n_buf
+        assert tb * n_buf == total, name
+        got = SL.boundary_tiles(tb, T)
+        assert got == [t for t in expect if t < T], (n, s, name, got)
+        for lim in (2 ** 31, 2 ** 32):
+            if lim < T * tb:
+                t = lim // tb
+                assert t in got and t * tb <= lim < (t + 1) * tb
+
+
+@pytest.mark.parametrize("max_ctas", [132, 114, 66, 16])
+def test_replicated_wgrad_plan_fits_the_scratch_and_covers_every_tile_once(max_ctas):
+    """wgrad_plan / split_ranges restate launch_wgrad's plan: its per-job costs are the kJobChunks table of wgrad.cu, its
+    CTAs fit the device and the scratch partials (nrn_wgrad_scratch_bytes), and every job's splits own each tile exactly
+    once.  The greedy rule itself is a copy: nothing the library exposes pins it."""
+    from nonrigid_nerf_b200 import _lib
+    from tests import stage_reference as SR
+    lib = _lib.load()
+    parts = lib.nrn_wgrad_scratch_bytes() // (4 * SR.WG_SCRATCH_FLOATS)
+    assert parts * 4 * SR.WG_SCRATCH_FLOATS == lib.nrn_wgrad_scratch_bytes()
+    src = open(os.path.join(os.path.dirname(_lib.__file__), "csrc", "wgrad.cu")).read()
+    table = re.search(r"kJobChunks\[12\]\s*=\s*\{([^}]*)\}", src).group(1)
+    assert [sum(int(t) for t in x.split("+")) for x in table.split(",")] == SR._JOB_CHUNKS
+    for T in (1, 9, 1024, 4096, 8192, 53248):
+        for kw in (dict(has_bender=True), dict(has_bender=False), dict(compact=True)):
+            plan = SR.wgrad_plan(T, max_ctas, **kw)
+            halves = SR.wgrad_halves(**kw)
+            used = sum(plan[j] * halves[j] for j in plan)
+            assert used <= max(max_ctas, sum(halves.values())) and used <= parts, (T, kw, plan)
+            for j, n_split in plan.items():
+                ranges = SR.split_ranges(T, n_split)
+                assert ranges[0][0] == 0 and ranges[-1][1] == T and all(a[1] == b[0] for a, b in zip(ranges, ranges[1:]))
+                assert all(e > s for s, e in ranges) and len(ranges) <= n_split
