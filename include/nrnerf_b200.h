@@ -206,11 +206,45 @@ typedef struct NrnViewArgs {
   int64_t viewdirs_stride;    /* floats between rows, >= 3 */
   void* workspace;            /* with a bender: nrn_views_workspace_bytes(n_rays, n_samples), 16-byte aligned */
 } NrnViewArgs;
-/* args as for nrn_field_forward, with out_ch = 4 and no stash / relu_mask (training is not implemented).  With a bender
+/* args as for nrn_field_forward, with out_ch = 4 and no stash / relu_mask (training: nrn_field_forward_views_train).  With a bender
  * n_samples >= 2: the finite differences run over each ray's n_samples consecutive points.  Point mode takes
  * n_rays * n_samples points, n_samples consecutive ones forming a ray; latents (and viewdirs) are read per point.  With a
  * bender, raw = NULL runs the bend pass alone (the details: bent points, offsets, rigidity). */
 int nrn_field_forward_views(const NrnFieldArgs* args, const NrnViewArgs* views);
+/* ---- training the view-dependent head without a ray bender (rigid scenes; NeRF(use_viewdirs=True), ray_bender None):
+ * the view direction is the ray's own normalised direction, so the gradient stops at views_linears.0's direction
+ * columns.  The forward keeps, next to the trunk's stash and ReLU masks, a view stash (direction encoding, feature,
+ * post-ReLU views_linears.0 output) and the ReLU mask bits of that output; the backward runs the head's transposed
+ * steps in front of the trunk's DGRAD and the head's weight gradients in the same WGRAD launch.  Buffers are per
+ * 128-point tile, rounded up to an even tile count like nrn_stash_bytes. */
+size_t nrn_packed_views_t_bytes(void);   /* transposed head images: rgb_linear^T | views_linears.0[:, :256]^T | feature_linear^T */
+/* w[0] = feature_linear.weight [256][256], w[1] = views_linears.0.weight [128][256 + 27], w[2] = rgb_linear.weight [3][128] */
+int nrn_pack_views_t(const float* const* w, void* packed, void* stream);
+size_t nrn_views_stash_bytes(int n_rays, int n_samples);        /* 104 KB per tile */
+size_t nrn_views_grad_stash_bytes(int n_rays, int n_samples);   /* 96 KB per tile */
+size_t nrn_hv_mask_bytes(int n_rays, int n_samples);            /* 2 KB per tile */
+/* flat order of the view model's parameters: W0 b0 ... W7 b7 (as nrn_nerf_grad_floats), then views_linears.0.w [128][283]
+ * .b, feature_linear.w [256][256] .b, alpha_linear.w [1][256] .b, rgb_linear.w [3][128] .b: 595,844 floats */
+int nrn_nerf_views_grad_floats(void);
+typedef struct NrnViewTrainArgs {
+  void* views_stash;          /* nrn_views_stash_bytes(), 16-byte aligned */
+  void* hv_mask;              /* nrn_hv_mask_bytes(), 16-byte aligned */
+} NrnViewTrainArgs;
+/* The forward of nrn_field_forward_views without a bender, keeping what the backward needs: args in ray mode with
+ * out_ch = 4, bender_packed NULL, use_removal 0, stash and relu_mask given (nrn_stash_bytes / nrn_relu_mask_bytes);
+ * views->views_packed and views->viewdirs given.  raw equals nrn_field_forward_views' bit for bit. */
+int nrn_field_forward_views_train(const NrnFieldArgs* args, const NrnViewArgs* views, const NrnViewTrainArgs* train);
+typedef struct NrnViewBwdArgs {
+  const void* views_t_packed;   /* nrn_pack_views_t output */
+  const void* views_stash;      /* from the forward call */
+  void* views_grad_stash;       /* workspace, nrn_views_grad_stash_bytes() */
+  const void* hv_mask;          /* from the forward call */
+} NrnViewBwdArgs;
+/* Backward of nrn_field_forward_views_train: args as for nrn_field_backward with out_ch = 4, bender_packed NULL and
+ * nerf_packed the nrn_pack_nerf image the forward ran with (its head^T holds alpha_linear in column 3).  nerf_grad receives
+ * the flat layout of nrn_nerf_views_grad_floats(); nerf_grad_head, if not NULL, receives the head block (views_linears.0
+ * .. rgb_linear.b) instead of the tail of nerf_grad.  Deterministic: every sum runs in a fixed order. */
+int nrn_field_backward_views(const NrnFieldBwdArgs* args, const NrnViewBwdArgs* views);
 size_t nrn_tc_workspace_bytes(int n_rays);   /* per-ray sums [n][2][256] + latent columns of dW0 / dW5 [2][256][32] */
 typedef struct NrnTcBwdArgs {
   const float* latents;           /* [n_rays][32] the forward call's latents ... */
@@ -354,7 +388,8 @@ int nrn_peer_gather_rows(const NrnPeerCtx* ctx, const float* local, int n_per_ra
  * launch stream.  kinds: 0 field forward, 1 field DGRAD, 2 WGRAD (+reduce), 3 composite(+resample),
  * 4 composite backward, 5 divergence regulariser, 6 time-conditioned ray bias (nrn_tc_latent_bias), 7 time-conditioned
  * latent gradients (per-ray sums, d z, latent columns of dW0 / dW5), 8 bend pass of the view-dependent head, 9 its
- * view-head field kernel (nrn_field_forward_views).  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * view-head field kernel (nrn_field_forward_views), 10 its training forward (nrn_field_forward_views_train), 11 its DGRAD
+ * and 12 its WGRAD (+reduce) (nrn_field_backward_views).  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

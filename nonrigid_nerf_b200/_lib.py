@@ -41,6 +41,14 @@ class NrnViewArgs(C.Structure):
     ]
 
 
+class NrnViewTrainArgs(C.Structure):
+    _fields_ = [("views_stash", _vp), ("hv_mask", _vp)]
+
+
+class NrnViewBwdArgs(C.Structure):
+    _fields_ = [("views_t_packed", _vp), ("views_stash", _vp), ("views_grad_stash", _vp), ("hv_mask", _vp)]
+
+
 class NrnFieldBwdArgs(C.Structure):
     _fields_ = [
         ("n_rays", C.c_int32), ("n_samples", C.c_int32), ("out_ch", C.c_int32),
@@ -163,6 +171,14 @@ SYMBOLS = {
     "nrn_views_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "nrn_field_forward_views": (C.c_int, [C.POINTER(NrnFieldArgs), C.POINTER(NrnViewArgs)]),
     "nrn_field_backward_tc": (C.c_int, [C.POINTER(NrnFieldBwdArgs), C.POINTER(NrnTcBwdArgs)]),
+    "nrn_packed_views_t_bytes": (C.c_size_t, []),
+    "nrn_pack_views_t": (C.c_int, [C.POINTER(_vp), _vp, _vp]),
+    "nrn_views_stash_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "nrn_views_grad_stash_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "nrn_hv_mask_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "nrn_nerf_views_grad_floats": (C.c_int, []),
+    "nrn_field_forward_views_train": (C.c_int, [C.POINTER(NrnFieldArgs), C.POINTER(NrnViewArgs), C.POINTER(NrnViewTrainArgs)]),
+    "nrn_field_backward_views": (C.c_int, [C.POINTER(NrnFieldBwdArgs), C.POINTER(NrnViewBwdArgs)]),
     "nrn_div_stash_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "nrn_div_grad_stash_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "nrn_divergence_forward": (C.c_int, [C.POINTER(NrnDivArgs)]),
@@ -187,6 +203,8 @@ KERNEL_KINDS = ("field_fwd", "field_dgrad", "wgrad", "composite", "composite_bwd
 TC_KERNEL_KINDS = ("tc_latent_bias", "tc_latent_bwd")
 # the view-dependent head's kernels (bend pass, view-head field kernel), timing kinds 8 and 9
 VIEW_KERNEL_KINDS = ("views_bend", "views_field")
+# training the view-dependent head (training forward, its DGRAD, its WGRAD + reduce), timing kinds 10 to 12
+VIEW_TRAIN_KERNEL_KINDS = ("views_field_train", "views_dgrad", "views_wgrad")
 
 
 def timing_enable(on: bool) -> None:
@@ -195,7 +213,7 @@ def timing_enable(on: bool) -> None:
 
 def timing_read(kinds=KERNEL_KINDS):
     """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True); `kinds` is KERNEL_KINDS,
-    KERNEL_KINDS + TC_KERNEL_KINDS or KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS."""
+    KERNEL_KINDS + TC_KERNEL_KINDS, KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS or that + VIEW_TRAIN_KERNEL_KINDS."""
     n = len(kinds)
     ms = (C.c_double * n)()
     cnt = (C.c_int * n)()

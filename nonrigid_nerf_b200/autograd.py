@@ -507,27 +507,116 @@ def _needs_grad(net, latents) -> bool:
     return bender is not None and any(p.requires_grad for p in bender.parameters())
 
 
-def views_check(net, latents=None) -> None:
-    """Raise for what the view-dependent head (use_viewdirs=True) does not support: a seated bender with exact view
-    directions or without rays of at least two samples, and any differentiable call (training is not implemented)."""
+_SEATED = object()
+
+
+def views_check(net, latents=None, bender=_SEATED) -> None:
+    """Raise for what the view-dependent head (use_viewdirs=True) does not support: with a bender (the seated one, or
+    `bender`, which the caller is about to seat), exact view directions, rays of fewer than two samples and any
+    differentiable call (training with a bender is not implemented; without one the head trains)."""
     if not getattr(net, "use_viewdirs", False):
         return
-    if net.ray_bender[0] is not None:
-        if not net.approx_nonrigid_viewdirs:
-            raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True with approx_nonrigid_viewdirs=False (exact view directions "
-                               "through the ray bender) is not implemented")
-        if net.num_ray_samples is None or net.num_ray_samples < 2:
-            raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True with a ray bender needs num_ray_samples >= 2 (the view "
-                               f"directions are finite differences along each ray; got {net.num_ray_samples})")
-    if _needs_grad(net, latents):
+    if bender is _SEATED:
+        bender = net.ray_bender[0]
+    if bender is None:
+        return
+    if not net.approx_nonrigid_viewdirs:
+        raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True with approx_nonrigid_viewdirs=False (exact view directions "
+                           "through the ray bender) is not implemented")
+    if net.num_ray_samples is None or net.num_ray_samples < 2:
+        raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True with a ray bender needs num_ray_samples >= 2 (the view "
+                           f"directions are finite differences along each ray; got {net.num_ray_samples})")
+    if _needs_grad(net, latents) or (torch.is_grad_enabled() and any(p.requires_grad for p in bender.parameters())):
         raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True: training with the view-dependent head is not implemented yet; "
                            "rendering works under torch.no_grad()")
 
 
+def _views_flat_params(net):
+    """A use_viewdirs=True NeRF's parameters in the flat order of nrn_field_backward_views: the trunk's (W0 b0 .. W7 b7),
+    then the head block in module order."""
+    ws, bs = ops._views_trunk_params(net)
+    trunk = []
+    for w, b in zip(ws[:8], bs[:8]):
+        trunk += [w, b]
+    head = [net.views_linears[0].weight, net.views_linears[0].bias, net.feature_linear.weight, net.feature_linear.bias,
+            net.alpha_linear.weight, net.alpha_linear.bias, net.rgb_linear.weight, net.rgb_linear.bias]
+    return trunk, head
+
+
+class _ViewsTrainFn(torch.autograd.Function):
+    """The view-dependent head without a bender: raw (differentiable) + point details (not).  params = the trunk's
+    parameters, then the head block's (_views_flat_params).  The view direction is the ray's own, so like the reference no
+    gradient leaves the field but the parameters': the latents get none."""
+
+    @staticmethod
+    def forward(ctx, net, rays, z_vals, viewdirs, n_trunk, *params):
+        if getattr(net, "test_time_nonrigid_object_removal_threshold", None) is not None:
+            raise RuntimeError("nonrigid_nerf_b200: test_time_nonrigid_object_removal_threshold is a test-time knob; "
+                               "it is not differentiable")
+        nerf_pack, views_pack = ops.pack_nerf(net), ops.pack_views(net)
+        views_t = ops.pack_views_t(net)   # the weights this forward ran with, for the backward
+        raw, det, bufs = ops.field_forward_views_train(rays, z_vals, viewdirs, nerf_pack, views_pack, True)
+        ctx.n_trunk, ctx.params = n_trunk, params
+        ctx.shape = z_vals.shape
+        ctx.packs = (nerf_pack, views_t)
+        # the stashes live as long as the autograd node (a second backward over a retained graph reads them again)
+        ctx.bufs = bufs
+        ctx.set_materialize_grads(False)
+        ctx.mark_non_differentiable(det["initial_input_pts"], det["input_pts"])
+        return raw, det["initial_input_pts"], det["input_pts"]
+
+    @staticmethod
+    def backward(ctx, d_raw, *rest):
+        n, s = ctx.shape
+        nerf_pack, views_t = ctx.packs
+        bufs = ctx.bufs
+        dev = nerf_pack.device
+        lib = _lib.load()
+        if d_raw is None:
+            d_raw = torch.zeros(n, s, 4, dtype=torch.float32, device=dev)
+        d_raw = d_raw.contiguous().float()
+        a = _lib.NrnFieldBwdArgs()
+        a.n_rays, a.n_samples, a.out_ch = n, s, 4
+        a.d_raw = d_raw.data_ptr()
+        a.stash, a.relu_mask = bufs["stash"].data_ptr(), bufs["relu_mask"].data_ptr()
+        gstash = torch.empty(lib.nrn_grad_stash_bytes(n, s), dtype=torch.uint8, device=dev)
+        vgstash = torch.empty(lib.nrn_views_grad_stash_bytes(n, s), dtype=torch.uint8, device=dev)
+        scratch = torch.empty(lib.nrn_wgrad_scratch_bytes(), dtype=torch.uint8, device=dev)
+        a.grad_stash, a.wgrad_scratch = gstash.data_ptr(), scratch.data_ptr()
+        a.nerf_packed = nerf_pack.data_ptr()
+        # in place into optim.Adam's arena when the trunk's and the head block's .grad tensors each lie back to back there
+        # (as in _FieldTrainFn), else fresh flat buffers handed to autograd as per-parameter views
+        params = list(ctx.params)
+        trunk_p, head_p = params[:ctx.n_trunk], params[ctx.n_trunk:]
+        trunk_dst = _arena_destination(trunk_p) if all(p.requires_grad for p in params) else None
+        head_dst = _arena_destination(head_p) if trunk_dst is not None else None
+        flat = None
+        if head_dst is not None:
+            a.nerf_grad, a.nerf_grad_head, a.accumulate_nerf = trunk_dst, head_dst, 1
+        else:
+            flat = torch.empty(lib.nrn_nerf_views_grad_floats(), dtype=torch.float32, device=dev)
+            a.nerf_grad = flat.data_ptr()
+        a.stream = torch.cuda.current_stream().cuda_stream
+        v = _lib.NrnViewBwdArgs()
+        v.views_t_packed, v.views_stash, v.views_grad_stash, v.hv_mask = (
+            views_t.data_ptr(), bufs["views_stash"].data_ptr(), vgstash.data_ptr(), bufs["hv_mask"].data_ptr())
+        with torch.cuda.device(dev):
+            _lib.check(lib.nrn_field_backward_views(C.byref(a), C.byref(v)), "field_backward_views")
+        if flat is None:
+            grads = [None] * len(params)
+        else:
+            grads = [g if p.requires_grad else None for g, p in zip(_split_flat(flat, params), params)]
+        return (None, None, None, None, None, *grads)
+
+
 def field_views(net, rays, z_vals, points, latents, viewdirs, want_details, bend_only=False):
     """The view-dependent head (inference): ray mode (rays, z_vals) or point mode (points grouped into rays of
-    net.num_ray_samples).  bend_only: the bend pass alone (details only, raw is None)."""
+    net.num_ray_samples).  bend_only: the bend pass alone (details only, raw is None).  Differentiable ray-mode calls
+    without a bender go through field()."""
     views_check(net, latents)
+    if _needs_grad(net, latents):
+        raise RuntimeError("nonrigid_nerf_b200: the point-wise NeRF.forward / run_network entry is inference-only; "
+                           "differentiable rendering goes through render() / render_rays()")
     bender = net.ray_bender[0]
     cutoff, scaling, removal = _knobs(net)
     nerf_pack = ops.pack_nerf(net)
@@ -546,6 +635,11 @@ def field(net, rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[torch
     if getattr(net, "use_viewdirs", False):
         if viewdirs is None:
             raise RuntimeError("nonrigid_nerf_b200: a use_viewdirs=True model needs ray batches with view directions (11 columns)")
+        views_check(net, latents)   # with a bender: raises for a differentiable call
+        if bender is None and _needs_grad(net, latents):
+            trunk, head = _views_flat_params(net)
+            raw, init, bent = _ViewsTrainFn.apply(net, rays, z_vals, viewdirs, len(trunk), *trunk, *head)
+            return raw, ({"initial_input_pts": init, "input_pts": bent} if want_details else {})
         return field_views(net, rays, z_vals, None, latents, viewdirs, want_details)
     _tc_net(net)
     if not _needs_grad(net, latents):

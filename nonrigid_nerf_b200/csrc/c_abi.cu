@@ -23,6 +23,8 @@ cudaError_t launch_tc_latent_bias(const float* lat, long long lat_stride, int n_
 cudaError_t launch_tc_latent_bwd(const TcBwdParams& p, cudaStream_t stream);
 cudaError_t launch_field_bend(const FieldFwdParams& p, const ViewParams& v, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_views(const FieldFwdParams& p, const ViewParams& v, int num_sms, cudaStream_t stream);
+cudaError_t launch_field_views_train(const FieldFwdParams& p, const ViewParams& v, const ViewTrainParams& t, int num_sms, cudaStream_t stream);
+cudaError_t launch_field_bwd_views(const FieldBwdParams& p, const ViewBwdParams& v, int num_sms, cudaStream_t stream);
 }
 
 namespace {
@@ -350,6 +352,132 @@ int nrn_field_forward_views(const NrnFieldArgs* a, const NrnViewArgs* v) {
   p.raw = a->raw;
   { ScopedTimer tm(9, st); e = nrn::launch_field_views(p, vp, ds->num_sms, st); }
   return e == cudaSuccess ? NRN_OK : cuda_fail(e, "field_views_kernel");
+}
+
+// ---- training the view-dependent head without a bender ----
+size_t nrn_packed_views_t_bytes(void) { return nrn::kViewsTWBytes; }
+
+int nrn_pack_views_t(const float* const* w, void* packed, void* stream) {
+  if (!w || !packed) return fail(NRN_E_INVALID, "nrn_pack_views_t: null argument");
+  if (!aligned16(packed)) return fail(NRN_E_INVALID, "nrn_pack_views_t: packed buffer must be 16-byte aligned");
+  nrn::ViewsSrc src{};
+  for (int i = 0; i < 3; ++i) {
+    if (!w[i]) return fail(NRN_E_INVALID, "nrn_pack_views_t: null layer %d", i);
+    src.w[i] = w[i];
+  }
+  const cudaError_t e = nrn::launch_pack_views_t(src, packed, static_cast<cudaStream_t>(stream));
+  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "pack_views_t_kernel");
+}
+
+static long long even_tiles(int n_rays, int n_samples);
+size_t nrn_views_stash_bytes(int n_rays, int n_samples) {
+  return n_rays < 0 || n_samples < 1 ? 0 : static_cast<size_t>(even_tiles(n_rays, n_samples)) * nrn::kVStashTileBytes;
+}
+size_t nrn_views_grad_stash_bytes(int n_rays, int n_samples) {
+  return n_rays < 0 || n_samples < 1 ? 0 : static_cast<size_t>(even_tiles(n_rays, n_samples)) * nrn::kVGradTileBytes;
+}
+size_t nrn_hv_mask_bytes(int n_rays, int n_samples) {
+  return n_rays < 0 || n_samples < 1 ? 0 : static_cast<size_t>(even_tiles(n_rays, n_samples)) * nrn::kHvMaskTileBytes;
+}
+int nrn_nerf_views_grad_floats(void) { return nrn::nerf_views_grad_floats(); }
+
+int nrn_field_forward_views_train(const NrnFieldArgs* a, const NrnViewArgs* v, const NrnViewTrainArgs* t) {
+  const char* who = "nrn_field_forward_views_train";
+  if (!a || !v || !t) return fail(NRN_E_INVALID, "%s: null args", who);
+  if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "%s: bad sizes n=%d S=%d", who, a->n_rays, a->n_samples);
+  if (a->bender_packed)
+    return fail(NRN_E_INVALID, "%s: training with the view-dependent head is not implemented with a ray bender (bender_packed must be NULL)", who);
+  if (a->points) return fail(NRN_E_INVALID, "%s: training needs ray mode (points must be NULL)", who);
+  if (a->out_ch != 4) return fail(NRN_E_INVALID, "%s: out_ch=%d unsupported (use_viewdirs=True: 4 = rgb + alpha)", who, a->out_ch);
+  if (a->use_removal) return fail(NRN_E_INVALID, "%s: the object removal is a test-time knob; it is not differentiable", who);
+  if (!v->viewdirs || v->viewdirs_stride < 3) return fail(NRN_E_INVALID, "%s: needs viewdirs with viewdirs_stride >= 3", who);
+  if (a->n_rays == 0) return NRN_OK;
+  if (!a->rays || !a->z_vals || !a->raw || !a->nerf_packed || !v->views_packed) return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (!a->stash || !a->relu_mask || !t->views_stash || !t->hv_mask)
+    return fail(NRN_E_INVALID, "%s: null stash, relu_mask, views_stash or hv_mask", who);
+  if (!aligned16(a->nerf_packed) || !aligned16(v->views_packed) || !aligned16(a->stash) || !aligned16(a->relu_mask) ||
+      !aligned16(t->views_stash) || !aligned16(t->hv_mask))
+    return fail(NRN_E_INVALID, "%s: packed weights and stashes must be 16-byte aligned", who);
+  const long long P = static_cast<long long>(a->n_rays) * a->n_samples;
+  const long long tiles = (P + nrn::kTileM - 1) / nrn::kTileM;
+  if (tiles > 0x7fffffffLL) return fail(NRN_E_INVALID, "%s: too many points", who);
+  DeviceState* ds;
+  int rc = device_state(&ds);
+  if (rc) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  nrn::FieldFwdParams p{};
+  p.rays = a->rays; p.z_vals = a->z_vals;
+  p.n_rays = a->n_rays; p.S = a->n_samples; p.P = P; p.n_tiles = static_cast<int>(tiles);
+  const uint8_t* np = static_cast<const uint8_t*>(a->nerf_packed);
+  p.nerf_w = np; p.nerf_bias = reinterpret_cast<const float*>(np + nrn::kNerfWBytes);
+  p.out_ch = 4; p.err = ds->err_word;
+  p.raw = a->raw; p.d_init = a->initial_input_pts; p.d_bent = a->input_pts;
+  p.stash = static_cast<uint8_t*>(a->stash); p.relu_mask = static_cast<uint8_t*>(a->relu_mask);
+  nrn::ViewParams vp{};
+  const uint8_t* vw = static_cast<const uint8_t*>(v->views_packed);
+  vp.w = vw; vp.bias = reinterpret_cast<const float*>(vw + nrn::kViewsWBytes);
+  vp.viewdirs = v->viewdirs; vp.viewdirs_stride = v->viewdirs_stride;
+  nrn::ViewTrainParams tp{static_cast<uint8_t*>(t->views_stash), static_cast<uint8_t*>(t->hv_mask)};
+  cudaError_t e;
+  { ScopedTimer tm(10, st); e = nrn::launch_field_views_train(p, vp, tp, ds->num_sms, st); }
+  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "field_views_train_kernel");
+}
+
+int nrn_field_backward_views(const NrnFieldBwdArgs* a, const NrnViewBwdArgs* v) {
+  const char* who = "nrn_field_backward_views";
+  if (!a || !v) return fail(NRN_E_INVALID, "%s: null args", who);
+  if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "%s: bad sizes", who);
+  if (a->out_ch != 4) return fail(NRN_E_INVALID, "%s: out_ch=%d unsupported (use_viewdirs=True: 4 = rgb + alpha)", who, a->out_ch);
+  if (a->bender_packed)
+    return fail(NRN_E_INVALID, "%s: training with the view-dependent head is not implemented with a ray bender (bender_packed must be NULL)", who);
+  if (!a->nerf_grad) return fail(NRN_E_INVALID, "%s: null nerf_grad", who);
+  const int n_all = nrn::nerf_views_grad_floats();
+  cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  if (a->n_rays == 0) {   // an empty shard contributes zero gradients
+    cudaError_t e = cudaSuccess;
+    if (!a->accumulate_nerf) {
+      const int head_n = a->nerf_grad_head ? n_all - nrn::kViewsTrunkFloats : 0;
+      e = cudaMemsetAsync(a->nerf_grad, 0, sizeof(float) * (n_all - head_n), st);
+      if (e == cudaSuccess && head_n) e = cudaMemsetAsync(a->nerf_grad_head, 0, sizeof(float) * head_n, st);
+    }
+    return e == cudaSuccess ? NRN_OK : cuda_fail(e, "memset grads");
+  }
+  if (!a->d_raw || !a->stash || !a->grad_stash || !a->wgrad_scratch || !a->relu_mask || !a->nerf_packed)
+    return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (!v->views_t_packed || !v->views_stash || !v->views_grad_stash || !v->hv_mask)
+    return fail(NRN_E_INVALID, "%s: null views_t_packed, views_stash, views_grad_stash or hv_mask", who);
+  if (!aligned16(a->nerf_packed) || !aligned16(v->views_t_packed) || !aligned16(a->stash) || !aligned16(a->grad_stash) ||
+      !aligned16(a->relu_mask) || !aligned16(v->views_stash) || !aligned16(v->views_grad_stash) || !aligned16(v->hv_mask))
+    return fail(NRN_E_INVALID, "%s: packed weights and stashes must be 16-byte aligned", who);
+  const long long P = static_cast<long long>(a->n_rays) * a->n_samples;
+  if ((P + nrn::kTileM - 1) / nrn::kTileM > 0x7fffffffLL) return fail(NRN_E_INVALID, "%s: too many points", who);
+  DeviceState* ds;
+  int rc = device_state(&ds);
+  if (rc) return rc;
+  if (ds->num_sms + 16 > nrn::kWgMaxCtas) return fail(NRN_E_INVALID, "%s: %d SMs exceed the scratch layout", who, ds->num_sms);
+  float* amax = reinterpret_cast<float*>(ds->err_word + 1);
+  nrn::FieldBwdParams p{};
+  p.P = P;
+  p.n_tiles = static_cast<int>((P + nrn::kTileM - 1) / nrn::kTileM);
+  p.S = a->n_samples; p.n_rays = a->n_rays; p.out_ch = 4;
+  p.d_raw = a->d_raw; p.amax = amax;
+  p.stash = static_cast<const uint8_t*>(a->stash); p.gstash = static_cast<uint8_t*>(a->grad_stash);
+  p.nerf_wT = static_cast<const uint8_t*>(a->nerf_packed) + nrn::kNerfTOffset;
+  p.err = ds->err_word;
+  p.relu_mask = static_cast<const uint8_t*>(a->relu_mask);
+  nrn::ViewBwdParams vp{static_cast<const uint8_t*>(v->views_t_packed), static_cast<const uint8_t*>(v->hv_mask),
+                        static_cast<uint8_t*>(v->views_grad_stash)};
+  // the loss scale: max |d_raw| over the four channels (rgb and alpha)
+  cudaError_t e = nrn::launch_absmax(a->d_raw, P * 4, amax, st, false, 4, 4);
+  if (e != cudaSuccess) return cuda_fail(e, "absmax_kernel");
+  { ScopedTimer tm(11, st); e = nrn::launch_field_bwd_views(p, vp, ds->num_sms, st); }
+  if (e != cudaSuccess) return cuda_fail(e, "field_bwd_views_kernel");
+  nrn::WgradParams w{};
+  w.stash = p.stash; w.gstash = p.gstash; w.scratch = a->wgrad_scratch; w.amax = amax; w.n_tiles = p.n_tiles; w.err = ds->err_word;
+  const nrn::WgradViewParams wv{static_cast<const uint8_t*>(v->views_stash), vp.vgstash};
+  const nrn::WgradDst dst{a->nerf_grad, a->nerf_grad_head, nullptr, n_all, 0, a->accumulate_nerf, 0};
+  { ScopedTimer tm(12, st); e = nrn::launch_wgrad_views(w, wv, ds->num_sms, dst, st); }
+  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "wgrad_views_kernel");
 }
 
 int nrn_tc_latent_bias(const float* latents, int64_t latent_stride, int n_rays, const float* w0, const float* b0, const float* w5,

@@ -16,6 +16,7 @@
 //   step  14     B0^T     d(bender input)             -> per-ray latent gradient (fp32 atomics)
 // All gradients travel in fp16 scaled by a power-of-two loss scale derived on the device from
 // max|d_raw| (no host sync); WGRAD and the latent reduction divide it out again in fp32.
+// field_bwd_views_kernel (view-dependent head, no bender): Rgb^T, ViewsF^T and Feature^T + head^T in front of L7^T.
 #include "field_mma.cuh"
 
 namespace nrn {
@@ -115,6 +116,36 @@ __device__ __forceinline__ void pe_backward(const float* de, const uint8_t* __re
     dx[d] += acc;
   }
 }
+
+// View head (training without a bender): NCOLS accumulator columns as fp16 (MASK: times the forward's ReLU mask bits `m`)
+// -> the next step's A fragments `a` and this warpgroup's rows of the view gradient-stash image `gs_img`
+template <int NCOLS, bool MASK, int NR>
+__device__ __forceinline__ void epi_views_frag(const float (&acc)[NR], const ReluMask<NCOLS>& m, uint32_t (&a)[NCOLS / 16][4],
+                                               uint8_t* gs_img, int g) {
+  const int r0 = g * kWgRows + acc_r0(), q = acc_q();
+#pragma unroll
+  for (int j = 0; j < NCOLS / 8; ++j) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      uint32_t g2 = pack_h2_sat(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+      if constexpr (MASK) g2 = m.apply(i, j, g2);
+      frag_pair(a, j, i) = g2;
+      *reinterpret_cast<uint32_t*>(gs_img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = g2;
+    }
+  }
+}
+
+// step -> shape in the view-head DGRAD's streaming order Rgb^T, ViewsF^T, Feature^T, head^T, L7^T, L6^T, L5h^T .. L1^T
+static_assert(vdgrad::step(vdgrad::FeatureT) == dgrad::step(dgrad::L7T), "step_at_views: Feature^T has the trunk's shape");
+__device__ __forceinline__ Step step_at_views(int step) {
+  switch (step) {
+    case dgrad::HeadT: return step_imm<dgrad::HeadT>();
+    case vdgrad::RgbT: return step_imm<vdgrad::RgbT>();
+    case vdgrad::ViewsFT: return step_imm<vdgrad::ViewsFT>();
+    default: return step_imm<dgrad::L7T>();   // Feature^T, L7^T, L6^T, L5h^T, L4^T .. L1^T
+  }
+}
+
 
 }  // namespace
 
@@ -345,6 +376,114 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
   if (wg_leader) tma_bulk_wait<0>();   // all gradient-stash stores complete before the CTA exits
 }
 
+
+// View-dependent head without a bender (training): Rgb^T, ViewsF^T and Feature^T + head^T replace head^T; then L7^T, L6^T
+// and L5h^T .. L1^T as in field_bwd_kernel.  L5e^T and L0^T only feed the embedding gradient, which has no consumer
+// without a bender: they are neither streamed nor run.
+__global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_views_kernel(const FieldBwdParams p, const ViewBwdParams v) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint8_t* ring_buf = smem + kBwdActBytes;           // the same shared-memory layout as field_bwd_kernel
+  float* stage_all = reinterpret_cast<float*>(ring_buf + kBwdRingStages * kRingStageBytes);
+  auto* sh = reinterpret_cast<RingShared<kBwdRingStages>*>(stage_all + 2 * kWgRows * kBwdStageLd);
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) sh->init();
+  __syncthreads();
+  const Waiter W{&sh->abort_flag, p.err};
+  Ring<kBwdRingStages> ring{ring_buf, sh->w_full, sh->w_empty};
+
+  if (warp >= 8) {
+    setmaxnreg_dec<kProducerRegs>();
+    // per tile: Rgb^T .. Feature^T (the view block), head^T, L7^T, L6^T, then L5h^T .. L1^T (skipping L5e^T and L0^T)
+    if (warp == 8 && lane == 0) {
+      auto put = [&](const uint8_t* src, int first, int last) {
+#pragma unroll 1
+        for (int step = first; step < last; ++step) {
+          const Step s = step_at_views(step);
+          for (uint32_t j = 0; j < s.nslabs; ++j) ring_put(ring, src + j * s.slab_bytes, s.slab_bytes, W);
+          src += s.nslabs * s.slab_bytes;
+        }
+      };
+      for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
+        put(v.wT, vdgrad::RgbT, vdgrad::kEnd);
+        put(p.nerf_wT, dgrad::HeadT, dgrad::L5eT);
+        put(p.nerf_wT + dgrad::w_off(dgrad::L5hT), dgrad::L5hT, dgrad::L0T);
+      }
+    }
+    return;
+  }
+
+  // ===================== consumer warpgroups =====================
+  setmaxnreg_inc<kConsumerRegs>();
+  const int g = warp >> 2;
+  const float scale = loss_scale(p.amax);   // max|d_raw| over the four channels
+
+  constexpr Step kTrunk = dgrad::step(dgrad::L7T), kRgbT = vdgrad::step(vdgrad::RgbT), kViewsFT = vdgrad::step(vdgrad::ViewsFT);
+  static_assert(kRgbT.nslabs == 1 && kRgbT.k16 == 1 && kViewsFT.N == kTrunk.N && kVgYv.chunks == 2 * kViewsFT.nslabs * kViewsFT.k16 &&
+                dgrad::step(dgrad::HeadT).N == kTrunk.N && dgrad::step(dgrad::HeadT).k16 == 1 && kGsRaw.chunks == 2,
+                "Rgb^T and head^T: one K = 16 MMA on the d_raw fragment; ViewsF^T: K = the 128 columns of dYv");
+  for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
+    uint8_t* gs = p.gstash + static_cast<long long>(tile) * kGradTileBytes;
+    uint8_t* vgs = v.vgstash + static_cast<long long>(tile) * kVGradTileBytes;
+    const uint8_t* mk = p.relu_mask + static_cast<long long>(tile) * kMaskTileBytes;
+    uint32_t h[kMaskHCols / 16][4];
+    // ---- A = d_raw [g_r g_g g_b g_alpha 0 ...] (K = 16), one fragment built from global memory, as field_bwd_kernel ----
+    const int r0 = g * kWgRows + acc_r0(), q = acc_q();
+    uint32_t a[1][4];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const long long pti = static_cast<long long>(tile) * kTileM + r0 + 8 * i;
+      float g0 = 0.f, g1 = 0.f;
+      if (q < 2 && pti < p.P) {
+        const float* src = p.d_raw + pti * p.out_ch + 2 * q;
+        g0 = clamp_h(__ldg(src) * scale);
+        g1 = clamp_h(__ldg(src + 1) * scale);
+      }
+      a[0][i] = q < 2 ? pack_h2(g0, g1) : 0u;
+      a[0][2 + i] = 0u;
+    }
+    // the same words -> the kGsRaw image (A of WGRAD's head and rgb_linear jobs)
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+        *reinterpret_cast<uint32_t*>(gs + kGsRaw.off + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = frag_pair(a, j, i);
+    uint32_t dyv[kVgYv.chunks / 2][4];
+    {   // ---- Rgb^T: dhv = d_raw . rgb_linear (channel 3 meets a zero column) -> dYv = dhv * [hv > 0] ----
+      Acc<vdgrad::RgbT> acc;
+      ReluMask<kMkHv.cols> m;
+      m.load(v.hv_mask + static_cast<long long>(tile) * kHvMaskTileBytes, g);
+      wg_gemm_rs<kRgbT.N, 1>(acc, a, ring, false, 0u, W, 320);
+      epi_views_frag<kMkHv.cols, true>(acc, m, dyv, vgs + kVgYv.off, g);
+    }
+    {   // ---- ViewsF^T: dF = dYv . views_linears.0[:, :256] (feature_linear has no ReLU) ----
+      Acc<vdgrad::ViewsFT> acc;
+      wg_gemm_rs<kViewsFT.N, kViewsFT.k16>(acc, dyv, ring, false, 0u, W, 321);
+      epi_views_frag<kMaskHCols, false>(acc, ReluMask<kMaskHCols>{}, h, vgs + kVgF.off, g);
+    }
+    {   // ---- Feature^T + head^T into one accumulator: dh8 = dF . feature_linear + d_alpha alpha_linear -> dY7 ----
+      Acc<vdgrad::FeatureT> acc;
+      ReluMask<kMaskHCols> m;
+      m.load(mk + kMkH + 7 * kMaskHBytes, g);
+      wg_gemm_rs<kTrunk.N, kTrunk.k16>(acc, h, ring, false, 0u, W, 322);
+      wg_gemm_rs<kTrunk.N, 1, 1, true>(acc, a, ring, false, 0u, W, 300);
+      epi_mask_frag(acc, m, h, gs + kGsY + 7 * kHBytes, g);
+    }
+    // ---- L7^T, L6^T : dY6, dY5; then L5h^T, L4^T .. L1^T : dY4 .. dY0 (one shape) ----
+#pragma unroll 1
+    for (int s = 0; s < 7; ++s) {
+      const int l = 6 - s;   // dY_l = dh_{l+1} * [h_{l+1} > 0]: dY6, dY5 (L7^T, L6^T), dY4 .. dY0 (L5h^T, L4^T .. L1^T)
+      Acc<dgrad::L7T> acc;
+      ReluMask<kMaskHCols> m;
+      m.load(mk + kMkH + l * kMaskHBytes, g);
+      wg_gemm_rs<kTrunk.N, kTrunk.k16>(acc, h, ring, false, 0u, W, 301 + s);
+      epi_mask_frag(acc, m, h, gs + kGsY + l * kHBytes, g);
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Time-conditioned baseline: the latent enters L0 and L5 as a per-ray bias (field_fwd.cu), so its gradients are per-ray
 // sums of those layers' pre-activation gradients dY0, dY5 (gradient stash):
@@ -408,6 +547,14 @@ __global__ void __launch_bounds__(256) tc_dw_lat_kernel(const TcBwdParams p) {
 
 cudaError_t launch_field_bwd(const FieldBwdParams& p, bool has_bender, int num_sms, cudaStream_t stream) {
   return launch_field(has_bender ? field_bwd_kernel<true> : field_bwd_kernel<false>, p, num_sms, kBwdSmemBytes, stream);
+}
+
+cudaError_t launch_field_bwd_views(const FieldBwdParams& p, const ViewBwdParams& v, int num_sms, cudaStream_t stream) {
+  if (p.n_tiles <= 0) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(field_bwd_views_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBwdSmemBytes);
+  if (e != cudaSuccess) return e;
+  field_bwd_views_kernel<<<p.n_tiles < num_sms ? p.n_tiles : num_sms, kFwdThreads, kBwdSmemBytes, stream>>>(p, v);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_tc_latent_bwd(const TcBwdParams& p, cudaStream_t stream) {

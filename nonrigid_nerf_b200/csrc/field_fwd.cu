@@ -18,13 +18,15 @@
 //
 // Shared memory (per CTA): bender H 24 KB + E 16 KB activations, 5 x 32 KB weight ring, per-row staging, barriers.
 //
-// View-dependent head (NeRF(use_viewdirs=True), inference only), two more instantiations of the same body:
+// View-dependent head (NeRF(use_viewdirs=True)), three more instantiations of the same body:
 //   bend pass (with a bender): B0..B4 only; every point's bent xyz and rigidity -> the bend workspace (16 B / point)
 //   view-head kernel: points from the workspace (or, without a bender, from rays + z), L0..L7, Head (alpha in column 3),
 //            Feature, ViewsE + ViewsF (one N = 128 accumulator), Rgb.  The direction of point r is the normalised
 //            backward difference of the bent points r - 1 and r of its ray (r + 1 and r for sample 0), read from the
 //            workspace in global memory, so it does not matter which tile or CTA owns the neighbour.  No bender H
 //            buffer: 24 KB less shared memory than the other kernels.
+//   view-head training kernel (no bender): the view-head kernel that also writes the trunk's stash and masks, the view
+//            stash (direction encoding, feature, hv) and hv's mask bits for field_bwd_views_kernel.
 #include "field_mma.cuh"
 
 namespace nrn {
@@ -172,19 +174,30 @@ __device__ __forceinline__ void write_dir_enc(const float (&d)[3], uint8_t* dst_
   }
 }
 
-// View head: accumulator columns [0, NCOLS) + bias (RELU: then ReLU), fp16 with saturation -> the next step's A fragments
-template <int NCOLS, bool RELU>
-__device__ __forceinline__ void epi_bias_frag(const float (&acc)[NCOLS / 2], const float* __restrict__ bias, uint32_t (&a)[NCOLS / 16][4]) {
+// View head: accumulator columns [0, NCOLS) + bias (RELU: then ReLU), fp16 with saturation -> the next step's A fragments.
+// TRAIN: also the fp16 pairs straight to this warpgroup's rows of the view-stash image `st_img`, and with RELU the mask
+// bits of those elements -> this thread's words of the tile's mask image `mask_img`.
+template <int NCOLS, bool RELU, bool TRAIN = false>
+__device__ __forceinline__ void epi_bias_frag(const float (&acc)[NCOLS / 2], const float* __restrict__ bias, uint32_t (&a)[NCOLS / 16][4],
+                                              uint8_t* st_img = nullptr, int g = 0, uint8_t* mask_img = nullptr) {
   const int q = acc_q();
+  ReluMask<NCOLS> m;
+  if constexpr (TRAIN && RELU) m.clear();
 #pragma unroll
   for (int j = 0; j < NCOLS / 8; ++j) {
     const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * q));
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const float u = acc[4 * j + 2 * i] + b.x, v = acc[4 * j + 2 * i + 1] + b.y;
-      frag_pair(a, j, i) = RELU ? pack_h2_relu_sat(u, v) : pack_h2_sat(u, v);
+      const uint32_t h2 = RELU ? pack_h2_relu_sat(u, v) : pack_h2_sat(u, v);
+      frag_pair(a, j, i) = h2;
+      if constexpr (TRAIN) {
+        if constexpr (RELU) m.pack(i, j, h2);
+        *reinterpret_cast<uint32_t*>(st_img + j * kChunkBytes + (g * kWgRows + acc_r0() + 8 * i) * 16 + 4 * q) = h2;
+      }
     }
   }
+  if constexpr (TRAIN && RELU) m.store(mask_img, g);
 }
 
 static_assert(views::step(views::Feature) == fwd::step(fwd::L1), "step_at_views: Feature has the trunk's shape");
@@ -209,12 +222,15 @@ enum Part : int { kFull, kBend, kViews };
 // TRAIN: p.stash and p.relu_mask are given (the inference kernel carries none of the mask code).
 // LATENT_BIAS (time-conditioned baseline, no bender): the L0 and L5 epilogues add the ray-bias rows p.ray_bias of their
 // rows' rays instead of the layers' bias vectors.
-// PART (view-dependent head, inference): kBend runs B0..B4 and writes v.ws; kViews (HAS_BENDER false) runs the trunk
-// and the view head, reading its points and rigidities from v.ws when that is given.
+// PART (view-dependent head): kBend runs B0..B4 and writes v.ws; kViews (HAS_BENDER false) runs the trunk and the view
+// head, reading its points and rigidities from v.ws when that is given.  kViews with TRAIN (no bender, v.ws null): the
+// trunk's stash and masks as the full kernel writes them, and the view stash and Hv masks of t.
 template <bool HAS_BENDER, bool TRAIN, bool LATENT_BIAS, int PART = kFull>
-__device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p, const ViewParams& v = ViewParams{}) {
+__device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p, const ViewParams& v = ViewParams{},
+                                               const ViewTrainParams& t = ViewTrainParams{}) {
   static_assert(!(HAS_BENDER && LATENT_BIAS), "the time-conditioned baseline has no bender");
-  static_assert(PART == kFull || (!TRAIN && !LATENT_BIAS && (PART == kBend) == HAS_BENDER), "view-head parts: inference only");
+  static_assert(PART == kFull || (!LATENT_BIAS && (PART == kBend) == HAS_BENDER && (!TRAIN || PART == kViews)),
+                "view-head parts: inference, or training of the view-head kernel without a bender");
   constexpr int kHBytes = PART == kViews ? 0 : kFwdHBytes;   // the view-head kernel has no bender images
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* act = smem;                                  // H (bender) | E, 128 rows
@@ -420,17 +436,26 @@ __device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p, const Vi
       }
     }
     if constexpr (PART == kViews) {
+      // training: the view stash of this tile (Dir by bulk store from E, F and Hv from registers) and its Hv masks
+      uint8_t* vst = TRAIN ? t.vstash + static_cast<long long>(tile) * kVStashTileBytes : nullptr;
+      const StashWriter<true> vsw{vst, wg_leader, bar, g};
       // ---- Head: alpha = alpha_linear(h) in column 3 (run_nerf_helpers.py:285) ----
       {
         Acc<fwd::Head> acc;
         wg_gemm_rs<fwd::step(fwd::Head).N, fwd::step(fwd::Head).k16>(acc, h, ring, false, 0u, W, 320);
         stage_cols<0, 1>(acc, stg, kFwdStageLd);
-        wg_bar(bar);   // also: every warp of this warpgroup is past L5, the last reader of E
+        // also: every warp of this warpgroup is past L5, the last reader of E; training: the bulk store of E to the stash
+        // has finished reading it before the direction encoding overwrites it
+        if constexpr (TRAIN) sw.begin();
+        else wg_bar(bar);
         if (row_thread) {
           float alpha = my_stg[3] + __ldg(p.nerf_bias + fwd::b_off(fwd::Head) + 3);
           // test-time non-rigid object removal (run_nerf_helpers.py:309-310)
           if (v.ws && p.use_removal && my_stg[11] >= p.removal) alpha *= 0.f;
-          const float d[3] = {my_stg[8], my_stg[9], my_stg[10]};
+          // training: rows past P (ragged last tile) never staged a direction; they encode d = 0, so that their stashed
+          // Dir and Hv rows are finite (WGRAD multiplies them by their zero gradients)
+          const bool dir_ok = !TRAIN || valid;
+          const float d[3] = {dir_ok ? my_stg[8] : 0.f, dir_ok ? my_stg[9] : 0.f, dir_ok ? my_stg[10] : 0.f};
           my_stg[11] = alpha;
           write_dir_enc(d, e_row);   // the direction encoding -> E, the A operand of ViewsE
         }
@@ -439,16 +464,22 @@ __device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p, const Vi
       {
         Acc<views::Feature> acc;
         wg_gemm_rs<views::step(views::Feature).N, views::step(views::Feature).k16>(acc, h, ring, false, 0u, W, 330);
-        epi_bias_frag<256, false>(acc, v.bias + views::b_off(views::Feature), h);
+        epi_bias_frag<256, false, TRAIN>(acc, v.bias + views::b_off(views::Feature), h, TRAIN ? vst + kVsF.off : nullptr, g);
       }
-      fence_proxy_async_smem();   // the direction encoding is visible to the tensor cores
-      wg_bar(bar);
+      // the direction encoding is visible to the tensor cores (training: and goes to the view stash)
+      if constexpr (TRAIN) {
+        vsw.ready(kVsDir, Es);
+      } else {
+        fence_proxy_async_smem();
+        wg_bar(bar);
+      }
       // ---- views_linears.0 on cat[feature, dirs]: ViewsE (E) then ViewsF (feature fragments), bias + ReLU ----
       uint32_t hv[8][4];
       {
         Acc<views::ViewsF> acc;
         wg_gemm_rs<views::step(views::ViewsF).N, views::step(views::ViewsF).k16, views::step(views::ViewsE).k16>(acc, h, ring, true, a_e, W, 331);
-        epi_bias_frag<128, true>(acc, v.bias + views::b_off(views::ViewsF), hv);
+        epi_bias_frag<128, true, TRAIN>(acc, v.bias + views::b_off(views::ViewsF), hv, TRAIN ? vst + kVsHv.off : nullptr, g,
+                                        TRAIN ? t.hv_mask + static_cast<long long>(tile) * kHvMaskTileBytes : nullptr);
       }
       // ---- Rgb: rgb_linear(hv); raw = [rgb, alpha] (run_nerf_helpers.py:303-304) ----
       {
@@ -495,6 +526,9 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bend_kernel(const FieldF
 }
 __global__ void __launch_bounds__(kFwdThreads, 1) field_views_kernel(const FieldFwdParams p, const ViewParams v) {
   field_fwd_body<false, false, false, kViews>(p, v);
+}
+__global__ void __launch_bounds__(kFwdThreads, 1) field_views_train_kernel(const FieldFwdParams p, const ViewParams v, const ViewTrainParams t) {
+  field_fwd_body<false, true, false, kViews>(p, v, t);
 }
 
 // Ray bias of the time-conditioned baseline: rb[n][l][o] = b_l[o] + sum_k W_l[o][63 + k] z[n][k] for l = L0, L5, in fp32
@@ -561,6 +595,16 @@ cudaError_t launch_field_views(const FieldFwdParams& p, const ViewParams& v, int
   cudaError_t e = cudaFuncSetAttribute(field_views_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   field_views_kernel<<<p.n_tiles < num_sms ? p.n_tiles : num_sms, kFwdThreads, smem, stream>>>(p, v);
+  return cudaGetLastError();
+}
+
+// Training the view-dependent head without a bender: p.stash / p.relu_mask and t's buffers are written
+cudaError_t launch_field_views_train(const FieldFwdParams& p, const ViewParams& v, const ViewTrainParams& t, int num_sms, cudaStream_t stream) {
+  if (p.n_tiles <= 0) return cudaSuccess;
+  const size_t smem = field_views_smem_bytes();
+  cudaError_t e = cudaFuncSetAttribute(field_views_train_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  field_views_train_kernel<<<p.n_tiles < num_sms ? p.n_tiles : num_sms, kFwdThreads, smem, stream>>>(p, v, t);
   return cudaGetLastError();
 }
 

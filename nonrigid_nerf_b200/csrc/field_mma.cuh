@@ -109,14 +109,17 @@ __device__ __forceinline__ void wg_gemm(float (&acc)[N / 2], Ring<S>& r, uint32_
 // wg_gemm with the A operand in registers: slab j (K16 MMAs) takes the A fragments K16 j .. K16 j + K16 - 1 of `a`, the
 // fragments of this warpgroup's 64 rows x 16 KF columns (sm90_ptx.cuh: wgmma_rs).  lead: one slab of K16 MMAs with A from
 // shared memory at a_lead (as in wg_gemm) comes first (the embedding columns of the skip layer); it has LEAD_K16 MMAs.
-template <int N, int K16, int LEAD_K16 = K16, int KF, int S>
+// ACC: add to the accumulators instead of overwriting them (two weight images into one accumulator).
+template <int N, int K16, int LEAD_K16 = K16, bool ACC = false, int KF, int S>
 __device__ __forceinline__ void wg_gemm_rs(float (&acc)[N / 2], uint32_t (&a)[KF][4], Ring<S>& r, bool lead, uint32_t a_lead,
                                            const Waiter& W, int code) {
   static_assert(KF % K16 == 0, "whole slabs of A fragments");
   const int lane = threadIdx.x & 31;
   uint32_t prev = 0;
+  if constexpr (!ACC) {
 #pragma unroll
-  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  }
   if (lead) {
     W.wait(&r.full[r.stage], r.phase, code);
     const uint64_t adesc = gmma_desc(a_lead, kChunkBytes, 128);
@@ -139,7 +142,7 @@ __device__ __forceinline__ void wg_gemm_rs(float (&acc)[N / 2], uint32_t (&a)[KF
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < K16; ++k)
-      wgmma_rs<N, 0>(acc, a[j * K16 + k], gmma_desc_advance(bdesc, k * 2 * N * 16), (lead || j || k) ? 1u : 0u);
+      wgmma_rs<N, 0>(acc, a[j * K16 + k], gmma_desc_advance(bdesc, k * 2 * N * 16), (ACC || lead || j || k) ? 1u : 0u);
     wgmma_commit();
     if (lead || j > 0) {   // the previous slab's MMAs have retired: hand its stage back while this slab's run
       wgmma_wait<1>();

@@ -129,6 +129,23 @@ constexpr int kViewsBiasFloats = views::b_off(views::kEnd);
 constexpr int kViewsPackedBytes = kViewsWBytes + kViewsBiasFloats * 4;
 static_assert(views::b_off(views::ViewsE) == 256 && views::b_off(views::ViewsF) == 256 && views::b_off(views::Rgb) == 384, "view biases");
 static_assert(kViewsWBytes == 208896 && kViewsPackedBytes == 210496, "view-head images");
+// Training the view-dependent head without a bender: the DGRAD steps in front of the trunk's, step ids continuing the DGRAD
+// table.  Rgb^T (A = d_raw, K = 16: rgb_linear has zero column 3, so alpha's channel drops out) -> dhv; ViewsF^T (A = dYv)
+// -> dF; Feature^T (A = dF) -> dh8, to which head^T of the NeRF pack adds alpha's term (its column 3 is alpha_linear,
+// the rest zero).  ViewsE^T is not needed: without a bender the direction gradient has no consumer.  The images are a
+// packed block of their own (nrn_pack_views_t): Rgb^T | ViewsF^T | Feature^T.
+namespace vdgrad {
+enum Id : int { RgbT = dgrad::kCount, ViewsFT, FeatureT, kEnd };
+__host__ __device__ constexpr int forward_of(int s) { return s == RgbT ? views::Rgb : s == ViewsFT ? views::ViewsF : views::Feature; }
+__host__ __device__ constexpr WImage image(int s) { return views::image(forward_of(s)).t(); }
+__host__ __device__ constexpr Step step(int s) { return make_step(image(s)); }
+__host__ __device__ constexpr int w_off(int s) { int o = 0; for (int i = RgbT; i < s; ++i) o += image(i).bytes(); return o; }
+}  // namespace vdgrad
+constexpr int kViewsTWBytes = vdgrad::w_off(vdgrad::kEnd);
+static_assert(vdgrad::image(vdgrad::RgbT).rows == 128 && vdgrad::image(vdgrad::RgbT).chunks == 2 &&
+              vdgrad::image(vdgrad::ViewsFT).rows == 256 && vdgrad::image(vdgrad::ViewsFT).chunks == 16 &&
+              vdgrad::image(vdgrad::FeatureT).rows == 256 && vdgrad::image(vdgrad::FeatureT).chunks == 32, "view-head transposed images");
+static_assert(kViewsTWBytes == 200704, "view-head transposed block");
 
 // A tile image of the stashes: `chunks` 8-column chunks of 128 rows (fp16, chunk-major) at byte `off` of the tile.
 struct Image {
@@ -186,6 +203,22 @@ constexpr MaskImage kMkHb4 = kMkHb3.next(8 * kStHb4.chunks);
 constexpr int kMaskTileBytes = kMkHb4.end();
 static_assert(kStashTileBytes == 634880 && kGradTileBytes == 618496 && kMaskTileBytes == 40960, "stash tiles");
 static_assert(kTanTileBytes == 94208 && kAdjTileBytes == 90112, "divergence stash tiles");
+// Training the view-dependent head (no bender), buffers of their own next to the trunk's:
+//   view stash, per tile: Dir (direction encoding, 27 columns + 5 zero), F (feature_linear output), Hv (post-ReLU
+//   views_linears.0 output); Dir and F are adjacent, the B operand [Dir | F] of views_linears.0's WGRAD.
+//   view gradient stash, per tile: dYv (pre-activation gradient of views_linears.0), dF (gradient of the feature).
+//   Hv mask, per tile: the ReLU mask bits of Hv (ReluMask<128>: 16 B per row).
+constexpr Image kVsDir{0, views::image(views::ViewsE).chunks};
+constexpr Image kVsF = kVsDir.next(views::image(views::Feature).rows / 8);
+constexpr Image kVsHv = kVsF.next(views::image(views::ViewsF).rows / 8);
+constexpr int kVStashTileBytes = kVsHv.end();
+constexpr Image kVgYv{0, views::image(views::ViewsF).rows / 8};
+constexpr Image kVgF = kVgYv.next(views::image(views::Feature).rows / 8);
+constexpr int kVGradTileBytes = kVgF.end();
+constexpr MaskImage kMkHv{0, views::image(views::ViewsF).rows};
+constexpr int kHvMaskTileBytes = kMkHv.end();
+static_assert(kVsDir.chunks == 4 && kVsF.chunks == 32 && kVsHv.chunks == 16 && kVgYv.chunks == 16 && kVgF.chunks == 32, "view stash images");
+static_assert(kVStashTileBytes == 106496 && kVGradTileBytes == 98304 && kHvMaskTileBytes == 2048, "view stash tiles");
 
 // Flat gradient buffers, in the reference's parameter order and shapes ([out][in] weights, then the bias):
 //   NeRF   : W0[256][63] b0 W1[256][256] b1 ... W5[256][63 + 256] b5 ... W7 b7 Wout[out_ch][256] bout
@@ -208,6 +241,17 @@ static_assert(nerf_grad_floats(4) == 494084 && nerf_grad_floats(5) == 494341 && 
 // and layer (L0, L5): the "ray bias" [rays][2][256].
 __host__ __device__ constexpr int nerf_tc_grad_floats(int out_ch) { return nerf_grad_floats(out_ch) + 2 * 256 * kLatent; }
 static_assert(nerf_tc_grad_floats(5) == 510725, "time-conditioned gradient buffer");
+// View-dependent head (NeRF(use_viewdirs=True), module parameter order): the trunk W0 b0 .. W7 b7, then the head block
+//   views_linears.0 W[128][256 + 27] b, feature_linear W[256][256] b, alpha_linear W[1][256] b, rgb_linear W[3][128] b
+namespace vparam {
+enum Id : int { ViewsW, ViewsB, FeatureW, FeatureB, AlphaW, AlphaB, RgbW, RgbB, kCount };
+constexpr int kShape[kCount][2] = {{128, 256 + views::kDirCols}, {128, 1}, {256, 256}, {256, 1}, {1, 256}, {1, 1}, {3, 128}, {3, 1}};
+__host__ __device__ constexpr int floats(int i) { return kShape[i][0] * kShape[i][1]; }
+__host__ __device__ constexpr int total() { int n = 0; for (int i = 0; i < kCount; ++i) n += floats(i); return n; }
+}  // namespace vparam
+constexpr int kViewsTrunkFloats = nerf_grad_floats(4) - 4 * 257;
+__host__ __device__ constexpr int nerf_views_grad_floats() { return kViewsTrunkFloats + vparam::total(); }
+static_assert(kViewsTrunkFloats == 493056 && vparam::total() == 102788 && nerf_views_grad_floats() == 595844, "view-head gradient buffer");
 
 struct FieldBwdParams {
   long long P;
@@ -269,6 +313,17 @@ struct ViewParams {
   const float* viewdirs;       // no bender: normalised view directions, one row per ray (ray mode) or point (point mode)
   long long viewdirs_stride;   // floats between rows
   float4* ws;                  // bend workspace [P]: bent xyz and rigidity of every point (bend pass out, view head in)
+};
+// Training the view-dependent head (no bender), next to a FieldFwdParams and a ViewParams
+struct ViewTrainParams {
+  uint8_t* vstash;             // view stash [n_tiles even][kVStashTileBytes]
+  uint8_t* hv_mask;            // ReLU masks of Hv [n_tiles even][kHvMaskTileBytes]
+};
+// Its DGRAD, next to a FieldBwdParams
+struct ViewBwdParams {
+  const uint8_t* wT;           // nrn_pack_views_t images
+  const uint8_t* hv_mask;      // the forward's Hv masks
+  uint8_t* vgstash;            // view gradient stash [n_tiles even][kVGradTileBytes]
 };
 
 // Time-conditioned backward: the per-ray sums s_l[ray] = sum over the ray's samples of dY_l (l = L0, L5), d z and the

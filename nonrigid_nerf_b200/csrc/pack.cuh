@@ -23,5 +23,6 @@ struct ViewsSrc {
 cudaError_t launch_pack_nerf(const NerfSrc& src, int in_ch, int out_ch, void* packed, cudaStream_t st);
 cudaError_t launch_pack_bender(const BenderSrc& src, void* packed, cudaStream_t st);
 cudaError_t launch_pack_views(const ViewsSrc& src, void* packed, cudaStream_t st);
+cudaError_t launch_pack_views_t(const ViewsSrc& src, void* packed, cudaStream_t st);   // weights only (src.b not read)
 
 }  // namespace nrn

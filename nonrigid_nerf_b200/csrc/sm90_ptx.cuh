@@ -184,6 +184,18 @@ __device__ __forceinline__ void wgmma_m64n16(float (&d)[8], uint64_t adesc, uint
 }
 
 template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n32(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "%16, %17, p, 1, 1, %19, %20;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
 __device__ __forceinline__ void wgmma_m64n48(float (&d)[24], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
@@ -257,8 +269,9 @@ __device__ __forceinline__ void wgmma_m64n256(float (&d)[128], uint64_t adesc, u
 
 template <int N, int TA, int TB>
 __device__ __forceinline__ void wgmma(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  static_assert(N == 16 || N == 48 || N == 64 || N == 80 || N == 96 || N == 128 || N == 256, "wgmma: N without a wrapper");
+  static_assert(N == 16 || N == 32 || N == 48 || N == 64 || N == 80 || N == 96 || N == 128 || N == 256, "wgmma: N without a wrapper");
   if constexpr (N == 16) wgmma_m64n16<TA, TB>(d, adesc, bdesc, accumulate);
+  else if constexpr (N == 32) wgmma_m64n32<TA, TB>(d, adesc, bdesc, accumulate);
   else if constexpr (N == 48) wgmma_m64n48<TA, TB>(d, adesc, bdesc, accumulate);
   else if constexpr (N == 64) wgmma_m64n64<TA, TB>(d, adesc, bdesc, accumulate);
   else if constexpr (N == 80) wgmma_m64n80<TA, TB>(d, adesc, bdesc, accumulate);

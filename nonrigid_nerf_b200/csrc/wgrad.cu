@@ -105,6 +105,37 @@ __device__ __forceinline__ Job job_desc(int j, int half, int g, int compact) {
   return jb;
 }
 
+// View-dependent head (training without a bender, wgrad_views_kernel): the trunk's jobs 0-9 (job 0's row 3 is
+// alpha_linear), then 12 = feature_linear (A = dF, B = H8; two halves like a NeRF layer), 13 and 15 = views_linears.0's
+// feature and direction columns (A = dYv, B = F / Dir of the view stash: 48 and 20 chunks a stage, so that the ring
+// holds two and four stages), 14 = rgb_linear (A = d_raw, B = Hv).
+// Scratch partial layout: job 12 [256 rows][256]; job 13 [128 rows][256] (+ the bias); job 15 [128 rows][32]; job 14
+// [16 rows][128].
+constexpr int kJobFeature = 12, kJobViewsF = 13, kJobRgb = 14, kJobViewsE = 15;
+__device__ __forceinline__ Job views_job_desc(int j, int half, int g) {
+  if (j <= 9) return job_desc(j, half, g, 0);
+  Job jb{};
+  jb.bias = 1;
+  if (j == kJobFeature) {
+    jb.a_off = kVgF.off + half * 16 * kChunkBytes; jb.a_chunks = 16;
+    jb.b_off = kStH + 7 * kHBytes; jb.b_chunks = kHChunks;
+    jb.bias_off = half * 128;
+    const int m0 = half * 128 + g * 64;
+    jb.u[0] = {8 * g, 0, m0 * 256, 256, 64};
+  } else if (j == kJobViewsF || j == kJobViewsE) {
+    const Image b = j == kJobViewsF ? kVsF : kVsDir;
+    jb.a_off = kVgYv.off; jb.a_chunks = kVgYv.chunks;
+    jb.b_off = b.off; jb.b_chunks = b.chunks;
+    jb.bias = j == kJobViewsF;   // the bias gradient once
+    jb.u[0] = {8 * g, 0, g * 64 * 8 * b.chunks, 8 * b.chunks, 64};
+  } else {
+    jb.a_off = kGsRaw.off; jb.a_chunks = kGsRaw.chunks;
+    jb.b_off = kVsHv.off; jb.b_chunks = kVsHv.chunks;
+    jb.u[0] = {0, 0, 0, 8 * kVsHv.chunks, g == 0 ? 8 * kGsRaw.chunks : 0};
+  }
+  return jb;
+}
+
 struct Shared {
   uint64_t full[kMaxStages];
   uint64_t empty[kMaxStages];
@@ -325,6 +356,103 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradParams 
   cluster_sync();
 }
 
+// The view-dependent head's job set (views_job_desc): wgrad_kernel with A and B blocks from the view stashes as well
+__global__ void __launch_bounds__(kWgThreads, 1) wgrad_views_kernel(const WgradParams p, const WgradViewParams v) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  Shared* sh = reinterpret_cast<Shared*>(smem + kRingBytes);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+  int job_id = 0, split = 0, nsplit = 1, half = 0, halves = 1, part_idx = 0;
+  const bool have = locate(p, blockIdx.x, job_id, split, nsplit, half, halves, part_idx);
+  const Job jb = views_job_desc(job_id, half, (warp >> 2) & 1);
+  // contiguous tile range of this split
+  const int per = (p.n_tiles + nsplit - 1) / nsplit;
+  const int t_begin = have ? min(split * per, p.n_tiles) : 0;
+  const int t_end = have ? min(t_begin + per, p.n_tiles) : 0;
+  const int n_local = t_end - t_begin;
+  // the two halves of a NeRF-layer split share their B blocks with the other CTA of the cluster; every other CTA
+  // (head, bender jobs, an idle CTA) works alone and shares only the cluster barriers with its neighbour
+  const bool paired = have && halves == 2;
+  const uint32_t rank = cluster_ctarank(), partner = rank ^ 1u;
+  // both halves of a split have the same A and B block sizes, hence the same stage layout
+  const int stage_bytes = (jb.a_chunks + jb.b_chunks) * kChunkBytes;
+  const int n_stages = min(kMaxStages, kRingBytes / stage_bytes);
+
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < n_stages; ++i) {
+      mbar_init(&sh->full[i], 1);
+      mbar_init(&sh->empty[i], paired ? 16 : 8);   // one arrival per consumer warp of every CTA that reads the stage
+    }
+    sh->abort_flag = 0;
+    fence_mbar_init();
+  }
+  // the partner's barriers are initialised before any multicast data or remote arrival can reach them
+  cluster_sync();
+  const Waiter W{&sh->abort_flag, p.err, paired, paired ? mapa_shared(&sh->abort_flag, partner) : 0u};
+  const Ring R{smem, stage_bytes, n_stages, paired, paired ? mapa_shared(&sh->empty[0], partner) : 0u};
+
+  if (warp >= 8) {
+    setmaxnreg_dec<kProducerRegs>();
+    // ===================== producer: one tile's A and B blocks per stage, 16 KB bulk copies =====================
+    if (warp == 8 && lane == 0) {
+      const uint32_t a_bytes = static_cast<uint32_t>(jb.a_chunks) * kChunkBytes, b_bytes = static_cast<uint32_t>(jb.b_chunks) * kChunkBytes;
+      // paired: this CTA fetches its own A block and its half of the B block, the latter multicast into both CTAs
+      const uint32_t b_begin = paired ? rank * (b_bytes / 2) : 0u, b_end = paired ? b_begin + b_bytes / 2 : b_bytes;
+      // the stashes the job's A and B blocks come from
+      const uint8_t* a_base = p.gstash;
+      const uint8_t* b_base = p.stash;
+      long long a_tile = p.gstash_tile_bytes, b_tile = p.stash_tile_bytes;
+      if (job_id == kJobFeature || job_id == kJobViewsF || job_id == kJobViewsE) { a_base = v.vgstash; a_tile = kVGradTileBytes; }
+      if (job_id == kJobViewsF || job_id == kJobViewsE || job_id == kJobRgb) { b_base = v.vstash; b_tile = kVStashTileBytes; }
+      uint32_t stage = 0, phase = 0;
+      for (int it = 0; it < n_local; ++it) {
+        const long long tile = t_begin + it;
+        const uint8_t* a_src = a_base + tile * a_tile + jb.a_off;
+        const uint8_t* b_src = b_base + tile * b_tile + jb.b_off;
+        W.wait(&sh->empty[stage], phase ^ 1u, 101);
+        mbar_arrive_expect_tx(&sh->full[stage], a_bytes + b_bytes);   // the partner delivers the other half of B
+        uint8_t* dst = smem + stage * stage_bytes;
+        for (uint32_t o = 0; o < a_bytes; o += kPieceBytes)
+          tma_bulk_g2s(dst + o, a_src + o, a_bytes - o < kPieceBytes ? a_bytes - o : kPieceBytes, &sh->full[stage]);
+        dst += a_bytes;
+        for (uint32_t o = b_begin; o < b_end; o += kPieceBytes) {
+          const uint32_t n = b_end - o < kPieceBytes ? b_end - o : kPieceBytes;
+          if (paired) tma_bulk_g2s_multicast(dst + o, b_src + o, n, &sh->full[stage], 0x3);
+          else tma_bulk_g2s(dst + o, b_src + o, n, &sh->full[stage]);
+        }
+        if (++stage == n_stages) { stage = 0; phase ^= 1u; }
+      }
+    }
+  } else {
+    setmaxnreg_inc<kConsumerRegs>();
+    const int g = warp >> 2;
+    float* part = p.scratch + static_cast<size_t>(part_idx) * kWgScratchFloats;
+    const Unit& u0 = jb.u[0];
+    const Unit& u1 = jb.u[1];
+    if (job_id == kJobViewsF) {
+      consume<8 * kVsF.chunks, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
+    } else if (job_id == kJobViewsE) {
+      consume<8 * kVsDir.chunks, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
+    } else if (job_id == kJobRgb) {
+      if (u0.rows > 0) consume<8 * kVsHv.chunks, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
+      else consume<0, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
+    } else {   // the trunk's jobs 0-9 and feature_linear (a NeRF layer's shape)
+      const bool mine = u0.rows > 0;
+      if (job_id == 8 || job_id == 9) {
+        if (mine) consume<8 * kStE.chunks, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
+        else consume<0, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
+      } else {
+        if (mine) consume<8 * kHChunks, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
+        else consume<0, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
+      }
+    }
+  }
+  // as wgrad_kernel: no CTA leaves while its partner may still arrive on its barriers or write its abort flag
+  __syncwarp();
+  cluster_sync();
+}
+
+
 // ------------------------------------------------------------------------------------------------
 // Deterministic reduction of the split partials into the reference's parameter layout.
 // One thread per destination element of the flat gradient buffers (their shapes: nrn_common.cuh).
@@ -436,7 +564,73 @@ __device__ __forceinline__ Src bender_src(int idx, bool& ok) {
   return {10, c_yb2 + 64, -1, 1};                                                 // rig_b2
 }
 
+// View-dependent head: the trunk as nerf_src (jobs 1-9), then the head block in module order (nrn_common.cuh: vparam)
+__device__ __forceinline__ Src views_src(int idx) {
+  bool ok;
+  if (idx < kViewsTrunkFloats) return nerf_src<false>(idx, 4, ok);
+  idx -= kViewsTrunkFloats;
+  using namespace vparam;
+  constexpr int kIn = kShape[ViewsW][1], kDir = 8 * kVsDir.chunks;
+  if (idx < floats(ViewsW)) {   // [feature | direction encoding] inputs: the feature job's and the direction job's partials
+    const int m = idx / kIn, k = idx % kIn;
+    return k < 256 ? Src{kJobViewsF, m * 256 + k, -1, 0} : Src{kJobViewsE, m * kDir + (k - 256), -1, 0};
+  }
+  idx -= floats(ViewsW);
+  if (idx < floats(ViewsB)) return {kJobViewsF, idx, -1, 1};
+  idx -= floats(ViewsB);
+  if (idx < floats(FeatureW)) return nerf_w(kJobFeature, idx >> 8, idx & 255);
+  idx -= floats(FeatureW);
+  if (idx < floats(FeatureB)) return nerf_b(kJobFeature, idx);
+  idx -= floats(FeatureB);
+  if (idx < floats(AlphaW)) return nerf_w(0, 3, idx);   // the head job's row 3
+  idx -= floats(AlphaW);
+  if (idx < floats(AlphaB)) return nerf_b(0, 3);
+  idx -= floats(AlphaB);
+  if (idx < floats(RgbW)) return {kJobRgb, (idx >> 7) * 128 + (idx & 127), -1, 0};
+  return {kJobRgb, idx - floats(RgbW), -1, 1};
+}
+
 }  // namespace
+
+// The fixed-order sum over the split partials of job s.job (split 0, 1, 2, ...), as wgrad_reduce's: deterministic gradients
+__device__ __forceinline__ float split_sum(const WgradParams& p, const Src& s) {
+  float sum = 0.f;
+  int base = 0, slot = -1;
+  for (int j = 0; j < p.n_jobs; ++j) {
+    if (p.job_ids[j] == s.job) { slot = j; break; }
+    base += p.splits[j];
+  }
+  if (slot >= 0) {
+    const int nsplit = p.splits[slot];
+    const int per = (p.n_tiles + nsplit - 1) / nsplit;
+    const int n_valid = min(nsplit, (p.n_tiles + per - 1) / per);   // splits beyond that owned no tiles: scratch unwritten
+    const float* __restrict__ src = p.scratch + static_cast<size_t>(base) * kWgScratchFloats + (s.bias ? 65536 + s.off : s.off);
+    const bool has2 = !s.bias && s.off2 >= 0;
+    const int d2 = has2 ? s.off2 - s.off : 0;
+    // fixed summation order (split 0, 1, 2, ...) = deterministic gradients; the loads of 8 splits are in flight together
+    int sp = 0;
+    for (; sp + 8 <= n_valid; sp += 8) {
+      float a[8], b[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float* q = src + static_cast<size_t>(sp + i) * kWgScratchFloats;
+        a[i] = __ldg(q);
+        b[i] = has2 ? __ldg(q + d2) : 0.f;
+      }
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        sum += a[i];
+        if (has2) sum += b[i];
+      }
+    }
+    for (; sp < n_valid; ++sp) {
+      const float* q = src + static_cast<size_t>(sp) * kWgScratchFloats;
+      sum += __ldg(q);
+      if (has2) sum += __ldg(q + d2);
+    }
+  }
+  return sum;
+}
 
 template <bool TC>
 __device__ __forceinline__ void wgrad_reduce(const WgradParams p, const WgradDst dst, int out_ch, const float* dw_lat) {
@@ -498,12 +692,88 @@ __device__ __forceinline__ void wgrad_reduce(const WgradParams p, const WgradDst
   *out = acc ? *out + v : v;
 }
 
+
 __global__ void wgrad_reduce_kernel(const WgradParams p, const WgradDst dst, int out_ch) { wgrad_reduce<false>(p, dst, out_ch, nullptr); }
 __global__ void wgrad_reduce_tc_kernel(const WgradParams p, const WgradDst dst, int out_ch, const float* dw_lat) {
   wgrad_reduce<true>(p, dst, out_ch, dw_lat);
 }
+// The view-dependent head's flat layout (nerf_views_grad_floats): dst.nerf the trunk, dst.nerf_head (or behind it) the
+// head block; dst.nerf_n is the whole count
+__global__ void wgrad_views_reduce_kernel(const WgradParams p, const WgradDst dst) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= dst.nerf_n) return;
+  const float v = split_sum(p, views_src(idx)) / loss_scale(p.amax);
+  float* out = (idx >= kViewsTrunkFloats && dst.nerf_head) ? dst.nerf_head + (idx - kViewsTrunkFloats) : dst.nerf + idx;
+  *out = dst.acc_nerf ? *out + v : v;
+}
 
 // ------------------------------------------------------------------------------------------------
+namespace {
+// Plans how the jobs jobs[0, n) (cost: relative bytes per tile of one of its CTAs; halves: CTAs per split) split their
+// tiles over the CTAs, writes the plan into p and launches `kernel` (wgrad_kernel or wgrad_views_kernel).
+template <typename... Args>
+cudaError_t launch_jobs(void (*kernel)(WgradParams, Args...), int* s_max_clusters, WgradParams& p, const int* jobs, const int* cost,
+                        const int* halves, int n, int num_sms, cudaStream_t st, Args... args) {
+  // Launched in clusters of 2 CTAs (the two halves of a NeRF-layer split).  A cluster lives inside one GPC, so the
+  // CTAs that can run at once are the resident clusters x 2, which can be fewer than the SMs.
+  const size_t smem = kRingBytes + sizeof(Shared) + 64;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  cudaLaunchAttribute cluster{};
+  cluster.id = cudaLaunchAttributeClusterDimension;
+  cluster.val.clusterDim.x = 2; cluster.val.clusterDim.y = 1; cluster.val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(2); cfg.blockDim = dim3(kWgThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cfg.attrs = &cluster; cfg.numAttrs = 1;
+  int dev = 0;
+  e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
+  if (s_max_clusters[dev] <= 0) {
+    e = cudaOccupancyMaxActiveClusters(&s_max_clusters[dev], kernel, &cfg);
+    if (e != cudaSuccess) return e;
+    if (s_max_clusters[dev] <= 0) return cudaErrorInvalidConfiguration;
+  }
+  const int max_ctas = min(num_sms, 2 * s_max_clusters[dev]) & ~1;
+
+  // Every CTA streams at about the same bytes/clk (the kernel is HBM-bound), so the launch ends when the CTA with the
+  // most bytes ends: start with one split per job and hand each further split (its halves' CTAs) to the job whose CTAs
+  // currently carry the most (chunks per tile x tiles per CTA).
+  int splits[16], used = 0;
+  for (int j = 0; j < n; ++j) {
+    splits[j] = 1;
+    used += halves[j];
+  }
+  const int tiles = p.n_tiles > 0 ? p.n_tiles : 1;
+  for (;;) {
+    int best = -1;
+    long long best_load = -1;
+    for (int j = 0; j < n; ++j) {
+      const int sp = splits[j];
+      if (sp >= tiles || used + halves[j] > max_ctas) continue;   // a CTA needs at least one tile
+      const long long load = static_cast<long long>(cost[j]) * ((tiles + sp - 1) / sp);
+      if (load > best_load) { best_load = load; best = j; }
+    }
+    if (best < 0) break;
+    ++splits[best];
+    used += halves[best];
+  }
+  // CTA order: the two-half jobs first, so that the halves of every split are the two CTAs of one cluster; then the
+  // one-CTA jobs (head, bender; all jobs of the compact launch), two splits to a cluster without multicast, and one
+  // idle CTA when their count is odd.  The scratch partials follow the same order (the reduce kernels look jobs up).
+  p.n_jobs = 0;
+  for (int h = 2; h >= 1; --h)
+    for (int j = 0; j < n; ++j)
+      if (halves[j] == h) { p.job_ids[p.n_jobs] = jobs[j]; p.splits[p.n_jobs] = splits[j]; p.halves[p.n_jobs] = h; ++p.n_jobs; }
+  if (p.n_tiles > 0) {
+    cfg.gridDim = dim3((used + 1) & ~1);
+    e = cudaLaunchKernelEx(&cfg, kernel, p, args...);
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
+}
+}  // namespace
+
 cudaError_t launch_wgrad(WgradParams p, bool has_bender, int num_sms, const WgradDst& dst, int out_ch, cudaStream_t st,
                          const float* tc_dw_lat) {
   // relative cost of one tile of every job's CTAs = 2 KB chunks a CTA receives (a NeRF layer's half: 16 gradient
@@ -515,67 +785,35 @@ cudaError_t launch_wgrad(WgradParams p, bool has_bender, int num_sms, const Wgra
   if (p.compact) { first = 10; last = 12; p.stash_tile_bytes = kTanTileBytes; p.gstash_tile_bytes = kAdjTileBytes; }
   else { p.stash_tile_bytes = kStashTileBytes; p.gstash_tile_bytes = kGradTileBytes; }
 
-  // Launched in clusters of 2 CTAs (the two halves of a NeRF-layer split).  A cluster lives inside one GPC, so the
-  // CTAs that can run at once are the resident clusters x 2, which can be fewer than the SMs.
-  const size_t smem = kRingBytes + sizeof(Shared) + 64;
-  cudaError_t e = cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  cudaLaunchAttribute cluster{};
-  cluster.id = cudaLaunchAttributeClusterDimension;
-  cluster.val.clusterDim.x = 2; cluster.val.clusterDim.y = 1; cluster.val.clusterDim.z = 1;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2); cfg.blockDim = dim3(kWgThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cfg.attrs = &cluster; cfg.numAttrs = 1;
-  static int s_max_clusters[64];   // per device
-  int dev = 0;
-  e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
-  if (s_max_clusters[dev] <= 0) {
-    e = cudaOccupancyMaxActiveClusters(&s_max_clusters[dev], wgrad_kernel, &cfg);
-    if (e != cudaSuccess) return e;
-    if (s_max_clusters[dev] <= 0) return cudaErrorInvalidConfiguration;
-  }
-  const int max_ctas = min(num_sms, 2 * s_max_clusters[dev]) & ~1;
-
-  // Every CTA streams at about the same bytes/clk (the kernel is HBM-bound), so the launch ends when the CTA with the
-  // most bytes ends: start with one split per job and hand each further split (its halves' CTAs) to the job whose CTAs
-  // currently carry the most (chunks per tile x tiles per CTA).
-  int splits[12], halves[12], used = 0;
+  int jobs[12], cost[12], halves[12], n_jobs = 0;
   for (int j = first; j < last; ++j) {
-    splits[j] = 1;
-    halves[j] = (j >= 1 && j <= 9) ? 2 : 1;   // the head's 16-row dW and the bender jobs fit one CTA
-    used += halves[j];
+    jobs[n_jobs] = j; cost[n_jobs] = kJobChunks[j];
+    halves[n_jobs++] = (j >= 1 && j <= 9) ? 2 : 1;   // the head's 16-row dW and the bender jobs fit one CTA
   }
-  const int tiles = p.n_tiles > 0 ? p.n_tiles : 1;
-  for (;;) {
-    int best = -1;
-    long long best_load = -1;
-    for (int j = first; j < last; ++j) {
-      const int sp = splits[j];
-      if (sp >= tiles || used + halves[j] > max_ctas) continue;   // a CTA needs at least one tile
-      const long long load = static_cast<long long>(kJobChunks[j]) * ((tiles + sp - 1) / sp);
-      if (load > best_load) { best_load = load; best = j; }
-    }
-    if (best < 0) break;
-    ++splits[best];
-    used += halves[best];
-  }
-  // CTA order: the two-half jobs first, so that the halves of every split are the two CTAs of one cluster; then the
-  // one-CTA jobs (head, bender; all jobs of the compact launch), two splits to a cluster without multicast, and one
-  // idle CTA when their count is odd.  The scratch partials follow the same order (wgrad_reduce_kernel looks jobs up).
-  p.n_jobs = 0;
-  for (int h = 2; h >= 1; --h)
-    for (int j = first; j < last; ++j)
-      if (halves[j] == h) { p.job_ids[p.n_jobs] = j; p.splits[p.n_jobs] = splits[j]; p.halves[p.n_jobs] = h; ++p.n_jobs; }
-  if (p.n_tiles > 0) {
-    cfg.gridDim = dim3((used + 1) & ~1);
-    e = cudaLaunchKernelEx(&cfg, wgrad_kernel, p);
-    if (e != cudaSuccess) return e;
-  }
+  static int s_max_clusters[64];   // per device
+  cudaError_t e = launch_jobs(wgrad_kernel, s_max_clusters, p, jobs, cost, halves, n_jobs, num_sms, st);
+  if (e != cudaSuccess) return e;
   const int n = dst.nerf_n + dst.bend_n;
   if (n > 0 && tc_dw_lat) wgrad_reduce_tc_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, dst, out_ch, tc_dw_lat);
   else if (n > 0) wgrad_reduce_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, dst, out_ch);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_wgrad_views(WgradParams p, const WgradViewParams& v, int num_sms, const WgradDst& dst, cudaStream_t st) {
+  // costs as launch_wgrad's (chunks a CTA receives per tile): the trunk's jobs unchanged; feature_linear's half 16 + 32
+  // like a NeRF layer's; views_linears.0's feature columns 16 + 32, its direction columns 16 + 4 (both one MMA over a
+  // double-buffered ring); rgb_linear 2 + 16 with the head job's surcharge
+  static const int kViewJobChunks[14] = {46, 48, 48, 48, 48, 48, 48, 48, 16 + 8 + 8, 16 + 8 + 8, 48, 48, 24, 20};
+  int jobs[14], halves[14];
+  for (int j = 0; j < 14; ++j) {
+    jobs[j] = j < 10 ? j : kJobFeature + (j - 10);   // 12 feature, 13 views (feature columns), 14 rgb, 15 views (directions)
+    halves[j] = (jobs[j] >= 1 && jobs[j] <= 9) || jobs[j] == kJobFeature ? 2 : 1;
+  }
+  p.stash_tile_bytes = kStashTileBytes; p.gstash_tile_bytes = kGradTileBytes;
+  static int s_max_clusters[64];   // per device
+  cudaError_t e = launch_jobs(wgrad_views_kernel, s_max_clusters, p, jobs, kViewJobChunks, halves, 14, num_sms, st, v);
+  if (e != cudaSuccess) return e;
+  if (dst.nerf_n > 0) wgrad_views_reduce_kernel<<<(dst.nerf_n + 255) / 256, 256, 0, st>>>(p, dst);
   return cudaGetLastError();
 }
 

@@ -36,6 +36,14 @@ struct WgradDst {
 // buffer (tc_dw_lat_kernel, field_bwd.cu)
 cudaError_t launch_wgrad(WgradParams p, bool has_bender, int num_sms, const WgradDst& dst, int out_ch, cudaStream_t st,
                          const float* tc_dw_lat = nullptr);
+// The view-dependent head (training without a bender): the stashes of its head layers, next to p's trunk stashes
+struct WgradViewParams {
+  const uint8_t* vstash;    // view stash (Dir | F | Hv per tile)
+  const uint8_t* vgstash;   // view gradient stash (dYv | dF per tile)
+};
+// the trunk's jobs and the head's in one launch, reduced into the view model's flat layout (nerf_views_grad_floats):
+// dst.nerf the trunk, dst.nerf_head (when given, else behind it) the head block, dst.nerf_n = the whole count
+cudaError_t launch_wgrad_views(WgradParams p, const WgradViewParams& v, int num_sms, const WgradDst& dst, cudaStream_t st);
 // amax[0] = max |x[i]| over n floats (device scalar, overwritten; accumulate: max with its value).  x as rows of
 // `row_len` floats: only the first `cols` of every row take part.
 cudaError_t launch_absmax(const float* x, long long n, float* amax, cudaStream_t st, bool accumulate = false, int row_len = 1,

@@ -132,6 +132,28 @@ def pack_views(net) -> torch.Tensor:
     return buf
 
 
+def pack_views_t(net) -> torch.Tensor:
+    """fp16 transposed images of the view-dependent head for its backward (rgb_linear, views_linears.0's feature columns,
+    feature_linear); cached like pack_views."""
+    ws, _ = views_param_list(net)
+    key = _versions(ws)
+    cache = getattr(net, "_nrn_pack_views_t", None)
+    if cache is not None and cache[0] == key and not FORCE_PACK:
+        return cache[1]
+    for t in ws:
+        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
+            raise RuntimeError("nonrigid_nerf_b200: NeRF parameters must be contiguous fp32 CUDA tensors")
+    if ws[0].shape != (256, 256) or ws[1].shape != (128, 256 + 27) or ws[2].shape != (3, 128):
+        raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True needs W=256 and input_ch_views=27 "
+                           f"(got view-head shapes {[tuple(w.shape) for w in ws]})")
+    lib = _lib.load()
+    buf = cache[1] if cache is not None else torch.empty(lib.nrn_packed_views_t_bytes(), dtype=torch.uint8, device=ws[0].device)
+    with torch.cuda.device(ws[0].device):
+        _lib.check(lib.nrn_pack_views_t(_ptr_array([w.detach() for w in ws]), _ptr(buf), _stream()), "pack_views_t")
+    net._nrn_pack_views_t = (key, buf)
+    return buf
+
+
 def pack_bender(bender) -> torch.Tensor:
     net_w, net_b, rig_w, rig_b = bender_param_list(bender)
     allp = net_w + net_b + rig_w + rig_b
@@ -373,6 +395,44 @@ def field_forward_views(rays: Optional[torch.Tensor], z_vals: Optional[torch.Ten
     with torch.cuda.device(dev):
         _lib.check(lib.nrn_field_forward_views(C.byref(a), C.byref(v)), "field_forward_views")
     return raw, details
+
+
+def field_forward_views_train(rays: torch.Tensor, z_vals: torch.Tensor, viewdirs: torch.Tensor, nerf_pack: torch.Tensor,
+                              views_pack: torch.Tensor, want_details: bool = False):
+    """The view-dependent head without a bender, keeping what its backward needs: raw [N, S, 4], details, and the buffers
+    (stash, relu_mask, views_stash, hv_mask)."""
+    rays = rays if (rays.dtype == torch.float32 and rays.stride(-1) == 1) else rays.float().contiguous()
+    if not rays.is_cuda:
+        raise RuntimeError("nonrigid_nerf_b200: rays must be a CUDA tensor (there is no CPU path)")
+    if rays.stride(0) != 8:
+        rays = rays[:, :8].contiguous()
+    z_vals = _f32c(z_vals, "z_vals")
+    n, s = z_vals.shape
+    dev = rays.device
+    if viewdirs.dtype != torch.float32 or viewdirs.dim() != 2 or viewdirs.stride(1) != 1 or not viewdirs.is_cuda:
+        viewdirs = viewdirs.reshape(viewdirs.shape[0], -1).float().contiguous().to(dev)
+    lib = _lib.load()
+    bufs = {k: torch.empty(f(n, s), dtype=torch.uint8, device=dev) for k, f in (
+        ("stash", lib.nrn_stash_bytes), ("relu_mask", lib.nrn_relu_mask_bytes), ("views_stash", lib.nrn_views_stash_bytes),
+        ("hv_mask", lib.nrn_hv_mask_bytes))}
+    a, v, t = _lib.NrnFieldArgs(), _lib.NrnViewArgs(), _lib.NrnViewTrainArgs()
+    a.rays, a.z_vals, a.n_rays, a.n_samples, a.out_ch = rays.data_ptr(), z_vals.data_ptr(), n, s, 4
+    a.nerf_packed = nerf_pack.data_ptr()
+    raw = torch.empty(n, s, 4, dtype=torch.float32, device=dev)
+    a.raw = raw.data_ptr()
+    details: Dict[str, torch.Tensor] = {}
+    if want_details:
+        details["initial_input_pts"] = torch.empty(n, s, 3, dtype=torch.float32, device=dev)
+        details["input_pts"] = torch.empty(n, s, 3, dtype=torch.float32, device=dev)
+        a.initial_input_pts, a.input_pts = details["initial_input_pts"].data_ptr(), details["input_pts"].data_ptr()
+    a.stash, a.relu_mask = bufs["stash"].data_ptr(), bufs["relu_mask"].data_ptr()
+    a.stream = torch.cuda.current_stream().cuda_stream
+    v.views_packed = views_pack.data_ptr()
+    v.viewdirs, v.viewdirs_stride = viewdirs.data_ptr(), viewdirs.stride(0) if viewdirs.shape[0] > 1 else 3
+    t.views_stash, t.hv_mask = bufs["views_stash"].data_ptr(), bufs["hv_mask"].data_ptr()
+    with torch.cuda.device(dev):
+        _lib.check(lib.nrn_field_forward_views_train(C.byref(a), C.byref(v), C.byref(t)), "field_forward_views_train")
+    return raw, details, bufs
 
 
 def composite(raw: torch.Tensor, z_vals: torch.Tensor, rays_d: torch.Tensor, noise: Optional[torch.Tensor] = None,

@@ -261,9 +261,10 @@ class training_wrapper_class(torch.nn.Module):
 
     def forward(self, args, rays_o, rays_d, i, render_kwargs_train, target_s, global_step, start, dataset_extras,
                 batch_pixel_indices):
-        for net in (self.coarse_model, self.fine_model):   # the view-dependent head cannot be trained yet: raise before any launch
+        # the view-dependent head cannot be trained with a bender yet: raise before any launch, for the bender seated below
+        for net in (self.coarse_model, self.fine_model):
             if net is not None:
-                _ag.views_check(net)
+                _ag.views_check(net, bender=self.ray_bender)
         self.coarse_model.ray_bender = (self.ray_bender,)
         render_kwargs_train["network_fn"] = self.coarse_model
         render_kwargs_train["ray_bender"] = self.ray_bender
