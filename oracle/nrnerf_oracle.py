@@ -400,15 +400,16 @@ def divergence_loss(bp, ret: Dict[str, Tensor], latents: Tensor, n_rays: int, s_
 
 def training_wrapper_loss(cp, fp, bp, rays: Dict[str, Tensor], latent_table: Tensor, imageid_to_timestepid, pixel_indices: Tensor,
                           rnd: Dict[str, Tensor], e: Tensor, global_step: int, n_iters: int, offsets_w: float,
-                          divergence_w: float, rigidity_w: float, s_c: int = 64, n_imp: int = 64):
+                          divergence_w: float, rigidity_w: float, s_c: int = 64, n_imp: int = 64, vpar_c=None, vpar_f=None):
     """Per-ray loss [N] of training_wrapper_class.forward (train.py:152-287): latent lookup by the ray's image id
     (:173-189), training-mode render, data terms, offsets / rigidity regulariser and divergence regulariser, both
-    scaled by the increasing schedule (1/100)^(1 - global_step / N_iters) (:229, :281).  Returns (loss, ret)."""
+    scaled by the increasing schedule (1/100)^(1 - global_step / N_iters) (:229, :281).  vpar_c / vpar_f
+    (make_view_params): the view-dependent heads (use_viewdirs=True), as in render_rays.  Returns (loss, ret)."""
     n = rays["rays_o"].shape[0]
     i2t = torch.as_tensor(imageid_to_timestepid, device=pixel_indices.device)
     lat = latent_table[i2t[pixel_indices[:, 0]], :]
     ret = render_rays(cp, fp, bp, rays["rays_o"], rays["rays_d"], rays["near"], rays["far"], lat, s_c, n_imp, perturb=True,
-                      raw_noise_std=1.0, rnd=rnd)
+                      raw_noise_std=1.0, rnd=rnd, vpar_c=vpar_c, vpar_f=vpar_f)
     sched = (1.0 / 100.0) ** (1 - (global_step / n_iters))
     loss = training_loss(ret, rays["target"], offsets_w, rigidity_w, sched)
     if divergence_w > 0.0:

@@ -118,11 +118,15 @@ def _lib():
 _MODELS = {}
 
 
-def models(bender, tc=False):
-    """(coarse NeRF, bender); tc: the time-conditioned baseline's NeRF (W0 [256][95], W5 [256][351]), no bender."""
-    key = "tc" if tc else bender
+def models(bender, tc=False, views=False):
+    """(coarse NeRF, bender); tc: the time-conditioned baseline's NeRF (W0 [256][95], W5 [256][351]), no bender; views:
+    NeRF(use_viewdirs=True) with tests/viewdirs_reference's weights, no bender."""
+    key = "views" if views else ("tc" if tc else bender)
     if key not in _MODELS:
-        if tc:
+        if views:
+            from tests.viewdirs_reference import build_view_models
+            _MODELS[key] = (build_view_models(O, SEED, DEV, with_bender=False)[0], None)
+        elif tc:
             from nonrigid_nerf_b200 import run_nerf_helpers as H
             cp, _ = TR.make_params(SEED)
             kw = dict(D=8, W=256, input_ch=63, output_ch=5, skips=[4], input_ch_views=0, use_viewdirs=False, ray_bender=None,
@@ -148,11 +152,14 @@ def pack_nerf(ws, bs, out_ch, input_ch=63):
 
 
 class Case:
-    """tc: the time-conditioned baseline (no bender); lat_stride0: one latent row for every ray (latent_stride 0)."""
+    """tc: the time-conditioned baseline (no bender); lat_stride0: one latent row for every ray (latent_stride 0);
+    views: the view-dependent head without a bender (out_ch 4), fed the normalised ray directions `vd`."""
     def __init__(self, n, s, bender=True, out_ch=5, cutoff=None, scaling=None, draw_mag=1.0, reg_mag=0.05, ch4=0.0,
-                 seed=0, tc=False, lat_stride0=False):
+                 seed=0, tc=False, lat_stride0=False, views=False):
         assert not (tc and bender), "the time-conditioned baseline has no bender"
-        self.n, self.s, self.bender, self.out_ch, self.tc = n, s, bender, out_ch, tc
+        if views:
+            bender, out_ch = False, 4
+        self.n, self.s, self.bender, self.out_ch, self.tc, self.views = n, s, bender, out_ch, tc, views
         self.cutoff, self.scaling = cutoff, scaling
         self.P = n * s
         self.T = -(-self.P // SL.TILE_M)
@@ -163,6 +170,7 @@ class Case:
         u = (torch.arange(s, dtype=torch.float32) + torch.rand(n, s, generator=g)) / s
         self.z = (r["near"] + (r["far"] - r["near"]) * u).to(DEV).contiguous()
         self.lat = r["latents"].to(DEV).contiguous()
+        self.vd = torch.nn.functional.normalize(self.rays[:, 3:6], dim=-1).contiguous() if views else None
         if lat_stride0:
             self.lat = self.lat[:1].expand(n, 32)
         mags = torch.tensor([0.3, 0.3, 0.3, 2.0, 0.0][:out_ch])
@@ -183,6 +191,9 @@ def run_forward(cs, train=True, removal=None, points=None):
     """The training kernel (stash and ReLU masks), or with train=False the inference kernel render() runs; `removal`: its
     object-removal threshold; `points` [P, stride >= 3]: point mode (NeRF.forward(x)) instead of cs.rays / cs.z."""
     from nonrigid_nerf_b200 import ops
+    if cs.views:
+        assert train and removal is None and points is None
+        return run_forward_views(cs)
     L = _lib()
     lib = L.load()
     coarse, bend = models(cs.bender, cs.tc)
@@ -230,7 +241,61 @@ def run_forward(cs, train=True, removal=None, points=None):
     return o
 
 
+def run_forward_views(cs):
+    """nrn_field_forward_views_train (autograd._ViewsTrainFn's forward): the trunk's stash and masks, the view stash and
+    the Hv masks; o["ws"] / o["bs"] are the trunk's and alpha_linear's parameters, o["net"] the module."""
+    from nonrigid_nerf_b200 import ops
+    L = _lib()
+    lib = L.load()
+    net, _ = models(False, views=True)
+    ws, bs = ops._views_trunk_params(net)
+    o = {"npk": ops.pack_nerf(net), "vpk": ops.pack_views(net), "vtpk": ops.pack_views_t(net), "net": net, "bend": None,
+         "ws": [w.detach() for w in ws], "bs": [b.detach() for b in bs]}
+    a, v, t = L.NrnFieldArgs(), L.NrnViewArgs(), L.NrnViewTrainArgs()
+    a.rays, a.z_vals, a.n_rays, a.n_samples, a.out_ch = cs.rays.data_ptr(), cs.z.data_ptr(), cs.n, cs.s, 4
+    a.nerf_packed = o["npk"].data_ptr()
+    o["raw"], o["init"], o["bent"] = poison_f32(cs.P, 4), poison_f32(cs.P, 3), poison_f32(cs.P, 3)
+    a.raw, a.initial_input_pts, a.input_pts = o["raw"].data_ptr(), o["init"].data_ptr(), o["bent"].data_ptr()
+    for k, f in (("stash", lib.nrn_stash_bytes), ("mask", lib.nrn_relu_mask_bytes), ("vstash", lib.nrn_views_stash_bytes),
+                 ("hv_mask", lib.nrn_hv_mask_bytes)):
+        o[k] = poison_bytes(f(cs.n, cs.s))
+    a.stash, a.relu_mask = o["stash"].data_ptr(), o["mask"].data_ptr()
+    a.stream = torch.cuda.current_stream().cuda_stream
+    v.views_packed, v.viewdirs, v.viewdirs_stride = o["vpk"].data_ptr(), cs.vd.data_ptr(), cs.vd.stride(0)
+    t.views_stash, t.hv_mask = o["vstash"].data_ptr(), o["hv_mask"].data_ptr()
+    L.check(lib.nrn_field_forward_views_train(C.byref(a), C.byref(v), C.byref(t)), "field_forward_views_train")
+    L.device_error_check()
+    return o
+
+
+def run_backward_views(cs, o, d_raw=None, nerf_grad=None, nerf_head=None, accumulate=False):
+    """nrn_field_backward_views into poisoned buffers: b["nerf_grad"] the flat layout (or the trunk, with `nerf_head` the
+    head block's own destination), b["gstash"] / b["vgstash"] the trunk's and the head's gradient stashes."""
+    L = _lib()
+    lib = L.load()
+    d_raw = cs.d_raw if d_raw is None else d_raw
+    a, v = L.NrnFieldBwdArgs(), L.NrnViewBwdArgs()
+    a.n_rays, a.n_samples, a.out_ch = cs.n, cs.s, 4
+    a.d_raw, a.stash, a.relu_mask, a.nerf_packed = d_raw.data_ptr(), o["stash"].data_ptr(), o["mask"].data_ptr(), o["npk"].data_ptr()
+    b = {"gstash": poison_bytes(lib.nrn_grad_stash_bytes(cs.n, cs.s)), "vgstash": poison_bytes(lib.nrn_views_grad_stash_bytes(cs.n, cs.s)),
+         "scratch": poison_bytes(lib.nrn_wgrad_scratch_bytes())}
+    b["nerf_grad"] = poison_f32(lib.nrn_nerf_views_grad_floats()) if nerf_grad is None else nerf_grad
+    b["nerf_head"] = nerf_head
+    a.grad_stash, a.wgrad_scratch, a.nerf_grad = b["gstash"].data_ptr(), b["scratch"].data_ptr(), b["nerf_grad"].data_ptr()
+    if nerf_head is not None:
+        a.nerf_grad_head = nerf_head.data_ptr()
+    a.accumulate_nerf = 1 if accumulate else 0
+    a.stream = torch.cuda.current_stream().cuda_stream
+    v.views_t_packed, v.views_stash, v.views_grad_stash, v.hv_mask = (o["vtpk"].data_ptr(), o["vstash"].data_ptr(),
+                                                                     b["vgstash"].data_ptr(), o["hv_mask"].data_ptr())
+    L.check(lib.nrn_field_backward_views(C.byref(a), C.byref(v)), "field_backward_views")
+    L.device_error_check()
+    return b
+
+
 def run_backward(cs, o, d_raw=None, nerf_grad=None, nerf_head=None, bender_grad=None, accumulate=False):
+    if cs.views:
+        return run_backward_views(cs, o, d_raw, nerf_grad, nerf_head, accumulate)
     L = _lib()
     lib = L.load()
     d_raw = cs.d_raw if d_raw is None else d_raw
@@ -447,8 +512,11 @@ def check_forward(cs, o, rep, tiles=None):
         Wl = W0p if l == 0 else (W5p if l == 5 else W[l])
         v, a = mm(inp, Wl)
         rep.check(f"H{l + 1}", H[l], torch.relu(v + b[l]), a + b[l].abs(), c_mma(Wl.shape[1]), True)
-    v, a = mm(H[7][:P], W[8])
-    rep.check("raw", sub.pt(o["raw"]), v + b[8], a + b[8].abs(), c_mma(256))
+    if cs.views:
+        check_view_head(cs, o, rep, sub, H[7])
+    else:
+        v, a = mm(H[7][:P], W[8])
+        rep.check("raw", sub.pt(o["raw"]), v + b[8], a + b[8].abs(), c_mma(256))
     # ReLU mask bits: the encoding of stash image > 0, every bit of every word, rows past P included
     imgs = [sub.img(st, SL.STASH_TILE, oc) for oc in SL.ST_H]
     names = [f"H{l + 1}" for l in range(8)]
@@ -461,12 +529,75 @@ def check_forward(cs, o, rep, tiles=None):
         assert torch.equal(got, enc), f"ReLU mask of {nm}: {int((got != enc).sum())} bytes differ from stash > 0"
 
 
+# The direction encoding's sin / cos: the phase 2^k d / 2 pi is reduced exactly to [-1/2, 1/2) turns (field_fwd.cu,
+# encode_octaves); the reduced phase (one fp32 add), its product with fl(2 pi) (one fp32 multiply, fl(2 pi) itself within
+# 2^-24 relative) put the angle in [-pi, pi] within 2^-22 absolute, and __sinf / __cosf err by at most 2^-21.41 / 2^-21.19
+# there (CUDA C++ Programming Guide, intrinsic functions).  |d sin / d angle| <= 1, so the fp32 value lies within
+# 2^-21.19 + 2^-22 (6.6e-7; DESIGN section 2: about 4e-7 for MUFU alone) of the exact encoding of the fp32 direction,
+# and its fp16 image within half an ulp more.
+E_DIR_ENC = 2.0 ** -21.19 + 2.0 ** -22
+
+
+def direction_encoding64(d):
+    """[d, sin(2^k d), cos(2^k d)] (k = 0..3, embeddirs_fn's order) of fp64 directions [R, 3] -> [R, 27]."""
+    k = 2.0 ** torch.arange(4, dtype=F64, device=d.device)
+    arg = d[:, None, :] * k[None, :, None]
+    return torch.cat([d, torch.stack([torch.sin(arg), torch.cos(arg)], 2).reshape(d.shape[0], 24)], 1)
+
+
+def view_head_weights(net):
+    """fp16(w) of the head as the kernels hold it, fp32 biases; fp64 on DEV."""
+    g = lambda m: (h16(m.weight), m.bias.detach().to(F64))
+    wv, bv = g(net.views_linears[0])
+    wf, bf = g(net.feature_linear)
+    wa, ba = g(net.alpha_linear)
+    wr, br = g(net.rgb_linear)
+    return dict(wvf=wv[:, :256], wve=wv[:, 256:], bv=bv, wf=wf, bf=bf, wa=wa, ba=ba, wr=wr, br=br)
+
+
+def check_view_head(cs, o, rep, sub, H8):
+    """The view stash and the head's outputs on sub's tiles, each from the kernel's own operands:
+        Dir  = fp16 of the encoding of the fp32 direction, within 0.5 ulp + E_DIR_ENC; rows past P encode d = 0 (the
+               kernel keeps every stashed row finite); columns 27..31 exactly 0
+        F    = fp16(H8 Wf^T + bf)                                      c_mma(256) + 0.5 ulp
+        Hv   = relu(fp16(F WvF^T + Dir WvE^T + bv))                    c_mma(256 + 32): one N = 128 accumulator
+        raw  = [Hv Wr^T + br | H8 Wa^T + ba]                           c_mma(128) / c_mma(256), fp32
+    and the Hv mask bits equal the encoding of Hv > 0 byte for byte."""
+    R, P = sub.R, sub.n
+    img = lambda oc: sub.img(o["vstash"], SL.V_STASH_TILE, oc).to(F64)
+    Dir, F, Hv = img(SL.VS_DIR), img(SL.VS_F), img(SL.VS_HV)
+    w = view_head_weights(o["net"])
+    d = torch.zeros(R, 3, dtype=F64, device=DEV)
+    d[:P] = sub.ray_rows(cs.vd).to(F64)
+    assert torch.equal(Dir[:, :3], d.half().to(F64)), "Dir columns 0-2 are not fp16(direction)"
+    assert bool((Dir[:, 27:] == 0).all()), "Dir columns 27-31 are not 0"
+    enc = direction_encoding64(d)
+    rep.check("Dir (sin / cos)", Dir[:, 3:27], enc[:, 3:], torch.full_like(enc[:, 3:], E_DIR_ENC / U), 1.0, True)
+    v, a = mm(H8, w["wf"])
+    rep.check("F", F, v + w["bf"], a + w["bf"].abs(), c_mma(256), True)
+    v1, a1 = mm(F, w["wvf"])
+    v2, a2 = mm(Dir[:, :27], w["wve"])
+    rep.check("Hv", Hv, torch.relu(v1 + v2 + w["bv"]), a1 + a2 + w["bv"].abs(), c_mma(256 + 32), True)
+    rgb, rgb_a = mm(Hv[:P], w["wr"])
+    alpha, alpha_a = mm(H8[:P], w["wa"])
+    raw = sub.pt(o["raw"])
+    rep.check("raw rgb", raw[:, :3], rgb + w["br"], rgb_a + w["br"].abs(), c_mma(128))
+    rep.check("raw alpha", raw[:, 3:], alpha + w["ba"], alpha_a + w["ba"].abs(), c_mma(256))
+    enc_bits = SL.encode_relu_bits(sub.img(o["vstash"], SL.V_STASH_TILE, SL.VS_HV) > 0)
+    got = SL.tile_slices(o["hv_mask"], SL.HV_MASK_TILE, 0, SL.HV_MASK_TILE, sub.T, sub.idx)
+    assert torch.equal(got, enc_bits), f"Hv mask: {int((got != enc_bits).sum())} bytes differ from Hv > 0"
+
+
 def wgrad_images(cs, o, b, sub):
     """The decoded fp16 operands of WGRAD on the tiles of sub: E, H1..H8, d_raw, dY0..dY7, and with a bender its input,
     Hb1..Hb4 and dYb0..dYb4."""
     img = lambda oc: sub.img(o["stash"], SL.STASH_TILE, oc).to(F64)
     gimg = lambda oc: sub.img(b["gstash"], SL.GRAD_TILE, oc).to(F64)
     out = {"E": img(SL.ST_E), "H": [img(oc) for oc in SL.ST_H], "Draw": gimg(SL.GS_RAW), "dY": [gimg(oc) for oc in SL.GS_Y]}
+    if cs.views:
+        vimg = lambda oc: sub.img(o["vstash"], SL.V_STASH_TILE, oc).to(F64)
+        vgimg = lambda oc: sub.img(b["vgstash"], SL.V_GRAD_TILE, oc).to(F64)
+        out.update(Dir=vimg(SL.VS_DIR), F=vimg(SL.VS_F), Hv=vimg(SL.VS_HV), dYv=vgimg(SL.VG_YV), dF=vgimg(SL.VG_F))
     if cs.bender:
         out.update(Bin=img(SL.ST_BIN), Hb=[img(SL.ST_HB1), img(SL.ST_HB2), img(SL.ST_HB3), img(SL.ST_HB4)],
                    Yb=[gimg(oc) for oc in (SL.GS_YB0, SL.GS_YB1, SL.GS_YB2, SL.GS_YB3, SL.GS_YB4)])
@@ -486,8 +617,21 @@ def dgrad_reference(cs, o, b, rep, scale, tiles=None):
     assert torch.equal(Draw[:P, :4], exp_raw), "d_raw image is not fp16(clamp(d_raw[:, :4] * scale))"
     assert bool((Draw[:P, 4:] == 0).all()) and bool((Draw[P:] == 0).all()), "d_raw image: padding is not zero"
     m = [mbits(oc) for oc in SL.MK_H]
-    v, a = dmm(Draw[:, :cs.out_ch], W[8])
-    rep.check("dY7", dY[7], v * m[7], a * m[7], c_mma(16), True)
+    if cs.views:
+        # Rgb^T, ViewsF^T, then Feature^T and alpha's column into one accumulator, each from the kernel's own operands
+        w = view_head_weights(o["net"])
+        mv = SL.relu_bits(o["hv_mask"], 0, 128, sub.T, tile_bytes=SL.HV_MASK_TILE, tiles=sub.idx).to(F64)
+        dYv, dF = out["dYv"], out["dF"]
+        v, a = dmm(Draw[:, :3], w["wr"])
+        rep.check("dYv", dYv, v * mv, a * mv, c_mma(16), True)
+        v, a = dmm(dYv, w["wvf"])
+        rep.check("dF", dF, v, a, c_mma(128), True)
+        v1, a1 = dmm(dF, w["wf"])
+        v2, a2 = dmm(Draw[:, 3:4], w["wa"])
+        rep.check("dY7", dY[7], (v1 + v2) * m[7], (a1 + a2) * m[7], c_mma(256 + 16), True)
+    else:
+        v, a = dmm(Draw[:, :cs.out_ch], W[8])
+        rep.check("dY7", dY[7], v * m[7], a * m[7], c_mma(16), True)
     for l in (6, 5):
         v, a = dmm(dY[l + 1], W[l + 1])
         rep.check(f"dY{l}", dY[l], v * m[l], a * m[l], c_mma(256), True)
@@ -497,6 +641,8 @@ def dgrad_reference(cs, o, b, rep, scale, tiles=None):
     for l in (3, 2, 1, 0):
         v, a = dmm(dY[l + 1], W[l + 1])
         rep.check(f"dY{l}", dY[l], v * m[l], a * m[l], c_mma(256), True)
+    if cs.views:
+        return out            # no L5e^T / L0^T: the embedding gradient has no consumer without a bender
     dE0, dE0a = dmm(dY[0], W[0][:, :63])
     pad = lambda t: torch.cat([t, torch.zeros(R, 1, dtype=F64, device=DEV)], 1)
     dx5, ax5 = pe_backward(pad(dE5), pad(dE5a), E)
@@ -610,6 +756,16 @@ def wgrad_reference(cs, imgs):
         else:
             ref[f"w{l}"] = wsum(dY[l], H[l - 1])
         ref[f"b{l}"] = (dY[l].sum(0), dY[l].abs().sum(0))
+    if cs.views:
+        # the head block; job 0 (the trunk's head job) contributes alpha_linear only: d_raw column 3 (x) H8
+        bsum = lambda y: (y.sum(0), y.abs().sum(0))
+        Dir, F, Hv, dYv, dF = imgs["Dir"], imgs["F"], imgs["Hv"], imgs["dYv"], imgs["dF"]
+        ref["views_linears.0.weight"] = wsum(dYv, torch.cat([F, Dir[:, :27]], 1))
+        ref["views_linears.0.bias"] = bsum(dYv)
+        ref["feature_linear.weight"], ref["feature_linear.bias"] = wsum(dF, H[7]), bsum(dF)
+        ref["alpha_linear.weight"], ref["alpha_linear.bias"] = wsum(Draw[:, 3:4], H[7]), bsum(Draw[:, 3:4])
+        ref["rgb_linear.weight"], ref["rgb_linear.bias"] = wsum(Draw[:, :3], Hv), bsum(Draw[:, :3])
+        return ref, None
     v, a = wsum(Draw[:, :4], H[7])
     z = torch.zeros(cs.out_ch - 4, 256, dtype=F64, device=DEV)
     ref["w_out"] = (torch.cat([v, z]), torch.cat([a, z]))
@@ -625,10 +781,11 @@ def check_wgrad(cs, b, imgs, rep, scale, nerf_flat=None, bend_flat=None, base_ne
     and at relative L2 `rel_l2` per NeRF tensor."""
     ref, bref = wgrad_reference(cs, imgs) if refs is None else refs
     c = c_wgrad(imgs["sub"].count if refs is None else n_tiles)
-    shapes = SL.nerf_param_shapes(cs.out_ch, cs.tc)
+    shapes = SL.views_param_shapes() if cs.views else SL.nerf_param_shapes(cs.out_ch, cs.tc)
     got = SL.split_flat(b["nerf_grad"] if nerf_flat is None else nerf_flat, shapes)
     if b["nerf_head"] is not None:
-        got.update(SL.split_flat(b["nerf_head"], shapes[-2:]))
+        got.update(SL.split_flat(b["nerf_head"], SL.HEAD_SHAPES if cs.views else shapes[-2:]))
+    assert set(got) == set(ref), set(got) ^ set(ref)
     base = SL.split_flat(base_nerf, shapes) if base_nerf is not None else None
     for name, (v, a) in ref.items():
         g = got[name].to(F64) - (base[name].to(F64) if base is not None else 0.0)
@@ -787,14 +944,25 @@ def run_all(cs, tag, divergence=True):
 
 # ---- WGRAD's split plan (wgrad.cu, launch_wgrad), replicated ----
 _JOB_CHUNKS = [46, 48, 48, 48, 48, 48, 48, 48, 32, 32, 54, 42]
+# launch_wgrad_views: per position 0..13 of the jobs 0..9, 12 (feature_linear), 13 (views_linears.0, feature columns),
+# 14 (rgb_linear), 15 (views_linears.0, direction columns)
+_VIEW_JOB_CHUNKS = [46, 48, 48, 48, 48, 48, 48, 48, 32, 32, 48, 48, 24, 20]
+VIEW_HEAD_JOBS = (12, 13, 14, 15)
 WG_SCRATCH_FLOATS = 256 * 256 + 256   # one partial per (job, split, half): kWgScratchFloats
 
 
-def wgrad_halves(has_bender=True, compact=False):
-    """{job: CTAs per split}: the NeRF layer jobs 1..9 take two; the head (0) and bender jobs (10, 11) one.  The
-    divergence kernels' compact launch runs the bender jobs only."""
+def wgrad_halves(has_bender=True, compact=False, views=False):
+    """{job: CTAs per split}, in the launch's job order: the NeRF layer jobs 1..9 take two; the head (0) and bender jobs
+    (10, 11) one.  The divergence kernels' compact launch runs the bender jobs only.  views: launch_wgrad_views' jobs,
+    where feature_linear (12) takes two like a NeRF layer and the other head jobs one."""
+    if views:
+        return {j: 2 if 1 <= j <= 9 or j == 12 else 1 for j in (*range(10), *VIEW_HEAD_JOBS)}
     jobs = range(10, 12) if compact else range(12 if has_bender else 10)
     return {j: 2 if 1 <= j <= 9 else 1 for j in jobs}
+
+
+def _job_cost(j, views):
+    return _VIEW_JOB_CHUNKS[j if j < 10 else j - 2] if views else _JOB_CHUNKS[j]
 
 
 def wgrad_rel_l2(split_tiles):
@@ -806,8 +974,8 @@ def wgrad_rel_l2(split_tiles):
     return max(WGRAD_REL_L2, 2.5 * 2.0 ** -22 * split_tiles)
 
 
-def wgrad_plan(n_tiles, max_ctas, has_bender=True, compact=False):
-    halves = wgrad_halves(has_bender, compact)
+def wgrad_plan(n_tiles, max_ctas, has_bender=True, compact=False, views=False):
+    halves = wgrad_halves(has_bender, compact, views)
     splits = {j: 1 for j in halves}
     used, tiles = sum(halves.values()), max(n_tiles, 1)
     while True:
@@ -815,7 +983,7 @@ def wgrad_plan(n_tiles, max_ctas, has_bender=True, compact=False):
         for j in halves:
             if splits[j] >= tiles or used + halves[j] > max_ctas:
                 continue
-            load = _JOB_CHUNKS[j] * -(-tiles // splits[j])
+            load = _job_cost(j, views) * -(-tiles // splits[j])
             if load > best_load:
                 best, best_load = j, load
         if best < 0:

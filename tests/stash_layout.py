@@ -45,6 +45,18 @@ MK_HB4 = (MK_HB3[0] + MASK_B_BYTES, 64)
 MASK_TILE = MK_HB4[0] + MASK_B_BYTES
 MASK_IMAGES = [*MK_H, MK_HB1, MK_HB2, MK_HB3, MK_HB4]
 
+# view-dependent head (nrn_common.cuh kVs* / kVg* / kMkHv): view stash [Dir 27 + 5 zero | F | Hv], view gradient stash
+# [dYv | dF] and the Hv mask, per tile
+VS_DIR, VS_F, VS_HV = (0, 4), (4 * CHUNK, 32), (36 * CHUNK, 16)
+V_STASH_TILE = VS_HV[0] + 16 * CHUNK
+VG_YV, VG_F = (0, 16), (16 * CHUNK, 32)
+V_GRAD_TILE = VG_F[0] + 32 * CHUNK
+HV_MASK_TILE = TILE_M * 16                                      # 128 columns, one 16-byte row
+TRUNK_FLOATS = 493056                                           # W0 b0 .. W7 b7 of nrn_nerf_views_grad_floats
+HEAD_SHAPES = [("views_linears.0.weight", (128, 283)), ("views_linears.0.bias", (128,)), ("feature_linear.weight", (256, 256)),
+               ("feature_linear.bias", (256,)), ("alpha_linear.weight", (1, 256)), ("alpha_linear.bias", (1,)),
+               ("rgb_linear.weight", (3, 128)), ("rgb_linear.bias", (3,))]
+
 # divergence regulariser: tangent stash [e | t1 s1 | t2 s2 | t3 | t4] and adjoint stash, per tile
 T_E, T_1, T_2, T_3, T_4 = (0, 6), (6 * CHUNK, 12), (18 * CHUNK, 12), (30 * CHUNK, 8), (38 * CHUNK, 8)
 TAN_TILE = 46 * CHUNK
@@ -128,6 +140,11 @@ def nerf_param_shapes(out_ch, tc=False):
     for l in range(1, 8):
         shapes += [(f"w{l}", (256, in_ch + 256 if l == 5 else 256)), (f"b{l}", (256,))]
     return shapes + [("w_out", (out_ch, 256)), ("b_out", (out_ch,))]
+
+
+def views_param_shapes():
+    """nrn_nerf_views_grad_floats: the trunk W0 b0 .. W7 b7 (no output layer), then the head block in module order."""
+    return nerf_param_shapes(4)[:-2] + HEAD_SHAPES
 
 
 def bender_param_shapes():

@@ -252,6 +252,45 @@ def test_caseK_view_dependent_head_and_finite_difference_viewdirs():
     close(gr[torch.from_numpy(g[nm + ".idx"])], g[nm + ".val"], 1e-7, 2e-3, name=nm)
 
 
+VIEW_HEAD_KEYS = (("views_linears.0", "views"), ("feature_linear", "feature"), ("alpha_linear", "alpha"), ("rgb_linear", "rgb"))
+
+
+def view_model_tensors(p, v):
+    """{reference parameter name: oracle tensor} of one NeRF(use_viewdirs=True) (make_nerf_params / make_view_params)."""
+    out = {}
+    for i in range(8):
+        out[f"pts_linears.{i}.weight"], out[f"pts_linears.{i}.bias"] = p["pts_w"][i], p["pts_b"][i]
+    for mod, key in VIEW_HEAD_KEYS:
+        out[f"{mod}.weight"], out[f"{mod}.bias"] = v[key + "_w"], v[key + "_b"]
+    return out
+
+
+def test_caseM_training_wrapper_with_the_view_dependent_head():
+    """Training the view-dependent head without a bender: the oracle's training_wrapper_loss (vpar_c / vpar_f) against
+    the executed training_wrapper_class, per-ray loss and every coarse and fine parameter's gradient; the latents get
+    no gradient in the reference."""
+    g = load("caseM_viewdirs_train.npz")
+    seed, n = int(g["seed"]), int(g["n"])
+    cp, fp, _ = models(seed, with_bender=False)
+    vc, vf = O.make_view_params(seed + 10, 30.0), O.make_view_params(seed + 11, 30.0)
+    cp, fp, vc, vf = (O.clone_params(q, True) for q in (cp, fp, vc, vf))
+    r = O.make_rays(seed, n)
+    rnd = O.make_randomness(seed, n, 64, 64)
+    table = torch.from_numpy(g["latent_table"]).clone().requires_grad_(True)
+    loss, _ = O.training_wrapper_loss(cp, fp, None, r, table, g["i2t"], torch.from_numpy(g["pix"]), rnd, None,
+                                      int(g["global_step"]), int(g["N_iters"]), 0.0, 0.0, 0.0, vpar_c=vc, vpar_f=vf)
+    close(loss, g["loss"], 5e-6, name="loss")
+    loss.mean().backward()
+    assert not bool(g["latents_got_grad"]) and (table.grad is None or not bool(table.grad.any()))
+    tensors = {f"coarse.{k}": t for k, t in view_model_tensors(cp, vc).items()}
+    tensors.update({f"fine.{k}": t for k, t in view_model_tensors(fp, vf).items()})
+    assert set(str(k) for k in g["grad_names"]) == set(tensors)
+    for nm, t in tensors.items():
+        gr = t.grad.reshape(-1)
+        close(gr[torch.from_numpy(g[nm + ".idx"])], g[nm + ".val"], 1e-7, 2e-3, name=nm)
+        assert abs(float(gr.norm()) - float(g[nm + ".norm"][0])) <= 2e-3 * float(g[nm + ".norm"][0]) + 1e-9, nm
+
+
 def test_flop_ledger():
     cp = O.make_nerf_params(0)
     bp = O.make_bender_params(0)

@@ -66,13 +66,14 @@ LIMITS = (2 ** 31, 2 ** 32, 2 ** 33, 2 ** 34)
 
 
 def tile_bytes(lib, n, s):
-    """Per-tile bytes of every buffer a pass writes, from the library's sizes: the field stashes and masks hold an even
-    tile count, the divergence stashes the point tiles."""
+    """Per-tile bytes of every buffer a pass writes, from the library's sizes: the field stashes and masks (the view
+    head's included) hold an even tile count, the divergence stashes the point tiles."""
     T = -(-n * s // SL.TILE_M)
     even = T + (T & 1)
     return {"stash": lib.nrn_stash_bytes(n, s) // even, "grad stash": lib.nrn_grad_stash_bytes(n, s) // even,
             "masks": lib.nrn_relu_mask_bytes(n, s) // even, "tangent": lib.nrn_div_stash_bytes(n, s) // T,
-            "adjoint": lib.nrn_div_grad_stash_bytes(n, s) // T}
+            "adjoint": lib.nrn_div_grad_stash_bytes(n, s) // T, "views stash": lib.nrn_views_stash_bytes(n, s) // even,
+            "views grad stash": lib.nrn_views_grad_stash_bytes(n, s) // even, "hv mask": lib.nrn_hv_mask_bytes(n, s) // even}
 
 
 def sample_tiles(cs, buffers):

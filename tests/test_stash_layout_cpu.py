@@ -43,6 +43,26 @@ def test_image_offsets_tile_the_library_buffers():
         assert lib.nrn_div_grad_stash_bytes(n, s) == tiles * SL.ADJ_TILE
 
 
+def test_view_stash_images_tile_the_library_buffers():
+    """The view stash [Dir | F | Hv], the view gradient stash [dYv | dF] and the Hv mask, against the library's sizes (an
+    even tile count, as the trunk's stashes), and the views gradient layout against nrn_nerf_views_grad_floats."""
+    from nonrigid_nerf_b200 import _lib
+    lib = _lib.load()
+    _contiguous([SL.VS_DIR, SL.VS_F, SL.VS_HV], SL.V_STASH_TILE, SL.CHUNK)
+    _contiguous([SL.VG_YV, SL.VG_F], SL.V_GRAD_TILE, SL.CHUNK)
+    assert SL.VS_DIR[1] * 8 == 32 and SL.VS_F[1] * 8 == 256 and SL.VS_HV[1] * 8 == 128
+    assert SL.VG_YV[1] * 8 == 128 and SL.VG_F[1] * 8 == 256 and SL.HV_MASK_TILE == SL.TILE_M * 16
+    for n, s in ((1, 7), (2, 64), (3, 100), (11, 100), (1023, 64), (1024, 128), (22528, 128)):
+        tiles = -(-n * s // SL.TILE_M)
+        even = tiles + (tiles & 1)
+        assert lib.nrn_views_stash_bytes(n, s) == even * SL.V_STASH_TILE
+        assert lib.nrn_views_grad_stash_bytes(n, s) == even * SL.V_GRAD_TILE
+        assert lib.nrn_hv_mask_bytes(n, s) == even * SL.HV_MASK_TILE
+    shapes = SL.views_param_shapes()
+    assert sum(math.prod(s) for _, s in shapes[:16]) == SL.TRUNK_FLOATS == lib.nrn_nerf_grad_floats(4) - 4 * 257
+    assert sum(math.prod(s) for _, s in shapes) == lib.nrn_nerf_views_grad_floats() == 595844
+
+
 @pytest.mark.parametrize("out_ch", [4, 5])
 def test_gradient_parameter_maps_match_the_library(out_ch):
     from nonrigid_nerf_b200 import _lib
@@ -164,3 +184,28 @@ def test_replicated_wgrad_plan_fits_the_scratch_and_covers_every_tile_once(max_c
                 ranges = SR.split_ranges(T, n_split)
                 assert ranges[0][0] == 0 and ranges[-1][1] == T and all(a[1] == b[0] for a, b in zip(ranges, ranges[1:]))
                 assert all(e > s for s, e in ranges) and len(ranges) <= n_split
+
+
+@pytest.mark.parametrize("max_ctas", [132, 114, 66, 16])
+def test_replicated_views_wgrad_plan_fits_the_scratch_and_covers_every_tile_once(max_ctas):
+    """The same for launch_wgrad_views: its 14 jobs (the trunk's 0-9, then feature_linear 12, views_linears.0's feature
+    columns 13, rgb_linear 14 and views_linears.0's direction columns 15) with the kViewJobChunks costs; feature_linear
+    takes two CTAs per split like a NeRF layer."""
+    from nonrigid_nerf_b200 import _lib
+    from tests import stage_reference as SR
+    lib = _lib.load()
+    parts = lib.nrn_wgrad_scratch_bytes() // (4 * SR.WG_SCRATCH_FLOATS)
+    src = open(os.path.join(os.path.dirname(_lib.__file__), "csrc", "wgrad.cu")).read()
+    table = re.search(r"kViewJobChunks\[14\]\s*=\s*\{([^}]*)\}", src).group(1)
+    assert [sum(int(t) for t in x.split("+")) for x in table.split(",")] == SR._VIEW_JOB_CHUNKS
+    halves = SR.wgrad_halves(views=True)
+    assert list(halves) == [*range(10), 12, 13, 14, 15]
+    assert [j for j, h in halves.items() if h == 2] == [*range(1, 10), 12]
+    for T in (1, 9, 1024, 4096, 8192, 22528, 40960):
+        plan = SR.wgrad_plan(T, max_ctas, views=True)
+        used = sum(plan[j] * halves[j] for j in plan)
+        assert used <= max(max_ctas, sum(halves.values())) and used <= parts, (T, plan)
+        for j, n_split in plan.items():
+            ranges = SR.split_ranges(T, n_split)
+            assert ranges[0][0] == 0 and ranges[-1][1] == T and all(a[1] == b[0] for a, b in zip(ranges, ranges[1:]))
+            assert all(e > s for s, e in ranges) and len(ranges) <= n_split

@@ -9,7 +9,13 @@ Which wrong implementation each check catches:
 - per-ray loss and per-tensor gradients against the oracle: the Hv mask not applied in DGRAD, the alpha term dropped from
   dY7 (alpha_linear's and the trunk's gradients), ViewsF^T reading the direction columns (feature_linear's and the trunk's),
   a wrong block order of the head in the flat layout (every head tensor), rgb_linear's gradient from the wrong A columns;
-- two runs bit-identical, arena == fresh buffers: a non-deterministic reduce or a wrong in-place destination."""
+- two runs bit-identical, arena == fresh buffers: a non-deterministic reduce or a wrong in-place destination;
+- a separate head destination (trunk and head apart in the arena), a second backward without zero_grad (g1 + g2) and one
+  over a retained graph (2 g): the head block written behind the trunk instead of to nerf_grad_head, accumulation that
+  overwrites, stashes freed after the first backward;
+- a frozen trunk: the in-place path taken for a partly trainable model (the frozen slots would be written);
+- n_rays = 0: destinations not zeroed, an accumulating arena cleared, a kernel launched on an empty batch;
+- golden case M: the whole wrapper against the executed reference."""
 import pytest
 import torch
 
@@ -176,3 +182,190 @@ def test_bender_training_still_raises_before_any_launch():
         _lib.timing_enable(False)
     counts = {k: c for k, (_, c) in _lib.timing_read(kinds).items()}
     assert sum(counts.values()) == 0, counts
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# gradient destinations and edges
+# ----------------------------------------------------------------------------------------------------------------------
+def _render_loss(coarse, fine, r):
+    from nonrigid_nerf_b200 import train as T
+    kw = dict(network_query_fn=None, perturb=0.0, N_importance=64, network_fine=fine, N_samples=64, network_fn=coarse,
+              white_bkgd=False, raw_noise_std=0.0, ndc=False, lindisp=False)
+    rgb, _, _, ex = T.render(r["rays_o"].to(DEV), r["rays_d"].to(DEV), chunk=1 << 20, near=r["near"], far=r["far"], use_viewdirs=True,
+                             additional_pixel_information={"ray_bending_latents": r["latents"].to(DEV)}, retraw=True, **kw)
+    tgt = r["target"].to(DEV)
+    return (((rgb - tgt) ** 2).mean(-1) + ((ex["rgb0"] - tgt) ** 2).mean(-1)).sum()
+
+
+def _grads_equal(models, expect, what):
+    for m, pre in zip(models, ("c.", "f.")):
+        for k, p in m.named_parameters():
+            if pre + k in expect:
+                assert torch.equal(p.grad, expect[pre + k]), (what, pre + k)
+
+
+@pytest.mark.parametrize("layout", ["adjacent", "separate"])
+def test_arena_destinations_and_accumulation_equal_fresh_buffers(layout):
+    """optim.Adam's arena with each model's trunk and head block back to back ("adjacent": one flat destination) or each
+    contiguous but apart ("separate": [*heads, *latents, *trunks], nerf_grad_head set): the in-place backward equals the
+    fresh-buffer path bit for bit, and a second backward without zero_grad gives fp32(g1 + g2) bit for bit."""
+    from nonrigid_nerf_b200 import _lib, optim
+    from nonrigid_nerf_b200.autograd import _arena_destination, _views_flat_params
+    seed = 6500
+    coarse, fine, _, _ = build_view_models(O, seed, DEV, with_bender=False)
+    r1, r2 = O.make_rays(seed, 512), O.make_rays(seed + 1, 512)
+    _, g1 = _train_grads(coarse, fine, r1)
+    _, g2 = _train_grads(coarse, fine, r2)
+    split = {id(m): _views_flat_params(m) for m in (coarse, fine)}
+    lat = [torch.zeros(32, device=DEV, requires_grad=True) for _ in range(3)]
+    if layout == "adjacent":
+        params = [p for m in (coarse, fine) for part in split[id(m)] for p in part] + lat
+    else:
+        params = [p for m in (coarse, fine) for p in split[id(m)][1]] + lat + [p for m in (coarse, fine) for p in split[id(m)][0]]
+    opt = optim.Adam(params, lr=1e-3)
+    opt.zero_grad()
+    _render_loss(coarse, fine, r1).backward()
+    _lib.device_error_check()
+    for m in (coarse, fine):
+        trunk, head = split[id(m)]
+        t_dst, h_dst = _arena_destination(trunk), _arena_destination(head)
+        assert t_dst is not None and h_dst is not None
+        adjacent = h_dst == t_dst + 4 * SL.TRUNK_FLOATS
+        assert adjacent == (layout == "adjacent"), (layout, t_dst, h_dst)
+    _grads_equal((coarse, fine), g1, "arena from zero")
+    _render_loss(coarse, fine, r2).backward()
+    _lib.device_error_check()
+    _grads_equal((coarse, fine), {k: g1[k] + g2[k] for k in g1}, "second backward without zero_grad")
+
+
+def test_backward_twice_over_a_retained_graph():
+    """The stashes live as long as the autograd node: a second backward reads them again, so .grad = g + g = 2 g."""
+    from nonrigid_nerf_b200 import _lib
+    seed = 6600
+    coarse, fine, _, _ = build_view_models(O, seed, DEV, with_bender=False)
+    r = O.make_rays(seed, 256)
+    _, g1 = _train_grads(coarse, fine, r)
+    for m in (coarse, fine):
+        m.zero_grad(set_to_none=True)
+    loss = _render_loss(coarse, fine, r)
+    loss.backward(retain_graph=True)
+    loss.backward()
+    _lib.device_error_check()
+    _grads_equal((coarse, fine), {k: g1[k] + g1[k] for k in g1}, "retain_graph")
+
+
+def test_frozen_trunk_trains_the_head_through_fresh_buffers():
+    """Trunk frozen, head trained: the head's gradients equal the fully trainable run's bit for bit and the trunk's
+    .grad stays None; with optim.Adam's arena seated, the partly frozen model takes the fresh-buffer path, so the frozen
+    trunk's arena slots (preset to NaN) are never written."""
+    from nonrigid_nerf_b200 import _lib, optim
+    from nonrigid_nerf_b200.autograd import _views_flat_params
+    seed = 6700
+    coarse, fine, _, _ = build_view_models(O, seed, DEV, with_bender=False)
+    r = O.make_rays(seed, 256)
+    _, g_all = _train_grads(coarse, fine, r)
+    trunks = [p for m in (coarse, fine) for p in _views_flat_params(m)[0]]
+    for p in trunks:
+        p.requires_grad_(False)
+    _, g = _train_grads(coarse, fine, r)
+    _lib.device_error_check()
+    assert all(p.grad is None for p in trunks)
+    head_keys = {k for k in g_all if not k[2:].startswith("pts_linears")}
+    assert set(g) == head_keys, set(g) ^ head_keys
+    for k in head_keys:
+        assert torch.equal(g[k], g_all[k]), k
+    params = [p for m in (coarse, fine) for part in _views_flat_params(m) for p in part]
+    opt = optim.Adam(params, lr=1e-3)
+    opt.zero_grad()
+    for p in trunks:
+        p.grad.fill_(float("nan"))
+    _render_loss(coarse, fine, r).backward()
+    _lib.device_error_check()
+    assert all(bool(torch.isnan(p.grad).all()) for p in trunks), "a frozen trunk's arena slot was written"
+    _grads_equal((coarse, fine), {k: g_all[k] for k in head_keys}, "frozen trunk, arena")
+
+
+@pytest.mark.parametrize("dest", ["flat", "separate", "accumulate"])
+def test_empty_batch_zeroes_the_destinations_and_launches_nothing(dest):
+    """nrn_field_backward_views at n_rays = 0 (an empty shard): the flat buffer, or both destinations, are zeroed when not
+    accumulating; an accumulating arena is left as it was; no kernel runs."""
+    import ctypes as C
+    from nonrigid_nerf_b200 import _lib
+    from tests.parity import poison_f32
+    lib = _lib.load()
+    n_all = lib.nrn_nerf_views_grad_floats()
+    n_head = n_all - SL.TRUNK_FLOATS
+    g = torch.Generator(device=DEV).manual_seed(11)
+    if dest == "accumulate":
+        trunk, head = torch.randn(n_all, generator=g, device=DEV), torch.randn(n_head, generator=g, device=DEV)
+    else:
+        trunk, head = poison_f32(n_all), poison_f32(n_head)
+    before = (trunk.clone(), head.clone())
+    a, v = _lib.NrnFieldBwdArgs(), _lib.NrnViewBwdArgs()
+    a.n_rays, a.n_samples, a.out_ch = 0, 64, 4
+    a.nerf_grad = trunk.data_ptr()
+    if dest != "flat":
+        a.nerf_grad_head = head.data_ptr()
+    a.accumulate_nerf = 1 if dest == "accumulate" else 0
+    a.stream = torch.cuda.current_stream().cuda_stream
+    _lib.timing_enable(True)
+    try:
+        _lib.check(lib.nrn_field_backward_views(C.byref(a), C.byref(v)), "field_backward_views")
+        torch.cuda.synchronize()
+    finally:
+        _lib.timing_enable(False)
+    _lib.device_error_check()
+    counts = {k: c for k, (_, c) in _lib.timing_read(_lib.VIEW_TRAIN_KERNEL_KINDS).items()}
+    assert sum(counts.values()) == 0, counts
+    if dest == "accumulate":
+        assert torch.equal(trunk, before[0]) and torch.equal(head, before[1])
+    elif dest == "separate":
+        assert bool((trunk[:SL.TRUNK_FLOATS] == 0).all()) and bool((head == 0).all())
+        assert bool(torch.isnan(trunk[SL.TRUNK_FLOATS:]).all()), "the head's slot of nerf_grad was written despite nerf_grad_head"
+    else:
+        assert bool((trunk == 0).all()) and bool(torch.isnan(head).all())
+
+
+def test_training_wrapper_matches_the_executed_reference_caseM():
+    """training_wrapper_class with the view-dependent head and no bender (perturb 1, noise 1, the reference's random
+    draws injected) against golden case M from the executed reference: per-ray loss and every coarse and fine
+    parameter's sampled gradient and norm within DESIGN section 2's bounds; the latents get no gradient."""
+    import os
+    import types
+    import numpy as np
+    from nonrigid_nerf_b200 import _lib, parallel
+    g = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "caseM_viewdirs_train.npz"))
+    seed, n = int(g["seed"]), int(g["n"])
+    coarse, fine, _, _ = build_view_models(O, seed, DEV, with_bender=False)
+    r = O.make_rays(seed, n)
+    rnd = {k: v.to(DEV) for k, v in O.make_randomness(seed, n, 64, 64).items()}
+    latents = [torch.from_numpy(row.copy()).to(DEV).requires_grad_(True) for row in g["latent_table"]]
+    targs = types.SimpleNamespace(chunk=32768, N_samples=64, N_importance=64, N_iters=int(g["N_iters"]), offsets_loss_weight=0.0,
+                                  divergence_loss_weight=0.0, rigidity_loss_weight=0.0, ray_bending_latent_size=32)
+    kw = {"network_query_fn": None, "perturb": 1.0, "N_importance": 64, "network_fine": fine, "N_samples": 64,
+          "network_fn": coarse, "ray_bender": None, "use_viewdirs": True, "white_bkgd": False, "raw_noise_std": 1.0,
+          "ndc": False, "lindisp": False, "near": r["near"], "far": r["far"], "randomness": rnd}
+    wrapper = parallel.training_wrapper_class(coarse, latents, fine_model=fine)
+    loss = wrapper(targs, r["rays_o"].to(DEV), r["rays_d"].to(DEV), 100, kw, r["target"].to(DEV), int(g["global_step"]), 0,
+                   {"imageid_to_timestepid": [int(v) for v in g["i2t"]]}, torch.from_numpy(g["pix"]).to(DEV))
+    loss.mean().backward()
+    _lib.device_error_check()
+    ref = torch.from_numpy(g["loss"])
+    d = float((loss.detach().cpu() - ref).abs().max())
+    rel = float((loss.detach().cpu().double() - ref.double()).norm() / ref.double().norm())
+    print(f"case M: per-ray loss vs executed reference: L-inf {d:.3e}, rel L2 {rel:.3e}")
+    assert d <= 2e-3 and rel <= 2e-3, (d, rel)
+    assert not bool(g["latents_got_grad"]) and all(l.grad is None or not bool(l.grad.any()) for l in latents)
+    named = dict([("coarse." + k, p) for k, p in coarse.named_parameters() if p.grad is not None] +
+                 [("fine." + k, p) for k, p in fine.named_parameters() if p.grad is not None])
+    assert set(named) == set(str(k) for k in g["grad_names"]), set(named) ^ set(str(k) for k in g["grad_names"])
+    worst = {}
+    for nm, p in named.items():
+        idx = torch.from_numpy(g[nm + ".idx"])
+        ours = p.grad.reshape(-1).cpu()[idx].double().numpy()
+        exp = g[nm + ".val"].astype(np.float64)
+        err = float(np.linalg.norm(ours - exp) / (np.linalg.norm(exp) + 1e-30))
+        nrm = abs(float(p.grad.norm()) - float(g[nm + ".norm"][0])) / (float(g[nm + ".norm"][0]) + 1e-30)
+        worst[nm] = max(err, nrm)
+        assert bool(torch.isfinite(p.grad).all()) and err <= 8e-2 and nrm <= 8e-2, (nm, err, nrm)
+    print(f"case M: worst sampled-gradient / norm relative error {max(worst.values()):.3e} ({max(worst, key=worst.get)})")
