@@ -292,6 +292,22 @@ typedef struct NrnDivArgs {
 int nrn_divergence_forward(const NrnDivArgs* args);
 int nrn_divergence_backward(const NrnDivArgs* args);
 
+/* ---- deterministic mode (what torch.use_deterministic_algorithms(True) selects): the per-ray sums that the entry points
+ * above form with fp32 atomics -- the latent gradient of nrn_field_backward with a bender, the loss of
+ * nrn_divergence_forward -- run in a fixed order instead, so that a training step is bit-reproducible on one GPU model.
+ * The kernels write per-point rows to a caller-owned workspace, then one small kernel sums each ray's rows in increasing
+ * point order: points form 32-aligned blocks [32k, 32k + 32); a block whose points all exist (32k + 31 < P) and lie in one
+ * ray holds its in-warp sum in the row of point 32k and is skipped as a whole, every other point holds its own row.
+ * Only the rows that order reaches are written, so the workspace needs no initialisation. ------------------------------ */
+size_t nrn_latent_rows_bytes(int n_rays, int n_samples);     /* [n_rays * n_samples][32] fp32 */
+size_t nrn_div_loss_rows_bytes(int n_rays, int n_samples);   /* [n_rays * n_samples] fp32 */
+/* nrn_field_backward with a bender (bender_packed and d_latents given); latent_rows: nrn_latent_rows_bytes(), 16-byte
+ * aligned.  d_latents is overwritten with the fixed-order sums; every other output is as nrn_field_backward's.  An
+ * empty batch (n_rays = 0) launches no kernel and, like nrn_field_backward, zeroes the gradients it does not accumulate. */
+int nrn_field_backward_det(const NrnFieldBwdArgs* args, float* latent_rows);
+/* nrn_divergence_forward with loss written in a fixed order; loss_rows: nrn_div_loss_rows_bytes() */
+int nrn_divergence_forward_det(const NrnDivArgs* args, float* loss_rows);
+
 /* ---- per-ray training loss of training_wrapper_class.forward (train.py:208-242): image terms (fine +
  * coarse) and the offsets / rigidity regulariser on the coarse samples, with the gradients per unit
  * upstream gradient written in the same pass (the loss is linear in dL/dloss[ray]). ----------------- */
@@ -389,7 +405,8 @@ int nrn_peer_gather_rows(const NrnPeerCtx* ctx, const float* local, int n_per_ra
  * 4 composite backward, 5 divergence regulariser, 6 time-conditioned ray bias (nrn_tc_latent_bias), 7 time-conditioned
  * latent gradients (per-ray sums, d z, latent columns of dW0 / dW5), 8 bend pass of the view-dependent head, 9 its
  * view-head field kernel (nrn_field_forward_views), 10 its training forward (nrn_field_forward_views_train), 11 its DGRAD
- * and 12 its WGRAD (+reduce) (nrn_field_backward_views).  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * and 12 its WGRAD (+reduce) (nrn_field_backward_views), 13 the fixed-order latent reduction (nrn_field_backward_det) and
+ * 14 the fixed-order divergence loss reduction (nrn_divergence_forward_det).  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

@@ -191,6 +191,11 @@ class _FieldTrainFn(torch.autograd.Function):
             t.d_latents, t.workspace = d_lat.data_ptr(), workspace.data_ptr()
             with torch.cuda.device(dev):
                 _lib.check(lib.nrn_field_backward_tc(C.byref(a), C.byref(t)), "field_backward_tc")
+        elif bender is not None and torch.are_deterministic_algorithms_enabled():
+            # the per-ray latent gradient in a fixed order (per-point rows, then one reduction) instead of fp32 atomics
+            rows = torch.empty(lib.nrn_latent_rows_bytes(n, s) // 4, dtype=torch.float32, device=dev)
+            with torch.cuda.device(dev):
+                _lib.check(lib.nrn_field_backward_det(C.byref(a), rows.data_ptr()), "field_backward_det")
         else:
             with torch.cuda.device(dev):
                 _lib.check(lib.nrn_field_backward(C.byref(a)), "field_backward")
@@ -227,7 +232,9 @@ def _bender_arena(bender):
 class _LatentGatherFn(torch.autograd.Function):
     """latents[timestep[i]] for every ray i (train.py:173-189: stack the per-frame latents, index by the ray's time step).
     The per-frame latents are views of the optimizer's flat buffer, so the table is read in place; the backward adds the
-    per-ray gradients [N, Z] into the latents' .grad arena with one index_add_ (fallback: per-latent gradient views)."""
+    per-ray gradients [N, Z] into the latents' .grad arena with one index_add_ (fallback: per-latent gradient views).
+    Under torch.use_deterministic_algorithms(True) PyTorch's CUDA index_add_ sums in a fixed order by itself (and can be
+    captured in a CUDA graph), so deterministic mode needs nothing of its own here."""
 
     @staticmethod
     def forward(ctx, timestep, *latents):
@@ -320,8 +327,13 @@ class _DivergenceFn(torch.autograd.Function):
         a.d, a.alpha, a.beta, a.tau_c = (scal[i].data_ptr() for i in range(4))
         a.loss = loss.data_ptr()
         a.stream = torch.cuda.current_stream().cuda_stream
-        with torch.cuda.device(dev):
-            _lib.check(lib.nrn_divergence_forward(C.byref(a)), "divergence_forward")
+        if torch.are_deterministic_algorithms_enabled():   # the per-ray loss in a fixed order instead of fp32 atomics
+            rows = torch.empty(lib.nrn_div_loss_rows_bytes(n, s) // 4, dtype=torch.float32, device=dev)
+            with torch.cuda.device(dev):
+                _lib.check(lib.nrn_divergence_forward_det(C.byref(a), rows.data_ptr()), "divergence_forward_det")
+        else:
+            with torch.cuda.device(dev):
+                _lib.check(lib.nrn_divergence_forward(C.byref(a)), "divergence_forward")
         ctx.keep = (un, rg, w, e, relu_mask, bender_pack, tan, scal, bender)
         ctx.bend_p = bend_p
         ctx.w_is_alpha = bool(w_is_alpha)

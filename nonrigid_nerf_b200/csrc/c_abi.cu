@@ -13,10 +13,12 @@
 #include "loss.cuh"
 #include "adam.cuh"
 #include "peer.cuh"
+#include "det_reduce.cuh"
 
 namespace nrn {
 cudaError_t launch_field_fwd(const FieldFwdParams& p, bool has_bender, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_bwd(const FieldBwdParams& p, bool has_bender, int num_sms, cudaStream_t stream);
+cudaError_t launch_field_bwd_det(const FieldBwdParams& p, float* latent_rows, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_fwd_tc(const FieldFwdParams& p, int num_sms, cudaStream_t stream);
 cudaError_t launch_tc_latent_bias(const float* lat, long long lat_stride, int n_rays, const float* w0, const float* b0, const float* w5,
                                   const float* b5, float* rb, cudaStream_t stream);
@@ -544,8 +546,9 @@ int nrn_bender_grad_floats(void) { return nrn::bparam::total(); }
 int nrn_nerf_tc_grad_floats(int out_ch) { return nrn::nerf_tc_grad_floats(out_ch); }
 size_t nrn_tc_workspace_bytes(int n_rays) { return n_rays < 0 ? 0 : (static_cast<size_t>(n_rays) * 2 * 256 + 2 * 256 * nrn::kLatent) * sizeof(float); }
 
-// nrn_field_backward, or with t (time-conditioned baseline, no bender) nrn_field_backward_tc
-static int field_backward(const NrnFieldBwdArgs* a, const NrnTcBwdArgs* t, const char* who) {
+// nrn_field_backward, or with t (time-conditioned baseline, no bender) nrn_field_backward_tc, or with latent_rows
+// (deterministic mode, bender) nrn_field_backward_det
+static int field_backward(const NrnFieldBwdArgs* a, const NrnTcBwdArgs* t, const char* who, float* latent_rows = nullptr) {
   if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
   if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "%s: bad sizes", who);
   if (a->out_ch < 4 || a->out_ch > 5) return fail(NRN_E_INVALID, "%s: out_ch=%d unsupported", who, a->out_ch);
@@ -562,7 +565,7 @@ static int field_backward(const NrnFieldBwdArgs* a, const NrnTcBwdArgs* t, const
   const int nerf_n = t ? nrn_nerf_tc_grad_floats(a->out_ch) : nrn_nerf_grad_floats(a->out_ch);
   const int bend_n = bend ? nrn_bender_grad_floats() : 0;
   cudaError_t e;
-  if (bend) {
+  if (bend && !latent_rows) {   // deterministic mode overwrites d_latents with the fixed-order sums
     e = cudaMemsetAsync(a->d_latents, 0, sizeof(float) * static_cast<size_t>(a->n_rays) * nrn::kLatent, st);
     if (e != cudaSuccess) return cuda_fail(e, "memset d_latents");
   }
@@ -598,8 +601,15 @@ static int field_backward(const NrnFieldBwdArgs* a, const NrnTcBwdArgs* t, const
   if (e == cudaSuccess && bend && p.d_unmasked_up) e = nrn::launch_absmax(p.d_unmasked_up, p.P * 3, amax, st, true);
   if (e == cudaSuccess && bend && p.d_rigid_up) e = nrn::launch_absmax(p.d_rigid_up, p.P, amax, st, true);
   if (e != cudaSuccess) return cuda_fail(e, "absmax_kernel");
-  { ScopedTimer tm(1, st); e = nrn::launch_field_bwd(p, bend, ds->num_sms, st); }
-  if (e != cudaSuccess) return cuda_fail(e, "field_bwd_kernel");
+  if (latent_rows) {
+    { ScopedTimer tm(1, st); e = nrn::launch_field_bwd_det(p, latent_rows, ds->num_sms, st); }
+    if (e != cudaSuccess) return cuda_fail(e, "field_bwd_det_kernel");
+    { ScopedTimer tm(13, st); e = nrn::launch_latent_reduce(latent_rows, a->d_latents, a->n_rays, a->n_samples, st); }
+    if (e != cudaSuccess) return cuda_fail(e, "latent_reduce_kernel");
+  } else {
+    { ScopedTimer tm(1, st); e = nrn::launch_field_bwd(p, bend, ds->num_sms, st); }
+    if (e != cudaSuccess) return cuda_fail(e, "field_bwd_kernel");
+  }
   float* dw_lat = nullptr;
   if (t) {   // per-ray sums of dY0 / dY5 -> d z and the latent columns of dW0 / dW5 (before WGRAD's reduction reads them)
     nrn::TcBwdParams q{};
@@ -617,6 +627,27 @@ static int field_backward(const NrnFieldBwdArgs* a, const NrnTcBwdArgs* t, const
 }
 
 int nrn_field_backward(const NrnFieldBwdArgs* a) { return field_backward(a, nullptr, "nrn_field_backward"); }
+
+size_t nrn_latent_rows_bytes(int n_rays, int n_samples) {
+  return n_rays < 0 || n_samples < 1 ? 0 : static_cast<size_t>(n_rays) * n_samples * nrn::kLatent * sizeof(float);
+}
+size_t nrn_div_loss_rows_bytes(int n_rays, int n_samples) {
+  return n_rays < 0 || n_samples < 1 ? 0 : static_cast<size_t>(n_rays) * n_samples * sizeof(float);
+}
+
+int nrn_field_backward_det(const NrnFieldBwdArgs* a, float* latent_rows) {
+  const char* who = "nrn_field_backward_det";
+  if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
+  if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "%s: bad sizes", who);
+  if (!a->bender_packed || !a->d_latents)
+    return fail(NRN_E_INVALID, "%s: needs a bender (bender_packed) and d_latents: only the bender's latent gradient has a fixed-order variant", who);
+  if (a->n_rays == 0) return field_backward(a, nullptr, who);   // an empty shard: zero gradients, no kernel
+  if (!a->d_raw || !a->stash || !a->grad_stash || !a->wgrad_scratch || !a->nerf_packed || !a->nerf_grad || !a->unmasked_offsets ||
+      !a->rigidity_mask || !a->bender_grad)
+    return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (!latent_rows || !aligned16(latent_rows)) return fail(NRN_E_INVALID, "%s: null or unaligned latent_rows (nrn_latent_rows_bytes, 16-byte aligned)", who);
+  return field_backward(a, nullptr, who, latent_rows);
+}
 
 int nrn_field_backward_tc(const NrnFieldBwdArgs* a, const NrnTcBwdArgs* t) {
   if (!a || !t) return fail(NRN_E_INVALID, "nrn_field_backward_tc: null args");
@@ -667,6 +698,26 @@ int nrn_divergence_forward(const NrnDivArgs* a) {
   p.loss = a->loss;
   { ScopedTimer tm(5, st); e = nrn::launch_div_fwd(p, ds->num_sms, st); }
   return e == cudaSuccess ? NRN_OK : cuda_fail(e, "div_fwd_kernel");
+}
+
+int nrn_divergence_forward_det(const NrnDivArgs* a, float* loss_rows) {
+  const char* who = "nrn_divergence_forward_det";
+  nrn::DivParams p{};
+  int rc = fill_div(a, p, who);
+  if (rc) return rc;
+  if (!a->loss) return fail(NRN_E_INVALID, "%s: null loss", who);
+  if (a->n_rays == 0) return NRN_OK;
+  if (!loss_rows) return fail(NRN_E_INVALID, "%s: null loss_rows (nrn_div_loss_rows_bytes)", who);
+  DeviceState* ds;
+  rc = device_state(&ds);
+  if (rc) return rc;
+  p.err = ds->err_word;
+  cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  cudaError_t e;
+  { ScopedTimer tm(5, st); e = nrn::launch_div_fwd_det(p, loss_rows, ds->num_sms, st); }
+  if (e != cudaSuccess) return cuda_fail(e, "div_fwd_det_kernel");
+  { ScopedTimer tm(14, st); e = nrn::launch_div_loss_reduce(loss_rows, a->loss, a->n_rays, a->n_samples, st); }
+  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "div_loss_reduce_kernel");
 }
 
 int nrn_divergence_backward(const NrnDivArgs* a) {

@@ -163,7 +163,11 @@ __device__ __forceinline__ void epi_mask_split(const float (&acc)[NR], const Rel
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kDivThreads, 1) div_fwd_kernel(const DivParams p) {
+// DET = false: the per-ray loss is added into p.loss with fp32 atomics, in no fixed order.
+// DET = true (deterministic mode): a warp whose 32 rows are all valid and of one ray stores its butterfly sum in
+// loss_rows[32k], its first point; any other warp stores each valid row's share; div_loss_reduce_kernel sums them per ray.
+template <bool DET>
+__device__ __forceinline__ void div_fwd_body(const DivParams& p, float* loss_rows) {
   extern __shared__ __align__(128) uint8_t smem[];
   const int wg = threadIdx.x >> 7;
   const int h = wg & 1;                   // half of the tile: rows [64 h, 64 h + 64)
@@ -272,15 +276,25 @@ __global__ void __launch_bounds__(kDivThreads, 1) div_fwd_kernel(const DivParams
         if (__all_sync(0xffffffffu, valid && ray == ray0)) {
 #pragma unroll
           for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-          if (lane == 0) atomicAdd(p.loss + ray0, part);
+          if constexpr (DET) {
+            if (lane == 0) loss_rows[pt] = part;   // lane 0's point is the warp's first, 32k
+          } else {
+            if (lane == 0) atomicAdd(p.loss + ray0, part);
+          }
         } else if (valid) {
-          atomicAdd(p.loss + ray, part);
+          if constexpr (DET) loss_rows[pt] = part;
+          else atomicAdd(p.loss + ray, part);
         }
       }
     }
     // the staging rows are rewritten only after the next tile's warpgroup barriers
   }
   if (wg_leader) tma_bulk_wait<0>();   // all tangent-stash stores complete before the CTA exits
+}
+
+__global__ void __launch_bounds__(kDivThreads, 1) div_fwd_kernel(const DivParams p) { div_fwd_body<false>(p, nullptr); }
+__global__ void __launch_bounds__(kDivThreads, 1) div_fwd_det_kernel(const DivParams p, float* loss_rows) {
+  div_fwd_body<true>(p, loss_rows);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -395,15 +409,15 @@ __global__ void div_G_kernel(const DivParams p, const float* __restrict__ g_ray,
   if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(reinterpret_cast<int*>(amax), __float_as_int(m));   // non-negative floats order like ints
 }
 
-template <typename Kernel>
-cudaError_t launch_div(Kernel kernel, int wbytes, const DivParams& p, int num_sms, cudaStream_t st) {
+template <typename Kernel, typename... Extra>
+cudaError_t launch_div(Kernel kernel, int wbytes, const DivParams& p, int num_sms, cudaStream_t st, const Extra&... extra) {
   const long long tiles = (p.P + kTileM - 1) / kTileM;
   if (tiles <= 0) return cudaSuccess;
   const int smem = static_cast<int>(div_smem_bytes(wbytes));
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) return e;
   const long long pairs = (tiles + kDivTilesPerCta - 1) / kDivTilesPerCta;
-  kernel<<<static_cast<unsigned>(pairs < num_sms ? pairs : num_sms), kDivThreads, smem, st>>>(p);
+  kernel<<<static_cast<unsigned>(pairs < num_sms ? pairs : num_sms), kDivThreads, smem, st>>>(p, extra...);
   return cudaGetLastError();
 }
 }  // namespace
@@ -420,6 +434,9 @@ cudaError_t launch_div_fwd(const DivParams& p, int num_sms, cudaStream_t st) {
 }
 cudaError_t launch_div_bwd(const DivParams& p, int num_sms, cudaStream_t st) {
   return launch_div(div_bwd_kernel, kDivBwdWBytes, p, num_sms, st);
+}
+cudaError_t launch_div_fwd_det(const DivParams& p, float* loss_rows, int num_sms, cudaStream_t st) {
+  return launch_div(div_fwd_det_kernel, kDivFwdWBytes, p, num_sms, st, loss_rows);
 }
 
 }  // namespace nrn

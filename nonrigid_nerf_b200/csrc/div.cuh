@@ -32,6 +32,8 @@ struct DivParams {
 
 cudaError_t launch_div_fwd(const DivParams& p, int num_sms, cudaStream_t st);
 cudaError_t launch_div_bwd(const DivParams& p, int num_sms, cudaStream_t st);
+// deterministic mode: per-point loss rows [P] instead of atomics into p.loss (launch_div_loss_reduce then writes p.loss)
+cudaError_t launch_div_fwd_det(const DivParams& p, float* loss_rows, int num_sms, cudaStream_t st);
 // G[pt] = g_ray[pt / S] * 2 * w * d / S (the gradient of mean_s(w d^2)) and amax = max|G| in one pass
 cudaError_t launch_div_G(const DivParams& p, const float* g_ray, float* G, float* amax, cudaStream_t st);
 

@@ -13,7 +13,8 @@
 //   steps 4..8   L5h^T, L4^T..L1^T                    -> dY4..dY0
 //   step  9      L0^T     dE += ...                   -> PE backward; bend backward -> dYb4
 //   steps 10..13 B4^T..B1^T (offset + rigidity MLPs, block diagonal) -> dYb3..dYb0
-//   step  14     B0^T     d(bender input)             -> per-ray latent gradient (fp32 atomics)
+//   step  14     B0^T     d(bender input)             -> per-ray latent gradient (fp32 atomics; field_bwd_det_kernel:
+//                                                         per-point rows for det_reduce.cu's fixed-order sum)
 // All gradients travel in fp16 scaled by a power-of-two loss scale derived on the device from
 // max|d_raw| (no host sync); WGRAD and the latent reduction divide it out again in fp32.
 // field_bwd_views_kernel (view-dependent head, no bender): Rgb^T, ViewsF^T and Feature^T + head^T in front of L7^T.
@@ -149,8 +150,12 @@ __device__ __forceinline__ Step step_at_views(int step) {
 
 }  // namespace
 
-template <bool HAS_BENDER>
-__global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBwdParams p) {
+// DET = false: B0^T adds each warp's latent rows into d_latents with fp32 atomics, in no fixed order.
+// DET = true (deterministic mode): it writes them to latent_rows [P][32] instead (det_reduce.cu's rule: a warp whose 32 rows
+// are all valid and of one ray stores their transpose-reduced sum in the row of its first point, 32k; any other warp stores
+// each valid row), and latent_reduce_kernel sums them per ray in a fixed order.
+template <bool HAS_BENDER, bool DET>
+__device__ __forceinline__ void field_bwd_body(const FieldBwdParams& p, float* latent_rows) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* act = smem;                               // bender gradient operand (24 KB), 128 rows
   uint8_t* ring_buf = smem + kBwdActBytes;           // kBwdRingStages x 32 KB
@@ -364,16 +369,30 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
         const long long ray0 = __shfl_sync(0xffffffffu, ray, 0);
         if (__all_sync(0xffffffffu, ray == ray0 && valid)) {
           const float tot = warp_transpose_reduce(dl, lane);   // lane j holds latent dim j
-          atomicAdd(p.d_latents + ray0 * kLatent + lane, tot);
+          if constexpr (DET) latent_rows[(pt - lane) * kLatent + lane] = tot;   // the row of the warp's first point, 32k
+          else atomicAdd(p.d_latents + ray0 * kLatent + lane, tot);
         } else if (valid) {
+          if constexpr (DET) {
+            float4* dst = reinterpret_cast<float4*>(latent_rows + pt * kLatent);
 #pragma unroll
-          for (int i = 0; i < 32; ++i) atomicAdd(p.d_latents + ray * kLatent + i, dl[i]);
+            for (int i = 0; i < 8; ++i) dst[i] = make_float4(dl[4 * i], dl[4 * i + 1], dl[4 * i + 2], dl[4 * i + 3]);
+          } else {
+#pragma unroll
+            for (int i = 0; i < 32; ++i) atomicAdd(p.d_latents + ray * kLatent + i, dl[i]);
+          }
         }
       }
     }
     // next: the next tile's L5e^T rewrites stg only after its own barrier; act only after the bender's sw.begin()
   }
   if (wg_leader) tma_bulk_wait<0>();   // all gradient-stash stores complete before the CTA exits
+}
+
+template <bool HAS_BENDER>
+__global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBwdParams p) { field_bwd_body<HAS_BENDER, false>(p, nullptr); }
+// deterministic mode (bender only): the per-ray latent gradient goes through latent_rows and latent_reduce_kernel
+__global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_det_kernel(const FieldBwdParams p, float* latent_rows) {
+  field_bwd_body<true, true>(p, latent_rows);
 }
 
 
@@ -547,6 +566,10 @@ __global__ void __launch_bounds__(256) tc_dw_lat_kernel(const TcBwdParams p) {
 
 cudaError_t launch_field_bwd(const FieldBwdParams& p, bool has_bender, int num_sms, cudaStream_t stream) {
   return launch_field(has_bender ? field_bwd_kernel<true> : field_bwd_kernel<false>, p, num_sms, kBwdSmemBytes, stream);
+}
+
+cudaError_t launch_field_bwd_det(const FieldBwdParams& p, float* latent_rows, int num_sms, cudaStream_t stream) {
+  return launch_field(field_bwd_det_kernel, p, num_sms, kBwdSmemBytes, stream, latent_rows);
 }
 
 cudaError_t launch_field_bwd_views(const FieldBwdParams& p, const ViewBwdParams& v, int num_sms, cudaStream_t stream) {

@@ -274,13 +274,14 @@ struct StashWriter {
   }
 };
 
-// Launch of a persistent field kernel: one CTA per SM at most, `smem` bytes of dynamic shared memory
-template <typename Kernel, typename Params>
-cudaError_t launch_field(Kernel kernel, const Params& p, int num_sms, size_t smem, cudaStream_t stream) {
+// Launch of a persistent field kernel: one CTA per SM at most, `smem` bytes of dynamic shared memory; `extra`: the kernel's
+// arguments after p
+template <typename Kernel, typename Params, typename... Extra>
+cudaError_t launch_field(Kernel kernel, const Params& p, int num_sms, size_t smem, cudaStream_t stream, const Extra&... extra) {
   if (p.n_tiles <= 0) return cudaSuccess;
   const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  kernel<<<p.n_tiles < num_sms ? p.n_tiles : num_sms, kFwdThreads, smem, stream>>>(p);
+  kernel<<<p.n_tiles < num_sms ? p.n_tiles : num_sms, kFwdThreads, smem, stream>>>(p, extra...);
   return cudaGetLastError();
 }
 
