@@ -138,23 +138,10 @@ class _FieldTrainFn(torch.autograd.Function):
         scratch = torch.empty(lib.nrn_wgrad_scratch_bytes(), dtype=torch.uint8, device=dev)
         a.grad_stash, a.wgrad_scratch = gstash.data_ptr(), scratch.data_ptr()
         a.nerf_packed = nerf_pack.data_ptr()
-        # Where the weight gradients go.  If the .grad tensors of this module's parameters lie back to back in one buffer
-        # (optim.Adam's arena) the WGRAD reduction ADDS into them in place and autograd gets nothing to accumulate;
-        # otherwise fresh flat buffers are handed to autograd as per-parameter views (torch.optim.Adam, or after the
-        # caller re-bound gradients -- the reference sets weights.grad = None between its two backward passes,
-        # train.py:1598-1604).
-        nerf_p = list(ctx.params[:ctx.n_nerf])
-        pts_dst = _arena_destination(nerf_p[:-2]) if all(p.requires_grad for p in nerf_p) else None
-        head_dst = _arena_destination(nerf_p[-2:]) if pts_dst is not None else None
-        nerf_grad = None
-        if head_dst is not None:
-            a.nerf_grad, a.nerf_grad_head, a.accumulate_nerf = pts_dst, head_dst, 1
-        else:
-            n_floats = lib.nrn_nerf_tc_grad_floats(out_ch) if ctx.tc_latents is not None else lib.nrn_nerf_grad_floats(out_ch)
-            nerf_grad = torch.empty(n_floats, dtype=torch.float32, device=dev)
-            a.nerf_grad = nerf_grad.data_ptr()
+        nerf_p = list(ctx.params[:ctx.n_nerf])   # the output_linear block (last two) goes to its own destination
+        n_floats = lib.nrn_nerf_tc_grad_floats(out_ch) if ctx.tc_latents is not None else lib.nrn_nerf_grad_floats(out_ch)
+        nerf_grad, a.nerf_grad, a.nerf_grad_head, a.accumulate_nerf = _grad_destination(nerf_p, len(nerf_p) - 2, n_floats, dev)
         bend_grad = d_lat = None
-        bend_in_place = False
         keep = [d_raw]
         if bender is not None:
             un, rig = ctx.saved_tensors
@@ -172,12 +159,8 @@ class _FieldTrainFn(torch.autograd.Function):
                 a.use_cutoff, a.rigidity_cutoff = 1, float(cutoff)
             if scaling is not None:
                 a.use_scaling, a.scaling = 1, float(scaling)
-            bend_dst = _bender_arena(bender)
-            if bend_dst is not None:
-                a.bender_grad, a.accumulate_bender, bend_in_place = bend_dst, 1, True
-            else:
-                bend_grad = torch.empty(lib.nrn_bender_grad_floats(), dtype=torch.float32, device=dev)
-                a.bender_grad = bend_grad.data_ptr()
+            bend_p = list(ctx.params[ctx.n_nerf:])
+            bend_grad, a.bender_grad, _, a.accumulate_bender = _grad_destination(bend_p, len(bend_p), lib.nrn_bender_grad_floats(), dev)
             d_lat = torch.empty(n, ops.LATENT, dtype=torch.float32, device=dev)
             a.d_latents = d_lat.data_ptr()
         a.stream = torch.cuda.current_stream().cuda_stream
@@ -201,16 +184,9 @@ class _FieldTrainFn(torch.autograd.Function):
                 _lib.check(lib.nrn_field_backward(C.byref(a)), "field_backward")
         # the stash and the ReLU masks live as long as the autograd node: backward(retain_graph=True) followed by a second backward()
         # over the same graph (test-latent pass of the reference loop, train.py:1595-1606) reads it again
-        if nerf_grad is None:
-            grads = [None] * len(nerf_p)
-        else:
-            grads = [g if p.requires_grad else None for g, p in zip(_split_flat(nerf_grad, nerf_p), nerf_p)]
+        grads = _param_grads(nerf_grad, nerf_p)
         if bender is not None:
-            bend_p = list(ctx.params[ctx.n_nerf:])
-            if bend_in_place:
-                grads += [None] * len(bend_p)
-            else:
-                grads += [g if p.requires_grad else None for g, p in zip(_split_flat(bend_grad, bend_p), bend_p)]
+            grads += _param_grads(bend_grad, bend_p)
         return (None, None, None, d_lat, None, *grads)
 
 
@@ -222,11 +198,29 @@ def _arena_destination(params):
     return arena_destination(list(params))
 
 
-def _bender_arena(bender):
-    _, bend_p = _flat_params(None, bender)
-    if not all(p.requires_grad for p in bend_p):
-        return None
-    return _arena_destination(bend_p)
+def _grad_destination(params, split: int, n_floats: int, dev):
+    """Where the WGRAD reduction puts the gradients of `params` (in its flat order; params[split:] is the block it writes
+    to a head destination of its own, none when split == len(params)).  When every parameter requires a gradient and the
+    .grad tensors of each block lie back to back in one buffer (optim.Adam's arena), it ADDS into them in place and
+    autograd gets nothing to accumulate: (None, block address, head block address or None, 1).  Otherwise a fresh flat
+    buffer of n_floats, handed to autograd as per-parameter views by _param_grads (torch.optim.Adam, or after the caller
+    re-bound gradients -- the reference sets weights.grad = None between its two backward passes, train.py:1598-1604):
+    (buffer, its address, None, 0)."""
+    if all(p.requires_grad for p in params):
+        dst = _arena_destination(params[:split])
+        head = _arena_destination(params[split:]) if dst is not None and split < len(params) else None
+        if dst is not None and (head is not None or split == len(params)):
+            return None, dst, head, 1
+    flat = torch.empty(n_floats, dtype=torch.float32, device=dev)
+    return flat, flat.data_ptr(), None, 0
+
+
+def _param_grads(flat: Optional[torch.Tensor], params):
+    """What backward returns for `params` after _grad_destination: nothing where WGRAD added into the arena, else views of
+    the flat buffer (None for a parameter that needs no gradient)."""
+    if flat is None:
+        return [None] * len(params)
+    return [g if p.requires_grad else None for g, p in zip(_split_flat(flat, params), params)]
 
 
 class _LatentGatherFn(torch.autograd.Function):
@@ -302,6 +296,20 @@ def lookup_relu_mask(unmasked: torch.Tensor) -> Optional[torch.Tensor]:
     return ref() if ref is not None else None
 
 
+def _div_args(ctx):
+    """The NrnDivArgs fields the divergence forward and backward share, from the tensors the forward keeps in ctx."""
+    un, rg, w, e, relu_mask, bender_pack, tan, scal = ctx.keep
+    a = _lib.NrnDivArgs()
+    a.n_rays, a.n_samples = ctx.shape
+    a.relu_mask, a.e, a.unmasked_offsets, a.rigidity_mask, a.weights = relu_mask.data_ptr(), e.data_ptr(), un.data_ptr(), rg.data_ptr(), w.data_ptr()
+    a.weights_are_opacity_alpha = 1 if ctx.w_is_alpha else 0
+    a.bender_packed = bender_pack.data_ptr()
+    a.tangent_stash = tan.data_ptr()
+    a.d, a.alpha, a.beta, a.tau_c = (scal[i].data_ptr() for i in range(4))
+    a.stream = torch.cuda.current_stream().cuda_stream
+    return a
+
+
 class _DivergenceFn(torch.autograd.Function):
     """per-ray mean_s(w * (e^T J e)^2) of the offset field, closed-form forward and backward (csrc/div.cu)."""
 
@@ -310,8 +318,6 @@ class _DivergenceFn(torch.autograd.Function):
         n, s = unmasked.shape[0], unmasked.shape[1]
         dev = unmasked.device
         lib = _lib.load()
-        a = _lib.NrnDivArgs()
-        a.n_rays, a.n_samples = n, s
         un = unmasked.detach().contiguous().float()
         rg = rigidity.detach().contiguous().float()
         w = weights.detach().contiguous().float()
@@ -320,13 +326,11 @@ class _DivergenceFn(torch.autograd.Function):
         tan = torch.empty(lib.nrn_div_stash_bytes(n, s), dtype=torch.uint8, device=dev)
         scal = torch.empty(4, n * s, dtype=torch.float32, device=dev)
         loss = torch.empty(n, dtype=torch.float32, device=dev)
-        a.relu_mask, a.e, a.unmasked_offsets, a.rigidity_mask, a.weights = relu_mask.data_ptr(), e.data_ptr(), un.data_ptr(), rg.data_ptr(), w.data_ptr()
-        a.weights_are_opacity_alpha = 1 if w_is_alpha else 0
-        a.bender_packed = bender_pack.data_ptr()
-        a.tangent_stash = tan.data_ptr()
-        a.d, a.alpha, a.beta, a.tau_c = (scal[i].data_ptr() for i in range(4))
+        ctx.keep = (un, rg, w, e, relu_mask, bender_pack, tan, scal)
+        ctx.w_is_alpha = bool(w_is_alpha)
+        ctx.shape = (n, s)
+        a = _div_args(ctx)
         a.loss = loss.data_ptr()
-        a.stream = torch.cuda.current_stream().cuda_stream
         if torch.are_deterministic_algorithms_enabled():   # the per-ray loss in a fixed order instead of fp32 atomics
             rows = torch.empty(lib.nrn_div_loss_rows_bytes(n, s) // 4, dtype=torch.float32, device=dev)
             with torch.cuda.device(dev):
@@ -334,52 +338,31 @@ class _DivergenceFn(torch.autograd.Function):
         else:
             with torch.cuda.device(dev):
                 _lib.check(lib.nrn_divergence_forward(C.byref(a)), "divergence_forward")
-        ctx.keep = (un, rg, w, e, relu_mask, bender_pack, tan, scal, bender)
         ctx.bend_p = bend_p
-        ctx.w_is_alpha = bool(w_is_alpha)
-        ctx.shape = (n, s)
         ctx.in_shapes = (unmasked.shape, rigidity.shape)
         return loss
 
     @staticmethod
     def backward(ctx, g):
-        un, rg, w, e, relu_mask, bender_pack, tan, scal, bender = ctx.keep
         n, s = ctx.shape
-        dev = un.device
+        dev = ctx.keep[0].device
         lib = _lib.load()
         # G = dL/dd per point = g_ray * 2 * w * d / S, computed (with its max, the loss-scale source) by the library
         g = g.reshape(n).contiguous().float()
         G = torch.empty(n * s, dtype=torch.float32, device=dev)
-        a = _lib.NrnDivArgs()
-        a.n_rays, a.n_samples = n, s
-        a.relu_mask, a.e, a.unmasked_offsets, a.rigidity_mask, a.weights = relu_mask.data_ptr(), e.data_ptr(), un.data_ptr(), rg.data_ptr(), w.data_ptr()
-        a.weights_are_opacity_alpha = 1 if ctx.w_is_alpha else 0
-        a.bender_packed = bender_pack.data_ptr()
-        a.tangent_stash = tan.data_ptr()
-        a.d, a.alpha, a.beta, a.tau_c = (scal[i].data_ptr() for i in range(4))
+        a = _div_args(ctx)
         a.g_ray, a.G_workspace = g.data_ptr(), G.data_ptr()
         adj = torch.empty(lib.nrn_div_grad_stash_bytes(n, s), dtype=torch.uint8, device=dev)
         scratch = torch.empty(lib.nrn_wgrad_scratch_bytes(), dtype=torch.uint8, device=dev)
         d_un = torch.empty(n * s, 3, dtype=torch.float32, device=dev)
         d_rg = torch.empty(n * s, dtype=torch.float32, device=dev)
-        bend_dst = _bender_arena(bender)
-        bend_grad = None
-        if bend_dst is not None:
-            a.bender_grad, a.accumulate_bender = bend_dst, 1
-        else:
-            bend_grad = torch.empty(lib.nrn_bender_grad_floats(), dtype=torch.float32, device=dev)
-            a.bender_grad = bend_grad.data_ptr()
+        bend_p = list(ctx.bend_p)
+        bend_grad, a.bender_grad, _, a.accumulate_bender = _grad_destination(bend_p, len(bend_p), lib.nrn_bender_grad_floats(), dev)
         a.adjoint_stash, a.wgrad_scratch = adj.data_ptr(), scratch.data_ptr()
         a.d_unmasked_offsets, a.d_rigidity_mask = d_un.data_ptr(), d_rg.data_ptr()
-        a.stream = torch.cuda.current_stream().cuda_stream
         with torch.cuda.device(dev):
             _lib.check(lib.nrn_divergence_backward(C.byref(a)), "divergence_backward")
-        bend_p = list(ctx.bend_p)
-        if bend_grad is None:
-            pgrads = [None] * len(bend_p)
-        else:
-            pgrads = [g if p.requires_grad else None for g, p in zip(_split_flat(bend_grad, bend_p), bend_p)]
-        return (d_un.view(ctx.in_shapes[0]), d_rg.view(ctx.in_shapes[1]), None, None, None, None, None, *pgrads)
+        return (d_un.view(ctx.in_shapes[0]), d_rg.view(ctx.in_shapes[1]), None, None, None, None, None, *_param_grads(bend_grad, bend_p))
 
 
 def divergence_loss(unmasked: torch.Tensor, rigidity: torch.Tensor, weights: Optional[torch.Tensor], bender,
@@ -596,29 +579,15 @@ class _ViewsTrainFn(torch.autograd.Function):
         scratch = torch.empty(lib.nrn_wgrad_scratch_bytes(), dtype=torch.uint8, device=dev)
         a.grad_stash, a.wgrad_scratch = gstash.data_ptr(), scratch.data_ptr()
         a.nerf_packed = nerf_pack.data_ptr()
-        # in place into optim.Adam's arena when the trunk's and the head block's .grad tensors each lie back to back there
-        # (as in _FieldTrainFn), else fresh flat buffers handed to autograd as per-parameter views
-        params = list(ctx.params)
-        trunk_p, head_p = params[:ctx.n_trunk], params[ctx.n_trunk:]
-        trunk_dst = _arena_destination(trunk_p) if all(p.requires_grad for p in params) else None
-        head_dst = _arena_destination(head_p) if trunk_dst is not None else None
-        flat = None
-        if head_dst is not None:
-            a.nerf_grad, a.nerf_grad_head, a.accumulate_nerf = trunk_dst, head_dst, 1
-        else:
-            flat = torch.empty(lib.nrn_nerf_views_grad_floats(), dtype=torch.float32, device=dev)
-            a.nerf_grad = flat.data_ptr()
+        params = list(ctx.params)   # the trunk's, then the head block's
+        flat, a.nerf_grad, a.nerf_grad_head, a.accumulate_nerf = _grad_destination(params, ctx.n_trunk, lib.nrn_nerf_views_grad_floats(), dev)
         a.stream = torch.cuda.current_stream().cuda_stream
         v = _lib.NrnViewBwdArgs()
         v.views_t_packed, v.views_stash, v.views_grad_stash, v.hv_mask = (
             views_t.data_ptr(), bufs["views_stash"].data_ptr(), vgstash.data_ptr(), bufs["hv_mask"].data_ptr())
         with torch.cuda.device(dev):
             _lib.check(lib.nrn_field_backward_views(C.byref(a), C.byref(v)), "field_backward_views")
-        if flat is None:
-            grads = [None] * len(params)
-        else:
-            grads = [g if p.requires_grad else None for g, p in zip(_split_flat(flat, params), params)]
-        return (None, None, None, None, None, *grads)
+        return (None, None, None, None, None, *_param_grads(flat, params))
 
 
 def field_views(net, rays, z_vals, points, latents, viewdirs, want_details, bend_only=False):

@@ -107,6 +107,132 @@ struct ScopedTimer {
   }
 };
 
+// One kernel launch `launch()`, timed as `kind`; a launch error is reported under the kernel's name
+template <typename Launch>
+int timed(int kind, cudaStream_t st, const char* kernel, Launch launch) {
+  cudaError_t e;
+  {
+    ScopedTimer tm(kind, st);
+    e = launch();
+  }
+  return e == cudaSuccess ? NRN_OK : cuda_fail(e, kernel);
+}
+
+// Tiles of kTileM points that P points fill
+long long tile_count(long long P) { return (P + nrn::kTileM - 1) / nrn::kTileM; }
+long long even_tiles(int n_rays, int n_samples) {
+  return (tile_count(static_cast<long long>(n_rays) * n_samples) + 1) & ~1LL;   // rounded up to an even count: the stash layout of ABI version 2
+}
+int checked_tiles(long long P, const char* who, int* tiles) {
+  const long long t = tile_count(P);
+  if (t > 0x7fffffffLL) return fail(NRN_E_INVALID, "%s: too many points", who);
+  *tiles = static_cast<int>(t);
+  return NRN_OK;
+}
+
+// The checks every field forward entry point applies to its NrnFieldArgs.  *P = n_rays * n_samples; for an empty batch
+// (P = 0) only the sizes and out_ch are checked, and nothing is to be launched.
+int check_field_args(const NrnFieldArgs* a, const char* who, long long* P, int* tiles) {
+  if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
+  if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "%s: bad sizes n=%d S=%d", who, a->n_rays, a->n_samples);
+  if (a->out_ch < 4 || a->out_ch > 5) return fail(NRN_E_INVALID, "%s: out_ch=%d unsupported (4 or 5)", who, a->out_ch);
+  if ((a->stash != nullptr) != (a->relu_mask != nullptr))
+    return fail(NRN_E_INVALID, "%s: training needs both the stash and the ReLU mask buffer (relu_mask)", who);
+  *P = static_cast<long long>(a->n_rays) * a->n_samples;
+  *tiles = 0;
+  if (*P == 0) return NRN_OK;
+  if (!a->nerf_packed) return fail(NRN_E_INVALID, "%s: null nerf_packed", who);
+  if (a->points) {
+    if (a->points_stride < 3) return fail(NRN_E_INVALID, "%s: point mode needs points_stride >= 3", who);
+  } else if (!a->rays || !a->z_vals) {
+    return fail(NRN_E_INVALID, "%s: null rays / z_vals", who);
+  }
+  if (a->bender_packed && !a->latents) return fail(NRN_E_INVALID, "%s: bender given without latents", who);
+  if (a->stash && a->points) return fail(NRN_E_INVALID, "%s: the training stash needs ray mode", who);
+  if (!aligned16(a->nerf_packed) || (a->bender_packed && !aligned16(a->bender_packed)))
+    return fail(NRN_E_INVALID, "%s: packed weights must be 16-byte aligned", who);
+  // the forward kernels store the stash with bulk copies, which need 16-byte aligned destinations
+  if (a->stash && (!aligned16(a->stash) || !aligned16(a->relu_mask)))
+    return fail(NRN_E_INVALID, "%s: stash and relu_mask must be 16-byte aligned", who);
+  return checked_tiles(*P, who, tiles);
+}
+
+nrn::FieldFwdParams field_fwd_params(const NrnFieldArgs* a, long long P, int tiles, int* err) {
+  nrn::FieldFwdParams p{};
+  p.rays = a->rays; p.z_vals = a->z_vals; p.pts = a->points; p.pts_stride = a->points_stride; p.latents = a->latents; p.latent_stride = a->latent_stride;
+  p.n_rays = a->n_rays; p.S = a->n_samples; p.P = P; p.n_tiles = tiles;
+  const uint8_t* np = static_cast<const uint8_t*>(a->nerf_packed);
+  p.nerf_w = np; p.nerf_bias = reinterpret_cast<const float*>(np + nrn::kNerfWBytes);
+  if (a->bender_packed) {
+    const uint8_t* bp = static_cast<const uint8_t*>(a->bender_packed);
+    p.bend_w = bp; p.bend_bias = reinterpret_cast<const float*>(bp + nrn::kBendWBytes);
+  }
+  p.cutoff = a->rigidity_cutoff; p.use_cutoff = a->use_cutoff;
+  p.scaling = a->scaling; p.use_scaling = a->use_scaling;
+  p.removal = a->removal_threshold; p.use_removal = a->use_removal;
+  p.out_ch = a->out_ch;
+  p.raw = a->raw; p.d_init = a->initial_input_pts; p.d_bent = a->input_pts; p.d_unmasked = a->unmasked_offsets;
+  p.d_masked = a->masked_offsets; p.d_rigid = a->rigidity_mask;
+  p.stash = static_cast<uint8_t*>(a->stash);
+  p.relu_mask = static_cast<uint8_t*>(a->relu_mask);
+  p.err = err;
+  return p;
+}
+
+// The checks every field backward entry point applies to its NrnFieldBwdArgs.  *P = n_rays * n_samples; an empty shard
+// (P = 0) needs only its gradient destinations.
+int check_field_bwd_args(const NrnFieldBwdArgs* a, const char* who, long long* P, int* tiles) {
+  if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
+  if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "%s: bad sizes", who);
+  if (a->out_ch < 4 || a->out_ch > 5) return fail(NRN_E_INVALID, "%s: out_ch=%d unsupported", who, a->out_ch);
+  if (!a->nerf_grad) return fail(NRN_E_INVALID, "%s: null nerf_grad", who);
+  if (a->bender_packed && (!a->unmasked_offsets || !a->rigidity_mask || !a->bender_grad || !a->d_latents))
+    return fail(NRN_E_INVALID, "%s: null argument: a bender needs unmasked_offsets, rigidity_mask, bender_grad, d_latents", who);
+  *P = static_cast<long long>(a->n_rays) * a->n_samples;
+  *tiles = 0;
+  if (*P == 0) return NRN_OK;
+  if (!a->nerf_packed || !a->d_raw || !a->stash || !a->grad_stash || !a->wgrad_scratch || !a->relu_mask)
+    return fail(NRN_E_INVALID, "%s: null argument: nerf_packed, d_raw, stash, grad_stash, wgrad_scratch or relu_mask (the ReLU masks of the forward call)", who);
+  if (!aligned16(a->nerf_packed) || !aligned16(a->stash) || !aligned16(a->grad_stash) || !aligned16(a->relu_mask))
+    return fail(NRN_E_INVALID, "%s: packed weights and stashes must be 16-byte aligned", who);
+  return checked_tiles(*P, who, tiles);
+}
+
+nrn::FieldBwdParams field_bwd_params(const NrnFieldBwdArgs* a, long long P, int tiles, float* amax, int* err) {
+  nrn::FieldBwdParams p{};
+  p.P = P; p.n_tiles = tiles;
+  p.S = a->n_samples; p.n_rays = a->n_rays; p.out_ch = a->out_ch;
+  p.d_raw = a->d_raw; p.amax = amax;
+  p.stash = static_cast<const uint8_t*>(a->stash); p.gstash = static_cast<uint8_t*>(a->grad_stash);
+  p.nerf_wT = static_cast<const uint8_t*>(a->nerf_packed) + nrn::kNerfTOffset;
+  if (a->bender_packed) p.bend_wT = static_cast<const uint8_t*>(a->bender_packed) + nrn::kBendTOffset;
+  p.unmasked = a->unmasked_offsets; p.rigidity = a->rigidity_mask;
+  p.d_unmasked_up = a->d_unmasked_offsets; p.d_rigid_up = a->d_rigidity_mask;
+  p.cutoff = a->rigidity_cutoff; p.use_cutoff = a->use_cutoff; p.scaling = a->scaling; p.use_scaling = a->use_scaling;
+  p.d_latents = a->d_latents; p.err = err;
+  p.relu_mask = static_cast<const uint8_t*>(a->relu_mask);
+  return p;
+}
+
+// An empty shard contributes zero gradients: the destinations that are overwritten rather than accumulated are cleared.
+// nerf_n floats of NeRF gradient, the last head_n of them at nerf_grad_head when that is given; bend_n of the bender's.
+int zero_grads(const NrnFieldBwdArgs* a, int nerf_n, int head_n, int bend_n, cudaStream_t st) {
+  cudaError_t e = cudaSuccess;
+  if (!a->accumulate_nerf) {
+    if (!a->nerf_grad_head) head_n = 0;
+    e = cudaMemsetAsync(a->nerf_grad, 0, sizeof(float) * (nerf_n - head_n), st);
+    if (e == cudaSuccess && head_n) e = cudaMemsetAsync(a->nerf_grad_head, 0, sizeof(float) * head_n, st);
+  }
+  if (e == cudaSuccess && bend_n && !a->accumulate_bender) e = cudaMemsetAsync(a->bender_grad, 0, sizeof(float) * bend_n, st);
+  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "memset grads");
+}
+
+nrn::WgradParams wgrad_params(const uint8_t* stash, uint8_t* gstash, float* scratch, float* amax, int n_tiles, int* err) {
+  nrn::WgradParams w{};
+  w.stash = stash; w.gstash = gstash; w.scratch = scratch; w.amax = amax; w.n_tiles = n_tiles; w.err = err;
+  return w;
+}
+
 }  // namespace
 
 extern "C" {
@@ -207,55 +333,20 @@ int nrn_median_visibility_index(const float* weights, int n_rays, int n_samples,
 
 // nrn_field_forward, or with ray_bias (time-conditioned baseline, no bender) nrn_field_forward_tc
 static int field_forward(const NrnFieldArgs* a, const float* ray_bias, const char* who) {
-  if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
-  if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "%s: bad sizes n=%d S=%d", who, a->n_rays, a->n_samples);
-  if (a->n_rays == 0) return NRN_OK;
-  if (!a->nerf_packed || !a->raw) return fail(NRN_E_INVALID, "%s: null argument", who);
-  if (a->points) {
-    if (a->n_samples != 1 || a->points_stride < 3) return fail(NRN_E_INVALID, "%s: point mode needs n_samples=1, stride>=3", who);
-  } else if (!a->rays || !a->z_vals) {
-    return fail(NRN_E_INVALID, "%s: null rays / z_vals", who);
-  }
-  if (a->bender_packed && !a->latents) return fail(NRN_E_INVALID, "%s: bender given without latents", who);
-  if (a->out_ch < 4 || a->out_ch > 5) return fail(NRN_E_INVALID, "%s: out_ch=%d unsupported (4 or 5)", who, a->out_ch);
-  if (!aligned16(a->nerf_packed) || (a->bender_packed && !aligned16(a->bender_packed)))
-    return fail(NRN_E_INVALID, "%s: packed weights must be 16-byte aligned", who);
-  if ((a->stash != nullptr) != (a->relu_mask != nullptr))
-    return fail(NRN_E_INVALID, "%s: training needs both the stash and the ReLU mask buffer (relu_mask)", who);
+  long long P;
+  int tiles;
+  int rc = check_field_args(a, who, &P, &tiles);
+  if (rc || P == 0) return rc;
+  if (!a->raw) return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (a->points && a->n_samples != 1) return fail(NRN_E_INVALID, "%s: point mode needs n_samples=1, stride>=3", who);
   DeviceState* ds;
-  int rc = device_state(&ds);
+  rc = device_state(&ds);
   if (rc) return rc;
-  nrn::FieldFwdParams p{};
-  p.rays = a->rays; p.z_vals = a->z_vals; p.pts = a->points; p.pts_stride = a->points_stride; p.latents = a->latents; p.latent_stride = a->latent_stride;
-  p.n_rays = a->n_rays; p.S = a->n_samples;
-  p.P = static_cast<long long>(a->n_rays) * a->n_samples;
-  const long long tiles = (p.P + nrn::kTileM - 1) / nrn::kTileM;
-  if (tiles > 0x7fffffffLL) return fail(NRN_E_INVALID, "nrn_field_forward: too many points");
-  p.n_tiles = static_cast<int>(tiles);
-  const uint8_t* np = static_cast<const uint8_t*>(a->nerf_packed);
-  p.nerf_w = np; p.nerf_bias = reinterpret_cast<const float*>(np + nrn::kNerfWBytes);
-  if (a->bender_packed) {
-    const uint8_t* bp = static_cast<const uint8_t*>(a->bender_packed);
-    p.bend_w = bp; p.bend_bias = reinterpret_cast<const float*>(bp + nrn::kBendWBytes);
-  }
-  p.cutoff = a->rigidity_cutoff; p.use_cutoff = a->use_cutoff;
-  p.scaling = a->scaling; p.use_scaling = a->use_scaling;
-  p.removal = a->removal_threshold; p.use_removal = a->use_removal;
-  p.out_ch = a->out_ch;
-  p.raw = a->raw; p.d_init = a->initial_input_pts; p.d_bent = a->input_pts; p.d_unmasked = a->unmasked_offsets;
-  p.d_masked = a->masked_offsets; p.d_rigid = a->rigidity_mask;
-  p.stash = static_cast<uint8_t*>(a->stash);
-  p.relu_mask = static_cast<uint8_t*>(a->relu_mask);
-  if (a->stash && a->points) return fail(NRN_E_INVALID, "%s: the training stash needs ray mode", who);
-  p.err = ds->err_word;
+  nrn::FieldFwdParams p = field_fwd_params(a, P, tiles, ds->err_word);
   p.ray_bias = ray_bias; p.ray_bias_stride = a->latent_stride == 0 ? 0 : 2 * 256;
-  cudaError_t e;
-  {
-    ScopedTimer tm(0, static_cast<cudaStream_t>(a->stream));
-    e = ray_bias ? nrn::launch_field_fwd_tc(p, ds->num_sms, static_cast<cudaStream_t>(a->stream))
-                 : nrn::launch_field_fwd(p, a->bender_packed != nullptr, ds->num_sms, static_cast<cudaStream_t>(a->stream));
-  }
-  return e == cudaSuccess ? NRN_OK : cuda_fail(e, ray_bias ? "field_fwd_tc_kernel" : "field_fwd_kernel");
+  cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  if (ray_bias) return timed(0, st, "field_fwd_tc_kernel", [&] { return nrn::launch_field_fwd_tc(p, ds->num_sms, st); });
+  return timed(0, st, "field_fwd_kernel", [&] { return nrn::launch_field_fwd(p, a->bender_packed != nullptr, ds->num_sms, st); });
 }
 
 int nrn_field_forward(const NrnFieldArgs* a) { return field_forward(a, nullptr, "nrn_field_forward"); }
@@ -293,9 +384,12 @@ size_t nrn_views_workspace_bytes(int n_rays, int n_samples) {
 int nrn_field_forward_views(const NrnFieldArgs* a, const NrnViewArgs* v) {
   const char* who = "nrn_field_forward_views";
   if (!a || !v) return fail(NRN_E_INVALID, "%s: null args", who);
-  if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "%s: bad sizes n=%d S=%d", who, a->n_rays, a->n_samples);
   if (a->stash || a->relu_mask)
     return fail(NRN_E_INVALID, "%s: use_viewdirs=True is inference only (stash / relu_mask must be NULL; training is not implemented)", who);
+  long long P;
+  int tiles;
+  int rc = check_field_args(a, who, &P, &tiles);
+  if (rc) return rc;
   if (a->out_ch != 4) return fail(NRN_E_INVALID, "%s: out_ch=%d unsupported (use_viewdirs=True: 4 = rgb + alpha)", who, a->out_ch);
   const bool bend = a->bender_packed != nullptr;
   if (bend && a->raw && a->n_samples < 2)
@@ -303,57 +397,29 @@ int nrn_field_forward_views(const NrnFieldArgs* a, const NrnViewArgs* v) {
   if (!bend && !a->raw) return fail(NRN_E_INVALID, "%s: raw is NULL without a bender (the bend pass alone needs one)", who);
   if (!bend && !v->viewdirs) return fail(NRN_E_INVALID, "%s: use_viewdirs=True without a bender needs viewdirs", who);
   if (!bend && v->viewdirs_stride < 3) return fail(NRN_E_INVALID, "%s: viewdirs_stride=%lld < 3", who, (long long)v->viewdirs_stride);
-  if (a->n_rays == 0) return NRN_OK;
-  if (!a->nerf_packed || (a->raw && !v->views_packed)) return fail(NRN_E_INVALID, "%s: null nerf_packed / views_packed", who);
-  if (a->points) {
-    if (a->points_stride < 3) return fail(NRN_E_INVALID, "%s: point mode needs points_stride >= 3", who);
-  } else if (!a->rays || !a->z_vals) {
-    return fail(NRN_E_INVALID, "%s: null rays / z_vals", who);
-  }
-  if (bend && !a->latents) return fail(NRN_E_INVALID, "%s: bender given without latents", who);
+  if (P == 0) return NRN_OK;
+  if (a->raw && !v->views_packed) return fail(NRN_E_INVALID, "%s: null nerf_packed / views_packed", who);
   if (bend && (!v->workspace || !aligned16(v->workspace)))
     return fail(NRN_E_INVALID, "%s: a bender needs the workspace (nrn_views_workspace_bytes, 16-byte aligned)", who);
-  if (!aligned16(a->nerf_packed) || (bend && !aligned16(a->bender_packed)) || (v->views_packed && !aligned16(v->views_packed)))
-    return fail(NRN_E_INVALID, "%s: packed weights must be 16-byte aligned", who);
-  const long long P = static_cast<long long>(a->n_rays) * a->n_samples;
-  const long long tiles = (P + nrn::kTileM - 1) / nrn::kTileM;
-  if (tiles > 0x7fffffffLL) return fail(NRN_E_INVALID, "%s: too many points", who);
+  if (v->views_packed && !aligned16(v->views_packed)) return fail(NRN_E_INVALID, "%s: packed weights must be 16-byte aligned", who);
   DeviceState* ds;
-  int rc = device_state(&ds);
+  rc = device_state(&ds);
   if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(a->stream);
-  nrn::FieldFwdParams p{};
-  p.rays = a->rays; p.z_vals = a->z_vals; p.pts = a->points; p.pts_stride = a->points_stride;
-  p.latents = a->latents; p.latent_stride = a->latent_stride;
-  p.n_rays = a->n_rays; p.S = a->n_samples; p.P = P; p.n_tiles = static_cast<int>(tiles);
-  const uint8_t* np = static_cast<const uint8_t*>(a->nerf_packed);
-  p.nerf_w = np; p.nerf_bias = reinterpret_cast<const float*>(np + nrn::kNerfWBytes);
-  p.cutoff = a->rigidity_cutoff; p.use_cutoff = a->use_cutoff;
-  p.scaling = a->scaling; p.use_scaling = a->use_scaling;
-  p.removal = a->removal_threshold; p.use_removal = a->use_removal;
-  p.out_ch = 4; p.err = ds->err_word;
+  nrn::FieldFwdParams p = field_fwd_params(a, P, tiles, ds->err_word);
   nrn::ViewParams vp{};
   const uint8_t* vw = static_cast<const uint8_t*>(v->views_packed);
   vp.w = vw; vp.bias = vw ? reinterpret_cast<const float*>(vw + nrn::kViewsWBytes) : nullptr;
   vp.viewdirs = v->viewdirs; vp.viewdirs_stride = v->viewdirs_stride;
-  cudaError_t e;
   if (bend) {
     nrn::FieldFwdParams b = p;   // point mode: every point its own latent row
     if (a->points) { b.n_rays = static_cast<int>(P); b.S = 1; }
-    const uint8_t* bp = static_cast<const uint8_t*>(a->bender_packed);
-    b.bend_w = bp; b.bend_bias = reinterpret_cast<const float*>(bp + nrn::kBendWBytes);
-    b.d_init = a->initial_input_pts; b.d_bent = a->input_pts; b.d_unmasked = a->unmasked_offsets;
-    b.d_masked = a->masked_offsets; b.d_rigid = a->rigidity_mask;
     vp.ws = static_cast<float4*>(v->workspace);
-    { ScopedTimer tm(8, st); e = nrn::launch_field_bend(b, vp, ds->num_sms, st); }
-    if (e != cudaSuccess) return cuda_fail(e, "field_bend_kernel");
-    if (!a->raw) return NRN_OK;
-  } else {
-    p.d_init = a->initial_input_pts; p.d_bent = a->input_pts;
+    rc = timed(8, st, "field_bend_kernel", [&] { return nrn::launch_field_bend(b, vp, ds->num_sms, st); });
+    if (rc || !a->raw) return rc;
+    p.d_init = p.d_bent = nullptr;   // the bend pass wrote them; the view-head kernel reads the bent points from the workspace
   }
-  p.raw = a->raw;
-  { ScopedTimer tm(9, st); e = nrn::launch_field_views(p, vp, ds->num_sms, st); }
-  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "field_views_kernel");
+  return timed(9, st, "field_views_kernel", [&] { return nrn::launch_field_views(p, vp, ds->num_sms, st); });
 }
 
 // ---- training the view-dependent head without a bender ----
@@ -371,7 +437,6 @@ int nrn_pack_views_t(const float* const* w, void* packed, void* stream) {
   return e == cudaSuccess ? NRN_OK : cuda_fail(e, "pack_views_t_kernel");
 }
 
-static long long even_tiles(int n_rays, int n_samples);
 size_t nrn_views_stash_bytes(int n_rays, int n_samples) {
   return n_rays < 0 || n_samples < 1 ? 0 : static_cast<size_t>(even_tiles(n_rays, n_samples)) * nrn::kVStashTileBytes;
 }
@@ -386,100 +451,69 @@ int nrn_nerf_views_grad_floats(void) { return nrn::nerf_views_grad_floats(); }
 int nrn_field_forward_views_train(const NrnFieldArgs* a, const NrnViewArgs* v, const NrnViewTrainArgs* t) {
   const char* who = "nrn_field_forward_views_train";
   if (!a || !v || !t) return fail(NRN_E_INVALID, "%s: null args", who);
-  if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "%s: bad sizes n=%d S=%d", who, a->n_rays, a->n_samples);
+  long long P;
+  int tiles;
+  int rc = check_field_args(a, who, &P, &tiles);
+  if (rc) return rc;
   if (a->bender_packed)
     return fail(NRN_E_INVALID, "%s: training with the view-dependent head is not implemented with a ray bender (bender_packed must be NULL)", who);
   if (a->points) return fail(NRN_E_INVALID, "%s: training needs ray mode (points must be NULL)", who);
   if (a->out_ch != 4) return fail(NRN_E_INVALID, "%s: out_ch=%d unsupported (use_viewdirs=True: 4 = rgb + alpha)", who, a->out_ch);
   if (a->use_removal) return fail(NRN_E_INVALID, "%s: the object removal is a test-time knob; it is not differentiable", who);
   if (!v->viewdirs || v->viewdirs_stride < 3) return fail(NRN_E_INVALID, "%s: needs viewdirs with viewdirs_stride >= 3", who);
-  if (a->n_rays == 0) return NRN_OK;
-  if (!a->rays || !a->z_vals || !a->raw || !a->nerf_packed || !v->views_packed) return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (P == 0) return NRN_OK;
+  if (!a->raw || !v->views_packed) return fail(NRN_E_INVALID, "%s: null argument", who);
   if (!a->stash || !a->relu_mask || !t->views_stash || !t->hv_mask)
     return fail(NRN_E_INVALID, "%s: null stash, relu_mask, views_stash or hv_mask", who);
-  if (!aligned16(a->nerf_packed) || !aligned16(v->views_packed) || !aligned16(a->stash) || !aligned16(a->relu_mask) ||
-      !aligned16(t->views_stash) || !aligned16(t->hv_mask))
+  if (!aligned16(v->views_packed) || !aligned16(t->views_stash) || !aligned16(t->hv_mask))
     return fail(NRN_E_INVALID, "%s: packed weights and stashes must be 16-byte aligned", who);
-  const long long P = static_cast<long long>(a->n_rays) * a->n_samples;
-  const long long tiles = (P + nrn::kTileM - 1) / nrn::kTileM;
-  if (tiles > 0x7fffffffLL) return fail(NRN_E_INVALID, "%s: too many points", who);
   DeviceState* ds;
-  int rc = device_state(&ds);
+  rc = device_state(&ds);
   if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(a->stream);
-  nrn::FieldFwdParams p{};
-  p.rays = a->rays; p.z_vals = a->z_vals;
-  p.n_rays = a->n_rays; p.S = a->n_samples; p.P = P; p.n_tiles = static_cast<int>(tiles);
-  const uint8_t* np = static_cast<const uint8_t*>(a->nerf_packed);
-  p.nerf_w = np; p.nerf_bias = reinterpret_cast<const float*>(np + nrn::kNerfWBytes);
-  p.out_ch = 4; p.err = ds->err_word;
-  p.raw = a->raw; p.d_init = a->initial_input_pts; p.d_bent = a->input_pts;
-  p.stash = static_cast<uint8_t*>(a->stash); p.relu_mask = static_cast<uint8_t*>(a->relu_mask);
+  const nrn::FieldFwdParams p = field_fwd_params(a, P, tiles, ds->err_word);
   nrn::ViewParams vp{};
   const uint8_t* vw = static_cast<const uint8_t*>(v->views_packed);
   vp.w = vw; vp.bias = reinterpret_cast<const float*>(vw + nrn::kViewsWBytes);
   vp.viewdirs = v->viewdirs; vp.viewdirs_stride = v->viewdirs_stride;
-  nrn::ViewTrainParams tp{static_cast<uint8_t*>(t->views_stash), static_cast<uint8_t*>(t->hv_mask)};
-  cudaError_t e;
-  { ScopedTimer tm(10, st); e = nrn::launch_field_views_train(p, vp, tp, ds->num_sms, st); }
-  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "field_views_train_kernel");
+  const nrn::ViewTrainParams tp{static_cast<uint8_t*>(t->views_stash), static_cast<uint8_t*>(t->hv_mask)};
+  return timed(10, st, "field_views_train_kernel", [&] { return nrn::launch_field_views_train(p, vp, tp, ds->num_sms, st); });
 }
 
 int nrn_field_backward_views(const NrnFieldBwdArgs* a, const NrnViewBwdArgs* v) {
   const char* who = "nrn_field_backward_views";
   if (!a || !v) return fail(NRN_E_INVALID, "%s: null args", who);
-  if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "%s: bad sizes", who);
-  if (a->out_ch != 4) return fail(NRN_E_INVALID, "%s: out_ch=%d unsupported (use_viewdirs=True: 4 = rgb + alpha)", who, a->out_ch);
   if (a->bender_packed)
     return fail(NRN_E_INVALID, "%s: training with the view-dependent head is not implemented with a ray bender (bender_packed must be NULL)", who);
-  if (!a->nerf_grad) return fail(NRN_E_INVALID, "%s: null nerf_grad", who);
+  long long P;
+  int tiles;
+  int rc = check_field_bwd_args(a, who, &P, &tiles);
+  if (rc) return rc;
+  if (a->out_ch != 4) return fail(NRN_E_INVALID, "%s: out_ch=%d unsupported (use_viewdirs=True: 4 = rgb + alpha)", who, a->out_ch);
   const int n_all = nrn::nerf_views_grad_floats();
   cudaStream_t st = static_cast<cudaStream_t>(a->stream);
-  if (a->n_rays == 0) {   // an empty shard contributes zero gradients
-    cudaError_t e = cudaSuccess;
-    if (!a->accumulate_nerf) {
-      const int head_n = a->nerf_grad_head ? n_all - nrn::kViewsTrunkFloats : 0;
-      e = cudaMemsetAsync(a->nerf_grad, 0, sizeof(float) * (n_all - head_n), st);
-      if (e == cudaSuccess && head_n) e = cudaMemsetAsync(a->nerf_grad_head, 0, sizeof(float) * head_n, st);
-    }
-    return e == cudaSuccess ? NRN_OK : cuda_fail(e, "memset grads");
-  }
-  if (!a->d_raw || !a->stash || !a->grad_stash || !a->wgrad_scratch || !a->relu_mask || !a->nerf_packed)
-    return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (P == 0) return zero_grads(a, n_all, n_all - nrn::kViewsTrunkFloats, 0, st);
   if (!v->views_t_packed || !v->views_stash || !v->views_grad_stash || !v->hv_mask)
     return fail(NRN_E_INVALID, "%s: null views_t_packed, views_stash, views_grad_stash or hv_mask", who);
-  if (!aligned16(a->nerf_packed) || !aligned16(v->views_t_packed) || !aligned16(a->stash) || !aligned16(a->grad_stash) ||
-      !aligned16(a->relu_mask) || !aligned16(v->views_stash) || !aligned16(v->views_grad_stash) || !aligned16(v->hv_mask))
+  if (!aligned16(v->views_t_packed) || !aligned16(v->views_stash) || !aligned16(v->views_grad_stash) || !aligned16(v->hv_mask))
     return fail(NRN_E_INVALID, "%s: packed weights and stashes must be 16-byte aligned", who);
-  const long long P = static_cast<long long>(a->n_rays) * a->n_samples;
-  if ((P + nrn::kTileM - 1) / nrn::kTileM > 0x7fffffffLL) return fail(NRN_E_INVALID, "%s: too many points", who);
   DeviceState* ds;
-  int rc = device_state(&ds);
+  rc = device_state(&ds);
   if (rc) return rc;
   if (ds->num_sms + 16 > nrn::kWgMaxCtas) return fail(NRN_E_INVALID, "%s: %d SMs exceed the scratch layout", who, ds->num_sms);
   float* amax = reinterpret_cast<float*>(ds->err_word + 1);
-  nrn::FieldBwdParams p{};
-  p.P = P;
-  p.n_tiles = static_cast<int>((P + nrn::kTileM - 1) / nrn::kTileM);
-  p.S = a->n_samples; p.n_rays = a->n_rays; p.out_ch = 4;
-  p.d_raw = a->d_raw; p.amax = amax;
-  p.stash = static_cast<const uint8_t*>(a->stash); p.gstash = static_cast<uint8_t*>(a->grad_stash);
-  p.nerf_wT = static_cast<const uint8_t*>(a->nerf_packed) + nrn::kNerfTOffset;
-  p.err = ds->err_word;
-  p.relu_mask = static_cast<const uint8_t*>(a->relu_mask);
-  nrn::ViewBwdParams vp{static_cast<const uint8_t*>(v->views_t_packed), static_cast<const uint8_t*>(v->hv_mask),
-                        static_cast<uint8_t*>(v->views_grad_stash)};
+  const nrn::FieldBwdParams p = field_bwd_params(a, P, tiles, amax, ds->err_word);
+  const nrn::ViewBwdParams vp{static_cast<const uint8_t*>(v->views_t_packed), static_cast<const uint8_t*>(v->hv_mask),
+                              static_cast<uint8_t*>(v->views_grad_stash)};
   // the loss scale: max |d_raw| over the four channels (rgb and alpha)
-  cudaError_t e = nrn::launch_absmax(a->d_raw, P * 4, amax, st, false, 4, 4);
+  const cudaError_t e = nrn::launch_absmax(a->d_raw, P * 4, amax, st, false, 4, 4);
   if (e != cudaSuccess) return cuda_fail(e, "absmax_kernel");
-  { ScopedTimer tm(11, st); e = nrn::launch_field_bwd_views(p, vp, ds->num_sms, st); }
-  if (e != cudaSuccess) return cuda_fail(e, "field_bwd_views_kernel");
-  nrn::WgradParams w{};
-  w.stash = p.stash; w.gstash = p.gstash; w.scratch = a->wgrad_scratch; w.amax = amax; w.n_tiles = p.n_tiles; w.err = ds->err_word;
+  rc = timed(11, st, "field_bwd_views_kernel", [&] { return nrn::launch_field_bwd_views(p, vp, ds->num_sms, st); });
+  if (rc) return rc;
+  const nrn::WgradParams w = wgrad_params(p.stash, p.gstash, a->wgrad_scratch, amax, tiles, ds->err_word);
   const nrn::WgradViewParams wv{static_cast<const uint8_t*>(v->views_stash), vp.vgstash};
   const nrn::WgradDst dst{a->nerf_grad, a->nerf_grad_head, nullptr, n_all, 0, a->accumulate_nerf, 0};
-  { ScopedTimer tm(12, st); e = nrn::launch_wgrad_views(w, wv, ds->num_sms, dst, st); }
-  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "wgrad_views_kernel");
+  return timed(12, st, "wgrad_views_kernel", [&] { return nrn::launch_wgrad_views(w, wv, ds->num_sms, dst, st); });
 }
 
 int nrn_tc_latent_bias(const float* latents, int64_t latent_stride, int n_rays, const float* w0, const float* b0, const float* w5,
@@ -487,10 +521,9 @@ int nrn_tc_latent_bias(const float* latents, int64_t latent_stride, int n_rays, 
   if (n_rays < 0 || latent_stride < 0) return fail(NRN_E_INVALID, "nrn_tc_latent_bias: bad sizes n=%d stride=%lld", n_rays, (long long)latent_stride);
   if (n_rays == 0) return NRN_OK;
   if (!latents || !w0 || !b0 || !w5 || !b5 || !ray_bias) return fail(NRN_E_INVALID, "nrn_tc_latent_bias: null argument");
-  cudaError_t e;
-  { ScopedTimer tm(6, static_cast<cudaStream_t>(stream));
-    e = nrn::launch_tc_latent_bias(latents, latent_stride, n_rays, w0, b0, w5, b5, ray_bias, static_cast<cudaStream_t>(stream)); }
-  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "tc_latent_bias_kernel");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return timed(6, st, "tc_latent_bias_kernel",
+               [&] { return nrn::launch_tc_latent_bias(latents, latent_stride, n_rays, w0, b0, w5, b5, ray_bias, st); });
 }
 
 int nrn_composite(const NrnCompositeArgs* a) {
@@ -506,8 +539,8 @@ int nrn_composite(const NrnCompositeArgs* a) {
   p.n = a->n_rays; p.S = a->n_samples; p.C = a->channels; p.white_bkgd = a->white_bkgd;
   p.rgb = a->rgb_map; p.disp = a->disp_map; p.acc = a->acc_map; p.depth = a->depth_map; p.weights = a->weights; p.alpha = a->alpha;
   p.n_imp = a->n_importance; p.u = a->u; p.z_out = a->z_vals_out; p.z_std = a->z_std;
-  cudaError_t e; { ScopedTimer tm(3, static_cast<cudaStream_t>(a->stream)); e = nrn::launch_composite(p, static_cast<cudaStream_t>(a->stream)); }
-  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "composite_kernel");
+  cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  return timed(3, st, "composite_kernel", [&] { return nrn::launch_composite(p, st); });
 }
 
 int nrn_sample_pdf(const float* bins, const float* weights, const float* u, int n, int nbins, int n_samples, float* samples,
@@ -528,15 +561,10 @@ int nrn_composite_backward(const NrnCompositeBwdArgs* a) {
   p.raw = a->raw; p.z = a->z_vals; p.rays_d = a->rays_d; p.rays_d_stride = a->rays_d_stride; p.noise = a->noise;
   p.n = a->n_rays; p.S = a->n_samples; p.C = a->channels; p.white_bkgd = a->white_bkgd;
   p.d_rgb = a->d_rgb_map; p.d_acc = a->d_acc_map; p.d_raw = a->d_raw;
-  cudaError_t e; { ScopedTimer tm(4, static_cast<cudaStream_t>(a->stream)); e = nrn::launch_composite_bwd(p, static_cast<cudaStream_t>(a->stream)); }
-  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "composite_bwd_kernel");
+  cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  return timed(4, st, "composite_bwd_kernel", [&] { return nrn::launch_composite_bwd(p, st); });
 }
 
-static long long even_tiles(int n_rays, int n_samples) {
-  const long long P = static_cast<long long>(n_rays) * n_samples;
-  const long long tiles = (P + nrn::kTileM - 1) / nrn::kTileM;
-  return (tiles + 1) & ~1LL;   // rounded up to an even count: the stash layout of ABI version 2
-}
 size_t nrn_stash_bytes(int n_rays, int n_samples) { return static_cast<size_t>(even_tiles(n_rays, n_samples)) * nrn::kStashTileBytes; }
 size_t nrn_grad_stash_bytes(int n_rays, int n_samples) { return static_cast<size_t>(even_tiles(n_rays, n_samples)) * nrn::kGradTileBytes; }
 size_t nrn_relu_mask_bytes(int n_rays, int n_samples) { return static_cast<size_t>(even_tiles(n_rays, n_samples)) * nrn::kMaskTileBytes; }
@@ -549,19 +577,16 @@ size_t nrn_tc_workspace_bytes(int n_rays) { return n_rays < 0 ? 0 : (static_cast
 // nrn_field_backward, or with t (time-conditioned baseline, no bender) nrn_field_backward_tc, or with latent_rows
 // (deterministic mode, bender) nrn_field_backward_det
 static int field_backward(const NrnFieldBwdArgs* a, const NrnTcBwdArgs* t, const char* who, float* latent_rows = nullptr) {
-  if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
-  if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "%s: bad sizes", who);
-  if (a->out_ch < 4 || a->out_ch > 5) return fail(NRN_E_INVALID, "%s: out_ch=%d unsupported", who, a->out_ch);
-  if (!a->nerf_packed || !a->nerf_grad) return fail(NRN_E_INVALID, "%s: null argument", who);
-  const bool bend = a->bender_packed != nullptr;
-  if (bend && (!a->unmasked_offsets || !a->rigidity_mask || !a->bender_grad || !a->d_latents))
-    return fail(NRN_E_INVALID, "%s: bender needs unmasked_offsets, rigidity_mask, bender_grad, d_latents", who);
-  if (a->n_rays > 0 && !a->relu_mask) return fail(NRN_E_INVALID, "%s: null relu_mask (the ReLU masks of the forward call)", who);
+  long long P;
+  int tiles;
+  int rc = check_field_bwd_args(a, who, &P, &tiles);
+  if (rc) return rc;
   DeviceState* ds;
-  int rc = device_state(&ds);
+  rc = device_state(&ds);
   if (rc) return rc;
   if (ds->num_sms + 16 > nrn::kWgMaxCtas) return fail(NRN_E_INVALID, "%s: %d SMs exceed the scratch layout", who, ds->num_sms);
   cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  const bool bend = a->bender_packed != nullptr;
   const int nerf_n = t ? nrn_nerf_tc_grad_floats(a->out_ch) : nrn_nerf_grad_floats(a->out_ch);
   const int bend_n = bend ? nrn_bender_grad_floats() : 0;
   cudaError_t e;
@@ -569,61 +594,36 @@ static int field_backward(const NrnFieldBwdArgs* a, const NrnTcBwdArgs* t, const
     e = cudaMemsetAsync(a->d_latents, 0, sizeof(float) * static_cast<size_t>(a->n_rays) * nrn::kLatent, st);
     if (e != cudaSuccess) return cuda_fail(e, "memset d_latents");
   }
-  if (a->n_rays == 0) {   // an empty shard contributes zero gradients
-    e = cudaSuccess;
-    if (!a->accumulate_nerf) {
-      const int head_n = a->nerf_grad_head ? a->out_ch * 257 : 0;
-      e = cudaMemsetAsync(a->nerf_grad, 0, sizeof(float) * (nerf_n - head_n), st);
-      if (e == cudaSuccess && head_n) e = cudaMemsetAsync(a->nerf_grad_head, 0, sizeof(float) * head_n, st);
-    }
-    if (e == cudaSuccess && bend && !a->accumulate_bender) e = cudaMemsetAsync(a->bender_grad, 0, sizeof(float) * bend_n, st);
-    return e == cudaSuccess ? NRN_OK : cuda_fail(e, "memset grads");
-  }
-  if (!a->d_raw || !a->stash || !a->grad_stash || !a->wgrad_scratch) return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (P == 0) return zero_grads(a, nerf_n, a->out_ch * 257, bend_n, st);
   float* amax = reinterpret_cast<float*>(ds->err_word + 1);
-  nrn::FieldBwdParams p{};
-  p.P = static_cast<long long>(a->n_rays) * a->n_samples;
-  p.n_tiles = static_cast<int>((p.P + nrn::kTileM - 1) / nrn::kTileM);
-  p.S = a->n_samples; p.n_rays = a->n_rays; p.out_ch = a->out_ch;
-  p.d_raw = a->d_raw; p.amax = amax;
-  p.stash = static_cast<const uint8_t*>(a->stash); p.gstash = static_cast<uint8_t*>(a->grad_stash);
-  p.nerf_wT = static_cast<const uint8_t*>(a->nerf_packed) + nrn::kNerfTOffset;
-  if (bend) p.bend_wT = static_cast<const uint8_t*>(a->bender_packed) + nrn::kBendTOffset;
-  p.unmasked = a->unmasked_offsets; p.rigidity = a->rigidity_mask;
-  p.d_unmasked_up = a->d_unmasked_offsets; p.d_rigid_up = a->d_rigidity_mask;
-  p.cutoff = a->rigidity_cutoff; p.use_cutoff = a->use_cutoff; p.scaling = a->scaling; p.use_scaling = a->use_scaling;
-  p.d_latents = a->d_latents; p.err = ds->err_word;
-  p.relu_mask = static_cast<const uint8_t*>(a->relu_mask);
+  const nrn::FieldBwdParams p = field_bwd_params(a, P, tiles, amax, ds->err_word);
   // DGRAD reads channels 0-3 of d_raw; channel 4 never reaches the loss and must not set the scale
-  e = nrn::launch_absmax(a->d_raw, p.P * a->out_ch, amax, st, false, a->out_ch, 4);
+  e = nrn::launch_absmax(a->d_raw, P * a->out_ch, amax, st, false, a->out_ch, 4);
   // the regularisers' upstream gradients share the fp16 loss scale: they take part in the maximum, otherwise a large
   // offsets_loss_weight saturates them (or, with a vanishing data term, lets them underflow)
-  if (e == cudaSuccess && bend && p.d_unmasked_up) e = nrn::launch_absmax(p.d_unmasked_up, p.P * 3, amax, st, true);
-  if (e == cudaSuccess && bend && p.d_rigid_up) e = nrn::launch_absmax(p.d_rigid_up, p.P, amax, st, true);
+  if (e == cudaSuccess && bend && p.d_unmasked_up) e = nrn::launch_absmax(p.d_unmasked_up, P * 3, amax, st, true);
+  if (e == cudaSuccess && bend && p.d_rigid_up) e = nrn::launch_absmax(p.d_rigid_up, P, amax, st, true);
   if (e != cudaSuccess) return cuda_fail(e, "absmax_kernel");
   if (latent_rows) {
-    { ScopedTimer tm(1, st); e = nrn::launch_field_bwd_det(p, latent_rows, ds->num_sms, st); }
-    if (e != cudaSuccess) return cuda_fail(e, "field_bwd_det_kernel");
-    { ScopedTimer tm(13, st); e = nrn::launch_latent_reduce(latent_rows, a->d_latents, a->n_rays, a->n_samples, st); }
-    if (e != cudaSuccess) return cuda_fail(e, "latent_reduce_kernel");
+    rc = timed(1, st, "field_bwd_det_kernel", [&] { return nrn::launch_field_bwd_det(p, latent_rows, ds->num_sms, st); });
+    if (rc) return rc;
+    rc = timed(13, st, "latent_reduce_kernel", [&] { return nrn::launch_latent_reduce(latent_rows, a->d_latents, a->n_rays, a->n_samples, st); });
   } else {
-    { ScopedTimer tm(1, st); e = nrn::launch_field_bwd(p, bend, ds->num_sms, st); }
-    if (e != cudaSuccess) return cuda_fail(e, "field_bwd_kernel");
+    rc = timed(1, st, "field_bwd_kernel", [&] { return nrn::launch_field_bwd(p, bend, ds->num_sms, st); });
   }
+  if (rc) return rc;
   float* dw_lat = nullptr;
   if (t) {   // per-ray sums of dY0 / dY5 -> d z and the latent columns of dW0 / dW5 (before WGRAD's reduction reads them)
     nrn::TcBwdParams q{};
-    q.gstash = p.gstash; q.amax = amax; q.P = p.P; q.S = p.S; q.n_rays = a->n_rays;
+    q.gstash = p.gstash; q.amax = amax; q.P = P; q.S = p.S; q.n_rays = a->n_rays;
     q.latents = t->latents; q.latent_stride = t->latent_stride; q.w0 = t->w0; q.w5 = t->w5;
     q.sums = t->workspace; q.dw_lat = dw_lat = t->workspace + static_cast<size_t>(a->n_rays) * 2 * 256; q.d_latents = t->d_latents;
-    { ScopedTimer tm(7, st); e = nrn::launch_tc_latent_bwd(q, st); }
-    if (e != cudaSuccess) return cuda_fail(e, "tc_ray_sums_kernel");
+    rc = timed(7, st, "tc_ray_sums_kernel", [&] { return nrn::launch_tc_latent_bwd(q, st); });
+    if (rc) return rc;
   }
-  nrn::WgradParams w{};
-  w.stash = p.stash; w.gstash = p.gstash; w.scratch = a->wgrad_scratch; w.amax = amax; w.n_tiles = p.n_tiles; w.err = ds->err_word;
+  const nrn::WgradParams w = wgrad_params(p.stash, p.gstash, a->wgrad_scratch, amax, tiles, ds->err_word);
   const nrn::WgradDst dst{a->nerf_grad, a->nerf_grad_head, a->bender_grad, nerf_n, bend_n, a->accumulate_nerf, a->accumulate_bender};
-  { ScopedTimer tm(2, st); e = nrn::launch_wgrad(w, bend, ds->num_sms, dst, a->out_ch, st, dw_lat); }
-  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "wgrad_kernel");
+  return timed(2, st, "wgrad_kernel", [&] { return nrn::launch_wgrad(w, bend, ds->num_sms, dst, a->out_ch, st, dw_lat); });
 }
 
 int nrn_field_backward(const NrnFieldBwdArgs* a) { return field_backward(a, nullptr, "nrn_field_backward"); }
@@ -638,13 +638,9 @@ size_t nrn_div_loss_rows_bytes(int n_rays, int n_samples) {
 int nrn_field_backward_det(const NrnFieldBwdArgs* a, float* latent_rows) {
   const char* who = "nrn_field_backward_det";
   if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
-  if (a->n_rays < 0 || a->n_samples < 1) return fail(NRN_E_INVALID, "%s: bad sizes", who);
   if (!a->bender_packed || !a->d_latents)
     return fail(NRN_E_INVALID, "%s: needs a bender (bender_packed) and d_latents: only the bender's latent gradient has a fixed-order variant", who);
   if (a->n_rays == 0) return field_backward(a, nullptr, who);   // an empty shard: zero gradients, no kernel
-  if (!a->d_raw || !a->stash || !a->grad_stash || !a->wgrad_scratch || !a->nerf_packed || !a->nerf_grad || !a->unmasked_offsets ||
-      !a->rigidity_mask || !a->bender_grad)
-    return fail(NRN_E_INVALID, "%s: null argument", who);
   if (!latent_rows || !aligned16(latent_rows)) return fail(NRN_E_INVALID, "%s: null or unaligned latent_rows (nrn_latent_rows_bytes, 16-byte aligned)", who);
   return field_backward(a, nullptr, who, latent_rows);
 }
@@ -658,11 +654,12 @@ int nrn_field_backward_tc(const NrnFieldBwdArgs* a, const NrnTcBwdArgs* t) {
   return field_backward(a, t, "nrn_field_backward_tc");
 }
 
-static long long point_tiles(int n_rays, int n_samples) {
-  return (static_cast<long long>(n_rays) * n_samples + nrn::kTileM - 1) / nrn::kTileM;
+size_t nrn_div_stash_bytes(int n_rays, int n_samples) {
+  return static_cast<size_t>(tile_count(static_cast<long long>(n_rays) * n_samples)) * nrn::kTanTileBytes;
 }
-size_t nrn_div_stash_bytes(int n_rays, int n_samples) { return static_cast<size_t>(point_tiles(n_rays, n_samples)) * nrn::kTanTileBytes; }
-size_t nrn_div_grad_stash_bytes(int n_rays, int n_samples) { return static_cast<size_t>(point_tiles(n_rays, n_samples)) * nrn::kAdjTileBytes; }
+size_t nrn_div_grad_stash_bytes(int n_rays, int n_samples) {
+  return static_cast<size_t>(tile_count(static_cast<long long>(n_rays) * n_samples)) * nrn::kAdjTileBytes;
+}
 
 static int fill_div(const NrnDivArgs* a, nrn::DivParams& p, const char* who) {
   if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
@@ -696,8 +693,7 @@ int nrn_divergence_forward(const NrnDivArgs* a) {
   cudaError_t e = cudaMemsetAsync(a->loss, 0, sizeof(float) * static_cast<size_t>(a->n_rays), st);
   if (e != cudaSuccess) return cuda_fail(e, "memset loss");
   p.loss = a->loss;
-  { ScopedTimer tm(5, st); e = nrn::launch_div_fwd(p, ds->num_sms, st); }
-  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "div_fwd_kernel");
+  return timed(5, st, "div_fwd_kernel", [&] { return nrn::launch_div_fwd(p, ds->num_sms, st); });
 }
 
 int nrn_divergence_forward_det(const NrnDivArgs* a, float* loss_rows) {
@@ -713,11 +709,9 @@ int nrn_divergence_forward_det(const NrnDivArgs* a, float* loss_rows) {
   if (rc) return rc;
   p.err = ds->err_word;
   cudaStream_t st = static_cast<cudaStream_t>(a->stream);
-  cudaError_t e;
-  { ScopedTimer tm(5, st); e = nrn::launch_div_fwd_det(p, loss_rows, ds->num_sms, st); }
-  if (e != cudaSuccess) return cuda_fail(e, "div_fwd_det_kernel");
-  { ScopedTimer tm(14, st); e = nrn::launch_div_loss_reduce(loss_rows, a->loss, a->n_rays, a->n_samples, st); }
-  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "div_loss_reduce_kernel");
+  rc = timed(5, st, "div_fwd_det_kernel", [&] { return nrn::launch_div_fwd_det(p, loss_rows, ds->num_sms, st); });
+  if (rc) return rc;
+  return timed(14, st, "div_loss_reduce_kernel", [&] { return nrn::launch_div_loss_reduce(loss_rows, a->loss, a->n_rays, a->n_samples, st); });
 }
 
 int nrn_divergence_backward(const NrnDivArgs* a) {
@@ -736,14 +730,12 @@ int nrn_divergence_backward(const NrnDivArgs* a) {
   p.d_unmasked = a->d_unmasked_offsets; p.d_rigid = a->d_rigidity_mask; p.err = ds->err_word;
   cudaError_t e = a->G ? nrn::launch_absmax(a->G, p.P, amax, st) : nrn::launch_div_G(p, a->g_ray, a->G_workspace, amax, st);
   if (e != cudaSuccess) return cuda_fail(e, "absmax_kernel");
-  { ScopedTimer tm(5, st); e = nrn::launch_div_bwd(p, ds->num_sms, st); }
-  if (e != cudaSuccess) return cuda_fail(e, "div_bwd_kernel");
-  nrn::WgradParams w{};
-  w.stash = p.tan; w.gstash = p.adj; w.scratch = a->wgrad_scratch; w.amax = amax; w.compact = 1;
-  w.n_tiles = static_cast<int>((p.P + nrn::kTileM - 1) / nrn::kTileM); w.err = ds->err_word;
+  rc = timed(5, st, "div_bwd_kernel", [&] { return nrn::launch_div_bwd(p, ds->num_sms, st); });
+  if (rc) return rc;
+  nrn::WgradParams w = wgrad_params(p.tan, p.adj, a->wgrad_scratch, amax, static_cast<int>(tile_count(p.P)), ds->err_word);
+  w.compact = 1;
   const nrn::WgradDst dst{nullptr, nullptr, a->bender_grad, 0, nrn_bender_grad_floats(), 0, a->accumulate_bender};
-  { ScopedTimer tm(2, st); e = nrn::launch_wgrad(w, true, ds->num_sms, dst, 5, st); }
-  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "wgrad_kernel (divergence)");
+  return timed(2, st, "wgrad_kernel (divergence)", [&] { return nrn::launch_wgrad(w, true, ds->num_sms, dst, 5, st); });
 }
 
 int nrn_ray_loss(const NrnRayLossArgs* a) {

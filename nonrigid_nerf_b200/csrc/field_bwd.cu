@@ -573,11 +573,7 @@ cudaError_t launch_field_bwd_det(const FieldBwdParams& p, float* latent_rows, in
 }
 
 cudaError_t launch_field_bwd_views(const FieldBwdParams& p, const ViewBwdParams& v, int num_sms, cudaStream_t stream) {
-  if (p.n_tiles <= 0) return cudaSuccess;
-  const cudaError_t e = cudaFuncSetAttribute(field_bwd_views_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBwdSmemBytes);
-  if (e != cudaSuccess) return e;
-  field_bwd_views_kernel<<<p.n_tiles < num_sms ? p.n_tiles : num_sms, kFwdThreads, kBwdSmemBytes, stream>>>(p, v);
-  return cudaGetLastError();
+  return launch_field(field_bwd_views_kernel, p, num_sms, kBwdSmemBytes, stream, v);
 }
 
 cudaError_t launch_tc_latent_bwd(const TcBwdParams& p, cudaStream_t stream) {

@@ -581,31 +581,16 @@ cudaError_t launch_field_fwd(const FieldFwdParams& p, bool has_bender, int num_s
 size_t field_views_smem_bytes() { return kFwdSmemBytes - kFwdHBytes; }
 
 cudaError_t launch_field_bend(const FieldFwdParams& p, const ViewParams& v, int num_sms, cudaStream_t stream) {
-  if (p.n_tiles <= 0) return cudaSuccess;
-  const size_t smem = field_fwd_smem_bytes();
-  cudaError_t e = cudaFuncSetAttribute(field_bend_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  field_bend_kernel<<<p.n_tiles < num_sms ? p.n_tiles : num_sms, kFwdThreads, smem, stream>>>(p, v);
-  return cudaGetLastError();
+  return launch_field(field_bend_kernel, p, num_sms, field_fwd_smem_bytes(), stream, v);
 }
 
 cudaError_t launch_field_views(const FieldFwdParams& p, const ViewParams& v, int num_sms, cudaStream_t stream) {
-  if (p.n_tiles <= 0) return cudaSuccess;
-  const size_t smem = field_views_smem_bytes();
-  cudaError_t e = cudaFuncSetAttribute(field_views_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  field_views_kernel<<<p.n_tiles < num_sms ? p.n_tiles : num_sms, kFwdThreads, smem, stream>>>(p, v);
-  return cudaGetLastError();
+  return launch_field(field_views_kernel, p, num_sms, field_views_smem_bytes(), stream, v);
 }
 
 // Training the view-dependent head without a bender: p.stash / p.relu_mask and t's buffers are written
 cudaError_t launch_field_views_train(const FieldFwdParams& p, const ViewParams& v, const ViewTrainParams& t, int num_sms, cudaStream_t stream) {
-  if (p.n_tiles <= 0) return cudaSuccess;
-  const size_t smem = field_views_smem_bytes();
-  cudaError_t e = cudaFuncSetAttribute(field_views_train_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  field_views_train_kernel<<<p.n_tiles < num_sms ? p.n_tiles : num_sms, kFwdThreads, smem, stream>>>(p, v, t);
-  return cudaGetLastError();
+  return launch_field(field_views_train_kernel, p, num_sms, field_views_smem_bytes(), stream, v, t);
 }
 
 cudaError_t launch_field_fwd_tc(const FieldFwdParams& p, int num_sms, cudaStream_t stream) {

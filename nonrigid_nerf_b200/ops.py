@@ -75,33 +75,47 @@ def _views_trunk_params(net):
             [net.pts_linears[i].bias for i in range(8)] + [net.alpha_linear.bias])
 
 
+def _cached_pack(owner, attr: str, params, kind: str, check_shapes, nbytes, pack) -> torch.Tensor:
+    """The packed image of `params`, kept as owner.<attr> = (key, buffer) and rewritten in place when a parameter
+    changed (or while FORCE_PACK is set).  `kind` names the parameters in the error; check_shapes() raises for a
+    geometry the kernels do not implement; pack(lib, buf) writes the image."""
+    key = _versions(params)
+    cache = getattr(owner, attr, None)
+    if cache is not None and cache[0] == key and not FORCE_PACK:
+        return cache[1]
+    for t in params:
+        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
+            raise RuntimeError(f"nonrigid_nerf_b200: {kind} parameters must be contiguous fp32 CUDA tensors")
+    check_shapes()
+    lib = _lib.load()
+    dev = params[0].device
+    buf = cache[1] if cache is not None else torch.empty(nbytes(lib), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        pack(lib, buf)
+    setattr(owner, attr, (key, buf))
+    return buf
+
+
 def pack_nerf(net) -> torch.Tensor:
     """fp16 wgmma operand image of a NeRF module's weights (see csrc/nrn_common.cuh).  With use_viewdirs=True the head
     of the image is alpha_linear in row 3 under three zero rows, so the head step yields alpha in channel 3."""
     views = getattr(net, "use_viewdirs", False)
     ws, bs = _views_trunk_params(net) if views else nerf_param_list(net)
-    key = _versions(ws + bs)
-    cache = getattr(net, "_nrn_pack", None)
-    if cache is not None and cache[0] == key and not FORCE_PACK:
-        return cache[1]
-    lib = _lib.load()
-    for t in ws + bs:
-        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
-            raise RuntimeError("nonrigid_nerf_b200: NeRF parameters must be contiguous fp32 CUDA tensors")
     in_ch = 63 + (LATENT if getattr(net, "time_conditioned_baseline", False) else 0)   # [embedding (| latent)]
-    if ws[0].shape != (256, in_ch) or ws[5].shape != (256, in_ch + 256) or ws[8].shape[1] != 256:
-        raise RuntimeError("nonrigid_nerf_b200: only D=8, W=256, skips=[4], multires=10, use_viewdirs=False is implemented "
-                           f"(got layer shapes {[tuple(w.shape) for w in ws]})")
-    buf = cache[1] if cache is not None else torch.empty(lib.nrn_packed_nerf_bytes(), dtype=torch.uint8, device=ws[0].device)
-    if views:   # [0, 0, 0, alpha]: the head rows of rgb + alpha
-        ws = ws[:8] + [torch.cat([ws[8].new_zeros(3, ws[8].shape[1]), ws[8]], 0)]
-        bs = bs[:8] + [torch.cat([bs[8].new_zeros(3), bs[8]], 0)]
-    out_ch = ws[8].shape[0]
-    with torch.cuda.device(ws[0].device):
-        _lib.check(lib.nrn_pack_nerf(_ptr_array([w.detach() for w in ws]), _ptr_array([b.detach() for b in bs]), in_ch, out_ch,
-                                     _ptr(buf), _stream()), "pack_nerf")
-    net._nrn_pack = (key, buf)
-    return buf
+
+    def check_shapes():
+        if ws[0].shape != (256, in_ch) or ws[5].shape != (256, in_ch + 256) or ws[8].shape[1] != 256:
+            raise RuntimeError("nonrigid_nerf_b200: only D=8, W=256, skips=[4], multires=10, use_viewdirs=False is implemented "
+                               f"(got layer shapes {[tuple(w.shape) for w in ws]})")
+
+    def pack(lib, buf):
+        hw, hb = ws[8], bs[8]
+        if views:   # [0, 0, 0, alpha]: the head rows of rgb + alpha
+            hw, hb = torch.cat([hw.new_zeros(3, hw.shape[1]), hw], 0), torch.cat([hb.new_zeros(3), hb], 0)
+        _lib.check(lib.nrn_pack_nerf(_ptr_array([w.detach() for w in ws[:8] + [hw]]), _ptr_array([b.detach() for b in bs[:8] + [hb]]),
+                                     in_ch, hw.shape[0], _ptr(buf), _stream()), "pack_nerf")
+
+    return _cached_pack(net, "_nrn_pack", ws + bs, "NeRF", check_shapes, lambda lib: lib.nrn_packed_nerf_bytes(), pack)
 
 
 def views_param_list(net):
@@ -110,70 +124,44 @@ def views_param_list(net):
     return ws, bs
 
 
-def pack_views(net) -> torch.Tensor:
-    """fp16 wgmma operand images of the view-dependent head (feature_linear, views_linears.0, rgb_linear)."""
-    ws, bs = views_param_list(net)
-    key = _versions(ws + bs)
-    cache = getattr(net, "_nrn_pack_views", None)
-    if cache is not None and cache[0] == key and not FORCE_PACK:
-        return cache[1]
-    lib = _lib.load()
-    for t in ws + bs:
-        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
-            raise RuntimeError("nonrigid_nerf_b200: NeRF parameters must be contiguous fp32 CUDA tensors")
+def _check_views_shapes(ws):
     if ws[0].shape != (256, 256) or ws[1].shape != (128, 256 + 27) or ws[2].shape != (3, 128):
         raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True needs W=256 and input_ch_views=27 "
                            f"(got view-head shapes {[tuple(w.shape) for w in ws]})")
-    buf = cache[1] if cache is not None else torch.empty(lib.nrn_packed_views_bytes(), dtype=torch.uint8, device=ws[0].device)
-    with torch.cuda.device(ws[0].device):
-        _lib.check(lib.nrn_pack_views(_ptr_array([w.detach() for w in ws]), _ptr_array([b.detach() for b in bs]), _ptr(buf), _stream()),
-                   "pack_views")
-    net._nrn_pack_views = (key, buf)
-    return buf
+
+
+def pack_views(net) -> torch.Tensor:
+    """fp16 wgmma operand images of the view-dependent head (feature_linear, views_linears.0, rgb_linear)."""
+    ws, bs = views_param_list(net)
+    return _cached_pack(net, "_nrn_pack_views", ws + bs, "NeRF", lambda: _check_views_shapes(ws), lambda lib: lib.nrn_packed_views_bytes(),
+                        lambda lib, buf: _lib.check(lib.nrn_pack_views(_ptr_array([w.detach() for w in ws]),
+                                                                       _ptr_array([b.detach() for b in bs]), _ptr(buf), _stream()),
+                                                    "pack_views"))
 
 
 def pack_views_t(net) -> torch.Tensor:
     """fp16 transposed images of the view-dependent head for its backward (rgb_linear, views_linears.0's feature columns,
     feature_linear); cached like pack_views."""
     ws, _ = views_param_list(net)
-    key = _versions(ws)
-    cache = getattr(net, "_nrn_pack_views_t", None)
-    if cache is not None and cache[0] == key and not FORCE_PACK:
-        return cache[1]
-    for t in ws:
-        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
-            raise RuntimeError("nonrigid_nerf_b200: NeRF parameters must be contiguous fp32 CUDA tensors")
-    if ws[0].shape != (256, 256) or ws[1].shape != (128, 256 + 27) or ws[2].shape != (3, 128):
-        raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True needs W=256 and input_ch_views=27 "
-                           f"(got view-head shapes {[tuple(w.shape) for w in ws]})")
-    lib = _lib.load()
-    buf = cache[1] if cache is not None else torch.empty(lib.nrn_packed_views_t_bytes(), dtype=torch.uint8, device=ws[0].device)
-    with torch.cuda.device(ws[0].device):
-        _lib.check(lib.nrn_pack_views_t(_ptr_array([w.detach() for w in ws]), _ptr(buf), _stream()), "pack_views_t")
-    net._nrn_pack_views_t = (key, buf)
-    return buf
+    return _cached_pack(net, "_nrn_pack_views_t", ws, "NeRF", lambda: _check_views_shapes(ws), lambda lib: lib.nrn_packed_views_t_bytes(),
+                        lambda lib, buf: _lib.check(lib.nrn_pack_views_t(_ptr_array([w.detach() for w in ws]), _ptr(buf), _stream()),
+                                                    "pack_views_t"))
 
 
 def pack_bender(bender) -> torch.Tensor:
     net_w, net_b, rig_w, rig_b = bender_param_list(bender)
-    allp = net_w + net_b + rig_w + rig_b
-    key = _versions(allp)
-    cache = getattr(bender, "_nrn_pack", None)
-    if cache is not None and cache[0] == key and not FORCE_PACK:
-        return cache[1]
-    lib = _lib.load()
-    for t in allp:
-        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
-            raise RuntimeError("nonrigid_nerf_b200: ray_bending parameters must be contiguous fp32 CUDA tensors")
-    if net_w[0].shape != (64, 3 + LATENT):
-        raise RuntimeError("nonrigid_nerf_b200: only ray_bending_latent_size=32, simple_neural is implemented")
-    buf = cache[1] if cache is not None else torch.empty(lib.nrn_packed_bender_bytes(), dtype=torch.uint8, device=net_w[0].device)
-    with torch.cuda.device(net_w[0].device):
+
+    def check_shapes():
+        if net_w[0].shape != (64, 3 + LATENT):
+            raise RuntimeError("nonrigid_nerf_b200: only ray_bending_latent_size=32, simple_neural is implemented")
+
+    def pack(lib, buf):
         _lib.check(lib.nrn_pack_bender(_ptr_array([t.detach() for t in net_w]), _ptr_array([t.detach() for t in net_b]),
                                        _ptr_array([t.detach() for t in rig_w]), _ptr_array([t.detach() for t in rig_b]),
                                        LATENT, _ptr(buf), _stream()), "pack_bender")
-    bender._nrn_pack = (key, buf)
-    return buf
+
+    return _cached_pack(bender, "_nrn_pack", net_w + net_b + rig_w + rig_b, "ray_bending", check_shapes,
+                        lambda lib: lib.nrn_packed_bender_bytes(), pack)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -221,71 +209,91 @@ def tc_ray_bias(net, latents: torch.Tensor, stride: int) -> torch.Tensor:
     return rb
 
 
-def _field(rays, z_vals, points, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details, stash=None, relu_mask=None,
-           tc_net=None):
+def _rays8(rays: torch.Tensor) -> torch.Tensor:
+    """rays [N, 8+] as the kernels read them: fp32 rows of 8 floats (o, d, near, far), 8 floats apart."""
+    if not rays.is_cuda:
+        raise RuntimeError("nonrigid_nerf_b200: rays must be a CUDA tensor (there is no CPU path)")
+    if rays.dtype == torch.float32 and rays.stride(-1) == 1 and rays.stride(0) == 8:
+        return rays
+    return rays[:, :8].float().contiguous()
+
+
+def _field_args(rays, z_vals, points, n_samples, latents, nerf_pack, bender_pack, out_ch, knobs, want_raw, want_details):
+    """NrnFieldArgs of one field call.  Ray mode: rays [N, 8+] and z_vals [N, S]; point mode: points [N * n_samples, 3+],
+    n_samples consecutive points forming one ray.  `latents` (None: not read) are those of each ray, or each point in
+    point mode; knobs = (cutoff, scaling, removal).  raw [N, S, out_ch] (when want_raw) and the details are allocated here.
+    Returns (args, raw, details, keep): keep holds the converted inputs the args point into (the latent rows last, when
+    latents are given) and must live until the call is enqueued."""
     a = _lib.NrnFieldArgs()
-    keep = []
     if points is None:
-        rays = _f32c(rays, "rays")
-        z_vals = _f32c(z_vals, "z_vals")
+        rays, z_vals = _rays8(rays), _f32c(z_vals, "z_vals")
         n, s = z_vals.shape
-        dev = rays.device
         a.rays, a.z_vals = rays.data_ptr(), z_vals.data_ptr()
-        keep += [rays, z_vals]
+        keep = [rays, z_vals]
     else:
         if not points.is_cuda:
             raise RuntimeError("nonrigid_nerf_b200: points must be a CUDA tensor (there is no CPU path)")
         if points.dtype != torch.float32 or points.dim() != 2 or points.stride(1) != 1:
             points = points.reshape(points.shape[0], -1).float().contiguous()
-        n, s = points.shape[0], 1
-        dev = points.device
+        s = n_samples
+        if points.shape[0] % s:
+            raise RuntimeError(f"nonrigid_nerf_b200: use_viewdirs=True: {points.shape[0]} points do not form rays of num_ray_samples={s}")
+        n = points.shape[0] // s
         a.points, a.points_stride = points.data_ptr(), points.stride(0)
-        keep.append(points)
-    a.n_rays, a.n_samples = n, s
+        keep = [points]
+    dev = keep[0].device
+    a.n_rays, a.n_samples, a.out_ch = n, s, out_ch
     a.nerf_packed = nerf_pack.data_ptr()
-    ray_bias = None
     if bender_pack is not None:
-        if latents is None:
-            raise RuntimeError("nonrigid_nerf_b200: ray bending needs latents")
-        latents, stride = latent_rows(latents, n, dev)
-        a.latents, a.latent_stride = latents.data_ptr(), stride
         a.bender_packed = bender_pack.data_ptr()
+    if latents is not None:
+        latents, a.latent_stride = latent_rows(latents, n * s if points is not None else n, dev)
+        a.latents = latents.data_ptr()
         keep.append(latents)
-    elif tc_net is not None:   # time-conditioned baseline: the latents enter as per-ray biases of L0 and L5
-        if latents is None:
-            raise RuntimeError("nonrigid_nerf_b200: time_conditioned_baseline needs latents")
-        latents, stride = latent_rows(latents, n, dev)
-        a.latents, a.latent_stride = latents.data_ptr(), stride
-        ray_bias = tc_ray_bias(tc_net, latents, stride)
-        keep += [latents, ray_bias]
-    a.out_ch = out_ch
+    cutoff, scaling, removal = knobs
     if cutoff is not None:
         a.use_cutoff, a.rigidity_cutoff = 1, float(cutoff)
     if scaling is not None:
         a.use_scaling, a.scaling = 1, float(scaling)
     if removal is not None:
         a.use_removal, a.removal_threshold = 1, float(removal)
-    raw = torch.empty(n, s, out_ch, dtype=torch.float32, device=dev)
-    a.raw = raw.data_ptr()
+    raw = None
+    if want_raw:
+        raw = torch.empty(n, s, out_ch, dtype=torch.float32, device=dev)
+        a.raw = raw.data_ptr()
     details: Dict[str, torch.Tensor] = {}
     if want_details:
-        details["initial_input_pts"] = torch.empty(n, s, 3, dtype=torch.float32, device=dev)
-        details["input_pts"] = torch.empty(n, s, 3, dtype=torch.float32, device=dev)
-        a.initial_input_pts, a.input_pts = details["initial_input_pts"].data_ptr(), details["input_pts"].data_ptr()
-        if bender_pack is not None:
-            details["unmasked_offsets"] = torch.empty(n, s, 3, dtype=torch.float32, device=dev)
-            details["masked_offsets"] = torch.empty(n, s, 3, dtype=torch.float32, device=dev)
-            details["rigidity_mask"] = torch.empty(n, s, 1, dtype=torch.float32, device=dev)
-            a.unmasked_offsets = details["unmasked_offsets"].data_ptr()
-            a.masked_offsets = details["masked_offsets"].data_ptr()
-            a.rigidity_mask = details["rigidity_mask"].data_ptr()
+        names = ["initial_input_pts", "input_pts"] + (["unmasked_offsets", "masked_offsets", "rigidity_mask"] if bender_pack is not None else [])
+        for k in names:
+            details[k] = torch.empty(n, s, 1 if k == "rigidity_mask" else 3, dtype=torch.float32, device=dev)
+            setattr(a, k, details[k].data_ptr())
+    a.stream = torch.cuda.current_stream().cuda_stream
+    return a, raw, details, keep
+
+
+def _viewdirs(viewdirs: Optional[torch.Tensor], dev) -> Tuple[torch.Tensor, int]:
+    """The view directions [N, 3+] as fp32 rows on `dev`, and their row stride in floats."""
+    if viewdirs is None:
+        raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True without a ray bender needs the view directions")
+    if viewdirs.dtype != torch.float32 or viewdirs.dim() != 2 or viewdirs.stride(1) != 1 or not viewdirs.is_cuda:
+        viewdirs = viewdirs.reshape(viewdirs.shape[0], -1).float().contiguous().to(dev)
+    return viewdirs, viewdirs.stride(0) if viewdirs.shape[0] > 1 else 3
+
+
+def _field(rays, z_vals, points, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details, stash=None, relu_mask=None,
+           tc_net=None):
+    tc = tc_net if bender_pack is None else None   # time-conditioned baseline: the latents enter as per-ray biases of L0 and L5
+    if latents is None and (bender_pack is not None or tc is not None):
+        raise RuntimeError("nonrigid_nerf_b200: " + ("ray bending" if tc is None else "time_conditioned_baseline") + " needs latents")
+    a, raw, details, keep = _field_args(rays, z_vals, points, 1, latents if bender_pack is not None or tc is not None else None, nerf_pack,
+                                        bender_pack, out_ch, (cutoff, scaling, removal), True, want_details)
     if stash is not None:
         a.stash = stash.data_ptr()
     if relu_mask is not None:
         a.relu_mask = relu_mask.data_ptr()
-    a.stream = torch.cuda.current_stream().cuda_stream
-    with torch.cuda.device(dev):
-        if ray_bias is not None:
+    with torch.cuda.device(keep[0].device):
+        if tc is not None:
+            ray_bias = tc_ray_bias(tc, keep[-1], a.latent_stride)
             _lib.check(_lib.load().nrn_field_forward_tc(C.byref(a), _ptr(ray_bias)), "field_forward_tc")
         else:
             _lib.check(_lib.load().nrn_field_forward(C.byref(a)), "field_forward")
@@ -322,76 +330,21 @@ def field_forward_views(rays: Optional[torch.Tensor], z_vals: Optional[torch.Ten
     differences of the bent points run inside each), latents per point.  With a bender the view directions are those
     differences; without one `viewdirs` (per ray, or per point in point mode) is used.  views_pack = None with a bender
     runs the bend pass alone (raw is None; the details are filled)."""
-    a = _lib.NrnFieldArgs()
-    v = _lib.NrnViewArgs()
-    keep = []
-    if points is None:
-        rays = rays if (rays.dtype == torch.float32 and rays.stride(-1) == 1) else rays.float().contiguous()
-        if not rays.is_cuda:
-            raise RuntimeError("nonrigid_nerf_b200: rays must be a CUDA tensor (there is no CPU path)")
-        z_vals = _f32c(z_vals, "z_vals")
-        n, s = z_vals.shape
-        dev = rays.device
-        if rays.stride(0) != 8:
-            rays = rays[:, :8].contiguous()
-        a.rays, a.z_vals = rays.data_ptr(), z_vals.data_ptr()
-        keep += [rays, z_vals]
-    else:
-        if not points.is_cuda:
-            raise RuntimeError("nonrigid_nerf_b200: points must be a CUDA tensor (there is no CPU path)")
-        if points.dtype != torch.float32 or points.dim() != 2 or points.stride(1) != 1:
-            points = points.reshape(points.shape[0], -1).float().contiguous()
-        s = n_samples
-        if points.shape[0] % s:
-            raise RuntimeError(f"nonrigid_nerf_b200: use_viewdirs=True: {points.shape[0]} points do not form rays of num_ray_samples={s}")
-        n = points.shape[0] // s
-        dev = points.device
-        a.points, a.points_stride = points.data_ptr(), points.stride(0)
-        keep.append(points)
-    a.n_rays, a.n_samples = n, s
-    a.nerf_packed = nerf_pack.data_ptr()
+    if bender_pack is not None and latents is None:
+        raise RuntimeError("nonrigid_nerf_b200: ray bending needs latents")
+    a, raw, details, keep = _field_args(rays, z_vals, points, n_samples, latents if bender_pack is not None else None, nerf_pack,
+                                        bender_pack, 4, (cutoff, scaling, removal), views_pack is not None, want_details)
+    n, s, dev = a.n_rays, a.n_samples, keep[0].device
     lib = _lib.load()
+    v = _lib.NrnViewArgs()
     if bender_pack is not None:
-        if latents is None:
-            raise RuntimeError("nonrigid_nerf_b200: ray bending needs latents")
-        latents, stride = latent_rows(latents, n * s if points is not None else n, dev)
-        a.latents, a.latent_stride = latents.data_ptr(), stride
-        a.bender_packed = bender_pack.data_ptr()
         ws = torch.empty(lib.nrn_views_workspace_bytes(n, s), dtype=torch.uint8, device=dev)
         v.workspace = ws.data_ptr()
-        keep += [latents, ws]
     else:
-        if viewdirs is None:
-            raise RuntimeError("nonrigid_nerf_b200: use_viewdirs=True without a ray bender needs the view directions")
-        if viewdirs.dtype != torch.float32 or viewdirs.dim() != 2 or viewdirs.stride(1) != 1 or not viewdirs.is_cuda:
-            viewdirs = viewdirs.reshape(viewdirs.shape[0], -1).float().contiguous().to(dev)
-        v.viewdirs, v.viewdirs_stride = viewdirs.data_ptr(), viewdirs.stride(0) if viewdirs.shape[0] > 1 else 3
-        keep.append(viewdirs)
-    a.out_ch = 4
-    if cutoff is not None:
-        a.use_cutoff, a.rigidity_cutoff = 1, float(cutoff)
-    if scaling is not None:
-        a.use_scaling, a.scaling = 1, float(scaling)
-    if removal is not None:
-        a.use_removal, a.removal_threshold = 1, float(removal)
-    raw = None
+        viewdirs, v.viewdirs_stride = _viewdirs(viewdirs, dev)
+        v.viewdirs = viewdirs.data_ptr()
     if views_pack is not None:
-        raw = torch.empty(n, s, 4, dtype=torch.float32, device=dev)
-        a.raw = raw.data_ptr()
         v.views_packed = views_pack.data_ptr()
-    details: Dict[str, torch.Tensor] = {}
-    if want_details:
-        details["initial_input_pts"] = torch.empty(n, s, 3, dtype=torch.float32, device=dev)
-        details["input_pts"] = torch.empty(n, s, 3, dtype=torch.float32, device=dev)
-        a.initial_input_pts, a.input_pts = details["initial_input_pts"].data_ptr(), details["input_pts"].data_ptr()
-        if bender_pack is not None:
-            details["unmasked_offsets"] = torch.empty(n, s, 3, dtype=torch.float32, device=dev)
-            details["masked_offsets"] = torch.empty(n, s, 3, dtype=torch.float32, device=dev)
-            details["rigidity_mask"] = torch.empty(n, s, 1, dtype=torch.float32, device=dev)
-            a.unmasked_offsets = details["unmasked_offsets"].data_ptr()
-            a.masked_offsets = details["masked_offsets"].data_ptr()
-            a.rigidity_mask = details["rigidity_mask"].data_ptr()
-    a.stream = torch.cuda.current_stream().cuda_stream
     with torch.cuda.device(dev):
         _lib.check(lib.nrn_field_forward_views(C.byref(a), C.byref(v)), "field_forward_views")
     return raw, details
@@ -401,34 +354,17 @@ def field_forward_views_train(rays: torch.Tensor, z_vals: torch.Tensor, viewdirs
                               views_pack: torch.Tensor, want_details: bool = False):
     """The view-dependent head without a bender, keeping what its backward needs: raw [N, S, 4], details, and the buffers
     (stash, relu_mask, views_stash, hv_mask)."""
-    rays = rays if (rays.dtype == torch.float32 and rays.stride(-1) == 1) else rays.float().contiguous()
-    if not rays.is_cuda:
-        raise RuntimeError("nonrigid_nerf_b200: rays must be a CUDA tensor (there is no CPU path)")
-    if rays.stride(0) != 8:
-        rays = rays[:, :8].contiguous()
-    z_vals = _f32c(z_vals, "z_vals")
-    n, s = z_vals.shape
-    dev = rays.device
-    if viewdirs.dtype != torch.float32 or viewdirs.dim() != 2 or viewdirs.stride(1) != 1 or not viewdirs.is_cuda:
-        viewdirs = viewdirs.reshape(viewdirs.shape[0], -1).float().contiguous().to(dev)
+    a, raw, details, keep = _field_args(rays, z_vals, None, 1, None, nerf_pack, None, 4, (None, None, None), True, want_details)
+    n, s, dev = a.n_rays, a.n_samples, keep[0].device
     lib = _lib.load()
     bufs = {k: torch.empty(f(n, s), dtype=torch.uint8, device=dev) for k, f in (
         ("stash", lib.nrn_stash_bytes), ("relu_mask", lib.nrn_relu_mask_bytes), ("views_stash", lib.nrn_views_stash_bytes),
         ("hv_mask", lib.nrn_hv_mask_bytes))}
-    a, v, t = _lib.NrnFieldArgs(), _lib.NrnViewArgs(), _lib.NrnViewTrainArgs()
-    a.rays, a.z_vals, a.n_rays, a.n_samples, a.out_ch = rays.data_ptr(), z_vals.data_ptr(), n, s, 4
-    a.nerf_packed = nerf_pack.data_ptr()
-    raw = torch.empty(n, s, 4, dtype=torch.float32, device=dev)
-    a.raw = raw.data_ptr()
-    details: Dict[str, torch.Tensor] = {}
-    if want_details:
-        details["initial_input_pts"] = torch.empty(n, s, 3, dtype=torch.float32, device=dev)
-        details["input_pts"] = torch.empty(n, s, 3, dtype=torch.float32, device=dev)
-        a.initial_input_pts, a.input_pts = details["initial_input_pts"].data_ptr(), details["input_pts"].data_ptr()
     a.stash, a.relu_mask = bufs["stash"].data_ptr(), bufs["relu_mask"].data_ptr()
-    a.stream = torch.cuda.current_stream().cuda_stream
+    v, t = _lib.NrnViewArgs(), _lib.NrnViewTrainArgs()
     v.views_packed = views_pack.data_ptr()
-    v.viewdirs, v.viewdirs_stride = viewdirs.data_ptr(), viewdirs.stride(0) if viewdirs.shape[0] > 1 else 3
+    viewdirs, v.viewdirs_stride = _viewdirs(viewdirs, dev)
+    v.viewdirs = viewdirs.data_ptr()
     t.views_stash, t.hv_mask = bufs["views_stash"].data_ptr(), bufs["hv_mask"].data_ptr()
     with torch.cuda.device(dev):
         _lib.check(lib.nrn_field_forward_views_train(C.byref(a), C.byref(v), C.byref(t)), "field_forward_views_train")

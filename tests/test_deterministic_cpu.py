@@ -64,6 +64,11 @@ def test_field_backward_det_validates_its_arguments():
     bad(a, p, b"relu_mask")
     a = _bwd_args(p); a.out_ch = 6
     bad(a, p, b"out_ch=6")
+    for name in ("nerf_packed", "stash", "grad_stash", "relu_mask"):
+        a = _bwd_args(p); setattr(a, name, p.value + 4)
+        bad(a, p, b"16-byte aligned")
+    a = _bwd_args(p); a.n_rays = a.n_samples = 0x7fffffff
+    bad(a, p, b"nrn_field_backward_det: too many points")
 
 
 def test_divergence_forward_det_validates_its_arguments():
