@@ -47,3 +47,16 @@ def rays8(r, device):
     near = torch.full((n, 1), float(r["near"]))
     far = torch.full((n, 1), float(r["far"]))
     return torch.cat([r["rays_o"], r["rays_d"], near, far], -1).to(device)
+
+
+def tc_models(seed, device):
+    """(coarse, fine) NeRF(time_conditioned_baseline=True) modules with tests/tc_reference's case-L parameters (W0 [256][95],
+    W5 [256][351]), and those parameter dicts (cp, fp)."""
+    from nonrigid_nerf_b200 import run_nerf_helpers as H
+    from tests import tc_reference as R
+    cp, fp = R.make_params(seed)
+    kw = dict(D=8, W=256, input_ch=63, output_ch=5, skips=[4], input_ch_views=0, use_viewdirs=False, ray_bender=None,
+              ray_bending_latent_size=32, time_conditioned_baseline=True)
+    coarse = load_nerf_module(H.NeRF(num_ray_samples=64, **kw), cp).to(device)
+    fine = load_nerf_module(H.NeRF(num_ray_samples=128, **kw), fp).to(device)
+    return coarse, fine, (cp, fp)

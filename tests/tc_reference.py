@@ -25,14 +25,14 @@ def query(npar, pts: torch.Tensor, latents: torch.Tensor) -> torch.Tensor:
 
 def render_rays(cp, fp, rays_o, rays_d, near, far, latents, s_c=64, n_imp=64, perturb=False, raw_noise_std=0.0, rnd=None):
     """render_rays (train.py:792-980) with the time-conditioned coarse / fine NeRFs and no bender."""
-    n = rays_o.shape[0]
-    near_t = torch.full((n, 1), float(near))
-    far_t = torch.full((n, 1), float(far))
+    n, dev = rays_o.shape[0], rays_o.device
+    near_t = torch.full((n, 1), float(near), device=dev)
+    far_t = torch.full((n, 1), float(far), device=dev)
     z = O.stratified_z(near_t, far_t, s_c, rnd["t_rand"] if perturb else None)
     raw = query(cp, rays_o[:, None, :] + rays_d[:, None, :] * z[:, :, None], latents)
     noise_c = rnd["noise_c"] * raw_noise_std if raw_noise_std > 0 else None
     rgb0, _, acc0, _, w, _ = O.raw2outputs(raw, z, rays_d, noise_c)
-    u = rnd["u"] if perturb else O.det_u(n, n_imp)
+    u = rnd["u"] if perturb else O.det_u(n, n_imp, dev)
     z_samples = O.sample_pdf(0.5 * (z[:, 1:] + z[:, :-1]), w[:, 1:-1], u).detach()
     z_f, _ = torch.sort(torch.cat([z, z_samples], -1), -1)
     raw = query(fp, rays_o[:, None, :] + rays_d[:, None, :] * z_f[:, :, None], latents)
@@ -46,10 +46,17 @@ def training_loss(g, cp, fp, latent_table: torch.Tensor):
     render (perturb = 1, raw_noise_std = 1), fine + coarse image terms."""
     seed, n = int(g["seed"]), int(g["n"])
     r = O.make_rays(seed, n)
-    rnd = O.make_randomness(seed, n, 64, 64)
-    lat = latent_table[torch.from_numpy(g["i2t"])[torch.from_numpy(g["pix"])[:, 0]], :]
-    ret = render_rays(cp, fp, r["rays_o"], r["rays_d"], r["near"], r["far"], lat, perturb=True, raw_noise_std=1.0, rnd=rnd)
-    return O.training_loss(ret, r["target"])
+    return training_loss_rays(cp, fp, r, latent_table, g["i2t"], torch.from_numpy(g["pix"]), O.make_randomness(seed, n, 64, 64))
+
+
+def training_loss_rays(cp, fp, rays, latent_table: torch.Tensor, imageid_to_timestepid, pixel_indices: torch.Tensor, rnd):
+    """training_loss on given rays (rays_o, rays_d, near, far, target), injected random draws, (image, y, x) pixel indices
+    and latent table, on their device."""
+    i2t = torch.as_tensor(imageid_to_timestepid, device=pixel_indices.device)
+    lat = latent_table[i2t[pixel_indices[:, 0]], :]
+    ret = render_rays(cp, fp, rays["rays_o"], rays["rays_d"], rays["near"], rays["far"], lat, perturb=True, raw_noise_std=1.0,
+                      rnd=rnd)
+    return O.training_loss(ret, rays["target"])
 
 
 def rel(a, b) -> float:

@@ -202,7 +202,7 @@ def _setup(seed, n, s_c=64, n_imp=64, n_images=86):
 def _setup_tc(seed, n):
     """The time-conditioned baseline (no bender) with a trainable latent table, optim.Adam."""
     from nonrigid_nerf_b200 import optim, parallel
-    from tests import test_time_conditioned_gpu as TC
+    from tests import helpers, test_time_conditioned_gpu as TC
     g = TC._golden()
     r = O.make_rays(seed, n)
     rnd = {k: v.to(DEV) for k, v in O.make_randomness(seed, n, 64, 64).items()}
@@ -212,7 +212,7 @@ def _setup_tc(seed, n):
     pix = torch.stack([torch.randint(0, n_images, (n,), generator=gen), torch.randint(0, 384, (n,), generator=gen),
                        torch.randint(0, 512, (n,), generator=gen)], 1).to(DEV)
     torch.manual_seed(seed)
-    coarse, fine, _ = TC._models(seed)
+    coarse, fine, _ = helpers.tc_models(seed, DEV)
     params = latents + list(coarse.parameters()) + list(fine.parameters())
     opt = optim.Adam(params, lr=5e-4)
     wrapper = parallel.training_wrapper_class(coarse, latents, fine_model=fine, ray_bender=None)

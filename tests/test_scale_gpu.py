@@ -1,6 +1,10 @@
 """The fused training kernels at the benchmark's cfg4 batch (8192 rays: 4,096 coarse and 8,192 fine tiles, stashes past
-2^31 and 2^32 bytes) and at 53,248 x 128 points (ReLU masks past 2^31 bytes, divergence stashes past 2^32), stage by
-stage against the fp64 references of tests/stage_reference.py, with the bounds of tests/test_stage_parity_gpu.py.
+2^31 and 2^32 bytes), at 53,248 x 128 points (ReLU masks past 2^31 bytes, divergence stashes past 2^32) and at
+52,480 x 128 (DGRAD and WGRAD on masks past 2^31), stage by stage against the fp64 references of
+tests/stage_reference.py, with the bounds of tests/test_stage_parity_gpu.py.  The cfg4 passes, the coverage sweep, the
+52,480 x 128 case and the render chunk run for the bending model and for the time-conditioned baseline (the latent as a
+per-ray bias of L0 / L5; its per-ray sums of dY0 / dY5, d z and the latent columns of W0 / W5 are checked too, and
+WGRAD runs the bender-less plan and wgrad_reduce_tc_kernel).
 
 Every stage is row-local, so it is checked on sampled tiles: 0 and T - 1, the tiles whose byte range in some buffer holds
 byte 2^31 or 2^32 and their neighbours (from the library's per-tile sizes), and the tiles of the persistent CTAs' first
@@ -19,7 +23,15 @@ and last grid sweep.  WGRAD sums over every tile; it is checked twice:
             it: a tile dropped, repeated or read from the wrong address fails by two orders of magnitude, where the
             dense check's relative L2 cannot see it (one tile of 8,192 moves a gradient by about 1.2e-4).
 The divergence kernels' compact WGRAD gets the same sweep, with g_ray non-zero only on the rays of the pass's tiles.
-DGRAD reading masks past 2^31 would need a 33 GB gradient stash on top of the forward stash; it is not run here.
+  52,480 x 128  the smallest shape whose masks pass 2^31 bytes (51 of its 52,480 tiles lie past tile 52,428, which holds
+            byte 2^31); stash 33.3 GB, gradient stash 32.5 GB, masks 2.15 GB, 63.3 GiB in all, skipped with the GiB it
+            needs when the device has less free.  Forward, DGRAD and the gradient-stash statistics on the tiles at the
+            2^31 .. 2^34 boundaries of all three buffers, dense WGRAD, then a second backward on the same forward stash
+            with upstreams only on those tiles, every WGRAD element at c_wgrad(len(tiles)): the dense relative L2 moves
+            by about 2e-5 for one misaddressed tile of 52,480, this check by orders of magnitude.
+The latent columns of W0 / W5 (tc_dw_lat_kernel, one fp32 FMA per ray) are held per element to c_latent_columns(n) and,
+in the dense checks, to the relative L2 bound of the plan: one ray left out stays inside the per-element worst case at
+8,192 rays but moves the columns by about 1 / sqrt(n).
 
 Beyond single kernels:
   render chunk   render() at 65,536 rays (64 + 64 samples, the render workload's settings): 40 sampled rays equal a
@@ -32,7 +44,8 @@ Beyond single kernels:
 
 Every caller-owned buffer is filled with 0xFF before the calls, as in the stage test.
 
-Measured on one H100 80GB HBM3 (700 W power limit, 132 SMs), printed with `pytest -s`; the file runs in about 45 s.
+Measured on one H100 80GB HBM3 (700 W power limit, 132 SMs), printed with `pytest -s`; the file runs in about 45 s, the
+52,480 x 128 cases in 4 to 6 s each (two runs), with 80 GB on the card.
   worst c_obs   forward H1 .. H8 and raw at most 6.32 of c = 322 (H6); bender steps 0.92 of 98; DGRAD dY0 .. dY7 4.94 of
                 258, dY7 2.41 of 18; bender DGRAD 2.56 of 82; divergence chains at most 9.7 of 64 (t2), closed forms
                 4.0 of 16; WGRAD dense 61.6 of c = 131,136 (W0, 8,192 tiles), swept 8.06 of 1,424, divergence compact
@@ -47,8 +60,17 @@ Measured on one H100 80GB HBM3 (700 W power limit, 132 SMs), printed with `pytes
   cfg4 step     per-ray loss 2.3e-6 L-inf, 3.0e-6 relative L2; gradients at most 1.64e-2 (coarse W0) for the NeRF
                 layers, 2.5e-4 for the heads, 3.0e-2 for the bender, 4.1e-2 for the latent table
   graph replay  relative L2 to eager 0 to 3.2e-7 per step; two eager runs differ by 3.2e-7
+  52,480 x 128  worst c_obs H1 .. H8 5.62 of 322 (H6), dY0 .. dY7 3.02 of 258, dY7 1.67 of 18, bender DGRAD 1.07 of 82;
+                WGRAD dense 134.5 of c = 839,744 (W0), on the boundary tiles only 7.43 of 592; dense relative L2 at most
+                1.86e-3 (W0, bending; deepest split 13,120 tiles, bound 7.8e-3) and 1.55e-3 (W5, time-conditioned;
+                10,496 tiles, bound 6.3e-3)
+  time-cond.    at 8,192 x 64 / 128 worst c_obs ray bias 4.48 of 34, H1 .. H8 4.67 of 322, dY0 .. dY7 2.45 of 258,
+                per-ray sums 0.69 of 130, d z 7.81 of 514, dense WGRAD 44.9 of 131,136, swept 6.39 of 1,424; the latent
+                columns of W0 / W5 3.56 of c_latent_columns(8,192) = 32,776 (5.83 swept) and 3.98 of 209,928 at 52,480
+                rays, relative L2 1.6e-6 and 4.1e-6; the render chunk's compositing 13.0 of 592
 """
 import copy
+import time
 
 import pytest
 import torch
@@ -94,18 +116,19 @@ def tile_set(cs, m, j):
     return [t for t in range(j, cs.T, m)]
 
 
-def only_on_tiles(cs, m, j):
-    """cs with d_raw and the regulariser upstreams zero on every point outside the tiles t = j (mod m), and g_ray zero on
-    every ray that does not lie inside one of them."""
-    pt_tile = torch.arange(cs.P, device=DEV) // SL.TILE_M
-    keep = (pt_tile % m == j)
+def only_on_tiles(cs, tiles):
+    """cs with d_raw and the regulariser upstreams zero on every point outside the listed tiles, and g_ray zero on every
+    ray that does not lie inside one of them."""
+    on = torch.zeros(cs.T, dtype=torch.bool, device=DEV)
+    on[torch.tensor(tiles, dtype=torch.long, device=DEV)] = True
+    keep = on[torch.arange(cs.P, device=DEV) // SL.TILE_M]
     c = copy.copy(cs)
     c.d_raw = cs.d_raw * keep[:, None]
     c.d_un_up = None if cs.d_un_up is None else cs.d_un_up * keep[:, None]
     c.d_rig_up = None if cs.d_rig_up is None else cs.d_rig_up * keep
     ray = torch.arange(cs.n, device=DEV)
     first, last = ray * cs.s // SL.TILE_M, ((ray + 1) * cs.s - 1) // SL.TILE_M
-    c.g_ray = cs.g_ray * ((first % m == j) & (first == last))
+    c.g_ray = cs.g_ray * (on[first] & (first == last))
     return c
 
 
@@ -113,7 +136,7 @@ def grad_stash_stats(cs, o, b, tag):
     """Saturation of every gradient-stash image, and the share of the trunk's gradients dY0 .. dY7 that flush to fp16 zero
     or subnormal where their ReLU mask bit is set (a zero there is not the mask's)."""
     g_max, n_on, n_zero, n_sub = 0.0, 0, 0, 0
-    chunks = SL.GRAD_TILE // SL.CHUNK
+    chunks = (SL.GRAD_TILE if cs.bender else SL.GS_YB4[0]) // SL.CHUNK    # without a bender no dYb image is written
     for t0 in range(0, cs.T, BLOCK):
         sub = Tiles(cs, range(t0, min(t0 + BLOCK, cs.T)))
         g_max = max(g_max, float(sub.img(b["gstash"], SL.GRAD_TILE, (0, chunks)).float().abs().max()))
@@ -140,7 +163,7 @@ def dense_wgrad(cs, o, b, rep, scale):
             tot = refs
         else:
             for d, r in zip(tot, refs):
-                for k, (v, a) in r.items():
+                for k, (v, a) in (r or {}).items():          # no bender: no bender sums
                     d[k] = (d[k][0] + v, d[k][1] + a)
     sms = torch.cuda.get_device_properties(DEV).multi_processor_count
     plan = wgrad_plan(cs.T, sms & ~1, cs.bender)
@@ -153,7 +176,11 @@ def dense_wgrad(cs, o, b, rep, scale):
 SHAPES = {
     "8192x64_div": dict(n=8192, s=64),       # cfg4's coarse pass: stash and gradient stash past 2^31
     "8192x128": dict(n=8192, s=128),         # cfg4's fine pass: both past 2^32
+    # the time-conditioned baseline's passes: every sampled tile holds whole rays, so their per-ray sums are checked
+    "8192x64_tc": dict(n=8192, s=64, bender=False, tc=True),
+    "8192x128_tc": dict(n=8192, s=128, bender=False, tc=True),
 }
+MODELS = {"bender": dict(), "tc": dict(bender=False, tc=True)}   # the bending model and the time-conditioned baseline
 
 
 @pytest.mark.parametrize("name", list(SHAPES))
@@ -175,23 +202,35 @@ def test_cfg4_pass_every_stage_on_sampled_tiles_and_dense_wgrad(name):
         check_divergence(cs, o, d, rep, tiles, wgrad=False)
 
 
-def test_every_tile_enters_every_wgrad_job_exactly_once():
-    """cfg4's fine pass: M_SWEEP backward passes on one forward stash, each with upstreams on one residue class of tiles."""
-    cs = Case(8192, 128)
+def wgrad_sweep(model):
+    """cfg4's fine pass of `model` (a key of MODELS): M_SWEEP backward passes on one forward stash, each with upstreams on
+    one residue class of tiles."""
+    cs = Case(8192, 128, **MODELS[model])
     o = run_forward(cs)
-    rep = Report(f"8192x128 sweep m={M_SWEEP}", quiet=True)
+    rep = Report(f"{model} 8192x128 sweep m={M_SWEEP}", quiet=True)
     for j in range(M_SWEEP):
-        cj = only_on_tiles(cs, M_SWEEP, j)
+        cj = only_on_tiles(cs, tile_set(cs, M_SWEEP, j))
         b = run_backward(cj, o)
         imgs = dgrad_reference(cj, o, b, rep, expected_scale(cj), tile_set(cs, M_SWEEP, j))
         check_wgrad(cj, b, imgs, rep, expected_scale(cj))
     rep.worst()
 
 
+def test_every_tile_enters_every_wgrad_job_exactly_once():
+    """The bending model's fine pass at cfg4: every WGRAD job of the plan with a bender."""
+    wgrad_sweep("bender")
+
+
+def test_every_tile_enters_every_tc_wgrad_job_exactly_once():
+    """The time-conditioned baseline's fine pass at cfg4: the bender-less plan and wgrad_reduce_tc_kernel, the latent
+    columns of W0 / W5 from the pass's rays only."""
+    wgrad_sweep("tc")
+
+
 def divergence_sweep(cs, o, d, m, tag):
     rep = Report(tag, quiet=True)
     for j in range(m):
-        cj = only_on_tiles(cs, m, j)
+        cj = only_on_tiles(cs, tile_set(cs, m, j))
         run_divergence_backward(cj, o, d)
         check_divergence(cj, o, d, rep, tile_set(cs, m, j))
     rep.worst()
@@ -234,6 +273,46 @@ def test_masks_past_2_31_and_divergence_stashes_past_2_32():
           f"adjoint {lib.nrn_div_grad_stash_bytes(n, s)} B")
 
 
+@pytest.mark.parametrize("model", list(MODELS))
+def test_dgrad_and_wgrad_on_masks_past_2_31(model):
+    """52,480 x 128 points, the smallest shape whose ReLU masks (2.15 GB) pass 2^31 bytes, forward and backward: the stash
+    (33.3 GB) and gradient stash (32.5 GB) past 2^34.  Every stage on the tiles at the byte boundaries of all three
+    buffers (and the persistent CTAs' last sweep, which straddles the masks' 2^31); dense WGRAD; then a second backward
+    on the same forward stash with upstreams only on those tiles, whose WGRAD is checked per element at
+    c_wgrad(len(tiles)): one tile read from the wrong place fails it by orders of magnitude, where the dense relative L2
+    moves by about 2e-5."""
+    n, s = 52480, 128
+    lib = _lib().load()
+    need = lib.nrn_stash_bytes(n, s) + lib.nrn_relu_mask_bytes(n, s) + lib.nrn_grad_stash_bytes(n, s) + (3 << 30)
+    torch.cuda.empty_cache()      # what earlier tests left in the caching allocator is free for this case
+    free, _ = torch.cuda.mem_get_info()
+    if free < need:
+        pytest.skip(f"needs {need / 2 ** 30:.1f} GiB of device memory, {free / 2 ** 30:.1f} GiB free")
+    assert lib.nrn_relu_mask_bytes(n, s) > 2 ** 31 and lib.nrn_grad_stash_bytes(n, s) > 2 ** 34
+    t_start = time.perf_counter()
+    cs = Case(n, s, **MODELS[model])
+    tag = f"{model} {n}x{s}"
+    rep = Report(tag)
+    tiles = sample_tiles(cs, ("stash", "masks", "grad stash"))
+    print(f"  [{tag}] {cs.T} tiles; sampled {tiles}")
+    o = run_forward(cs)
+    check_forward(cs, o, rep, tiles)
+    b = run_backward(cs, o)
+    scale = expected_scale(cs)
+    dgrad_reference(cs, o, b, rep, scale, tiles)
+    grad_stash_stats(cs, o, b, tag)
+    dense_wgrad(cs, o, b, Report(f"{tag} dense"), scale)
+    del b
+    cj = only_on_tiles(cs, tiles)
+    b = run_backward(cj, o)
+    rep = Report(f"{tag} upstream on the sampled tiles only")
+    scale = expected_scale(cj)
+    check_wgrad(cj, b, dgrad_reference(cj, o, b, rep, scale, tiles), rep, scale)
+    torch.cuda.synchronize()
+    print(f"  [{tag}] ran: stash {lib.nrn_stash_bytes(n, s)} B, masks {lib.nrn_relu_mask_bytes(n, s)} B, gradient stash "
+          f"{lib.nrn_grad_stash_bytes(n, s)} B; {time.perf_counter() - t_start:.1f} s")
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 # inference at the render chunk, and the whole cfg4 training step
 # ----------------------------------------------------------------------------------------------------------------------
@@ -245,10 +324,12 @@ def f32_bits_equal(a, b):
     return a.shape == b.shape and torch.equal(a.contiguous().view(torch.int32), b.contiguous().view(torch.int32))
 
 
-def test_render_chunk_rays_equal_a_small_call_and_composite_within_fp64_bounds():
-    """render() at one 65,536-ray chunk as the render workload runs it (64 coarse + 64 importance samples, perturb 0, no
-    noise, one latent row for every ray, detailed output): 98,304 fine tiles per field launch.  Sampled rays (the first,
-    the last, those of the persistent CTAs' first and last sweep, and random ones) equal a separate call on just those
+def render_chunk(model):
+    """render() of `model` (a key of MODELS) at one 65,536-ray chunk as the render workload runs it (64 coarse + 64
+    importance samples, perturb 0, no noise, one latent row for every ray, detailed output): 98,304 fine tiles per field
+    launch; for the time-conditioned baseline that broadcast latent is a single ray-bias row for every ray.  Sampled rays
+    (the first, the last, those of the persistent CTAs' first and last sweep, and random ones) equal a separate call on
+    just those
     rays bit for bit, every per-ray and per-sample output included; and the fine compositing of those rays holds the fp64
     bounds of tests/test_ray_kernels_parity_gpu.py on the kernel's own raw and alpha."""
     import oracle.nrnerf_oracle as O
@@ -256,7 +337,11 @@ def test_render_chunk_rays_equal_a_small_call_and_composite_within_fp64_bounds()
     from tests import helpers, ray_reference as RR
     from tests.test_ray_kernels_parity_gpu import UNDERFLOW, c_scan
     n, S = 65536, 128
-    coarse, fine, bender, _ = helpers.build_models(O, SEED_STEP, DEV)
+    if model == "tc":
+        coarse, fine, _ = helpers.tc_models(SEED_STEP, DEV)
+        bender = None
+    else:
+        coarse, fine, bender, _ = helpers.build_models(O, SEED_STEP, DEV)
     r = O.make_rays(SEED_STEP, n)
     ro, rd = r["rays_o"].to(DEV), r["rays_d"].to(DEV)
     lat = r["latents"][0].to(DEV)
@@ -286,12 +371,22 @@ def test_render_chunk_rays_equal_a_small_call_and_composite_within_fp64_bounds()
     for k, v in full.items():
         if v.is_floating_point() and v.shape[0] == n:
             assert f32_bits_equal(v[sel], small[k]), f"{k}: the {n}-ray chunk differs from a {sel.shape[0]}-ray call"
-    print(f"  [render {n} rays] {sel.shape[0]} sampled rays equal a separate call bit for bit in {len(full)} outputs")
-    rep = Report(f"render {n} rays, sampled")
+    print(f"  [{model} render {n} rays] {sel.shape[0]} sampled rays equal a separate call bit for bit in {len(full)} outputs")
+    rep = Report(f"{model} render {n} rays, sampled")
     raw, alpha = small["raw"], small["fine_opacity_alpha"]
     ref = RR.composite_ref(alpha, raw, torch.zeros_like(alpha))          # depth and disp need z, which render() keeps
     for k, got in (("weights", small["fine_visibility_weights"]), ("rgb", small["rgb_map"]), ("acc", small["acc_map"])):
         rep.check(f"fine {k}", got, *ref[k], c_scan(S + 64), floor=UNDERFLOW)
+
+
+def test_render_chunk_rays_equal_a_small_call_and_composite_within_fp64_bounds():
+    """The bending model's render chunk (render_chunk)."""
+    render_chunk("bender")
+
+
+def test_tc_render_chunk_rays_equal_a_small_call_and_composite_within_fp64_bounds():
+    """The time-conditioned baseline's render chunk (render_chunk): one ray-bias row serves all 65,536 rays."""
+    render_chunk("tc")
 
 
 def cfg4_setup(seed, n, n_iters):

@@ -28,16 +28,6 @@ def _golden():
     return np.load(os.path.join(GOLD, "caseL_time_conditioned.npz"))
 
 
-def _models(seed):
-    from nonrigid_nerf_b200 import run_nerf_helpers as H
-    cp, fp = R.make_params(seed)
-    kw = dict(D=8, W=256, input_ch=63, output_ch=5, skips=[4], input_ch_views=0, use_viewdirs=False, ray_bender=None,
-              ray_bending_latent_size=32, time_conditioned_baseline=True)
-    coarse = helpers.load_nerf_module(H.NeRF(num_ray_samples=64, **kw), cp).to(DEV)
-    fine = helpers.load_nerf_module(H.NeRF(num_ray_samples=128, **kw), fp).to(DEV)
-    return coarse, fine, (cp, fp)
-
-
 def _kwargs(coarse, fine, r, rnd=None, perturb=0.0, noise=0.0):
     kw = {"network_query_fn": None, "perturb": perturb, "N_importance": 64, "network_fine": fine, "N_samples": 64,
           "network_fn": coarse, "ray_bender": None, "use_viewdirs": False, "white_bkgd": False, "raw_noise_std": noise,
@@ -59,7 +49,7 @@ def test_render_and_point_mode_match_golden_and_oracle():
     from nonrigid_nerf_b200 import _lib
     g = _golden()
     seed, n = int(g["seed"]), int(g["n"])
-    coarse, fine, (cp, fp) = _models(seed)
+    coarse, fine, (cp, fp) = helpers.tc_models(seed, DEV)
     r = O.make_rays(seed, n)
     lat = torch.from_numpy(g["latents"])
     rgb, acc, extras = _render(coarse, fine, r, lat.to(DEV))
@@ -89,7 +79,7 @@ def test_render_and_point_mode_match_golden_and_oracle():
 def test_broadcast_latent_and_chunking_are_exact():
     g = _golden()
     seed, n = int(g["seed"]), int(g["n"])
-    coarse, fine, _ = _models(seed)
+    coarse, fine, _ = helpers.tc_models(seed, DEV)
     r = O.make_rays(seed, n)
     row = torch.from_numpy(g["latents"][3]).to(DEV)
     rgb_b, acc_b, ex_b = _render(coarse, fine, r, row[None, :].expand(n, 32))        # stride 0: one ray-bias row
@@ -105,7 +95,7 @@ def test_broadcast_latent_and_chunking_are_exact():
 
 def test_ray_bias_matches_fp64():
     from nonrigid_nerf_b200 import ops
-    coarse, _, _ = _models(R.SEED)
+    coarse, _, _ = helpers.tc_models(R.SEED, DEV)
     lat = torch.randn(300, 32, generator=torch.Generator().manual_seed(3)).to(DEV)
     rb = ops.tc_ray_bias(coarse, lat, lat.stride(0))
     w0, b0 = coarse.pts_linears[0].weight.detach().double(), coarse.pts_linears[0].bias.detach().double()
@@ -124,7 +114,7 @@ def test_per_ray_sums_latent_gradient_and_latent_columns_match_fp64():
     import ctypes as C
     from nonrigid_nerf_b200 import _lib, ops
     lib = _lib.load()
-    coarse, _, _ = _models(R.SEED)
+    coarse, _, _ = helpers.tc_models(R.SEED, DEV)
     n, s, out_ch = 40, 96, 5
     gen = torch.Generator().manual_seed(5)
     r = O.make_rays(7, n)
@@ -187,7 +177,7 @@ def _targs(**over):
 def _run_wrapper(g, use_arena):
     from nonrigid_nerf_b200 import _lib, optim, parallel
     seed, n = int(g["seed"]), int(g["n"])
-    coarse, fine, _ = _models(seed)
+    coarse, fine, _ = helpers.tc_models(seed, DEV)
     r = O.make_rays(seed, n)
     rnd = dict(O.make_randomness(seed, n, 64, 64))
     latents = [torch.from_numpy(row.copy()).to(DEV).requires_grad_(True) for row in g["latent_table"]]
@@ -244,7 +234,7 @@ def test_training_wrapper_loss_and_gradients_match_golden_fresh_and_arena():
 
 def test_two_backward_passes_are_bit_identical():
     from nonrigid_nerf_b200 import autograd as ag, ops
-    coarse, _, _ = _models(R.SEED)
+    coarse, _, _ = helpers.tc_models(R.SEED, DEV)
     n, s = 50, 80
     gen = torch.Generator().manual_seed(9)
     rays = helpers.rays8(O.make_rays(11, n), DEV)
@@ -277,7 +267,7 @@ def test_cuda_graph_replay_matches_eager_training_step():
     i2t = {"imageid_to_timestepid": [int(v) for v in g["i2t"]]}
     losses = {}
     for mode in ("eager", "graph"):
-        coarse, fine, _ = _models(seed)
+        coarse, fine, _ = helpers.tc_models(seed, DEV)
         opt = optim.Adam(list(coarse.parameters()) + list(fine.parameters()), lr=5e-4)
         wrapper = parallel.training_wrapper_class(coarse, latents, fine_model=fine, ray_bender=None)
         kw = _kwargs(coarse, fine, r, rnd, 1.0, 1.0)

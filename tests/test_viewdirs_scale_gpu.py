@@ -106,7 +106,7 @@ def test_every_tile_enters_every_views_wgrad_job_exactly_once():
     o = run_forward(cs)
     rep = Report(f"views 8192x128 sweep m={M_SWEEP}", quiet=True)
     for j in range(M_SWEEP):
-        cj = only_on_tiles(cs, M_SWEEP, j)
+        cj = only_on_tiles(cs, tile_set(cs, M_SWEEP, j))
         b = run_backward(cj, o)
         scale = expected_scale(cj)
         imgs = dgrad_reference(cj, o, b, rep, scale, tile_set(cs, M_SWEEP, j))
