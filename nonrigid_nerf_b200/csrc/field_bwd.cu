@@ -26,7 +26,7 @@ namespace {
 
 constexpr int kBwdStageLd = 66;   // floats per staged row (64 used)
 // Gradient images in shared memory: only the bender chain's (A operands of B4^T..B0^T, at most 96 columns).  The trunk's
-// 256-wide gradients stay in registers (epi_mask_frag), so the rest of shared memory goes to the weight ring.
+// 256-wide gradients stay in registers (epi_grad_frag), so the rest of shared memory goes to the weight ring.
 constexpr int kBwdActBytes = kGsYb1.chunks * kChunkBytes;   // 24 KB
 static_assert(kGsYb4.chunks <= kGsYb1.chunks && kGsYb3.chunks <= kGsYb1.chunks && kGsYb2.chunks <= kGsYb1.chunks &&
               kGsYb0.chunks <= kGsYb1.chunks, "bender gradient images fit act");
@@ -75,25 +75,50 @@ __device__ __forceinline__ void epi_mask_store(const float (&acc)[NR], const Rel
   }
 }
 
-// The same for a 256-wide trunk gradient that stays in registers: dY = dh * [h > 0] as fp16 -> the next step's A fragments
-// `a`, and the same fp16 pairs straight to this warpgroup's rows of the tile's gradient-stash image `gs_img` (a warp's 32
-// words of one column group and row half are one contiguous 128-byte line of the chunk-major image).
-__device__ __forceinline__ void epi_mask_frag(const float (&acc)[kMaskHCols / 2], const ReluMask<kMaskHCols>& m,
-                                              uint32_t (&a)[kMaskHCols / 16][4], uint8_t* gs_img, int g) {
+// The same for a gradient that stays in registers: NCOLS accumulator columns as fp16 (MASK: dY = dh * [h > 0] with the
+// forward's ReLU mask bits `m`) -> the next step's A fragments `a` (wg_gemm_rs), and the same fp16 pairs straight to this
+// warpgroup's rows of the tile's gradient-stash image `gs_img` (a warp's 32 words of one column group and row half are one
+// contiguous 128-byte line of the chunk-major image).
+template <int NCOLS, bool MASK, int NR>
+__device__ __forceinline__ void epi_grad_frag(const float (&acc)[NR], const ReluMask<NCOLS>& m, uint32_t (&a)[NCOLS / 16][4],
+                                              uint8_t* gs_img, int g) {
   const int r0 = g * kWgRows + acc_r0(), q = acc_q();
 #pragma unroll
-  for (int j = 0; j < kMaskHCols / 8; ++j) {
+  for (int j = 0; j < NCOLS / 8; ++j) {
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-      const uint32_t g2 = m.apply(i, j, pack_h2_sat(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]));
+      uint32_t g2 = pack_h2_sat(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+      if constexpr (MASK) g2 = m.apply(i, j, g2);
       frag_pair(a, j, i) = g2;
       *reinterpret_cast<uint32_t*>(gs_img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = g2;
     }
   }
 }
 
-__device__ __forceinline__ float h_lo(uint32_t w) { return __half2float(__ushort_as_half(static_cast<unsigned short>(w & 0xffffu))); }
-__device__ __forceinline__ float h_hi(uint32_t w) { return __half2float(__ushort_as_half(static_cast<unsigned short>(w >> 16))); }
+// A = d_raw [4 channels, 0 ...] (K = 16) of this warpgroup's rows, times the loss scale and clamped to fp16: one register
+// fragment built from global memory (lanes q < 2 hold columns 2q, 2q + 1 of rows r0, r0 + 8; every other word is zero,
+// rows past P too), and the same words -> the tile's kGsRaw image, its zero columns and zero second chunk included (A of
+// WGRAD's head and rgb_linear jobs)
+__device__ __forceinline__ void d_raw_frag(const FieldBwdParams& p, int tile, float scale, uint8_t* gs, int g, uint32_t (&a)[1][4]) {
+  const int r0 = g * kWgRows + acc_r0(), q = acc_q();
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const long long pti = static_cast<long long>(tile) * kTileM + r0 + 8 * i;
+    float g0 = 0.f, g1 = 0.f;
+    if (q < 2 && pti < p.P) {
+      const float* src = p.d_raw + pti * p.out_ch + 2 * q;
+      g0 = clamp_h(__ldg(src) * scale);
+      g1 = clamp_h(__ldg(src + 1) * scale);
+    }
+    a[0][i] = q < 2 ? pack_h2(g0, g1) : 0u;
+    a[0][2 + i] = 0u;
+  }
+#pragma unroll
+  for (int j = 0; j < 2; ++j)
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+      *reinterpret_cast<uint32_t*>(gs + kGsRaw.off + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = frag_pair(a, j, i);
+}
 
 // Backward of the positional encoding: dx_d += dE[d] + sum_k 2^k (dE[sin_kd] cos_kd - dE[cos_kd] sin_kd)
 // de: this row's 64 staged accumulator columns; sin/cos: the forward embedding stashed as fp16.
@@ -115,24 +140,6 @@ __device__ __forceinline__ void pe_backward(const float* de, const uint8_t* __re
       acc += f * (de[3 + 6 * k + d] * c - de[3 + 6 * k + 3 + d] * s);
     }
     dx[d] += acc;
-  }
-}
-
-// View head (training without a bender): NCOLS accumulator columns as fp16 (MASK: times the forward's ReLU mask bits `m`)
-// -> the next step's A fragments `a` and this warpgroup's rows of the view gradient-stash image `gs_img`
-template <int NCOLS, bool MASK, int NR>
-__device__ __forceinline__ void epi_views_frag(const float (&acc)[NR], const ReluMask<NCOLS>& m, uint32_t (&a)[NCOLS / 16][4],
-                                               uint8_t* gs_img, int g) {
-  const int r0 = g * kWgRows + acc_r0(), q = acc_q();
-#pragma unroll
-  for (int j = 0; j < NCOLS / 8; ++j) {
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      uint32_t g2 = pack_h2_sat(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-      if constexpr (MASK) g2 = m.apply(i, j, g2);
-      frag_pair(a, j, i) = g2;
-      *reinterpret_cast<uint32_t*>(gs_img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = g2;
-    }
   }
 }
 
@@ -218,32 +225,13 @@ __device__ __forceinline__ void field_bwd_body(const FieldBwdParams& p, float* l
     {
       static_assert(dgrad::step(dgrad::HeadT).N == kTrunk.N && dgrad::step(dgrad::HeadT).nslabs == 1 &&
                     dgrad::step(dgrad::HeadT).k16 == 1 && kGsRaw.chunks == 2, "head^T: one K = 16 MMA");
-      const int r0 = g * kWgRows + acc_r0(), q = acc_q();
       uint32_t a[1][4];
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        // lanes q < 2 hold columns 2q, 2q + 1 of rows r0, r0 + 8; every other word is zero (rows past P too)
-        const long long pti = static_cast<long long>(tile) * kTileM + r0 + 8 * i;
-        float g0 = 0.f, g1 = 0.f;
-        if (q < 2 && pti < p.P) {
-          const float* src = p.d_raw + pti * p.out_ch + 2 * q;
-          g0 = clamp_h(__ldg(src) * scale);
-          g1 = clamp_h(__ldg(src + 1) * scale);
-        }
-        a[0][i] = q < 2 ? pack_h2(g0, g1) : 0u;
-        a[0][2 + i] = 0u;
-      }
-      // the same words -> the kGsRaw image (its zero columns and zero second chunk included)
-#pragma unroll
-      for (int j = 0; j < 2; ++j)
-#pragma unroll
-        for (int i = 0; i < 2; ++i)
-          *reinterpret_cast<uint32_t*>(gs + kGsRaw.off + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = frag_pair(a, j, i);
+      d_raw_frag(p, tile, scale, gs, g, a);
       Acc<dgrad::HeadT> acc;
       ReluMask<kMaskHCols> m;
       m.load(mk + kMkH + 7 * kMaskHBytes, g);
       wg_gemm_rs<kTrunk.N, 1>(acc, a, ring, false, 0u, W, 300);
-      epi_mask_frag(acc, m, h, gs + kGsY + 7 * kHBytes, g);
+      epi_grad_frag<kMaskHCols, true>(acc, m, h, gs + kGsY + 7 * kHBytes, g);
     }
     float dx[3] = {0.f, 0.f, 0.f};
     // ---- L7^T, L6^T : dY6, dY5 ----
@@ -254,7 +242,7 @@ __device__ __forceinline__ void field_bwd_body(const FieldBwdParams& p, float* l
       m.load(mk + kMkH + (6 - s) * kMaskHBytes, g);
       wg_gemm_rs<kTrunk.N, kTrunk.k16>(acc, h, ring, false, 0u, W, 301 + s);
       if (s == 1) prefetch_e();
-      epi_mask_frag(acc, m, h, gs + kGsY + (6 - s) * kHBytes, g);
+      epi_grad_frag<kMaskHCols, true>(acc, m, h, gs + kGsY + (6 - s) * kHBytes, g);
     }
     // ---- L5e^T: gradient into the skip-connected embedding; h (dY5) stays as it is for L5h^T ----
     {
@@ -273,7 +261,7 @@ __device__ __forceinline__ void field_bwd_body(const FieldBwdParams& p, float* l
       m.load(mk + kMkH + (4 - s) * kMaskHBytes, g);
       wg_gemm_rs<kTrunk.N, kTrunk.k16>(acc, h, ring, false, 0u, W, 304 + s);
       if (s == 4) prefetch_e();
-      epi_mask_frag(acc, m, h, gs + kGsY + (4 - s) * kHBytes, g);
+      epi_grad_frag<kMaskHCols, true>(acc, m, h, gs + kGsY + (4 - s) * kHBytes, g);
     }
     // ---- L0^T: gradient into the embedding; then through the bend ----
     {
@@ -448,39 +436,21 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_views_kernel(const F
     uint8_t* vgs = v.vgstash + static_cast<long long>(tile) * kVGradTileBytes;
     const uint8_t* mk = p.relu_mask + static_cast<long long>(tile) * kMaskTileBytes;
     uint32_t h[kMaskHCols / 16][4];
-    // ---- A = d_raw [g_r g_g g_b g_alpha 0 ...] (K = 16), one fragment built from global memory, as field_bwd_kernel ----
-    const int r0 = g * kWgRows + acc_r0(), q = acc_q();
+    // ---- A = d_raw [g_r g_g g_b g_alpha 0 ...] (K = 16) ----
     uint32_t a[1][4];
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const long long pti = static_cast<long long>(tile) * kTileM + r0 + 8 * i;
-      float g0 = 0.f, g1 = 0.f;
-      if (q < 2 && pti < p.P) {
-        const float* src = p.d_raw + pti * p.out_ch + 2 * q;
-        g0 = clamp_h(__ldg(src) * scale);
-        g1 = clamp_h(__ldg(src + 1) * scale);
-      }
-      a[0][i] = q < 2 ? pack_h2(g0, g1) : 0u;
-      a[0][2 + i] = 0u;
-    }
-    // the same words -> the kGsRaw image (A of WGRAD's head and rgb_linear jobs)
-#pragma unroll
-    for (int j = 0; j < 2; ++j)
-#pragma unroll
-      for (int i = 0; i < 2; ++i)
-        *reinterpret_cast<uint32_t*>(gs + kGsRaw.off + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = frag_pair(a, j, i);
+    d_raw_frag(p, tile, scale, gs, g, a);
     uint32_t dyv[kVgYv.chunks / 2][4];
     {   // ---- Rgb^T: dhv = d_raw . rgb_linear (channel 3 meets a zero column) -> dYv = dhv * [hv > 0] ----
       Acc<vdgrad::RgbT> acc;
       ReluMask<kMkHv.cols> m;
       m.load(v.hv_mask + static_cast<long long>(tile) * kHvMaskTileBytes, g);
       wg_gemm_rs<kRgbT.N, 1>(acc, a, ring, false, 0u, W, 320);
-      epi_views_frag<kMkHv.cols, true>(acc, m, dyv, vgs + kVgYv.off, g);
+      epi_grad_frag<kMkHv.cols, true>(acc, m, dyv, vgs + kVgYv.off, g);
     }
     {   // ---- ViewsF^T: dF = dYv . views_linears.0[:, :256] (feature_linear has no ReLU) ----
       Acc<vdgrad::ViewsFT> acc;
       wg_gemm_rs<kViewsFT.N, kViewsFT.k16>(acc, dyv, ring, false, 0u, W, 321);
-      epi_views_frag<kMaskHCols, false>(acc, ReluMask<kMaskHCols>{}, h, vgs + kVgF.off, g);
+      epi_grad_frag<kMaskHCols, false>(acc, ReluMask<kMaskHCols>{}, h, vgs + kVgF.off, g);
     }
     {   // ---- Feature^T + head^T into one accumulator: dh8 = dF . feature_linear + d_alpha alpha_linear -> dY7 ----
       Acc<vdgrad::FeatureT> acc;
@@ -488,7 +458,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_views_kernel(const F
       m.load(mk + kMkH + 7 * kMaskHBytes, g);
       wg_gemm_rs<kTrunk.N, kTrunk.k16>(acc, h, ring, false, 0u, W, 322);
       wg_gemm_rs<kTrunk.N, 1, 1, true>(acc, a, ring, false, 0u, W, 300);
-      epi_mask_frag(acc, m, h, gs + kGsY + 7 * kHBytes, g);
+      epi_grad_frag<kMaskHCols, true>(acc, m, h, gs + kGsY + 7 * kHBytes, g);
     }
     // ---- L7^T, L6^T : dY6, dY5; then L5h^T, L4^T .. L1^T : dY4 .. dY0 (one shape) ----
 #pragma unroll 1
@@ -498,7 +468,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_views_kernel(const F
       ReluMask<kMaskHCols> m;
       m.load(mk + kMkH + l * kMaskHBytes, g);
       wg_gemm_rs<kTrunk.N, kTrunk.k16>(acc, h, ring, false, 0u, W, 301 + s);
-      epi_mask_frag(acc, m, h, gs + kGsY + l * kHBytes, g);
+      epi_grad_frag<kMaskHCols, true>(acc, m, h, gs + kGsY + l * kHBytes, g);
     }
   }
 }
@@ -527,8 +497,8 @@ __global__ void __launch_bounds__(256) tc_ray_sums_kernel(const TcBwdParams p) {
     const uint32_t wv[4] = {w.x, w.y, w.z, w.w};
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
-      acc[2 * q] += __half2float(__ushort_as_half(static_cast<unsigned short>(wv[q] & 0xffffu)));
-      acc[2 * q + 1] += __half2float(__ushort_as_half(static_cast<unsigned short>(wv[q] >> 16)));
+      acc[2 * q] += h_lo(wv[q]);
+      acc[2 * q + 1] += h_hi(wv[q]);
     }
   }
   float* dst = p.sums + static_cast<long long>(ray) * 512 + l * 256 + c * 8;

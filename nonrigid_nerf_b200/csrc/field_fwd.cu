@@ -35,7 +35,7 @@ namespace {
 
 constexpr int kFwdStageLd = 12;   // floats per staged row (8 used)
 // Activations in shared memory: the bender's hidden images (A operands of B1..B4, at most 96 columns) and E.  The trunk's
-// 256-wide activations stay in registers (epi_bias_relu_frag), so the rest of shared memory goes to the weight ring.
+// 256-wide activations stay in registers (epi_bias_frag), so the rest of shared memory goes to the weight ring.
 constexpr int kFwdHBytes = kStHb1.chunks * kChunkBytes;   // 24 KB
 static_assert(kStHb2.chunks <= kStHb1.chunks && kStHb3.chunks <= kStHb1.chunks && kStHb4.chunks <= kStHb1.chunks, "bender images fit H");
 constexpr int kFwdRingStages = 5;
@@ -83,35 +83,52 @@ __device__ __forceinline__ void epi_bias_relu_store(const float (&acc)[NR], cons
   if constexpr (MASK) m.store(mask_tile + mask_off, g);
 }
 
-// The same for a 256-wide trunk layer whose output stays in registers: bias, ReLU, fp16 -> the next step's A fragments
-// `a`.  TRAIN: also the mask bits, and the fp16 pairs straight to this warpgroup's rows of the tile's stash image `st_img`
-// (a warp's 32 words of one column group and row half are one contiguous 128-byte line of the chunk-major image).
-// ROW_BIAS (time-conditioned L0 / L5): accumulator rows r0 and r0 + 8 take their biases from their own rows `bias` and
-// `bias8` (their rays' ray-bias rows) instead of one vector.
-template <bool TRAIN, bool ROW_BIAS = false>
-__device__ __forceinline__ void epi_bias_relu_frag(const float (&acc)[kMaskHCols / 2], const float* __restrict__ bias,
-                                                   uint32_t (&a)[kMaskHCols / 16][4], uint8_t* st_img, int g,
-                                                   uint8_t* mask_tile, int mask_off, const float* __restrict__ bias8 = nullptr) {
+// The same for a layer whose output stays in registers: accumulator columns [0, NCOLS) + bias (RELU: then ReLU), fp16
+// with saturation -> the next step's A fragments `a`.  TRAIN: also the fp16 pairs straight to this warpgroup's rows of the
+// tile's stash image `st_img` (a warp's 32 words of one column group and row half are one contiguous 128-byte line of the
+// chunk-major image), and with RELU the mask bits of those elements -> this thread's words of the tile's mask image
+// `mask_img`.  ROW_BIAS (time-conditioned L0 / L5): accumulator rows r0 and r0 + 8 take their biases from their own rows
+// `bias` and `bias8` (their rays' ray-bias rows) instead of one vector.
+template <int NCOLS, bool RELU, bool TRAIN, bool ROW_BIAS = false>
+__device__ __forceinline__ void epi_bias_frag(const float (&acc)[NCOLS / 2], const float* __restrict__ bias, uint32_t (&a)[NCOLS / 16][4],
+                                              uint8_t* st_img, int g, uint8_t* mask_img = nullptr,
+                                              const float* __restrict__ bias8 = nullptr) {
   const int r0 = g * kWgRows + acc_r0(), q = acc_q();
-  ReluMask<kMaskHCols> m;
-  if constexpr (TRAIN) m.clear();
+  ReluMask<NCOLS> m;
+  if constexpr (TRAIN && RELU) m.clear();
 #pragma unroll
-  for (int j = 0; j < kMaskHCols / 8; ++j) {
+  for (int j = 0; j < NCOLS / 8; ++j) {
     const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * q));
     float2 b8 = b;
     if constexpr (ROW_BIAS) b8 = __ldg(reinterpret_cast<const float2*>(bias8 + 8 * j + 2 * q));
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const float2 bi = i ? b8 : b;
-      const uint32_t h2 = pack_h2_relu_sat(acc[4 * j + 2 * i] + bi.x, acc[4 * j + 2 * i + 1] + bi.y);
+      const float u = acc[4 * j + 2 * i] + bi.x, v = acc[4 * j + 2 * i + 1] + bi.y;
+      const uint32_t h2 = RELU ? pack_h2_relu_sat(u, v) : pack_h2_sat(u, v);
       frag_pair(a, j, i) = h2;
       if constexpr (TRAIN) {
-        m.pack(i, j, h2);
+        if constexpr (RELU) m.pack(i, j, h2);
         *reinterpret_cast<uint32_t*>(st_img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = h2;
       }
     }
   }
-  if constexpr (TRAIN) m.store(mask_tile + mask_off, g);
+  if constexpr (TRAIN && RELU) m.store(mask_img, g);
+}
+
+// The floats f as fp16 -> chunks 0 .. NF / 8 - 1 of a chunk-major image row
+template <int NF>
+__device__ __forceinline__ void pack_row(const float (&f)[NF], uint8_t* dst_row) {
+  static_assert(NF % 8 == 0, "whole 8-column chunks");
+#pragma unroll
+  for (int c = 0; c < NF / 8; ++c) {
+    uint4 pk;
+    pk.x = pack_h2(f[c * 8 + 0], f[c * 8 + 1]);
+    pk.y = pack_h2(f[c * 8 + 2], f[c * 8 + 3]);
+    pk.z = pack_h2(f[c * 8 + 4], f[c * 8 + 5]);
+    pk.w = pack_h2(f[c * 8 + 6], f[c * 8 + 7]);
+    *reinterpret_cast<uint4*>(dst_row + c * kChunkBytes) = pk;
+  }
 }
 
 // Positional encoding of one point (Embedder.embed, run_nerf_helpers.py:149-150 with the settings of
@@ -145,15 +162,7 @@ __device__ __forceinline__ void write_pe(const float (&x)[3], uint8_t* dst_row) 
   float f[64];
   encode_octaves<10>(x, f);
   f[63] = 1.f;  // pad column: its weight column is zero (forward unaffected); WGRAD reads it as the bias input
-#pragma unroll
-  for (int c = 0; c < 8; ++c) {
-    uint4 pk;
-    pk.x = pack_h2(f[c * 8 + 0], f[c * 8 + 1]);
-    pk.y = pack_h2(f[c * 8 + 2], f[c * 8 + 3]);
-    pk.z = pack_h2(f[c * 8 + 4], f[c * 8 + 5]);
-    pk.w = pack_h2(f[c * 8 + 6], f[c * 8 + 7]);
-    *reinterpret_cast<uint4*>(dst_row + c * kChunkBytes) = pk;
-  }
+  pack_row(f, dst_row);
 }
 
 // Direction encoding of the view-dependent head (embeddirs_fn, get_embedder(multires_views = 4): d, then sin(2^k d),
@@ -163,41 +172,7 @@ __device__ __forceinline__ void write_dir_enc(const float (&d)[3], uint8_t* dst_
   encode_octaves<4>(d, f);
 #pragma unroll
   for (int i = views::kDirCols; i < 32; ++i) f[i] = 0.f;
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
-    uint4 pk;
-    pk.x = pack_h2(f[c * 8 + 0], f[c * 8 + 1]);
-    pk.y = pack_h2(f[c * 8 + 2], f[c * 8 + 3]);
-    pk.z = pack_h2(f[c * 8 + 4], f[c * 8 + 5]);
-    pk.w = pack_h2(f[c * 8 + 6], f[c * 8 + 7]);
-    *reinterpret_cast<uint4*>(dst_row + c * kChunkBytes) = pk;
-  }
-}
-
-// View head: accumulator columns [0, NCOLS) + bias (RELU: then ReLU), fp16 with saturation -> the next step's A fragments.
-// TRAIN: also the fp16 pairs straight to this warpgroup's rows of the view-stash image `st_img`, and with RELU the mask
-// bits of those elements -> this thread's words of the tile's mask image `mask_img`.
-template <int NCOLS, bool RELU, bool TRAIN = false>
-__device__ __forceinline__ void epi_bias_frag(const float (&acc)[NCOLS / 2], const float* __restrict__ bias, uint32_t (&a)[NCOLS / 16][4],
-                                              uint8_t* st_img = nullptr, int g = 0, uint8_t* mask_img = nullptr) {
-  const int q = acc_q();
-  ReluMask<NCOLS> m;
-  if constexpr (TRAIN && RELU) m.clear();
-#pragma unroll
-  for (int j = 0; j < NCOLS / 8; ++j) {
-    const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * q));
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const float u = acc[4 * j + 2 * i] + b.x, v = acc[4 * j + 2 * i + 1] + b.y;
-      const uint32_t h2 = RELU ? pack_h2_relu_sat(u, v) : pack_h2_sat(u, v);
-      frag_pair(a, j, i) = h2;
-      if constexpr (TRAIN) {
-        if constexpr (RELU) m.pack(i, j, h2);
-        *reinterpret_cast<uint32_t*>(st_img + j * kChunkBytes + (g * kWgRows + acc_r0() + 8 * i) * 16 + 4 * q) = h2;
-      }
-    }
-  }
-  if constexpr (TRAIN && RELU) m.store(mask_img, g);
+  pack_row(f, dst_row);
 }
 
 static_assert(views::step(views::Feature) == fwd::step(fwd::L1), "step_at_views: Feature has the trunk's shape");
@@ -330,15 +305,7 @@ __device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p, const Vi
         for (int i = 0; i < kLatent; ++i) in[6 + i] = valid ? __ldg(lat + i) : 0.f;
 #pragma unroll
         for (int i = 38; i < 48; ++i) in[i] = 0.f;
-#pragma unroll
-        for (int c = 0; c < 6; ++c) {
-          uint4 pk;
-          pk.x = pack_h2(in[c * 8 + 0], in[c * 8 + 1]);
-          pk.y = pack_h2(in[c * 8 + 2], in[c * 8 + 3]);
-          pk.z = pack_h2(in[c * 8 + 4], in[c * 8 + 5]);
-          pk.w = pack_h2(in[c * 8 + 6], in[c * 8 + 7]);
-          *reinterpret_cast<uint4*>(e_row + c * kChunkBytes) = pk;
-        }
+        pack_row(in, e_row);
       }
       sw.ready(kStBin, Es);
       // ---- B0, B1: 96 hidden units (64 offset | 32 rigidity) ----
@@ -429,10 +396,11 @@ __device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p, const Vi
       else wg_gemm_rs<fwd::step(fwd::L1).N, fwd::step(fwd::L1).k16>(acc, h, ring, L == 5, a_e, W, 310 + L);
       if (LATENT_BIAS && (L == 0 || L == 5)) {
         const float* rb = p.ray_bias + (L == 5 ? fwd::b_off(fwd::L1) : 0);
-        epi_bias_relu_frag<TRAIN, true>(acc, rb + ray_r0 * p.ray_bias_stride, h, st + st_h(L + 1).off, g, mk, kMkH + L * kMaskHBytes,
-                                        rb + ray_r8 * p.ray_bias_stride);
+        epi_bias_frag<kMaskHCols, true, TRAIN, true>(acc, rb + ray_r0 * p.ray_bias_stride, h, st + st_h(L + 1).off, g,
+                                                     mk + kMkH + L * kMaskHBytes, rb + ray_r8 * p.ray_bias_stride);
       } else {
-        epi_bias_relu_frag<TRAIN>(acc, p.nerf_bias + L * fwd::b_off(fwd::L1), h, st + st_h(L + 1).off, g, mk, kMkH + L * kMaskHBytes);
+        epi_bias_frag<kMaskHCols, true, TRAIN>(acc, p.nerf_bias + L * fwd::b_off(fwd::L1), h, st + st_h(L + 1).off, g,
+                                               mk + kMkH + L * kMaskHBytes);
       }
     }
     if constexpr (PART == kViews) {

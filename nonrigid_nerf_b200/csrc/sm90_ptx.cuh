@@ -371,6 +371,9 @@ __device__ __forceinline__ uint32_t pack_h2_sat(float a, float b) {
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(b), "f"(a));
   return d;
 }
+// the low / high half of a packed fp16 pair as float (pack_h2's inverse)
+__device__ __forceinline__ float h_lo(uint32_t w) { return __half2float(__ushort_as_half(static_cast<unsigned short>(w & 0xffffu))); }
+__device__ __forceinline__ float h_hi(uint32_t w) { return __half2float(__ushort_as_half(static_cast<unsigned short>(w >> 16))); }
 __device__ __forceinline__ uint32_t pack_bf2(float a, float b) {
   __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&h);

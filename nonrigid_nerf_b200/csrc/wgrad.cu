@@ -235,8 +235,8 @@ __device__ __forceinline__ void consume(const Job& jb, const Unit& u0, const Uni
             const uint32_t wv[4] = {w.x, w.y, w.z, w.w};   // unpacked by value: no address of a local, no stack frame
 #pragma unroll
             for (int qq = 0; qq < 4; ++qq) {
-              t8[2 * qq] += __half2float(__ushort_as_half(static_cast<unsigned short>(wv[qq] & 0xffffu)));
-              t8[2 * qq + 1] += __half2float(__ushort_as_half(static_cast<unsigned short>(wv[qq] >> 16)));
+              t8[2 * qq] += h_lo(wv[qq]);
+              t8[2 * qq + 1] += h_hi(wv[qq]);
             }
           }
         }
@@ -263,108 +263,16 @@ __device__ __forceinline__ void consume(const Job& jb, const Unit& u0, const Uni
   if constexpr (N1 > 0) unit_drain(acc1, u1, part);
 }
 
-}  // namespace
-
-__global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradParams p) {
+// VIEWS: the view-dependent head's job set (views_job_desc), whose jobs 12-15 read A and B blocks from the view stashes
+template <bool VIEWS>
+__device__ __forceinline__ void wgrad_body(const WgradParams& p, const WgradViewParams& v) {
   extern __shared__ __align__(1024) uint8_t smem[];
   Shared* sh = reinterpret_cast<Shared*>(smem + kRingBytes);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   int job_id = 0, split = 0, nsplit = 1, half = 0, halves = 1, part_idx = 0;
   const bool have = locate(p, blockIdx.x, job_id, split, nsplit, half, halves, part_idx);
-  const Job jb = job_desc(job_id, half, (warp >> 2) & 1, p.compact);
-  // contiguous tile range of this split
-  const int per = (p.n_tiles + nsplit - 1) / nsplit;
-  const int t_begin = have ? min(split * per, p.n_tiles) : 0;
-  const int t_end = have ? min(t_begin + per, p.n_tiles) : 0;
-  const int n_local = t_end - t_begin;
-  // the two halves of a NeRF-layer split share their B blocks with the other CTA of the cluster; every other CTA
-  // (head, bender jobs, an idle CTA) works alone and shares only the cluster barriers with its neighbour
-  const bool paired = have && halves == 2;
-  const uint32_t rank = cluster_ctarank(), partner = rank ^ 1u;
-  // both halves of a split have the same A and B block sizes, hence the same stage layout
-  const int stage_bytes = (jb.a_chunks + jb.b_chunks) * kChunkBytes;
-  const int n_stages = min(kMaxStages, kRingBytes / stage_bytes);
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < n_stages; ++i) {
-      mbar_init(&sh->full[i], 1);
-      mbar_init(&sh->empty[i], paired ? 16 : 8);   // one arrival per consumer warp of every CTA that reads the stage
-    }
-    sh->abort_flag = 0;
-    fence_mbar_init();
-  }
-  // the partner's barriers are initialised before any multicast data or remote arrival can reach them
-  cluster_sync();
-  const Waiter W{&sh->abort_flag, p.err, paired, paired ? mapa_shared(&sh->abort_flag, partner) : 0u};
-  const Ring R{smem, stage_bytes, n_stages, paired, paired ? mapa_shared(&sh->empty[0], partner) : 0u};
-
-  if (warp >= 8) {
-    setmaxnreg_dec<kProducerRegs>();
-    // ===================== producer: one tile's A and B blocks per stage, 16 KB bulk copies =====================
-    if (warp == 8 && lane == 0) {
-      const uint32_t a_bytes = static_cast<uint32_t>(jb.a_chunks) * kChunkBytes, b_bytes = static_cast<uint32_t>(jb.b_chunks) * kChunkBytes;
-      // paired: this CTA fetches its own A block and its half of the B block, the latter multicast into both CTAs
-      const uint32_t b_begin = paired ? rank * (b_bytes / 2) : 0u, b_end = paired ? b_begin + b_bytes / 2 : b_bytes;
-      uint32_t stage = 0, phase = 0;
-      for (int it = 0; it < n_local; ++it) {
-        const long long tile = t_begin + it;
-        const uint8_t* a_src = p.gstash + tile * p.gstash_tile_bytes + jb.a_off;
-        const uint8_t* b_src = p.stash + tile * p.stash_tile_bytes + jb.b_off;
-        W.wait(&sh->empty[stage], phase ^ 1u, 101);
-        mbar_arrive_expect_tx(&sh->full[stage], a_bytes + b_bytes);   // the partner delivers the other half of B
-        uint8_t* dst = smem + stage * stage_bytes;
-        for (uint32_t o = 0; o < a_bytes; o += kPieceBytes)
-          tma_bulk_g2s(dst + o, a_src + o, a_bytes - o < kPieceBytes ? a_bytes - o : kPieceBytes, &sh->full[stage]);
-        dst += a_bytes;
-        for (uint32_t o = b_begin; o < b_end; o += kPieceBytes) {
-          const uint32_t n = b_end - o < kPieceBytes ? b_end - o : kPieceBytes;
-          if (paired) tma_bulk_g2s_multicast(dst + o, b_src + o, n, &sh->full[stage], 0x3);
-          else tma_bulk_g2s(dst + o, b_src + o, n, &sh->full[stage]);
-        }
-        if (++stage == n_stages) { stage = 0; phase ^= 1u; }
-      }
-    }
-  } else {
-    setmaxnreg_inc<kConsumerRegs>();
-    const int g = warp >> 2;
-    float* part = p.scratch + static_cast<size_t>(part_idx) * kWgScratchFloats;
-    const Unit& u0 = jb.u[0];
-    const Unit& u1 = jb.u[1];
-    if (job_id <= 9) {
-      const bool mine = u0.rows > 0;
-      // N = columns of the job's activation image
-      if (job_id == 8 || job_id == 9) {
-        if (mine) consume<8 * kStE.chunks, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
-        else consume<0, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
-      } else {
-        if (mine) consume<8 * kHChunks, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
-        else consume<0, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
-      }
-    } else if (job_id == 10) {
-      if (g == 0) consume<8 * kStHb4.chunks, 8 * kStHb3.chunks>(jb, u0, u1, R, sh, W, n_local, part, have);
-      else consume<8 * kStHb2.chunks, 8 * kStHb2.chunks>(jb, u0, u1, R, sh, W, n_local, part, have);
-    } else {
-      if (g == 0) consume<8 * kStHb1.chunks, 8 * kStHb1.chunks>(jb, u0, u1, R, sh, W, n_local, part, have);
-      else consume<8 * kStBin.chunks, 8 * kStBin.chunks>(jb, u0, u1, R, sh, W, n_local, part, have);
-    }
-  }
-  // No CTA leaves while its partner may still arrive on its barriers or write its abort flag.  Multicast data has
-  // landed: each CTA's consumers waited for every tile's full barrier.  Every thread gets here after a finite number of
-  // bounded waits (an abort reaches the partner through its abort flag), so this barrier cannot hang.
-  __syncwarp();
-  cluster_sync();
-}
-
-// The view-dependent head's job set (views_job_desc): wgrad_kernel with A and B blocks from the view stashes as well
-__global__ void __launch_bounds__(kWgThreads, 1) wgrad_views_kernel(const WgradParams p, const WgradViewParams v) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  Shared* sh = reinterpret_cast<Shared*>(smem + kRingBytes);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  int job_id = 0, split = 0, nsplit = 1, half = 0, halves = 1, part_idx = 0;
-  const bool have = locate(p, blockIdx.x, job_id, split, nsplit, half, halves, part_idx);
-  const Job jb = views_job_desc(job_id, half, (warp >> 2) & 1);
+  const Job jb = VIEWS ? views_job_desc(job_id, half, (warp >> 2) & 1) : job_desc(job_id, half, (warp >> 2) & 1, p.compact);
   // contiguous tile range of this split
   const int per = (p.n_tiles + nsplit - 1) / nsplit;
   const int t_begin = have ? min(split * per, p.n_tiles) : 0;
@@ -402,8 +310,10 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_views_kernel(const WgradP
       const uint8_t* a_base = p.gstash;
       const uint8_t* b_base = p.stash;
       long long a_tile = p.gstash_tile_bytes, b_tile = p.stash_tile_bytes;
-      if (job_id == kJobFeature || job_id == kJobViewsF || job_id == kJobViewsE) { a_base = v.vgstash; a_tile = kVGradTileBytes; }
-      if (job_id == kJobViewsF || job_id == kJobViewsE || job_id == kJobRgb) { b_base = v.vstash; b_tile = kVStashTileBytes; }
+      if constexpr (VIEWS) {
+        if (job_id == kJobFeature || job_id == kJobViewsF || job_id == kJobViewsE) { a_base = v.vgstash; a_tile = kVGradTileBytes; }
+        if (job_id == kJobViewsF || job_id == kJobViewsE || job_id == kJobRgb) { b_base = v.vstash; b_tile = kVStashTileBytes; }
+      }
       uint32_t stage = 0, phase = 0;
       for (int it = 0; it < n_local; ++it) {
         const long long tile = t_begin + it;
@@ -429,15 +339,16 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_views_kernel(const WgradP
     float* part = p.scratch + static_cast<size_t>(part_idx) * kWgScratchFloats;
     const Unit& u0 = jb.u[0];
     const Unit& u1 = jb.u[1];
-    if (job_id == kJobViewsF) {
+    if (VIEWS && job_id == kJobViewsF) {
       consume<8 * kVsF.chunks, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
-    } else if (job_id == kJobViewsE) {
+    } else if (VIEWS && job_id == kJobViewsE) {
       consume<8 * kVsDir.chunks, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
-    } else if (job_id == kJobRgb) {
+    } else if (VIEWS && job_id == kJobRgb) {
       if (u0.rows > 0) consume<8 * kVsHv.chunks, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
       else consume<0, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
-    } else {   // the trunk's jobs 0-9 and feature_linear (a NeRF layer's shape)
+    } else if (VIEWS || job_id <= 9) {   // the trunk's jobs 0-9 and feature_linear (a NeRF layer's shape)
       const bool mine = u0.rows > 0;
+      // N = columns of the job's activation image
       if (job_id == 8 || job_id == 9) {
         if (mine) consume<8 * kStE.chunks, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
         else consume<0, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
@@ -445,11 +356,26 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_views_kernel(const WgradP
         if (mine) consume<8 * kHChunks, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
         else consume<0, 0>(jb, u0, u1, R, sh, W, n_local, part, have);
       }
+    } else if (job_id == 10) {
+      if (g == 0) consume<8 * kStHb4.chunks, 8 * kStHb3.chunks>(jb, u0, u1, R, sh, W, n_local, part, have);
+      else consume<8 * kStHb2.chunks, 8 * kStHb2.chunks>(jb, u0, u1, R, sh, W, n_local, part, have);
+    } else {
+      if (g == 0) consume<8 * kStHb1.chunks, 8 * kStHb1.chunks>(jb, u0, u1, R, sh, W, n_local, part, have);
+      else consume<8 * kStBin.chunks, 8 * kStBin.chunks>(jb, u0, u1, R, sh, W, n_local, part, have);
     }
   }
-  // as wgrad_kernel: no CTA leaves while its partner may still arrive on its barriers or write its abort flag
+  // No CTA leaves while its partner may still arrive on its barriers or write its abort flag.  Multicast data has
+  // landed: each CTA's consumers waited for every tile's full barrier.  Every thread gets here after a finite number of
+  // bounded waits (an abort reaches the partner through its abort flag), so this barrier cannot hang.
   __syncwarp();
   cluster_sync();
+}
+
+}  // namespace
+
+__global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradParams p) { wgrad_body<false>(p, WgradViewParams{}); }
+__global__ void __launch_bounds__(kWgThreads, 1) wgrad_views_kernel(const WgradParams p, const WgradViewParams v) {
+  wgrad_body<true>(p, v);
 }
 
 
@@ -592,7 +518,7 @@ __device__ __forceinline__ Src views_src(int idx) {
 
 }  // namespace
 
-// The fixed-order sum over the split partials of job s.job (split 0, 1, 2, ...), as wgrad_reduce's: deterministic gradients
+// The fixed-order sum over the split partials of job s.job (split 0, 1, 2, ...): deterministic gradients
 __device__ __forceinline__ float split_sum(const WgradParams& p, const Src& s) {
   float sum = 0.f;
   int base = 0, slot = -1;
@@ -642,42 +568,7 @@ __device__ __forceinline__ void wgrad_reduce(const WgradParams p, const WgradDst
   const float scale = loss_scale(p.amax);
   float sum = 0.f;
   const bool lat = TC && s.job == kLatJob;   // tc_dw_lat_kernel's sums: already divided by the loss scale
-  if (ok && !lat && !(s.bias && p.compact)) {
-    int base = 0, slot = -1;
-    for (int j = 0; j < p.n_jobs; ++j) {
-      if (p.job_ids[j] == s.job) { slot = j; break; }
-      base += p.splits[j];
-    }
-    if (slot >= 0) {
-      const int nsplit = p.splits[slot];
-      const int per = (p.n_tiles + nsplit - 1) / nsplit;
-      const int n_valid = min(nsplit, (p.n_tiles + per - 1) / per);   // splits beyond that owned no tiles: scratch unwritten
-      const float* __restrict__ src = p.scratch + static_cast<size_t>(base) * kWgScratchFloats + (s.bias ? 65536 + s.off : s.off);
-      const bool has2 = !s.bias && s.off2 >= 0;
-      const int d2 = has2 ? s.off2 - s.off : 0;
-      // fixed summation order (split 0, 1, 2, ...) = deterministic gradients; the loads of 8 splits are in flight together
-      int sp = 0;
-      for (; sp + 8 <= n_valid; sp += 8) {
-        float a[8], b[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float* q = src + static_cast<size_t>(sp + i) * kWgScratchFloats;
-          a[i] = __ldg(q);
-          b[i] = has2 ? __ldg(q + d2) : 0.f;
-        }
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          sum += a[i];
-          if (has2) sum += b[i];
-        }
-      }
-      for (; sp < n_valid; ++sp) {
-        const float* q = src + static_cast<size_t>(sp) * kWgScratchFloats;
-        sum += __ldg(q);
-        if (has2) sum += __ldg(q + d2);
-      }
-    }
-  }
+  if (ok && !lat && !(s.bias && p.compact)) sum = split_sum(p, s);
   const float v = lat ? __ldg(dw_lat + s.off) : sum / scale;
   float* out;
   bool acc;
@@ -709,11 +600,21 @@ __global__ void wgrad_views_reduce_kernel(const WgradParams p, const WgradDst ds
 
 // ------------------------------------------------------------------------------------------------
 namespace {
-// Plans how the jobs jobs[0, n) (cost: relative bytes per tile of one of its CTAs; halves: CTAs per split) split their
-// tiles over the CTAs, writes the plan into p and launches `kernel` (wgrad_kernel or wgrad_views_kernel).
+// Relative cost of one tile of every job's CTAs, by job id = 2 KB chunks a CTA receives (a NeRF layer's half: 16 gradient
+// chunks + the activation block; feature_linear's half likewise; views_linears.0's feature columns 16 + 32, its direction
+// columns 16 + 4, both one MMA over a double-buffered ring).  The head job, rgb_linear (2 + 16) and the three-MMA bender
+// job stream a little slower per byte, hence their surcharge.  The plan decides how the fp32 partial sums associate:
+// changing a weight changes the gradients' last bits.
+constexpr int kJobCost[16] = {46, 48, 48, 48, 48, 48, 48, 48, 16 + 8 + 8, 16 + 8 + 8, 54, 24 + 18, 48, 48, 24, 20};
+// CTAs per split: a NeRF layer's and feature_linear's 256-row dW take two; the head's 16-row dW, the bender jobs and the
+// other view-head jobs fit one CTA
+constexpr int job_halves(int j) { return (j >= 1 && j <= 9) || j == kJobFeature ? 2 : 1; }
+
+// Plans how the jobs jobs[0, n) split their tiles over the CTAs, writes the plan into p and launches `kernel`
+// (wgrad_kernel or wgrad_views_kernel).
 template <typename... Args>
-cudaError_t launch_jobs(void (*kernel)(WgradParams, Args...), int* s_max_clusters, WgradParams& p, const int* jobs, const int* cost,
-                        const int* halves, int n, int num_sms, cudaStream_t st, Args... args) {
+cudaError_t launch_jobs(void (*kernel)(WgradParams, Args...), int* s_max_clusters, WgradParams& p, const int* jobs, int n,
+                        int num_sms, cudaStream_t st, Args... args) {
   // Launched in clusters of 2 CTAs (the two halves of a NeRF-layer split).  A cluster lives inside one GPC, so the
   // CTAs that can run at once are the resident clusters x 2, which can be fewer than the SMs.
   const size_t smem = kRingBytes + sizeof(Shared) + 64;
@@ -739,9 +640,10 @@ cudaError_t launch_jobs(void (*kernel)(WgradParams, Args...), int* s_max_cluster
   // Every CTA streams at about the same bytes/clk (the kernel is HBM-bound), so the launch ends when the CTA with the
   // most bytes ends: start with one split per job and hand each further split (its halves' CTAs) to the job whose CTAs
   // currently carry the most (chunks per tile x tiles per CTA).
-  int splits[16], used = 0;
+  int splits[16], halves[16], used = 0;
   for (int j = 0; j < n; ++j) {
     splits[j] = 1;
+    halves[j] = job_halves(jobs[j]);
     used += halves[j];
   }
   const int tiles = p.n_tiles > 0 ? p.n_tiles : 1;
@@ -751,7 +653,7 @@ cudaError_t launch_jobs(void (*kernel)(WgradParams, Args...), int* s_max_cluster
     for (int j = 0; j < n; ++j) {
       const int sp = splits[j];
       if (sp >= tiles || used + halves[j] > max_ctas) continue;   // a CTA needs at least one tile
-      const long long load = static_cast<long long>(cost[j]) * ((tiles + sp - 1) / sp);
+      const long long load = static_cast<long long>(kJobCost[jobs[j]]) * ((tiles + sp - 1) / sp);
       if (load > best_load) { best_load = load; best = j; }
     }
     if (best < 0) break;
@@ -776,22 +678,14 @@ cudaError_t launch_jobs(void (*kernel)(WgradParams, Args...), int* s_max_cluster
 
 cudaError_t launch_wgrad(WgradParams p, bool has_bender, int num_sms, const WgradDst& dst, int out_ch, cudaStream_t st,
                          const float* tc_dw_lat) {
-  // relative cost of one tile of every job's CTAs = 2 KB chunks a CTA receives (a NeRF layer's half: 16 gradient
-  // chunks + the activation block); the head job and the three-MMA bender job stream a little slower per byte, hence
-  // their surcharge.  The plan decides how the fp32 partial sums associate: changing a weight changes the gradients'
-  // last bits.
-  static const int kJobChunks[12] = {46, 48, 48, 48, 48, 48, 48, 48, 16 + 8 + 8, 16 + 8 + 8, 54, 24 + 18};
   int first = 0, last = has_bender ? 12 : 10;
   if (p.compact) { first = 10; last = 12; p.stash_tile_bytes = kTanTileBytes; p.gstash_tile_bytes = kAdjTileBytes; }
   else { p.stash_tile_bytes = kStashTileBytes; p.gstash_tile_bytes = kGradTileBytes; }
 
-  int jobs[12], cost[12], halves[12], n_jobs = 0;
-  for (int j = first; j < last; ++j) {
-    jobs[n_jobs] = j; cost[n_jobs] = kJobChunks[j];
-    halves[n_jobs++] = (j >= 1 && j <= 9) ? 2 : 1;   // the head's 16-row dW and the bender jobs fit one CTA
-  }
+  int jobs[12], n_jobs = 0;
+  for (int j = first; j < last; ++j) jobs[n_jobs++] = j;
   static int s_max_clusters[64];   // per device
-  cudaError_t e = launch_jobs(wgrad_kernel, s_max_clusters, p, jobs, cost, halves, n_jobs, num_sms, st);
+  cudaError_t e = launch_jobs(wgrad_kernel, s_max_clusters, p, jobs, n_jobs, num_sms, st);
   if (e != cudaSuccess) return e;
   const int n = dst.nerf_n + dst.bend_n;
   if (n > 0 && tc_dw_lat) wgrad_reduce_tc_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, dst, out_ch, tc_dw_lat);
@@ -800,18 +694,12 @@ cudaError_t launch_wgrad(WgradParams p, bool has_bender, int num_sms, const Wgra
 }
 
 cudaError_t launch_wgrad_views(WgradParams p, const WgradViewParams& v, int num_sms, const WgradDst& dst, cudaStream_t st) {
-  // costs as launch_wgrad's (chunks a CTA receives per tile): the trunk's jobs unchanged; feature_linear's half 16 + 32
-  // like a NeRF layer's; views_linears.0's feature columns 16 + 32, its direction columns 16 + 4 (both one MMA over a
-  // double-buffered ring); rgb_linear 2 + 16 with the head job's surcharge
-  static const int kViewJobChunks[14] = {46, 48, 48, 48, 48, 48, 48, 48, 16 + 8 + 8, 16 + 8 + 8, 48, 48, 24, 20};
-  int jobs[14], halves[14];
-  for (int j = 0; j < 14; ++j) {
-    jobs[j] = j < 10 ? j : kJobFeature + (j - 10);   // 12 feature, 13 views (feature columns), 14 rgb, 15 views (directions)
-    halves[j] = (jobs[j] >= 1 && jobs[j] <= 9) || jobs[j] == kJobFeature ? 2 : 1;
-  }
+  // the trunk's jobs 0-9, then 12 feature, 13 views (feature columns), 14 rgb, 15 views (directions)
+  int jobs[14];
+  for (int j = 0; j < 14; ++j) jobs[j] = j < 10 ? j : kJobFeature + (j - 10);
   p.stash_tile_bytes = kStashTileBytes; p.gstash_tile_bytes = kGradTileBytes;
   static int s_max_clusters[64];   // per device
-  cudaError_t e = launch_jobs(wgrad_views_kernel, s_max_clusters, p, jobs, kViewJobChunks, halves, 14, num_sms, st, v);
+  cudaError_t e = launch_jobs(wgrad_views_kernel, s_max_clusters, p, jobs, 14, num_sms, st, v);
   if (e != cudaSuccess) return e;
   if (dst.nerf_n > 0) wgrad_views_reduce_kernel<<<(dst.nerf_n + 255) / 256, 256, 0, st>>>(p, dst);
   return cudaGetLastError();

@@ -946,11 +946,10 @@ def run_all(cs, tag, divergence=True):
     return o, b, d
 
 
-# ---- WGRAD's split plan (wgrad.cu, launch_wgrad), replicated ----
-_JOB_CHUNKS = [46, 48, 48, 48, 48, 48, 48, 48, 32, 32, 54, 42]
-# launch_wgrad_views: per position 0..13 of the jobs 0..9, 12 (feature_linear), 13 (views_linears.0, feature columns),
-# 14 (rgb_linear), 15 (views_linears.0, direction columns)
-_VIEW_JOB_CHUNKS = [46, 48, 48, 48, 48, 48, 48, 48, 32, 32, 48, 48, 24, 20]
+# ---- WGRAD's split plan (wgrad.cu, launch_jobs), replicated ----
+# kJobCost: per job id 0..15 (0 head, 1..9 NeRF layers, 10 / 11 bender, 12 feature_linear, 13 views_linears.0's feature
+# columns, 14 rgb_linear, 15 views_linears.0's direction columns)
+_JOB_COST = [46, 48, 48, 48, 48, 48, 48, 48, 32, 32, 54, 42, 48, 48, 24, 20]
 VIEW_HEAD_JOBS = (12, 13, 14, 15)
 WG_SCRATCH_FLOATS = 256 * 256 + 256   # one partial per (job, split, half): kWgScratchFloats
 
@@ -963,10 +962,6 @@ def wgrad_halves(has_bender=True, compact=False, views=False):
         return {j: 2 if 1 <= j <= 9 or j == 12 else 1 for j in (*range(10), *VIEW_HEAD_JOBS)}
     jobs = range(10, 12) if compact else range(12 if has_bender else 10)
     return {j: 2 if 1 <= j <= 9 else 1 for j in jobs}
-
-
-def _job_cost(j, views):
-    return _VIEW_JOB_CHUNKS[j if j < 10 else j - 2] if views else _JOB_CHUNKS[j]
 
 
 def wgrad_rel_l2(split_tiles):
@@ -987,7 +982,7 @@ def wgrad_plan(n_tiles, max_ctas, has_bender=True, compact=False, views=False):
         for j in halves:
             if splits[j] >= tiles or used + halves[j] > max_ctas:
                 continue
-            load = _job_cost(j, views) * -(-tiles // splits[j])
+            load = _JOB_COST[j] * -(-tiles // splits[j])
             if load > best_load:
                 best, best_load = j, load
         if best < 0:

@@ -162,8 +162,8 @@ def test_boundary_tiles_hold_the_32_bit_limits_of_the_library_buffers():
 
 
 @pytest.mark.parametrize("max_ctas", [132, 114, 66, 16])
-def test_replicated_wgrad_plan_fits_the_scratch_and_covers_every_tile_once(max_ctas):
-    """wgrad_plan / split_ranges restate launch_wgrad's plan: its per-job costs are the kJobChunks table of wgrad.cu, its
+def test_replicated_wgrad_plan_follows_the_job_cost_table_fits_the_scratch_and_covers_every_tile_once(max_ctas):
+    """wgrad_plan / split_ranges restate launch_wgrad's plan: its per-job costs are the kJobCost table of wgrad.cu, its
     CTAs fit the device and the scratch partials (nrn_wgrad_scratch_bytes), and every job's splits own each tile exactly
     once.  The greedy rule itself is a copy: nothing the library exposes pins it."""
     from nonrigid_nerf_b200 import _lib
@@ -172,8 +172,9 @@ def test_replicated_wgrad_plan_fits_the_scratch_and_covers_every_tile_once(max_c
     parts = lib.nrn_wgrad_scratch_bytes() // (4 * SR.WG_SCRATCH_FLOATS)
     assert parts * 4 * SR.WG_SCRATCH_FLOATS == lib.nrn_wgrad_scratch_bytes()
     src = open(os.path.join(os.path.dirname(_lib.__file__), "csrc", "wgrad.cu")).read()
-    table = re.search(r"kJobChunks\[12\]\s*=\s*\{([^}]*)\}", src).group(1)
-    assert [sum(int(t) for t in x.split("+")) for x in table.split(",")] == SR._JOB_CHUNKS
+    table = re.search(r"kJobCost\[16\]\s*=\s*\{([^}]*)\}", src).group(1)
+    assert [sum(int(t) for t in x.split("+")) for x in table.split(",")] == SR._JOB_COST
+    assert SR._JOB_COST[:12] == [46, 48, 48, 48, 48, 48, 48, 48, 32, 32, 54, 42]
     for T in (1, 9, 1024, 4096, 8192, 53248):
         for kw in (dict(has_bender=True), dict(has_bender=False), dict(compact=True)):
             plan = SR.wgrad_plan(T, max_ctas, **kw)
@@ -187,17 +188,18 @@ def test_replicated_wgrad_plan_fits_the_scratch_and_covers_every_tile_once(max_c
 
 
 @pytest.mark.parametrize("max_ctas", [132, 114, 66, 16])
-def test_replicated_views_wgrad_plan_fits_the_scratch_and_covers_every_tile_once(max_ctas):
+def test_replicated_views_wgrad_plan_follows_the_job_cost_table_fits_the_scratch_and_covers_every_tile_once(max_ctas):
     """The same for launch_wgrad_views: its 14 jobs (the trunk's 0-9, then feature_linear 12, views_linears.0's feature
-    columns 13, rgb_linear 14 and views_linears.0's direction columns 15) with the kViewJobChunks costs; feature_linear
+    columns 13, rgb_linear 14 and views_linears.0's direction columns 15) with their kJobCost costs; feature_linear
     takes two CTAs per split like a NeRF layer."""
     from nonrigid_nerf_b200 import _lib
     from tests import stage_reference as SR
     lib = _lib.load()
     parts = lib.nrn_wgrad_scratch_bytes() // (4 * SR.WG_SCRATCH_FLOATS)
     src = open(os.path.join(os.path.dirname(_lib.__file__), "csrc", "wgrad.cu")).read()
-    table = re.search(r"kViewJobChunks\[14\]\s*=\s*\{([^}]*)\}", src).group(1)
-    assert [sum(int(t) for t in x.split("+")) for x in table.split(",")] == SR._VIEW_JOB_CHUNKS
+    table = re.search(r"kJobCost\[16\]\s*=\s*\{([^}]*)\}", src).group(1)
+    assert [sum(int(t) for t in x.split("+")) for x in table.split(",")] == SR._JOB_COST
+    assert [SR._JOB_COST[j] for j in (*range(10), 12, 13, 14, 15)] == [46, 48, 48, 48, 48, 48, 48, 48, 32, 32, 48, 48, 24, 20]
     halves = SR.wgrad_halves(views=True)
     assert list(halves) == [*range(10), 12, 13, 14, 15]
     assert [j for j, h in halves.items() if h == 2] == [*range(1, 10), 12]
