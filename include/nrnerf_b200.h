@@ -308,6 +308,23 @@ int nrn_field_backward_det(const NrnFieldBwdArgs* args, float* latent_rows);
 /* nrn_divergence_forward with loss written in a fixed order; loss_rows: nrn_div_loss_rows_bytes() */
 int nrn_divergence_forward_det(const NrnDivArgs* args, float* loss_rows);
 
+/* ---- held-out rays: the reference trains the latent codes of held-out frames (test_block_size, train.py:1376-1395) with a
+ * second backward pass whose network gradients it discards (train.py:1595-1608).  These entry points give one backward
+ * both: held_out_rays [n_rays] (device, one byte per ray, nonzero = held out) marks rays whose gradient reaches their
+ * latent code only.  Every kernel step runs as without it; the gradient-stash rows (adjoint-stash rows for the divergence
+ * regulariser) of a held-out ray's points are written as zeros, so the weight gradients leave them out.  With
+ * held_out_rays all zero the results equal those of the entry points without the suffix bit for bit.  Without a bender a
+ * held-out ray contributes nothing at all: zero its rows of d_raw and call nrn_field_backward (or _tc / _views). ------- */
+/* nrn_field_backward with a bender (bender_packed and d_latents given): d_latents as nrn_field_backward forms it for
+ * every ray; nerf_grad and bender_grad without the held-out rays' share (the data terms and the offsets / rigidity
+ * upstream gradients alike) */
+int nrn_field_backward_held_out(const NrnFieldBwdArgs* args, const uint8_t* held_out_rays);
+/* the same in deterministic mode: d_latents as nrn_field_backward_det forms it */
+int nrn_field_backward_det_held_out(const NrnFieldBwdArgs* args, float* latent_rows, const uint8_t* held_out_rays);
+/* nrn_divergence_backward with bender_grad without the held-out rays' share; d_unmasked_offsets and d_rigidity_mask, which
+ * carry their latent gradient into nrn_field_backward_held_out, as nrn_divergence_backward writes them */
+int nrn_divergence_backward_held_out(const NrnDivArgs* args, const uint8_t* held_out_rays);
+
 /* ---- per-ray training loss of training_wrapper_class.forward (train.py:208-242): image terms (fine +
  * coarse) and the offsets / rigidity regulariser on the coarse samples, with the gradients per unit
  * upstream gradient written in the same pass (the loss is linear in dL/dloss[ray]). ----------------- */
@@ -406,7 +423,9 @@ int nrn_peer_gather_rows(const NrnPeerCtx* ctx, const float* local, int n_per_ra
  * latent gradients (per-ray sums, d z, latent columns of dW0 / dW5), 8 bend pass of the view-dependent head, 9 its
  * view-head field kernel (nrn_field_forward_views), 10 its training forward (nrn_field_forward_views_train), 11 its DGRAD
  * and 12 its WGRAD (+reduce) (nrn_field_backward_views), 13 the fixed-order latent reduction (nrn_field_backward_det) and
- * 14 the fixed-order divergence loss reduction (nrn_divergence_forward_det).  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * 14 the fixed-order divergence loss reduction (nrn_divergence_forward_det), 15 the held-out DGRAD
+ * (nrn_field_backward_held_out, nrn_field_backward_det_held_out) and 16 the held-out divergence backward
+ * (nrn_divergence_backward_held_out; its WGRAD is kind 2).  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

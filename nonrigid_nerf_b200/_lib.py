@@ -187,6 +187,9 @@ SYMBOLS = {
     "nrn_div_loss_rows_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "nrn_field_backward_det": (C.c_int, [C.POINTER(NrnFieldBwdArgs), _vp]),
     "nrn_divergence_forward_det": (C.c_int, [C.POINTER(NrnDivArgs), _vp]),
+    "nrn_field_backward_held_out": (C.c_int, [C.POINTER(NrnFieldBwdArgs), _vp]),
+    "nrn_field_backward_det_held_out": (C.c_int, [C.POINTER(NrnFieldBwdArgs), _vp, _vp]),
+    "nrn_divergence_backward_held_out": (C.c_int, [C.POINTER(NrnDivArgs), _vp]),
     "nrn_ray_loss": (C.c_int, [C.POINTER(NrnRayLossArgs)]),
     "nrn_scale_rows": (C.c_int, [_vp, _vp, _vp, C.c_int64, C.c_int, _vp]),
     "nrn_ray_loss_backward": (C.c_int, [C.POINTER(NrnRayLossBwdArgs)]),
@@ -211,6 +214,8 @@ VIEW_KERNEL_KINDS = ("views_bend", "views_field")
 VIEW_TRAIN_KERNEL_KINDS = ("views_field_train", "views_dgrad", "views_wgrad")
 # deterministic mode's fixed-order per-ray reductions (latent gradient, divergence loss), timing kinds 13 and 14
 DET_KERNEL_KINDS = ("latent_reduce", "div_loss_reduce")
+# the held-out variants of DGRAD and of the divergence backward (render(..., held_out=)), timing kinds 15 and 16
+HELD_OUT_KERNEL_KINDS = ("field_dgrad_held_out", "div_bwd_held_out")
 
 
 def timing_enable(on: bool) -> None:
@@ -219,8 +224,8 @@ def timing_enable(on: bool) -> None:
 
 def timing_read(kinds=KERNEL_KINDS):
     """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True); `kinds` is KERNEL_KINDS,
-    KERNEL_KINDS + TC_KERNEL_KINDS, KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS, that + VIEW_TRAIN_KERNEL_KINDS or
-    that + DET_KERNEL_KINDS."""
+    KERNEL_KINDS + TC_KERNEL_KINDS, KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS, that + VIEW_TRAIN_KERNEL_KINDS,
+    that + DET_KERNEL_KINDS or that + HELD_OUT_KERNEL_KINDS."""
     n = len(kinds)
     ms = (C.c_double * n)()
     cnt = (C.c_int * n)()

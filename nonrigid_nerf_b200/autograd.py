@@ -69,14 +69,42 @@ def _split_flat(flat: torch.Tensor, like):
     return out
 
 
+def check_held_out(held_out: Optional[torch.Tensor], n_rays: int, device) -> Optional[torch.Tensor]:
+    """The per-ray held-out mask of render(..., held_out=) as the kernels read it (one byte per ray, nonzero = held out), or
+    None.  Raises, before any launch, unless it is an [n_rays] bool or uint8 tensor on `device`.  Its contents are not read
+    on the host, so a CUDA graph may replay a step with new ones."""
+    if held_out is None:
+        return None
+    if not isinstance(held_out, torch.Tensor):
+        raise RuntimeError("nonrigid_nerf_b200: held_out must be a tensor ([N] bool or uint8, one entry per ray)")
+    if held_out.dtype not in (torch.bool, torch.uint8):
+        raise RuntimeError(f"nonrigid_nerf_b200: held_out must be bool or uint8 (0/1 per ray), got {held_out.dtype}")
+    if held_out.dim() != 1 or held_out.shape[0] != n_rays:
+        raise RuntimeError(f"nonrigid_nerf_b200: held_out must have shape [{n_rays}] (one entry per ray), got {list(held_out.shape)}")
+    if held_out.device != torch.device(device):
+        raise RuntimeError(f"nonrigid_nerf_b200: held_out must be on the rays' device {device}, got {held_out.device}")
+    return held_out.contiguous().view(torch.uint8)
+
+
+def _zero_held_rows(d_raw: torch.Tensor, held: Optional[torch.Tensor]) -> torch.Tensor:
+    """Without a bender a held-out ray contributes nothing (the reference's second backward pass only runs with a bender,
+    train.py:1595-1597): its rows of the upstream gradient d_raw [N, S, C] are zeroed, which gives every parameter and latent
+    the gradient of the loss weighted by the training rays alone."""
+    if held is None:
+        return d_raw
+    return d_raw.masked_fill(held.view(-1, 1, 1).bool(), 0.0)
+
+
 class _FieldTrainFn(torch.autograd.Function):
     """raw, unmasked_offsets, rigidity_mask (differentiable) + point details (not differentiable).
     params = the NeRF's parameters in WGRAD order, followed (with a bender) by the bender's parameters in WGRAD order.
+    held: None, or the uint8 per-ray mask of check_held_out: with a bender a held-out ray's gradient reaches its latent
+    only (the held-out DGRAD leaves it out of the weight gradients), without one it is dropped (_zero_held_rows).
     (No autograd object outlives an iteration: a cached graph fragment would pin AccumulateGrad nodes -- and the CUDA
     stream they were created on -- across iterations, which breaks CUDA-graph capture of the step.)"""
 
     @staticmethod
-    def forward(ctx, net, rays, z_vals, latents, n_nerf, *params):
+    def forward(ctx, net, rays, z_vals, latents, held, n_nerf, *params):
         bender = net.ray_bender[0]
         cutoff, scaling, removal = _knobs(net)
         if removal is not None:
@@ -103,6 +131,7 @@ class _FieldTrainFn(torch.autograd.Function):
         ctx.stash = stash
         ctx.relu_mask = relu_mask
         ctx.params = params
+        ctx.held = held
         ctx.set_materialize_grads(False)
         if bender is not None:
             _register_relu_mask(det["unmasked_offsets"], relu_mask)
@@ -129,6 +158,9 @@ class _FieldTrainFn(torch.autograd.Function):
             d_un, d_rig = rest[0], rest[1]
         if d_raw is None:
             d_raw = torch.zeros(n, s, out_ch, dtype=torch.float32, device=dev)
+        held = ctx.held
+        if bender is None:
+            d_raw, held = _zero_held_rows(d_raw, held), None
         a = _lib.NrnFieldBwdArgs()
         a.n_rays, a.n_samples, a.out_ch = n, s, out_ch
         d_raw = d_raw.contiguous().float()
@@ -178,7 +210,13 @@ class _FieldTrainFn(torch.autograd.Function):
             # the per-ray latent gradient in a fixed order (per-point rows, then one reduction) instead of fp32 atomics
             rows = torch.empty(lib.nrn_latent_rows_bytes(n, s) // 4, dtype=torch.float32, device=dev)
             with torch.cuda.device(dev):
-                _lib.check(lib.nrn_field_backward_det(C.byref(a), rows.data_ptr()), "field_backward_det")
+                if held is not None:
+                    _lib.check(lib.nrn_field_backward_det_held_out(C.byref(a), rows.data_ptr(), held.data_ptr()), "field_backward_det_held_out")
+                else:
+                    _lib.check(lib.nrn_field_backward_det(C.byref(a), rows.data_ptr()), "field_backward_det")
+        elif held is not None:
+            with torch.cuda.device(dev):
+                _lib.check(lib.nrn_field_backward_held_out(C.byref(a), held.data_ptr()), "field_backward_held_out")
         else:
             with torch.cuda.device(dev):
                 _lib.check(lib.nrn_field_backward(C.byref(a)), "field_backward")
@@ -187,7 +225,7 @@ class _FieldTrainFn(torch.autograd.Function):
         grads = _param_grads(nerf_grad, nerf_p)
         if bender is not None:
             grads += _param_grads(bend_grad, bend_p)
-        return (None, None, None, d_lat, None, *grads)
+        return (None, None, None, d_lat, None, None, *grads)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -311,10 +349,12 @@ def _div_args(ctx):
 
 
 class _DivergenceFn(torch.autograd.Function):
-    """per-ray mean_s(w * (e^T J e)^2) of the offset field, closed-form forward and backward (csrc/div.cu)."""
+    """per-ray mean_s(w * (e^T J e)^2) of the offset field, closed-form forward and backward (csrc/div.cu).  held: None or
+    the uint8 per-ray mask of check_held_out: a held-out ray's term then reaches the bender's weights not at all, its
+    latent through the gradients w.r.t. unmasked / rigidity."""
 
     @staticmethod
-    def forward(ctx, unmasked, rigidity, weights, e, relu_mask, bender, w_is_alpha, *bend_p):
+    def forward(ctx, unmasked, rigidity, weights, e, relu_mask, bender, w_is_alpha, held, *bend_p):
         n, s = unmasked.shape[0], unmasked.shape[1]
         dev = unmasked.device
         lib = _lib.load()
@@ -339,6 +379,7 @@ class _DivergenceFn(torch.autograd.Function):
             with torch.cuda.device(dev):
                 _lib.check(lib.nrn_divergence_forward(C.byref(a)), "divergence_forward")
         ctx.bend_p = bend_p
+        ctx.held = held
         ctx.in_shapes = (unmasked.shape, rigidity.shape)
         return loss
 
@@ -361,18 +402,25 @@ class _DivergenceFn(torch.autograd.Function):
         a.adjoint_stash, a.wgrad_scratch = adj.data_ptr(), scratch.data_ptr()
         a.d_unmasked_offsets, a.d_rigidity_mask = d_un.data_ptr(), d_rg.data_ptr()
         with torch.cuda.device(dev):
-            _lib.check(lib.nrn_divergence_backward(C.byref(a)), "divergence_backward")
-        return (d_un.view(ctx.in_shapes[0]), d_rg.view(ctx.in_shapes[1]), None, None, None, None, None, *_param_grads(bend_grad, bend_p))
+            if ctx.held is not None:
+                _lib.check(lib.nrn_divergence_backward_held_out(C.byref(a), ctx.held.data_ptr()), "divergence_backward_held_out")
+            else:
+                _lib.check(lib.nrn_divergence_backward(C.byref(a)), "divergence_backward")
+        return (d_un.view(ctx.in_shapes[0]), d_rg.view(ctx.in_shapes[1]), None, None, None, None, None, None,
+                *_param_grads(bend_grad, bend_p))
 
 
 def divergence_loss(unmasked: torch.Tensor, rigidity: torch.Tensor, weights: Optional[torch.Tensor], bender,
-                    e: Optional[torch.Tensor] = None, opacity_alpha: Optional[torch.Tensor] = None) -> torch.Tensor:
+                    e: Optional[torch.Tensor] = None, opacity_alpha: Optional[torch.Tensor] = None,
+                    held_out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Fused divergence regulariser on the coarse samples of the LAST differentiable coarse pass.
     unmasked [N,S,3], rigidity [N,S,1] must be that pass's outputs (they locate its ReLU masks and
     carry the gradient w.r.t. the primal bender evaluation); weights [N,S] are used detached; `e` [N*S,3]
     are the Hutchinson probes (drawn with torch.randn like run_nerf_helpers.py:110 when None).
     Instead of `weights`, `opacity_alpha` [N,S] may be given: the kernels then apply the reference's
-    1 - exp(-relu(opacity_alpha)) (train.py:267) themselves."""
+    1 - exp(-relu(opacity_alpha)) (train.py:267) themselves.  held_out [N] (bool or uint8): rays whose term reaches their
+    latent only, not the bender's weights (render(..., held_out=))."""
+    held = check_held_out(held_out, unmasked.shape[0], unmasked.device)
     relu_mask = lookup_relu_mask(unmasked)
     if relu_mask is None:
         raise RuntimeError("nonrigid_nerf_b200: no ReLU masks for these offsets -- the fused divergence term needs the "
@@ -382,8 +430,8 @@ def divergence_loss(unmasked: torch.Tensor, rigidity: torch.Tensor, weights: Opt
         e = torch.randn(n * s, 3, device=unmasked.device)
     _, bend_p = _flat_params(None, bender)
     if opacity_alpha is not None:
-        return _DivergenceFn.apply(unmasked, rigidity, opacity_alpha, e, relu_mask, bender, True, *bend_p)
-    return _DivergenceFn.apply(unmasked, rigidity, weights, e, relu_mask, bender, False, *bend_p)
+        return _DivergenceFn.apply(unmasked, rigidity, opacity_alpha, e, relu_mask, bender, True, held, *bend_p)
+    return _DivergenceFn.apply(unmasked, rigidity, weights, e, relu_mask, bender, False, held, *bend_p)
 
 
 class _RayLossFn(torch.autograd.Function):
@@ -544,7 +592,7 @@ class _ViewsTrainFn(torch.autograd.Function):
     gradient leaves the field but the parameters': the latents get none."""
 
     @staticmethod
-    def forward(ctx, net, rays, z_vals, viewdirs, n_trunk, *params):
+    def forward(ctx, net, rays, z_vals, viewdirs, held, n_trunk, *params):
         if getattr(net, "test_time_nonrigid_object_removal_threshold", None) is not None:
             raise RuntimeError("nonrigid_nerf_b200: test_time_nonrigid_object_removal_threshold is a test-time knob; "
                                "it is not differentiable")
@@ -556,6 +604,7 @@ class _ViewsTrainFn(torch.autograd.Function):
         ctx.packs = (nerf_pack, views_t)
         # the stashes live as long as the autograd node (a second backward over a retained graph reads them again)
         ctx.bufs = bufs
+        ctx.held = held
         ctx.set_materialize_grads(False)
         ctx.mark_non_differentiable(det["initial_input_pts"], det["input_pts"])
         return raw, det["initial_input_pts"], det["input_pts"]
@@ -569,7 +618,7 @@ class _ViewsTrainFn(torch.autograd.Function):
         lib = _lib.load()
         if d_raw is None:
             d_raw = torch.zeros(n, s, 4, dtype=torch.float32, device=dev)
-        d_raw = d_raw.contiguous().float()
+        d_raw = _zero_held_rows(d_raw, ctx.held).contiguous().float()
         a = _lib.NrnFieldBwdArgs()
         a.n_rays, a.n_samples, a.out_ch = n, s, 4
         a.d_raw = d_raw.data_ptr()
@@ -587,7 +636,7 @@ class _ViewsTrainFn(torch.autograd.Function):
             views_t.data_ptr(), bufs["views_stash"].data_ptr(), vgstash.data_ptr(), bufs["hv_mask"].data_ptr())
         with torch.cuda.device(dev):
             _lib.check(lib.nrn_field_backward_views(C.byref(a), C.byref(v)), "field_backward_views")
-        return (None, None, None, None, None, *_param_grads(flat, params))
+        return (None, None, None, None, None, None, *_param_grads(flat, params))
 
 
 def field_views(net, rays, z_vals, points, latents, viewdirs, want_details, bend_only=False):
@@ -609,9 +658,12 @@ def field_views(net, rays, z_vals, points, latents, viewdirs, want_details, bend
 
 
 def field(net, rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[torch.Tensor],
-          want_details: bool, viewdirs: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
+          want_details: bool, viewdirs: Optional[torch.Tensor] = None,
+          held_out: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
     """Fused field evaluation for rays x samples; differentiable when autograd is recording.  viewdirs [N, 3]: the
-    normalised ray directions a use_viewdirs=True model takes."""
+    normalised ray directions a use_viewdirs=True model takes.  held_out [N] (bool or uint8): rays whose gradient reaches
+    their latent only with a bender, and nothing without one (check_held_out)."""
+    held = check_held_out(held_out, rays.shape[0], rays.device)
     bender = net.ray_bender[0]
     if getattr(net, "use_viewdirs", False):
         if viewdirs is None:
@@ -619,14 +671,14 @@ def field(net, rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[torch
         views_check(net, latents)   # with a bender: raises for a differentiable call
         if bender is None and _needs_grad(net, latents):
             trunk, head = _views_flat_params(net)
-            raw, init, bent = _ViewsTrainFn.apply(net, rays, z_vals, viewdirs, len(trunk), *trunk, *head)
+            raw, init, bent = _ViewsTrainFn.apply(net, rays, z_vals, viewdirs, held, len(trunk), *trunk, *head)
             return raw, ({"initial_input_pts": init, "input_pts": bent} if want_details else {})
         return field_views(net, rays, z_vals, None, latents, viewdirs, want_details)
     _tc_net(net)
     if not _needs_grad(net, latents):
         return field_rays(net, rays, z_vals, latents, want_details)
     nerf_p, bend_p = _flat_params(net, bender)
-    outs = _FieldTrainFn.apply(net, rays, z_vals, latents, len(nerf_p), *nerf_p, *bend_p)
+    outs = _FieldTrainFn.apply(net, rays, z_vals, latents, held, len(nerf_p), *nerf_p, *bend_p)
     if bender is not None:
         raw, un, rig, init, bent, masked = outs
         details = {"initial_input_pts": init, "unmasked_offsets": un, "rigidity_mask": rig, "masked_offsets": masked,

@@ -19,6 +19,7 @@ namespace nrn {
 cudaError_t launch_field_fwd(const FieldFwdParams& p, bool has_bender, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_bwd(const FieldBwdParams& p, bool has_bender, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_bwd_det(const FieldBwdParams& p, float* latent_rows, int num_sms, cudaStream_t stream);
+cudaError_t launch_field_bwd_held(const FieldBwdParams& p, float* latent_rows, const uint8_t* held, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_fwd_tc(const FieldFwdParams& p, int num_sms, cudaStream_t stream);
 cudaError_t launch_tc_latent_bias(const float* lat, long long lat_stride, int n_rays, const float* w0, const float* b0, const float* w5,
                                   const float* b5, float* rb, cudaStream_t stream);
@@ -575,8 +576,9 @@ int nrn_nerf_tc_grad_floats(int out_ch) { return nrn::nerf_tc_grad_floats(out_ch
 size_t nrn_tc_workspace_bytes(int n_rays) { return n_rays < 0 ? 0 : (static_cast<size_t>(n_rays) * 2 * 256 + 2 * 256 * nrn::kLatent) * sizeof(float); }
 
 // nrn_field_backward, or with t (time-conditioned baseline, no bender) nrn_field_backward_tc, or with latent_rows
-// (deterministic mode, bender) nrn_field_backward_det
-static int field_backward(const NrnFieldBwdArgs* a, const NrnTcBwdArgs* t, const char* who, float* latent_rows = nullptr) {
+// (deterministic mode, bender) nrn_field_backward_det; with held (bender) the held-out variants of the last two
+static int field_backward(const NrnFieldBwdArgs* a, const NrnTcBwdArgs* t, const char* who, float* latent_rows = nullptr,
+                          const uint8_t* held = nullptr) {
   long long P;
   int tiles;
   int rc = check_field_bwd_args(a, who, &P, &tiles);
@@ -604,14 +606,18 @@ static int field_backward(const NrnFieldBwdArgs* a, const NrnTcBwdArgs* t, const
   if (e == cudaSuccess && bend && p.d_unmasked_up) e = nrn::launch_absmax(p.d_unmasked_up, P * 3, amax, st, true);
   if (e == cudaSuccess && bend && p.d_rigid_up) e = nrn::launch_absmax(p.d_rigid_up, P, amax, st, true);
   if (e != cudaSuccess) return cuda_fail(e, "absmax_kernel");
-  if (latent_rows) {
+  if (held) {
+    rc = timed(15, st, "field_bwd_held_kernel", [&] { return nrn::launch_field_bwd_held(p, latent_rows, held, ds->num_sms, st); });
+  } else if (latent_rows) {
     rc = timed(1, st, "field_bwd_det_kernel", [&] { return nrn::launch_field_bwd_det(p, latent_rows, ds->num_sms, st); });
-    if (rc) return rc;
-    rc = timed(13, st, "latent_reduce_kernel", [&] { return nrn::launch_latent_reduce(latent_rows, a->d_latents, a->n_rays, a->n_samples, st); });
   } else {
     rc = timed(1, st, "field_bwd_kernel", [&] { return nrn::launch_field_bwd(p, bend, ds->num_sms, st); });
   }
   if (rc) return rc;
+  if (latent_rows) {
+    rc = timed(13, st, "latent_reduce_kernel", [&] { return nrn::launch_latent_reduce(latent_rows, a->d_latents, a->n_rays, a->n_samples, st); });
+    if (rc) return rc;
+  }
   float* dw_lat = nullptr;
   if (t) {   // per-ray sums of dY0 / dY5 -> d z and the latent columns of dW0 / dW5 (before WGRAD's reduction reads them)
     nrn::TcBwdParams q{};
@@ -643,6 +649,32 @@ int nrn_field_backward_det(const NrnFieldBwdArgs* a, float* latent_rows) {
   if (a->n_rays == 0) return field_backward(a, nullptr, who);   // an empty shard: zero gradients, no kernel
   if (!latent_rows || !aligned16(latent_rows)) return fail(NRN_E_INVALID, "%s: null or unaligned latent_rows (nrn_latent_rows_bytes, 16-byte aligned)", who);
   return field_backward(a, nullptr, who, latent_rows);
+}
+
+// the checks both held-out entry points add to those of field_backward
+static int check_held_out(const NrnFieldBwdArgs* a, const uint8_t* held, const char* who) {
+  if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
+  if (!a->bender_packed || !a->d_latents)
+    return fail(NRN_E_INVALID, "%s: needs a bender (bender_packed) and d_latents; without a bender a held-out ray contributes "
+                "nothing: zero its rows of d_raw and call nrn_field_backward", who);
+  if (a->n_rays > 0 && !held) return fail(NRN_E_INVALID, "%s: null held_out_rays", who);
+  return NRN_OK;
+}
+
+int nrn_field_backward_held_out(const NrnFieldBwdArgs* a, const uint8_t* held_out_rays) {
+  const char* who = "nrn_field_backward_held_out";
+  const int rc = check_held_out(a, held_out_rays, who);
+  if (rc) return rc;
+  return field_backward(a, nullptr, who, nullptr, a->n_rays > 0 ? held_out_rays : nullptr);
+}
+
+int nrn_field_backward_det_held_out(const NrnFieldBwdArgs* a, float* latent_rows, const uint8_t* held_out_rays) {
+  const char* who = "nrn_field_backward_det_held_out";
+  const int rc = check_held_out(a, held_out_rays, who);
+  if (rc) return rc;
+  if (a->n_rays == 0) return field_backward(a, nullptr, who);   // an empty shard: zero gradients, no kernel
+  if (!latent_rows || !aligned16(latent_rows)) return fail(NRN_E_INVALID, "%s: null or unaligned latent_rows (nrn_latent_rows_bytes, 16-byte aligned)", who);
+  return field_backward(a, nullptr, who, latent_rows, held_out_rays);
 }
 
 int nrn_field_backward_tc(const NrnFieldBwdArgs* a, const NrnTcBwdArgs* t) {
@@ -714,13 +746,14 @@ int nrn_divergence_forward_det(const NrnDivArgs* a, float* loss_rows) {
   return timed(14, st, "div_loss_reduce_kernel", [&] { return nrn::launch_div_loss_reduce(loss_rows, a->loss, a->n_rays, a->n_samples, st); });
 }
 
-int nrn_divergence_backward(const NrnDivArgs* a) {
+// nrn_divergence_backward, or with held its held-out variant
+static int divergence_backward(const NrnDivArgs* a, const uint8_t* held, const char* who) {
   nrn::DivParams p{};
-  int rc = fill_div(a, p, "nrn_divergence_backward");
+  int rc = fill_div(a, p, who);
   if (rc) return rc;
   if ((!a->G && !(a->g_ray && a->G_workspace)) || !a->adjoint_stash || !a->wgrad_scratch || !a->d_unmasked_offsets || !a->d_rigidity_mask ||
       !a->bender_grad)
-    return fail(NRN_E_INVALID, "nrn_divergence_backward: null argument");
+    return fail(NRN_E_INVALID, "%s: null argument", who);
   DeviceState* ds;
   rc = device_state(&ds);
   if (rc) return rc;
@@ -730,12 +763,21 @@ int nrn_divergence_backward(const NrnDivArgs* a) {
   p.d_unmasked = a->d_unmasked_offsets; p.d_rigid = a->d_rigidity_mask; p.err = ds->err_word;
   cudaError_t e = a->G ? nrn::launch_absmax(a->G, p.P, amax, st) : nrn::launch_div_G(p, a->g_ray, a->G_workspace, amax, st);
   if (e != cudaSuccess) return cuda_fail(e, "absmax_kernel");
-  rc = timed(5, st, "div_bwd_kernel", [&] { return nrn::launch_div_bwd(p, ds->num_sms, st); });
+  if (held) rc = timed(16, st, "div_bwd_held_kernel", [&] { return nrn::launch_div_bwd_held(p, held, ds->num_sms, st); });
+  else rc = timed(5, st, "div_bwd_kernel", [&] { return nrn::launch_div_bwd(p, ds->num_sms, st); });
   if (rc) return rc;
   nrn::WgradParams w = wgrad_params(p.tan, p.adj, a->wgrad_scratch, amax, static_cast<int>(tile_count(p.P)), ds->err_word);
   w.compact = 1;
   const nrn::WgradDst dst{nullptr, nullptr, a->bender_grad, 0, nrn_bender_grad_floats(), 0, a->accumulate_bender};
   return timed(2, st, "wgrad_kernel (divergence)", [&] { return nrn::launch_wgrad(w, true, ds->num_sms, dst, 5, st); });
+}
+
+int nrn_divergence_backward(const NrnDivArgs* a) { return divergence_backward(a, nullptr, "nrn_divergence_backward"); }
+
+int nrn_divergence_backward_held_out(const NrnDivArgs* a, const uint8_t* held_out_rays) {
+  const char* who = "nrn_divergence_backward_held_out";
+  if (a && a->n_rays > 0 && !held_out_rays) return fail(NRN_E_INVALID, "%s: null held_out_rays", who);
+  return divergence_backward(a, held_out_rays, who);
 }
 
 int nrn_ray_loss(const NrnRayLossArgs* a) {

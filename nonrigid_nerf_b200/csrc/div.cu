@@ -298,7 +298,11 @@ __global__ void __launch_bounds__(kDivThreads, 1) div_fwd_det_kernel(const DivPa
 }
 
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kDivThreads, 1) div_bwd_kernel(const DivParams p) {
+// HELD: `held` [n_rays] bytes, nonzero for a held-out ray.  The adjoint chain of a held-out ray's points starts from zero,
+// so its adjoint-stash rows are zero and the compact WGRAD (no bias term) leaves it out of the bender's weight gradient;
+// d_unmasked / d_rigid, which carry its latent gradient into DGRAD, are written as without it.
+template <bool HELD>
+__device__ __forceinline__ void div_bwd_body(const DivParams& p, const uint8_t* held) {
   extern __shared__ __align__(128) uint8_t smem[];
   const int wg = threadIdx.x >> 7;
   const int h = wg & 1;
@@ -336,7 +340,10 @@ __global__ void __launch_bounds__(kDivThreads, 1) div_bwd_kernel(const DivParams
       for (int d = 0; d < 3; ++d) p.d_unmasked[pt * 3 + d] = G * tau_r * e[d];
       p.d_rigid[pt] = G * (alpha + 2.0f * beta * tau_c * (1.0f - 2.0f * r));
     }
-    const float Gs = G * scale;
+    float Gs = G * scale;
+    if constexpr (HELD) {
+      if (valid && __ldg(held + pt / p.S)) Gs = 0.f;
+    }
     const float rp = 2.0f * r * (1.0f - r);
     const float tb_c = Gs * beta * rp;   // adjoint of tau_c
     // ---- [taubar_off (3) | 0], taubar_off = G r e ----
@@ -391,6 +398,11 @@ __global__ void __launch_bounds__(kDivThreads, 1) div_bwd_kernel(const DivParams
   if (wg_leader) tma_bulk_wait<0>();   // all adjoint-stash stores complete before the CTA exits
 }
 
+__global__ void __launch_bounds__(kDivThreads, 1) div_bwd_kernel(const DivParams p) { div_bwd_body<false>(p, nullptr); }
+__global__ void __launch_bounds__(kDivThreads, 1) div_bwd_held_kernel(const DivParams p, const uint8_t* held) {
+  div_bwd_body<true>(p, held);
+}
+
 // ------------------------------------------------------------------------------------------------
 namespace {
 __global__ void div_G_kernel(const DivParams p, const float* __restrict__ g_ray, float* __restrict__ G, float* __restrict__ amax) {
@@ -434,6 +446,9 @@ cudaError_t launch_div_fwd(const DivParams& p, int num_sms, cudaStream_t st) {
 }
 cudaError_t launch_div_bwd(const DivParams& p, int num_sms, cudaStream_t st) {
   return launch_div(div_bwd_kernel, kDivBwdWBytes, p, num_sms, st);
+}
+cudaError_t launch_div_bwd_held(const DivParams& p, const uint8_t* held, int num_sms, cudaStream_t st) {
+  return launch_div(div_bwd_held_kernel, kDivBwdWBytes, p, num_sms, st, held);
 }
 cudaError_t launch_div_fwd_det(const DivParams& p, float* loss_rows, int num_sms, cudaStream_t st) {
   return launch_div(div_fwd_det_kernel, kDivFwdWBytes, p, num_sms, st, loss_rows);

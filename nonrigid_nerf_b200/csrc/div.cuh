@@ -32,6 +32,8 @@ struct DivParams {
 
 cudaError_t launch_div_fwd(const DivParams& p, int num_sms, cudaStream_t st);
 cudaError_t launch_div_bwd(const DivParams& p, int num_sms, cudaStream_t st);
+// launch_div_bwd leaving the points of held-out rays (held [n_rays] bytes, nonzero = held out) out of the adjoint stash
+cudaError_t launch_div_bwd_held(const DivParams& p, const uint8_t* held, int num_sms, cudaStream_t st);
 // deterministic mode: per-point loss rows [P] instead of atomics into p.loss (launch_div_loss_reduce then writes p.loss)
 cudaError_t launch_div_fwd_det(const DivParams& p, float* loss_rows, int num_sms, cudaStream_t st);
 // G[pt] = g_ray[pt / S] * 2 * w * d / S (the gradient of mean_s(w d^2)) and amax = max|G| in one pass

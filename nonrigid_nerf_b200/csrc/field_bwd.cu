@@ -18,6 +18,7 @@
 // All gradients travel in fp16 scaled by a power-of-two loss scale derived on the device from
 // max|d_raw| (no host sync); WGRAD and the latent reduction divide it out again in fp32.
 // field_bwd_views_kernel (view-dependent head, no bender): Rgb^T, ViewsF^T and Feature^T + head^T in front of L7^T.
+// field_bwd_held_kernel (bender, held-out rays): the same chain; the gradient-stash rows of held-out rays' points are zero.
 #include "field_mma.cuh"
 
 namespace nrn {
@@ -120,6 +121,50 @@ __device__ __forceinline__ void d_raw_frag(const FieldBwdParams& p, int tile, fl
       *reinterpret_cast<uint32_t*>(gs + kGsRaw.off + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = frag_pair(a, j, i);
 }
 
+// Held-out rays (field_bwd_held_kernel): bit i is set when this thread's accumulator row r0 + 8 i is a point of a held-out
+// ray.  The epilogues store the gradient-stash words of every row as usual and then overwrite those of held-out rows with
+// zeros (clear_held_rows), so that the gradient itself travels on unchanged.
+struct HeldRows {
+  uint32_t bits = 0u;
+};
+
+// Held-out rays: which of this thread's accumulator rows of warpgroup g in `tile` are held out (rows past P are stored as
+// they are, like the bulk stores of field_bwd_kernel do)
+__device__ __forceinline__ HeldRows held_rows(const FieldBwdParams& p, const uint8_t* __restrict__ held, int tile, int g) {
+  HeldRows k;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const long long pt = static_cast<long long>(tile) * kTileM + g * kWgRows + acc_r0() + 8 * i;
+    if (pt < p.P && __ldg(held + pt / p.S)) k.bits |= 1u << i;
+  }
+  return k;
+}
+
+// Held-out rays: zeros over this thread's words of its held-out rows in columns [0, NCOLS) of the chunk-major image `img`
+// of warpgroup g, after the epilogue's own stores of them (same thread, so they land last)
+template <int NCOLS>
+__device__ __forceinline__ void clear_held_rows(uint8_t* img, int g, const HeldRows& k) {
+  if (!k.bits) return;
+  const int r0 = g * kWgRows + acc_r0(), q = acc_q();
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    if ((k.bits >> i) & 1u) {
+#pragma unroll
+      for (int j = 0; j < NCOLS / 8; ++j) *reinterpret_cast<uint32_t*>(img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = 0u;
+    }
+  }
+}
+
+// Held-out rays: a finished bender gradient image `im` of `act` (written, fenced and warpgroup-synced as for
+// StashWriter::ready) -> the tile's gradient stash by one row thread per row, as zeros for a held-out row.  act itself
+// stays as it is: it is the next step's A operand, which carries the held-out rays' latent gradient.
+__device__ __forceinline__ void store_row_held(uint8_t* gs, Image im, const uint8_t* act, int row, bool held_row) {
+  for (uint32_t c = 0; c < im.chunks; ++c) {
+    const uint4 v = held_row ? make_uint4(0u, 0u, 0u, 0u) : *reinterpret_cast<const uint4*>(act + c * kChunkBytes + row * 16);
+    *reinterpret_cast<uint4*>(gs + im.off + c * kChunkBytes + row * 16) = v;
+  }
+}
+
 // Backward of the positional encoding: dx_d += dE[d] + sum_k 2^k (dE[sin_kd] cos_kd - dE[cos_kd] sin_kd)
 // de: this row's 64 staged accumulator columns; sin/cos: the forward embedding stashed as fp16.
 __device__ __forceinline__ void pe_backward(const float* de, const uint8_t* __restrict__ e_row, float (&dx)[3]) {
@@ -161,8 +206,12 @@ __device__ __forceinline__ Step step_at_views(int step) {
 // DET = true (deterministic mode): it writes them to latent_rows [P][32] instead (det_reduce.cu's rule: a warp whose 32 rows
 // are all valid and of one ray stores their transpose-reduced sum in the row of its first point, 32k; any other warp stores
 // each valid row), and latent_reduce_kernel sums them per ray in a fixed order.
-template <bool HAS_BENDER, bool DET>
-__device__ __forceinline__ void field_bwd_body(const FieldBwdParams& p, float* latent_rows) {
+// HELD (bender only): `held` [n_rays] bytes, nonzero for a held-out ray.  Every step runs as without it, so a held-out ray's
+// latent gradient is formed as before, but every gradient-stash row of its points (kGsRaw, dY7 .. dY0, dYb4 .. dYb0) is
+// stored as zeros, so that WGRAD's weight and bias sums leave it out.  The bender images then go to the stash by per-row
+// stores instead of bulk stores of act.
+template <bool HAS_BENDER, bool DET, bool HELD = false>
+__device__ __forceinline__ void field_bwd_body(const FieldBwdParams& p, float* latent_rows, const uint8_t* held = nullptr) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* act = smem;                               // bender gradient operand (24 KB), 128 rows
   uint8_t* ring_buf = smem + kBwdActBytes;           // kBwdRingStages x 32 KB
@@ -221,17 +270,21 @@ __device__ __forceinline__ void field_bwd_body(const FieldBwdParams& p, float* l
     constexpr Step kTrunk = dgrad::step(dgrad::L7T), kEmb = dgrad::step(dgrad::L5eT);
     static_assert(dgrad::step(dgrad::L0T) == kEmb && kEmb.nslabs == 1 && kEmb.k16 == kMaskHCols / 16, "L5e^T, L0^T: one slab, K = 256");
     uint32_t h[kMaskHCols / 16][4];
+    HeldRows hr;
+    if constexpr (HELD) hr = held_rows(p, held, tile, g);
     // ---- head^T: A = d_raw [g_r g_g g_b g_sigma 0 ...] (K = 16), one fragment built from global memory ----
     {
       static_assert(dgrad::step(dgrad::HeadT).N == kTrunk.N && dgrad::step(dgrad::HeadT).nslabs == 1 &&
                     dgrad::step(dgrad::HeadT).k16 == 1 && kGsRaw.chunks == 2, "head^T: one K = 16 MMA");
       uint32_t a[1][4];
       d_raw_frag(p, tile, scale, gs, g, a);
+      if constexpr (HELD) clear_held_rows<16>(gs + kGsRaw.off, g, hr);
       Acc<dgrad::HeadT> acc;
       ReluMask<kMaskHCols> m;
       m.load(mk + kMkH + 7 * kMaskHBytes, g);
       wg_gemm_rs<kTrunk.N, 1>(acc, a, ring, false, 0u, W, 300);
       epi_grad_frag<kMaskHCols, true>(acc, m, h, gs + kGsY + 7 * kHBytes, g);
+      if constexpr (HELD) clear_held_rows<kMaskHCols>(gs + kGsY + 7 * kHBytes, g, hr);
     }
     float dx[3] = {0.f, 0.f, 0.f};
     // ---- L7^T, L6^T : dY6, dY5 ----
@@ -243,6 +296,7 @@ __device__ __forceinline__ void field_bwd_body(const FieldBwdParams& p, float* l
       wg_gemm_rs<kTrunk.N, kTrunk.k16>(acc, h, ring, false, 0u, W, 301 + s);
       if (s == 1) prefetch_e();
       epi_grad_frag<kMaskHCols, true>(acc, m, h, gs + kGsY + (6 - s) * kHBytes, g);
+      if constexpr (HELD) clear_held_rows<kMaskHCols>(gs + kGsY + (6 - s) * kHBytes, g, hr);
     }
     // ---- L5e^T: gradient into the skip-connected embedding; h (dY5) stays as it is for L5h^T ----
     {
@@ -262,6 +316,7 @@ __device__ __forceinline__ void field_bwd_body(const FieldBwdParams& p, float* l
       wg_gemm_rs<kTrunk.N, kTrunk.k16>(acc, h, ring, false, 0u, W, 304 + s);
       if (s == 4) prefetch_e();
       epi_grad_frag<kMaskHCols, true>(acc, m, h, gs + kGsY + (4 - s) * kHBytes, g);
+      if constexpr (HELD) clear_held_rows<kMaskHCols>(gs + kGsY + (4 - s) * kHBytes, g, hr);
     }
     // ---- L0^T: gradient into the embedding; then through the bend ----
     {
@@ -273,6 +328,18 @@ __device__ __forceinline__ void field_bwd_body(const FieldBwdParams& p, float* l
       if (row_thread) pe_backward(my_stg, st + kStE.off, dx);
     }
     if (!HAS_BENDER) continue;   // xyz has no learnable upstream without a bender (appendix C)
+    // a finished bender image of act -> the stash: bulk stores, or (HELD) per-row stores that zero the held-out rows
+    bool held_row = false;
+    if constexpr (HELD) held_row = valid && __ldg(held + pt / p.S);
+    auto ready = [&](Image im) {
+      if constexpr (HELD) {
+        fence_proxy_async_smem();
+        wg_bar(bar);
+        if (row_thread) store_row_held(gs, im, act, row, held_row);
+      } else {
+        sw.ready(im, act);
+      }
+    };
 
     float drpre = 0.f;
     sw.begin();
@@ -303,7 +370,7 @@ __device__ __forceinline__ void field_bwd_body(const FieldBwdParams& p, float* l
       *reinterpret_cast<uint4*>(a_row) = make_uint4(pack_h2(clamp_h(dun[0]), clamp_h(dun[1])), pack_h2(clamp_h(dun[2]), 0.f), 0u, 0u);
       *reinterpret_cast<uint4*>(a_row + kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
     }
-    sw.ready(kGsYb4, act);
+    ready(kGsYb4);
     // ---- B4^T -> dYb3 ----
     {
       Acc<dgrad::B4T> acc;
@@ -312,7 +379,7 @@ __device__ __forceinline__ void field_bwd_body(const FieldBwdParams& p, float* l
       wg_gemm_step<dgrad::B4T>(acc, ring, a_slab, W, 310);
       sw.begin();
       epi_mask_store<kMkHb4.cols>(acc, m, act, g);
-      sw.ready(kGsYb3, act);
+      ready(kGsYb3);
     }
     // ---- B3^T -> dYb2 = [dh * mask (64) | d rigidity pre-activation | 0 (15)] ----
     {
@@ -326,7 +393,7 @@ __device__ __forceinline__ void field_bwd_body(const FieldBwdParams& p, float* l
         *reinterpret_cast<uint4*>(a_row + 8 * kChunkBytes) = make_uint4(pack_h2(clamp_h(drpre), 0.f), 0u, 0u, 0u);
         *reinterpret_cast<uint4*>(a_row + 9 * kChunkBytes) = make_uint4(0u, 0u, 0u, 0u);
       }
-      sw.ready(kGsYb2, act);
+      ready(kGsYb2);
     }
     // ---- B2^T -> dYb1, B1^T -> dYb0 ----
     {
@@ -336,12 +403,12 @@ __device__ __forceinline__ void field_bwd_body(const FieldBwdParams& p, float* l
       wg_gemm_step<dgrad::B2T>(acc, ring, a_slab, W, 312);
       sw.begin();
       epi_mask_store<kMkHb2.cols>(acc, m, act, g);
-      sw.ready(kGsYb1, act);
+      ready(kGsYb1);
       m.load(mk + kMkHb1.off, g);
       wg_gemm_step<dgrad::B1T>(acc, ring, a_slab, W, 313);
       sw.begin();
       epi_mask_store<kMkHb1.cols>(acc, m, act, g);
-      sw.ready(kGsYb0, act);
+      ready(kGsYb0);
     }
     // ---- B0^T: d(bender input); columns 6..37 are the latent code -> per-ray reduction ----
     {
@@ -381,6 +448,12 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_kernel(const FieldBw
 // deterministic mode (bender only): the per-ray latent gradient goes through latent_rows and latent_reduce_kernel
 __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_det_kernel(const FieldBwdParams p, float* latent_rows) {
   field_bwd_body<true, true>(p, latent_rows);
+}
+// held-out rays (bender only): the latent gradient as field_bwd_kernel (DET = false) or field_bwd_det_kernel (DET = true)
+// forms it, the gradient-stash rows of held-out rays zero
+template <bool DET>
+__global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_held_kernel(const FieldBwdParams p, float* latent_rows, const uint8_t* held) {
+  field_bwd_body<true, DET, true>(p, latent_rows, held);
 }
 
 
@@ -540,6 +613,11 @@ cudaError_t launch_field_bwd(const FieldBwdParams& p, bool has_bender, int num_s
 
 cudaError_t launch_field_bwd_det(const FieldBwdParams& p, float* latent_rows, int num_sms, cudaStream_t stream) {
   return launch_field(field_bwd_det_kernel, p, num_sms, kBwdSmemBytes, stream, latent_rows);
+}
+
+cudaError_t launch_field_bwd_held(const FieldBwdParams& p, float* latent_rows, const uint8_t* held, int num_sms, cudaStream_t stream) {
+  if (latent_rows) return launch_field(field_bwd_held_kernel<true>, p, num_sms, kBwdSmemBytes, stream, latent_rows, held);
+  return launch_field(field_bwd_held_kernel<false>, p, num_sms, kBwdSmemBytes, stream, latent_rows, held);
 }
 
 cudaError_t launch_field_bwd_views(const FieldBwdParams& p, const ViewBwdParams& v, int num_sms, cudaStream_t stream) {

@@ -260,11 +260,17 @@ class training_wrapper_class(torch.nn.Module):
         self.ray_bender = ray_bender
 
     def forward(self, args, rays_o, rays_d, i, render_kwargs_train, target_s, global_step, start, dataset_extras,
-                batch_pixel_indices):
+                batch_pixel_indices, held_out=None):
+        """held_out [N] (bool or uint8, on the rays' device): rays of held-out frames (test_block_size, train.py:1376-1395),
+        whose loss reaches only their latent codes with a ray bender and nothing without one, so that one
+        ((train + test) * loss).mean().backward() with held_out=test gives the gradients of the reference's two backward
+        passes (train.py:1595-1608)."""
         # the view-dependent head cannot be trained with a bender yet: raise before any launch, for the bender seated below
         for net in (self.coarse_model, self.fine_model):
             if net is not None:
                 _ag.views_check(net, bender=self.ray_bender)
+        if held_out is not None:
+            _ag.check_held_out(held_out, rays_o.shape[0], target_s.device)
         self.coarse_model.ray_bender = (self.ray_bender,)
         render_kwargs_train["network_fn"] = self.coarse_model
         render_kwargs_train["ray_bender"] = self.ray_bender
@@ -282,7 +288,8 @@ class training_wrapper_class(torch.nn.Module):
         info = {"ray_bending_latents": _ag.gather_latents(self.latents, timestep)}
         detailed = args.offsets_loss_weight > 0.0 or args.divergence_loss_weight > 0.0
         rgb, disp, acc, extras = T.render(rays_o, rays_d, chunk=args.chunk, verbose=i < 10, retraw=True,
-                                          additional_pixel_information=info, detailed_output=detailed, **render_kwargs_train)
+                                          additional_pixel_information=info, detailed_output=detailed, held_out=held_out,
+                                          **render_kwargs_train)
         # increasing schedule of the regularisers, (1/100)^(1 - global_step / N_iters) (train.py:229, :281).  `global_step` may be
         # a 0-dim CUDA tensor: the schedule is then evaluated inside the loss kernel, so a step captured in a CUDA graph
         # follows it when replayed.
@@ -300,7 +307,8 @@ class training_wrapper_class(torch.nn.Module):
             rnd = render_kwargs_train.get("randomness")
             probes = rnd.get("e") if isinstance(rnd, dict) else None
             div = _ag.divergence_loss(extras["unmasked_offsets"], extras["rigidity_mask"], None, self.ray_bender,
-                                      e=None if probes is None else probes.to(dev).reshape(-1, 3), opacity_alpha=extras["opacity_alpha"])
+                                      e=None if probes is None else probes.to(dev).reshape(-1, 3), opacity_alpha=extras["opacity_alpha"],
+                                      held_out=held_out)
         # data term (fine + coarse), offsets / rigidity regulariser (train.py:208-242) and the weighted divergence term
         # (train.py:278-286) in one fused kernel
         loss = _ag.ray_loss(rgb, extras.get("rgb0"), target_s,

@@ -77,13 +77,17 @@ def raw2outputs(raw, z_vals, rays_d, raw_noise_std=0, white_bkgd=False, pytest=F
 # ---- render_rays (train.py:792-980) ---------------------------------------------------------------
 def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False, lindisp=False, perturb=0.0,
                 N_importance=0, network_fine=None, white_bkgd=False, raw_noise_std=0.0,
-                additional_pixel_information=None, detailed_output=False, verbose=False, pytest=False, **dummy_kwargs):
+                additional_pixel_information=None, detailed_output=False, verbose=False, pytest=False, held_out=None, **dummy_kwargs):
     """Volumetric rendering of a ray batch [N, 8] = (o, d, near, far).  `network_query_fn` is accepted
     for signature compatibility; the field is evaluated by the fused kernel on `network_fn` /
     `network_fine` (which carry their ray bender as `.ray_bender[0]`).
     Extra keyword `randomness` (dict with t_rand, noise_c, u, noise_f; unit-variance noise) replaces
     the internal draws -- the supported way to reproduce a run exactly (the reference's `pytest` hook
-    re-seeds numpy instead, train.py:863-867)."""
+    re-seeds numpy instead, train.py:863-867).
+    held_out [N] (bool or uint8, on the rays' device): rays of held-out frames.  With a ray bender their gradient reaches
+    only their latent codes, not the coarse, fine or bender weights; without one they contribute no gradient at all.  So
+    one backward of ((train + held_out) * loss).mean() gives the gradients of the reference's two backward passes
+    (train.py:1595-1608).  None: the ordinary path."""
     if pytest:
         raise RuntimeError("nonrigid_nerf_b200: the pytest= numpy-random hook is not supported")
     if not isinstance(network_fn, NeRF) or (network_fine is not None and not isinstance(network_fine, NeRF)):
@@ -91,6 +95,7 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     _check_views(ray_batch.shape[-1] > 8, network_fn, network_fine if N_importance > 0 else None, additional_pixel_information)
     n = ray_batch.shape[0]
     dev = ray_batch.device
+    _ag.check_held_out(held_out, n, dev)
     rays = ray_batch if (ray_batch.dtype == torch.float32 and ray_batch.is_contiguous()) else ray_batch.float().contiguous()
     viewdirs = None
     if rays.shape[-1] > 8:   # (o, d, near, far, viewdirs): train.py:843
@@ -134,7 +139,7 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     # coarse depths (train.py:847-869); t_rand drawn first, like the reference
     t_rand = draw("t_rand", torch.rand, n, N_samples) if perturb > 0.0 else None
     z_vals = ops.sample_coarse(rays, N_samples, t_rand, lindisp)
-    raw, details = _ag.field(network_fn, rays, z_vals, latents, detailed_output, viewdirs)
+    raw, details = _ag.field(network_fn, rays, z_vals, latents, detailed_output, viewdirs, held_out)
     noise = draw("noise_c", torch.randn, n, N_samples) if raw_noise_std > 0.0 else None   # already scaled by raw_noise_std
 
     if N_importance > 0:
@@ -142,7 +147,7 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
         c0 = _ag.composite(raw, z_vals, rays_d, noise, white_bkgd, N_importance, u)
         z_fine = c0["z_vals_out"]   # sorted union, detached (train.py:918-920)
         run_fn = network_fn if network_fine is None else network_fine
-        raw, fine_details = _ag.field(run_fn, rays, z_fine, latents, detailed_output, viewdirs)
+        raw, fine_details = _ag.field(run_fn, rays, z_fine, latents, detailed_output, viewdirs, held_out)
         noise_f = draw("noise_f", torch.randn, n, n_fine) if raw_noise_std > 0.0 else None
         c1 = _ag.composite(raw, z_fine, rays_d, noise_f, white_bkgd)
     else:
@@ -211,9 +216,12 @@ def _check_views(batch_has_viewdirs, network_fn, network_fine, additional_pixel_
 def batchify_rays(rays_flat, additional_pixel_information, chunk=1024 * 32, detailed_output=False, **kwargs):
     """Render rays in chunks (`chunk` only bounds the per-launch working set; results do not depend on it)."""
     all_ret = {}
+    held_out = kwargs.pop("held_out", None)
     for i in range(0, rays_flat.shape[0], chunk):
         info = {"ray_bending_latents": additional_pixel_information["ray_bending_latents"][i:i + chunk, :]}
-        ret = render_rays(rays_flat[i:i + chunk], additional_pixel_information=info, detailed_output=detailed_output, **kwargs)
+        held = None if held_out is None else held_out[i:i + chunk]
+        ret = render_rays(rays_flat[i:i + chunk], additional_pixel_information=info, detailed_output=detailed_output,
+                          held_out=held, **kwargs)
         for k in ret:
             all_ret.setdefault(k, []).append(ret[k])
     return {k: (v[0] if len(v) == 1 else torch.cat(v, 0)) for k, v in all_ret.items()}
@@ -221,7 +229,8 @@ def batchify_rays(rays_flat, additional_pixel_information, chunk=1024 * 32, deta
 
 def render(rays_o, rays_d, chunk=1024 * 32, ndc=True, near=0.0, far=1.0, use_viewdirs=False, c2w_staticcam=None,
            additional_pixel_information=None, detailed_output=False, **kwargs):
-    """Render rays.  Returns [rgb_map, disp_map, acc_map, extras] (train.py:326-416)."""
+    """Render rays.  Returns [rgb_map, disp_map, acc_map, extras] (train.py:326-416).  Keyword held_out [N] (one entry
+    per ray of the flattened batch): see render_rays."""
     if kwargs.get("network_fn") is not None:
         _check_views(bool(use_viewdirs), kwargs["network_fn"], kwargs.get("network_fine") if kwargs.get("N_importance", 0) > 0 else None,
                      additional_pixel_information)
@@ -238,6 +247,7 @@ def render(rays_o, rays_d, chunk=1024 * 32, ndc=True, near=0.0, far=1.0, use_vie
         raise RuntimeError("nonrigid_nerf_b200: rays must be CUDA tensors (there is no CPU path)")
     rays_o = torch.reshape(rays_o, [-1, 3]).float()
     rays_d = torch.reshape(rays_d, [-1, 3]).float()
+    _ag.check_held_out(kwargs.get("held_out"), rays_d.shape[0], rays_d.device)
     if isinstance(near, torch.Tensor) or isinstance(far, torch.Tensor) or np.ndim(near) > 0 or np.ndim(far) > 0:
         near_t = torch.as_tensor(near, dtype=torch.float32, device=rays_d.device) * torch.ones_like(rays_d[..., :1])
         far_t = torch.as_tensor(far, dtype=torch.float32, device=rays_d.device) * torch.ones_like(rays_d[..., :1])
