@@ -416,6 +416,48 @@ typedef struct NrnPeerCtx {
 int nrn_peer_reduce_adam(const NrnPeerCtx* ctx, const NrnAdamArgs* adam);
 int nrn_peer_gather_rows(const NrnPeerCtx* ctx, const float* local, int n_per_rank, float* out, void* stream);
 
+/* ---- evaluation and visualisation of rendered frames: what free_viewpoint_rendering.py does on the host with numpy,
+ * scikit-image and matplotlib once the frames are rendered.  Frames are fp32 [n_frames][height][width][3] (disparity
+ * [n_frames][height][width]), any sizes >= 1; n_frames = 0 returns NRN_OK and launches nothing.  Every score is a sum in
+ * a fixed order (no atomics): bit-reproducible.  Colour images index matplotlib's 256-entry cm.jet table with
+ * uint8(255 * clip(v, 0, 1)) (truncation, as .astype("uint8")); a NaN value takes entry 0. ---------------------------- */
+/* The cm.jet table the kernels use, built from matplotlib's published segment data (_jet_data) the way matplotlib's
+ * LinearSegmentedColormap builds it: rgb [256][3] = cm.jet(i)[:3] (float64), rgb8 [256][3] = to8b(rgb); either may be
+ * NULL.  Host only: no CUDA call. */
+int nrn_jet_colormap(double* rgb, uint8_t* rgb8);
+/* Scores of free_viewpoint_rendering.py:818-862.  The mask (:820-823): pixels whose ground-truth channels sum to 0 in the
+ * FIRST frame scored are zeroed in both images of every frame.  psnr = -10 log10(mean((gt - gen)^2)) over all
+ * height * width * 3 values (+inf for identical frames, as the reference's log10(0)).  ssim = skimage
+ * structural_similarity(data_range=1, gaussian_weights=True, sigma=1.5, use_sample_covariance=False, multichannel=True,
+ * full=True): per channel, 11-tap Gaussian window (truncate 3.5) with mode "reflect", C1 = 0.01^2, C2 = 0.03^2; the
+ * score is the mean of the map S over the frame cropped by 5 pixels on every side and over the channels (NaN when
+ * height or width <= 10, as the mean of an empty crop).  The error images (:845-856) are to8b(jet(clip(10 |gt - gen|_2 /
+ * sqrt(3)))) and to8b(jet(1 - mean_c S)).  The Gaussian moments and S in fp64 (S written as fp32), sums in fp64. */
+size_t nrn_image_scores_bytes(int n_frames, int height, int width);   /* workspace: per-tile partial sums + a derived mask */
+typedef struct NrnImageScoreArgs {
+  const float* gt;            /* [F][H][W][3] ground truth */
+  const float* generated;     /* [F][H][W][3] rendered */
+  const uint8_t* mask;        /* [H][W] nonzero = masked, or NULL: derived from gt frame 0 into the workspace */
+  int32_t n_frames, height, width;
+  float* psnr;                /* out [F] */
+  float* ssim;                /* out [F] */
+  float* ssim_map;            /* out [F][H][W][3] the map S, or NULL */
+  uint8_t* error_rgb;         /* out [F][H][W][3] scaled RGB error on jet, or NULL */
+  uint8_t* error_ssim;        /* out [F][H][W][3] 1 - SSIM on jet, or NULL */
+  void* workspace;            /* nrn_image_scores_bytes(), 16-byte aligned */
+  void* stream;
+} NrnImageScoreArgs;
+int nrn_image_scores(const NrnImageScoreArgs* args);
+/* visualize_disparity_with_jet_color_scheme and visualize_disparity_with_blinn_phong (run_nerf_helpers.py:701-793) for
+ * every frame of disp [F][H][W]: jet [F][H][W][3] = the cm.jet colour of clip(d, 0, 1); phong [F][H][W][3] = the
+ * reference's Blinn-Phong shading of the normals of np.gradient(d, 2 / (H - 1)) (needs H, W >= 2, as np.gradient does),
+ * in fp32 (the reference mixes float32 and float64).  Either output may be NULL, not both. */
+int nrn_disparity_images(const float* disp, int n_frames, int height, int width, float* jet, float* phong, void* stream);
+/* Background stability of a fixed-camera sequence (free_viewpoint_rendering.py:770-785) over rgbs [F][H][W][3]:
+ * std [H][W][3] = np.std(rgbs, axis=0) (ddof 0, two passes in fp32, frame-ordered sums as numpy's), image [H][W][3] =
+ * the cm.jet colour of 10 * mean_c std.  Either output may be NULL, not both. */
+int nrn_frame_std_image(const float* rgbs, int n_frames, int height, int width, float* std, float* image, void* stream);
+
 /* ---- optional per-kernel timing (measurement aid for bench.py) ---------------------------------
  * While enabled, every launch of the kernel kinds below is bracketed by CUDA events recorded on the
  * launch stream.  kinds: 0 field forward, 1 field DGRAD, 2 WGRAD (+reduce), 3 composite(+resample),
@@ -425,7 +467,8 @@ int nrn_peer_gather_rows(const NrnPeerCtx* ctx, const float* local, int n_per_ra
  * and 12 its WGRAD (+reduce) (nrn_field_backward_views), 13 the fixed-order latent reduction (nrn_field_backward_det) and
  * 14 the fixed-order divergence loss reduction (nrn_divergence_forward_det), 15 the held-out DGRAD
  * (nrn_field_backward_held_out, nrn_field_backward_det_held_out) and 16 the held-out divergence backward
- * (nrn_divergence_backward_held_out; its WGRAD is kind 2).  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * (nrn_divergence_backward_held_out; its WGRAD is kind 2), 17 nrn_image_scores (mask, SSIM tiles, per-frame reduction),
+ * 18 nrn_disparity_images and 19 nrn_frame_std_image.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

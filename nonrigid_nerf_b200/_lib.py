@@ -137,6 +137,15 @@ class NrnCompositeBwdArgs(C.Structure):
     ]
 
 
+class NrnImageScoreArgs(C.Structure):
+    _fields_ = [
+        ("gt", _vp), ("generated", _vp), ("mask", _vp),
+        ("n_frames", C.c_int32), ("height", C.c_int32), ("width", C.c_int32),
+        ("psnr", _vp), ("ssim", _vp), ("ssim_map", _vp), ("error_rgb", _vp), ("error_ssim", _vp),
+        ("workspace", _vp), ("stream", _vp),
+    ]
+
+
 # every symbol include/nrnerf_b200.h declares: (restype, argtypes)
 SYMBOLS = {
     "nrn_abi_version": (C.c_int, []),
@@ -201,6 +210,11 @@ SYMBOLS = {
     "nrn_peer_free": (C.c_int, [_vp]),
     "nrn_peer_reduce_adam": (C.c_int, [C.POINTER(NrnPeerCtx), C.POINTER(NrnAdamArgs)]),
     "nrn_peer_gather_rows": (C.c_int, [C.POINTER(NrnPeerCtx), _vp, C.c_int, _vp, _vp]),
+    "nrn_jet_colormap": (C.c_int, [_vp, _vp]),
+    "nrn_image_scores_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "nrn_image_scores": (C.c_int, [C.POINTER(NrnImageScoreArgs)]),
+    "nrn_disparity_images": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),
+    "nrn_frame_std_image": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),
     "nrn_timing_enable": (C.c_int, [C.c_int]),
     "nrn_timing_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int), C.c_int]),
 }
@@ -216,6 +230,8 @@ VIEW_TRAIN_KERNEL_KINDS = ("views_field_train", "views_dgrad", "views_wgrad")
 DET_KERNEL_KINDS = ("latent_reduce", "div_loss_reduce")
 # the held-out variants of DGRAD and of the divergence backward (render(..., held_out=)), timing kinds 15 and 16
 HELD_OUT_KERNEL_KINDS = ("field_dgrad_held_out", "div_bwd_held_out")
+# evaluation of rendered frames (image scores, disparity images, background stability), timing kinds 17 to 19
+EVAL_KERNEL_KINDS = ("image_scores", "disparity_images", "frame_std_image")
 
 
 def timing_enable(on: bool) -> None:
@@ -225,7 +241,7 @@ def timing_enable(on: bool) -> None:
 def timing_read(kinds=KERNEL_KINDS):
     """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True); `kinds` is KERNEL_KINDS,
     KERNEL_KINDS + TC_KERNEL_KINDS, KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS, that + VIEW_TRAIN_KERNEL_KINDS,
-    that + DET_KERNEL_KINDS or that + HELD_OUT_KERNEL_KINDS."""
+    that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS or that + EVAL_KERNEL_KINDS."""
     n = len(kinds)
     ms = (C.c_double * n)()
     cnt = (C.c_int * n)()

@@ -14,6 +14,7 @@
 #include "adam.cuh"
 #include "peer.cuh"
 #include "det_reduce.cuh"
+#include "eval.cuh"
 
 namespace nrn {
 cudaError_t launch_field_fwd(const FieldFwdParams& p, bool has_bender, int num_sms, cudaStream_t stream);
@@ -937,6 +938,77 @@ int nrn_peer_gather_rows(const NrnPeerCtx* c, const float* local, int n_per_rank
   if (rc) return rc;
   const cudaError_t e = nrn::launch_peer_gather(pc, static_cast<uint32_t*>(c->state), local, n_per_rank, out, ds->err_word, static_cast<cudaStream_t>(stream));
   return e == cudaSuccess ? NRN_OK : cuda_fail(e, "peer_collect_kernel");
+}
+
+// ---- evaluation and visualisation of rendered frames (eval.cu) ----
+int nrn_jet_colormap(double* rgb, uint8_t* rgb8) {
+  if (!rgb && !rgb8) return fail(NRN_E_INVALID, "nrn_jet_colormap: null argument");
+  nrn::jet_table(rgb, rgb8);
+  return NRN_OK;
+}
+
+static bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }   // NULL passes
+static size_t eval_mask_offset(int F, int H, int W) { return (nrn::eval_partials_bytes(F, H, W) + 15) / 16 * 16; }
+
+size_t nrn_image_scores_bytes(int n_frames, int height, int width) {
+  if (n_frames < 0 || height < 1 || width < 1) return 0;
+  return eval_mask_offset(n_frames, height, width) + (static_cast<size_t>(height) * width + 15) / 16 * 16;
+}
+
+// The sizes every evaluation entry point accepts: n_frames >= 0, height and width >= 1, and a grid of at most 2^31 - 1
+// blocks of `per_block` elements (n_frames * height * width pixels or SSIM tiles)
+static int check_frames(int F, int H, int W, long long per_frame, long long per_block, const char* who) {
+  if (F < 0 || H < 1 || W < 1) return fail(NRN_E_INVALID, "%s: bad sizes F=%d H=%d W=%d", who, F, H, W);
+  if ((static_cast<long long>(F) * per_frame + per_block - 1) / per_block > 0x7fffffffLL) return fail(NRN_E_INVALID, "%s: too many frames", who);
+  return NRN_OK;
+}
+
+int nrn_image_scores(const NrnImageScoreArgs* a) {
+  const char* who = "nrn_image_scores";
+  if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
+  int rc = check_frames(a->n_frames, a->height, a->width, nrn::eval_tiles_per_frame(a->height, a->width), 1, who);
+  if (rc) return rc;
+  if (a->n_frames == 0) return NRN_OK;
+  if (!a->gt || !a->generated || !a->psnr || !a->ssim || !a->workspace) return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (!aligned16(a->workspace)) return fail(NRN_E_INVALID, "%s: workspace must be 16-byte aligned", who);
+  if (!aligned4(a->gt) || !aligned4(a->generated) || !aligned4(a->psnr) || !aligned4(a->ssim) || !aligned4(a->ssim_map))
+    return fail(NRN_E_INVALID, "%s: float arrays must be 4-byte aligned", who);
+  const int F = a->n_frames, H = a->height, W = a->width;
+  uint8_t* derived = static_cast<uint8_t*>(a->workspace) + eval_mask_offset(F, H, W);
+  nrn::ImageScoreParams p{a->gt, a->generated, a->mask ? a->mask : derived, F, H, W, a->psnr, a->ssim, a->ssim_map,
+                          a->error_rgb, a->error_ssim, static_cast<double*>(a->workspace)};
+  const cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  if (!a->mask) {
+    rc = timed(17, st, "frame_mask_kernel", [&] { return nrn::launch_frame_mask(a->gt, H, W, derived, st); });
+    if (rc) return rc;
+  }
+  rc = timed(17, st, "ssim_tile_kernel", [&] { return nrn::launch_image_scores(p, st); });
+  if (rc) return rc;
+  return timed(17, st, "score_reduce_kernel", [&] { return nrn::launch_score_reduce(p, st); });
+}
+
+int nrn_disparity_images(const float* disp, int F, int H, int W, float* jet, float* phong, void* stream) {
+  const char* who = "nrn_disparity_images";
+  int rc = check_frames(F, H, W, static_cast<long long>(H) * W, 256, who);
+  if (rc) return rc;
+  if (phong && (H < 2 || W < 2)) return fail(NRN_E_INVALID, "%s: the Phong image needs height and width >= 2 (np.gradient)", who);
+  if (F == 0) return NRN_OK;
+  if (!disp || (!jet && !phong)) return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (!aligned4(disp) || !aligned4(jet) || !aligned4(phong)) return fail(NRN_E_INVALID, "%s: float arrays must be 4-byte aligned", who);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return timed(18, st, "disparity_kernel", [&] { return nrn::launch_disparity_images(disp, F, H, W, jet, phong, st); });
+}
+
+int nrn_frame_std_image(const float* rgbs, int F, int H, int W, float* std_out, float* image, void* stream) {
+  const char* who = "nrn_frame_std_image";
+  int rc = check_frames(1, H, W, static_cast<long long>(H) * W, 128, who);
+  if (rc) return rc;
+  if (F < 0) return fail(NRN_E_INVALID, "%s: bad sizes F=%d", who, F);
+  if (F == 0) return NRN_OK;
+  if (!rgbs || (!std_out && !image)) return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (!aligned4(rgbs) || !aligned4(std_out) || !aligned4(image)) return fail(NRN_E_INVALID, "%s: float arrays must be 4-byte aligned", who);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return timed(19, st, "frame_std_kernel", [&] { return nrn::launch_frame_std(rgbs, F, H, W, std_out, image, st); });
 }
 
 // Turning timing off only stops recording: a CUDA graph captured while it was on keeps event-record nodes that refer to

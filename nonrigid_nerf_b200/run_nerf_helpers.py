@@ -6,7 +6,7 @@ output_linear.*, network.N.*, rigidity_network.N.*), but every forward dispatche
 sm_90a kernels through the C ABI.  There is no PyTorch fallback: unsupported configurations raise.
 
 Reference: run_nerf_helpers.py:10-19 (misc), :120-168 (Embedder), :172-385 (NeRF), :388-584
-(ray_bending), :651-698 (sample_pdf).
+(ray_bending), :651-698 (sample_pdf), :701-793 (disparity visualisation).
 """
 from __future__ import annotations
 
@@ -216,6 +216,27 @@ def sample_pdf(bins, weights, N_samples, det=False, pytest=False):
     out = ops.sample_pdf_op(bins.reshape(-1, bins.shape[-1]), weights.reshape(-1, weights.shape[-1]), N_samples,
                             None if u is None else u.reshape(-1, N_samples))
     return out.reshape(*lead, N_samples)
+
+
+# ---- disparity visualisation (run_nerf_helpers.py:701-793) ------------------------------------------------
+def _disparity_image(depth_map, which: int):
+    """One disparity map [H, W] through evaluation.disparity_images: a CUDA tensor gives a CUDA tensor [H, W, 3] (no
+    host copy), anything else is read as a numpy array and gives a numpy array, like the reference."""
+    from . import evaluation
+    if isinstance(depth_map, torch.Tensor) and depth_map.is_cuda:
+        return evaluation.disparity_images(depth_map[None], jet=which == 0, phong=which == 1)[which][0]
+    d = torch.from_numpy(np.ascontiguousarray(depth_map, dtype=np.float32)).cuda()
+    return evaluation.disparity_images(d[None], jet=which == 0, phong=which == 1)[which][0].cpu().numpy()
+
+
+def visualize_disparity_with_jet_color_scheme(depth_map_in):
+    """cm.jet colours [H, W, 3] of clip(depth_map_in, 0, 1) (fp32 values of the float64 table)."""
+    return _disparity_image(depth_map_in, 0)
+
+
+def visualize_disparity_with_blinn_phong(depth_map):
+    """The reference's Blinn-Phong shading [H, W, 3] of the normals of the disparity map [H, W] (H, W >= 2), in fp32."""
+    return _disparity_image(depth_map, 1)
 
 
 # ---- divergence regulariser (run_nerf_helpers.py:22-116) --------------------------------------------
