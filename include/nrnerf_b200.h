@@ -457,6 +457,41 @@ int nrn_disparity_images(const float* disp, int n_frames, int height, int width,
  * std [H][W][3] = np.std(rgbs, axis=0) (ddof 0, two passes in fp32, frame-ordered sums as numpy's), image [H][W][3] =
  * the cm.jet colour of 10 * mean_c std.  Either output may be NULL, not both. */
 int nrn_frame_std_image(const float* rgbs, int n_frames, int height, int width, float* std, float* image, void* stream);
+/* The 8-bit images free_viewpoint_rendering.py saves per frame and as videos (:615-766), for a stack of F frames of
+ * H x W pixels, in at most two launches (the per-frame maxima of disp, then every image).  Each output is written only
+ * when its pointer is not NULL, and needs its input:
+ *   out_rgb [F][H][W][3]             to8b(rgb)                                   (convert_rgb_to_saveable)
+ *   out_disp [F][H][W]               to8b(disp / max of that frame), fp32        (convert_disparity_to_saveable)
+ *   out_disp_video [F][H][W]         to8b(disp / max over all F frames)          (the disparity video, :725-730)
+ *   out_disp_jet [F][H][W][3]        to8b(jet(disp / frame max))                 (convert_disparity_to_jet)
+ *   out_disp_phong [F][H][W][3]      to8b of nrn_disparity_images' fp32 Phong value of disp / frame max (needs H, W >= 2)
+ *   out_correspondences [F][H][W][3] c = (p - min) / (max - min) * 100 in fp64, to8b(c - trunc(c))    (:640-644)
+ *   out_rigidity [F][H][W]           to8b(rigidity)                              (normalize=False)
+ *   out_rigidity_jet [F][H][W][3]    to8b(jet(rigidity))                         (normalize=False)
+ * to8b(v) = uint8(255 * clip(v, 0, 1)), truncated, NaN -> 0.  The disparity maxima follow np.max (a NaN makes the frame's
+ * maximum NaN) and are written to disp_max, which every disparity output needs.  NULL args, negative sizes, an output
+ * without its input, max_point <= min_point on an axis and float arrays not 4-byte aligned return NRN_E_INVALID before
+ * any CUDA call; F = 0 or H * W = 0 returns NRN_OK and launches nothing. */
+typedef struct NrnFrameImageArgs {
+  const float* rgb;                /* [F][H][W][3] rendered colours, or NULL */
+  const float* disp;               /* [F][H][W] disparity, or NULL */
+  const float* surface_pts;        /* [F][H*W][3] canonical point of each pixel's median-visibility sample, or NULL */
+  const float* surface_rigidity;   /* [F][H*W] its rigidity, or NULL (no bender) */
+  const double* min_point;         /* host [3]: the checkpoint's min_nerf_volume_point (needed by out_correspondences) */
+  const double* max_point;         /* host [3]: max_nerf_volume_point */
+  int32_t n_frames, height, width;
+  float* disp_max;                 /* out [F]: the maximum of each disparity frame (needed by every disparity output) */
+  uint8_t* out_rgb;
+  uint8_t* out_disp;
+  uint8_t* out_disp_video;
+  uint8_t* out_disp_jet;
+  uint8_t* out_disp_phong;
+  uint8_t* out_correspondences;
+  uint8_t* out_rigidity;
+  uint8_t* out_rigidity_jet;
+  void* stream;
+} NrnFrameImageArgs;
+int nrn_frame_images(const NrnFrameImageArgs* args);
 
 /* ---- optional per-kernel timing (measurement aid for bench.py) ---------------------------------
  * While enabled, every launch of the kernel kinds below is bracketed by CUDA events recorded on the
@@ -468,7 +503,7 @@ int nrn_frame_std_image(const float* rgbs, int n_frames, int height, int width, 
  * 14 the fixed-order divergence loss reduction (nrn_divergence_forward_det), 15 the held-out DGRAD
  * (nrn_field_backward_held_out, nrn_field_backward_det_held_out) and 16 the held-out divergence backward
  * (nrn_divergence_backward_held_out; its WGRAD is kind 2), 17 nrn_image_scores (mask, SSIM tiles, per-frame reduction),
- * 18 nrn_disparity_images and 19 nrn_frame_std_image.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * 18 nrn_disparity_images, 19 nrn_frame_std_image and 20 nrn_frame_images.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

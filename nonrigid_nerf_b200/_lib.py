@@ -146,6 +146,18 @@ class NrnImageScoreArgs(C.Structure):
     ]
 
 
+class NrnFrameImageArgs(C.Structure):
+    _fields_ = [
+        ("rgb", _vp), ("disp", _vp), ("surface_pts", _vp), ("surface_rigidity", _vp),
+        ("min_point", _vp), ("max_point", _vp),
+        ("n_frames", C.c_int32), ("height", C.c_int32), ("width", C.c_int32),
+        ("disp_max", _vp),
+        ("out_rgb", _vp), ("out_disp", _vp), ("out_disp_video", _vp), ("out_disp_jet", _vp), ("out_disp_phong", _vp),
+        ("out_correspondences", _vp), ("out_rigidity", _vp), ("out_rigidity_jet", _vp),
+        ("stream", _vp),
+    ]
+
+
 # every symbol include/nrnerf_b200.h declares: (restype, argtypes)
 SYMBOLS = {
     "nrn_abi_version": (C.c_int, []),
@@ -215,6 +227,7 @@ SYMBOLS = {
     "nrn_image_scores": (C.c_int, [C.POINTER(NrnImageScoreArgs)]),
     "nrn_disparity_images": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),
     "nrn_frame_std_image": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),
+    "nrn_frame_images": (C.c_int, [C.POINTER(NrnFrameImageArgs)]),
     "nrn_timing_enable": (C.c_int, [C.c_int]),
     "nrn_timing_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int), C.c_int]),
 }
@@ -232,6 +245,8 @@ DET_KERNEL_KINDS = ("latent_reduce", "div_loss_reduce")
 HELD_OUT_KERNEL_KINDS = ("field_dgrad_held_out", "div_bwd_held_out")
 # evaluation of rendered frames (image scores, disparity images, background stability), timing kinds 17 to 19
 EVAL_KERNEL_KINDS = ("image_scores", "disparity_images", "frame_std_image")
+# the saved 8-bit images of rendered frames (disparity maxima + every image), timing kind 20
+FRAME_IMAGE_KERNEL_KINDS = ("frame_images",)
 
 
 def timing_enable(on: bool) -> None:
@@ -241,7 +256,7 @@ def timing_enable(on: bool) -> None:
 def timing_read(kinds=KERNEL_KINDS):
     """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True); `kinds` is KERNEL_KINDS,
     KERNEL_KINDS + TC_KERNEL_KINDS, KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS, that + VIEW_TRAIN_KERNEL_KINDS,
-    that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS or that + EVAL_KERNEL_KINDS."""
+    that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS, that + EVAL_KERNEL_KINDS or that + FRAME_IMAGE_KERNEL_KINDS."""
     n = len(kinds)
     ms = (C.c_double * n)()
     cnt = (C.c_int * n)()

@@ -1011,6 +1011,49 @@ int nrn_frame_std_image(const float* rgbs, int F, int H, int W, float* std_out, 
   return timed(19, st, "frame_std_kernel", [&] { return nrn::launch_frame_std(rgbs, F, H, W, std_out, image, st); });
 }
 
+int nrn_frame_images(const NrnFrameImageArgs* a) {
+  const char* who = "nrn_frame_images";
+  if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
+  const int F = a->n_frames, H = a->height, W = a->width;
+  if (F < 0 || H < 0 || W < 0) return fail(NRN_E_INVALID, "%s: bad sizes F=%d H=%d W=%d", who, F, H, W);
+  if (static_cast<double>(F) * H * W * 3 > 9.0e18) return fail(NRN_E_INVALID, "%s: too many pixels", who);
+  if (static_cast<long long>(F) * H * W == 0) return NRN_OK;
+  const bool disp_out = a->out_disp || a->out_disp_video || a->out_disp_jet || a->out_disp_phong;
+  if (!a->out_rgb && !disp_out && !a->out_correspondences && !a->out_rigidity && !a->out_rigidity_jet)
+    return fail(NRN_E_INVALID, "%s: no output", who);
+  if ((a->out_rgb && !a->rgb) || (disp_out && (!a->disp || !a->disp_max)) ||
+      (a->out_correspondences && (!a->surface_pts || !a->min_point || !a->max_point)) ||
+      ((a->out_rigidity || a->out_rigidity_jet) && !a->surface_rigidity))
+    return fail(NRN_E_INVALID, "%s: an output without its input (null argument)", who);
+  if (a->out_disp_phong && (H < 2 || W < 2))
+    return fail(NRN_E_INVALID, "%s: the Phong image needs height and width >= 2 (np.gradient)", who);
+  if (!aligned4(a->rgb) || !aligned4(a->disp) || !aligned4(a->surface_pts) || !aligned4(a->surface_rigidity) || !aligned4(a->disp_max))
+    return fail(NRN_E_INVALID, "%s: float arrays must be 4-byte aligned", who);
+  nrn::FrameImageParams p{};
+  if (a->out_correspondences)
+    for (int c = 0; c < 3; ++c) {
+      if (!(a->max_point[c] > a->min_point[c])) return fail(NRN_E_INVALID, "%s: max_point must exceed min_point on every axis", who);
+      p.min_point[c] = a->min_point[c];
+      p.max_point[c] = a->max_point[c];
+    }
+  // inputs whose outputs are not asked for stay unread
+  p.rgb = a->out_rgb ? a->rgb : nullptr;
+  p.disp = disp_out ? a->disp : nullptr;
+  p.surface_pts = a->out_correspondences ? a->surface_pts : nullptr;
+  p.surface_rigidity = (a->out_rigidity || a->out_rigidity_jet) ? a->surface_rigidity : nullptr;
+  p.F = F; p.H = H; p.W = W;
+  p.disp_max = a->disp_max;
+  p.out_rgb = a->out_rgb; p.out_disp = a->out_disp; p.out_disp_video = a->out_disp_video; p.out_disp_jet = a->out_disp_jet;
+  p.out_disp_phong = a->out_disp_phong; p.out_correspondences = a->out_correspondences; p.out_rigidity = a->out_rigidity;
+  p.out_rigidity_jet = a->out_rigidity_jet;
+  const cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  if (disp_out) {
+    const int rc = timed(20, st, "disp_max_kernel", [&] { return nrn::launch_disp_max(a->disp, F, H, W, a->disp_max, st); });
+    if (rc) return rc;
+  }
+  return timed(20, st, "frame_images_kernel", [&] { return nrn::launch_frame_images(p, st); });
+}
+
 // Turning timing off only stops recording: a CUDA graph captured while it was on keeps event-record nodes that refer to
 // these events and may still be replayed.  They are released when a new timing session starts.
 int nrn_timing_enable(int on) {

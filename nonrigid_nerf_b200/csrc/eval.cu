@@ -235,24 +235,11 @@ __global__ void score_reduce_kernel(ImageScoreParams p, int tiles_per_frame) {
 }
 
 // ---- disparity images, run_nerf_helpers.py:701-793 ----------------------------------------------------------------------
-// jet: the LUT colour of clip(d, 0, 1).  Blinn-Phong: normals from np.gradient(d, 2 / (H - 1)) (central differences
-// inside, one-sided at the edges, fp32 as numpy computes them for a float32 map), then the reference's light / view /
-// half vectors and constants, in fp32
-__global__ void disparity_kernel(const float* __restrict__ disp, int F, int H, int W, float* __restrict__ jet,
-                                 float* __restrict__ phong, float inv_c, float inv_e) {
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  const long long n_pix = static_cast<long long>(H) * W;
-  if (i >= n_pix * F) return;
-  const long long f = i / n_pix;
-  const int y = static_cast<int>((i - f * n_pix) / W), x = static_cast<int>(i - f * n_pix - static_cast<long long>(y) * W);
-  const float* dm = disp + f * n_pix;
-  const float d = dm[static_cast<long long>(y) * W + x];
-  if (jet) {
-    const int k = lut_index(d);
-    for (int c = 0; c < 3; ++c) jet[i * 3 + c] = c_jet.rgbf[k * 3 + c];
-  }
-  if (!phong) return;
-  auto at = [&](int yy, int xx) { return dm[static_cast<long long>(yy) * W + xx]; };
+// Blinn-Phong colour of pixel (y, x) of an H x W disparity map read through at(yy, xx), d = at(y, x): normals from
+// np.gradient(d, 2 / (H - 1)) (central differences inside, one-sided at the edges, fp32 as numpy computes them for a
+// float32 map), then the reference's light / view / half vectors and constants, in fp32
+template <typename At>
+__device__ __forceinline__ void blinn_phong(At at, float d, int y, int x, int H, int W, float inv_c, float inv_e, float rgb[3]) {
   const float zy = y == 0 ? __fdiv_rn(__fsub_rn(at(1, x), at(0, x)), inv_e)
                  : y == H - 1 ? __fdiv_rn(__fsub_rn(at(H - 1, x), at(H - 2, x)), inv_e)
                               : __fdiv_rn(__fsub_rn(at(y + 1, x), at(y - 1, x)), inv_c);
@@ -279,8 +266,119 @@ __global__ void disparity_kernel(const float* __restrict__ disp, int F, int H, i
   const float specular = lambertian <= 0.f ? 0.f : spec_angle * spec_angle;   // invalid_mask
   const float light_power = 2.f;
   const float diffuse[3] = {0.5f, 0.f, 0.f}, ambient[3] = {0.1f, 0.f, 0.f};
-  for (int c = 0; c < 3; ++c)
-    phong[i * 3 + c] = lambertian * diffuse[c] * light_power / att + specular * light_power / att + ambient[c];
+  for (int c = 0; c < 3; ++c) rgb[c] = lambertian * diffuse[c] * light_power / att + specular * light_power / att + ambient[c];
+}
+
+// jet: the LUT colour of clip(d, 0, 1); Blinn-Phong as above
+__global__ void disparity_kernel(const float* __restrict__ disp, int F, int H, int W, float* __restrict__ jet,
+                                 float* __restrict__ phong, float inv_c, float inv_e) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const long long n_pix = static_cast<long long>(H) * W;
+  if (i >= n_pix * F) return;
+  const long long f = i / n_pix;
+  const int y = static_cast<int>((i - f * n_pix) / W), x = static_cast<int>(i - f * n_pix - static_cast<long long>(y) * W);
+  const float* dm = disp + f * n_pix;
+  const float d = dm[static_cast<long long>(y) * W + x];
+  if (jet) {
+    const int k = lut_index(d);
+    for (int c = 0; c < 3; ++c) jet[i * 3 + c] = c_jet.rgbf[k * 3 + c];
+  }
+  if (!phong) return;
+  float rgb[3];
+  blinn_phong([&](int yy, int xx) { return dm[static_cast<long long>(yy) * W + xx]; }, d, y, x, H, W, inv_c, inv_e, rgb);
+  for (int c = 0; c < 3; ++c) phong[i * 3 + c] = rgb[c];
+}
+
+// ---- the saved 8-bit images of free_viewpoint_rendering.py:615-766 ------------------------------------------------------
+// to8b(v) = uint8(255 * clip(v, 0, 1)) is lut_index(v): the fp32 form for the float32 arrays (rgb, disparity, rigidity,
+// the Phong value), the fp64 form for the float64 correspondence image.
+constexpr int kMaxThreads = 1024;
+// The canonical space is cut into 100 voxels per axis, each spanning the whole colour cube (free_viewpoint_rendering.py:641)
+constexpr int kCorrespondenceVoxels = 100;
+constexpr int kImageThreads = 256;
+constexpr unsigned kImageMaxBlocks = 16384;   // grid-stride beyond this: the stack maximum is reduced once per block
+
+// np.max semantics: a NaN anywhere makes the maximum NaN
+__device__ __forceinline__ float max_nan(float a, float b) { return (a != a || a > b) ? a : b; }
+__device__ __forceinline__ float warp_max_nan(float v) {
+  for (int o = 16; o > 0; o >>= 1) v = max_nan(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// One block per frame: disp_max[f] = np.max(disp[f]).  A maximum does not depend on the order it is taken in.
+__global__ void __launch_bounds__(kMaxThreads) disp_max_kernel(const float* __restrict__ disp, long long n_pix,
+                                                               float* __restrict__ disp_max) {
+  __shared__ float red[kMaxThreads / 32];
+  const float* d = disp + static_cast<long long>(blockIdx.x) * n_pix;
+  float m = -INFINITY;
+#pragma unroll 8
+  for (long long i = threadIdx.x; i < n_pix; i += kMaxThreads) m = max_nan(m, __ldg(d + i));
+  m = warp_max_nan(m);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x / 32] = m;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    m = warp_max_nan(red[threadIdx.x]);
+    if (threadIdx.x == 0) disp_max[blockIdx.x] = m;
+  }
+}
+
+// Every requested uint8 image of every pixel of the stack.  The correspondence image (:640-644) is float64 in the
+// reference (float32 points minus the float64 extent of the checkpoint): c = (p - min) / (max - min) * 100 with _rn
+// intrinsics so that nothing is contracted into an FMA, then c - c.astype(int).  astype(int) truncates toward zero, so a
+// point below min gives a negative fraction that to8b clips to 0 (c - floor(c) would not); out of int64's range (and
+// for NaN) it gives INT64_MIN on x86 hosts, which the fraction reproduces.  disp / max is a float32 division (numpy
+// divides the float32 map by its float32 maximum), the video's by the maximum over the whole stack (:727).
+__global__ void __launch_bounds__(kImageThreads) frame_images_kernel(FrameImageParams p, float inv_c, float inv_e) {
+  __shared__ float s_stack_max;
+  const long long n_pix = static_cast<long long>(p.H) * p.W, n = n_pix * p.F;
+  const int W = p.W;
+  if (p.out_disp_video) {
+    if (threadIdx.x < 32) {
+      float m = -INFINITY;
+      for (int f = threadIdx.x; f < p.F; f += 32) m = max_nan(m, p.disp_max[f]);
+      m = warp_max_nan(m);
+      if (threadIdx.x == 0) s_stack_max = m;
+    }
+    __syncthreads();
+  }
+  for (long long i = static_cast<long long>(blockIdx.x) * kImageThreads + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * kImageThreads) {
+    const long long f = i / n_pix, pix = i - f * n_pix;
+    if (p.out_rgb)
+      for (int c = 0; c < 3; ++c) p.out_rgb[i * 3 + c] = static_cast<uint8_t>(lut_index(__ldg(p.rgb + i * 3 + c)));
+    if (p.disp) {
+      const float* dm = p.disp + f * n_pix;
+      const float m = __ldg(p.disp_max + f);
+      const float raw = __ldg(dm + pix);
+      const float d = __fdiv_rn(raw, m);
+      const int k = lut_index(d);
+      if (p.out_disp) p.out_disp[i] = static_cast<uint8_t>(k);
+      if (p.out_disp_video) p.out_disp_video[i] = static_cast<uint8_t>(lut_index(__fdiv_rn(raw, s_stack_max)));
+      if (p.out_disp_jet)
+        for (int c = 0; c < 3; ++c) p.out_disp_jet[i * 3 + c] = c_jet.rgb8[k * 3 + c];
+      if (p.out_disp_phong) {
+        const int y = static_cast<int>(pix / W), x = static_cast<int>(pix - static_cast<long long>(y) * W);
+        float rgb[3];
+        blinn_phong([&](int yy, int xx) { return __fdiv_rn(__ldg(dm + static_cast<long long>(yy) * W + xx), m); }, d, y, x,
+                    p.H, W, inv_c, inv_e, rgb);
+        for (int c = 0; c < 3; ++c) p.out_disp_phong[i * 3 + c] = static_cast<uint8_t>(lut_index(rgb[c]));
+      }
+    }
+    if (p.out_correspondences)
+      for (int c = 0; c < 3; ++c) {
+        const double v = __dmul_rn(__ddiv_rn(__dsub_rn(static_cast<double>(__ldg(p.surface_pts + i * 3 + c)), p.min_point[c]),
+                                             __dsub_rn(p.max_point[c], p.min_point[c])),
+                                   static_cast<double>(kCorrespondenceVoxels));
+        const double t = fabs(v) < 0x1p63 ? trunc(v) : -0x1p63;
+        p.out_correspondences[i * 3 + c] = static_cast<uint8_t>(lut_index(__dsub_rn(v, t)));
+      }
+    if (p.surface_rigidity) {
+      const int k = lut_index(__ldg(p.surface_rigidity + i));
+      if (p.out_rigidity) p.out_rigidity[i] = static_cast<uint8_t>(k);
+      if (p.out_rigidity_jet)
+        for (int c = 0; c < 3; ++c) p.out_rigidity_jet[i * 3 + c] = c_jet.rgb8[k * 3 + c];
+    }
+  }
 }
 
 // ---- background stability, free_viewpoint_rendering.py:770-785 ---------------------------------------------------------
@@ -313,6 +411,14 @@ __global__ void frame_std_kernel(const float* __restrict__ rgbs, int F, long lon
 }
 
 unsigned blocks_for(long long n, int threads) { return static_cast<unsigned>((n + threads - 1) / threads); }
+
+// np.gradient(d, spacing) divides by 2 * spacing inside and by spacing at the edges, both Python floats that numpy
+// rounds to float32 for a float32 map
+void gradient_divisors(int H, float* inv_c, float* inv_e) {
+  const double spacing = H > 1 ? 2.0 / (H - 1) : 1.0;
+  *inv_c = static_cast<float>(2.0 * spacing);
+  *inv_e = static_cast<float>(spacing);
+}
 
 }  // namespace
 
@@ -358,12 +464,23 @@ cudaError_t launch_score_reduce(const ImageScoreParams& p, cudaStream_t st) {
 }
 
 cudaError_t launch_disparity_images(const float* disp, int F, int H, int W, float* jet, float* phong, cudaStream_t st) {
-  // np.gradient(d, spacing) divides by 2 * spacing inside and by spacing at the edges, both Python floats that numpy
-  // rounds to float32 for a float32 map
-  const double spacing = H > 1 ? 2.0 / (H - 1) : 1.0;
+  float inv_c, inv_e;
+  gradient_divisors(H, &inv_c, &inv_e);
   const long long n = static_cast<long long>(F) * H * W;
-  disparity_kernel<<<blocks_for(n, 256), 256, 0, st>>>(disp, F, H, W, jet, phong, static_cast<float>(2.0 * spacing),
-                                                      static_cast<float>(spacing));
+  disparity_kernel<<<blocks_for(n, 256), 256, 0, st>>>(disp, F, H, W, jet, phong, inv_c, inv_e);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_disp_max(const float* disp, int F, int H, int W, float* disp_max, cudaStream_t st) {
+  disp_max_kernel<<<F, kMaxThreads, 0, st>>>(disp, static_cast<long long>(H) * W, disp_max);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_frame_images(const FrameImageParams& p, cudaStream_t st) {
+  float inv_c, inv_e;
+  gradient_divisors(p.H, &inv_c, &inv_e);
+  const long long blocks = (static_cast<long long>(p.F) * p.H * p.W + kImageThreads - 1) / kImageThreads;
+  frame_images_kernel<<<blocks < kImageMaxBlocks ? static_cast<unsigned>(blocks) : kImageMaxBlocks, kImageThreads, 0, st>>>(p, inv_c, inv_e);
   return cudaGetLastError();
 }
 

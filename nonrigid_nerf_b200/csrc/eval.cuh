@@ -23,6 +23,25 @@ struct ImageScoreParams {
   double* partials;         // [F][tiles per frame][2] workspace: (squared-error sum, cropped SSIM sum) per tile
 };
 
+// The saved 8-bit images of F frames of H x W pixels; an output is written only when its pointer is not null
+struct FrameImageParams {
+  const float* rgb;                 // [F][H][W][3]
+  const float* disp;                // [F][H][W]
+  const float* surface_pts;         // [F][H * W][3]
+  const float* surface_rigidity;    // [F][H * W]
+  double min_point[3], max_point[3];
+  int F, H, W;
+  const float* disp_max;            // [F] np.max of each disparity frame (launch_disp_max)
+  uint8_t* out_rgb;                 // [F][H][W][3] to8b(rgb)
+  uint8_t* out_disp;                // [F][H][W]    to8b(disp / frame max)
+  uint8_t* out_disp_video;          // [F][H][W]    to8b(disp / stack max)
+  uint8_t* out_disp_jet;            // [F][H][W][3] to8b(jet(disp / frame max))
+  uint8_t* out_disp_phong;          // [F][H][W][3] to8b(phong(disp / frame max))
+  uint8_t* out_correspondences;     // [F][H][W][3]
+  uint8_t* out_rigidity;            // [F][H][W]    to8b(rigidity)
+  uint8_t* out_rigidity_jet;        // [F][H][W][3] to8b(jet(rigidity))
+};
+
 // Number of SSIM tiles of one frame and the workspace layout: partials first, then the derived mask (H * W bytes)
 long long eval_tiles_per_frame(int H, int W);
 size_t eval_partials_bytes(int F, int H, int W);
@@ -35,5 +54,7 @@ cudaError_t launch_image_scores(const ImageScoreParams& p, cudaStream_t st);
 cudaError_t launch_score_reduce(const ImageScoreParams& p, cudaStream_t st);
 cudaError_t launch_disparity_images(const float* disp, int F, int H, int W, float* jet, float* phong, cudaStream_t st);
 cudaError_t launch_frame_std(const float* rgbs, int F, int H, int W, float* std_out, float* image, cudaStream_t st);
+cudaError_t launch_disp_max(const float* disp, int F, int H, int W, float* disp_max, cudaStream_t st);
+cudaError_t launch_frame_images(const FrameImageParams& p, cudaStream_t st);
 
 }  // namespace nrn
