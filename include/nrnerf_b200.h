@@ -493,6 +493,53 @@ typedef struct NrnFrameImageArgs {
 } NrnFrameImageArgs;
 int nrn_frame_images(const NrnFrameImageArgs* args);
 
+/* ---- triangle meshes: density grids and marching cubes (geometry.py) -------------------------
+ * No reference counterpart (the reference exports no geometry).  The grid has nx x ny x nz points; point (i, j, k) is
+ * (x_i, y_j, z_k) with x_i = lo + (hi - lo) * (i / (n - 1)) per axis, each operation rounded in fp32 (lo, hi are fp32),
+ * and x_{n-1} = hi exactly.  Sizes: 2 <= n <= 2^24 per axis and nx * ny <= 2^28.  A grid point is occupied when
+ * sigma > threshold (NaN is not, and counts as 0 when a vertex is placed).
+ *
+ * nrn_mesh_grid_points: points [ny][nx][3] of z-plane k, the input of a point-mode nrn_field_forward.
+ * nrn_mesh_sigma: sigma[i] = relu(raw[i][3]) (NaN stays NaN) of n rows of out_ch floats. */
+int nrn_mesh_grid_points(const float* min_point, const float* max_point, int nx, int ny, int nz, int k, float* points, void* stream);
+int nrn_mesh_sigma(const float* raw, long long n, int out_ch, float* sigma, void* stream);
+/* The volume is meshed one z-slab at a time, in this order for k = 0 .. nz - 1 (nrn_mesh_count(k + 1) may be enqueued
+ * before nrn_mesh_emit(k): the workspace keeps three planes' states):
+ *   nrn_mesh_count(k): per point of plane k its crossed edges to +x, +y and (sigma1 = plane k + 1 given, k < nz - 1) +z,
+ *     per cell between planes k and k + 1 its case index and triangle count; both scanned in place.  totals (device
+ *     int32 [2]) receives the number of vertices of plane k and of faces of cell layer k.
+ *   nrn_mesh_emit(k): the vertices of plane k at rows vertex_base.. of vertices [V][3] (ordered by edge key (j, i, axis)),
+ *     each at p_a + ((t - s_a) / (s_b - s_a)) * (p_b - p_a) from its lower end a; and for k >= 1 the faces of cell layer
+ *     k - 1 at rows face_base.. of faces [T][3] (ordered by cell (j, i), then by table order), whose vertex ids count from
+ *     vertex_base_prev (plane k - 1) and vertex_base (plane k).
+ * The caller carries the running bases (sums of totals) and keeps V and T below 2^31.  NULL args, bad sizes, a missing
+ * pointer, a negative base and misaligned arrays return NRN_E_INVALID before any CUDA call. */
+typedef struct NrnMeshSlabArgs {
+  const float* sigma0;        /* [ny][nx] density of plane k */
+  const float* sigma1;        /* [ny][nx] density of plane k + 1, NULL for k = nz - 1 */
+  const float* min_point;     /* host [3], needed by nrn_mesh_emit */
+  const float* max_point;     /* host [3] */
+  float threshold;
+  int32_t nx, ny, nz, k;
+  void* workspace;            /* nrn_mesh_workspace_bytes(nx, ny), 256-byte aligned, the same for every k of one volume */
+  int32_t* totals;            /* count: out device [2] */
+  int64_t vertex_base_prev;   /* emit: global id of plane k - 1's first vertex */
+  int64_t vertex_base;        /* emit: global id of plane k's first vertex */
+  int64_t face_base;          /* emit: index of cell layer k - 1's first face */
+  float* vertices;            /* emit: out [V][3] */
+  int32_t* faces;             /* emit: out [T][3] */
+  void* stream;
+} NrnMeshSlabArgs;
+size_t nrn_mesh_workspace_bytes(int nx, int ny);   /* 0 for sizes out of range */
+int nrn_mesh_count(const NrnMeshSlabArgs* args);
+int nrn_mesh_emit(const NrnMeshSlabArgs* args);
+/* colors [n][3] = to8b(sigmoid(raw[i][0:3])) of n rows of out_ch floats (to8b as in nrn_frame_images). */
+int nrn_mesh_colors(const float* raw, long long n, int out_ch, uint8_t* colors, void* stream);
+/* Host copy of the cube table: counts [256] triangles per case, edges [256][5][3] their edges (-1 padded).  Corner c is
+ * at offset (c & 1, c >> 1 & 1, c >> 2 & 1); edge e = 4 * axis + r runs along axis from the corner whose other two
+ * offsets are (r & 1, r >> 1).  DESIGN.md describes the construction.  Either pointer may be NULL. */
+int nrn_mesh_cube_table(int32_t* counts, int8_t* edges);
+
 /* ---- optional per-kernel timing (measurement aid for bench.py) ---------------------------------
  * While enabled, every launch of the kernel kinds below is bracketed by CUDA events recorded on the
  * launch stream.  kinds: 0 field forward, 1 field DGRAD, 2 WGRAD (+reduce), 3 composite(+resample),
@@ -503,7 +550,8 @@ int nrn_frame_images(const NrnFrameImageArgs* args);
  * 14 the fixed-order divergence loss reduction (nrn_divergence_forward_det), 15 the held-out DGRAD
  * (nrn_field_backward_held_out, nrn_field_backward_det_held_out) and 16 the held-out divergence backward
  * (nrn_divergence_backward_held_out; its WGRAD is kind 2), 17 nrn_image_scores (mask, SSIM tiles, per-frame reduction),
- * 18 nrn_disparity_images, 19 nrn_frame_std_image and 20 nrn_frame_images.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * 18 nrn_disparity_images, 19 nrn_frame_std_image and 20 nrn_frame_images, 21 nrn_mesh_grid_points and nrn_mesh_sigma, 22
+ * nrn_mesh_count (counts and scans), 23 nrn_mesh_emit (vertices and faces) and 24 nrn_mesh_colors.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

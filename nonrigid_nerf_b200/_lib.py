@@ -158,6 +158,18 @@ class NrnFrameImageArgs(C.Structure):
     ]
 
 
+class NrnMeshSlabArgs(C.Structure):
+    _fields_ = [
+        ("sigma0", _vp), ("sigma1", _vp), ("min_point", _vp), ("max_point", _vp),
+        ("threshold", C.c_float),
+        ("nx", C.c_int32), ("ny", C.c_int32), ("nz", C.c_int32), ("k", C.c_int32),
+        ("workspace", _vp), ("totals", _vp),
+        ("vertex_base_prev", C.c_int64), ("vertex_base", C.c_int64), ("face_base", C.c_int64),
+        ("vertices", _vp), ("faces", _vp),
+        ("stream", _vp),
+    ]
+
+
 # every symbol include/nrnerf_b200.h declares: (restype, argtypes)
 SYMBOLS = {
     "nrn_abi_version": (C.c_int, []),
@@ -228,6 +240,13 @@ SYMBOLS = {
     "nrn_disparity_images": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),
     "nrn_frame_std_image": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),
     "nrn_frame_images": (C.c_int, [C.POINTER(NrnFrameImageArgs)]),
+    "nrn_mesh_grid_points": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, _vp]),
+    "nrn_mesh_sigma": (C.c_int, [_vp, C.c_longlong, C.c_int, _vp, _vp]),
+    "nrn_mesh_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "nrn_mesh_count": (C.c_int, [C.POINTER(NrnMeshSlabArgs)]),
+    "nrn_mesh_emit": (C.c_int, [C.POINTER(NrnMeshSlabArgs)]),
+    "nrn_mesh_colors": (C.c_int, [_vp, C.c_longlong, C.c_int, _vp, _vp]),
+    "nrn_mesh_cube_table": (C.c_int, [_vp, _vp]),
     "nrn_timing_enable": (C.c_int, [C.c_int]),
     "nrn_timing_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int), C.c_int]),
 }
@@ -247,6 +266,8 @@ HELD_OUT_KERNEL_KINDS = ("field_dgrad_held_out", "div_bwd_held_out")
 EVAL_KERNEL_KINDS = ("image_scores", "disparity_images", "frame_std_image")
 # the saved 8-bit images of rendered frames (disparity maxima + every image), timing kind 20
 FRAME_IMAGE_KERNEL_KINDS = ("frame_images",)
+# triangle meshes (grid points + density, counts + scans, vertices + faces, vertex colours), timing kinds 21 to 24
+MESH_KERNEL_KINDS = ("mesh_points", "mesh_count", "mesh_emit", "mesh_colors")
 
 
 def timing_enable(on: bool) -> None:
@@ -256,7 +277,7 @@ def timing_enable(on: bool) -> None:
 def timing_read(kinds=KERNEL_KINDS):
     """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True); `kinds` is KERNEL_KINDS,
     KERNEL_KINDS + TC_KERNEL_KINDS, KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS, that + VIEW_TRAIN_KERNEL_KINDS,
-    that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS, that + EVAL_KERNEL_KINDS or that + FRAME_IMAGE_KERNEL_KINDS."""
+    that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS, that + EVAL_KERNEL_KINDS, that + FRAME_IMAGE_KERNEL_KINDS or that + MESH_KERNEL_KINDS."""
     n = len(kinds)
     ms = (C.c_double * n)()
     cnt = (C.c_int * n)()

@@ -15,6 +15,7 @@
 #include "peer.cuh"
 #include "det_reduce.cuh"
 #include "eval.cuh"
+#include "mesh.cuh"
 
 namespace nrn {
 cudaError_t launch_field_fwd(const FieldFwdParams& p, bool has_bender, int num_sms, cudaStream_t stream);
@@ -1052,6 +1053,125 @@ int nrn_frame_images(const NrnFrameImageArgs* a) {
     if (rc) return rc;
   }
   return timed(20, st, "frame_images_kernel", [&] { return nrn::launch_frame_images(p, st); });
+}
+
+// ---- triangle meshes --------------------------------------------------------------------------------------------------
+static bool mesh_plane_ok(int nx, int ny) {
+  return nx >= 2 && ny >= 2 && nx <= nrn::kMeshMaxAxis && ny <= nrn::kMeshMaxAxis && static_cast<long long>(nx) * ny <= nrn::kMeshMaxPlane;
+}
+
+// The grid of a slab call: sizes in range, 0 <= k < nz, and (when the extent is needed) finite min < max on every axis
+static int mesh_grid(const float* lo, const float* hi, int nx, int ny, int nz, int k, bool need_extent, const char* who, nrn::MeshGrid* g) {
+  if (!mesh_plane_ok(nx, ny) || nz < 2 || nz > nrn::kMeshMaxAxis || k < 0 || k >= nz)
+    return fail(NRN_E_INVALID, "%s: bad sizes nx=%d ny=%d nz=%d k=%d (2 <= n <= 2^24 per axis, nx * ny <= 2^28, 0 <= k < nz)", who, nx, ny, nz, k);
+  *g = nrn::MeshGrid{};
+  g->n[0] = nx; g->n[1] = ny; g->n[2] = nz;
+  if (!need_extent) return NRN_OK;
+  if (!lo || !hi) return fail(NRN_E_INVALID, "%s: null min_point / max_point", who);
+  for (int a = 0; a < 3; ++a) {
+    if (!(hi[a] > lo[a]) || !isfinite(lo[a]) || !isfinite(hi[a]))
+      return fail(NRN_E_INVALID, "%s: max_point must exceed min_point on every axis (finite values)", who);
+    g->lo[a] = lo[a]; g->hi[a] = hi[a];
+  }
+  return NRN_OK;
+}
+
+int nrn_mesh_grid_points(const float* min_point, const float* max_point, int nx, int ny, int nz, int k, float* points, void* stream) {
+  const char* who = "nrn_mesh_grid_points";
+  nrn::MeshGrid g;
+  const int rc = mesh_grid(min_point, max_point, nx, ny, nz, k, true, who, &g);
+  if (rc) return rc;
+  if (!points) return fail(NRN_E_INVALID, "%s: null points", who);
+  if (!aligned4(points)) return fail(NRN_E_INVALID, "%s: points must be 4-byte aligned", who);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return timed(21, st, "mesh_grid_points_kernel", [&] { return nrn::launch_mesh_grid_points(g, k, points, st); });
+}
+
+int nrn_mesh_sigma(const float* raw, long long n, int out_ch, float* sigma, void* stream) {
+  const char* who = "nrn_mesh_sigma";
+  if (n < 0 || out_ch < 4 || out_ch > 5 || n > (1LL << 40)) return fail(NRN_E_INVALID, "%s: bad sizes n=%lld out_ch=%d", who, n, out_ch);
+  if (n == 0) return NRN_OK;
+  if (!raw || !sigma) return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (!aligned4(raw) || !aligned4(sigma)) return fail(NRN_E_INVALID, "%s: float arrays must be 4-byte aligned", who);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return timed(21, st, "mesh_sigma_kernel", [&] { return nrn::launch_mesh_sigma(raw, n, out_ch, sigma, st); });
+}
+
+size_t nrn_mesh_workspace_bytes(int nx, int ny) { return mesh_plane_ok(nx, ny) ? nrn::mesh_workspace_bytes(nx, ny) : 0; }
+
+// The checks both slab entry points share: sizes, the planes (sigma1 exactly when k < nz - 1) and the workspace
+static int mesh_slab(const NrnMeshSlabArgs* a, bool emit, const char* who, nrn::MeshGrid* g) {
+  if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
+  const int rc = mesh_grid(a->min_point, a->max_point, a->nx, a->ny, a->nz, a->k, emit, who, g);
+  if (rc) return rc;
+  if (!a->sigma0 || !a->workspace) return fail(NRN_E_INVALID, "%s: null sigma0 / workspace", who);
+  if ((a->sigma1 != nullptr) != (a->k + 1 < a->nz))
+    return fail(NRN_E_INVALID, "%s: sigma1 (plane k + 1) must be given exactly when k < nz - 1", who);
+  if (!(a->threshold == a->threshold)) return fail(NRN_E_INVALID, "%s: threshold is NaN", who);
+  if (!aligned4(a->sigma0) || !aligned4(a->sigma1) || (reinterpret_cast<uintptr_t>(a->workspace) & 255u))
+    return fail(NRN_E_INVALID, "%s: sigma must be 4-byte and the workspace 256-byte aligned", who);
+  return NRN_OK;
+}
+
+int nrn_mesh_count(const NrnMeshSlabArgs* a) {
+  const char* who = "nrn_mesh_count";
+  nrn::MeshGrid g;
+  int rc = mesh_slab(a, false, who, &g);
+  if (rc) return rc;
+  if (!a->totals || !aligned4(a->totals)) return fail(NRN_E_INVALID, "%s: null or misaligned totals", who);
+  const int nx = a->nx, ny = a->ny;
+  const long long n = static_cast<long long>(nx) * ny, nc = static_cast<long long>(nx - 1) * (ny - 1);
+  const nrn::MeshPlaneState s = nrn::mesh_plane_state(a->workspace, nx, ny, a->k % nrn::kMeshSlots);
+  int32_t* partials = nrn::mesh_scan_partials(a->workspace, nx, ny);
+  const cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  return timed(22, st, "mesh_count_kernel", [&] {
+    cudaError_t e = nrn::launch_mesh_count(g, a->sigma0, a->sigma1, a->threshold, s, st);
+    if (e == cudaSuccess) e = nrn::launch_mesh_scan(s.voff, n + 1, partials, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(a->totals, s.voff + n, sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess && a->sigma1) e = nrn::launch_mesh_scan(s.toff, nc + 1, partials, st);
+    if (e == cudaSuccess) e = a->sigma1 ? cudaMemcpyAsync(a->totals + 1, s.toff + nc, sizeof(int32_t), cudaMemcpyDeviceToDevice, st)
+                                        : cudaMemsetAsync(a->totals + 1, 0, sizeof(int32_t), st);
+    return e;
+  });
+}
+
+int nrn_mesh_emit(const NrnMeshSlabArgs* a) {
+  const char* who = "nrn_mesh_emit";
+  nrn::MeshGrid g;
+  int rc = mesh_slab(a, true, who, &g);
+  if (rc) return rc;
+  if (!a->vertices || (a->k > 0 && !a->faces)) return fail(NRN_E_INVALID, "%s: null vertices / faces", who);
+  if (!aligned4(a->vertices) || !aligned4(a->faces)) return fail(NRN_E_INVALID, "%s: vertices and faces must be 4-byte aligned", who);
+  const long long lim = 0x7fffffffLL;
+  if (a->vertex_base < 0 || a->vertex_base_prev < 0 || a->face_base < 0 || a->vertex_base > lim || a->face_base > lim ||
+      (a->k > 0 && a->vertex_base_prev > a->vertex_base))
+    return fail(NRN_E_INVALID, "%s: bases out of range (0 <= vertex_base_prev <= vertex_base < 2^31, 0 <= face_base < 2^31)", who);
+  const int slot = a->k % nrn::kMeshSlots;
+  const nrn::MeshPlaneState s = nrn::mesh_plane_state(a->workspace, a->nx, a->ny, slot);
+  const cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  return timed(23, st, "mesh_emit_kernels", [&] {
+    cudaError_t e = nrn::launch_mesh_vertices(g, a->k, a->sigma0, a->sigma1, a->threshold, s, a->vertex_base, a->vertices, st);
+    if (e == cudaSuccess && a->k > 0) {
+      const nrn::MeshPlaneState lower = nrn::mesh_plane_state(a->workspace, a->nx, a->ny, (a->k - 1) % nrn::kMeshSlots);
+      e = nrn::launch_mesh_faces(g, lower, s, a->vertex_base_prev, a->vertex_base, a->face_base, a->faces, st);
+    }
+    return e;
+  });
+}
+
+int nrn_mesh_colors(const float* raw, long long n, int out_ch, uint8_t* colors, void* stream) {
+  const char* who = "nrn_mesh_colors";
+  if (n < 0 || out_ch < 4 || out_ch > 5 || n > (1LL << 40)) return fail(NRN_E_INVALID, "%s: bad sizes n=%lld out_ch=%d", who, n, out_ch);
+  if (n == 0) return NRN_OK;
+  if (!raw || !colors) return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (!aligned4(raw)) return fail(NRN_E_INVALID, "%s: raw must be 4-byte aligned", who);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return timed(24, st, "mesh_colors_kernel", [&] { return nrn::launch_mesh_colors(raw, n, out_ch, colors, st); });
+}
+
+int nrn_mesh_cube_table(int32_t* counts, int8_t* edges) {
+  nrn::mesh_cube_table(counts, edges);
+  return NRN_OK;
 }
 
 // Turning timing off only stops recording: a CUDA graph captured while it was on keeps event-record nodes that refer to

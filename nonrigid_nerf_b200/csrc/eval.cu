@@ -67,17 +67,6 @@ constexpr JetDeviceTables make_jet_device_tables() {
 }
 __constant__ JetDeviceTables c_jet = make_jet_device_tables();
 
-// uint8(255 * clip(v, 0, 1)) as numpy's .astype("uint8") truncates it; NaN (clip keeps it) maps to index 0, what the
-// float -> uint8 cast gives on x86 hosts
-__device__ __forceinline__ int lut_index(float v) {
-  if (!(v == v)) return 0;
-  return static_cast<int>(__fmul_rn(255.f, fminf(fmaxf(v, 0.f), 1.f)));
-}
-__device__ __forceinline__ int lut_index(double v) {
-  if (!(v == v)) return 0;
-  return static_cast<int>(255.0 * fmin(fmax(v, 0.0), 1.0));
-}
-
 // numpy's sum over a contiguous axis of three: ((a + b) + c)
 __device__ __forceinline__ float sum3(float a, float b, float c) { return __fadd_rn(__fadd_rn(a, b), c); }
 __device__ __forceinline__ float sumsq3(float a, float b, float c) {

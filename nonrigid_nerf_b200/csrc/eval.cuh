@@ -7,6 +7,17 @@
 
 namespace nrn {
 
+// uint8(255 * clip(v, 0, 1)) as numpy's .astype("uint8") truncates it (to8b); NaN (clip keeps it) maps to index 0, what
+// the float -> uint8 cast gives on x86 hosts
+__device__ __forceinline__ int lut_index(float v) {
+  if (!(v == v)) return 0;
+  return static_cast<int>(__fmul_rn(255.f, fminf(fmaxf(v, 0.f), 1.f)));
+}
+__device__ __forceinline__ int lut_index(double v) {
+  if (!(v == v)) return 0;
+  return static_cast<int>(255.0 * fmin(fmax(v, 0.0), 1.0));
+}
+
 constexpr int kEvalTileW = 32;   // SSIM output tile (pixels); the window reaches 5 pixels past it on every side
 constexpr int kEvalTileH = 8;
 

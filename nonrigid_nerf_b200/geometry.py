@@ -1,0 +1,300 @@
+"""Triangle meshes of the scene: density grids through the fused field kernel and marching cubes on the GPU (csrc/mesh.cu).
+
+The reference exports no geometry; these functions give the canonical mesh, the mesh of any frame in world space (the grid
+points bent by that frame's latent code) and the rigidity painted onto the surface.
+
+Grid.  `resolution` is an int or (nx, ny, nz), each at least 2.  Point (i, j, k) is (x_i, y_j, z_k) with, per axis and in
+fp32, lo = float32(min), hi = float32(max), x_i = lo + (hi - lo) * (i / (n - 1)), each of the four operations rounded on its
+own (no fused multiply-add), and x_{n-1} = hi exactly.  Grids are [nz, ny, nx]: x varies fastest.
+
+Density.  sigma = relu(raw[..., 3]) of NeRF.forward in point mode at the grid point, with the model's test-time knobs
+(the bender's rigidity_test_time_cutoff and test_time_scaling, the NeRF's test_time_nonrigid_object_removal_threshold).
+With a ray bender and a latent code the points are bent by that latent (the frame's geometry in world space); with a bender
+and latent=None the bender is off, as render_canonical turns it off (the canonical geometry).  A time-conditioned baseline
+needs the latent; a view-dependent model (use_viewdirs=True) is refused.
+
+Surface.  A grid point is occupied when sigma > threshold (NaN is not).  Each grid edge with exactly one occupied end gets
+one vertex, p_a + ((t - s_a) / (s_b - s_a)) * (p_b - p_a) from its lower end a (NaN counts as 0 there), shared by every
+cell around the edge.  Vertices are ordered by edge key (k, j, i, axis), faces by cell (k, j, i) and then by the cube
+table's order (DESIGN.md describes its construction); face normals, by the right-hand rule, point out of the occupied region.
+The result is bit-reproducible.
+
+Memory.  The volume is meshed in z-slabs: three density planes and three planes of counts are resident, so device memory is
+O(nx * ny) plus the mesh.  density_grid alone materialises the whole volume.  V and T must stay below 2^31.
+"""
+from __future__ import annotations
+
+import ctypes as C
+from typing import NamedTuple, Optional
+
+import numpy as np
+import torch
+
+from . import _lib, ops
+from . import autograd as _ag
+
+_ID_LIMIT = 2 ** 31
+_ATTR_CHUNK = 1 << 22   # vertices per point-mode pass of the attributes
+
+
+class Mesh(NamedTuple):
+    vertices: torch.Tensor              # [V, 3] fp32
+    faces: torch.Tensor                 # [T, 3] int32 vertex ids
+    colors: Optional[torch.Tensor]      # [V, 3] uint8 to8b(sigmoid(raw[:3])) at each vertex
+    rigidity: Optional[torch.Tensor]    # [V] fp32 the bender's rigidity at each vertex (None: no bender, or canonical)
+    vertex_offsets: np.ndarray          # [nz + 1] int64: the vertices of z-plane k's edges are rows vertex_offsets[k]..[k+1]
+    face_offsets: np.ndarray            # [nz] int64: the faces of cell layer k (between planes k, k + 1) start at face_offsets[k]; [-1] = T
+
+
+def _resolution(resolution):
+    r = (resolution,) * 3 if isinstance(resolution, (int, np.integer)) else tuple(resolution)
+    if len(r) != 3 or any(not isinstance(n, (int, np.integer)) or isinstance(n, bool) for n in r):
+        raise RuntimeError(f"nonrigid_nerf_b200: resolution must be an int or (nx, ny, nz), got {resolution!r}")
+    if any(n < 2 for n in r):
+        raise RuntimeError(f"nonrigid_nerf_b200: resolution must be at least 2 on every axis, got {r}")
+    if any(n > 2 ** 24 for n in r) or r[0] * r[1] > 2 ** 28:
+        raise RuntimeError(f"nonrigid_nerf_b200: resolution {r} too large (at most 2^24 per axis and nx * ny <= 2^28)")
+    return tuple(int(n) for n in r)
+
+
+def _extent(min_point, max_point):
+    """The volume extent as the fp32 values the grid is built from (host arrays the C ABI reads)."""
+    lo, hi = (np.ascontiguousarray(np.asarray(p, dtype=np.float64).reshape(-1).astype(np.float32)) for p in (min_point, max_point))
+    if lo.shape != (3,) or hi.shape != (3,):
+        raise RuntimeError("nonrigid_nerf_b200: min_point and max_point must hold 3 values each")
+    if not (np.all(np.isfinite(lo)) and np.all(np.isfinite(hi)) and np.all(hi > lo)):
+        raise RuntimeError(f"nonrigid_nerf_b200: max_point {hi.tolist()} must exceed min_point {lo.tolist()} on every axis "
+                           "(finite, in fp32)")
+    return lo, hi
+
+
+class _PointField:
+    """NeRF.forward in point mode at given points, with one latent code for every point (or none)."""
+
+    def __init__(self, network_fn, latent):
+        if getattr(network_fn, "use_viewdirs", False):
+            raise RuntimeError("nonrigid_nerf_b200: meshes of a view-dependent model (use_viewdirs=True) are not implemented")
+        tc = _ag._tc_net(network_fn)
+        bender = network_fn.ray_bender[0]
+        if tc is not None and latent is None:
+            raise RuntimeError("nonrigid_nerf_b200: a time_conditioned_baseline model needs the latent code of a frame")
+        if tc is None and bender is None and latent is not None:
+            raise RuntimeError("nonrigid_nerf_b200: a latent code was given, but the model has no ray bender")
+        self.net, self.tc = network_fn, tc
+        self.bent = bender is not None and latent is not None
+        self.dev = network_fn.output_linear.weight.device
+        if self.dev.type != "cuda":
+            raise RuntimeError("nonrigid_nerf_b200: the model must be on a CUDA device (there is no CPU path)")
+        self.out_ch = network_fn.output_linear.weight.shape[0]
+        self.knobs = _ag._knobs(network_fn) if self.bent else (None, None, None)
+        with torch.no_grad():
+            self.nerf_pack = ops.pack_nerf(network_fn)
+            self.bender_pack = ops.pack_bender(bender) if self.bent else None
+        self.latent = None
+        if latent is not None:
+            lat = torch.as_tensor(latent).detach().to(device=self.dev, dtype=torch.float32).reshape(-1)
+            if lat.numel() != ops.LATENT:
+                raise RuntimeError(f"nonrigid_nerf_b200: the latent code must hold {ops.LATENT} values, got {lat.numel()}")
+            self.latent = lat.reshape(1, ops.LATENT).contiguous()
+
+    def __call__(self, points: torch.Tensor, want_details: bool = False):
+        """raw [P, out_ch] and the details (point mode) at points [P, 3]."""
+        lat = None if self.latent is None else self.latent.expand(points.shape[0], ops.LATENT)
+        raw, det = ops.field_forward_points(points, lat, self.nerf_pack, self.bender_pack, self.out_ch, *self.knobs,
+                                            want_details=want_details, tc_net=self.tc)
+        return raw.view(points.shape[0], self.out_ch), det
+
+
+def _stream():
+    return torch.cuda.current_stream().cuda_stream
+
+
+def _density_plane(field: _PointField, lo, hi, n3, k, points: torch.Tensor, out: torch.Tensor) -> None:
+    """sigma of z-plane k into out [ny, nx] (points: a [ny * nx, 3] scratch buffer)."""
+    lib = _lib.load()
+    nx, ny, nz = n3
+    _lib.check(lib.nrn_mesh_grid_points(lo.ctypes.data, hi.ctypes.data, nx, ny, nz, k, points.data_ptr(), _stream()), "mesh_grid_points")
+    raw, _ = field(points)
+    _lib.check(lib.nrn_mesh_sigma(raw.data_ptr(), nx * ny, field.out_ch, out.data_ptr(), _stream()), "mesh_sigma")
+
+
+def density_grid(network_fn, min_point, max_point, resolution, latent=None) -> torch.Tensor:
+    """sigma [nz, ny, nx] fp32 on the model's device: relu(raw[..., 3]) of NeRF.forward (point mode) at every grid point."""
+    nx, ny, nz = _resolution(resolution)
+    lo, hi = _extent(min_point, max_point)
+    field = _PointField(network_fn, latent)
+    with torch.cuda.device(field.dev), torch.no_grad():
+        sigma = torch.empty(nz, ny, nx, dtype=torch.float32, device=field.dev)
+        points = torch.empty(ny * nx, 3, dtype=torch.float32, device=field.dev)
+        for k in range(nz):
+            _density_plane(field, lo, hi, (nx, ny, nz), k, points, sigma[k])
+    return sigma
+
+
+def _grow(buf: torch.Tensor, used: int, need: int) -> torch.Tensor:
+    if need <= buf.shape[0]:
+        return buf
+    new = torch.empty((max(need, 2 * buf.shape[0]),) + tuple(buf.shape[1:]), dtype=buf.dtype, device=buf.device)
+    new[:used].copy_(buf[:used])
+    return new
+
+
+def _march(dev, n3, lo, hi, threshold: float, plane):
+    """Marching cubes over the planes plane(0), plane(1), ... (each [ny, nx] fp32, asked for once and in order; a plane
+    must stay valid until plane(k + 3) is asked for).  Returns (vertices, faces, vertex_offsets, face_offsets)."""
+    lib = _lib.load()
+    nx, ny, nz = n3
+    t = float(np.float32(threshold))
+    if t != t:
+        raise RuntimeError("nonrigid_nerf_b200: threshold is NaN")
+    ws = torch.empty(lib.nrn_mesh_workspace_bytes(nx, ny), dtype=torch.uint8, device=dev)
+    totals = torch.zeros(3, 2, dtype=torch.int32, device=dev)
+    totals_host = torch.zeros(3, 2, dtype=torch.int32).pin_memory()
+    done = [torch.cuda.Event() for _ in range(3)]
+    sig = {0: plane(0), 1: plane(1)}
+
+    def args(k):
+        a = _lib.NrnMeshSlabArgs()
+        a.sigma0, a.sigma1 = sig[k].data_ptr(), (sig[k + 1].data_ptr() if k + 1 < nz else None)
+        a.min_point, a.max_point = lo.ctypes.data, hi.ctypes.data
+        a.threshold, a.nx, a.ny, a.nz, a.k = t, nx, ny, nz, k
+        a.workspace, a.stream = ws.data_ptr(), _stream()
+        return a
+
+    def count(k):
+        a = args(k)
+        a.totals = totals[k % 3].data_ptr()
+        _lib.check(lib.nrn_mesh_count(C.byref(a)), "mesh_count")
+        totals_host[k % 3].copy_(totals[k % 3], non_blocking=True)
+        done[k % 3].record()
+
+    verts = torch.empty(max(1024, 2 * nx * ny), 3, dtype=torch.float32, device=dev)
+    faces = torch.empty(max(1024, 4 * nx * ny), 3, dtype=torch.int32, device=dev)
+    voff, foff, nf_prev = [0], [0], 0
+    count(0)
+    for k in range(nz):
+        if k + 2 < nz:
+            sig.pop(k - 1, None)
+            sig[k + 2] = plane(k + 2)
+        if k + 1 < nz:
+            count(k + 1)          # enqueued before waiting for plane k's totals: the device keeps working meanwhile
+        done[k % 3].synchronize()
+        nv, nf = (int(x) for x in totals_host[k % 3].tolist())
+        v_end, f_end = voff[k] + nv, foff[-1] + (nf_prev if k > 0 else 0)
+        if v_end >= _ID_LIMIT or f_end >= _ID_LIMIT:
+            raise RuntimeError(f"nonrigid_nerf_b200: the mesh would have {v_end} vertices and {f_end} faces by plane {k}; "
+                               "V and T must stay below 2^31 (lower the resolution)")
+        verts = _grow(verts, voff[k], v_end)
+        faces = _grow(faces, foff[-1], f_end)
+        a = args(k)
+        a.vertex_base_prev, a.vertex_base = voff[k - 1] if k > 0 else 0, voff[k]
+        a.face_base = foff[-1]
+        a.vertices, a.faces = verts.data_ptr(), faces.data_ptr()
+        _lib.check(lib.nrn_mesh_emit(C.byref(a)), "mesh_emit")
+        voff.append(v_end)
+        if k > 0:
+            foff.append(f_end)
+        nf_prev = nf
+    v, f = voff[-1], foff[-1]
+    verts = verts[:v] if verts.shape[0] == v else verts[:v].clone()
+    faces = faces[:f] if faces.shape[0] == f else faces[:f].clone()
+    return verts, faces, np.array(voff, dtype=np.int64), np.array(foff, dtype=np.int64)
+
+
+def marching_cubes(sigma: torch.Tensor, min_point, max_point, threshold: float) -> Mesh:
+    """The surface sigma = threshold of a density grid sigma [nz, ny, nx] (fp32 CUDA) whose points span min_point ..
+    max_point as density_grid's do.  colors and rigidity are None."""
+    if not isinstance(sigma, torch.Tensor) or not sigma.is_cuda:
+        raise RuntimeError("nonrigid_nerf_b200: sigma must be a CUDA tensor (there is no CPU path)")
+    if sigma.dim() != 3:
+        raise RuntimeError(f"nonrigid_nerf_b200: sigma must be [nz, ny, nx], got {tuple(sigma.shape)}")
+    nz, ny, nx = sigma.shape
+    _resolution((nx, ny, nz))
+    lo, hi = _extent(min_point, max_point)
+    sigma = sigma.float().contiguous()
+    with torch.cuda.device(sigma.device):
+        v, f, vo, fo = _march(sigma.device, (nx, ny, nz), lo, hi, threshold, lambda k: sigma[k])
+    return Mesh(v, f, None, None, vo, fo)
+
+
+def extract_mesh(network_fn, min_point, max_point, resolution, threshold: float, latent=None, colors: bool = True,
+                 rigidity: bool = True) -> Mesh:
+    """The surface sigma = threshold of network_fn's density over the grid, without materialising the grid: equal to
+    marching_cubes(density_grid(...), ...) bit for bit.  colors: to8b(sigmoid(raw[:3])) at each vertex; rigidity: the
+    bender's rigidity at each vertex (None without a bender, and for the canonical mesh).  Both come from one more
+    point-mode pass over the vertices with the same latent and knobs."""
+    n3 = _resolution(resolution)
+    nx, ny, nz = n3
+    lo, hi = _extent(min_point, max_point)
+    field = _PointField(network_fn, latent)
+    dev = field.dev
+    with torch.cuda.device(dev), torch.no_grad():
+        points = torch.empty(ny * nx, 3, dtype=torch.float32, device=dev)
+        ring = [torch.empty(ny, nx, dtype=torch.float32, device=dev) for _ in range(3)]
+
+        def plane(k):
+            _density_plane(field, lo, hi, n3, k, points, ring[k % 3])
+            return ring[k % 3]
+
+        v, f, vo, fo = _march(dev, n3, lo, hi, threshold, plane)
+        col = torch.empty(v.shape[0], 3, dtype=torch.uint8, device=dev) if colors else None
+        rig = torch.empty(v.shape[0], dtype=torch.float32, device=dev) if rigidity and field.bent else None
+        if col is not None or rig is not None:
+            for c0 in range(0, v.shape[0], _ATTR_CHUNK):
+                c1 = min(c0 + _ATTR_CHUNK, v.shape[0])
+                raw, det = field(v[c0:c1], want_details=rig is not None)
+                if col is not None:
+                    _lib.check(_lib.load().nrn_mesh_colors(raw.data_ptr(), c1 - c0, field.out_ch, col[c0:c1].data_ptr(), _stream()),
+                               "mesh_colors")
+                if rig is not None:
+                    rig[c0:c1].copy_(det["rigidity_mask"].view(-1))
+    return Mesh(v, f, col, rig, vo, fo)
+
+
+# ---- host-side writers --------------------------------------------------------------------------------------------------
+def _host(mesh: Mesh):
+    v = mesh.vertices.detach().cpu().numpy().astype("<f4", copy=False).reshape(-1, 3)
+    f = mesh.faces.detach().cpu().numpy().astype("<i4", copy=False).reshape(-1, 3)
+    col = None if mesh.colors is None else mesh.colors.detach().cpu().numpy().astype(np.uint8, copy=False).reshape(-1, 3)
+    rig = None if mesh.rigidity is None else mesh.rigidity.detach().cpu().numpy().astype("<f4", copy=False).reshape(-1)
+    return v, f, col, rig
+
+
+def write_ply(path, mesh: Mesh) -> None:
+    """Binary little-endian PLY: float x, y, z (+ uchar red, green, blue when the mesh has colours, + float rigidity when
+    it has rigidity) per vertex, and an int vertex_indices list of 3 per face."""
+    v, f, col, rig = _host(mesh)
+    fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
+    props = ["property float x", "property float y", "property float z"]
+    if col is not None:
+        fields += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
+        props += ["property uchar red", "property uchar green", "property uchar blue"]
+    if rig is not None:
+        fields.append(("rigidity", "<f4"))
+        props.append("property float rigidity")
+    vert = np.empty(len(v), dtype=fields)
+    vert["x"], vert["y"], vert["z"] = v[:, 0], v[:, 1], v[:, 2]
+    if col is not None:
+        vert["red"], vert["green"], vert["blue"] = col[:, 0], col[:, 1], col[:, 2]
+    if rig is not None:
+        vert["rigidity"] = rig
+    face = np.empty(len(f), dtype=[("n", "u1"), ("v", "<i4", (3,))])
+    face["n"], face["v"] = 3, f
+    header = "\n".join(["ply", "format binary_little_endian 1.0", f"element vertex {len(v)}"] + props +
+                       [f"element face {len(f)}", "property list uchar int vertex_indices", "end_header"]) + "\n"
+    with open(path, "wb") as fh:
+        fh.write(header.encode("ascii"))
+        fh.write(vert.tobytes())
+        fh.write(face.tobytes())
+
+
+def write_obj(path, mesh: Mesh) -> None:
+    """Wavefront OBJ: 'v x y z' per vertex (+ ' r g b' in [0, 1] when the mesh has colours, c / 255), 'f a b c' per face
+    (1-based).  Coordinates are written with 9 significant digits, which restore the fp32 values exactly."""
+    v, f, col, _ = _host(mesh)
+    with open(path, "w") as fh:
+        if col is None:
+            np.savetxt(fh, v, fmt="v %.9g %.9g %.9g")
+        else:
+            np.savetxt(fh, np.concatenate([v.astype(np.float64), col / 255.0], 1), fmt="v %.9g %.9g %.9g %.9g %.9g %.9g")
+        np.savetxt(fh, f.astype(np.int64) + 1, fmt="f %d %d %d")
