@@ -540,6 +540,47 @@ int nrn_mesh_colors(const float* raw, long long n, int out_ch, uint8_t* colors, 
  * offsets are (r & 1, r >> 1).  DESIGN.md describes the construction.  Either pointer may be NULL. */
 int nrn_mesh_cube_table(int32_t* counts, int8_t* edges);
 
+/* ---- LPIPS: the perceptual score of rendered frames (evaluation.py) ---------------------------
+ * lpips.LPIPS(net='alex') (v0.1, eval mode) as free_viewpoint_rendering.py:788-849 scores every frame and :868 averages
+ * the scores.  Per frame pair: zero the masked pixels of both images, t = 2x - 1, s = (t - shift) / scale (fp32), the
+ * AlexNet features (conv1 11x11/4 pad 2 -> 64, max-pool 3/2, conv2 5x5 pad 2 -> 192, max-pool 3/2, conv3 3x3 -> 384,
+ * conv4 -> 256, conv5 -> 256, each conv + bias + ReLU; the five ReLU outputs are the taps), and per tap k the mean over
+ * its pixels of sum_c w_k[c] (f_gt[c] / (|f_gt| + 1e-10) - f_gen[c] / (|f_gen| + 1e-10))^2; LPIPS is the sum of the five.
+ * The convolutions run on fp16 operands with fp32 accumulation, activations are stored in fp16, the distances are fp32
+ * per pixel and fp64 per frame, summed in a fixed order: a frame's score does not depend on the batch or chunk it is in.
+ *
+ * nrn_lpips_pack: the packed weight block (nrn_lpips_packed_bytes(), 16-byte aligned, device) from 17 device fp32 arrays:
+ *   tensors[2 l], tensors[2 l + 1]  conv weight (OIHW) and bias of layer l = 0..4 (net.slice1.0, net.slice2.3,
+ *                                   net.slice3.6, net.slice4.8, net.slice5.10)
+ *   tensors[10 + k]                 tap weights w_k [C_k] (lin{k}.model.1.weight)
+ *   tensors[15], tensors[16]        shift [3] and scale [3] (scaling_layer)
+ * Once per weight set; the sources may be freed after the stream has run the pack.
+ * nrn_lpips_workspace_bytes(F, H, W): the workspace nrn_lpips uses for F frames of H x W by default: the derived mask,
+ *   ceil(H * W / 256) * 256 bytes, plus min(F, max(1, 256 MiB / B), 4096) frames of B bytes each, B the activations of
+ *   both images of a frame at every stage (fp16 NHWC) and its distance partials.  nrn_lpips_workspace_bytes(1, H, W) -
+ *   nrn_lpips_workspace_bytes(0, H, W) is B.  0 for sizes out of range.
+ * nrn_lpips: lpips [F] and, when per_layer is not NULL, the tap scores per_layer [F][5].  Frames go in chunks of
+ *   (workspace_bytes - mask bytes) / B frames (at most 4096).  NULL args or pointers, negative sizes, H or W below 31 (the
+ *   smallest frame every tap has a pixel of) or above 16384, float arrays not 4-byte aligned, packed weights not 16-byte
+ *   aligned, a workspace not 256-byte aligned or too small for one frame return NRN_E_INVALID before any CUDA call;
+ *   n_frames = 0 returns NRN_OK and launches nothing. */
+typedef struct NrnLpipsArgs {
+  const float* gt;            /* [F][H][W][3] ground truth in [0, 1] */
+  const float* generated;     /* [F][H][W][3] renders */
+  const uint8_t* mask;        /* [H][W] nonzero = masked, or NULL: the pixels of gt frame 0 whose channels sum to 0 */
+  int32_t n_frames, height, width;
+  const void* packed;         /* nrn_lpips_pack output */
+  float* lpips;               /* out [F] */
+  float* per_layer;           /* out [F][5] tap scores, or NULL */
+  void* workspace;            /* 256-byte aligned */
+  size_t workspace_bytes;
+  void* stream;
+} NrnLpipsArgs;
+size_t nrn_lpips_packed_bytes(void);
+int nrn_lpips_pack(const float* const* tensors, void* packed, void* stream);
+size_t nrn_lpips_workspace_bytes(int n_frames, int height, int width);
+int nrn_lpips(const NrnLpipsArgs* args);
+
 /* ---- optional per-kernel timing (measurement aid for bench.py) ---------------------------------
  * While enabled, every launch of the kernel kinds below is bracketed by CUDA events recorded on the
  * launch stream.  kinds: 0 field forward, 1 field DGRAD, 2 WGRAD (+reduce), 3 composite(+resample),
@@ -551,7 +592,8 @@ int nrn_mesh_cube_table(int32_t* counts, int8_t* edges);
  * (nrn_field_backward_held_out, nrn_field_backward_det_held_out) and 16 the held-out divergence backward
  * (nrn_divergence_backward_held_out; its WGRAD is kind 2), 17 nrn_image_scores (mask, SSIM tiles, per-frame reduction),
  * 18 nrn_disparity_images, 19 nrn_frame_std_image and 20 nrn_frame_images, 21 nrn_mesh_grid_points and nrn_mesh_sigma, 22
- * nrn_mesh_count (counts and scans), 23 nrn_mesh_emit (vertices and faces) and 24 nrn_mesh_colors.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * nrn_mesh_count (counts and scans), 23 nrn_mesh_emit (vertices and faces) and 24 nrn_mesh_colors, and of nrn_lpips 25 the
+ * mask and input scaling, 26 the convolutions, 27 the max-pools and 28 the distances and per-frame sums.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

@@ -170,6 +170,15 @@ class NrnMeshSlabArgs(C.Structure):
     ]
 
 
+class NrnLpipsArgs(C.Structure):
+    _fields_ = [
+        ("gt", _vp), ("generated", _vp), ("mask", _vp),
+        ("n_frames", C.c_int32), ("height", C.c_int32), ("width", C.c_int32),
+        ("packed", _vp), ("lpips", _vp), ("per_layer", _vp),
+        ("workspace", _vp), ("workspace_bytes", C.c_size_t), ("stream", _vp),
+    ]
+
+
 # every symbol include/nrnerf_b200.h declares: (restype, argtypes)
 SYMBOLS = {
     "nrn_abi_version": (C.c_int, []),
@@ -247,6 +256,10 @@ SYMBOLS = {
     "nrn_mesh_emit": (C.c_int, [C.POINTER(NrnMeshSlabArgs)]),
     "nrn_mesh_colors": (C.c_int, [_vp, C.c_longlong, C.c_int, _vp, _vp]),
     "nrn_mesh_cube_table": (C.c_int, [_vp, _vp]),
+    "nrn_lpips_packed_bytes": (C.c_size_t, []),
+    "nrn_lpips_pack": (C.c_int, [C.POINTER(_vp), _vp, _vp]),
+    "nrn_lpips_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "nrn_lpips": (C.c_int, [C.POINTER(NrnLpipsArgs)]),
     "nrn_timing_enable": (C.c_int, [C.c_int]),
     "nrn_timing_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int), C.c_int]),
 }
@@ -268,6 +281,8 @@ EVAL_KERNEL_KINDS = ("image_scores", "disparity_images", "frame_std_image")
 FRAME_IMAGE_KERNEL_KINDS = ("frame_images",)
 # triangle meshes (grid points + density, counts + scans, vertices + faces, vertex colours), timing kinds 21 to 24
 MESH_KERNEL_KINDS = ("mesh_points", "mesh_count", "mesh_emit", "mesh_colors")
+# LPIPS (mask + input scaling, convolutions, max-pools, distances + per-frame sums), timing kinds 25 to 28
+LPIPS_KERNEL_KINDS = ("lpips_input", "lpips_conv", "lpips_pool", "lpips_distance")
 
 
 def timing_enable(on: bool) -> None:
@@ -277,7 +292,7 @@ def timing_enable(on: bool) -> None:
 def timing_read(kinds=KERNEL_KINDS):
     """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True); `kinds` is KERNEL_KINDS,
     KERNEL_KINDS + TC_KERNEL_KINDS, KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS, that + VIEW_TRAIN_KERNEL_KINDS,
-    that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS, that + EVAL_KERNEL_KINDS, that + FRAME_IMAGE_KERNEL_KINDS or that + MESH_KERNEL_KINDS."""
+    that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS, that + EVAL_KERNEL_KINDS, that + FRAME_IMAGE_KERNEL_KINDS, that + MESH_KERNEL_KINDS or that + LPIPS_KERNEL_KINDS."""
     n = len(kinds)
     ms = (C.c_double * n)()
     cnt = (C.c_int * n)()

@@ -16,6 +16,7 @@
 #include "det_reduce.cuh"
 #include "eval.cuh"
 #include "mesh.cuh"
+#include "lpips.cuh"
 
 namespace nrn {
 cudaError_t launch_field_fwd(const FieldFwdParams& p, bool has_bender, int num_sms, cudaStream_t stream);
@@ -1171,6 +1172,99 @@ int nrn_mesh_colors(const float* raw, long long n, int out_ch, uint8_t* colors, 
 
 int nrn_mesh_cube_table(int32_t* counts, int8_t* edges) {
   nrn::mesh_cube_table(counts, edges);
+  return NRN_OK;
+}
+
+// ---- LPIPS (lpips.cu) -------------------------------------------------------------------------------------------------
+size_t nrn_lpips_packed_bytes(void) { return nrn::kLpipsPackedBytes; }
+
+int nrn_lpips_pack(const float* const* tensors, void* packed, void* stream) {
+  const char* who = "nrn_lpips_pack";
+  if (!tensors || !packed) return fail(NRN_E_INVALID, "%s: null argument", who);
+  for (int i = 0; i < 17; ++i)
+    if (!tensors[i]) return fail(NRN_E_INVALID, "%s: null tensor %d", who, i);
+    else if (!aligned4(tensors[i])) return fail(NRN_E_INVALID, "%s: tensor %d must be 4-byte aligned", who, i);
+  if (!aligned16(packed)) return fail(NRN_E_INVALID, "%s: packed buffer must be 16-byte aligned", who);
+  nrn::LpipsPackSources s;
+  for (int l = 0; l < nrn::kLpipsTaps; ++l) {
+    s.conv_w[l] = tensors[2 * l];
+    s.conv_b[l] = tensors[2 * l + 1];
+    s.lin[l] = tensors[10 + l];
+  }
+  s.shift = tensors[15];
+  s.scale = tensors[16];
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const cudaError_t e = nrn::launch_lpips_pack(s, static_cast<uint8_t*>(packed), st);
+  return e == cudaSuccess ? NRN_OK : cuda_fail(e, "lpips_pack_kernel");
+}
+
+static bool lpips_size_ok(int H, int W) {
+  return H >= nrn::kLpipsMinSide && W >= nrn::kLpipsMinSide && H <= nrn::kLpipsMaxSide && W <= nrn::kLpipsMaxSide;
+}
+
+size_t nrn_lpips_workspace_bytes(int n_frames, int height, int width) {
+  if (n_frames < 0 || !lpips_size_ok(height, width)) return 0;
+  const size_t frame = nrn::lpips_frame_bytes(height, width);
+  size_t fc = nrn::kLpipsChunkBudget / frame;
+  fc = fc < 1 ? 1 : (fc > static_cast<size_t>(nrn::kLpipsMaxChunk) ? nrn::kLpipsMaxChunk : fc);
+  if (fc > static_cast<size_t>(n_frames)) fc = n_frames;
+  return nrn::lpips_mask_bytes(height, width) + fc * frame;
+}
+
+int nrn_lpips(const NrnLpipsArgs* a) {
+  const char* who = "nrn_lpips";
+  if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
+  const int F = a->n_frames, H = a->height, W = a->width;
+  if (F < 0 || H < 0 || W < 0) return fail(NRN_E_INVALID, "%s: bad sizes F=%d H=%d W=%d", who, F, H, W);
+  if (!lpips_size_ok(H, W))
+    return fail(NRN_E_INVALID, "%s: frames of %d x %d pixels: height and width must be at least %d (every AlexNet tap needs a pixel) "
+                "and at most %d", who, H, W, nrn::kLpipsMinSide, nrn::kLpipsMaxSide);
+  if (F == 0) return NRN_OK;
+  if (!a->gt || !a->generated || !a->packed || !a->lpips || !a->workspace) return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (!aligned4(a->gt) || !aligned4(a->generated) || !aligned4(a->lpips) || !aligned4(a->per_layer))
+    return fail(NRN_E_INVALID, "%s: float arrays must be 4-byte aligned", who);
+  if (!aligned16(a->packed) || (reinterpret_cast<uintptr_t>(a->workspace) & 255u))
+    return fail(NRN_E_INVALID, "%s: packed weights must be 16-byte and the workspace 256-byte aligned", who);
+  const size_t mask_bytes = nrn::lpips_mask_bytes(H, W), frame = nrn::lpips_frame_bytes(H, W);
+  if (a->workspace_bytes < mask_bytes + frame)
+    return fail(NRN_E_INVALID, "%s: workspace of %zu bytes holds no frame (%zu needed for one)", who, a->workspace_bytes, mask_bytes + frame);
+  size_t fc_max = (a->workspace_bytes - mask_bytes) / frame;
+  if (fc_max > static_cast<size_t>(nrn::kLpipsMaxChunk)) fc_max = nrn::kLpipsMaxChunk;
+  DeviceState* ds = nullptr;
+  int rc = device_state(&ds);
+  if (rc) return rc;
+  const cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  const uint8_t* packed = static_cast<const uint8_t*>(a->packed);
+  uint8_t* mask = static_cast<uint8_t*>(a->workspace);
+  if (a->mask) mask = const_cast<uint8_t*>(a->mask);
+  else if ((rc = timed(25, st, "frame_mask_kernel", [&] { return nrn::launch_frame_mask(a->gt, H, W, mask, st); }))) return rc;
+  const nrn::LpipsDims d = nrn::lpips_dims(H, W);
+  const size_t frame_floats = static_cast<size_t>(H) * W * 3;
+  for (int f0 = 0; f0 < F; f0 += static_cast<int>(fc_max)) {
+    const int fc = F - f0 < static_cast<int>(fc_max) ? F - f0 : static_cast<int>(fc_max);
+    const nrn::LpipsChunk c = nrn::lpips_chunk(a->workspace, fc, H, W);
+    rc = timed(25, st, "lpips_input_kernel", [&] {
+      return nrn::launch_lpips_input(a->gt + f0 * frame_floats, a->generated + f0 * frame_floats, mask, packed, fc, H, W, c.act[0], st);
+    });
+    for (int l = 0; l < nrn::kLpipsTaps && !rc; ++l) {
+      const int si = nrn::kLpipsTapStage[l];
+      if (l == 1 || l == 2)   // conv2 and conv3 read the max-pool of the stage before theirs
+        rc = timed(27, st, "lpips_pool_kernel", [&] {
+          return nrn::launch_lpips_pool(c.act[si - 2], c.act[si - 1], 2 * fc, d.h[si - 2], d.w[si - 2], d.h[si - 1], d.w[si - 1],
+                                        nrn::kLpipsStageChannels[si - 2], st);
+        });
+      if (!rc)
+        rc = timed(26, st, "lpips_conv_kernel", [&] {
+          return nrn::launch_lpips_conv(l, d, c.act[l == 0 ? 0 : si - 1], c.act[si], packed, 2 * fc, ds->num_sms, ds->err_word, st);
+        });
+      if (!rc) rc = timed(28, st, "lpips_distance_kernel", [&] { return nrn::launch_lpips_distance(l, d, c, packed, st); });
+    }
+    if (!rc)
+      rc = timed(28, st, "lpips_reduce_kernel", [&] {
+        return nrn::launch_lpips_reduce(d, c, a->lpips + f0, a->per_layer ? a->per_layer + static_cast<size_t>(f0) * nrn::kLpipsTaps : nullptr, st);
+      });
+    if (rc) return rc;
+  }
   return NRN_OK;
 }
 

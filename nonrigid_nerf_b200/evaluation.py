@@ -188,3 +188,128 @@ def frame_images(rgbs: Optional[torch.Tensor] = None, disps: Optional[torch.Tens
         a.stream = _stream().value
         _lib.check(_lib.load().nrn_frame_images(C.byref(a)), "frame_images")
     return out
+
+
+# ---- LPIPS (free_viewpoint_rendering.py:788-849, :868) ------------------------------------------------------------------
+# lpips.LPIPS(net='alex') state-dict keys: the AlexNet convolutions ([out, in, k, k] weight, [out] bias), the tap weights
+# lin{k}.model.1.weight [1, C_k, 1, 1] and the scaling layer's shift / scale [1, 3, 1, 1] (defaults when absent)
+LPIPS_CONVS = (("net.slice1.0", 64, 3, 11), ("net.slice2.3", 192, 64, 5), ("net.slice3.6", 384, 192, 3),
+               ("net.slice4.8", 256, 384, 3), ("net.slice5.10", 256, 256, 3))
+LPIPS_SHIFT = (-0.030, -0.088, -0.188)
+LPIPS_SCALE = (0.458, 0.448, 0.450)
+LPIPS_MIN_SIDE = 31   # the smallest frame height and width for which every tap has a pixel
+
+
+def lpips_state(source) -> list:
+    """The 17 fp32 tensors nrn_lpips_pack takes, in its order (conv weight and bias of the five layers, the five tap
+    weights flattened to [C_k], shift [3], scale [3]), from an lpips.LPIPS(net='alex') module or its state dict.
+    Raises before anything reaches the device when the source is not that network: another backbone (VGG, SqueezeNet),
+    missing keys, wrong shapes, or a module configured for a different score (version 0.0, spatial maps)."""
+    if isinstance(source, torch.nn.Module):
+        if str(getattr(source, "version", "0.1")) != "0.1":
+            raise RuntimeError(f"nonrigid_nerf_b200: LPIPS version {source.version} is not supported (0.1 only)")
+        if getattr(source, "spatial", False):
+            raise RuntimeError("nonrigid_nerf_b200: spatial LPIPS maps are not supported (one score per frame)")
+        if getattr(source, "pnet_type", "alex") != "alex":
+            raise RuntimeError(f"nonrigid_nerf_b200: the {source.pnet_type} backbone is not supported (net='alex' only)")
+        source = source.state_dict()
+    if not isinstance(source, dict):
+        raise RuntimeError(f"nonrigid_nerf_b200: lpips weights come from an lpips.LPIPS module or its state dict, got {type(source)}")
+    if any(k in source for k in ("lin5.model.1.weight", "lin6.model.1.weight")):
+        raise RuntimeError("nonrigid_nerf_b200: this LPIPS state dict has more than five taps (SqueezeNet); net='alex' only")
+
+    def get(key, shape):
+        if key not in source:
+            raise RuntimeError(f"nonrigid_nerf_b200: LPIPS state dict lacks {key} (net='alex' only)")
+        t = source[key]
+        if not isinstance(t, torch.Tensor) or tuple(t.shape) != shape:
+            got = tuple(t.shape) if isinstance(t, torch.Tensor) else type(t)
+            raise RuntimeError(f"nonrigid_nerf_b200: LPIPS {key} must be {list(shape)}, got {got} "
+                               "(net='alex' only; VGG and SqueezeNet backbones are not supported)")
+        t = t.detach().float()
+        if not bool(torch.isfinite(t).all()):
+            raise RuntimeError(f"nonrigid_nerf_b200: LPIPS {key} holds non-finite values")
+        return t
+
+    out = []
+    for key, cout, cin, k in LPIPS_CONVS:
+        out += [get(key + ".weight", (cout, cin, k, k)), get(key + ".bias", (cout,))]
+    out += [get(f"lin{k}.model.1.weight", (1, c[1], 1, 1)).reshape(-1) for k, c in enumerate(LPIPS_CONVS)]
+    for key, default in (("scaling_layer.shift", LPIPS_SHIFT), ("scaling_layer.scale", LPIPS_SCALE)):
+        out.append(get(key, (1, 3, 1, 1)).reshape(-1) if key in source else torch.tensor(default, dtype=torch.float32))
+    return out
+
+
+class LpipsWeights:
+    """An LPIPS weight set packed for the kernels (nrn_lpips_pack): fp16 convolution images, fp32 biases, tap weights and
+    scaling.  Made once by lpips_weights(); `packed` lives on `device`."""
+
+    def __init__(self, packed: torch.Tensor, sources: list):
+        self.packed = packed
+        self.device = packed.device
+        self._sources = sources   # the pack reads them on the stream; kept alive with the packed block
+
+
+def lpips_weights(source, device=None) -> LpipsWeights:
+    """Validate an lpips.LPIPS(net='alex') module or its state dict (lpips_state) and pack it once on `device` (default:
+    the current CUDA device), on the current stream."""
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    if dev.type != "cuda":
+        raise RuntimeError("nonrigid_nerf_b200: LPIPS weights are packed on a CUDA device (there is no CPU path)")
+    state = lpips_state(source)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        src = [t.to(dev).contiguous() for t in state]
+        packed = torch.empty(int(lib.nrn_lpips_packed_bytes()), dtype=torch.uint8, device=dev)
+        ptrs = (C.c_void_p * len(src))(*[t.data_ptr() for t in src])
+        _lib.check(lib.nrn_lpips_pack(ptrs, packed.data_ptr(), _stream()), "lpips_weights")
+    return LpipsWeights(packed, src)
+
+
+def lpips(gt: torch.Tensor, generated: torch.Tensor, weights: LpipsWeights, mask: Optional[torch.Tensor] = None,
+          per_layer: bool = False, *, chunk_frames: Optional[int] = None):
+    """LPIPS (v0.1, AlexNet) of every frame of generated [F, H, W, 3] against gt in [0, 1], as
+    free_viewpoint_rendering.py:836-849 scores them: [F] fp32, or ([F], [F, 5] tap scores) with per_layer=True.  mask
+    [H, W] (nonzero = pixel zeroed in both images) defaults to the pixels of gt[0] whose channels sum to 0, as in
+    image_scores.  H and W must be at least 31.  Frames go through the network in chunks of chunk_frames (default: as
+    many as fit 256 MiB of activations); a frame's score does not depend on the chunk or batch it is in."""
+    if not isinstance(weights, LpipsWeights):
+        raise RuntimeError("nonrigid_nerf_b200: weights must come from evaluation.lpips_weights()")
+    gt = _frames(gt, "gt", 4)
+    generated = _frames(generated, "generated", 4)
+    if gt.shape != generated.shape or gt.device != generated.device:
+        raise RuntimeError(f"nonrigid_nerf_b200: gt {tuple(gt.shape)} and generated {tuple(generated.shape)} differ")
+    f, h, w, _ = gt.shape
+    dev = gt.device
+    if weights.device != dev:
+        raise RuntimeError(f"nonrigid_nerf_b200: LPIPS weights are on {weights.device}, the frames on {dev}")
+    if h < LPIPS_MIN_SIDE or w < LPIPS_MIN_SIDE:
+        raise RuntimeError(f"nonrigid_nerf_b200: LPIPS needs frames of at least {LPIPS_MIN_SIDE} x {LPIPS_MIN_SIDE} pixels "
+                           f"(every AlexNet tap needs a pixel), got {h} x {w}")
+    if mask is not None:
+        if tuple(mask.shape) != (h, w) or mask.device != dev:
+            raise RuntimeError(f"nonrigid_nerf_b200: mask must be [{h}, {w}] on {dev}, got {tuple(mask.shape)}")
+        mask = (mask != 0).to(torch.uint8).contiguous()
+    lib = _lib.load()
+    if chunk_frames is None:
+        ws_bytes = int(lib.nrn_lpips_workspace_bytes(f, h, w))
+    else:
+        if int(chunk_frames) < 1:
+            raise RuntimeError(f"nonrigid_nerf_b200: chunk_frames must be at least 1, got {chunk_frames}")
+        base = int(lib.nrn_lpips_workspace_bytes(0, h, w))
+        ws_bytes = base + min(int(chunk_frames), f) * (int(lib.nrn_lpips_workspace_bytes(1, h, w)) - base)
+    if ws_bytes == 0:
+        raise RuntimeError(f"nonrigid_nerf_b200: LPIPS frames of {h} x {w} pixels are out of range")
+    out = torch.empty(f, dtype=torch.float32, device=dev)
+    layers = torch.empty((f, 5), dtype=torch.float32, device=dev) if per_layer else None
+    if f > 0:
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        a = _lib.NrnLpipsArgs()
+        a.gt, a.generated, a.mask = gt.data_ptr(), generated.data_ptr(), None if mask is None else mask.data_ptr()
+        a.n_frames, a.height, a.width = f, h, w
+        a.packed, a.lpips, a.per_layer = weights.packed.data_ptr(), out.data_ptr(), None if layers is None else layers.data_ptr()
+        a.workspace, a.workspace_bytes = ws.data_ptr(), ws_bytes
+        with torch.cuda.device(dev):
+            a.stream = _stream().value
+            _lib.check(lib.nrn_lpips(C.byref(a)), "lpips")
+    return (out, layers) if per_layer else out
