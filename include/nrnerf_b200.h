@@ -581,6 +581,53 @@ int nrn_lpips_pack(const float* const* tensors, void* packed, void* stream);
 size_t nrn_lpips_workspace_bytes(int n_frames, int height, int width);
 int nrn_lpips(const NrnLpipsArgs* args);
 
+/* ---- correspondences between rendered frames (correspondence.py) ------------------------------
+ * render(..., surface_output=True) gives every pixel its canonical surface point (train.py:159-176: the median-visibility
+ * sample mapped back through the ray bender); free_viewpoint_rendering.py:615-645 only paints those points as a
+ * checkerboard.  nrn_match turns them into pixel correspondences: for every valid query pixel, the target pixel of the paired
+ * frame whose canonical point is nearest.
+ *
+ * Pairs: F = max(Fq, Ft) frame pairs, query frame (Fq == 1 ? 0 : f) against target frame (Ft == 1 ? 0 : f); Fq == Ft, Fq
+ * == 1 or Ft == 1.  A point is valid when its mask byte is nonzero (or the mask is NULL) and its coordinates are finite.
+ * The distance is d2 = (dx*dx + dy*dy) + dz*dz in fp32, each operation rounded on its own; the match is the valid target
+ * point of smallest (d2, index), kept when d2 <= fl(max_distance^2): the brute-force answer, whatever the search order.
+ *   index [F][Hq][Wq]       y * Wt + x of the match, or -1 (query pixel invalid, no valid target, or beyond max_distance)
+ *   distance [F][Hq][Wq]    sqrt(d2) of the match, +inf where index is -1
+ *   flow [F][Hq][Wq][2]     (x_t - x_q, y_t - y_q) in pixels, NaN where index is -1
+ *   consistent [F][Hq][Wq]  (round_trip) 1 when the match's own match in the query frame, by the same rule, lies within
+ *                           round_trip_pixels of the query pixel (fl(dx*dx + dy*dy) <= fl(tol^2)); 0 where index is -1
+ * Each target frame's valid points go into an n^3 uniform grid over their bounding box (n^3 <= max(1, Ht*Wt / 2), n as
+ * large as that allows), and each query searches rings of cells until no unsearched cell can hold a closer point.
+ *
+ * nrn_match_workspace_bytes: the workspace for these sizes (the target frames' grids, and with round_trip the query
+ *   frames' grids), a sum of 256-byte aligned sections: per frame set of F frames of N = H * W points with C = n^3 cells,
+ *   32 F, 4 F C, 4 F (C + 1) and 16 F N bytes.  0 for sizes out of range or frame counts that do not pair.
+ * nrn_match: NULL args or pointers (consistent is needed with round_trip), H or W outside 1..2^24, H * W above 2^31 - 1,
+ *   frame counts above 65535 or that do not pair, a NaN or negative max_distance or round_trip_pixels, float and index
+ *   arrays not 4-byte aligned, a workspace not 256-byte aligned or smaller than nrn_match_workspace_bytes return
+ *   NRN_E_INVALID before any CUDA call; F = 0 returns NRN_OK and launches nothing. */
+typedef struct NrnMatchArgs {
+  const float* query;           /* [Fq][Hq][Wq][3] canonical surface points */
+  const float* target;          /* [Ft][Ht][Wt][3] */
+  const uint8_t* query_mask;    /* [Fq][Hq][Wq] nonzero = a surface point, or NULL */
+  const uint8_t* target_mask;   /* [Ft][Ht][Wt], or NULL */
+  int32_t n_query_frames, query_height, query_width;
+  int32_t n_target_frames, target_height, target_width;
+  float max_distance;           /* canonical-space radius; +inf for none */
+  int32_t round_trip;
+  float round_trip_pixels;
+  int32_t* index;               /* out [F][Hq][Wq] */
+  float* distance;              /* out [F][Hq][Wq] */
+  float* flow;                  /* out [F][Hq][Wq][2] */
+  uint8_t* consistent;          /* out [F][Hq][Wq] (round_trip), else ignored */
+  void* workspace;              /* 256-byte aligned */
+  size_t workspace_bytes;
+  void* stream;
+} NrnMatchArgs;
+size_t nrn_match_workspace_bytes(int n_query_frames, int query_height, int query_width, int n_target_frames, int target_height,
+                                 int target_width, int round_trip);
+int nrn_match(const NrnMatchArgs* args);
+
 /* ---- optional per-kernel timing (measurement aid for bench.py) ---------------------------------
  * While enabled, every launch of the kernel kinds below is bracketed by CUDA events recorded on the
  * launch stream.  kinds: 0 field forward, 1 field DGRAD, 2 WGRAD (+reduce), 3 composite(+resample),
@@ -593,7 +640,8 @@ int nrn_lpips(const NrnLpipsArgs* args);
  * (nrn_divergence_backward_held_out; its WGRAD is kind 2), 17 nrn_image_scores (mask, SSIM tiles, per-frame reduction),
  * 18 nrn_disparity_images, 19 nrn_frame_std_image and 20 nrn_frame_images, 21 nrn_mesh_grid_points and nrn_mesh_sigma, 22
  * nrn_mesh_count (counts and scans), 23 nrn_mesh_emit (vertices and faces) and 24 nrn_mesh_colors, and of nrn_lpips 25 the
- * mask and input scaling, 26 the convolutions, 27 the max-pools and 28 the distances and per-frame sums.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * mask and input scaling, 26 the convolutions, 27 the max-pools and 28 the distances and per-frame sums, and of nrn_match 29
+ * the grid builds (boxes, counts, scans, scatters) and 30 the queries with their round trips.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

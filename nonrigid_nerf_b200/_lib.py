@@ -179,6 +179,17 @@ class NrnLpipsArgs(C.Structure):
     ]
 
 
+class NrnMatchArgs(C.Structure):
+    _fields_ = [
+        ("query", _vp), ("target", _vp), ("query_mask", _vp), ("target_mask", _vp),
+        ("n_query_frames", C.c_int32), ("query_height", C.c_int32), ("query_width", C.c_int32),
+        ("n_target_frames", C.c_int32), ("target_height", C.c_int32), ("target_width", C.c_int32),
+        ("max_distance", C.c_float), ("round_trip", C.c_int32), ("round_trip_pixels", C.c_float),
+        ("index", _vp), ("distance", _vp), ("flow", _vp), ("consistent", _vp),
+        ("workspace", _vp), ("workspace_bytes", C.c_size_t), ("stream", _vp),
+    ]
+
+
 # every symbol include/nrnerf_b200.h declares: (restype, argtypes)
 SYMBOLS = {
     "nrn_abi_version": (C.c_int, []),
@@ -260,6 +271,8 @@ SYMBOLS = {
     "nrn_lpips_pack": (C.c_int, [C.POINTER(_vp), _vp, _vp]),
     "nrn_lpips_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     "nrn_lpips": (C.c_int, [C.POINTER(NrnLpipsArgs)]),
+    "nrn_match_workspace_bytes": (C.c_size_t, [C.c_int] * 7),
+    "nrn_match": (C.c_int, [C.POINTER(NrnMatchArgs)]),
     "nrn_timing_enable": (C.c_int, [C.c_int]),
     "nrn_timing_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int), C.c_int]),
 }
@@ -283,6 +296,8 @@ FRAME_IMAGE_KERNEL_KINDS = ("frame_images",)
 MESH_KERNEL_KINDS = ("mesh_points", "mesh_count", "mesh_emit", "mesh_colors")
 # LPIPS (mask + input scaling, convolutions, max-pools, distances + per-frame sums), timing kinds 25 to 28
 LPIPS_KERNEL_KINDS = ("lpips_input", "lpips_conv", "lpips_pool", "lpips_distance")
+# frame correspondences (grid builds, queries with their round trips), timing kinds 29 and 30
+MATCH_KERNEL_KINDS = ("match_build", "match_query")
 
 
 def timing_enable(on: bool) -> None:
@@ -292,7 +307,7 @@ def timing_enable(on: bool) -> None:
 def timing_read(kinds=KERNEL_KINDS):
     """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True); `kinds` is KERNEL_KINDS,
     KERNEL_KINDS + TC_KERNEL_KINDS, KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS, that + VIEW_TRAIN_KERNEL_KINDS,
-    that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS, that + EVAL_KERNEL_KINDS, that + FRAME_IMAGE_KERNEL_KINDS, that + MESH_KERNEL_KINDS or that + LPIPS_KERNEL_KINDS."""
+    that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS, that + EVAL_KERNEL_KINDS, that + FRAME_IMAGE_KERNEL_KINDS, that + MESH_KERNEL_KINDS, that + LPIPS_KERNEL_KINDS or that + MATCH_KERNEL_KINDS."""
     n = len(kinds)
     ms = (C.c_double * n)()
     cnt = (C.c_int * n)()

@@ -17,6 +17,7 @@
 #include "eval.cuh"
 #include "mesh.cuh"
 #include "lpips.cuh"
+#include "match.cuh"
 
 namespace nrn {
 cudaError_t launch_field_fwd(const FieldFwdParams& p, bool has_bender, int num_sms, cudaStream_t stream);
@@ -1266,6 +1267,79 @@ int nrn_lpips(const NrnLpipsArgs* a) {
     if (rc) return rc;
   }
   return NRN_OK;
+}
+
+// ---- correspondences (match.cu) ---------------------------------------------------------------------------------------
+static bool match_frame_ok(int H, int W) {
+  return H >= 1 && W >= 1 && H <= nrn::kMatchMaxSide && W <= nrn::kMatchMaxSide &&
+         static_cast<long long>(H) * W <= nrn::kMatchMaxPoints;
+}
+
+// The output frame count of Fq query frames against Ft target frames, or -1 when they do not pair
+static int match_pairs(int Fq, int Ft) {
+  if (Fq < 0 || Ft < 0 || Fq > nrn::kMatchMaxFrames || Ft > nrn::kMatchMaxFrames) return -1;
+  if (Fq == Ft || Ft == 1) return Fq;
+  if (Fq == 1) return Ft;
+  return -1;
+}
+
+size_t nrn_match_workspace_bytes(int n_query_frames, int query_height, int query_width, int n_target_frames, int target_height,
+                                 int target_width, int round_trip) {
+  if (match_pairs(n_query_frames, n_target_frames) < 0 || !match_frame_ok(query_height, query_width) ||
+      !match_frame_ok(target_height, target_width))
+    return 0;
+  size_t b = nrn::match_cloud_bytes(n_target_frames, static_cast<long long>(target_height) * target_width);
+  if (round_trip) b += nrn::match_cloud_bytes(n_query_frames, static_cast<long long>(query_height) * query_width);
+  return b;
+}
+
+int nrn_match(const NrnMatchArgs* a) {
+  const char* who = "nrn_match";
+  if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
+  const int Fq = a->n_query_frames, Ft = a->n_target_frames;
+  if (!match_frame_ok(a->query_height, a->query_width) || !match_frame_ok(a->target_height, a->target_width))
+    return fail(NRN_E_INVALID, "%s: frames of %d x %d (query) and %d x %d (target) pixels: height and width must be 1 to %d and "
+                "a frame at most %lld points", who, a->query_height, a->query_width, a->target_height, a->target_width,
+                nrn::kMatchMaxSide, nrn::kMatchMaxPoints);
+  const int F = match_pairs(Fq, Ft);
+  if (F < 0)
+    return fail(NRN_E_INVALID, "%s: %d query frames do not pair with %d target frames (equal counts, or one frame on either "
+                "side, at most %d)", who, Fq, Ft, nrn::kMatchMaxFrames);
+  if (!(a->max_distance >= 0.f)) return fail(NRN_E_INVALID, "%s: max_distance %g must be >= 0 (not NaN)", who, a->max_distance);
+  if (a->round_trip && !(a->round_trip_pixels >= 0.f))
+    return fail(NRN_E_INVALID, "%s: round_trip_pixels %g must be >= 0 (not NaN)", who, a->round_trip_pixels);
+  if (F == 0) return NRN_OK;
+  if (!a->query || !a->target || !a->index || !a->distance || !a->flow || !a->workspace || (a->round_trip && !a->consistent))
+    return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (!aligned4(a->query) || !aligned4(a->target) || !aligned4(a->index) || !aligned4(a->distance) || !aligned4(a->flow))
+    return fail(NRN_E_INVALID, "%s: float and index arrays must be 4-byte aligned", who);
+  if (reinterpret_cast<uintptr_t>(a->workspace) & 255u) return fail(NRN_E_INVALID, "%s: the workspace must be 256-byte aligned", who);
+  const size_t need = nrn_match_workspace_bytes(Fq, a->query_height, a->query_width, Ft, a->target_height, a->target_width, a->round_trip);
+  if (a->workspace_bytes < need) return fail(NRN_E_INVALID, "%s: workspace of %zu bytes, %zu needed", who, a->workspace_bytes, need);
+  DeviceState* ds = nullptr;
+  int rc = device_state(&ds);
+  if (rc) return rc;
+  const cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  const long long Nq = static_cast<long long>(a->query_height) * a->query_width;
+  const long long Nt = static_cast<long long>(a->target_height) * a->target_width;
+  nrn::MatchQueryParams p{};
+  p.t = nrn::match_cloud(a->workspace, a->target, a->target_mask, Ft, Nt);
+  if (a->round_trip) {
+    p.q = nrn::match_cloud(static_cast<uint8_t*>(a->workspace) + nrn::match_cloud_bytes(Ft, Nt), a->query, a->query_mask, Fq, Nq);
+  } else {
+    p.q = nrn::MatchCloud{};
+    p.q.pts = a->query; p.q.mask = a->query_mask; p.q.F = Fq; p.q.N = Nq;
+  }
+  p.F = F; p.Wq = a->query_width; p.Wt = a->target_width;
+  p.max_d2 = a->max_distance * a->max_distance;
+  p.round_trip = a->round_trip ? 1 : 0;
+  p.rt_tol2 = a->round_trip_pixels * a->round_trip_pixels;
+  p.index = a->index; p.distance = a->distance; p.flow = a->flow;
+  p.consistent = a->round_trip ? a->consistent : nullptr;
+  rc = timed(29, st, "match_build_kernels", [&] { return nrn::launch_match_build(p.t, ds->num_sms, st); });
+  if (!rc && a->round_trip) rc = timed(29, st, "match_build_kernels", [&] { return nrn::launch_match_build(p.q, ds->num_sms, st); });
+  if (!rc) rc = timed(30, st, "match_query_kernel", [&] { return nrn::launch_match_query(p, st); });
+  return rc;
 }
 
 // Turning timing off only stops recording: a CUDA graph captured while it was on keeps event-record nodes that refer to
