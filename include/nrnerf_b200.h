@@ -628,6 +628,43 @@ size_t nrn_match_workspace_bytes(int n_query_frames, int query_height, int query
                                  int target_width, int round_trip);
 int nrn_match(const NrnMatchArgs* args);
 
+/* ---- occupancy grid: render passes that skip the NeRF trunk for samples in empty canonical space --------------------
+ * A grid of nx * ny * nz cells over [min_point, max_point]; cell (i, j, k) is bit c % 32 of bits[c / 32], c = (k * ny + j)
+ * * nx + i.  A point is KEPT when a coordinate is non-finite or outside the box (x < min or x > max), or when its cell is
+ * occupied; its cell is min(floor(fl(fl(x - min) * scale)), n - 1) per axis with scale = fl(n / fl(max - min)), every
+ * operation an fp32 one rounded on its own.
+ *
+ * nrn_occupancy_build: sigma [nz + 1][ny + 1][nx + 1] densities at the cells' corners.  A cell is occupied when any of its
+ *   8 corners has sigma > threshold or NaN; the occupied set is then dilated by `dilation` cells (Chebyshev distance).
+ *   bits: nrn_occupancy_words(nx, ny, nz) words; workspace: nrn_occupancy_build_workspace_bytes.  Sides outside
+ *   1..4096, dilation outside 0..4096, a NaN threshold or null pointers return NRN_E_INVALID before any CUDA call.
+ * nrn_occupancy_compact: the lookup of points [n_points][points_stride] (xyz first): kept points' xyz -> kept_xyz [K][3]
+ *   and their indices -> kept_index [K] in ascending order, K -> *count (device memory); the order comes from a fixed
+ *   block scan, so reruns are identical.  workspace: nrn_occupancy_compact_workspace_bytes(n_points), 256-byte aligned.
+ * nrn_field_forward_occupancy: one inference pass of nrn_field_forward in ray mode (args as there, no stash / relu_mask,
+ *   points NULL) that evaluates the NeRF trunk only on kept samples: with a bender the bend pass (bent points, rigidities
+ *   and the details), then the lookup of the bent points (without one, of rays_o + rays_d * z), the point-mode trunk on
+ *   the K kept points (K read on the device: no host synchronisation, CUDA-graph capturable), and the scatter.  raw of a
+ *   kept sample equals nrn_field_forward's bit for bit (object removal included); raw of a skipped sample is 0.  The
+ *   details are those of nrn_field_forward for every sample.  workspace: nrn_occupancy_workspace_bytes(n_rays, n_samples,
+ *   out_ch, bender_packed != NULL), 256-byte aligned.  A malformed grid, more than 2^31 - 1 points or a short workspace
+ *   return NRN_E_INVALID before any CUDA call. */
+typedef struct NrnOccupancyGrid {
+  const uint32_t* bits;
+  int32_t nx, ny, nz;         /* cells per axis, 1..4096 */
+  float min_point[3];
+  float max_point[3];
+} NrnOccupancyGrid;
+size_t nrn_occupancy_words(int nx, int ny, int nz);
+size_t nrn_occupancy_build_workspace_bytes(int nx, int ny, int nz);
+int nrn_occupancy_build(const float* sigma, int nx, int ny, int nz, float threshold, int dilation, void* workspace, uint32_t* bits,
+                        void* stream);
+size_t nrn_occupancy_compact_workspace_bytes(int64_t n_points);
+int nrn_occupancy_compact(const NrnOccupancyGrid* grid, const float* points, int64_t n_points, int64_t points_stride, float* kept_xyz,
+                          int32_t* kept_index, int32_t* count, void* workspace, void* stream);
+size_t nrn_occupancy_workspace_bytes(int n_rays, int n_samples, int out_ch, int has_bender);
+int nrn_field_forward_occupancy(const NrnFieldArgs* args, const NrnOccupancyGrid* grid, void* workspace, size_t workspace_bytes);
+
 /* ---- optional per-kernel timing (measurement aid for bench.py) ---------------------------------
  * While enabled, every launch of the kernel kinds below is bracketed by CUDA events recorded on the
  * launch stream.  kinds: 0 field forward, 1 field DGRAD, 2 WGRAD (+reduce), 3 composite(+resample),
@@ -641,7 +678,9 @@ int nrn_match(const NrnMatchArgs* args);
  * 18 nrn_disparity_images, 19 nrn_frame_std_image and 20 nrn_frame_images, 21 nrn_mesh_grid_points and nrn_mesh_sigma, 22
  * nrn_mesh_count (counts and scans), 23 nrn_mesh_emit (vertices and faces) and 24 nrn_mesh_colors, and of nrn_lpips 25 the
  * mask and input scaling, 26 the convolutions, 27 the max-pools and 28 the distances and per-frame sums, and of nrn_match 29
- * the grid builds (boxes, counts, scans, scatters) and 30 the queries with their round trips.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * the grid builds (boxes, counts, scans, scatters) and 30 the queries with their round trips, 31 nrn_occupancy_build, and of
+ * nrn_field_forward_occupancy 32 the bend pass, 33 the lookup and compaction (also nrn_occupancy_compact), 34 the trunk on
+ * the kept points and 35 the scatter.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

@@ -190,6 +190,13 @@ class NrnMatchArgs(C.Structure):
     ]
 
 
+class NrnOccupancyGrid(C.Structure):
+    _fields_ = [
+        ("bits", _vp), ("nx", C.c_int32), ("ny", C.c_int32), ("nz", C.c_int32),
+        ("min_point", C.c_float * 3), ("max_point", C.c_float * 3),
+    ]
+
+
 # every symbol include/nrnerf_b200.h declares: (restype, argtypes)
 SYMBOLS = {
     "nrn_abi_version": (C.c_int, []),
@@ -273,6 +280,13 @@ SYMBOLS = {
     "nrn_lpips": (C.c_int, [C.POINTER(NrnLpipsArgs)]),
     "nrn_match_workspace_bytes": (C.c_size_t, [C.c_int] * 7),
     "nrn_match": (C.c_int, [C.POINTER(NrnMatchArgs)]),
+    "nrn_occupancy_words": (C.c_size_t, [C.c_int] * 3),
+    "nrn_occupancy_build_workspace_bytes": (C.c_size_t, [C.c_int] * 3),
+    "nrn_occupancy_build": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, _vp, _vp, _vp]),
+    "nrn_occupancy_compact_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "nrn_occupancy_compact": (C.c_int, [C.POINTER(NrnOccupancyGrid), _vp, C.c_int64, C.c_int64, _vp, _vp, _vp, _vp, _vp]),
+    "nrn_occupancy_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
+    "nrn_field_forward_occupancy": (C.c_int, [C.POINTER(NrnFieldArgs), C.POINTER(NrnOccupancyGrid), _vp, C.c_size_t]),
     "nrn_timing_enable": (C.c_int, [C.c_int]),
     "nrn_timing_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int), C.c_int]),
 }
@@ -298,6 +312,9 @@ MESH_KERNEL_KINDS = ("mesh_points", "mesh_count", "mesh_emit", "mesh_colors")
 LPIPS_KERNEL_KINDS = ("lpips_input", "lpips_conv", "lpips_pool", "lpips_distance")
 # frame correspondences (grid builds, queries with their round trips), timing kinds 29 and 30
 MATCH_KERNEL_KINDS = ("match_build", "match_query")
+# occupancy grids (grid build; of a render pass: bend pass, lookup + compaction, trunk on the kept points, scatter),
+# timing kinds 31 to 35
+OCCUPANCY_KERNEL_KINDS = ("occupancy_build", "occupancy_bend", "occupancy_compact", "occupancy_field", "occupancy_scatter")
 
 
 def timing_enable(on: bool) -> None:
@@ -307,7 +324,8 @@ def timing_enable(on: bool) -> None:
 def timing_read(kinds=KERNEL_KINDS):
     """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True); `kinds` is KERNEL_KINDS,
     KERNEL_KINDS + TC_KERNEL_KINDS, KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS, that + VIEW_TRAIN_KERNEL_KINDS,
-    that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS, that + EVAL_KERNEL_KINDS, that + FRAME_IMAGE_KERNEL_KINDS, that + MESH_KERNEL_KINDS, that + LPIPS_KERNEL_KINDS or that + MATCH_KERNEL_KINDS."""
+    that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS, that + EVAL_KERNEL_KINDS, that + FRAME_IMAGE_KERNEL_KINDS, that + MESH_KERNEL_KINDS, that + LPIPS_KERNEL_KINDS, that + MATCH_KERNEL_KINDS or that
+    + OCCUPANCY_KERNEL_KINDS."""
     n = len(kinds)
     ms = (C.c_double * n)()
     cnt = (C.c_int * n)()

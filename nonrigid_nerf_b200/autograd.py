@@ -689,6 +689,33 @@ def field(net, rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[torch
     return raw, (details if want_details else {})
 
 
+def occupancy_check(net, latents, grid) -> None:
+    """Raise, before any launch, for what render(..., occupancy=grid) does not support: the view-dependent head, the
+    time-conditioned baseline and differentiable calls."""
+    from .geometry import OccupancyGrid
+    if not isinstance(grid, OccupancyGrid):
+        raise RuntimeError(f"nonrigid_nerf_b200: occupancy must be a geometry.OccupancyGrid, got {type(grid).__name__}")
+    if getattr(net, "use_viewdirs", False):
+        raise RuntimeError("nonrigid_nerf_b200: rendering with an occupancy grid is not implemented for use_viewdirs=True")
+    if getattr(net, "time_conditioned_baseline", False):
+        raise RuntimeError("nonrigid_nerf_b200: rendering with an occupancy grid is not implemented for time_conditioned_baseline=True")
+    if _needs_grad(net, latents):
+        raise RuntimeError("nonrigid_nerf_b200: rendering with an occupancy grid is inference only; call render() under "
+                           "torch.no_grad() (skipped samples would get no gradient)")
+
+
+def field_occupancy(net, rays, z_vals, latents, want_details, grid):
+    """field_rays that evaluates the NeRF trunk only on the samples the occupancy grid keeps; raw is 0 for the others."""
+    occupancy_check(net, latents, grid)
+    bender = net.ray_bender[0]
+    cutoff, scaling, removal = _knobs(net)
+    nerf_pack = ops.pack_nerf(net)
+    bender_pack = ops.pack_bender(bender) if bender is not None else None
+    out_ch = net.output_linear.weight.shape[0]
+    return ops.field_forward_occupancy(rays, z_vals, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details,
+                                       grid)
+
+
 def field_rays(net, rays, z_vals, latents, want_details):
     """Inference path (no stash)."""
     bender = net.ray_bender[0]

@@ -1,5 +1,6 @@
 // extern "C" boundary of libnrnerf_b200.so (declarations: include/nrnerf_b200.h).
 // Argument validation, launch, error reporting.  No exceptions cross this file.
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -18,6 +19,7 @@
 #include "mesh.cuh"
 #include "lpips.cuh"
 #include "match.cuh"
+#include "occupancy.cuh"
 
 namespace nrn {
 cudaError_t launch_field_fwd(const FieldFwdParams& p, bool has_bender, int num_sms, cudaStream_t stream);
@@ -32,6 +34,7 @@ cudaError_t launch_field_bend(const FieldFwdParams& p, const ViewParams& v, int 
 cudaError_t launch_field_views(const FieldFwdParams& p, const ViewParams& v, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_views_train(const FieldFwdParams& p, const ViewParams& v, const ViewTrainParams& t, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_bwd_views(const FieldBwdParams& p, const ViewBwdParams& v, int num_sms, cudaStream_t stream);
+cudaError_t launch_field_fwd_kept(const FieldFwdParams& p, const int* kept, int num_sms, cudaStream_t stream);
 }
 
 namespace {
@@ -1340,6 +1343,150 @@ int nrn_match(const NrnMatchArgs* a) {
   if (!rc && a->round_trip) rc = timed(29, st, "match_build_kernels", [&] { return nrn::launch_match_build(p.q, ds->num_sms, st); });
   if (!rc) rc = timed(30, st, "match_query_kernel", [&] { return nrn::launch_match_query(p, st); });
   return rc;
+}
+
+// ---- occupancy grid: build, lookup + compaction, and the render pass that skips empty cells ----
+static size_t align256(size_t n) { return (n + 255) & ~static_cast<size_t>(255); }
+static bool occ_sides_ok(int nx, int ny, int nz) {
+  return nx >= 1 && ny >= 1 && nz >= 1 && nx <= nrn::kOccMaxSide && ny <= nrn::kOccMaxSide && nz <= nrn::kOccMaxSide;
+}
+static size_t occ_block_count_bytes(long long P) { return align256(sizeof(int32_t) * ((P + nrn::kOccTile - 1) / nrn::kOccTile + 1)); }
+
+// The grid as the kernels read it; NRN_E_INVALID for a malformed one
+static int occ_grid(const NrnOccupancyGrid* g, const char* who, nrn::OccGrid* out) {
+  if (!g) return fail(NRN_E_INVALID, "%s: null grid", who);
+  if (!occ_sides_ok(g->nx, g->ny, g->nz))
+    return fail(NRN_E_INVALID, "%s: grid resolution %d x %d x %d out of range (1..%d cells per axis)", who, g->nx, g->ny, g->nz, nrn::kOccMaxSide);
+  if (!g->bits || (reinterpret_cast<uintptr_t>(g->bits) & 3u)) return fail(NRN_E_INVALID, "%s: grid bits null or not 4-byte aligned", who);
+  nrn::OccGrid o{};
+  o.bits = g->bits; o.nx = g->nx; o.ny = g->ny; o.nz = g->nz;
+  const int n[3] = {g->nx, g->ny, g->nz};
+  for (int d = 0; d < 3; ++d) {
+    const float lo = g->min_point[d], hi = g->max_point[d];
+    if (!(std::isfinite(lo) && std::isfinite(hi) && hi > lo)) return fail(NRN_E_INVALID, "%s: grid box must be finite with max > min on every axis", who);
+    const float ext = hi - lo;
+    const float sc = static_cast<float>(n[d]) / ext;
+    if (!(std::isfinite(ext) && std::isfinite(sc) && sc > 0.f)) return fail(NRN_E_INVALID, "%s: grid box extent out of fp32 range", who);
+    o.lo[d] = lo; o.hi[d] = hi; o.scale[d] = sc;
+  }
+  *out = o;
+  return NRN_OK;
+}
+
+size_t nrn_occupancy_words(int nx, int ny, int nz) {
+  if (!occ_sides_ok(nx, ny, nz)) return 0;
+  return static_cast<size_t>((static_cast<long long>(nx) * ny * nz + 31) / 32);
+}
+
+size_t nrn_occupancy_build_workspace_bytes(int nx, int ny, int nz) {
+  if (!occ_sides_ok(nx, ny, nz)) return 0;
+  return 2 * static_cast<size_t>(nx) * ny * nz;
+}
+
+int nrn_occupancy_build(const float* sigma, int nx, int ny, int nz, float threshold, int dilation, void* workspace, uint32_t* bits,
+                        void* stream) {
+  const char* who = "nrn_occupancy_build";
+  if (!occ_sides_ok(nx, ny, nz)) return fail(NRN_E_INVALID, "%s: resolution %d x %d x %d out of range (1..%d cells per axis)", who, nx, ny, nz, nrn::kOccMaxSide);
+  if (dilation < 0 || dilation > nrn::kOccMaxDilation) return fail(NRN_E_INVALID, "%s: dilation=%d out of range (0..%d)", who, dilation, nrn::kOccMaxDilation);
+  if (threshold != threshold) return fail(NRN_E_INVALID, "%s: threshold is NaN", who);
+  if (!sigma || !workspace || !bits) return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (reinterpret_cast<uintptr_t>(bits) & 3u) return fail(NRN_E_INVALID, "%s: bits must be 4-byte aligned", who);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return timed(31, st, "occupancy_build", [&] {
+    return nrn::launch_occupancy_build(sigma, nx, ny, nz, threshold, dilation, static_cast<uint8_t*>(workspace), bits, st);
+  });
+}
+
+size_t nrn_occupancy_compact_workspace_bytes(int64_t n_points) {
+  if (n_points < 0 || n_points > nrn::kOccMaxPoints) return 0;
+  return occ_block_count_bytes(n_points);
+}
+
+int nrn_occupancy_compact(const NrnOccupancyGrid* grid, const float* points, int64_t n_points, int64_t points_stride, float* kept_xyz,
+                          int32_t* kept_index, int32_t* count, void* workspace, void* stream) {
+  const char* who = "nrn_occupancy_compact";
+  nrn::OccGrid g;
+  int rc = occ_grid(grid, who, &g);
+  if (rc) return rc;
+  if (n_points < 0 || n_points > nrn::kOccMaxPoints) return fail(NRN_E_INVALID, "%s: n_points=%lld out of range (0..2^31 - 1)", who, (long long)n_points);
+  if (points_stride < 3) return fail(NRN_E_INVALID, "%s: points_stride < 3", who);
+  if (!count || !workspace || (n_points > 0 && (!points || !kept_xyz || !kept_index))) return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (reinterpret_cast<uintptr_t>(workspace) & 255u) return fail(NRN_E_INVALID, "%s: workspace must be 256-byte aligned", who);
+  nrn::OccPoints s{};
+  s.pts = points; s.pts_stride = points_stride; s.P = n_points; s.S = 1;
+  nrn::OccCompact c{};
+  c.kept_xyz = kept_xyz; c.kept_idx = kept_index; c.count = count; c.block_counts = static_cast<int32_t*>(workspace);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return timed(33, st, "occupancy_compact", [&] { return nrn::launch_occupancy_compact(g, s, c, st); });
+}
+
+size_t nrn_occupancy_workspace_bytes(int n_rays, int n_samples, int out_ch, int has_bender) {
+  if (n_rays < 0 || n_samples < 1 || out_ch < 4 || out_ch > 5) return 0;
+  const long long P = static_cast<long long>(n_rays) * n_samples;
+  if (P > nrn::kOccMaxPoints) return 0;
+  const size_t p = static_cast<size_t>(P);
+  return (has_bender ? align256(p * sizeof(float4)) : 0) + align256(p * 3 * sizeof(float)) + align256(p * sizeof(int32_t)) +
+         align256(p * out_ch * sizeof(float)) + align256(sizeof(int32_t)) + occ_block_count_bytes(P);
+}
+
+int nrn_field_forward_occupancy(const NrnFieldArgs* a, const NrnOccupancyGrid* grid, void* workspace, size_t workspace_bytes) {
+  const char* who = "nrn_field_forward_occupancy";
+  long long P;
+  int tiles;
+  int rc = check_field_args(a, who, &P, &tiles);
+  if (rc) return rc;
+  if (a->stash || a->relu_mask) return fail(NRN_E_INVALID, "%s: inference only (stash / relu_mask must be NULL)", who);
+  if (a->points) return fail(NRN_E_INVALID, "%s: needs ray mode (rays and z_vals; points must be NULL)", who);
+  nrn::OccGrid g;
+  rc = occ_grid(grid, who, &g);
+  if (rc) return rc;
+  if (P > nrn::kOccMaxPoints) return fail(NRN_E_INVALID, "%s: %lld points in one pass (at most 2^31 - 1)", who, P);
+  if (P == 0) return NRN_OK;
+  const bool bend = a->bender_packed != nullptr;
+  if (!a->raw) return fail(NRN_E_INVALID, "%s: null raw", who);
+  const size_t need = nrn_occupancy_workspace_bytes(a->n_rays, a->n_samples, a->out_ch, bend);
+  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255u) || workspace_bytes < need)
+    return fail(NRN_E_INVALID, "%s: workspace null, not 256-byte aligned or smaller than nrn_occupancy_workspace_bytes (%zu)", who, need);
+  DeviceState* ds;
+  rc = device_state(&ds);
+  if (rc) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  const size_t p = static_cast<size_t>(P);
+  uint8_t* w = static_cast<uint8_t*>(workspace);
+  float4* ws = nullptr;
+  if (bend) { ws = reinterpret_cast<float4*>(w); w += align256(p * sizeof(float4)); }
+  float* kept_xyz = reinterpret_cast<float*>(w); w += align256(p * 3 * sizeof(float));
+  int32_t* kept_idx = reinterpret_cast<int32_t*>(w); w += align256(p * sizeof(int32_t));
+  float* craw = reinterpret_cast<float*>(w); w += align256(p * a->out_ch * sizeof(float));
+  int32_t* count = reinterpret_cast<int32_t*>(w); w += align256(sizeof(int32_t));
+  int32_t* block_counts = reinterpret_cast<int32_t*>(w);
+
+  nrn::FieldFwdParams p0 = field_fwd_params(a, P, tiles, ds->err_word);
+  // a. the bend pass: bent points and rigidities -> ws, and the details
+  if (bend) {
+    nrn::ViewParams vp{};
+    vp.ws = ws;
+    rc = timed(32, st, "field_bend_kernel", [&] { return nrn::launch_field_bend(p0, vp, ds->num_sms, st); });
+    if (rc) return rc;
+  }
+  // b. lookup and compaction (without a bender the points come from the rays and depths, with their details)
+  nrn::OccPoints s{};
+  s.ws = ws; s.rays = a->rays; s.z_vals = a->z_vals; s.S = a->n_samples; s.P = P;
+  nrn::OccCompact c{};
+  c.kept_xyz = kept_xyz; c.kept_idx = kept_idx; c.count = count; c.block_counts = block_counts;
+  if (!bend) { c.d_init = a->initial_input_pts; c.d_bent = a->input_pts; }
+  rc = timed(33, st, "occupancy_compact", [&] { return nrn::launch_occupancy_compact(g, s, c, st); });
+  if (rc) return rc;
+  // c. the point-mode trunk on the kept points, their count read on the device
+  nrn::FieldFwdParams q{};
+  q.pts = kept_xyz; q.pts_stride = 3; q.n_rays = static_cast<int>(P); q.S = 1; q.P = P; q.n_tiles = tiles;
+  q.nerf_w = p0.nerf_w; q.nerf_bias = p0.nerf_bias; q.out_ch = a->out_ch; q.raw = craw; q.err = ds->err_word;
+  rc = timed(34, st, "field_fwd_kept_kernel", [&] { return nrn::launch_field_fwd_kept(q, count, ds->num_sms, st); });
+  if (rc) return rc;
+  // d. raw of every sample: the trunk's where kept (with the object removal), zero elsewhere
+  return timed(35, st, "occupancy_scatter", [&] {
+    return nrn::launch_occupancy_scatter(craw, kept_idx, count, P, a->out_ch, ws, a->use_removal, a->removal_threshold, a->raw, ds->num_sms, st);
+  });
 }
 
 // Turning timing off only stops recording: a CUDA graph captured while it was on keeps event-record nodes that refer to

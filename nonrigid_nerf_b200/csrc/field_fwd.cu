@@ -495,6 +495,14 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bend_kernel(const FieldF
 __global__ void __launch_bounds__(kFwdThreads, 1) field_views_kernel(const FieldFwdParams p, const ViewParams v) {
   field_fwd_body<false, false, false, kViews>(p, v);
 }
+// The point-mode trunk (no bender) over the points an occupancy lookup kept (occupancy.cu): their count is read from device
+// memory, so a render pass that skips empty space needs no host synchronisation and can be captured in a CUDA graph
+__global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kept_kernel(FieldFwdParams p, const int* __restrict__ kept) {
+  p.P = *kept;
+  p.n_rays = static_cast<int>(p.P);
+  p.n_tiles = static_cast<int>((p.P + kTileM - 1) / kTileM);
+  field_fwd_body<false, false, false>(p);
+}
 __global__ void __launch_bounds__(kFwdThreads, 1) field_views_train_kernel(const FieldFwdParams p, const ViewParams v, const ViewTrainParams t) {
   field_fwd_body<false, true, false, kViews>(p, v, t);
 }
@@ -559,6 +567,11 @@ cudaError_t launch_field_views(const FieldFwdParams& p, const ViewParams& v, int
 // Training the view-dependent head without a bender: p.stash / p.relu_mask and t's buffers are written
 cudaError_t launch_field_views_train(const FieldFwdParams& p, const ViewParams& v, const ViewTrainParams& t, int num_sms, cudaStream_t stream) {
   return launch_field(field_views_train_kernel, p, num_sms, field_views_smem_bytes(), stream, v, t);
+}
+
+// p.P (and p.n_tiles) bound the kept count: they size the grid; the kernel takes the count itself from `kept`
+cudaError_t launch_field_fwd_kept(const FieldFwdParams& p, const int* kept, int num_sms, cudaStream_t stream) {
+  return launch_field(field_fwd_kept_kernel, p, num_sms, field_fwd_smem_bytes(), stream, kept);
 }
 
 cudaError_t launch_field_fwd_tc(const FieldFwdParams& p, int num_sms, cudaStream_t stream) {

@@ -25,7 +25,8 @@ O(nx * ny) plus the mesh.  density_grid alone materialises the whole volume.  V 
 from __future__ import annotations
 
 import ctypes as C
-from typing import NamedTuple, Optional
+import dataclasses
+from typing import NamedTuple, Optional, Tuple
 
 import numpy as np
 import torch
@@ -249,6 +250,90 @@ def extract_mesh(network_fn, min_point, max_point, resolution, threshold: float,
                 if rig is not None:
                     rig[c0:c1].copy_(det["rigidity_mask"].view(-1))
     return Mesh(v, f, col, rig, vo, fo)
+
+
+# ---- occupancy grids ------------------------------------------------------------------------------------------------------
+@dataclasses.dataclass(frozen=True, eq=False)
+class OccupancyGrid:
+    """Which cells of the canonical volume may hold density, for render(..., occupancy=grid).  nx * ny * nz cells over
+    [min_point, max_point]; cell (i, j, k) is bit c % 32 of word c // 32 of `bits`, c = (k * ny + j) * nx + i.  A sample is
+    evaluated when its (bent) point lies in an occupied cell, outside the box, or has a non-finite coordinate; its cell is
+    min(floor(fl(fl(x - min) * scale)), n - 1) per axis with scale = fl(n / fl(max - min)), all in fp32.  Not a tuple, so
+    the ray-sharded render wrapper hands it to every rank as it is."""
+    bits: torch.Tensor                 # [ceil(nx * ny * nz / 32)] int32 on the model's device
+    min_point: np.ndarray              # [3] float32
+    max_point: np.ndarray              # [3] float32
+    resolution: Tuple[int, int, int]   # (nx, ny, nz) cells
+
+    def c_struct(self, device) -> "_lib.NrnOccupancyGrid":
+        """The grid as the C ABI reads it; raises unless the bits are a contiguous int32 tensor of the right length on `device`."""
+        nx, ny, nz = self.resolution
+        words = _lib.load().nrn_occupancy_words(nx, ny, nz)
+        b = self.bits
+        if not (isinstance(b, torch.Tensor) and b.dtype == torch.int32 and b.dim() == 1 and b.is_contiguous() and b.numel() == words):
+            raise RuntimeError(f"nonrigid_nerf_b200: occupancy bits must be a contiguous [{words}] int32 tensor for resolution "
+                               f"{self.resolution}")
+        if b.device != torch.device(device):
+            raise RuntimeError(f"nonrigid_nerf_b200: the occupancy grid is on {b.device}, the rays on {device}")
+        g = _lib.NrnOccupancyGrid()
+        g.bits, g.nx, g.ny, g.nz = b.data_ptr(), nx, ny, nz
+        g.min_point[:] = [float(v) for v in self.min_point]
+        g.max_point[:] = [float(v) for v in self.max_point]
+        return g
+
+    def occupied_fraction(self) -> float:
+        """The fraction of cells marked occupied (reads the bits back to the host)."""
+        nx, ny, nz = self.resolution
+        words = self.bits.cpu().numpy().view(np.uint8)
+        return float(np.unpackbits(words, bitorder="little")[:nx * ny * nz].sum()) / (nx * ny * nz)
+
+
+def _cells(resolution):
+    r = (resolution,) * 3 if isinstance(resolution, (int, np.integer)) else tuple(resolution)
+    if len(r) != 3 or any(not isinstance(n, (int, np.integer)) or isinstance(n, bool) for n in r):
+        raise RuntimeError(f"nonrigid_nerf_b200: resolution must be an int or (nx, ny, nz) cells, got {resolution!r}")
+    if any(n < 1 or n > 4096 for n in r):
+        raise RuntimeError(f"nonrigid_nerf_b200: occupancy resolution must be 1..4096 cells on every axis, got {r}")
+    return tuple(int(n) for n in r)
+
+
+def occupancy_from_sigma(sigma: torch.Tensor, min_point, max_point, threshold: float, dilation: int = 1) -> OccupancyGrid:
+    """The occupancy grid of densities sigma [nz + 1, ny + 1, nx + 1] (fp32 CUDA) at the corners of nx * ny * nz cells
+    spanning min_point .. max_point, as density_grid lays them out: a cell is occupied when any of its 8 corners has
+    sigma > threshold or NaN, and the occupied set is then dilated by `dilation` cells (Chebyshev distance)."""
+    if not isinstance(sigma, torch.Tensor) or not sigma.is_cuda or sigma.dim() != 3:
+        raise RuntimeError("nonrigid_nerf_b200: sigma must be a [nz + 1, ny + 1, nx + 1] CUDA tensor (there is no CPU path)")
+    nx, ny, nz = _cells((sigma.shape[2] - 1, sigma.shape[1] - 1, sigma.shape[0] - 1))
+    lo, hi = _extent(min_point, max_point)
+    if isinstance(dilation, bool) or not isinstance(dilation, (int, np.integer)) or not 0 <= dilation <= 4096:
+        raise RuntimeError(f"nonrigid_nerf_b200: dilation must be an int in 0..4096, got {dilation!r}")
+    t = float(np.float32(threshold))
+    if t != t:
+        raise RuntimeError("nonrigid_nerf_b200: threshold is NaN")
+    lib = _lib.load()
+    sigma = sigma.float().contiguous()
+    dev = sigma.device
+    bits = torch.empty(lib.nrn_occupancy_words(nx, ny, nz), dtype=torch.int32, device=dev)
+    ws = torch.empty(lib.nrn_occupancy_build_workspace_bytes(nx, ny, nz), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.nrn_occupancy_build(sigma.data_ptr(), nx, ny, nz, t, int(dilation), ws.data_ptr(), bits.data_ptr(), _stream()),
+                   "occupancy_build")
+    return OccupancyGrid(bits, lo, hi, (nx, ny, nz))
+
+
+def occupancy_grid(network_fn, min_point, max_point, resolution, threshold: float, dilation: int = 1) -> OccupancyGrid:
+    """The occupancy grid of network_fn's canonical density (the bender off, as render_canonical renders) on
+    resolution = n or (nx, ny, nz) cells over min_point .. max_point (for example the scene's min_nerf_volume_point /
+    max_nerf_volume_point): occupancy_from_sigma(density_grid(network_fn, min_point, max_point, (nx + 1, ny + 1, nz + 1)),
+    ...).  The model's test-time knobs of the NeRF (object removal needs a bender, so it never applies here) are as in
+    density_grid.  Not implemented for use_viewdirs=True and time_conditioned_baseline=True models."""
+    if getattr(network_fn, "use_viewdirs", False):
+        raise RuntimeError("nonrigid_nerf_b200: occupancy grids of a view-dependent model (use_viewdirs=True) are not implemented")
+    if getattr(network_fn, "time_conditioned_baseline", False):
+        raise RuntimeError("nonrigid_nerf_b200: occupancy grids of a time_conditioned_baseline=True model are not implemented")
+    nx, ny, nz = _cells(resolution)
+    sigma = density_grid(network_fn, min_point, max_point, (nx + 1, ny + 1, nz + 1), latent=None)
+    return occupancy_from_sigma(sigma, min_point, max_point, threshold, dilation)
 
 
 # ---- host-side writers --------------------------------------------------------------------------------------------------

@@ -77,7 +77,8 @@ def raw2outputs(raw, z_vals, rays_d, raw_noise_std=0, white_bkgd=False, pytest=F
 # ---- render_rays (train.py:792-980) ---------------------------------------------------------------
 def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False, lindisp=False, perturb=0.0,
                 N_importance=0, network_fine=None, white_bkgd=False, raw_noise_std=0.0,
-                additional_pixel_information=None, detailed_output=False, verbose=False, pytest=False, held_out=None, **dummy_kwargs):
+                additional_pixel_information=None, detailed_output=False, verbose=False, pytest=False, held_out=None, occupancy=None,
+                **dummy_kwargs):
     """Volumetric rendering of a ray batch [N, 8] = (o, d, near, far).  `network_query_fn` is accepted
     for signature compatibility; the field is evaluated by the fused kernel on `network_fn` /
     `network_fine` (which carry their ray bender as `.ray_bender[0]`).
@@ -87,7 +88,10 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     held_out [N] (bool or uint8, on the rays' device): rays of held-out frames.  With a ray bender their gradient reaches
     only their latent codes, not the coarse, fine or bender weights; without one they contribute no gradient at all.  So
     one backward of ((train + held_out) * loss).mean() gives the gradients of the reference's two backward passes
-    (train.py:1595-1608).  None: the ordinary path."""
+    (train.py:1595-1608).  None: the ordinary path.
+    occupancy (geometry.OccupancyGrid, under torch.no_grad() only): each pass evaluates the NeRF trunk only on samples
+    whose bent point lies in an occupied cell, outside the grid's box, or is not finite; the others get raw = 0.  None:
+    every sample is evaluated."""
     if pytest:
         raise RuntimeError("nonrigid_nerf_b200: the pytest= numpy-random hook is not supported")
     if not isinstance(network_fn, NeRF) or (network_fine is not None and not isinstance(network_fine, NeRF)):
@@ -105,6 +109,13 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     latents = None
     if network_fn.ray_bender[0] is not None or getattr(network_fn, "time_conditioned_baseline", False):
         latents = additional_pixel_information["ray_bending_latents"]
+    if occupancy is not None:
+        _check_occupancy(occupancy, network_fn, network_fine if N_importance > 0 else None, latents)
+
+    def field(net, z):
+        if occupancy is None:
+            return _ag.field(net, rays, z, latents, detailed_output, viewdirs, held_out)
+        return _ag.field_occupancy(net, rays, z, latents, detailed_output, occupancy)
 
     rnd = dummy_kwargs.get("randomness", None)
 
@@ -139,7 +150,7 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     # coarse depths (train.py:847-869); t_rand drawn first, like the reference
     t_rand = draw("t_rand", torch.rand, n, N_samples) if perturb > 0.0 else None
     z_vals = ops.sample_coarse(rays, N_samples, t_rand, lindisp)
-    raw, details = _ag.field(network_fn, rays, z_vals, latents, detailed_output, viewdirs, held_out)
+    raw, details = field(network_fn, z_vals)
     noise = draw("noise_c", torch.randn, n, N_samples) if raw_noise_std > 0.0 else None   # already scaled by raw_noise_std
 
     if N_importance > 0:
@@ -147,7 +158,7 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
         c0 = _ag.composite(raw, z_vals, rays_d, noise, white_bkgd, N_importance, u)
         z_fine = c0["z_vals_out"]   # sorted union, detached (train.py:918-920)
         run_fn = network_fn if network_fine is None else network_fine
-        raw, fine_details = _ag.field(run_fn, rays, z_fine, latents, detailed_output, viewdirs, held_out)
+        raw, fine_details = field(run_fn, z_fine)
         noise_f = draw("noise_f", torch.randn, n, n_fine) if raw_noise_std > 0.0 else None
         c1 = _ag.composite(raw, z_fine, rays_d, noise_f, white_bkgd)
     else:
@@ -212,6 +223,13 @@ def _check_views(batch_has_viewdirs, network_fn, network_fine, additional_pixel_
         _ag.views_check(net, info.get("ray_bending_latents"))
 
 
+def _check_occupancy(occupancy, network_fn, network_fine, latents):
+    """Before any launch: render(..., occupancy=grid) is refused for what it does not support (_ag.occupancy_check)."""
+    for net in (network_fn, network_fine):
+        if net is not None:
+            _ag.occupancy_check(net, latents, occupancy)
+
+
 # ---- batchify_rays / render (train.py:108-137, :326-416) --------------------------------------------
 def batchify_rays(rays_flat, additional_pixel_information, chunk=1024 * 32, detailed_output=False, **kwargs):
     """Render rays in chunks (`chunk` only bounds the per-launch working set; results do not depend on it)."""
@@ -230,7 +248,10 @@ def batchify_rays(rays_flat, additional_pixel_information, chunk=1024 * 32, deta
 def render(rays_o, rays_d, chunk=1024 * 32, ndc=True, near=0.0, far=1.0, use_viewdirs=False, c2w_staticcam=None,
            additional_pixel_information=None, detailed_output=False, **kwargs):
     """Render rays.  Returns [rgb_map, disp_map, acc_map, extras] (train.py:326-416).  Keyword held_out [N] (one entry
-    per ray of the flattened batch): see render_rays."""
+    per ray of the flattened batch) and keyword occupancy (a geometry.OccupancyGrid): see render_rays."""
+    if kwargs.get("network_fn") is not None and kwargs.get("occupancy") is not None:
+        _check_occupancy(kwargs["occupancy"], kwargs["network_fn"], kwargs.get("network_fine") if kwargs.get("N_importance", 0) > 0 else None,
+                         (additional_pixel_information or {}).get("ray_bending_latents"))
     if kwargs.get("network_fn") is not None:
         _check_views(bool(use_viewdirs), kwargs["network_fn"], kwargs.get("network_fine") if kwargs.get("N_importance", 0) > 0 else None,
                      additional_pixel_information)
