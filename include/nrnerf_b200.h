@@ -665,6 +665,39 @@ int nrn_occupancy_compact(const NrnOccupancyGrid* grid, const float* points, int
 size_t nrn_occupancy_workspace_bytes(int n_rays, int n_samples, int out_ch, int has_bender);
 int nrn_field_forward_occupancy(const NrnFieldArgs* args, const NrnOccupancyGrid* grid, void* workspace, size_t workspace_bytes);
 
+/* ---- early ray termination: render passes that stop evaluating a ray's samples once its transmittance is small ------
+ * The reference evaluates every sample of every ray (train.py:876-886, :927-937); this pass is an inference-only option
+ * it does not have.  Samples 0..S-1 of a ray are split into segments of K = nrn_termination_segment() samples; round r
+ * evaluates segment r, samples [r K, min((r + 1) K, S)), of every ray still alive (all rays are alive at round 0), and
+ * ceil(S / K) rounds make a pass.  After round r every alive ray updates T <- T * (1 - alpha_i + 1e-10) over the
+ * segment's samples in order, in fp32 with one rounded multiply per step, from T = 1, where alpha_i is compositing's own
+ * (nrn_composite; train.py:740-761: relu(sigma + noise), the distance to the next depth, 1e10 past the last, times |d|)
+ * on the raw that round wrote, object removal included.  The ray dies when T < threshold; a NaN T never does, nor does
+ * any T for threshold 0.  A sample not evaluated gets raw = 0 (so alpha = 0 and a factor of exactly 1).
+ *
+ * nrn_field_forward_terminate: one inference pass of nrn_field_forward in ray mode (args as there, no stash / relu_mask,
+ *   points NULL).  With a bender the bend pass runs first over every sample (bent points, rigidities and the details);
+ *   then per round the lookup and compaction of that segment's samples only (kept: the ray is alive and, when grid is
+ *   not NULL, the grid keeps the point, as in nrn_field_forward_occupancy; without a bender this step also writes every
+ *   sample's initial_input_pts / input_pts), the point-mode trunk on the kept points, the scatter into raw (zeroed once
+ *   before round 0) and the transmittance update.  raw of an evaluated sample equals nrn_field_forward's bit for bit.
+ *   The rounds come from the shapes, so nothing waits on the host and the pass can be captured in a CUDA graph.
+ *   termination_index [n_rays] (int32): the first sample skipped because of termination, i.e. the end of the segment in
+ *   which T fell below the threshold, or S if the ray never died.  noise [n_rays][n_samples]: the additive sigma noise
+ *   (already scaled by raw_noise_std) that compositing will use, or NULL.  workspace:
+ *   nrn_termination_workspace_bytes(n_rays, n_samples, out_ch, bender_packed != NULL), 256-byte aligned.  A threshold
+ *   outside [0, 1] or NaN, a null termination_index, a malformed grid, more than 2^31 - 1 points or a short workspace
+ *   return NRN_E_INVALID before any CUDA call; n_rays = 0 launches nothing. */
+typedef struct NrnTerminationArgs {
+  float threshold;              /* in [0, 1]: a ray dies when its transmittance T < threshold */
+  const float* noise;           /* [n_rays][n_samples] additive sigma noise, or NULL */
+  int32_t* termination_index;   /* [n_rays] out */
+} NrnTerminationArgs;
+int nrn_termination_segment(void);
+size_t nrn_termination_workspace_bytes(int n_rays, int n_samples, int out_ch, int has_bender);
+int nrn_field_forward_terminate(const NrnFieldArgs* args, const NrnOccupancyGrid* grid /* NULL: none */, const NrnTerminationArgs* term,
+                                void* workspace, size_t workspace_bytes);
+
 /* ---- optional per-kernel timing (measurement aid for bench.py) ---------------------------------
  * While enabled, every launch of the kernel kinds below is bracketed by CUDA events recorded on the
  * launch stream.  kinds: 0 field forward, 1 field DGRAD, 2 WGRAD (+reduce), 3 composite(+resample),
@@ -680,7 +713,9 @@ int nrn_field_forward_occupancy(const NrnFieldArgs* args, const NrnOccupancyGrid
  * mask and input scaling, 26 the convolutions, 27 the max-pools and 28 the distances and per-frame sums, and of nrn_match 29
  * the grid builds (boxes, counts, scans, scatters) and 30 the queries with their round trips, 31 nrn_occupancy_build, and of
  * nrn_field_forward_occupancy 32 the bend pass, 33 the lookup and compaction (also nrn_occupancy_compact), 34 the trunk on
- * the kept points and 35 the scatter.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * the kept points and 35 the scatter, and of nrn_field_forward_terminate 36 the bend pass, 37 the lookups and compactions,
+ * 38 the trunk on the kept points, 39 the scatters (and the zeroing of raw) and 40 the transmittance updates (and their
+ * initialisation).  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

@@ -197,6 +197,10 @@ class NrnOccupancyGrid(C.Structure):
     ]
 
 
+class NrnTerminationArgs(C.Structure):
+    _fields_ = [("threshold", C.c_float), ("noise", _vp), ("termination_index", _vp)]
+
+
 # every symbol include/nrnerf_b200.h declares: (restype, argtypes)
 SYMBOLS = {
     "nrn_abi_version": (C.c_int, []),
@@ -287,6 +291,10 @@ SYMBOLS = {
     "nrn_occupancy_compact": (C.c_int, [C.POINTER(NrnOccupancyGrid), _vp, C.c_int64, C.c_int64, _vp, _vp, _vp, _vp, _vp]),
     "nrn_occupancy_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
     "nrn_field_forward_occupancy": (C.c_int, [C.POINTER(NrnFieldArgs), C.POINTER(NrnOccupancyGrid), _vp, C.c_size_t]),
+    "nrn_termination_segment": (C.c_int, []),
+    "nrn_termination_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
+    "nrn_field_forward_terminate": (C.c_int, [C.POINTER(NrnFieldArgs), C.POINTER(NrnOccupancyGrid), C.POINTER(NrnTerminationArgs), _vp,
+                                              C.c_size_t]),
     "nrn_timing_enable": (C.c_int, [C.c_int]),
     "nrn_timing_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int), C.c_int]),
 }
@@ -315,6 +323,10 @@ MATCH_KERNEL_KINDS = ("match_build", "match_query")
 # occupancy grids (grid build; of a render pass: bend pass, lookup + compaction, trunk on the kept points, scatter),
 # timing kinds 31 to 35
 OCCUPANCY_KERNEL_KINDS = ("occupancy_build", "occupancy_bend", "occupancy_compact", "occupancy_field", "occupancy_scatter")
+# early-terminating render passes (bend pass, lookups + compactions, trunk on the kept points, scatters, transmittance
+# updates), timing kinds 36 to 40
+TERMINATION_KERNEL_KINDS = ("termination_bend", "termination_compact", "termination_field", "termination_scatter",
+                            "termination_transmittance")
 
 
 def timing_enable(on: bool) -> None:
@@ -324,8 +336,8 @@ def timing_enable(on: bool) -> None:
 def timing_read(kinds=KERNEL_KINDS):
     """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True); `kinds` is KERNEL_KINDS,
     KERNEL_KINDS + TC_KERNEL_KINDS, KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS, that + VIEW_TRAIN_KERNEL_KINDS,
-    that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS, that + EVAL_KERNEL_KINDS, that + FRAME_IMAGE_KERNEL_KINDS, that + MESH_KERNEL_KINDS, that + LPIPS_KERNEL_KINDS, that + MATCH_KERNEL_KINDS or that
-    + OCCUPANCY_KERNEL_KINDS."""
+    that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS, that + EVAL_KERNEL_KINDS, that + FRAME_IMAGE_KERNEL_KINDS, that + MESH_KERNEL_KINDS, that + LPIPS_KERNEL_KINDS, that + MATCH_KERNEL_KINDS, that
+    + OCCUPANCY_KERNEL_KINDS or that + TERMINATION_KERNEL_KINDS."""
     n = len(kinds)
     ms = (C.c_double * n)()
     cnt = (C.c_int * n)()

@@ -14,8 +14,10 @@ z_vals, ray origins/directions and the importance samples carry no gradient (tra
 from __future__ import annotations
 
 import ctypes as C
+import numbers
 from typing import Dict, Optional, Tuple
 
+import numpy as np
 import torch
 
 from . import _lib, ops
@@ -714,6 +716,46 @@ def field_occupancy(net, rays, z_vals, latents, want_details, grid):
     out_ch = net.output_linear.weight.shape[0]
     return ops.field_forward_occupancy(rays, z_vals, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details,
                                        grid)
+
+
+def termination_threshold(threshold) -> float:
+    """The early-termination threshold as a float; raises unless it is a finite real number in [0, 1] (not a bool or a
+    tensor)."""
+    if isinstance(threshold, (bool, np.bool_, torch.Tensor)) or not isinstance(threshold, numbers.Real):
+        raise RuntimeError(f"nonrigid_nerf_b200: early_termination must be a real number in [0, 1], got {type(threshold).__name__}")
+    t = float(threshold)
+    if not (0.0 <= t <= 1.0):
+        raise RuntimeError(f"nonrigid_nerf_b200: early_termination must be a finite real number in [0, 1], got {t!r}")
+    return t
+
+
+def termination_check(net, latents, threshold) -> float:
+    """Raise, before any launch, for what render(..., early_termination=t) does not support: a threshold that is not a
+    finite real in [0, 1], the view-dependent head, the time-conditioned baseline and differentiable calls.  Returns t."""
+    t = termination_threshold(threshold)
+    if getattr(net, "use_viewdirs", False):
+        raise RuntimeError("nonrigid_nerf_b200: rendering with early_termination is not implemented for use_viewdirs=True")
+    if getattr(net, "time_conditioned_baseline", False):
+        raise RuntimeError("nonrigid_nerf_b200: rendering with early_termination is not implemented for time_conditioned_baseline=True")
+    if _needs_grad(net, latents):
+        raise RuntimeError("nonrigid_nerf_b200: rendering with early_termination is inference only; call render() under "
+                           "torch.no_grad() (samples that are not evaluated would get no gradient)")
+    return t
+
+
+def field_terminate(net, rays, z_vals, latents, want_details, threshold, grid=None, noise=None):
+    """field_rays with early ray termination (and, with `grid`, the occupancy grid's skipping): raw is 0 for samples not
+    evaluated.  Returns (raw, details, termination_index)."""
+    t = termination_check(net, latents, threshold)
+    if grid is not None:
+        occupancy_check(net, latents, grid)
+    bender = net.ray_bender[0]
+    cutoff, scaling, removal = _knobs(net)
+    nerf_pack = ops.pack_nerf(net)
+    bender_pack = ops.pack_bender(bender) if bender is not None else None
+    out_ch = net.output_linear.weight.shape[0]
+    return ops.field_forward_terminate(rays, z_vals, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details, t,
+                                       grid, noise)
 
 
 def field_rays(net, rays, z_vals, latents, want_details):

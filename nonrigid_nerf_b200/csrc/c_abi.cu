@@ -1,5 +1,6 @@
 // extern "C" boundary of libnrnerf_b200.so (declarations: include/nrnerf_b200.h).
 // Argument validation, launch, error reporting.  No exceptions cross this file.
+#include <algorithm>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -1487,6 +1488,113 @@ int nrn_field_forward_occupancy(const NrnFieldArgs* a, const NrnOccupancyGrid* g
   return timed(35, st, "occupancy_scatter", [&] {
     return nrn::launch_occupancy_scatter(craw, kept_idx, count, P, a->out_ch, ws, a->use_removal, a->removal_threshold, a->raw, ds->num_sms, st);
   });
+}
+
+// ---- early ray termination: a render pass in depth-ordered rounds over segments of nrn_termination_segment() samples ----
+int nrn_termination_segment(void) { return nrn::kTermSegment; }
+
+size_t nrn_termination_workspace_bytes(int n_rays, int n_samples, int out_ch, int has_bender) {
+  if (n_rays < 0 || n_samples < 1 || out_ch < 4 || out_ch > 5) return 0;
+  const long long P = static_cast<long long>(n_rays) * n_samples;
+  if (P > nrn::kOccMaxPoints) return 0;
+  const size_t p = static_cast<size_t>(P);
+  const long long Pk = static_cast<long long>(n_rays) * std::min(nrn::kTermSegment, n_samples);   // the slots of one round
+  const size_t pk = static_cast<size_t>(Pk);
+  return (has_bender ? align256(p * sizeof(float4)) : 0) + align256(pk * 3 * sizeof(float)) + align256(pk * sizeof(int32_t)) +
+         align256(pk * out_ch * sizeof(float)) + align256(sizeof(int32_t)) + occ_block_count_bytes(Pk) +
+         align256(static_cast<size_t>(n_rays) * sizeof(float));
+}
+
+int nrn_field_forward_terminate(const NrnFieldArgs* a, const NrnOccupancyGrid* grid, const NrnTerminationArgs* term, void* workspace,
+                                size_t workspace_bytes) {
+  const char* who = "nrn_field_forward_terminate";
+  long long P;
+  int tiles;
+  int rc = check_field_args(a, who, &P, &tiles);
+  if (rc) return rc;
+  if (a->stash || a->relu_mask) return fail(NRN_E_INVALID, "%s: inference only (stash / relu_mask must be NULL)", who);
+  if (a->points) return fail(NRN_E_INVALID, "%s: needs ray mode (rays and z_vals; points must be NULL)", who);
+  if (!term) return fail(NRN_E_INVALID, "%s: null termination args", who);
+  if (!(term->threshold >= 0.f && term->threshold <= 1.f))
+    return fail(NRN_E_INVALID, "%s: early-termination threshold %g outside [0, 1]", who, static_cast<double>(term->threshold));
+  nrn::OccGrid g{};
+  if (grid) {
+    rc = occ_grid(grid, who, &g);
+    if (rc) return rc;
+  }
+  if (P > nrn::kOccMaxPoints) return fail(NRN_E_INVALID, "%s: %lld points in one pass (at most 2^31 - 1)", who, P);
+  if (P == 0) return NRN_OK;
+  const bool bend = a->bender_packed != nullptr;
+  if (!a->raw) return fail(NRN_E_INVALID, "%s: null raw", who);
+  if (!term->termination_index) return fail(NRN_E_INVALID, "%s: null termination_index", who);
+  const size_t need = nrn_termination_workspace_bytes(a->n_rays, a->n_samples, a->out_ch, bend);
+  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255u) || workspace_bytes < need)
+    return fail(NRN_E_INVALID, "%s: workspace null, not 256-byte aligned or smaller than nrn_termination_workspace_bytes (%zu)", who, need);
+  DeviceState* ds;
+  rc = device_state(&ds);
+  if (rc) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  const int S = a->n_samples, K = std::min(nrn::kTermSegment, S);
+  const size_t p = static_cast<size_t>(P);
+  const long long Pk = static_cast<long long>(a->n_rays) * K;
+  const size_t pk = static_cast<size_t>(Pk);
+  uint8_t* w = static_cast<uint8_t*>(workspace);
+  float4* ws = nullptr;
+  if (bend) { ws = reinterpret_cast<float4*>(w); w += align256(p * sizeof(float4)); }
+  float* kept_xyz = reinterpret_cast<float*>(w); w += align256(pk * 3 * sizeof(float));
+  int32_t* kept_idx = reinterpret_cast<int32_t*>(w); w += align256(pk * sizeof(int32_t));
+  float* craw = reinterpret_cast<float*>(w); w += align256(pk * a->out_ch * sizeof(float));
+  int32_t* count = reinterpret_cast<int32_t*>(w); w += align256(sizeof(int32_t));
+  int32_t* block_counts = reinterpret_cast<int32_t*>(w); w += occ_block_count_bytes(Pk);
+  float* T = reinterpret_cast<float*>(w);
+
+  nrn::FieldFwdParams p0 = field_fwd_params(a, P, tiles, ds->err_word);
+  // the bend pass over every sample: bent points and rigidities -> ws, and the details
+  if (bend) {
+    nrn::ViewParams vp{};
+    vp.ws = ws;
+    rc = timed(36, st, "field_bend_kernel", [&] { return nrn::launch_field_bend(p0, vp, ds->num_sms, st); });
+    if (rc) return rc;
+  }
+  nrn::TermPass t{};
+  t.raw = a->raw; t.z = a->z_vals; t.rays = a->rays; t.noise = term->noise;
+  t.n = a->n_rays; t.S = S; t.out_ch = a->out_ch; t.threshold = term->threshold;
+  t.T = T; t.term = term->termination_index;
+  // raw is zeroed once: a sample no round evaluates keeps 0
+  rc = timed(39, st, "termination_zero_raw", [&] { return cudaMemsetAsync(a->raw, 0, p * a->out_ch * sizeof(float), st); });
+  if (rc) return rc;
+  rc = timed(40, st, "term_init_kernel", [&] { return nrn::launch_termination_init(t, st); });
+  if (rc) return rc;
+  nrn::OccPoints s{};
+  s.ws = ws; s.rays = a->rays; s.z_vals = a->z_vals; s.S = S; s.P = P;
+  nrn::OccCompact c{};
+  c.kept_xyz = kept_xyz; c.kept_idx = kept_idx; c.count = count; c.block_counts = block_counts;
+  if (!bend) { c.d_init = a->initial_input_pts; c.d_bent = a->input_pts; }
+  nrn::FieldFwdParams q{};
+  q.pts = kept_xyz; q.pts_stride = 3; q.n_rays = static_cast<int>(Pk); q.S = 1; q.P = Pk; q.n_tiles = static_cast<int>(tile_count(Pk));
+  q.nerf_w = p0.nerf_w; q.nerf_bias = p0.nerf_bias; q.out_ch = a->out_ch; q.raw = craw; q.err = ds->err_word;
+  for (int s0 = 0; s0 < S; s0 += K) {
+    const int len = std::min(K, S - s0);
+    nrn::OccSegment seg{};
+    seg.s0 = s0; seg.len = len; seg.P = static_cast<long long>(a->n_rays) * len; seg.term = term->termination_index;
+    seg.use_grid = grid != nullptr;
+    // 1. the lookup of this segment's samples: the ray alive (and the grid keeping the point), compacted in order
+    rc = timed(37, st, "termination_compact", [&] { return nrn::launch_termination_compact(g, s, seg, c, st); });
+    if (rc) return rc;
+    // 2. the point-mode trunk on the kept points, their count read on the device
+    rc = timed(38, st, "field_fwd_kept_kernel", [&] { return nrn::launch_field_fwd_kept(q, count, ds->num_sms, st); });
+    if (rc) return rc;
+    // 3. their raw into the pass's output (with the object removal)
+    rc = timed(39, st, "occ_scatter_kernel", [&] {
+      return nrn::launch_termination_scatter(craw, kept_idx, count, seg.P, a->out_ch, ws, a->use_removal, a->removal_threshold, a->raw,
+                                             ds->num_sms, st);
+    });
+    if (rc) return rc;
+    // 4. the transmittance over the segment; rays below the threshold die
+    rc = timed(40, st, "term_transmittance_kernel", [&] { return nrn::launch_termination_transmittance(t, s0, len, st); });
+    if (rc) return rc;
+  }
+  return NRN_OK;
 }
 
 // Turning timing off only stops recording: a CUDA graph captured while it was on keeps event-record nodes that refer to

@@ -44,6 +44,38 @@ struct OccCompact {
   float* d_bent;
 };
 
+// Samples per segment of an early-terminating render pass (nrn_field_forward_terminate): round r evaluates samples
+// [r K, min((r + 1) K, S)) of the rays still alive.  Chosen by measurement (DESIGN.md); a build may override it with
+// -DNRN_TERM_SEGMENT=K to repeat that measurement.
+#ifndef NRN_TERM_SEGMENT
+#define NRN_TERM_SEGMENT 16
+#endif
+constexpr int kTermSegment = NRN_TERM_SEGMENT;
+static_assert(kTermSegment >= 1, "NRN_TERM_SEGMENT must be positive");
+
+// One round of an early-terminating pass: lookup slot q (0 <= q < P = n_rays * len) is sample s0 + q % len of ray q / len.
+// A slot is kept while its ray is alive (its sample index < term[ray]; term holds S until the ray dies) and, when
+// use_grid is set, the grid keeps its point.
+struct OccSegment {
+  int s0, len;
+  long long P;
+  const int32_t* term;
+  int use_grid;
+};
+
+// The state of an early-terminating pass: per ray the transmittance T and termination_index (term), and what the alphas
+// of the round's samples are made of (the field's raw after the scatter, the depths, the ray directions, the noise)
+struct TermPass {
+  const float* raw;     // [n][S][out_ch]
+  const float* z;       // [n][S]
+  const float* rays;    // [n][8]
+  const float* noise;   // [n][S] or null
+  int n, S, out_ch;
+  float threshold;
+  float* T;             // [n]
+  int32_t* term;        // [n]
+};
+
 cudaError_t launch_occupancy_build(const float* sigma, int nx, int ny, int nz, float threshold, int dilation, uint8_t* ws,
                                    uint32_t* bits, cudaStream_t st);
 cudaError_t launch_occupancy_compact(const OccGrid& g, const OccPoints& pts, const OccCompact& c, cudaStream_t st);
@@ -51,5 +83,16 @@ cudaError_t launch_occupancy_compact(const OccGrid& g, const OccPoints& pts, con
 // the point's rigidity >= removal (the fused kernel's test-time object removal)
 cudaError_t launch_occupancy_scatter(const float* compact_raw, const int32_t* kept_idx, const int32_t* count, long long P, int out_ch,
                                      const float4* ws, int use_removal, float removal, float* raw, int num_sms, cudaStream_t st);
+
+// Early termination (nrn_field_forward_terminate).  init: T = 1 and term = S for every ray.  compact: the lookup and
+// compaction of one segment's slots (kept indices are the samples' indices in the pass, so the scatter takes them as they
+// are).  scatter: launch_occupancy_scatter without zeroing raw first (the pass zeroes it once).  transmittance: every
+// alive ray multiplies T by (1 - alpha + 1e-10) over samples [s0, s0 + len), in order, and dies (term = s0 + len) when
+// T < threshold.
+cudaError_t launch_termination_init(const TermPass& t, cudaStream_t st);
+cudaError_t launch_termination_compact(const OccGrid& g, const OccPoints& pts, const OccSegment& seg, const OccCompact& c, cudaStream_t st);
+cudaError_t launch_termination_scatter(const float* compact_raw, const int32_t* kept_idx, const int32_t* count, long long max_kept, int out_ch,
+                                       const float4* ws, int use_removal, float removal, float* raw, int num_sms, cudaStream_t st);
+cudaError_t launch_termination_transmittance(const TermPass& t, int s0, int len, cudaStream_t st);
 
 }  // namespace nrn

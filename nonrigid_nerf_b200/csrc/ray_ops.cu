@@ -126,7 +126,7 @@ composite_kernel(const CompositeParams p) {
 
   const float* d = p.rays_d + static_cast<long long>(ray) * p.rays_d_stride;
   const float dx = d[0], dy = d[1], dz = d[2];
-  const float dnorm = sqrtf(dx * dx + dy * dy + dz * dz);
+  const float dnorm = ray_dnorm(dx, dy, dz);
   const float* zr = p.z + static_cast<long long>(ray) * S;
   const float* rawr = p.raw + static_cast<long long>(ray) * S * p.C;
   for (int i = lane; i < S; i += 32) z_s[i] = zr[i];
@@ -138,11 +138,11 @@ composite_kernel(const CompositeParams p) {
     float alpha = 0.f, r = 0.f, g = 0.f, b = 0.f, zi = 0.f;
     if (i < S) {
       zi = z_s[i];
-      const float dist = (i + 1 < S ? z_s[i + 1] - zi : 1e10f) * dnorm;  // train.py:743-748
+      const float gap = i + 1 < S ? z_s[i + 1] - zi : 1e10f;            // train.py:743-748
       const float* q = rawr + static_cast<long long>(i) * p.C;
       float sigma = q[3];
       if (p.noise) sigma += p.noise[static_cast<long long>(ray) * S + i];  // noise already scaled by raw_noise_std
-      alpha = 1.0f - expf(-fmaxf(sigma, 0.f) * dist);                 // :740-741, 761
+      alpha = composite_alpha(sigma, gap, dnorm);                      // :740-741, 761
       r = 1.0f / (1.0f + expf(-q[0]));
       g = 1.0f / (1.0f + expf(-q[1]));
       b = 1.0f / (1.0f + expf(-q[2]));
@@ -241,7 +241,7 @@ composite_bwd_kernel(const CompositeBwdParams p) {
   const int S = p.S;
   float* gw_s = sm + static_cast<size_t>(warp) * S;  // g_i * w_i
   const float* d = p.rays_d + static_cast<long long>(ray) * p.rays_d_stride;
-  const float dnorm = sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+  const float dnorm = ray_dnorm(d[0], d[1], d[2]);
   const float* zr = p.z + static_cast<long long>(ray) * S;
   const float* rawr = p.raw + static_cast<long long>(ray) * S * p.C;
   float* outr = p.d_raw + static_cast<long long>(ray) * S * p.C;
@@ -257,11 +257,11 @@ composite_bwd_kernel(const CompositeBwdParams p) {
     float alpha = 0.f, gi = 0.f;
     if (i < S) {
       const float zi = zr[i];
-      const float dist = (i + 1 < S ? zr[i + 1] - zi : 1e10f) * dnorm;
+      const float gap = i + 1 < S ? zr[i + 1] - zi : 1e10f;
       const float* q = rawr + static_cast<long long>(i) * p.C;
       float sigma = q[3];
       if (p.noise) sigma += p.noise[static_cast<long long>(ray) * S + i];
-      alpha = 1.0f - expf(-fmaxf(sigma, 0.f) * dist);
+      alpha = composite_alpha(sigma, gap, dnorm);
       const float r = 1.0f / (1.0f + expf(-q[0])), g = 1.0f / (1.0f + expf(-q[1])), b = 1.0f / (1.0f + expf(-q[2]));
       gi = gr * r + gg * g + gb * b + ga + g_white;
     }

@@ -36,6 +36,19 @@ struct CompositeBwdParams {
   float* d_raw;         // [n][S][C]
 };
 
+// |d| of a ray direction, as compositing scales the sample distances by it (train.py:748)
+__device__ __forceinline__ float ray_dnorm(float dx, float dy, float dz) { return sqrtf(dx * dx + dy * dy + dz * dz); }
+
+// The opacity of a sample (raw2outputs, train.py:740-761): 1 - exp(-relu(sigma) * gap * |d|), where sigma is the raw
+// sigma plus the sample's noise (already scaled by raw_noise_std) when there is noise, and gap = z[i + 1] - z[i], or 1e10
+// for the last sample (:743-748).  composite_kernel and the early-termination pass (occupancy.cu) share it, so the
+// transmittance that decides termination is made of the very alphas compositing uses.  It takes values, not pointers:
+// the loads stay in the callers, which keeps composite_kernel's code as it was.
+__device__ __forceinline__ float composite_alpha(float sigma, float gap, float dnorm) {
+  const float dist = gap * dnorm;
+  return 1.0f - expf(-fmaxf(sigma, 0.f) * dist);
+}
+
 cudaError_t launch_sample_coarse(const float* rays, const float* t_rand, int n, int S, int lindisp, float* z_out,
                                  cudaStream_t st);
 cudaError_t launch_composite(const CompositeParams& p, cudaStream_t st);

@@ -340,6 +340,39 @@ def field_forward_occupancy(rays: torch.Tensor, z_vals: torch.Tensor, latents: O
     return raw, details
 
 
+def field_forward_terminate(rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[torch.Tensor], nerf_pack: torch.Tensor,
+                            bender_pack: Optional[torch.Tensor], out_ch: int, cutoff=None, scaling=None, removal=None,
+                            want_details: bool = False, threshold: float = 0.0, grid=None, noise: Optional[torch.Tensor] = None
+                            ) -> Tuple[torch.Tensor, Dict[str, torch.Tensor], torch.Tensor]:
+    """field_forward (inference) with early ray termination (nrn_field_forward_terminate): the samples run in segments of
+    nrn_termination_segment(), and a ray stops being evaluated after the segment in which its transmittance falls below
+    `threshold`; with `grid` (geometry.OccupancyGrid) a sample is also skipped where the grid would skip it.  noise [N, S]:
+    the sigma noise compositing will add (already scaled), or None.  Returns raw [N, S, out_ch] (field_forward's where
+    evaluated, 0 elsewhere), the details for every sample, and termination_index [N] int32."""
+    if bender_pack is not None and latents is None:
+        raise RuntimeError("nonrigid_nerf_b200: ray bending needs latents")
+    a, raw, details, keep = _field_args(rays, z_vals, None, 1, latents if bender_pack is not None else None, nerf_pack, bender_pack,
+                                        out_ch, (cutoff, scaling, removal), True, want_details)
+    dev = keep[0].device
+    g = grid.c_struct(dev) if grid is not None else None
+    t = _lib.NrnTerminationArgs()
+    t.threshold = float(threshold)
+    if noise is not None:
+        noise = _f32c(noise, "noise")
+        if tuple(noise.shape) != (a.n_rays, a.n_samples):
+            raise RuntimeError(f"nonrigid_nerf_b200: noise must be [{a.n_rays}, {a.n_samples}], got {list(noise.shape)}")
+        t.noise = noise.data_ptr()
+    term = torch.empty(a.n_rays, dtype=torch.int32, device=dev)
+    t.termination_index = term.data_ptr()
+    lib = _lib.load()
+    nbytes = lib.nrn_termination_workspace_bytes(a.n_rays, a.n_samples, out_ch, int(bender_pack is not None))
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.nrn_field_forward_terminate(C.byref(a), C.byref(g) if g is not None else None, C.byref(t), _ptr(ws), nbytes),
+                   "field_forward_terminate")
+    return raw, details, term
+
+
 def field_forward_views(rays: Optional[torch.Tensor], z_vals: Optional[torch.Tensor], points: Optional[torch.Tensor], n_samples: int,
                         latents: Optional[torch.Tensor], viewdirs: Optional[torch.Tensor], nerf_pack: torch.Tensor,
                         bender_pack: Optional[torch.Tensor], views_pack: Optional[torch.Tensor], cutoff=None, scaling=None,

@@ -321,8 +321,9 @@ class training_wrapper_class(torch.nn.Module):
 
 
 class render_wrapper_class(torch.nn.Module):
-    """train.render with the wrapped models; every keyword (held_out, occupancy, ...) is passed on.  An occupancy grid
-    reaches every rank whole: it is not a tensor or a tuple, so RayShardedFunction does not shard it."""
+    """train.render with the wrapped models; every keyword (held_out, occupancy, early_termination, ...) is passed on.  An
+    occupancy grid and an early-termination threshold reach every rank whole: neither is a tensor or a tuple, so
+    RayShardedFunction does not shard them."""
 
     def __init__(self, coarse_model, fine_model=None, ray_bender=None):
         super().__init__()

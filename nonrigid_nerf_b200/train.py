@@ -78,7 +78,7 @@ def raw2outputs(raw, z_vals, rays_d, raw_noise_std=0, white_bkgd=False, pytest=F
 def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False, lindisp=False, perturb=0.0,
                 N_importance=0, network_fine=None, white_bkgd=False, raw_noise_std=0.0,
                 additional_pixel_information=None, detailed_output=False, verbose=False, pytest=False, held_out=None, occupancy=None,
-                **dummy_kwargs):
+                early_termination=None, **dummy_kwargs):
     """Volumetric rendering of a ray batch [N, 8] = (o, d, near, far).  `network_query_fn` is accepted
     for signature compatibility; the field is evaluated by the fused kernel on `network_fn` /
     `network_fine` (which carry their ray bender as `.ray_bender[0]`).
@@ -91,7 +91,17 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     (train.py:1595-1608).  None: the ordinary path.
     occupancy (geometry.OccupancyGrid, under torch.no_grad() only): each pass evaluates the NeRF trunk only on samples
     whose bent point lies in an occupied cell, outside the grid's box, or is not finite; the others get raw = 0.  None:
-    every sample is evaluated."""
+    every sample is evaluated.
+    early_termination (a float t in [0, 1], under torch.no_grad() only; the reference has no such option): each pass
+    evaluates its samples in segments of nrn_termination_segment() consecutive samples, in depth order, and stops
+    evaluating a ray after the segment in which its transmittance T = prod (1 - alpha_i + 1e-10) (compositing's own
+    alphas and noise, fp32, sample by sample) falls below t.  Samples not evaluated get raw = 0; with occupancy as well, a
+    sample is evaluated only when both allow it.  extras["termination_index"] (int32 [N]) is the first sample the last
+    pass skipped because of termination (S when the ray never died), and extras["termination_index0"] the coarse pass's
+    when N_importance > 0.  Per ray |rgb - rgb_full| <= T and |acc - acc_full| <= T (2 T for rgb with white_bkgd) against
+    the render without termination at the same depths, up to rounding, where T is the transmittance at which the ray
+    died; the coarse weights of skipped samples are 0, so the fine depths follow a pdf within t of mass of the full one.
+    t = 0 terminates nothing, nor does a NaN T.  None: every sample is evaluated (no termination_index keys)."""
     if pytest:
         raise RuntimeError("nonrigid_nerf_b200: the pytest= numpy-random hook is not supported")
     if not isinstance(network_fn, NeRF) or (network_fine is not None and not isinstance(network_fine, NeRF)):
@@ -111,8 +121,14 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
         latents = additional_pixel_information["ray_bending_latents"]
     if occupancy is not None:
         _check_occupancy(occupancy, network_fn, network_fine if N_importance > 0 else None, latents)
+    if early_termination is not None:
+        early_termination = _check_termination(early_termination, network_fn, network_fine if N_importance > 0 else None, latents)
+    term_index = {}
 
-    def field(net, z):
+    def field(net, z, noise, key):
+        if early_termination is not None:
+            raw, det, term_index[key] = _ag.field_terminate(net, rays, z, latents, detailed_output, early_termination, occupancy, noise)
+            return raw, det
         if occupancy is None:
             return _ag.field(net, rays, z, latents, detailed_output, viewdirs, held_out)
         return _ag.field_occupancy(net, rays, z, latents, detailed_output, occupancy)
@@ -150,16 +166,17 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     # coarse depths (train.py:847-869); t_rand drawn first, like the reference
     t_rand = draw("t_rand", torch.rand, n, N_samples) if perturb > 0.0 else None
     z_vals = ops.sample_coarse(rays, N_samples, t_rand, lindisp)
-    raw, details = field(network_fn, z_vals)
+    # the noise is drawn before the field call: an early-terminating pass feeds it into its transmittance
     noise = draw("noise_c", torch.randn, n, N_samples) if raw_noise_std > 0.0 else None   # already scaled by raw_noise_std
+    raw, details = field(network_fn, z_vals, noise, "coarse")
 
     if N_importance > 0:
         u = draw("u", torch.rand, n, N_importance) if perturb > 0.0 else None   # det=(perturb == 0), train.py:915
         c0 = _ag.composite(raw, z_vals, rays_d, noise, white_bkgd, N_importance, u)
         z_fine = c0["z_vals_out"]   # sorted union, detached (train.py:918-920)
         run_fn = network_fn if network_fine is None else network_fine
-        raw, fine_details = field(run_fn, z_fine)
         noise_f = draw("noise_f", torch.randn, n, n_fine) if raw_noise_std > 0.0 else None
+        raw, fine_details = field(run_fn, z_fine, noise_f, "fine")
         c1 = _ag.composite(raw, z_fine, rays_d, noise_f, white_bkgd)
     else:
         c0 = None
@@ -187,6 +204,10 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
             ret["surface_rigidity"] = det["rigidity_mask"].reshape(n)
     if retraw:
         ret["raw"] = raw
+    if early_termination is not None:
+        ret["termination_index"] = term_index["fine" if N_importance > 0 else "coarse"]
+        if N_importance > 0:
+            ret["termination_index0"] = term_index["coarse"]
     if N_importance > 0:
         ret["rgb0"], ret["disp0"], ret["acc0"] = c0["rgb_map"], c0["disp_map"], c0["acc_map"]
         ret["z_std"] = c0["z_std"]
@@ -230,6 +251,16 @@ def _check_occupancy(occupancy, network_fn, network_fine, latents):
             _ag.occupancy_check(net, latents, occupancy)
 
 
+def _check_termination(early_termination, network_fn, network_fine, latents) -> float:
+    """Before any launch: render(..., early_termination=t) is refused for what it does not support
+    (_ag.termination_check); returns t as a float."""
+    t = _ag.termination_threshold(early_termination)
+    for net in (network_fn, network_fine):
+        if net is not None:
+            _ag.termination_check(net, latents, t)
+    return t
+
+
 # ---- batchify_rays / render (train.py:108-137, :326-416) --------------------------------------------
 def batchify_rays(rays_flat, additional_pixel_information, chunk=1024 * 32, detailed_output=False, **kwargs):
     """Render rays in chunks (`chunk` only bounds the per-launch working set; results do not depend on it)."""
@@ -248,7 +279,13 @@ def batchify_rays(rays_flat, additional_pixel_information, chunk=1024 * 32, deta
 def render(rays_o, rays_d, chunk=1024 * 32, ndc=True, near=0.0, far=1.0, use_viewdirs=False, c2w_staticcam=None,
            additional_pixel_information=None, detailed_output=False, **kwargs):
     """Render rays.  Returns [rgb_map, disp_map, acc_map, extras] (train.py:326-416).  Keyword held_out [N] (one entry
-    per ray of the flattened batch) and keyword occupancy (a geometry.OccupancyGrid): see render_rays."""
+    per ray of the flattened batch), keyword occupancy (a geometry.OccupancyGrid) and keyword early_termination (a float
+    in [0, 1]): see render_rays."""
+    if kwargs.get("early_termination") is not None:
+        t = _ag.termination_threshold(kwargs["early_termination"])
+        if kwargs.get("network_fn") is not None:
+            _check_termination(t, kwargs["network_fn"], kwargs.get("network_fine") if kwargs.get("N_importance", 0) > 0 else None,
+                               (additional_pixel_information or {}).get("ray_bending_latents"))
     if kwargs.get("network_fn") is not None and kwargs.get("occupancy") is not None:
         _check_occupancy(kwargs["occupancy"], kwargs["network_fn"], kwargs.get("network_fine") if kwargs.get("N_importance", 0) > 0 else None,
                          (additional_pixel_information or {}).get("ray_bending_latents"))
