@@ -698,6 +698,36 @@ size_t nrn_termination_workspace_bytes(int n_rays, int n_samples, int out_ch, in
 int nrn_field_forward_terminate(const NrnFieldArgs* args, const NrnOccupancyGrid* grid /* NULL: none */, const NrnTerminationArgs* term,
                                 void* workspace, size_t workspace_bytes);
 
+/* ---- the inverse of the ray bender: canonical points into every frame (geometry.deform_points) -------------------------
+ * The ray bender maps an observed point x of a frame with latent z to the canonical point c = b(x; z) = x + s r~(x) o(x, z)
+ * (run_nerf_helpers.py:507-584: o the offset MLP on [x, z], r = (tanh(rho(x)) + 1) / 2 the rigidity, r~ = 0 where
+ * r <= rigidity_cutoff (use_cutoff), s = scaling (use_scaling) or 1).  nrn_deform_points solves b(x; z_f) = c for every
+ * canonical point c and every latent z_f: x_0 = c - s r~(c) o(c, z_f), then `iterations` Newton steps
+ * x <- x - J(x)^-1 (b(x) - c), J = I + s (r~ do/dx + o grad(r~)^T).  A point whose |b(x) - c|_2 <= tol is frozen (its
+ * later steps are skipped).  Where J is singular (|det J| <= 1e-6 |J e_0| |J e_1| |J e_2|) or the Newton step is not
+ * finite, the step is the fixed-point one, x <- x - (b(x) - c).  Then residual = |b(x) - c|_2 at the result, converged =
+ * residual <= tol, rigidity = r~(x).  A point or latent with a non-finite value gives NaN out, residual and rigidity and
+ * converged = 0.  b and J are evaluated at fp32 accuracy.  The launch count does not depend on the data, so the call can
+ * be captured in a CUDA graph, and a frame's results do not depend on the other frames of the call.
+ *
+ * NULL args, points, latents, bender_packed or out, negative sizes, latent_stride below 32, iterations outside 1..64,
+ * a NaN, infinite or negative tol, a non-finite scaling or rigidity_cutoff (when used), float arrays not 4-byte aligned
+ * or bender_packed not 16-byte aligned return NRN_E_INVALID before any CUDA call; n_points = 0 or n_latents = 0 returns
+ * NRN_OK and launches nothing. */
+typedef struct NrnDeformArgs {
+  const float* points;  int64_t n_points;                          /* canonical c [P][3] */
+  const float* latents; int32_t n_latents; int64_t latent_stride;  /* [F][32] */
+  const void* bender_packed;                                       /* nrn_pack_bender output, 16-byte aligned */
+  int32_t use_cutoff; float rigidity_cutoff; int32_t use_scaling; float scaling;
+  int32_t iterations; float tol;
+  float* out;            /* [F][P][3] */
+  float* residual;       /* [F][P] or NULL */
+  uint8_t* converged;    /* [F][P] or NULL */
+  float* rigidity;       /* [F][P] r~ at the result, or NULL */
+  void* stream;
+} NrnDeformArgs;
+int nrn_deform_points(const NrnDeformArgs* args);
+
 /* ---- optional per-kernel timing (measurement aid for bench.py) ---------------------------------
  * While enabled, every launch of the kernel kinds below is bracketed by CUDA events recorded on the
  * launch stream.  kinds: 0 field forward, 1 field DGRAD, 2 WGRAD (+reduce), 3 composite(+resample),
@@ -715,7 +745,7 @@ int nrn_field_forward_terminate(const NrnFieldArgs* args, const NrnOccupancyGrid
  * nrn_field_forward_occupancy 32 the bend pass, 33 the lookup and compaction (also nrn_occupancy_compact), 34 the trunk on
  * the kept points and 35 the scatter, and of nrn_field_forward_terminate 36 the bend pass, 37 the lookups and compactions,
  * 38 the trunk on the kept points, 39 the scatters (and the zeroing of raw) and 40 the transmittance updates (and their
- * initialisation).  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * initialisation), 41 nrn_deform_points.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

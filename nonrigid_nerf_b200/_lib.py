@@ -201,6 +201,18 @@ class NrnTerminationArgs(C.Structure):
     _fields_ = [("threshold", C.c_float), ("noise", _vp), ("termination_index", _vp)]
 
 
+class NrnDeformArgs(C.Structure):
+    _fields_ = [
+        ("points", _vp), ("n_points", C.c_int64),
+        ("latents", _vp), ("n_latents", C.c_int32), ("latent_stride", C.c_int64),
+        ("bender_packed", _vp),
+        ("use_cutoff", C.c_int32), ("rigidity_cutoff", C.c_float), ("use_scaling", C.c_int32), ("scaling", C.c_float),
+        ("iterations", C.c_int32), ("tol", C.c_float),
+        ("out", _vp), ("residual", _vp), ("converged", _vp), ("rigidity", _vp),
+        ("stream", _vp),
+    ]
+
+
 # every symbol include/nrnerf_b200.h declares: (restype, argtypes)
 SYMBOLS = {
     "nrn_abi_version": (C.c_int, []),
@@ -295,6 +307,7 @@ SYMBOLS = {
     "nrn_termination_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
     "nrn_field_forward_terminate": (C.c_int, [C.POINTER(NrnFieldArgs), C.POINTER(NrnOccupancyGrid), C.POINTER(NrnTerminationArgs), _vp,
                                               C.c_size_t]),
+    "nrn_deform_points": (C.c_int, [C.POINTER(NrnDeformArgs)]),
     "nrn_timing_enable": (C.c_int, [C.c_int]),
     "nrn_timing_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int), C.c_int]),
 }
@@ -327,6 +340,8 @@ OCCUPANCY_KERNEL_KINDS = ("occupancy_build", "occupancy_bend", "occupancy_compac
 # updates), timing kinds 36 to 40
 TERMINATION_KERNEL_KINDS = ("termination_bend", "termination_compact", "termination_field", "termination_scatter",
                             "termination_transmittance")
+# the inverse of the ray bender (geometry.deform_points), timing kind 41
+DEFORM_KERNEL_KINDS = ("deform",)
 
 
 def timing_enable(on: bool) -> None:
@@ -337,7 +352,7 @@ def timing_read(kinds=KERNEL_KINDS):
     """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True); `kinds` is KERNEL_KINDS,
     KERNEL_KINDS + TC_KERNEL_KINDS, KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS, that + VIEW_TRAIN_KERNEL_KINDS,
     that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS, that + EVAL_KERNEL_KINDS, that + FRAME_IMAGE_KERNEL_KINDS, that + MESH_KERNEL_KINDS, that + LPIPS_KERNEL_KINDS, that + MATCH_KERNEL_KINDS, that
-    + OCCUPANCY_KERNEL_KINDS or that + TERMINATION_KERNEL_KINDS."""
+    + OCCUPANCY_KERNEL_KINDS, that + TERMINATION_KERNEL_KINDS or that + DEFORM_KERNEL_KINDS."""
     n = len(kinds)
     ms = (C.c_double * n)()
     cnt = (C.c_int * n)()

@@ -21,6 +21,7 @@
 #include "lpips.cuh"
 #include "match.cuh"
 #include "occupancy.cuh"
+#include "deform.cuh"
 
 namespace nrn {
 cudaError_t launch_field_fwd(const FieldFwdParams& p, bool has_bender, int num_sms, cudaStream_t stream);
@@ -1595,6 +1596,40 @@ int nrn_field_forward_terminate(const NrnFieldArgs* a, const NrnOccupancyGrid* g
     if (rc) return rc;
   }
   return NRN_OK;
+}
+
+// ---- the inverse of the ray bender ----
+int nrn_deform_points(const NrnDeformArgs* a) {
+  const char* who = "nrn_deform_points";
+  if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
+  if (!a->points || !a->latents || !a->bender_packed || !a->out) return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (a->n_points < 0 || a->n_latents < 0)
+    return fail(NRN_E_INVALID, "%s: negative sizes (n_points %lld, n_latents %d)", who, static_cast<long long>(a->n_points), a->n_latents);
+  if (a->latent_stride < nrn::kLatent) return fail(NRN_E_INVALID, "%s: latent_stride %lld below %d", who, static_cast<long long>(a->latent_stride), nrn::kLatent);
+  if (a->iterations < 1 || a->iterations > nrn::kDeformMaxIterations)
+    return fail(NRN_E_INVALID, "%s: iterations %d outside 1..%d", who, a->iterations, nrn::kDeformMaxIterations);
+  if (!(std::isfinite(a->tol) && a->tol >= 0.f)) return fail(NRN_E_INVALID, "%s: tol %g must be finite and >= 0", who, a->tol);
+  if (a->use_scaling && !std::isfinite(a->scaling)) return fail(NRN_E_INVALID, "%s: scaling %g is not finite", who, a->scaling);
+  if (a->use_cutoff && !std::isfinite(a->rigidity_cutoff))
+    return fail(NRN_E_INVALID, "%s: rigidity_cutoff %g is not finite", who, a->rigidity_cutoff);
+  if (!aligned4(a->points) || !aligned4(a->latents) || !aligned4(a->out) || !aligned4(a->residual) || !aligned4(a->rigidity))
+    return fail(NRN_E_INVALID, "%s: float arrays must be 4-byte aligned", who);
+  if (!aligned16(a->bender_packed)) return fail(NRN_E_INVALID, "%s: bender_packed must be 16-byte aligned", who);
+  if (a->n_points == 0 || a->n_latents == 0) return NRN_OK;
+  DeviceState* ds = nullptr;
+  const int rc = device_state(&ds);
+  if (rc) return rc;
+  const cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  nrn::DeformParams p{};
+  p.points = a->points; p.P = a->n_points;
+  p.latents = a->latents; p.latent_stride = a->latent_stride; p.F = a->n_latents;
+  p.bender = static_cast<const uint8_t*>(a->bender_packed);
+  p.use_cutoff = a->use_cutoff ? 1 : 0; p.cutoff = a->rigidity_cutoff;
+  p.use_scaling = a->use_scaling ? 1 : 0; p.scaling = a->scaling;
+  p.iterations = a->iterations; p.tol = a->tol;
+  p.out = a->out; p.residual = a->residual; p.converged = a->converged; p.rigidity = a->rigidity;
+  p.err = ds->err_word;
+  return timed(41, st, "deform_kernel", [&] { return nrn::launch_deform(p, ds->num_sms, st); });
 }
 
 // Turning timing off only stops recording: a CUDA graph captured while it was on keeps event-record nodes that refer to

@@ -33,132 +33,18 @@
 // CTA: four consumer warpgroups, persistent over tiles; warpgroups 2p and 2p + 1 work on one tile (rows 0-63 / 64-127), so
 // two tiles are in flight per SM.  The weight images and their residuals (104 KB forward, 86 KB backward) are loaded once
 // per CTA by bulk TMA and stay resident, so there is no producer warp and no ring.
-#include "field_mma.cuh"
+#include "resident_mma.cuh"
 #include "div.cuh"
 
 namespace nrn {
 
 namespace {
 
-constexpr int kDivTilesPerCta = 2;                       // tiles in flight per CTA, two warpgroups each
-constexpr int kDivWgs = 2 * kDivTilesPerCta;
-constexpr int kDivThreads = 128 * kDivWgs;
-constexpr int kDivStageLd = 12;                          // floats per staged row: B4 columns 0-7, tau_c at 8
-constexpr int kDivImgBytes = kStHb1.chunks * kChunkBytes;  // widest image of either chain: 96 columns
-constexpr float kLoInv = 1.0f / kBendLoScale;
-
 // resident weights (each with its residual image): B0..B4 (forward); B4^T..B1^T (backward: the probe e is not
 // differentiated)
 constexpr int kDivFwdWBytes = kBendWBytes;
 constexpr int kDivBwdWBytes = dgrad::w_off(dgrad::B0T);
-
-struct DivShared {
-  uint64_t w_full;
-  int abort_flag;
-};
-
-// shared memory: [per tile in flight: A image hi | A image lo] [weights hi | weights lo] [per-row staging] [barrier]
-constexpr size_t div_smem_bytes(int wbytes) {
-  return 2 * kDivTilesPerCta * kDivImgBytes + 2 * wbytes + kDivWgs * kWgRows * kDivStageLd * sizeof(float) + sizeof(DivShared);
-}
-static_assert(div_smem_bytes(kDivFwdWBytes) <= 227 * 1024, "div kernels: shared memory of one CTA per SM");
-
-struct DivSmem {
-  uint8_t* img_hi;   // this warpgroup's tile: fp16 parts (the images stored for WGRAD)
-  uint8_t* img_lo;   //                        scaled residuals
-  uint8_t* w_hi;
-  uint8_t* w_lo;
-  float* stage;      // this warpgroup's 64 rows
-  DivShared* sh;
-};
-__device__ __forceinline__ DivSmem div_smem(uint8_t* smem, int wbytes, int wg) {
-  DivSmem s;
-  s.img_hi = smem + (wg >> 1) * 2 * kDivImgBytes;
-  s.img_lo = s.img_hi + kDivImgBytes;
-  s.w_hi = smem + 2 * kDivTilesPerCta * kDivImgBytes;
-  s.w_lo = s.w_hi + wbytes;
-  float* stage_all = reinterpret_cast<float*>(s.w_lo + wbytes);
-  s.stage = stage_all + wg * kWgRows * kDivStageLd;
-  s.sh = reinterpret_cast<DivShared*>(stage_all + kDivWgs * kWgRows * kDivStageLd);
-  return s;
-}
-
-// one thread starts the bulk copies of the weight images and their residuals; every consumer waits on sh->w_full
-// (phase 0) before its first MMA
-__device__ __forceinline__ void load_resident_weights(const DivSmem& s, const uint8_t* hi, const uint8_t* lo, uint32_t bytes) {
-  if (threadIdx.x == 0) {
-    mbar_init(&s.sh->w_full, 1);
-    s.sh->abort_flag = 0;
-    fence_mbar_init();
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    mbar_arrive_expect_tx(&s.sh->w_full, 2 * bytes);
-    for (uint32_t off = 0; off < bytes; off += 16384u) {
-      tma_bulk_g2s(s.w_hi + off, hi + off, min(bytes - off, 16384u), &s.sh->w_full);
-      tma_bulk_g2s(s.w_lo + off, lo + off, min(bytes - off, 16384u), &s.sh->w_full);
-    }
-  }
-}
-
-// acc[64 x N] = (A_lo . W_hi + A_hi . W_lo) / kBendLoScale + A_hi . W_hi over the k16 steps of 16 columns of bender step S
-// (fwd:: or dgrad::), all operands in shared memory: A = this warpgroup's rows of chunk-major images of kTileM rows (fenced
-// for the async proxy, warpgroup synced), W = the step's resident N-row weight images.  A_LO = false: the A residual is
-// zero (the probe input, whose hi / lo split lives in its columns).  The small terms are summed first, scaled exactly,
-// then the main products added.
-template <auto S, bool A_LO>
-__device__ __forceinline__ void wg_mma_split(Acc<S>& acc, uint32_t a_hi, uint32_t a_lo, const DivSmem& s) {
-  constexpr int N = step(S).N;
-  constexpr uint32_t w0 = w_off(S), k16 = step(S).k16;
-  const uint64_t ahi = gmma_desc(a_hi, kChunkBytes, 128), alo = gmma_desc(a_lo, kChunkBytes, 128);
-  const uint64_t whi = gmma_desc(smem_u32(s.w_hi) + w0, N * 16, 128), wlo = gmma_desc(smem_u32(s.w_lo) + w0, N * 16, 128);
-#pragma unroll
-  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
-  acc_fence(acc);
-  wgmma_fence();
-#pragma unroll 1
-  for (uint32_t k = 0; k < k16; ++k) {
-    if (A_LO) wgmma<N, 0, 0>(acc, gmma_desc_advance(alo, k * 2 * kChunkBytes), gmma_desc_advance(whi, k * 2 * N * 16), 1u);
-    wgmma<N, 0, 0>(acc, gmma_desc_advance(ahi, k * 2 * kChunkBytes), gmma_desc_advance(wlo, k * 2 * N * 16), 1u);
-  }
-  wgmma_commit();
-  wgmma_wait<0>();
-  acc_fence(acc);
-#pragma unroll
-  for (int i = 0; i < N / 2; ++i) acc[i] *= kLoInv;
-  acc_fence(acc);
-  wgmma_fence();
-#pragma unroll 1
-  for (uint32_t k = 0; k < k16; ++k)
-    wgmma<N, 0, 0>(acc, gmma_desc_advance(ahi, k * 2 * kChunkBytes), gmma_desc_advance(whi, k * 2 * N * 16), 1u);
-  wgmma_commit();
-  wgmma_wait<0>();
-  acc_fence(acc);
-}
-
-// fp32 pair -> {fp16 part, scaled fp16 residual}, each packed as fp16x2 (saturating)
-__device__ __forceinline__ uint2 split_h2(float a, float b) {
-  const uint32_t hi = pack_h2_sat(a, b);
-  const float2 h = __half22float2(*reinterpret_cast<const __half2*>(&hi));
-  return make_uint2(hi, pack_h2_sat((a - h.x) * kBendLoScale, (b - h.y) * kBendLoScale));
-}
-
-// Accumulator columns [0, NCOLS) times the primal ReLU mask bits -> this warpgroup's rows (half `h` of the tile) of the
-// next A operand, as fp16 parts (img_hi) and residuals (img_lo)
-template <int NCOLS, int NR>
-__device__ __forceinline__ void epi_mask_split(const float (&acc)[NR], const ReluMask<NCOLS>& m, const DivSmem& s, int h) {
-  const int r0 = h * kWgRows + acc_r0(), q = acc_q();
-#pragma unroll
-  for (int j = 0; j < NCOLS / 8; ++j) {
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const uint2 v = split_h2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-      const int off = j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q;
-      *reinterpret_cast<uint32_t*>(s.img_hi + off) = m.apply(i, j, v.x);
-      *reinterpret_cast<uint32_t*>(s.img_lo + off) = m.apply(i, j, v.y);
-    }
-  }
-}
+static_assert(res_smem_bytes(kDivFwdWBytes) <= 227 * 1024, "div kernels: shared memory of one CTA per SM");
 
 }  // namespace
 
@@ -171,7 +57,7 @@ __device__ __forceinline__ void div_fwd_body(const DivParams& p, float* loss_row
   extern __shared__ __align__(128) uint8_t smem[];
   const int wg = threadIdx.x >> 7;
   const int h = wg & 1;                   // half of the tile: rows [64 h, 64 h + 64)
-  const DivSmem s = div_smem(smem, kDivFwdWBytes, wg);
+  const ResSmem s = res_smem(smem, kDivFwdWBytes, wg);
   load_resident_weights(s, p.bender, p.bender + kBendLoOffset, kDivFwdWBytes);
   const Waiter W{&s.sh->abort_flag, p.err};
 
@@ -182,11 +68,11 @@ __device__ __forceinline__ void div_fwd_body(const DivParams& p, float* loss_row
   const bool wg_leader = tw == 0;
   const int row_off = (h * kWgRows + tw) * 16;
   const uint32_t a_hi = smem_u32(s.img_hi) + h * kWgRows * 16, a_lo = smem_u32(s.img_lo) + h * kWgRows * 16;
-  const float* my_stg = s.stage + tw * kDivStageLd;
+  const float* my_stg = s.stage + tw * kResStageLd;
   const long long n_tiles = (p.P + kTileM - 1) / kTileM;
 
-  for (long long tile = static_cast<long long>(blockIdx.x) * kDivTilesPerCta + (wg >> 1); tile < n_tiles;
-       tile += static_cast<long long>(gridDim.x) * kDivTilesPerCta) {
+  for (long long tile = static_cast<long long>(blockIdx.x) * kResTilesPerCta + (wg >> 1); tile < n_tiles;
+       tile += static_cast<long long>(gridDim.x) * kResTilesPerCta) {
     const long long pt = tile * kTileM + h * kWgRows + tw;
     const bool valid = row_thread && pt < p.P;
     uint8_t* tn = p.tan + tile * kTanTileBytes;
@@ -239,8 +125,8 @@ __device__ __forceinline__ void div_fwd_body(const DivParams& p, float* loss_row
       sw.begin();
       epi_mask_split<kMkHb3.cols>(acc, m, s, h);
       if (acc_q() == 0) {
-        s.stage[acc_r0() * kDivStageLd + 8] = acc[32];
-        s.stage[(acc_r0() + 8) * kDivStageLd + 8] = acc[34];
+        s.stage[acc_r0() * kResStageLd + 8] = acc[32];
+        s.stage[(acc_r0() + 8) * kResStageLd + 8] = acc[34];
       }
       sw.ready(tan_image(kStHb3), s.img_hi);
     }
@@ -258,7 +144,7 @@ __device__ __forceinline__ void div_fwd_body(const DivParams& p, float* loss_row
     {
       Acc<fwd::B4> acc;
       wg_mma_split<fwd::B4, true>(acc, a_hi, a_lo, s);
-      stage_cols<0, 1>(acc, s.stage, kDivStageLd);
+      stage_cols<0, 1>(acc, s.stage, kResStageLd);
       wg_bar(bar);
       if (row_thread) {   // warps 0 and 1 of the warpgroup: 32 consecutive rows each
         const float tau_c = my_stg[8];
@@ -292,8 +178,8 @@ __device__ __forceinline__ void div_fwd_body(const DivParams& p, float* loss_row
   if (wg_leader) tma_bulk_wait<0>();   // all tangent-stash stores complete before the CTA exits
 }
 
-__global__ void __launch_bounds__(kDivThreads, 1) div_fwd_kernel(const DivParams p) { div_fwd_body<false>(p, nullptr); }
-__global__ void __launch_bounds__(kDivThreads, 1) div_fwd_det_kernel(const DivParams p, float* loss_rows) {
+__global__ void __launch_bounds__(kResThreads, 1) div_fwd_kernel(const DivParams p) { div_fwd_body<false>(p, nullptr); }
+__global__ void __launch_bounds__(kResThreads, 1) div_fwd_det_kernel(const DivParams p, float* loss_rows) {
   div_fwd_body<true>(p, loss_rows);
 }
 
@@ -306,7 +192,7 @@ __device__ __forceinline__ void div_bwd_body(const DivParams& p, const uint8_t* 
   extern __shared__ __align__(128) uint8_t smem[];
   const int wg = threadIdx.x >> 7;
   const int h = wg & 1;
-  const DivSmem s = div_smem(smem, kDivBwdWBytes, wg);
+  const ResSmem s = res_smem(smem, kDivBwdWBytes, wg);
   load_resident_weights(s, p.bender + kBendTOffset, p.bender + kBendTLoOffset, kDivBwdWBytes);
   const Waiter W{&s.sh->abort_flag, p.err};
 
@@ -320,8 +206,8 @@ __device__ __forceinline__ void div_bwd_body(const DivParams& p, const uint8_t* 
 
   const float scale = loss_scale(p.amax);   // max|G| is written by div_G_kernel / absmax
 
-  for (long long tile = static_cast<long long>(blockIdx.x) * kDivTilesPerCta + (wg >> 1); tile < n_tiles;
-       tile += static_cast<long long>(gridDim.x) * kDivTilesPerCta) {
+  for (long long tile = static_cast<long long>(blockIdx.x) * kResTilesPerCta + (wg >> 1); tile < n_tiles;
+       tile += static_cast<long long>(gridDim.x) * kResTilesPerCta) {
     const long long pt = tile * kTileM + h * kWgRows + tw;
     const bool valid = row_thread && pt < p.P;
     uint8_t* ad = p.adj + tile * kAdjTileBytes;
@@ -398,8 +284,8 @@ __device__ __forceinline__ void div_bwd_body(const DivParams& p, const uint8_t* 
   if (wg_leader) tma_bulk_wait<0>();   // all adjoint-stash stores complete before the CTA exits
 }
 
-__global__ void __launch_bounds__(kDivThreads, 1) div_bwd_kernel(const DivParams p) { div_bwd_body<false>(p, nullptr); }
-__global__ void __launch_bounds__(kDivThreads, 1) div_bwd_held_kernel(const DivParams p, const uint8_t* held) {
+__global__ void __launch_bounds__(kResThreads, 1) div_bwd_kernel(const DivParams p) { div_bwd_body<false>(p, nullptr); }
+__global__ void __launch_bounds__(kResThreads, 1) div_bwd_held_kernel(const DivParams p, const uint8_t* held) {
   div_bwd_body<true>(p, held);
 }
 
@@ -425,11 +311,11 @@ template <typename Kernel, typename... Extra>
 cudaError_t launch_div(Kernel kernel, int wbytes, const DivParams& p, int num_sms, cudaStream_t st, const Extra&... extra) {
   const long long tiles = (p.P + kTileM - 1) / kTileM;
   if (tiles <= 0) return cudaSuccess;
-  const int smem = static_cast<int>(div_smem_bytes(wbytes));
+  const int smem = static_cast<int>(res_smem_bytes(wbytes));
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) return e;
-  const long long pairs = (tiles + kDivTilesPerCta - 1) / kDivTilesPerCta;
-  kernel<<<static_cast<unsigned>(pairs < num_sms ? pairs : num_sms), kDivThreads, smem, st>>>(p, extra...);
+  const long long pairs = (tiles + kResTilesPerCta - 1) / kResTilesPerCta;
+  kernel<<<static_cast<unsigned>(pairs < num_sms ? pairs : num_sms), kResThreads, smem, st>>>(p, extra...);
   return cudaGetLastError();
 }
 }  // namespace

@@ -383,3 +383,96 @@ def write_obj(path, mesh: Mesh) -> None:
         else:
             np.savetxt(fh, np.concatenate([v.astype(np.float64), col / 255.0], 1), fmt="v %.9g %.9g %.9g %.9g %.9g %.9g")
         np.savetxt(fh, f.astype(np.int64) + 1, fmt="f %d %d %d")
+
+
+# ---- the inverse of the ray bender: canonical points and meshes into frames ----------------------------------------------
+# Defaults of deform_points / deform_mesh (DESIGN.md, "Inverse bending", gives the measured convergence behind them)
+DEFORM_ITERATIONS = 8
+DEFORM_TOL = 1e-5
+
+
+class Deformed(NamedTuple):
+    points: torch.Tensor      # [P, 3] or [F, P, 3] fp32: x with b(x; z) = c
+    residual: torch.Tensor    # [P] or [F, P] fp32: |b(x; z) - c|_2 at x
+    converged: torch.Tensor   # [P] or [F, P] bool: residual <= tol
+    rigidity: torch.Tensor    # [P] or [F, P] fp32: the bender's rigidity r~ at x (after the test-time cutoff)
+
+
+class DeformedMesh(NamedTuple):
+    mesh: Mesh                # the canonical mesh with its vertices moved into the frame, rigidity = r~ at them
+    residual: torch.Tensor    # [V] fp32
+    converged: torch.Tensor   # [V] bool
+
+
+def deform_points(ray_bender, points: torch.Tensor, latents: torch.Tensor, iterations: int = DEFORM_ITERATIONS,
+                  tol: float = DEFORM_TOL) -> Deformed:
+    """Canonical points into frames: for every canonical point c (points [P, 3], CUDA) and every latent code z (latents
+    [32], giving results [P, ...], or [F, 32], giving [F, P, ...]), the observed point x whose bend is c, b(x; z) = c, with
+    b = ray_bender's forward including its test-time knobs (rigidity_test_time_cutoff, test_time_scaling).
+
+    x_0 = c - s r~(c) o(c, z), then `iterations` (1..64) Newton steps on J = db/dx at fp32 accuracy (csrc/deform.cu); a point
+    is frozen once |b(x) - c|_2 <= tol, and where J is singular the step is the fixed-point one.  Points that do not
+    converge (the bending folds, or too few steps) keep their last x and report converged = False with their residual; a
+    non-finite point or latent gives NaN.  The defaults, 8 steps and tol = 1e-5, come from the measured convergence on
+    benders with offsets of 0.01 and 0.1 (DESIGN.md): tol is two orders above the fp32 evaluation error of b on the example
+    volume, and 8 steps leave room over the iterations those benders need.
+
+    Inference only: no autograd node is recorded; with parameters or inputs that require grad the call still runs, on
+    detached values.  Runs on the current stream without host synchronisation (CUDA-graph capturable); a frame's results
+    do not depend on the other frames of the call."""
+    from .run_nerf_helpers import ray_bending
+    if ray_bender is None or not isinstance(ray_bender, ray_bending):
+        raise RuntimeError(f"nonrigid_nerf_b200: deform_points needs the model's ray_bending module, got {type(ray_bender).__name__}")
+    if not isinstance(points, torch.Tensor) or not isinstance(latents, torch.Tensor):
+        raise RuntimeError("nonrigid_nerf_b200: points and latents must be tensors")
+    if points.dim() != 2 or points.shape[1] != 3:
+        raise RuntimeError(f"nonrigid_nerf_b200: points must be [P, 3], got {tuple(points.shape)}")
+    if latents.dim() not in (1, 2) or latents.shape[-1] != ops.LATENT:
+        raise RuntimeError(f"nonrigid_nerf_b200: latents must be [{ops.LATENT}] or [F, {ops.LATENT}], got {tuple(latents.shape)}")
+    if isinstance(iterations, bool) or not isinstance(iterations, (int, np.integer)) or not 1 <= iterations <= 64:
+        raise RuntimeError(f"nonrigid_nerf_b200: iterations must be an int in 1..64, got {iterations!r}")
+    if isinstance(tol, bool) or not isinstance(tol, (int, float, np.floating)) or not np.isfinite(tol) or tol < 0:
+        raise RuntimeError(f"nonrigid_nerf_b200: tol must be a finite float >= 0, got {tol!r}")
+    if not points.is_cuda or not latents.is_cuda:
+        raise RuntimeError("nonrigid_nerf_b200: points and latents must be CUDA tensors (there is no CPU path)")
+    dev = ray_bender.network[0].weight.device
+    if points.device != dev or latents.device != dev:
+        raise RuntimeError(f"nonrigid_nerf_b200: points ({points.device}) and latents ({latents.device}) must be on the bender's "
+                           f"device ({dev})")
+    cutoff = getattr(ray_bender, "rigidity_test_time_cutoff", None)
+    scaling = getattr(ray_bender, "test_time_scaling", None)
+    pts = points.detach().float().contiguous()
+    lat = latents.detach().float().reshape(-1, ops.LATENT).contiguous()
+    F, P = lat.shape[0], pts.shape[0]
+    with torch.cuda.device(dev), torch.no_grad():
+        out = torch.empty(F, P, 3, dtype=torch.float32, device=dev)
+        residual = torch.empty(F, P, dtype=torch.float32, device=dev)
+        converged = torch.empty(F, P, dtype=torch.bool, device=dev)
+        rigidity = torch.empty(F, P, dtype=torch.float32, device=dev)
+        if F > 0 and P > 0:
+            pack = ops.pack_bender(ray_bender)
+            a = _lib.NrnDeformArgs()
+            a.points, a.n_points = pts.data_ptr(), P
+            a.latents, a.n_latents, a.latent_stride = lat.data_ptr(), F, ops.LATENT
+            a.bender_packed = pack.data_ptr()
+            a.use_cutoff, a.rigidity_cutoff = int(cutoff is not None), float(cutoff) if cutoff is not None else 0.0
+            a.use_scaling, a.scaling = int(scaling is not None), float(scaling) if scaling is not None else 1.0
+            a.iterations, a.tol = int(iterations), float(tol)
+            a.out, a.residual, a.converged, a.rigidity = out.data_ptr(), residual.data_ptr(), converged.data_ptr(), rigidity.data_ptr()
+            a.stream = _stream()
+            _lib.check(_lib.load().nrn_deform_points(C.byref(a)), "deform_points")
+    if latents.dim() == 1:
+        return Deformed(out[0], residual[0], converged[0], rigidity[0])
+    return Deformed(out, residual, converged, rigidity)
+
+
+def deform_mesh(ray_bender, mesh: Mesh, latent: torch.Tensor, iterations: int = DEFORM_ITERATIONS,
+                tol: float = DEFORM_TOL) -> DeformedMesh:
+    """The canonical mesh moved into the frame of `latent` ([32]): its vertices through deform_points, so every frame's
+    mesh has the canonical faces and vertex order (one topology across the sequence).  faces, vertex_offsets, face_offsets
+    and colors are the canonical mesh's (a canonical point's colour does not depend on the frame); rigidity is r~ at the
+    moved vertices.  Vertices that did not converge keep their last iterate; `converged` tells them apart."""
+    if latent is None or not isinstance(latent, torch.Tensor) or latent.dim() != 1:
+        raise RuntimeError(f"nonrigid_nerf_b200: deform_mesh needs one latent code [{ops.LATENT}]")
+    d = deform_points(ray_bender, mesh.vertices, latent, iterations, tol)
+    return DeformedMesh(mesh._replace(vertices=d.points, rigidity=d.rigidity), d.residual, d.converged)
