@@ -728,6 +728,42 @@ typedef struct NrnDeformArgs {
 } NrnDeformArgs;
 int nrn_deform_points(const NrnDeformArgs* args);
 
+/* ---- surface normals: the density gradient at points (geometry.density_gradient) -------------------------------------
+ * grad[i] = d raw[i][3] / d x_i of NeRF.forward in point mode: the density before its ReLU, through the ray bender when
+ * bender_packed is given (bent = x + r~ o (* s), with the test-time knobs use_cutoff / use_scaling, and raw[3] -- so its
+ * gradient -- zeroed where r~ >= removal_threshold when use_removal), through the trunk alone otherwise.  The
+ * time-conditioned baseline passes its fp32 nn.Linear weights tc_w0 [256][95], tc_b0, tc_w5 [256][351], tc_b5 (all four
+ * or none; no bender), which fold each point's latent into L0 / L5 biases.  A view-dependent model passes its trunk
+ * image (alpha in head row 3): the density needs only the trunk and the bender.
+ * Points run in chunks of nrn_density_gradient_chunk() points; per chunk one forward kernel writes the ReLU mask bits, the
+ * positional encoding and the bender's offsets and rigidity into the workspace, and one DGRAD kernel with d raw = e_3
+ * (loss scale 2^9) writes grad.  The workspace holds one chunk, so its size is bounded independently of n_points.
+ * Workspace layout for n = min(n_points, chunk) points in T = ceil(n / 128) rounded up to even tiles, each piece on a
+ * 256-byte boundary: ReLU mask bits [T][40960] (the training layout), the positional encoding E [T][16384] (the training
+ * stash's first image), unmasked offsets [n][3] fp32, rigidity [n] fp32, time-conditioned ray biases.  After the call it
+ * holds the last chunk's.  No
+ * host synchronisation: the call can be captured in a CUDA graph.  A non-finite point gives a non-finite gradient.
+ *
+ * NULL args, points, grad or nerf_packed, n_points < 0, points_stride < 3, latent_stride neither 0 nor >= 32, a bender
+ * or time-conditioned weights without latents, latents with neither, a bender with time-conditioned weights, only some of
+ * the four time-conditioned weights, a non-finite knob in use, float arrays not 4-byte aligned, packed weights or the
+ * workspace not 16-byte aligned, or workspace_bytes below nrn_density_gradient_workspace_bytes(n_points, latents per
+ * point of a time-conditioned call) return NRN_E_INVALID before any CUDA call; n_points = 0 launches nothing. */
+typedef struct NrnDensityGradArgs {
+  const float* points; int64_t n_points; int64_t points_stride;   /* [P][points_stride], xyz first */
+  const float* latents; int64_t latent_stride;                    /* [P][latent_stride] (0: one row for every point) or NULL */
+  const void* nerf_packed;                                        /* nrn_pack_nerf output */
+  const void* bender_packed;                                      /* nrn_pack_bender output, or NULL */
+  const float* tc_w0; const float* tc_b0; const float* tc_w5; const float* tc_b5;   /* time-conditioned baseline, or NULL */
+  int32_t use_cutoff; float rigidity_cutoff; int32_t use_scaling; float scaling; int32_t use_removal; float removal_threshold;
+  float* grad;                                                    /* [P][3] out */
+  void* workspace; size_t workspace_bytes;
+  void* stream;
+} NrnDensityGradArgs;
+int64_t nrn_density_gradient_chunk(void);
+size_t nrn_density_gradient_workspace_bytes(int64_t n_points, int per_point_ray_bias);
+int nrn_field_density_gradient(const NrnDensityGradArgs* args);
+
 /* ---- optional per-kernel timing (measurement aid for bench.py) ---------------------------------
  * While enabled, every launch of the kernel kinds below is bracketed by CUDA events recorded on the
  * launch stream.  kinds: 0 field forward, 1 field DGRAD, 2 WGRAD (+reduce), 3 composite(+resample),
@@ -745,7 +781,8 @@ int nrn_deform_points(const NrnDeformArgs* args);
  * nrn_field_forward_occupancy 32 the bend pass, 33 the lookup and compaction (also nrn_occupancy_compact), 34 the trunk on
  * the kept points and 35 the scatter, and of nrn_field_forward_terminate 36 the bend pass, 37 the lookups and compactions,
  * 38 the trunk on the kept points, 39 the scatters (and the zeroing of raw) and 40 the transmittance updates (and their
- * initialisation), 41 nrn_deform_points.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * initialisation), 41 nrn_deform_points, and of nrn_field_density_gradient 42 the forward (with the time-conditioned
+ * biases) and 43 the DGRAD.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

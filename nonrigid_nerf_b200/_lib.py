@@ -213,6 +213,19 @@ class NrnDeformArgs(C.Structure):
     ]
 
 
+class NrnDensityGradArgs(C.Structure):
+    _fields_ = [
+        ("points", _vp), ("n_points", C.c_int64), ("points_stride", C.c_int64),
+        ("latents", _vp), ("latent_stride", C.c_int64),
+        ("nerf_packed", _vp), ("bender_packed", _vp),
+        ("tc_w0", _vp), ("tc_b0", _vp), ("tc_w5", _vp), ("tc_b5", _vp),
+        ("use_cutoff", C.c_int32), ("rigidity_cutoff", C.c_float), ("use_scaling", C.c_int32), ("scaling", C.c_float),
+        ("use_removal", C.c_int32), ("removal_threshold", C.c_float),
+        ("grad", _vp), ("workspace", _vp), ("workspace_bytes", C.c_size_t),
+        ("stream", _vp),
+    ]
+
+
 # every symbol include/nrnerf_b200.h declares: (restype, argtypes)
 SYMBOLS = {
     "nrn_abi_version": (C.c_int, []),
@@ -308,6 +321,9 @@ SYMBOLS = {
     "nrn_field_forward_terminate": (C.c_int, [C.POINTER(NrnFieldArgs), C.POINTER(NrnOccupancyGrid), C.POINTER(NrnTerminationArgs), _vp,
                                               C.c_size_t]),
     "nrn_deform_points": (C.c_int, [C.POINTER(NrnDeformArgs)]),
+    "nrn_density_gradient_chunk": (C.c_int64, []),
+    "nrn_density_gradient_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "nrn_field_density_gradient": (C.c_int, [C.POINTER(NrnDensityGradArgs)]),
     "nrn_timing_enable": (C.c_int, [C.c_int]),
     "nrn_timing_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int), C.c_int]),
 }
@@ -342,6 +358,8 @@ TERMINATION_KERNEL_KINDS = ("termination_bend", "termination_compact", "terminat
                             "termination_transmittance")
 # the inverse of the ray bender (geometry.deform_points), timing kind 41
 DEFORM_KERNEL_KINDS = ("deform",)
+# the density gradient (geometry.density_gradient: point-gradient forward, its DGRAD), timing kinds 42 and 43
+NORMAL_KERNEL_KINDS = ("density_grad_fwd", "density_grad_dgrad")
 
 
 def timing_enable(on: bool) -> None:
@@ -352,7 +370,7 @@ def timing_read(kinds=KERNEL_KINDS):
     """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True); `kinds` is KERNEL_KINDS,
     KERNEL_KINDS + TC_KERNEL_KINDS, KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS, that + VIEW_TRAIN_KERNEL_KINDS,
     that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS, that + EVAL_KERNEL_KINDS, that + FRAME_IMAGE_KERNEL_KINDS, that + MESH_KERNEL_KINDS, that + LPIPS_KERNEL_KINDS, that + MATCH_KERNEL_KINDS, that
-    + OCCUPANCY_KERNEL_KINDS, that + TERMINATION_KERNEL_KINDS or that + DEFORM_KERNEL_KINDS."""
+    + OCCUPANCY_KERNEL_KINDS, that + TERMINATION_KERNEL_KINDS, that + DEFORM_KERNEL_KINDS or that + NORMAL_KERNEL_KINDS."""
     n = len(kinds)
     ms = (C.c_double * n)()
     cnt = (C.c_int * n)()

@@ -37,6 +37,8 @@ cudaError_t launch_field_views(const FieldFwdParams& p, const ViewParams& v, int
 cudaError_t launch_field_views_train(const FieldFwdParams& p, const ViewParams& v, const ViewTrainParams& t, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_bwd_views(const FieldBwdParams& p, const ViewBwdParams& v, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_fwd_kept(const FieldFwdParams& p, const int* kept, int num_sms, cudaStream_t stream);
+cudaError_t launch_field_fwd_grad(const FieldFwdParams& p, bool has_bender, int num_sms, cudaStream_t stream);
+cudaError_t launch_field_bwd_grad(const FieldBwdParams& p, const PointGradParams& pg, bool has_bender, int num_sms, cudaStream_t stream);
 }
 
 namespace {
@@ -1630,6 +1632,113 @@ int nrn_deform_points(const NrnDeformArgs* a) {
   p.out = a->out; p.residual = a->residual; p.converged = a->converged; p.rigidity = a->rigidity;
   p.err = ds->err_word;
   return timed(41, st, "deform_kernel", [&] { return nrn::launch_deform(p, ds->num_sms, st); });
+}
+
+// ---- the density gradient ----
+namespace {
+// Points per launch pair: 512 tiles, about four waves of persistent CTAs on 132 SMs
+constexpr long long kGradChunk = 1LL << 16;
+// Workspace of one chunk of n points (256-byte aligned pieces): ReLU masks, E, unmasked offsets [n][3], rigidity [n], and
+// the time-conditioned ray biases ([n][2][256] with latents per point, else one row)
+struct GradWorkspace {
+  size_t mask, e, unmasked, rigidity, ray_bias, total;
+};
+GradWorkspace grad_workspace(long long n_points, bool per_point_ray_bias) {
+  const long long n = std::min(std::max(n_points, 0LL), kGradChunk);
+  const long long tiles = (tile_count(n) + 1) & ~1LL;
+  auto up = [](size_t b) { return (b + 255) / 256 * 256; };
+  GradWorkspace w;
+  w.mask = 0;
+  w.e = w.mask + up(static_cast<size_t>(tiles) * nrn::kMaskTileBytes);
+  w.unmasked = w.e + up(static_cast<size_t>(tiles) * nrn::kEBytes);
+  w.rigidity = w.unmasked + up(static_cast<size_t>(n) * 3 * sizeof(float));
+  w.ray_bias = w.rigidity + up(static_cast<size_t>(n) * sizeof(float));
+  w.total = w.ray_bias + up(static_cast<size_t>(per_point_ray_bias ? n : 1) * 2 * 256 * sizeof(float));
+  return w;
+}
+bool knob_ok(int use, float v) { return !use || std::isfinite(v); }
+}  // namespace
+
+int64_t nrn_density_gradient_chunk(void) { return kGradChunk; }
+
+size_t nrn_density_gradient_workspace_bytes(int64_t n_points, int per_point_ray_bias) {
+  return n_points < 0 ? 0 : grad_workspace(n_points, per_point_ray_bias != 0).total;
+}
+
+int nrn_field_density_gradient(const NrnDensityGradArgs* a) {
+  const char* who = "nrn_field_density_gradient";
+  if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
+  if (!a->points || !a->grad || !a->nerf_packed) return fail(NRN_E_INVALID, "%s: null argument (points, grad or nerf_packed)", who);
+  if (a->n_points < 0) return fail(NRN_E_INVALID, "%s: n_points %lld < 0", who, static_cast<long long>(a->n_points));
+  if (a->points_stride < 3) return fail(NRN_E_INVALID, "%s: points_stride %lld below 3", who, static_cast<long long>(a->points_stride));
+  const int n_tc = (a->tc_w0 != nullptr) + (a->tc_b0 != nullptr) + (a->tc_w5 != nullptr) + (a->tc_b5 != nullptr);
+  if (n_tc != 0 && n_tc != 4) return fail(NRN_E_INVALID, "%s: the time-conditioned baseline needs all of tc_w0, tc_b0, tc_w5, tc_b5", who);
+  const bool tc = n_tc == 4, bender = a->bender_packed != nullptr;
+  if (tc && bender) return fail(NRN_E_INVALID, "%s: the time-conditioned baseline has no bender (bender_packed must be NULL)", who);
+  if ((tc || bender) != (a->latents != nullptr))
+    return fail(NRN_E_INVALID, "%s: latents are needed exactly with a bender or the time-conditioned weights", who);
+  if (a->latents && a->latent_stride != 0 && a->latent_stride < nrn::kLatent)
+    return fail(NRN_E_INVALID, "%s: latent_stride %lld must be 0 or at least %d", who, static_cast<long long>(a->latent_stride), nrn::kLatent);
+  if (!knob_ok(a->use_cutoff, a->rigidity_cutoff) || !knob_ok(a->use_scaling, a->scaling) || !knob_ok(a->use_removal, a->removal_threshold))
+    return fail(NRN_E_INVALID, "%s: a test-time knob in use (rigidity_cutoff, scaling, removal_threshold) is not finite", who);
+  if (!aligned4(a->points) || !aligned4(a->latents) || !aligned4(a->grad) || !aligned4(a->tc_w0) || !aligned4(a->tc_b0) ||
+      !aligned4(a->tc_w5) || !aligned4(a->tc_b5))
+    return fail(NRN_E_INVALID, "%s: float arrays must be 4-byte aligned", who);
+  if (!aligned16(a->nerf_packed) || (bender && !aligned16(a->bender_packed)) || !aligned16(a->workspace))
+    return fail(NRN_E_INVALID, "%s: packed weights and the workspace must be 16-byte aligned", who);
+  const bool per_point_bias = tc && a->latent_stride != 0;
+  const GradWorkspace w = grad_workspace(a->n_points, per_point_bias);
+  if (a->n_points == 0) return NRN_OK;
+  if (!a->workspace || a->workspace_bytes < w.total)
+    return fail(NRN_E_INVALID, "%s: workspace of %zu bytes, %zu needed (nrn_density_gradient_workspace_bytes)", who, a->workspace_bytes, w.total);
+  DeviceState* ds = nullptr;
+  int rc = device_state(&ds);
+  if (rc) return rc;
+  const cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  uint8_t* ws = static_cast<uint8_t*>(a->workspace);
+  float* unmasked = reinterpret_cast<float*>(ws + w.unmasked);
+  float* rigidity = reinterpret_cast<float*>(ws + w.rigidity);
+  float* ray_bias = reinterpret_cast<float*>(ws + w.ray_bias);
+  const uint8_t* np = static_cast<const uint8_t*>(a->nerf_packed);
+  const uint8_t* bp = static_cast<const uint8_t*>(a->bender_packed);
+  for (long long c0 = 0; c0 < a->n_points; c0 += kGradChunk) {
+    const long long n = std::min(kGradChunk, static_cast<long long>(a->n_points) - c0);
+    const int tiles = static_cast<int>(tile_count(n));
+    nrn::FieldFwdParams p{};
+    p.pts = a->points + c0 * a->points_stride; p.pts_stride = a->points_stride;
+    if (a->latents) { p.latents = a->latents + c0 * a->latent_stride; p.latent_stride = a->latent_stride; }
+    p.n_rays = static_cast<int>(n); p.S = 1; p.P = n; p.n_tiles = tiles;
+    p.nerf_w = np; p.nerf_bias = reinterpret_cast<const float*>(np + nrn::kNerfWBytes);
+    if (bender) { p.bend_w = bp; p.bend_bias = reinterpret_cast<const float*>(bp + nrn::kBendWBytes); }
+    p.cutoff = a->rigidity_cutoff; p.use_cutoff = a->use_cutoff;
+    p.scaling = a->scaling; p.use_scaling = a->use_scaling;
+    p.out_ch = 4;
+    if (bender) { p.d_unmasked = unmasked; p.d_rigid = rigidity; }
+    p.stash = ws + w.e; p.relu_mask = ws + w.mask;
+    p.err = ds->err_word;
+    if (tc) { p.ray_bias = ray_bias; p.ray_bias_stride = per_point_bias ? 2 * 256 : 0; }
+    rc = timed(42, st, "field_fwd_grad_kernel", [&] {
+      if (tc) {
+        const cudaError_t e = nrn::launch_tc_latent_bias(p.latents, a->latent_stride, per_point_bias ? p.n_rays : 1, a->tc_w0, a->tc_b0,
+                                                         a->tc_w5, a->tc_b5, ray_bias, st);
+        if (e != cudaSuccess) return e;
+      }
+      return nrn::launch_field_fwd_grad(p, bender, ds->num_sms, st);
+    });
+    if (rc) return rc;
+    nrn::FieldBwdParams q{};
+    q.P = n; q.n_tiles = tiles; q.S = 1; q.n_rays = static_cast<int>(n); q.out_ch = 4;
+    q.stash = ws + w.e; q.relu_mask = ws + w.mask;
+    q.nerf_wT = np + nrn::kNerfTOffset;
+    if (bender) { q.bend_wT = bp + nrn::kBendTOffset; q.unmasked = unmasked; q.rigidity = rigidity; }
+    q.cutoff = a->rigidity_cutoff; q.use_cutoff = a->use_cutoff; q.scaling = a->scaling; q.use_scaling = a->use_scaling;
+    q.err = ds->err_word;
+    nrn::PointGradParams pg{};
+    pg.grad = a->grad + c0 * 3; pg.removal = a->removal_threshold; pg.use_removal = bender && a->use_removal;
+    rc = timed(43, st, "field_bwd_grad_kernel", [&] { return nrn::launch_field_bwd_grad(q, pg, bender, ds->num_sms, st); });
+    if (rc) return rc;
+  }
+  return NRN_OK;
 }
 
 // Turning timing off only stops recording: a CUDA graph captured while it was on keeps event-record nodes that refer to

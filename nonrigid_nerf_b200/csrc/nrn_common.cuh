@@ -273,6 +273,14 @@ struct FieldBwdParams {
   const uint8_t* relu_mask;    // ReLU masks of the forward call [n_tiles even][kMaskTileBytes]
 };
 
+// The point gradient d raw[3] / d x (field_bwd_grad_kernel), next to a FieldBwdParams: grad [P][3] out; the test-time
+// object removal zeroes raw[3], and so the gradient, where rigidity >= removal (use_removal)
+struct PointGradParams {
+  float* grad;
+  float removal;
+  int use_removal;
+};
+
 // ------------------------------------------------------------------------------------------
 // Kernel parameter blocks
 // ------------------------------------------------------------------------------------------

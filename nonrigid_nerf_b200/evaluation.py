@@ -313,3 +313,22 @@ def lpips(gt: torch.Tensor, generated: torch.Tensor, weights: LpipsWeights, mask
             a.stream = _stream().value
             _lib.check(lib.nrn_lpips(C.byref(a)), "lpips")
     return (out, layers) if per_layer else out
+
+
+def normal_images(normals: torch.Tensor, c2w: torch.Tensor) -> torch.Tensor:
+    """uint8 [F, H, W, 3] images of world-space unit normals [F, H, W, 3] (render(..., surface_normals=True)) seen from the
+    cameras c2w [F, 3, 4+] (camera-to-world, get_rays convention: x right, y up, z toward the viewer).  Per pixel, in
+    fp32 with every operation rounded on its own: c_k = (R[0][k] n_0 + R[1][k] n_1) + R[2][k] n_2 (R = c2w[:, :3, :3], so
+    c = R^T n), v = (c + 1) * 0.5, out = to8b(v) = uint8(trunc(255 * clip(v, 0, 1))); a zero normal (no surface) gives 0."""
+    normals = _frames(normals, "normals", 4)
+    if normals.shape[-1] != 3:
+        raise RuntimeError(f"nonrigid_nerf_b200: normals must be [F, H, W, 3], got {tuple(normals.shape)}")
+    if not isinstance(c2w, torch.Tensor) or c2w.dim() != 3 or c2w.shape[0] != normals.shape[0] or c2w.shape[1] < 3 or c2w.shape[2] < 3:
+        raise RuntimeError(f"nonrigid_nerf_b200: c2w must be [F, 3, 4] for {normals.shape[0]} frames")
+    r = c2w[:, :3, :3].to(device=normals.device, dtype=torch.float32)[:, None, None]   # [F, 1, 1, 3, 3]
+    n = normals
+    c = [(r[..., 0, k] * n[..., 0] + r[..., 1, k] * n[..., 1]) + r[..., 2, k] * n[..., 2] for k in range(3)]
+    v = (torch.stack(c, -1) + 1.0) * 0.5
+    out = (255.0 * v.clamp(0.0, 1.0)).to(torch.uint8)
+    zero = (n == 0).all(-1, keepdim=True)
+    return torch.where(zero, torch.zeros_like(out), out)

@@ -345,12 +345,27 @@ def _host(mesh: Mesh):
     return v, f, col, rig
 
 
-def write_ply(path, mesh: Mesh) -> None:
-    """Binary little-endian PLY: float x, y, z (+ uchar red, green, blue when the mesh has colours, + float rigidity when
-    it has rigidity) per vertex, and an int vertex_indices list of 3 per face."""
+def _host_normals(normals, n_vertices: int):
+    if normals is None:
+        return None
+    nrm = normals.detach().cpu().numpy() if isinstance(normals, torch.Tensor) else np.asarray(normals)
+    nrm = nrm.astype("<f4", copy=False).reshape(-1, 3)
+    if nrm.shape[0] != n_vertices:
+        raise RuntimeError(f"nonrigid_nerf_b200: normals must be [{n_vertices}, 3], got {tuple(nrm.shape)}")
+    return nrm
+
+
+def write_ply(path, mesh: Mesh, normals=None) -> None:
+    """Binary little-endian PLY: float x, y, z (+ float nx, ny, nz when `normals` [V, 3] are given, + uchar red, green,
+    blue when the mesh has colours, + float rigidity when it has rigidity) per vertex, and an int vertex_indices list of 3
+    per face."""
     v, f, col, rig = _host(mesh)
+    nrm = _host_normals(normals, len(v))
     fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
     props = ["property float x", "property float y", "property float z"]
+    if nrm is not None:
+        fields += [("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4")]
+        props += ["property float nx", "property float ny", "property float nz"]
     if col is not None:
         fields += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
         props += ["property uchar red", "property uchar green", "property uchar blue"]
@@ -359,6 +374,8 @@ def write_ply(path, mesh: Mesh) -> None:
         props.append("property float rigidity")
     vert = np.empty(len(v), dtype=fields)
     vert["x"], vert["y"], vert["z"] = v[:, 0], v[:, 1], v[:, 2]
+    if nrm is not None:
+        vert["nx"], vert["ny"], vert["nz"] = nrm[:, 0], nrm[:, 1], nrm[:, 2]
     if col is not None:
         vert["red"], vert["green"], vert["blue"] = col[:, 0], col[:, 1], col[:, 2]
     if rig is not None:
@@ -373,16 +390,23 @@ def write_ply(path, mesh: Mesh) -> None:
         fh.write(face.tobytes())
 
 
-def write_obj(path, mesh: Mesh) -> None:
-    """Wavefront OBJ: 'v x y z' per vertex (+ ' r g b' in [0, 1] when the mesh has colours, c / 255), 'f a b c' per face
-    (1-based).  Coordinates are written with 9 significant digits, which restore the fp32 values exactly."""
+def write_obj(path, mesh: Mesh, normals=None) -> None:
+    """Wavefront OBJ: 'v x y z' per vertex (+ ' r g b' in [0, 1] when the mesh has colours, c / 255), then, when `normals`
+    [V, 3] are given, 'vn nx ny nz' per vertex, and 'f a b c' per face (1-based; 'f a//a b//b c//c' with normals, vertex
+    i using normal i).  Numbers are written with 9 significant digits, which restore the fp32 values exactly."""
     v, f, col, _ = _host(mesh)
+    nrm = _host_normals(normals, len(v))
     with open(path, "w") as fh:
         if col is None:
             np.savetxt(fh, v, fmt="v %.9g %.9g %.9g")
         else:
             np.savetxt(fh, np.concatenate([v.astype(np.float64), col / 255.0], 1), fmt="v %.9g %.9g %.9g %.9g %.9g %.9g")
-        np.savetxt(fh, f.astype(np.int64) + 1, fmt="f %d %d %d")
+        if nrm is None:
+            np.savetxt(fh, f.astype(np.int64) + 1, fmt="f %d %d %d")
+        else:
+            np.savetxt(fh, nrm, fmt="vn %.9g %.9g %.9g")
+            fi = np.repeat(f.astype(np.int64) + 1, 2, axis=1)
+            np.savetxt(fh, fi, fmt="f %d//%d %d//%d %d//%d")
 
 
 # ---- the inverse of the ray bender: canonical points and meshes into frames ----------------------------------------------
@@ -476,3 +500,103 @@ def deform_mesh(ray_bender, mesh: Mesh, latent: torch.Tensor, iterations: int = 
         raise RuntimeError(f"nonrigid_nerf_b200: deform_mesh needs one latent code [{ops.LATENT}]")
     d = deform_points(ray_bender, mesh.vertices, latent, iterations, tol)
     return DeformedMesh(mesh._replace(vertices=d.points, rigidity=d.rigidity), d.residual, d.converged)
+
+
+# ---- surface normals: the density gradient through the fused DGRAD chain (csrc/field_bwd.cu) -------------------------------
+def _grad_latents(network_fn, latent, n: int, dev):
+    """(latent rows [n or 1, 32] fp32, row stride) for the density gradient, after the refusals of _PointField."""
+    tc = _ag._tc_net(network_fn)
+    bender = network_fn.ray_bender[0]
+    if tc is not None and latent is None:
+        raise RuntimeError("nonrigid_nerf_b200: a time_conditioned_baseline model needs the latent code of a frame")
+    if tc is None and bender is None and latent is not None:
+        raise RuntimeError("nonrigid_nerf_b200: a latent code was given, but the model has no ray bender")
+    if latent is None:
+        return None, 0
+    lat = torch.as_tensor(latent).detach().to(device=dev, dtype=torch.float32)
+    if lat.dim() == 1 and lat.numel() == ops.LATENT:
+        return lat.reshape(1, ops.LATENT).contiguous(), 0
+    if lat.dim() == 2 and lat.shape == (n, ops.LATENT):
+        return lat.contiguous(), ops.LATENT
+    raise RuntimeError(f"nonrigid_nerf_b200: the latent code must be [{ops.LATENT}] or [P, {ops.LATENT}], got {tuple(lat.shape)}")
+
+
+def density_gradient(network_fn, points: torch.Tensor, latent=None) -> torch.Tensor:
+    """g [P, 3] fp32 = d raw[..., 3] / d x of NeRF.forward in point mode at points [P, 3] (CUDA): the gradient of the
+    density before its ReLU, so points just outside the surface have one too.  With a ray bender and a latent code ([32]
+    for every point, or [P, 32]) the gradient passes through the bend, bent = x + rigidity * unmasked (* scaling): the
+    frame's world space.  With no latent, or no bender, it is the canonical one.  The test-time knobs apply as in point
+    mode (rigidity cutoff, scaling, object removal, which zeroes g where it zeroes raw[..., 3]).  The time-conditioned
+    baseline needs its latent; a view-dependent model's density is its trunk's alpha.
+
+    One forward and one DGRAD kernel per chunk of nrn_density_gradient_chunk() points, on the current stream without host
+    synchronisation (CUDA-graph capturable); the workspace is one chunk's (DESIGN.md gives its size).  Inference only: no
+    autograd node is recorded.  A non-finite point gives a non-finite g."""
+    return _density_gradient(network_fn, points, latent)
+
+
+def _density_gradient(network_fn, points: torch.Tensor, latent=None, workspace: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """density_gradient; `workspace` (uint8, at least nrn_density_gradient_workspace_bytes) replaces the call's own, so
+    that a test can read back the last chunk's mask bits, encoding, offsets and rigidity (layout in nrnerf_b200.h)."""
+    if not isinstance(points, torch.Tensor) or points.dim() != 2 or points.shape[1] != 3:
+        raise RuntimeError(f"nonrigid_nerf_b200: points must be a [P, 3] tensor, got {getattr(points, 'shape', type(points))}")
+    dev = network_fn.pts_linears[0].weight.device
+    if dev.type != "cuda" or not points.is_cuda:
+        raise RuntimeError("nonrigid_nerf_b200: the model and the points must be on a CUDA device (there is no CPU path)")
+    if points.device != dev:
+        raise RuntimeError(f"nonrigid_nerf_b200: points ({points.device}) must be on the model's device ({dev})")
+    P = points.shape[0]
+    lat, stride = _grad_latents(network_fn, latent, P, dev)
+    tc = _ag._tc_net(network_fn)
+    bent = network_fn.ray_bender[0] is not None and lat is not None
+    cutoff, scaling, removal = _ag._knobs(network_fn) if bent else (None, None, None)
+    pts = points.detach().float().contiguous()
+    lib = _lib.load()
+    with torch.cuda.device(dev), torch.no_grad():
+        grad = torch.empty(P, 3, dtype=torch.float32, device=dev)
+        if P == 0:
+            return grad
+        nerf_pack = ops.pack_nerf(network_fn)
+        bender_pack = ops.pack_bender(network_fn.ray_bender[0]) if bent else None
+        nbytes = int(lib.nrn_density_gradient_workspace_bytes(P, int(tc is not None and stride != 0)))
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev) if workspace is None else workspace
+        nbytes = ws.numel()
+        a = _lib.NrnDensityGradArgs()
+        a.points, a.n_points, a.points_stride = pts.data_ptr(), P, 3
+        if lat is not None:
+            a.latents, a.latent_stride = lat.data_ptr(), stride
+        a.nerf_packed = nerf_pack.data_ptr()
+        if bender_pack is not None:
+            a.bender_packed = bender_pack.data_ptr()
+        if tc is not None:
+            tw = [tc.pts_linears[0].weight, tc.pts_linears[0].bias, tc.pts_linears[5].weight, tc.pts_linears[5].bias]
+            for t in tw:
+                if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
+                    raise RuntimeError("nonrigid_nerf_b200: NeRF parameters must be contiguous fp32 CUDA tensors")
+            a.tc_w0, a.tc_b0, a.tc_w5, a.tc_b5 = (t.data_ptr() for t in tw)
+        if cutoff is not None:
+            a.use_cutoff, a.rigidity_cutoff = 1, float(cutoff)
+        if scaling is not None:
+            a.use_scaling, a.scaling = 1, float(scaling)
+        if removal is not None:
+            a.use_removal, a.removal_threshold = 1, float(removal)
+        a.grad, a.workspace, a.workspace_bytes = grad.data_ptr(), ws.data_ptr(), nbytes
+        a.stream = _stream()
+        _lib.check(lib.nrn_field_density_gradient(C.byref(a)), "field_density_gradient")
+    return grad
+
+
+def normals_from_gradient(g: torch.Tensor) -> torch.Tensor:
+    """Unit normals n = -g / |g| (out of the occupied region, like the mesh's face normals); n = 0 where |g| = 0 or g is
+    not finite.  |g| = sqrt(gx^2 + gy^2 + gz^2) in fp32, n = -g / |g| elementwise."""
+    gx, gy, gz = g[..., 0], g[..., 1], g[..., 2]
+    norm = torch.sqrt(gx * gx + gy * gy + gz * gz)
+    ok = torch.isfinite(norm) & (norm > 0)
+    n = -g / torch.where(ok, norm, torch.ones_like(norm))[..., None]
+    return torch.where(ok[..., None], n, torch.zeros_like(n))
+
+
+def vertex_normals(network_fn, mesh: Mesh, latent=None) -> torch.Tensor:
+    """Unit normals [V, 3] at the mesh's vertices: normals_from_gradient(density_gradient(network_fn, mesh.vertices,
+    latent)).  Pass the latent the mesh was built with (extract_mesh's, or deform_mesh's for a frame's mesh)."""
+    return normals_from_gradient(density_gradient(network_fn, mesh.vertices, latent))

@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 from . import autograd as _ag
-from . import ops
+from . import geometry, ops
 from .run_nerf_helpers import NeRF, img2mse, mse2psnr  # noqa: F401  (same star-import surface)
 
 DEBUG = False  # reference: train.py:24 (NaN/Inf scan of every output when True)
@@ -101,7 +101,11 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     when N_importance > 0.  Per ray |rgb - rgb_full| <= T and |acc - acc_full| <= T (2 T for rgb with white_bkgd) against
     the render without termination at the same depths, up to rounding, where T is the transmittance at which the ray
     died; the coarse weights of skipped samples are 0, so the fine depths follow a pdf within t of mass of the full one.
-    t = 0 terminates nothing, nor does a NaN T.  None: every sample is evaluated (no termination_index keys)."""
+    t = 0 terminates nothing, nor does a NaN T.  None: every sample is evaluated (no termination_index keys).
+    surface_normals=True (with surface_output=True) adds ret["surface_normals"] [N, 3]: the world-space unit normal
+    geometry.normals_from_gradient(geometry.density_gradient(...)) of the pass's model, with the ray's latent code, at
+    the frame-space point of the median-visibility sample (the point surface_pts and surface_rigidity are taken at).
+    No other output changes.  Default False."""
     if pytest:
         raise RuntimeError("nonrigid_nerf_b200: the pytest= numpy-random hook is not supported")
     if not isinstance(network_fn, NeRF) or (network_fine is not None and not isinstance(network_fine, NeRF)):
@@ -198,6 +202,9 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
                 _, det = _ag.field_views(run_fn, None, None, pts, latents, None, True, bend_only=True)
             else:                                     # no bender: the point itself
                 det = {"input_pts": pts}
+            if dummy_kwargs.get("surface_normals", False):
+                # world-space unit normals of the frame's density at the median sample's frame-space point
+                ret["surface_normals"] = geometry.normals_from_gradient(geometry.density_gradient(run_fn, pts, latents))
         ret["median_indices"] = idx
         ret["surface_pts"] = det["input_pts"].reshape(n, 3)
         if "rigidity_mask" in det:
