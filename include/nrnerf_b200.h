@@ -548,6 +548,8 @@ int nrn_mesh_cube_table(int32_t* counts, int8_t* edges);
  * its pixels of sum_c w_k[c] (f_gt[c] / (|f_gt| + 1e-10) - f_gen[c] / (|f_gen| + 1e-10))^2; LPIPS is the sum of the five.
  * The convolutions run on fp16 operands with fp32 accumulation, activations are stored in fp16, the distances are fp32
  * per pixel and fp64 per frame, summed in a fixed order: a frame's score does not depend on the batch or chunk it is in.
+ * A convolution output above 65504 (the largest fp16) cannot be stored: a frame either of whose images has one scores
+ * NaN, and so do its tap scores from that convolution's tap on (no synchronisation; the call stays graph-capturable).
  *
  * nrn_lpips_pack: the packed weight block (nrn_lpips_packed_bytes(), 16-byte aligned, device) from 17 device fp32 arrays:
  *   tensors[2 l], tensors[2 l + 1]  conv weight (OIHW) and bias of layer l = 0..4 (net.slice1.0, net.slice2.3,
@@ -557,8 +559,8 @@ int nrn_mesh_cube_table(int32_t* counts, int8_t* edges);
  * Once per weight set; the sources may be freed after the stream has run the pack.
  * nrn_lpips_workspace_bytes(F, H, W): the workspace nrn_lpips uses for F frames of H x W by default: the derived mask,
  *   ceil(H * W / 256) * 256 bytes, plus min(F, max(1, 256 MiB / B), 4096) frames of B bytes each, B the activations of
- *   both images of a frame at every stage (fp16 NHWC) and its distance partials.  nrn_lpips_workspace_bytes(1, H, W) -
- *   nrn_lpips_workspace_bytes(0, H, W) is B.  0 for sizes out of range.
+ *   both images of a frame at every stage (fp16 NHWC), its distance partials and saturation words.
+ *   nrn_lpips_workspace_bytes(1, H, W) - nrn_lpips_workspace_bytes(0, H, W) is B.  0 for sizes out of range.
  * nrn_lpips: lpips [F] and, when per_layer is not NULL, the tap scores per_layer [F][5].  Frames go in chunks of
  *   (workspace_bytes - mask bytes) / B frames (at most 4096).  NULL args or pointers, negative sizes, H or W below 31 (the
  *   smallest frame every tap has a pixel of) or above 16384, float arrays not 4-byte aligned, packed weights not 16-byte

@@ -1251,6 +1251,8 @@ int nrn_lpips(const NrnLpipsArgs* a) {
   for (int f0 = 0; f0 < F; f0 += static_cast<int>(fc_max)) {
     const int fc = F - f0 < static_cast<int>(fc_max) ? F - f0 : static_cast<int>(fc_max);
     const nrn::LpipsChunk c = nrn::lpips_chunk(a->workspace, fc, H, W);
+    const cudaError_t ze = cudaMemsetAsync(c.sat, 0, 2 * static_cast<size_t>(fc) * sizeof(unsigned), st);
+    if (ze != cudaSuccess) return cuda_fail(ze, "lpips saturation words");
     rc = timed(25, st, "lpips_input_kernel", [&] {
       return nrn::launch_lpips_input(a->gt + f0 * frame_floats, a->generated + f0 * frame_floats, mask, packed, fc, H, W, c.act[0], st);
     });
@@ -1263,7 +1265,7 @@ int nrn_lpips(const NrnLpipsArgs* a) {
         });
       if (!rc)
         rc = timed(26, st, "lpips_conv_kernel", [&] {
-          return nrn::launch_lpips_conv(l, d, c.act[l == 0 ? 0 : si - 1], c.act[si], packed, 2 * fc, ds->num_sms, ds->err_word, st);
+          return nrn::launch_lpips_conv(l, d, c.act[l == 0 ? 0 : si - 1], c.act[si], packed, 2 * fc, ds->num_sms, ds->err_word, c.sat, st);
         });
       if (!rc) rc = timed(28, st, "lpips_distance_kernel", [&] { return nrn::launch_lpips_distance(l, d, c, packed, st); });
     }

@@ -7,7 +7,9 @@
 // ring of the field kernels (field_mma.cuh).  Each consumer thread gathers, per slab, four 16-byte chunks of its pixel's
 // receptive field (8 input channels of one tap; zeros outside the image and past K) with cp.async into a 4-stage A ring of
 // its warpgroup, two slabs ahead of the MMAs.  The epilogue adds the bias, applies ReLU and stores fp16 NHWC with a
-// saturating convert.  Nothing is split across images or along K, so an image's features do not depend on its batch.
+// saturating convert; a value above 65504 (the largest fp16) sets bit L of its image's saturation word, and the reduce
+// kernel scores such a frame NaN from that tap on.  Nothing is split across images or along K, so an image's features do
+// not depend on its batch.
 #include "field_mma.cuh"
 #include "lpips.cuh"
 
@@ -54,6 +56,7 @@ struct ConvParams {
   int hin, win, hout, wout;
   int tiles_per_image, n_items;
   int* err;
+  unsigned* sat;           // [images] saturation words: bit L set when layer L clamped an output of the image
 };
 
 template <int L>
@@ -147,10 +150,11 @@ __global__ void __launch_bounds__(kFwdThreads, 1) lpips_conv_kernel(ConvParams p
     if (lane == 0) mbar_arrive(&ring.empty[prev]);
     cp_async_wait<0>();
 
-    // epilogue: bias, ReLU, fp16 (saturating) NHWC
+    // epilogue: bias, ReLU, fp16 (saturating) NHWC; the largest value before the convert flags a clamped output
     const int r0 = acc_r0(), q = acc_q();
     const float* bias = p.bias + half * N;
     __half* out = p.out + static_cast<size_t>(img) * hw * S.cout + half * N;
+    float vmax = 0.f;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const int px = pix0 + r0 + 8 * i;
@@ -159,9 +163,12 @@ __global__ void __launch_bounds__(kFwdThreads, 1) lpips_conv_kernel(ConvParams p
 #pragma unroll
       for (int j = 0; j < N / 8; ++j) {
         const int col = 8 * j + 2 * q;
-        o[col / 2] = pack_h2_relu_sat(acc[4 * j + 2 * i] + __ldg(bias + col), acc[4 * j + 2 * i + 1] + __ldg(bias + col + 1));
+        const float a = acc[4 * j + 2 * i] + __ldg(bias + col), b = acc[4 * j + 2 * i + 1] + __ldg(bias + col + 1);
+        vmax = fmaxf(vmax, fmaxf(a, b));
+        o[col / 2] = pack_h2_relu_sat(a, b);
       }
     }
+    if (__any_sync(0xffffffffu, vmax > kLpipsHalfMax) && lane == 0) atomicOr(p.sat + img, 1u << L);
   }
 }
 
@@ -297,17 +304,20 @@ struct TapCounts {
   double px[kLpipsTaps];
 };
 
-// per frame: the tap means (block partials in block order, fp64) and their sum in tap order
-__global__ void lpips_reduce_kernel(const double* __restrict__ partials, int fc, int stride, TapCounts tc, float* __restrict__ lpips,
-                                    float* __restrict__ per_layer) {
+// per frame: the tap means (block partials in block order, fp64) and their sum in tap order; NaN from the first tap
+// whose convolution clamped an output of either image of the frame on
+__global__ void lpips_reduce_kernel(const double* __restrict__ partials, const unsigned* __restrict__ sat, int fc, int stride,
+                                    TapCounts tc, float* __restrict__ lpips, float* __restrict__ per_layer) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= fc) return;
+  const unsigned clamped = sat[f] | sat[fc + f];
+  const int first = clamped ? __ffs(static_cast<int>(clamped)) - 1 : kLpipsTaps;
   double total = 0.0;
   for (int k = 0; k < kLpipsTaps; ++k) {
     const double* p = partials + (static_cast<size_t>(k) * fc + f) * stride;
     double s = 0.0;
     for (int b = 0; b < tc.blocks[k]; ++b) s += p[b];
-    const double mean = s / tc.px[k];
+    const double mean = k < first ? s / tc.px[k] : __longlong_as_double(0x7ff8000000000000LL);
     if (per_layer) per_layer[f * kLpipsTaps + k] = static_cast<float>(mean);
     total += mean;
   }
@@ -316,7 +326,7 @@ __global__ void lpips_reduce_kernel(const double* __restrict__ partials, int fc,
 
 template <int L>
 cudaError_t launch_conv_layer(const LpipsDims& d, const __half* in, __half* out, const uint8_t* packed, int n_images, int num_sms,
-                              int* err, cudaStream_t st) {
+                              int* err, unsigned* sat, cudaStream_t st) {
   constexpr LpipsConv S = kLpipsConv[L];
   constexpr int kInStage[kLpipsTaps] = {0, 2, 4, 5, 6};
   const int so = kInStage[L], si = kLpipsTapStage[L];
@@ -330,6 +340,7 @@ cudaError_t launch_conv_layer(const LpipsDims& d, const __half* in, __half* out,
   const long long items = static_cast<long long>(n_images) * p.tiles_per_image * S.split;
   p.n_items = static_cast<int>(items);
   p.err = err;
+  p.sat = sat;
   if (items <= 0) return cudaSuccess;
   const cudaError_t e = cudaFuncSetAttribute(lpips_conv_kernel<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, kLpConvSmem);
   if (e != cudaSuccess) return e;
@@ -367,7 +378,7 @@ size_t lpips_frame_bytes(int H, int W) {
   const LpipsDims d = lpips_dims(H, W);
   size_t b = 0;
   for (int s = 0; s < kLpipsStages; ++s) b += align256(2 * static_cast<size_t>(d.image_bytes(s)));
-  return b + align256(static_cast<size_t>(kLpipsTaps) * max_dist_blocks(d) * sizeof(double));
+  return b + align256(static_cast<size_t>(kLpipsTaps) * max_dist_blocks(d) * sizeof(double) + 2 * sizeof(unsigned));
 }
 
 LpipsChunk lpips_chunk(void* ws, int fc, int H, int W) {
@@ -381,6 +392,7 @@ LpipsChunk lpips_chunk(void* ws, int fc, int H, int W) {
     p += align256(2 * static_cast<size_t>(fc) * d.image_bytes(s));
   }
   c.partials = reinterpret_cast<double*>(p);
+  c.sat = reinterpret_cast<unsigned*>(c.partials + static_cast<size_t>(kLpipsTaps) * fc * c.max_blocks);
   return c;
 }
 
@@ -409,13 +421,13 @@ cudaError_t launch_lpips_input(const float* gt, const float* gen, const uint8_t*
 }
 
 cudaError_t launch_lpips_conv(int layer, const LpipsDims& d, const __half* in, __half* out, const uint8_t* packed, int n_images,
-                              int num_sms, int* err, cudaStream_t st) {
+                              int num_sms, int* err, unsigned* sat, cudaStream_t st) {
   switch (layer) {
-    case 0: return launch_conv_layer<0>(d, in, out, packed, n_images, num_sms, err, st);
-    case 1: return launch_conv_layer<1>(d, in, out, packed, n_images, num_sms, err, st);
-    case 2: return launch_conv_layer<2>(d, in, out, packed, n_images, num_sms, err, st);
-    case 3: return launch_conv_layer<3>(d, in, out, packed, n_images, num_sms, err, st);
-    default: return launch_conv_layer<4>(d, in, out, packed, n_images, num_sms, err, st);
+    case 0: return launch_conv_layer<0>(d, in, out, packed, n_images, num_sms, err, sat, st);
+    case 1: return launch_conv_layer<1>(d, in, out, packed, n_images, num_sms, err, sat, st);
+    case 2: return launch_conv_layer<2>(d, in, out, packed, n_images, num_sms, err, sat, st);
+    case 3: return launch_conv_layer<3>(d, in, out, packed, n_images, num_sms, err, sat, st);
+    default: return launch_conv_layer<4>(d, in, out, packed, n_images, num_sms, err, sat, st);
   }
 }
 
@@ -448,7 +460,7 @@ cudaError_t launch_lpips_reduce(const LpipsDims& d, const LpipsChunk& c, float* 
     tc.blocks[k] = d.dist_blocks(k);
     tc.px[k] = static_cast<double>(d.px(kLpipsTapStage[k]));
   }
-  lpips_reduce_kernel<<<blocks_of(c.fc, 128), 128, 0, st>>>(c.partials, c.fc, c.max_blocks, tc, lpips, per_layer);
+  lpips_reduce_kernel<<<blocks_of(c.fc, 128), 128, 0, st>>>(c.partials, c.sat, c.fc, c.max_blocks, tc, lpips, per_layer);
   return cudaGetLastError();
 }
 

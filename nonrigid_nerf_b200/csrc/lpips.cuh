@@ -7,9 +7,11 @@
 //
 // Workspace of one call (nrn_lpips_workspace_bytes): the derived mask (H * W bytes, rounded up to 256), then frames in
 // chunks of Fc.  A chunk of Fc frames holds its 2 Fc images (ground truth first, then renders) at every stage, each stage
-// one 256-byte aligned buffer, then the distance partials [5][Fc][max blocks] fp64.  lpips_frame_bytes(H, W) bounds one
-// frame's share of that, so a workspace of mask + Fc * lpips_frame_bytes(H, W) bytes holds a chunk of Fc frames.  The
-// default chunk is as many frames as fit kLpipsChunkBudget (at least one, at most the call's frames and kLpipsMaxChunk).
+// one 256-byte aligned buffer, then the distance partials [5][Fc][max blocks] fp64 and right after them the saturation
+// words [2 Fc] u32 (bit l: conv l + 1 clamped an output of the image above 65504; zeroed per chunk).
+// lpips_frame_bytes(H, W) bounds one frame's share of that, so a workspace of mask + Fc * lpips_frame_bytes(H, W) bytes
+// holds a chunk of Fc frames.  The default chunk is as many frames as fit kLpipsChunkBudget (at least one, at most the
+// call's frames and kLpipsMaxChunk).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -24,6 +26,7 @@ constexpr int kLpipsMaxSide = 16384;
 constexpr size_t kLpipsChunkBudget = 256ull << 20;      // default bytes of one chunk's activations
 constexpr int kLpipsMaxChunk = 4096;                    // frames per chunk at most (the distance grid's y extent)
 constexpr int kLpipsSlabChunks = 8;                     // K columns per weight slab / A stage: 8 chunks of 8 channels
+constexpr float kLpipsHalfMax = 65504.f;                // the largest fp16: a convolution output above it is clamped
 
 // One convolution as the kernels run it: cin is the channel count of its NHWC input (conv1: 3 padded to 8), cin_real
 // that of the weight tensor; the output channels go in `split` launches-worth of N = cout / split columns.
@@ -72,6 +75,7 @@ struct LpipsChunk {
   int fc;                          // frames; images 0..fc-1 ground truth, fc..2fc-1 renders
   __half* act[kLpipsStages];       // [2 fc][h][w][channels]
   double* partials;                // [5][fc][max dist blocks]
+  unsigned* sat;                   // [2 fc] saturation words, after the partials
   int max_blocks;
 };
 LpipsChunk lpips_chunk(void* ws, int fc, int H, int W);
@@ -87,7 +91,7 @@ cudaError_t launch_lpips_pack(const LpipsPackSources& s, uint8_t* packed, cudaSt
 cudaError_t launch_lpips_input(const float* gt, const float* gen, const uint8_t* mask, const uint8_t* packed, int fc, int H, int W,
                                __half* out, cudaStream_t st);
 cudaError_t launch_lpips_conv(int layer, const LpipsDims& d, const __half* in, __half* out, const uint8_t* packed, int n_images,
-                              int num_sms, int* err, cudaStream_t st);
+                              int num_sms, int* err, unsigned* sat, cudaStream_t st);
 cudaError_t launch_lpips_pool(const __half* in, __half* out, int n_images, int hin, int win, int hout, int wout, int channels,
                               cudaStream_t st);
 cudaError_t launch_lpips_distance(int tap, const LpipsDims& d, const LpipsChunk& c, const uint8_t* packed, cudaStream_t st);

@@ -272,7 +272,10 @@ def lpips(gt: torch.Tensor, generated: torch.Tensor, weights: LpipsWeights, mask
     free_viewpoint_rendering.py:836-849 scores them: [F] fp32, or ([F], [F, 5] tap scores) with per_layer=True.  mask
     [H, W] (nonzero = pixel zeroed in both images) defaults to the pixels of gt[0] whose channels sum to 0, as in
     image_scores.  H and W must be at least 31.  Frames go through the network in chunks of chunk_frames (default: as
-    many as fit 256 MiB of activations); a frame's score does not depend on the chunk or batch it is in."""
+    many as fit 256 MiB of activations); a frame's score does not depend on the chunk or batch it is in.
+    Activations are stored in fp16.  A convolution output above 65504 (the largest fp16 value) would be clamped and
+    give a finite but wrong score, so a frame with such an output in either image scores NaN instead, and so do its tap
+    scores from that convolution's tap on; the earlier taps stay finite.  There is no higher-precision path."""
     if not isinstance(weights, LpipsWeights):
         raise RuntimeError("nonrigid_nerf_b200: weights must come from evaluation.lpips_weights()")
     gt = _frames(gt, "gt", 4)

@@ -34,6 +34,19 @@ def random_state_dict(seed: int, lin_scale: float = 1.0) -> dict:
     return sd
 
 
+def he_state_dict(seed: int, gain: float) -> dict:
+    """random_state_dict(seed) with every convolution replaced by He-normal weights (std sqrt(2 / fan_in), which keeps the
+    activations' second moment from layer to layer through ReLU) and biases uniform in +-0.1, both times `gain` per
+    layer, so that activations grow or shrink by about gain per layer: an activation scale set by the weights, as
+    trained weights set it."""
+    sd = random_state_dict(seed)
+    g = torch.Generator().manual_seed(1000 + seed)
+    for key, cout, cin, k, _, _ in CONVS:
+        sd[key + ".weight"] = torch.randn((cout, cin, k, k), generator=g) * (2.0 / (cin * k * k)) ** 0.5 * gain
+        sd[key + ".bias"] = (torch.rand((cout,), generator=g) * 0.2 - 0.1) * gain
+    return sd
+
+
 def taps(x: torch.Tensor, sd: dict) -> list:
     """The five ReLU outputs of the AlexNet features of x [N, 3, H, W] (already scaled), in fp64."""
     out = []

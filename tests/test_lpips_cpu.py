@@ -130,7 +130,7 @@ def test_packed_and_workspace_sizes():
         chans = (8, 64, 64, 192, 192, 384, 256, 256)
         b = sum(a256(2 * hh * ww * c * 2) for (hh, ww), c in zip(dims, chans))
         blocks = max((dims[s][0] * dims[s][1] + 255) // 256 for s in (1, 3, 5, 6, 7))
-        return b + a256(5 * blocks * 8)
+        return b + a256(5 * blocks * 8 + 2 * 4)   # the distance partials, then the two images' saturation words
 
     for h, w in ((378, 504), (756, 1008), (31, 31), (37, 53)):
         fb = frame_bytes(h, w)
