@@ -5,6 +5,7 @@ import torch
 from torch.func import grad, vmap
 
 import oracle.nrnerf_oracle as O
+from tests.parity import half_ulp
 
 
 def _t(p, fp16, device):
@@ -112,6 +113,8 @@ def fixed_mask_chain(npar, bp, masks, E, unmasked=None, rigidity=None, cutoff=No
     P = E.shape[0]
     m = {k: v.double() for k, v in masks.items()}
     E = E.double()
+    if eps is not None and "E" in eps:
+        E = E + eps["E"]
     in_ch = W[0].shape[1]
     w3 = npar["out_w"][3].expand(P, -1)
     dY = st("Y7", w3 * m["H8"], w3.abs() * m["H8"])
@@ -149,14 +152,25 @@ def fixed_mask_chain(npar, bp, masks, E, unmasked=None, rigidity=None, cutoff=No
     return g
 
 
-def rounding_bound(npar, bp, masks, E, unmasked=None, rigidity=None, **knobs):
+# The encoding E's sin / cos (columns 3..62) as pe_backward reads them: fp16 of the fp32 MUFU value, within half an fp16
+# ulp plus E_PE of the exact sin / cos of the fp32 point (stage_reference.check_forward's PE bound)
+E_PE = 1e-6
+
+
+def rounding_bound(npar, bp, masks, E, unmasked=None, rigidity=None, e_term=False, **knobs):
     """(g64, bound, sigma) [P, 3]: sigma is the standard deviation of the same first-order error when each rounding is an
     independent uniform error of at most U16 relative (variance U16^2 y^2 / 3), the scale of a typical error; fixed_mask_chain and, per component, the first-order effect of the kernels' roundings,
     sum over stages s and elements j of |d g_i / d y_sj| (U16 |y_sj| + ACC |y_prev| |W|_sj), with the derivatives of the
-    chain's own (signed) linear map, taken by autograd through additive perturbations at every stage."""
+    chain's own (signed) linear map, taken by autograd through additive perturbations at every stage.  e_term: the bound
+    also carries the stashed encoding's own error, sum_j |d g_i / d E_j| (half_ulp(E_j) + E_PE) over the sin / cos
+    columns, for a comparison against a chain fed the exact encoding."""
     cap = {}
     g = fixed_mask_chain(npar, bp, masks, E, unmasked, rigidity, capture=cap, **knobs)
     eps = {k: torch.zeros_like(y, requires_grad=True) for k, (y, _) in cap.items()}
+    if e_term:
+        E = E.double()
+        eps["E"] = torch.zeros_like(E, requires_grad=True)
+        cap["E"] = (E, None)
     with torch.enable_grad():
         gp = fixed_mask_chain(npar, bp, masks, E, unmasked, rigidity, eps=eps, **knobs)
         bound, var = torch.zeros_like(g), torch.zeros_like(g)
@@ -167,6 +181,9 @@ def rounding_bound(npar, bp, masks, E, unmasked=None, rigidity=None, **knobs):
                 if J is None:
                     continue
                 y, mag = cap[k]
+                if k == "E":
+                    bound[:, i] += (J[:, 3:63].abs() * (half_ulp(y[:, 3:63]) + E_PE)).sum(1)
+                    continue
                 J = J if J.dim() == y.dim() else J[:, None]
                 yy, mm = (y, mag) if y.dim() == 2 else (y[:, None], mag[:, None])
                 bound[:, i] += (J.abs() * (U16 * yy.abs() + ACC * mm)).sum(1)
