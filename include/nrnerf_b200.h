@@ -583,6 +583,27 @@ int nrn_lpips_pack(const float* const* tensors, void* packed, void* stream);
 size_t nrn_lpips_workspace_bytes(int n_frames, int height, int width);
 int nrn_lpips(const NrnLpipsArgs* args);
 
+/* Spatial LPIPS maps: what lpips.LPIPS(net='alex', spatial=True) returns (retPerLayer=True for the per-tap maps), which
+ * free_viewpoint_rendering.py does not compute.  Per frame of H x W and tap l with per-pixel distances d_l [h_l][w_l]
+ * (the values nrn_lpips averages): up_l = F.interpolate(d_l, size=(H, W), mode="bilinear", align_corners=False), in
+ * fp32 with each operation rounded on its own (scale = (float)h_l / H, src = max(scale (y + 0.5) - 0.5, 0), i0 = (int)src,
+ * i1 = i0 + (i0 < h_l - 1), l1 = src - i0, l0 = 1 - l1, the same along x, v = hl0 (wl0 x00 + wl1 x01) + hl1 (wl0 x10 +
+ * wl1 x11)), and map = (((up_0 + up_1) + up_2) + up_3) + up_4.  The mask zeroes pixels before the network as in nrn_lpips;
+ * the map covers every pixel.  A frame whose convolution l clamped an output gets NaN in up_l, in every later tap's map
+ * and in map; its earlier taps' maps stay finite.  lpips and per_layer are those of nrn_lpips, bit for bit, and a frame's
+ * maps do not depend on its chunk.
+ * nrn_lpips_maps_workspace_bytes(F, H, W): nrn_lpips's layout with frames of B' bytes, B' = B plus the five fp32 tap
+ *   maps of the frame (each rounded up to 256 bytes); chunks of min(F, max(1, 256 MiB / B'), 4096) frames by default.
+ * nrn_lpips_maps: everything nrn_lpips checks, with chunks of (workspace_bytes - mask bytes) / B' frames, plus a NULL
+ *   maps (always) or maps->map (n_frames > 0) and float outputs not 4-byte aligned: NRN_E_INVALID before any CUDA call. */
+typedef struct NrnLpipsMapArgs {
+  float* map;                 /* out [F][H][W], required */
+  float* layer_maps;          /* out [F][5][H][W] per-tap maps, or NULL */
+  uint8_t* error_image;       /* out [F][H][W][3] to8b(jet(clip(map, 0, 1))) (NaN: jet index 0), or NULL */
+} NrnLpipsMapArgs;
+size_t nrn_lpips_maps_workspace_bytes(int n_frames, int height, int width);
+int nrn_lpips_maps(const NrnLpipsArgs* args, const NrnLpipsMapArgs* maps);
+
 /* ---- correspondences between rendered frames (correspondence.py) ------------------------------
  * render(..., surface_output=True) gives every pixel its canonical surface point (train.py:159-176: the median-visibility
  * sample mapped back through the ray bender); free_viewpoint_rendering.py:615-645 only paints those points as a
@@ -784,7 +805,8 @@ int nrn_field_density_gradient(const NrnDensityGradArgs* args);
  * the kept points and 35 the scatter, and of nrn_field_forward_terminate 36 the bend pass, 37 the lookups and compactions,
  * 38 the trunk on the kept points, 39 the scatters (and the zeroing of raw) and 40 the transmittance updates (and their
  * initialisation), 41 nrn_deform_points, and of nrn_field_density_gradient 42 the forward (with the time-conditioned
- * biases) and 43 the DGRAD.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * biases) and 43 the DGRAD, 44 the upsampling of nrn_lpips_maps (its other kernels are kinds 25 to 28, the distances
+ * with their tap maps kind 28).  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

@@ -179,6 +179,10 @@ class NrnLpipsArgs(C.Structure):
     ]
 
 
+class NrnLpipsMapArgs(C.Structure):
+    _fields_ = [("map", _vp), ("layer_maps", _vp), ("error_image", _vp)]
+
+
 class NrnMatchArgs(C.Structure):
     _fields_ = [
         ("query", _vp), ("target", _vp), ("query_mask", _vp), ("target_mask", _vp),
@@ -307,6 +311,8 @@ SYMBOLS = {
     "nrn_lpips_pack": (C.c_int, [C.POINTER(_vp), _vp, _vp]),
     "nrn_lpips_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     "nrn_lpips": (C.c_int, [C.POINTER(NrnLpipsArgs)]),
+    "nrn_lpips_maps_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "nrn_lpips_maps": (C.c_int, [C.POINTER(NrnLpipsArgs), C.POINTER(NrnLpipsMapArgs)]),
     "nrn_match_workspace_bytes": (C.c_size_t, [C.c_int] * 7),
     "nrn_match": (C.c_int, [C.POINTER(NrnMatchArgs)]),
     "nrn_occupancy_words": (C.c_size_t, [C.c_int] * 3),
@@ -360,6 +366,9 @@ TERMINATION_KERNEL_KINDS = ("termination_bend", "termination_compact", "terminat
 DEFORM_KERNEL_KINDS = ("deform",)
 # the density gradient (geometry.density_gradient: point-gradient forward, its DGRAD), timing kinds 42 and 43
 NORMAL_KERNEL_KINDS = ("density_grad_fwd", "density_grad_dgrad")
+# spatial LPIPS maps (evaluation.lpips_maps: the upsampling of the tap maps into per-pixel maps and error images), timing
+# kind 44; the rest of the call is timed as LPIPS_KERNEL_KINDS
+LPIPS_MAP_KERNEL_KINDS = ("lpips_upsample",)
 
 
 def timing_enable(on: bool) -> None:
@@ -370,7 +379,8 @@ def timing_read(kinds=KERNEL_KINDS):
     """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True); `kinds` is KERNEL_KINDS,
     KERNEL_KINDS + TC_KERNEL_KINDS, KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS, that + VIEW_TRAIN_KERNEL_KINDS,
     that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS, that + EVAL_KERNEL_KINDS, that + FRAME_IMAGE_KERNEL_KINDS, that + MESH_KERNEL_KINDS, that + LPIPS_KERNEL_KINDS, that + MATCH_KERNEL_KINDS, that
-    + OCCUPANCY_KERNEL_KINDS, that + TERMINATION_KERNEL_KINDS, that + DEFORM_KERNEL_KINDS or that + NORMAL_KERNEL_KINDS."""
+    + OCCUPANCY_KERNEL_KINDS, that + TERMINATION_KERNEL_KINDS, that + DEFORM_KERNEL_KINDS, that + NORMAL_KERNEL_KINDS or
+    that + LPIPS_MAP_KERNEL_KINDS."""
     n = len(kinds)
     ms = (C.c_double * n)()
     cnt = (C.c_int * n)()

@@ -1210,17 +1210,27 @@ static bool lpips_size_ok(int H, int W) {
   return H >= nrn::kLpipsMinSide && W >= nrn::kLpipsMinSide && H <= nrn::kLpipsMaxSide && W <= nrn::kLpipsMaxSide;
 }
 
-size_t nrn_lpips_workspace_bytes(int n_frames, int height, int width) {
+// The default workspace of F frames whose per-frame bytes are frame_bytes(H, W)
+static size_t lpips_default_workspace(int n_frames, int height, int width, size_t (*frame_bytes)(int, int)) {
   if (n_frames < 0 || !lpips_size_ok(height, width)) return 0;
-  const size_t frame = nrn::lpips_frame_bytes(height, width);
+  const size_t frame = frame_bytes(height, width);
   size_t fc = nrn::kLpipsChunkBudget / frame;
   fc = fc < 1 ? 1 : (fc > static_cast<size_t>(nrn::kLpipsMaxChunk) ? nrn::kLpipsMaxChunk : fc);
   if (fc > static_cast<size_t>(n_frames)) fc = n_frames;
   return nrn::lpips_mask_bytes(height, width) + fc * frame;
 }
 
-int nrn_lpips(const NrnLpipsArgs* a) {
-  const char* who = "nrn_lpips";
+size_t nrn_lpips_workspace_bytes(int n_frames, int height, int width) {
+  return lpips_default_workspace(n_frames, height, width, nrn::lpips_frame_bytes);
+}
+
+size_t nrn_lpips_maps_workspace_bytes(int n_frames, int height, int width) {
+  return lpips_default_workspace(n_frames, height, width, nrn::lpips_map_frame_bytes);
+}
+
+// nrn_lpips (m == NULL) and nrn_lpips_maps: the same checks, chunks and kernels; with maps the distance kernels also
+// store their tap maps and the upsample kernel turns them into the chunk's maps after the reduce
+static int lpips_run(const NrnLpipsArgs* a, const NrnLpipsMapArgs* m, const char* who) {
   if (!a) return fail(NRN_E_INVALID, "%s: null args", who);
   const int F = a->n_frames, H = a->height, W = a->width;
   if (F < 0 || H < 0 || W < 0) return fail(NRN_E_INVALID, "%s: bad sizes F=%d H=%d W=%d", who, F, H, W);
@@ -1228,12 +1238,14 @@ int nrn_lpips(const NrnLpipsArgs* a) {
     return fail(NRN_E_INVALID, "%s: frames of %d x %d pixels: height and width must be at least %d (every AlexNet tap needs a pixel) "
                 "and at most %d", who, H, W, nrn::kLpipsMinSide, nrn::kLpipsMaxSide);
   if (F == 0) return NRN_OK;
-  if (!a->gt || !a->generated || !a->packed || !a->lpips || !a->workspace) return fail(NRN_E_INVALID, "%s: null argument", who);
-  if (!aligned4(a->gt) || !aligned4(a->generated) || !aligned4(a->lpips) || !aligned4(a->per_layer))
+  if (!a->gt || !a->generated || !a->packed || !a->lpips || !a->workspace || (m && !m->map))
+    return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (!aligned4(a->gt) || !aligned4(a->generated) || !aligned4(a->lpips) || !aligned4(a->per_layer) ||
+      (m && (!aligned4(m->map) || !aligned4(m->layer_maps))))
     return fail(NRN_E_INVALID, "%s: float arrays must be 4-byte aligned", who);
   if (!aligned16(a->packed) || (reinterpret_cast<uintptr_t>(a->workspace) & 255u))
     return fail(NRN_E_INVALID, "%s: packed weights must be 16-byte and the workspace 256-byte aligned", who);
-  const size_t mask_bytes = nrn::lpips_mask_bytes(H, W), frame = nrn::lpips_frame_bytes(H, W);
+  const size_t mask_bytes = nrn::lpips_mask_bytes(H, W), frame = m ? nrn::lpips_map_frame_bytes(H, W) : nrn::lpips_frame_bytes(H, W);
   if (a->workspace_bytes < mask_bytes + frame)
     return fail(NRN_E_INVALID, "%s: workspace of %zu bytes holds no frame (%zu needed for one)", who, a->workspace_bytes, mask_bytes + frame);
   size_t fc_max = (a->workspace_bytes - mask_bytes) / frame;
@@ -1267,15 +1279,47 @@ int nrn_lpips(const NrnLpipsArgs* a) {
         rc = timed(26, st, "lpips_conv_kernel", [&] {
           return nrn::launch_lpips_conv(l, d, c.act[l == 0 ? 0 : si - 1], c.act[si], packed, 2 * fc, ds->num_sms, ds->err_word, c.sat, st);
         });
-      if (!rc) rc = timed(28, st, "lpips_distance_kernel", [&] { return nrn::launch_lpips_distance(l, d, c, packed, st); });
+      if (!rc)
+        rc = timed(28, st, "lpips_distance_kernel", [&] {
+          return m ? nrn::launch_lpips_distance_map(l, d, c, packed, nrn::lpips_tap_map(a->workspace, fc, H, W, l), st)
+                   : nrn::launch_lpips_distance(l, d, c, packed, st);
+        });
     }
     if (!rc)
       rc = timed(28, st, "lpips_reduce_kernel", [&] {
         return nrn::launch_lpips_reduce(d, c, a->lpips + f0, a->per_layer ? a->per_layer + static_cast<size_t>(f0) * nrn::kLpipsTaps : nullptr, st);
       });
+    if (!rc && m)
+      rc = timed(44, st, "lpips_upsample_kernel", [&] {
+        nrn::LpipsUpsampleParams p;
+        for (int l = 0; l < nrn::kLpipsTaps; ++l) {
+          const int s = nrn::kLpipsTapStage[l];
+          p.tap[l] = nrn::lpips_tap_map(a->workspace, fc, H, W, l);
+          p.h[l] = d.h[s];
+          p.w[l] = d.w[s];
+          p.scale_y[l] = static_cast<float>(d.h[s]) / static_cast<float>(H);
+          p.scale_x[l] = static_cast<float>(d.w[s]) / static_cast<float>(W);
+        }
+        p.sat = c.sat;
+        p.fc = fc;
+        p.H = H;
+        p.W = W;
+        const size_t px0 = static_cast<size_t>(f0) * H * W;
+        p.map = m->map + px0;
+        p.layer_maps = m->layer_maps ? m->layer_maps + px0 * nrn::kLpipsTaps : nullptr;
+        p.error_image = m->error_image ? m->error_image + px0 * 3 : nullptr;
+        return nrn::launch_lpips_upsample(p, st);
+      });
     if (rc) return rc;
   }
   return NRN_OK;
+}
+
+int nrn_lpips(const NrnLpipsArgs* a) { return lpips_run(a, nullptr, "nrn_lpips"); }
+
+int nrn_lpips_maps(const NrnLpipsArgs* a, const NrnLpipsMapArgs* maps) {
+  if (!maps) return fail(NRN_E_INVALID, "nrn_lpips_maps: null args");
+  return lpips_run(a, maps, "nrn_lpips_maps");
 }
 
 // ---- correspondences (match.cu) ---------------------------------------------------------------------------------------

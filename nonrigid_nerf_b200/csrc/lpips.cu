@@ -12,6 +12,8 @@
 // not depend on its batch.
 #include "field_mma.cuh"
 #include "lpips.cuh"
+#include "eval.cuh"
+#include "jet.cuh"
 
 namespace nrn {
 namespace {
@@ -241,9 +243,10 @@ __device__ __forceinline__ float warp_sum(float v) {
 // ---- per-tap distance: per pixel sum_c w[c] (g_c / (|g| + 1e-10) - r_c / (|r| + 1e-10))^2, in fp32; one warp per
 // pixel, lanes over 8-channel chunks.  Block b of frame f sums pixels [256 b, 256 b + 256): warp w takes w, w + 8, ..
 // in order, then the 8 warp sums in warp order (fp64), into partials[f][b].  The layout depends only on the frame size.
-template <int C>
-__global__ void __launch_bounds__(256) lpips_distance_kernel(const __half* __restrict__ feat, int fc, long long hw,
-                                                             const float* __restrict__ w, double* __restrict__ partials, int stride) {
+// kMap: lane 0 also stores the pixel's distance, the value added to the sum, into map[f][px] (spatial maps).
+template <int C, bool kMap>
+__device__ __forceinline__ void lpips_distance(const __half* __restrict__ feat, int fc, long long hw, const float* __restrict__ w,
+                                               double* __restrict__ partials, int stride, float* __restrict__ map) {
   constexpr int kCh = C / 8, kPer = (kCh + 31) / 32;
   __shared__ double warp_sums[8];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, f = blockIdx.y;
@@ -288,6 +291,7 @@ __global__ void __launch_bounds__(256) lpips_distance_kernel(const __half* __res
         v = __fmaf_rn(wl[u][e], __fmul_rn(d, d), v);
       }
     v = warp_sum(v);
+    if (kMap && lane == 0) map[static_cast<size_t>(f) * hw + px] = v;
     sum += static_cast<double>(v);
   }
   if (lane == 0) warp_sums[warp] = sum;
@@ -296,6 +300,70 @@ __global__ void __launch_bounds__(256) lpips_distance_kernel(const __half* __res
     double s = 0.0;
     for (int k = 0; k < 8; ++k) s += warp_sums[k];
     partials[static_cast<size_t>(f) * stride + blockIdx.x] = s;
+  }
+}
+
+template <int C>
+__global__ void __launch_bounds__(256) lpips_distance_kernel(const __half* __restrict__ feat, int fc, long long hw,
+                                                             const float* __restrict__ w, double* __restrict__ partials, int stride) {
+  lpips_distance<C, false>(feat, fc, hw, w, partials, stride, nullptr);
+}
+template <int C>
+__global__ void __launch_bounds__(256) lpips_distance_map_kernel(const __half* __restrict__ feat, int fc, long long hw,
+                                                                 const float* __restrict__ w, double* __restrict__ partials,
+                                                                 int stride, float* __restrict__ map) {
+  lpips_distance<C, true>(feat, fc, hw, w, partials, stride, map);
+}
+
+// ---- spatial maps: one thread per output pixel of a chunk.  Per tap PyTorch's bilinear rule (align_corners=False, an
+// explicit output size) in fp32 with every operation rounded on its own: src = max(scale (y + 0.5) - 0.5, 0), i0 = (int)
+// src, i1 = i0 + (i0 < h_l - 1), l1 = src - i0, l0 = 1 - l1, v = hl0 (wl0 x00 + wl1 x01) + hl1 (wl0 x10 + wl1 x11); NaN
+// from the frame's first clamped tap on; map = (((up_0 + up_1) + up_2) + up_3) + up_4.  The 4 neighbours of every tap
+// map come from L2 (a 1008 x 756 frame's five maps are about 270 KB).
+struct UpsampleAxis {
+  int i0, i1;
+  float l0, l1;
+};
+__device__ __forceinline__ UpsampleAxis upsample_axis(int dst, float scale, int n) {
+  float src = __fsub_rn(__fmul_rn(scale, __fadd_rn(static_cast<float>(dst), 0.5f)), 0.5f);
+  src = src < 0.f ? 0.f : src;
+  UpsampleAxis a;
+  a.i0 = static_cast<int>(src);
+  a.i1 = a.i0 + (a.i0 < n - 1 ? 1 : 0);
+  a.l1 = __fsub_rn(src, static_cast<float>(a.i0));
+  a.l0 = __fsub_rn(1.f, a.l1);
+  return a;
+}
+
+__global__ void __launch_bounds__(256) lpips_upsample_kernel(LpipsUpsampleParams p) {
+  const long long hw = static_cast<long long>(p.H) * p.W;
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= p.fc * hw) return;
+  const int f = static_cast<int>(idx / hw);
+  const long long px = idx - f * hw;
+  const int y = static_cast<int>(px / p.W), x = static_cast<int>(px - static_cast<long long>(y) * p.W);
+  const unsigned clamped = p.sat[f] | p.sat[p.fc + f];
+  const int first = clamped ? __ffs(static_cast<int>(clamped)) - 1 : kLpipsTaps;
+  float total = 0.f;
+#pragma unroll
+  for (int l = 0; l < kLpipsTaps; ++l) {
+    const UpsampleAxis ay = upsample_axis(y, p.scale_y[l], p.h[l]), ax = upsample_axis(x, p.scale_x[l], p.w[l]);
+    const float* t = p.tap[l] + static_cast<size_t>(f) * p.h[l] * p.w[l];
+    const float* r0 = t + static_cast<size_t>(ay.i0) * p.w[l];
+    const float* r1 = t + static_cast<size_t>(ay.i1) * p.w[l];
+    const float top = __fadd_rn(__fmul_rn(ax.l0, __ldg(r0 + ax.i0)), __fmul_rn(ax.l1, __ldg(r0 + ax.i1)));
+    const float bot = __fadd_rn(__fmul_rn(ax.l0, __ldg(r1 + ax.i0)), __fmul_rn(ax.l1, __ldg(r1 + ax.i1)));
+    float v = __fadd_rn(__fmul_rn(ay.l0, top), __fmul_rn(ay.l1, bot));
+    if (l >= first) v = __int_as_float(0x7fc00000);
+    total = l == 0 ? v : __fadd_rn(total, v);
+    if (p.layer_maps) p.layer_maps[(static_cast<size_t>(f) * kLpipsTaps + l) * hw + px] = v;
+  }
+  p.map[idx] = total;
+  if (p.error_image) {
+    const int k = lut_index(total);
+    uint8_t* o = p.error_image + static_cast<size_t>(idx) * 3;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c] = c_jet.rgb8[k * 3 + c];
   }
 }
 
@@ -396,6 +464,21 @@ LpipsChunk lpips_chunk(void* ws, int fc, int H, int W) {
   return c;
 }
 
+// align256(fc * b) <= fc * align256(b) for fc >= 1, so fc map frames hold a chunk's buffers and its tap maps
+size_t lpips_map_frame_bytes(int H, int W) {
+  const LpipsDims d = lpips_dims(H, W);
+  size_t b = lpips_frame_bytes(H, W);
+  for (int k = 0; k < kLpipsTaps; ++k) b += align256(static_cast<size_t>(d.px(kLpipsTapStage[k])) * sizeof(float));
+  return b;
+}
+
+float* lpips_tap_map(void* ws, int fc, int H, int W, int tap) {
+  const LpipsDims d = lpips_dims(H, W);
+  uint8_t* p = static_cast<uint8_t*>(ws) + lpips_mask_bytes(H, W) + static_cast<size_t>(fc) * lpips_frame_bytes(H, W);
+  for (int k = 0; k < tap; ++k) p += align256(static_cast<size_t>(fc) * d.px(kLpipsTapStage[k]) * sizeof(float));
+  return reinterpret_cast<float*>(p);
+}
+
 cudaError_t launch_lpips_pack(const LpipsPackSources& s, uint8_t* packed, cudaStream_t st) {
   for (int l = 0; l < kLpipsTaps; ++l) {
     const long long n = kLpipsConv[l].w_bytes() / 2;
@@ -461,6 +544,29 @@ cudaError_t launch_lpips_reduce(const LpipsDims& d, const LpipsChunk& c, float* 
     tc.px[k] = static_cast<double>(d.px(kLpipsTapStage[k]));
   }
   lpips_reduce_kernel<<<blocks_of(c.fc, 128), 128, 0, st>>>(c.partials, c.sat, c.fc, c.max_blocks, tc, lpips, per_layer);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_lpips_distance_map(int tap, const LpipsDims& d, const LpipsChunk& c, const uint8_t* packed, float* tap_map,
+                                      cudaStream_t st) {
+  const int s = kLpipsTapStage[tap];
+  const dim3 grid(d.dist_blocks(tap), c.fc);
+  const float* w = reinterpret_cast<const float*>(packed + kLpipsLinOff) + lpips_c_off(tap);
+  double* part = c.partials + static_cast<size_t>(tap) * c.fc * c.max_blocks;
+  const long long hw = d.px(s);
+  switch (tap) {
+    case 0: lpips_distance_map_kernel<64><<<grid, 256, 0, st>>>(c.act[s], c.fc, hw, w, part, c.max_blocks, tap_map); break;
+    case 1: lpips_distance_map_kernel<192><<<grid, 256, 0, st>>>(c.act[s], c.fc, hw, w, part, c.max_blocks, tap_map); break;
+    case 2: lpips_distance_map_kernel<384><<<grid, 256, 0, st>>>(c.act[s], c.fc, hw, w, part, c.max_blocks, tap_map); break;
+    default: lpips_distance_map_kernel<256><<<grid, 256, 0, st>>>(c.act[s], c.fc, hw, w, part, c.max_blocks, tap_map); break;
+  }
+  return cudaGetLastError();
+}
+
+cudaError_t launch_lpips_upsample(const LpipsUpsampleParams& p, cudaStream_t st) {
+  const long long n = static_cast<long long>(p.fc) * p.H * p.W;
+  if (n == 0) return cudaSuccess;
+  lpips_upsample_kernel<<<blocks_of(n, 256), 256, 0, st>>>(p);
   return cudaGetLastError();
 }
 

@@ -12,6 +12,10 @@
 // lpips_frame_bytes(H, W) bounds one frame's share of that, so a workspace of mask + Fc * lpips_frame_bytes(H, W) bytes
 // holds a chunk of Fc frames.  The default chunk is as many frames as fit kLpipsChunkBudget (at least one, at most the
 // call's frames and kLpipsMaxChunk).
+//
+// Spatial maps (nrn_lpips_maps) use the same layout and add, right after the chunk's Fc * lpips_frame_bytes(H, W) bytes,
+// its tap maps: per tap l a 256-byte aligned buffer [Fc][h_l][w_l] fp32 of the per-pixel distances the distance kernel
+// sums.  lpips_map_frame_bytes(H, W) bounds one frame's share of both, and sizes the chunks of a map call.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -80,6 +84,24 @@ struct LpipsChunk {
 };
 LpipsChunk lpips_chunk(void* ws, int fc, int H, int W);
 
+// Spatial maps: a frame's bytes with its tap maps, and tap l's map [fc][h_l][w_l] fp32 of a chunk of fc frames
+size_t lpips_map_frame_bytes(int H, int W);
+float* lpips_tap_map(void* ws, int fc, int H, int W, int tap);
+
+// The per-pixel map of a chunk of fc frames of H x W from its tap maps (lpips.LPIPS(net='alex', spatial=True)): per tap
+// the bilinear upsample (align_corners=False) to H x W, NaN from the first tap whose convolution clamped an output of
+// the frame on, and their sum in tap order.  Outputs point at the chunk's first frame; layer_maps, error_image may be null.
+struct LpipsUpsampleParams {
+  const float* tap[kLpipsTaps];    // [fc][h_l][w_l]
+  int h[kLpipsTaps], w[kLpipsTaps];
+  float scale_y[kLpipsTaps], scale_x[kLpipsTaps];   // (float)h_l / H, (float)w_l / W
+  const unsigned* sat;             // [2 fc] the chunk's saturation words
+  int fc, H, W;
+  float* map;                      // [fc][H][W]
+  float* layer_maps;               // [fc][5][H][W]
+  uint8_t* error_image;            // [fc][H][W][3] to8b(jet(clip(map, 0, 1)))
+};
+
 struct LpipsPackSources {
   const float* conv_w[kLpipsTaps];   // OIHW
   const float* conv_b[kLpipsTaps];
@@ -96,5 +118,9 @@ cudaError_t launch_lpips_pool(const __half* in, __half* out, int n_images, int h
                               cudaStream_t st);
 cudaError_t launch_lpips_distance(int tap, const LpipsDims& d, const LpipsChunk& c, const uint8_t* packed, cudaStream_t st);
 cudaError_t launch_lpips_reduce(const LpipsDims& d, const LpipsChunk& c, float* lpips, float* per_layer, cudaStream_t st);
+// The distances of launch_lpips_distance that also stores each tap pixel's distance into tap_map [fc][h_l][w_l]
+cudaError_t launch_lpips_distance_map(int tap, const LpipsDims& d, const LpipsChunk& c, const uint8_t* packed, float* tap_map,
+                                      cudaStream_t st);
+cudaError_t launch_lpips_upsample(const LpipsUpsampleParams& p, cudaStream_t st);
 
 }  // namespace nrn

@@ -204,12 +204,14 @@ def lpips_state(source) -> list:
     """The 17 fp32 tensors nrn_lpips_pack takes, in its order (conv weight and bias of the five layers, the five tap
     weights flattened to [C_k], shift [3], scale [3]), from an lpips.LPIPS(net='alex') module or its state dict.
     Raises before anything reaches the device when the source is not that network: another backbone (VGG, SqueezeNet),
-    missing keys, wrong shapes, or a module configured for a different score (version 0.0, spatial maps)."""
+    missing keys, wrong shapes, or a module configured for a different score (version 0.0, spatial=True: per-pixel maps
+    come from the ordinary module's weights through lpips_maps())."""
     if isinstance(source, torch.nn.Module):
         if str(getattr(source, "version", "0.1")) != "0.1":
             raise RuntimeError(f"nonrigid_nerf_b200: LPIPS version {source.version} is not supported (0.1 only)")
         if getattr(source, "spatial", False):
-            raise RuntimeError("nonrigid_nerf_b200: spatial LPIPS maps are not supported (one score per frame)")
+            raise RuntimeError("nonrigid_nerf_b200: a spatial=True LPIPS module is not accepted; pack the net='alex' "
+                               "module built without spatial=True and call evaluation.lpips_maps for per-pixel maps")
         if getattr(source, "pnet_type", "alex") != "alex":
             raise RuntimeError(f"nonrigid_nerf_b200: the {source.pnet_type} backbone is not supported (net='alex' only)")
         source = source.state_dict()
@@ -276,6 +278,53 @@ def lpips(gt: torch.Tensor, generated: torch.Tensor, weights: LpipsWeights, mask
     Activations are stored in fp16.  A convolution output above 65504 (the largest fp16 value) would be clamped and
     give a finite but wrong score, so a frame with such an output in either image scores NaN instead, and so do its tap
     scores from that convolution's tap on; the earlier taps stay finite.  There is no higher-precision path."""
+    a, out, layers = _lpips_args(gt, generated, weights, mask, per_layer, chunk_frames, "nrn_lpips_workspace_bytes")
+    if a is not None:
+        with torch.cuda.device(out.device):
+            a.stream = _stream().value
+            _lib.check(_lib.load().nrn_lpips(C.byref(a)), "lpips")
+    return (out, layers) if per_layer else out
+
+
+class LpipsMaps(NamedTuple):
+    lpips: torch.Tensor                   # [F] fp32, lpips() bit for bit
+    per_layer: Optional[torch.Tensor]     # [F, 5] fp32 tap scores (per_layer=True)
+    map: torch.Tensor                     # [F, H, W] fp32
+    layer_maps: Optional[torch.Tensor]    # [F, 5, H, W] fp32 per-tap maps (per_layer=True)
+    error_image: Optional[torch.Tensor]   # [F, H, W, 3] uint8 to8b(jet(clip(map, 0, 1))) (error_images=True)
+
+
+def lpips_maps(gt: torch.Tensor, generated: torch.Tensor, weights: LpipsWeights, mask: Optional[torch.Tensor] = None,
+               per_layer: bool = False, error_images: bool = False, *, chunk_frames: Optional[int] = None) -> LpipsMaps:
+    """Per-pixel LPIPS maps of every frame of generated [F, H, W, 3] against gt: lpips.LPIPS(net='alex', spatial=True)
+    (retPerLayer=True for the per-tap maps), from the same weights and with the same arguments, checks and mask rule as
+    lpips().  Per tap, the per-pixel distances lpips() averages are upsampled to H x W (bilinear, align_corners=False, in
+    fp32 with every operation rounded on its own) and summed in tap order into `map`; the map covers masked pixels too.
+    `lpips` and `per_layer` equal lpips()'s bit for bit.  error_images=True adds to8b(jet(clip(map, 0, 1))) on the same
+    256-entry cm.jet table as image_scores' error images.  A frame with a clamped convolution output (see lpips()) gets
+    NaN in the maps from that convolution's tap on and in `map` (error-image colour jet(0)); its earlier taps' maps stay
+    finite.  Chunks are sized with the tap maps included; a frame's maps do not depend on its chunk."""
+    a, out, layers = _lpips_args(gt, generated, weights, mask, per_layer, chunk_frames, "nrn_lpips_maps_workspace_bytes")
+    f, h, w = gt.shape[:3]
+    dev = out.device
+    smap = torch.empty((f, h, w), dtype=torch.float32, device=dev)
+    lmaps = torch.empty((f, 5, h, w), dtype=torch.float32, device=dev) if per_layer else None
+    err = torch.empty((f, h, w, 3), dtype=torch.uint8, device=dev) if error_images else None
+    if a is not None:
+        m = _lib.NrnLpipsMapArgs()
+        m.map = smap.data_ptr()
+        m.layer_maps = None if lmaps is None else lmaps.data_ptr()
+        m.error_image = None if err is None else err.data_ptr()
+        with torch.cuda.device(dev):
+            a.stream = _stream().value
+            _lib.check(_lib.load().nrn_lpips_maps(C.byref(a), C.byref(m)), "lpips_maps")
+    return LpipsMaps(out, layers, smap, lmaps, err)
+
+
+def _lpips_args(gt, generated, weights, mask, per_layer, chunk_frames, workspace_fn: str):
+    """The checks and mask rule lpips() and lpips_maps() share, then their score outputs and workspace: (NrnLpipsArgs
+    without its stream, or None when there are no frames; lpips [F]; per_layer [F, 5] or None).  workspace_fn names the
+    library's default-workspace function of the call."""
     if not isinstance(weights, LpipsWeights):
         raise RuntimeError("nonrigid_nerf_b200: weights must come from evaluation.lpips_weights()")
     gt = _frames(gt, "gt", 4)
@@ -293,29 +342,28 @@ def lpips(gt: torch.Tensor, generated: torch.Tensor, weights: LpipsWeights, mask
         if tuple(mask.shape) != (h, w) or mask.device != dev:
             raise RuntimeError(f"nonrigid_nerf_b200: mask must be [{h}, {w}] on {dev}, got {tuple(mask.shape)}")
         mask = (mask != 0).to(torch.uint8).contiguous()
-    lib = _lib.load()
+    workspace_bytes = getattr(_lib.load(), workspace_fn)
     if chunk_frames is None:
-        ws_bytes = int(lib.nrn_lpips_workspace_bytes(f, h, w))
+        ws_bytes = int(workspace_bytes(f, h, w))
     else:
         if int(chunk_frames) < 1:
             raise RuntimeError(f"nonrigid_nerf_b200: chunk_frames must be at least 1, got {chunk_frames}")
-        base = int(lib.nrn_lpips_workspace_bytes(0, h, w))
-        ws_bytes = base + min(int(chunk_frames), f) * (int(lib.nrn_lpips_workspace_bytes(1, h, w)) - base)
+        base = int(workspace_bytes(0, h, w))
+        ws_bytes = base + min(int(chunk_frames), f) * (int(workspace_bytes(1, h, w)) - base)
     if ws_bytes == 0:
         raise RuntimeError(f"nonrigid_nerf_b200: LPIPS frames of {h} x {w} pixels are out of range")
     out = torch.empty(f, dtype=torch.float32, device=dev)
     layers = torch.empty((f, 5), dtype=torch.float32, device=dev) if per_layer else None
-    if f > 0:
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-        a = _lib.NrnLpipsArgs()
-        a.gt, a.generated, a.mask = gt.data_ptr(), generated.data_ptr(), None if mask is None else mask.data_ptr()
-        a.n_frames, a.height, a.width = f, h, w
-        a.packed, a.lpips, a.per_layer = weights.packed.data_ptr(), out.data_ptr(), None if layers is None else layers.data_ptr()
-        a.workspace, a.workspace_bytes = ws.data_ptr(), ws_bytes
-        with torch.cuda.device(dev):
-            a.stream = _stream().value
-            _lib.check(lib.nrn_lpips(C.byref(a)), "lpips")
-    return (out, layers) if per_layer else out
+    if f == 0:
+        return None, out, layers
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    a = _lib.NrnLpipsArgs()
+    a.gt, a.generated, a.mask = gt.data_ptr(), generated.data_ptr(), None if mask is None else mask.data_ptr()
+    a.n_frames, a.height, a.width = f, h, w
+    a.packed, a.lpips, a.per_layer = weights.packed.data_ptr(), out.data_ptr(), None if layers is None else layers.data_ptr()
+    a.workspace, a.workspace_bytes = ws.data_ptr(), ws_bytes
+    a.tensors = (gt, generated, mask, ws)   # what the pointers point into, kept alive until the call has enqueued its kernels
+    return a, out, layers
 
 
 def normal_images(normals: torch.Tensor, c2w: torch.Tensor) -> torch.Tensor:
