@@ -721,6 +721,37 @@ size_t nrn_termination_workspace_bytes(int n_rays, int n_samples, int out_ch, in
 int nrn_field_forward_terminate(const NrnFieldArgs* args, const NrnOccupancyGrid* grid /* NULL: none */, const NrnTerminationArgs* term,
                                 void* workspace, size_t workspace_bytes);
 
+/* ---- baked canonical radiance grids: render passes that sample a grid in place of the NeRF trunk ---------------------
+ * A grid of nx * ny * nz vertices (2..1024 per axis) over [min_point, max_point]: vertex (i, j, k) holds raw[0..3] of the
+ * canonical model (no bender) at nrn_mesh_grid_points' point (i, j, k), as fp16 at values[((k * ny + j) * nx + i) * 4 + c].
+ * A sample is LOOKED UP when its (bent) point is finite and min <= x <= max on every axis; per axis, every operation an
+ * fp32 one rounded on its own, scale = fl((n - 1) / fl(max - min)), u = fl(fl(x - min) * scale), i = min(floor(u), n - 2),
+ * f = fl(u - i), and the 8 corners blend along x, then y, then z, each step a + f (b - a).  Any other sample goes through
+ * the NeRF trunk.
+ *
+ * nrn_radiance_plane_f16: plane [n][4] fp16 (8-byte aligned) <- raw [n][out_ch] channels 0..3 (out_ch 4 or 5), rounded to
+ *   nearest even; finite values beyond fp16's range saturate to +-65504, inf and NaN stay non-finite.  The bake's store:
+ *   one call per z-plane on the raw of a point-mode nrn_field_forward at that plane's nrn_mesh_grid_points.
+ * nrn_field_forward_baked: one inference pass of nrn_field_forward in ray mode (args as there, no stash / relu_mask,
+ *   points NULL).  With a bender the bend pass runs with the lookup in its epilogue (bent points, rigidities and the
+ *   details as the bend pass writes them); without one the lookup runs at rays_o + rays_d * z.  The other samples are
+ *   compacted in ascending order as nrn_field_forward_occupancy compacts its kept samples (for a grid of one empty cell
+ *   over the same box; without a bender this step writes the details), the point-mode trunk runs on them (their count read
+ *   on the device: no host synchronisation, CUDA-graph capturable), and the scatter writes their raw.  So raw =
+ *   lookup where looked up, nrn_field_forward's raw bit for bit elsewhere; the object removal zeroes raw[3] of either
+ *   where rigidity >= removal_threshold, and raw[4] of a looked-up sample (out_ch 5) is 0.  workspace:
+ *   nrn_baked_workspace_bytes(n_rays, n_samples, out_ch, bender_packed != NULL), 256-byte aligned.  A malformed grid, more
+ *   than 2^31 - 1 points or a short workspace return NRN_E_INVALID before any CUDA call. */
+typedef struct NrnRadianceGrid {
+  const void* values;           /* [nz][ny][nx][4] fp16, 8-byte aligned */
+  int32_t nx, ny, nz;           /* vertices per axis, 2..1024 */
+  float min_point[3];
+  float max_point[3];
+} NrnRadianceGrid;
+int nrn_radiance_plane_f16(const float* raw, long long n, int out_ch, void* plane, void* stream);
+size_t nrn_baked_workspace_bytes(int n_rays, int n_samples, int out_ch, int has_bender);
+int nrn_field_forward_baked(const NrnFieldArgs* args, const NrnRadianceGrid* grid, void* workspace, size_t workspace_bytes);
+
 /* ---- the inverse of the ray bender: canonical points into every frame (geometry.deform_points) -------------------------
  * The ray bender maps an observed point x of a frame with latent z to the canonical point c = b(x; z) = x + s r~(x) o(x, z)
  * (run_nerf_helpers.py:507-584: o the offset MLP on [x, z], r = (tanh(rho(x)) + 1) / 2 the rigidity, r~ = 0 where
@@ -806,7 +837,9 @@ int nrn_field_density_gradient(const NrnDensityGradArgs* args);
  * 38 the trunk on the kept points, 39 the scatters (and the zeroing of raw) and 40 the transmittance updates (and their
  * initialisation), 41 nrn_deform_points, and of nrn_field_density_gradient 42 the forward (with the time-conditioned
  * biases) and 43 the DGRAD, 44 the upsampling of nrn_lpips_maps (its other kernels are kinds 25 to 28, the distances
- * with their tap maps kind 28).  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * with their tap maps kind 28), 45 nrn_radiance_plane_f16, and of nrn_field_forward_baked 46 the bend pass with the
+ * lookup (without a bender the lookup alone), 47 the compaction of the other samples, 48 the trunk on them and 49 the
+ * scatter.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

@@ -194,6 +194,13 @@ class NrnMatchArgs(C.Structure):
     ]
 
 
+class NrnRadianceGrid(C.Structure):
+    _fields_ = [
+        ("values", _vp), ("nx", C.c_int32), ("ny", C.c_int32), ("nz", C.c_int32),
+        ("min_point", C.c_float * 3), ("max_point", C.c_float * 3),
+    ]
+
+
 class NrnOccupancyGrid(C.Structure):
     _fields_ = [
         ("bits", _vp), ("nx", C.c_int32), ("ny", C.c_int32), ("nz", C.c_int32),
@@ -326,6 +333,9 @@ SYMBOLS = {
     "nrn_termination_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
     "nrn_field_forward_terminate": (C.c_int, [C.POINTER(NrnFieldArgs), C.POINTER(NrnOccupancyGrid), C.POINTER(NrnTerminationArgs), _vp,
                                               C.c_size_t]),
+    "nrn_radiance_plane_f16": (C.c_int, [_vp, C.c_longlong, C.c_int, _vp, _vp]),
+    "nrn_baked_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
+    "nrn_field_forward_baked": (C.c_int, [C.POINTER(NrnFieldArgs), C.POINTER(NrnRadianceGrid), _vp, C.c_size_t]),
     "nrn_deform_points": (C.c_int, [C.POINTER(NrnDeformArgs)]),
     "nrn_density_gradient_chunk": (C.c_int64, []),
     "nrn_density_gradient_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
@@ -369,6 +379,9 @@ NORMAL_KERNEL_KINDS = ("density_grad_fwd", "density_grad_dgrad")
 # spatial LPIPS maps (evaluation.lpips_maps: the upsampling of the tap maps into per-pixel maps and error images), timing
 # kind 44; the rest of the call is timed as LPIPS_KERNEL_KINDS
 LPIPS_MAP_KERNEL_KINDS = ("lpips_upsample",)
+# baked radiance grids (the bake's fp16 plane store; of a render pass: bend pass + lookup, compaction of the other samples,
+# trunk on them, scatter), timing kinds 45 to 49
+BAKED_KERNEL_KINDS = ("baked_plane", "baked_bend", "baked_compact", "baked_field", "baked_scatter")
 
 
 def timing_enable(on: bool) -> None:
@@ -379,8 +392,8 @@ def timing_read(kinds=KERNEL_KINDS):
     """{kind: (total_ms, launches)} for the launches recorded since timing_enable(True); `kinds` is KERNEL_KINDS,
     KERNEL_KINDS + TC_KERNEL_KINDS, KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS, that + VIEW_TRAIN_KERNEL_KINDS,
     that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS, that + EVAL_KERNEL_KINDS, that + FRAME_IMAGE_KERNEL_KINDS, that + MESH_KERNEL_KINDS, that + LPIPS_KERNEL_KINDS, that + MATCH_KERNEL_KINDS, that
-    + OCCUPANCY_KERNEL_KINDS, that + TERMINATION_KERNEL_KINDS, that + DEFORM_KERNEL_KINDS, that + NORMAL_KERNEL_KINDS or
-    that + LPIPS_MAP_KERNEL_KINDS."""
+    + OCCUPANCY_KERNEL_KINDS, that + TERMINATION_KERNEL_KINDS, that + DEFORM_KERNEL_KINDS, that + NORMAL_KERNEL_KINDS,
+    that + LPIPS_MAP_KERNEL_KINDS or that + BAKED_KERNEL_KINDS."""
     n = len(kinds)
     ms = (C.c_double * n)()
     cnt = (C.c_int * n)()

@@ -718,6 +718,29 @@ def field_occupancy(net, rays, z_vals, latents, want_details, grid):
                                        grid)
 
 
+def baked_check(net, latents, grid) -> None:
+    """Raise, before any launch, for what render(..., baked=) does not support: a pass without a geometry.RadianceGrid,
+    the view-dependent head, the time-conditioned baseline and differentiable calls."""
+    from .geometry import RadianceGrid, bake_check
+    if not isinstance(grid, RadianceGrid):
+        raise RuntimeError(f"nonrigid_nerf_b200: a baked render pass needs a geometry.RadianceGrid, got {type(grid).__name__}")
+    bake_check(net)
+    if _needs_grad(net, latents):
+        raise RuntimeError("nonrigid_nerf_b200: rendering from a baked radiance grid is inference only; call render() under "
+                           "torch.no_grad() (the grid carries no gradient)")
+
+
+def field_baked(net, rays, z_vals, latents, want_details, grid):
+    """field_rays that samples the radiance grid in place of the NeRF trunk for samples inside its box."""
+    baked_check(net, latents, grid)
+    bender = net.ray_bender[0]
+    cutoff, scaling, removal = _knobs(net)
+    nerf_pack = ops.pack_nerf(net)
+    bender_pack = ops.pack_bender(bender) if bender is not None else None
+    out_ch = net.output_linear.weight.shape[0]
+    return ops.field_forward_baked(rays, z_vals, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details, grid)
+
+
 def termination_threshold(threshold) -> float:
     """The early-termination threshold as a float; raises unless it is a finite real number in [0, 1] (not a bool or a
     tensor)."""

@@ -21,6 +21,7 @@
 #include "lpips.cuh"
 #include "match.cuh"
 #include "occupancy.cuh"
+#include "baked.cuh"
 #include "deform.cuh"
 
 namespace nrn {
@@ -37,6 +38,7 @@ cudaError_t launch_field_views(const FieldFwdParams& p, const ViewParams& v, int
 cudaError_t launch_field_views_train(const FieldFwdParams& p, const ViewParams& v, const ViewTrainParams& t, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_bwd_views(const FieldBwdParams& p, const ViewBwdParams& v, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_fwd_kept(const FieldFwdParams& p, const int* kept, int num_sms, cudaStream_t stream);
+cudaError_t launch_field_baked(const FieldFwdParams& p, const ViewParams& v, const BakedGrid& g, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_fwd_grad(const FieldFwdParams& p, bool has_bender, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_bwd_grad(const FieldBwdParams& p, const PointGradParams& pg, bool has_bender, int num_sms, cudaStream_t stream);
 }
@@ -1644,6 +1646,126 @@ int nrn_field_forward_terminate(const NrnFieldArgs* a, const NrnOccupancyGrid* g
     if (rc) return rc;
   }
   return NRN_OK;
+}
+
+// ---- baked canonical radiance grids: the bake's plane store, and the render pass that samples the grid ----
+static bool baked_sides_ok(int nx, int ny, int nz) {
+  const int n[3] = {nx, ny, nz};
+  for (int d = 0; d < 3; ++d)
+    if (n[d] < nrn::kBakedMinSide || n[d] > nrn::kBakedMaxSide) return false;
+  return true;
+}
+
+// The grid as the kernels read it; NRN_E_INVALID for a malformed one
+static int baked_grid(const NrnRadianceGrid* g, const char* who, nrn::BakedGrid* out) {
+  if (!g) return fail(NRN_E_INVALID, "%s: null grid", who);
+  if (!baked_sides_ok(g->nx, g->ny, g->nz))
+    return fail(NRN_E_INVALID, "%s: grid resolution %d x %d x %d out of range (%d..%d vertices per axis)", who, g->nx, g->ny, g->nz,
+                nrn::kBakedMinSide, nrn::kBakedMaxSide);
+  if (!g->values || (reinterpret_cast<uintptr_t>(g->values) & 7u)) return fail(NRN_E_INVALID, "%s: grid values null or not 8-byte aligned", who);
+  nrn::BakedGrid o{};
+  o.vox = static_cast<const uint2*>(g->values);
+  o.n[0] = g->nx; o.n[1] = g->ny; o.n[2] = g->nz;
+  for (int d = 0; d < 3; ++d) {
+    const float lo = g->min_point[d], hi = g->max_point[d];
+    if (!(std::isfinite(lo) && std::isfinite(hi) && hi > lo)) return fail(NRN_E_INVALID, "%s: grid box must be finite with max > min on every axis", who);
+    const float ext = hi - lo;
+    const float sc = static_cast<float>(o.n[d] - 1) / ext;
+    if (!(std::isfinite(ext) && std::isfinite(sc) && sc > 0.f)) return fail(NRN_E_INVALID, "%s: grid box extent out of fp32 range", who);
+    o.lo[d] = lo; o.hi[d] = hi; o.scale[d] = sc;
+  }
+  *out = o;
+  return NRN_OK;
+}
+
+int nrn_radiance_plane_f16(const float* raw, long long n, int out_ch, void* plane, void* stream) {
+  const char* who = "nrn_radiance_plane_f16";
+  if (n < 0 || out_ch < 4 || out_ch > 5 || n > (1LL << 40)) return fail(NRN_E_INVALID, "%s: bad sizes n=%lld out_ch=%d", who, n, out_ch);
+  if (n == 0) return NRN_OK;
+  if (!raw || !plane) return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (!aligned4(raw) || (reinterpret_cast<uintptr_t>(plane) & 7u)) return fail(NRN_E_INVALID, "%s: raw must be 4-byte and plane 8-byte aligned", who);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return timed(45, st, "baked_plane_kernel", [&] { return nrn::launch_baked_plane(raw, n, out_ch, static_cast<uint2*>(plane), st); });
+}
+
+// nrn_occupancy_workspace_bytes's layout, then one word that reads as an empty one-cell occupancy grid
+size_t nrn_baked_workspace_bytes(int n_rays, int n_samples, int out_ch, int has_bender) {
+  const size_t occ = nrn_occupancy_workspace_bytes(n_rays, n_samples, out_ch, has_bender);
+  return occ ? occ + align256(sizeof(uint32_t)) : 0;
+}
+
+int nrn_field_forward_baked(const NrnFieldArgs* a, const NrnRadianceGrid* grid, void* workspace, size_t workspace_bytes) {
+  const char* who = "nrn_field_forward_baked";
+  long long P;
+  int tiles;
+  int rc = check_field_args(a, who, &P, &tiles);
+  if (rc) return rc;
+  if (a->stash || a->relu_mask) return fail(NRN_E_INVALID, "%s: inference only (stash / relu_mask must be NULL)", who);
+  if (a->points) return fail(NRN_E_INVALID, "%s: needs ray mode (rays and z_vals; points must be NULL)", who);
+  nrn::BakedGrid bg;
+  rc = baked_grid(grid, who, &bg);
+  if (rc) return rc;
+  if (P > nrn::kOccMaxPoints) return fail(NRN_E_INVALID, "%s: %lld points in one pass (at most 2^31 - 1)", who, P);
+  if (P == 0) return NRN_OK;
+  const bool bend = a->bender_packed != nullptr;
+  if (!a->raw) return fail(NRN_E_INVALID, "%s: null raw", who);
+  const size_t need = nrn_baked_workspace_bytes(a->n_rays, a->n_samples, a->out_ch, bend);
+  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255u) || workspace_bytes < need)
+    return fail(NRN_E_INVALID, "%s: workspace null, not 256-byte aligned or smaller than nrn_baked_workspace_bytes (%zu)", who, need);
+  DeviceState* ds;
+  rc = device_state(&ds);
+  if (rc) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  const size_t p = static_cast<size_t>(P);
+  uint8_t* w = static_cast<uint8_t*>(workspace);
+  float4* ws = nullptr;
+  if (bend) { ws = reinterpret_cast<float4*>(w); w += align256(p * sizeof(float4)); }
+  float* kept_xyz = reinterpret_cast<float*>(w); w += align256(p * 3 * sizeof(float));
+  int32_t* kept_idx = reinterpret_cast<int32_t*>(w); w += align256(p * sizeof(int32_t));
+  float* craw = reinterpret_cast<float*>(w); w += align256(p * a->out_ch * sizeof(float));
+  int32_t* count = reinterpret_cast<int32_t*>(w); w += align256(sizeof(int32_t));
+  int32_t* block_counts = reinterpret_cast<int32_t*>(w); w += occ_block_count_bytes(P);
+  uint32_t* empty = reinterpret_cast<uint32_t*>(w);
+
+  nrn::FieldFwdParams p0 = field_fwd_params(a, P, tiles, ds->err_word);
+  // a. raw of the samples inside the grid's box: with a bender from the bend pass's epilogue (which also writes the bent
+  //    points and rigidities to ws, and the details), without one at rays_o + rays_d * z
+  if (bend) {
+    nrn::ViewParams vp{};
+    vp.ws = ws;
+    rc = timed(46, st, "field_baked_kernel", [&] { return nrn::launch_field_baked(p0, vp, bg, ds->num_sms, st); });
+  } else {
+    rc = timed(46, st, "baked_rays_kernel", [&] {
+      return nrn::launch_baked_rays(bg, a->rays, a->z_vals, a->n_samples, P, a->raw, a->out_ch, st);
+    });
+  }
+  if (rc) return rc;
+  // b. the samples outside the box or not finite, compacted in order: exactly those an occupancy grid of one empty cell
+  //    over the same box keeps (without a bender this step also writes the details)
+  nrn::OccGrid og{};
+  og.bits = empty; og.nx = og.ny = og.nz = 1;
+  for (int d = 0; d < 3; ++d) { og.lo[d] = bg.lo[d]; og.hi[d] = bg.hi[d]; og.scale[d] = 1.f / (bg.hi[d] - bg.lo[d]); }
+  nrn::OccPoints s{};
+  s.ws = ws; s.rays = a->rays; s.z_vals = a->z_vals; s.S = a->n_samples; s.P = P;
+  nrn::OccCompact c{};
+  c.kept_xyz = kept_xyz; c.kept_idx = kept_idx; c.count = count; c.block_counts = block_counts;
+  if (!bend) { c.d_init = a->initial_input_pts; c.d_bent = a->input_pts; }
+  rc = timed(47, st, "occupancy_compact", [&] {
+    const cudaError_t e = cudaMemsetAsync(empty, 0, sizeof(uint32_t), st);
+    return e != cudaSuccess ? e : nrn::launch_occupancy_compact(og, s, c, st);
+  });
+  if (rc) return rc;
+  // c. the point-mode trunk on them, their count read on the device
+  nrn::FieldFwdParams q{};
+  q.pts = kept_xyz; q.pts_stride = 3; q.n_rays = static_cast<int>(P); q.S = 1; q.P = P; q.n_tiles = tiles;
+  q.nerf_w = p0.nerf_w; q.nerf_bias = p0.nerf_bias; q.out_ch = a->out_ch; q.raw = craw; q.err = ds->err_word;
+  rc = timed(48, st, "field_fwd_kept_kernel", [&] { return nrn::launch_field_fwd_kept(q, count, ds->num_sms, st); });
+  if (rc) return rc;
+  // d. their raw into the pass's output (with the object removal), beside the grid's
+  return timed(49, st, "occ_scatter_kernel", [&] {
+    return nrn::launch_termination_scatter(craw, kept_idx, count, P, a->out_ch, ws, a->use_removal, a->removal_threshold, a->raw,
+                                           ds->num_sms, st);
+  });
 }
 
 // ---- the inverse of the ray bender ----

@@ -27,6 +27,10 @@
 //            buffer: 24 KB less shared memory than the other kernels.
 //   view-head training kernel (no bender): the view-head kernel that also writes the trunk's stash and masks, the view
 //            stash (direction encoding, feature, hv) and hv's mask bits for field_bwd_views_kernel.
+//
+// Baked radiance grid (render(..., baked=)): the bend pass that also looks every bent point up in the grid (baked.cuh)
+// and writes raw of the points inside its box; the trunk runs afterwards on the others alone (c_abi.cu).
+#include "baked.cuh"
 #include "field_mma.cuh"
 
 namespace nrn {
@@ -189,8 +193,9 @@ __device__ __forceinline__ Step step_at_views(int step) {
   }
 }
 
-// Which part of the forward a kernel runs: all of it, the bend pass of the view-dependent head, or its view-head kernel
-enum Part : int { kFull, kBend, kViews };
+// Which part of the forward a kernel runs: all of it, the bend pass of the view-dependent head, its view-head kernel, or
+// the bend pass with the baked grid's lookup
+enum Part : int { kFull, kBend, kViews, kBaked };
 
 }  // namespace
 
@@ -200,12 +205,13 @@ enum Part : int { kFull, kBend, kViews };
 // PART (view-dependent head): kBend runs B0..B4 and writes v.ws; kViews (HAS_BENDER false) runs the trunk and the view
 // head, reading its points and rigidities from v.ws when that is given.  kViews with TRAIN (no bender, v.ws null): the
 // trunk's stash and masks as the full kernel writes them, and the view stash and Hv masks of t.
+// kBaked (with a bender, inference): kBend, and each point inside the box of the grid bg gets raw from bg's lookup.
 template <bool HAS_BENDER, bool TRAIN, bool LATENT_BIAS, int PART = kFull>
 __device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p, const ViewParams& v = ViewParams{},
-                                               const ViewTrainParams& t = ViewTrainParams{}) {
+                                               const ViewTrainParams& t = ViewTrainParams{}, const BakedGrid& bg = BakedGrid{}) {
   static_assert(!(HAS_BENDER && LATENT_BIAS), "the time-conditioned baseline has no bender");
-  static_assert(PART == kFull || (!LATENT_BIAS && (PART == kBend) == HAS_BENDER && (!TRAIN || PART == kViews)),
-                "view-head parts: inference, or training of the view-head kernel without a bender");
+  static_assert(PART == kFull || (!LATENT_BIAS && (PART == kBend || PART == kBaked) == HAS_BENDER && (!TRAIN || PART == kViews)),
+                "bend and view-head parts: inference, or training of the view-head kernel without a bender");
   constexpr int kHBytes = PART == kViews ? 0 : kFwdHBytes;   // the view-head kernel has no bender images
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* act = smem;                                  // H (bender) | E, 128 rows
@@ -226,7 +232,8 @@ __device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p, const Vi
     // ===================== weight producer: global -> smem ring (bulk TMA) =====================
     if (warp == 8 && lane == 0) {
       if constexpr (PART == kViews) produce(p.nerf_w, v.w, p.n_tiles, fwd::L0, views::kEnd, views::Feature, step_at_views, ring, W);
-      else produce(p.bend_w, p.nerf_w, p.n_tiles, HAS_BENDER ? fwd::B0 : fwd::L0, PART == kBend ? fwd::L0 : fwd::kCount, fwd::L0, step_at, ring, W);
+      else produce(p.bend_w, p.nerf_w, p.n_tiles, HAS_BENDER ? fwd::B0 : fwd::L0, PART == kBend || PART == kBaked ? fwd::L0 : fwd::kCount, fwd::L0,
+                   step_at, ring, W);
     }
     return;
   }
@@ -372,8 +379,11 @@ __device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p, const Vi
     if (valid && p.d_bent) {
       p.d_bent[pt * 3 + 0] = x[0]; p.d_bent[pt * 3 + 1] = x[1]; p.d_bent[pt * 3 + 2] = x[2];
     }
-    if constexpr (PART == kBend) {   // the bend pass ends here: bent point and rigidity -> the workspace
+    if constexpr (PART == kBend || PART == kBaked) {   // the bend pass ends here: bent point and rigidity -> the workspace
       if (valid) v.ws[pt] = make_float4(x[0], x[1], x[2], rigidity);
+      // the baked grid: raw of a point inside its box, the object removal applied as the head below applies it
+      if constexpr (PART == kBaked)
+        if (valid) baked_raw(bg, x, p.use_removal && rigidity >= p.removal, p.raw, pt, p.out_ch);
       continue;
     }
     // ---- positional encoding of the (bent) point -> E ----
@@ -495,6 +505,9 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bend_kernel(const FieldF
 __global__ void __launch_bounds__(kFwdThreads, 1) field_views_kernel(const FieldFwdParams p, const ViewParams v) {
   field_fwd_body<false, false, false, kViews>(p, v);
 }
+__global__ void __launch_bounds__(kFwdThreads, 1) field_baked_kernel(const FieldFwdParams p, const ViewParams v, const BakedGrid g) {
+  field_fwd_body<true, false, false, kBaked>(p, v, ViewTrainParams{}, g);
+}
 // The point-mode trunk (no bender) over the points an occupancy lookup kept (occupancy.cu): their count is read from device
 // memory, so a render pass that skips empty space needs no host synchronisation and can be captured in a CUDA graph
 __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kept_kernel(FieldFwdParams p, const int* __restrict__ kept) {
@@ -558,6 +571,11 @@ size_t field_views_smem_bytes() { return kFwdSmemBytes - kFwdHBytes; }
 
 cudaError_t launch_field_bend(const FieldFwdParams& p, const ViewParams& v, int num_sms, cudaStream_t stream) {
   return launch_field(field_bend_kernel, p, num_sms, field_fwd_smem_bytes(), stream, v);
+}
+
+// The bend pass with the baked grid's lookup: v.ws as launch_field_bend writes it, and p.raw of the points inside g's box
+cudaError_t launch_field_baked(const FieldFwdParams& p, const ViewParams& v, const BakedGrid& g, int num_sms, cudaStream_t stream) {
+  return launch_field(field_baked_kernel, p, num_sms, field_fwd_smem_bytes(), stream, v, g);
 }
 
 cudaError_t launch_field_views(const FieldFwdParams& p, const ViewParams& v, int num_sms, cudaStream_t stream) {

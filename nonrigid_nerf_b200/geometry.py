@@ -336,6 +336,85 @@ def occupancy_grid(network_fn, min_point, max_point, resolution, threshold: floa
     return occupancy_from_sigma(sigma, min_point, max_point, threshold, dilation)
 
 
+# ---- baked canonical radiance grids ---------------------------------------------------------------------------------------
+@dataclasses.dataclass(frozen=True, eq=False)
+class RadianceGrid:
+    """The canonical model's raw, baked for render(..., baked=BakedScene(grid, ...)).  nx * ny * nz vertices over
+    [min_point, max_point]; values[k, j, i] holds raw[0:4] at density_grid's point (i, j, k) as fp16.  A sample whose (bent)
+    point is finite and inside the box takes raw from the trilinear lookup (nrnerf_b200.h gives the fp32 rule), every
+    other sample from the NeRF trunk."""
+    values: torch.Tensor               # [nz, ny, nx, 4] fp16 on the model's device
+    min_point: np.ndarray              # [3] float32
+    max_point: np.ndarray              # [3] float32
+    resolution: Tuple[int, int, int]   # (nx, ny, nz) vertices
+
+    def c_struct(self, device) -> "_lib.NrnRadianceGrid":
+        """The grid as the C ABI reads it; raises unless the values are a contiguous [nz, ny, nx, 4] fp16 tensor on `device`."""
+        nx, ny, nz = self.resolution
+        v = self.values
+        if not (isinstance(v, torch.Tensor) and v.dtype == torch.float16 and tuple(v.shape) == (nz, ny, nx, 4) and v.is_contiguous()):
+            raise RuntimeError(f"nonrigid_nerf_b200: radiance grid values must be a contiguous [{nz}, {ny}, {nx}, 4] float16 tensor "
+                               f"for resolution {self.resolution}")
+        if v.device != torch.device(device):
+            raise RuntimeError(f"nonrigid_nerf_b200: the radiance grid is on {v.device}, the rays on {device}")
+        g = _lib.NrnRadianceGrid()
+        g.values, g.nx, g.ny, g.nz = v.data_ptr(), nx, ny, nz
+        g.min_point[:] = [float(x) for x in self.min_point]
+        g.max_point[:] = [float(x) for x in self.max_point]
+        return g
+
+
+@dataclasses.dataclass(frozen=True, eq=False)
+class BakedScene:
+    """The grids render(..., baked=scene) samples: `coarse` for the coarse pass, `fine` for the fine pass (needed when
+    N_importance > 0; bake the model that pass runs).  Not a tuple, so the ray-sharded render wrapper hands it to every
+    rank as it is."""
+    coarse: RadianceGrid
+    fine: Optional[RadianceGrid] = None
+
+
+def _vertices(resolution):
+    r = (resolution,) * 3 if isinstance(resolution, (int, np.integer)) else resolution
+    if not isinstance(r, (tuple, list)) or len(r) != 3 or any(not isinstance(n, (int, np.integer)) or isinstance(n, bool) for n in r):
+        raise RuntimeError(f"nonrigid_nerf_b200: resolution must be an int or (nx, ny, nz) vertices, got {resolution!r}")
+    if any(n < 2 or n > 1024 for n in r):
+        raise RuntimeError(f"nonrigid_nerf_b200: radiance grid resolution must be 2..1024 vertices on every axis, got {r}")
+    return tuple(int(n) for n in r)
+
+
+def bake_check(network_fn) -> None:
+    """Raise for a model whose raw depends on more than the canonical point: the view-dependent head and the
+    time-conditioned baseline."""
+    if getattr(network_fn, "use_viewdirs", False):
+        raise RuntimeError("nonrigid_nerf_b200: a view-dependent model (use_viewdirs=True) cannot be baked: its raw depends on "
+                           "the view direction")
+    if getattr(network_fn, "time_conditioned_baseline", False):
+        raise RuntimeError("nonrigid_nerf_b200: a time_conditioned_baseline=True model cannot be baked: its raw depends on the "
+                           "latent code")
+
+
+def bake_radiance(network_fn, min_point, max_point, resolution) -> RadianceGrid:
+    """network_fn's canonical raw (the bender off, as render_canonical renders) on resolution = n or (nx, ny, nz) vertices
+    (2..1024 per axis) over min_point .. max_point: the point-mode NeRF trunk at density_grid's points, z-plane by
+    z-plane, stored as fp16 with round to nearest, finite values saturated to +-65504 and non-finite ones kept.  Bake the
+    coarse and the fine model separately.  Not implemented for use_viewdirs=True and time_conditioned_baseline=True."""
+    bake_check(network_fn)
+    nx, ny, nz = _vertices(resolution)
+    lo, hi = _extent(min_point, max_point)
+    field = _PointField(network_fn, None)
+    lib = _lib.load()
+    with torch.cuda.device(field.dev), torch.no_grad():
+        values = torch.empty(nz, ny, nx, 4, dtype=torch.float16, device=field.dev)
+        points = torch.empty(ny * nx, 3, dtype=torch.float32, device=field.dev)
+        for k in range(nz):
+            _lib.check(lib.nrn_mesh_grid_points(lo.ctypes.data, hi.ctypes.data, nx, ny, nz, k, points.data_ptr(), _stream()),
+                       "mesh_grid_points")
+            raw, _ = field(points)
+            _lib.check(lib.nrn_radiance_plane_f16(raw.data_ptr(), nx * ny, field.out_ch, values[k].data_ptr(), _stream()),
+                       "radiance_plane_f16")
+    return RadianceGrid(values, lo, hi, (nx, ny, nz))
+
+
 # ---- host-side writers --------------------------------------------------------------------------------------------------
 def _host(mesh: Mesh):
     v = mesh.vertices.detach().cpu().numpy().astype("<f4", copy=False).reshape(-1, 3)

@@ -340,6 +340,26 @@ def field_forward_occupancy(rays: torch.Tensor, z_vals: torch.Tensor, latents: O
     return raw, details
 
 
+def field_forward_baked(rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[torch.Tensor], nerf_pack: torch.Tensor,
+                        bender_pack: Optional[torch.Tensor], out_ch: int, cutoff=None, scaling=None, removal=None,
+                        want_details: bool = False, grid=None) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
+    """field_forward (inference) that samples the radiance grid (geometry.RadianceGrid) in place of the NeRF trunk for
+    samples whose (bent) point lies inside its box: raw [N, S, out_ch] from the lookup there (raw[..., 4] = 0), equal to
+    field_forward's elsewhere; the details for every sample."""
+    if bender_pack is not None and latents is None:
+        raise RuntimeError("nonrigid_nerf_b200: ray bending needs latents")
+    a, raw, details, keep = _field_args(rays, z_vals, None, 1, latents if bender_pack is not None else None, nerf_pack, bender_pack,
+                                        out_ch, (cutoff, scaling, removal), True, want_details)
+    dev = keep[0].device
+    g = grid.c_struct(dev)
+    lib = _lib.load()
+    nbytes = lib.nrn_baked_workspace_bytes(a.n_rays, a.n_samples, out_ch, int(bender_pack is not None))
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.nrn_field_forward_baked(C.byref(a), C.byref(g), _ptr(ws), nbytes), "field_forward_baked")
+    return raw, details
+
+
 def field_forward_terminate(rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[torch.Tensor], nerf_pack: torch.Tensor,
                             bender_pack: Optional[torch.Tensor], out_ch: int, cutoff=None, scaling=None, removal=None,
                             want_details: bool = False, threshold: float = 0.0, grid=None, noise: Optional[torch.Tensor] = None

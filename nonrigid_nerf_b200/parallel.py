@@ -321,9 +321,9 @@ class training_wrapper_class(torch.nn.Module):
 
 
 class render_wrapper_class(torch.nn.Module):
-    """train.render with the wrapped models; every keyword (held_out, occupancy, early_termination, ...) is passed on.  An
-    occupancy grid and an early-termination threshold reach every rank whole: neither is a tensor or a tuple, so
-    RayShardedFunction does not shard them."""
+    """train.render with the wrapped models; every keyword (held_out, occupancy, early_termination, baked, ...) is passed
+    on.  An occupancy grid, an early-termination threshold and a baked scene reach every rank whole: none is a tensor or a
+    tuple, so RayShardedFunction does not shard them."""
 
     def __init__(self, coarse_model, fine_model=None, ray_bender=None):
         super().__init__()

@@ -78,7 +78,7 @@ def raw2outputs(raw, z_vals, rays_d, raw_noise_std=0, white_bkgd=False, pytest=F
 def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False, lindisp=False, perturb=0.0,
                 N_importance=0, network_fine=None, white_bkgd=False, raw_noise_std=0.0,
                 additional_pixel_information=None, detailed_output=False, verbose=False, pytest=False, held_out=None, occupancy=None,
-                early_termination=None, **dummy_kwargs):
+                early_termination=None, baked=None, **dummy_kwargs):
     """Volumetric rendering of a ray batch [N, 8] = (o, d, near, far).  `network_query_fn` is accepted
     for signature compatibility; the field is evaluated by the fused kernel on `network_fn` /
     `network_fine` (which carry their ray bender as `.ray_bender[0]`).
@@ -102,6 +102,11 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     the render without termination at the same depths, up to rounding, where T is the transmittance at which the ray
     died; the coarse weights of skipped samples are 0, so the fine depths follow a pdf within t of mass of the full one.
     t = 0 terminates nothing, nor does a NaN T.  None: every sample is evaluated (no termination_index keys).
+    baked (geometry.BakedScene, under torch.no_grad() only; the reference has no such option): the coarse pass samples
+    baked.coarse and the fine pass baked.fine (required when N_importance > 0) in place of the NeRF trunk for every sample
+    whose bent point is finite and inside the grid's box: raw is the grid's trilinear lookup there (raw[..., 4] = 0, the
+    object removal applied) and the trunk's raw elsewhere, so a box that holds no sample renders as without it.  Not
+    combined with occupancy or early_termination.  None: the trunk evaluates every sample.
     surface_normals=True (with surface_output=True) adds ret["surface_normals"] [N, 3]: the world-space unit normal
     geometry.normals_from_gradient(geometry.density_gradient(...)) of the pass's model, with the ray's latent code, at
     the frame-space point of the median-visibility sample (the point surface_pts and surface_rigidity are taken at).
@@ -123,6 +128,8 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     latents = None
     if network_fn.ray_bender[0] is not None or getattr(network_fn, "time_conditioned_baseline", False):
         latents = additional_pixel_information["ray_bending_latents"]
+    if baked is not None:
+        _check_baked(baked, network_fn, network_fine, N_importance, latents, occupancy, early_termination)
     if occupancy is not None:
         _check_occupancy(occupancy, network_fn, network_fine if N_importance > 0 else None, latents)
     if early_termination is not None:
@@ -130,6 +137,8 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     term_index = {}
 
     def field(net, z, noise, key):
+        if baked is not None:
+            return _ag.field_baked(net, rays, z, latents, detailed_output, baked.coarse if key == "coarse" else baked.fine)
         if early_termination is not None:
             raw, det, term_index[key] = _ag.field_terminate(net, rays, z, latents, detailed_output, early_termination, occupancy, noise)
             return raw, det
@@ -268,6 +277,22 @@ def _check_termination(early_termination, network_fn, network_fine, latents) -> 
     return t
 
 
+def _check_baked(baked, network_fn, network_fine, n_importance, latents, occupancy, early_termination):
+    """Before any launch: render(..., baked=scene) is refused for what it does not support (_ag.baked_check), with occupancy
+    or early_termination, and without a fine grid when N_importance > 0."""
+    from .geometry import BakedScene
+    if not isinstance(baked, BakedScene):
+        raise RuntimeError(f"nonrigid_nerf_b200: baked must be a geometry.BakedScene, got {type(baked).__name__}")
+    if occupancy is not None or early_termination is not None:
+        raise RuntimeError("nonrigid_nerf_b200: rendering from a baked radiance grid is not combined with occupancy or "
+                           "early_termination")
+    _ag.baked_check(network_fn, latents, baked.coarse)
+    if n_importance > 0:
+        if baked.fine is None:
+            raise RuntimeError("nonrigid_nerf_b200: N_importance > 0 needs a fine grid (BakedScene(coarse, fine))")
+        _ag.baked_check(network_fn if network_fine is None else network_fine, latents, baked.fine)
+
+
 # ---- batchify_rays / render (train.py:108-137, :326-416) --------------------------------------------
 def batchify_rays(rays_flat, additional_pixel_information, chunk=1024 * 32, detailed_output=False, **kwargs):
     """Render rays in chunks (`chunk` only bounds the per-launch working set; results do not depend on it)."""
@@ -286,8 +311,12 @@ def batchify_rays(rays_flat, additional_pixel_information, chunk=1024 * 32, deta
 def render(rays_o, rays_d, chunk=1024 * 32, ndc=True, near=0.0, far=1.0, use_viewdirs=False, c2w_staticcam=None,
            additional_pixel_information=None, detailed_output=False, **kwargs):
     """Render rays.  Returns [rgb_map, disp_map, acc_map, extras] (train.py:326-416).  Keyword held_out [N] (one entry
-    per ray of the flattened batch), keyword occupancy (a geometry.OccupancyGrid) and keyword early_termination (a float
-    in [0, 1]): see render_rays."""
+    per ray of the flattened batch), keyword occupancy (a geometry.OccupancyGrid), keyword early_termination (a float
+    in [0, 1]) and keyword baked (a geometry.BakedScene): see render_rays."""
+    if kwargs.get("network_fn") is not None and kwargs.get("baked") is not None:
+        _check_baked(kwargs["baked"], kwargs["network_fn"], kwargs.get("network_fine"), kwargs.get("N_importance", 0),
+                     (additional_pixel_information or {}).get("ray_bending_latents"), kwargs.get("occupancy"),
+                     kwargs.get("early_termination"))
     if kwargs.get("early_termination") is not None:
         t = _ag.termination_threshold(kwargs["early_termination"])
         if kwargs.get("network_fn") is not None:
