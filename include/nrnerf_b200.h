@@ -752,6 +752,44 @@ int nrn_radiance_plane_f16(const float* raw, long long n, int out_ch, void* plan
 size_t nrn_baked_workspace_bytes(int n_rays, int n_samples, int out_ch, int has_bender);
 int nrn_field_forward_baked(const NrnFieldArgs* args, const NrnRadianceGrid* grid, void* workspace, size_t workspace_bytes);
 
+/* ---- baked per-frame deformation grids: render passes that look each sample's bend up in place of the ray bender -------
+ * The ray bender (run_nerf_helpers.py:507-584) maps a sample x of a frame with latent z to x + s r~(x) o(x, z): o the
+ * offset MLP on [x, z] (:523-541), r the rigidity MLP on x (:545-561), r~ = 0 where r <= the cut-off (:563-564), s the
+ * test-time scaling (:568-569).  A deformation grid holds, for each of n_frames frames, o and r at the same vertices as an
+ * NrnRadianceGrid (nrn_mesh_grid_points), as fp16 at values[(((f * nz + k) * ny + j) * nx + i) * 4 + c]: c = 0..2 the
+ * unmasked offset, c = 3 the rigidity, both evaluated with every test-time knob off.
+ *
+ * nrn_deformation_plane_f16: plane [n][4] fp16 (8-byte aligned) <- (offsets [n][3], rigidity [n]), with
+ *   nrn_radiance_plane_f16's rounding.  The bake's store: one call per frame and z-plane on the unmasked_offsets and
+ *   rigidity_mask of a point-mode bend pass (nrn_field_forward_views with raw NULL) at that plane's nrn_mesh_grid_points.
+ * nrn_field_forward_deformed: one inference pass of nrn_field_forward_baked (args as there, with a bender) that takes the
+ *   bends of frame `frame` from the deformation grid, per ray:
+ *   - a ray whose every sample x = rays_o + rays_d * z is finite and inside the deformation grid's box is DEFORMED: (o, r)
+ *     by NrnRadianceGrid's lookup rule, then, each operation an fp32 one rounded on its own, r~ = (use_cutoff && r <=
+ *     cutoff) ? 0 : r, m = r~ o, m = m * scaling (use_scaling), c = x + m.  Details: initial_input_pts x, input_pts c,
+ *     unmasked_offsets o, masked_offsets m, rigidity_mask r~.
+ *   - any other ray FALLS BACK: its samples are bent by the bend pass with the ray's latent, so its raw and details equal
+ *     nrn_field_forward_baked's bit for bit.  The rule is per ray, so a result does not depend on how rays are batched.
+ *   Then raw = the radiance grid's lookup at c where that is inside its box, the trunk's raw at c elsewhere, and the object
+ *   removal zeroes raw[3] where r~ >= removal_threshold, all as nrn_field_forward_baked.  The fallback rays are compacted
+ *   in ascending order with their count on the device: no host synchronisation, CUDA-graph capturable.  Replaces the bend
+ *   pass of the render (run_nerf_helpers.py:507-584 on every sample) for the deformed rays.  workspace:
+ *   nrn_deformed_workspace_bytes(n_rays, n_samples, out_ch, with_details), with_details nonzero when any detail pointer is
+ *   given; 256-byte aligned.  A null, misaligned or malformed grid, a frame out of range, no bender, more than 2^31 - 1
+ *   points or a short workspace return NRN_E_INVALID before any CUDA call. */
+typedef struct NrnDeformGrid {
+  const void* values;           /* [n_frames][nz][ny][nx][4] fp16, 8-byte aligned */
+  int32_t nx, ny, nz;           /* vertices per axis, 2..1024 */
+  float min_point[3];
+  float max_point[3];
+  int32_t n_frames;
+  int32_t frame;                /* the frame whose slab the pass reads, 0..n_frames - 1 */
+} NrnDeformGrid;
+int nrn_deformation_plane_f16(const float* offsets, const float* rigidity, long long n, void* plane, void* stream);
+size_t nrn_deformed_workspace_bytes(int n_rays, int n_samples, int out_ch, int with_details);
+int nrn_field_forward_deformed(const NrnFieldArgs* args, const NrnRadianceGrid* grid, const NrnDeformGrid* deform, void* workspace,
+                               size_t workspace_bytes);
+
 /* ---- the inverse of the ray bender: canonical points into every frame (geometry.deform_points) -------------------------
  * The ray bender maps an observed point x of a frame with latent z to the canonical point c = b(x; z) = x + s r~(x) o(x, z)
  * (run_nerf_helpers.py:507-584: o the offset MLP on [x, z], r = (tanh(rho(x)) + 1) / 2 the rigidity, r~ = 0 where
@@ -839,7 +877,10 @@ int nrn_field_density_gradient(const NrnDensityGradArgs* args);
  * biases) and 43 the DGRAD, 44 the upsampling of nrn_lpips_maps (its other kernels are kinds 25 to 28, the distances
  * with their tap maps kind 28), 45 nrn_radiance_plane_f16, and of nrn_field_forward_baked 46 the bend pass with the
  * lookup (without a bender the lookup alone), 47 the compaction of the other samples, 48 the trunk on them and 49 the
- * scatter.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
+ * scatter, 50 nrn_deformation_plane_f16, and of nrn_field_forward_deformed 51 the per-ray lookup of the bends (with the
+ * radiance lookup of the deformed rays' samples), 52 the compaction and gather of the fallback rays, 53 their bend pass, 54
+ * its scatter (with the radiance lookup of their samples), 55 the compaction of the samples outside the radiance grid's box,
+ * 56 the trunk on them and 57 their scatter.  nrn_timing_read synchronises the recorded events and returns per-kind sums.
  * nrn_timing_enable(0) stops recording and keeps the events; nrn_timing_enable(1) releases the previous session's events,
  * so a CUDA graph captured during that session must be released before timing is enabled again. */
 int nrn_timing_enable(int on);

@@ -201,6 +201,13 @@ class NrnRadianceGrid(C.Structure):
     ]
 
 
+class NrnDeformGrid(C.Structure):
+    _fields_ = [
+        ("values", _vp), ("nx", C.c_int32), ("ny", C.c_int32), ("nz", C.c_int32),
+        ("min_point", C.c_float * 3), ("max_point", C.c_float * 3), ("n_frames", C.c_int32), ("frame", C.c_int32),
+    ]
+
+
 class NrnOccupancyGrid(C.Structure):
     _fields_ = [
         ("bits", _vp), ("nx", C.c_int32), ("ny", C.c_int32), ("nz", C.c_int32),
@@ -336,6 +343,10 @@ SYMBOLS = {
     "nrn_radiance_plane_f16": (C.c_int, [_vp, C.c_longlong, C.c_int, _vp, _vp]),
     "nrn_baked_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
     "nrn_field_forward_baked": (C.c_int, [C.POINTER(NrnFieldArgs), C.POINTER(NrnRadianceGrid), _vp, C.c_size_t]),
+    "nrn_deformation_plane_f16": (C.c_int, [_vp, _vp, C.c_longlong, _vp, _vp]),
+    "nrn_deformed_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
+    "nrn_field_forward_deformed": (C.c_int, [C.POINTER(NrnFieldArgs), C.POINTER(NrnRadianceGrid), C.POINTER(NrnDeformGrid), _vp,
+                                             C.c_size_t]),
     "nrn_deform_points": (C.c_int, [C.POINTER(NrnDeformArgs)]),
     "nrn_density_gradient_chunk": (C.c_int64, []),
     "nrn_density_gradient_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
@@ -382,6 +393,11 @@ LPIPS_MAP_KERNEL_KINDS = ("lpips_upsample",)
 # baked radiance grids (the bake's fp16 plane store; of a render pass: bend pass + lookup, compaction of the other samples,
 # trunk on them, scatter), timing kinds 45 to 49
 BAKED_KERNEL_KINDS = ("baked_plane", "baked_bend", "baked_compact", "baked_field", "baked_scatter")
+# baked deformation grids (the bake's fp16 plane store; of a render pass: the per-ray bend lookup, the fallback rays'
+# compaction + gather, their bend pass, its scatter, and the radiance grid's compaction, trunk and scatter), timing kinds 50
+# to 57
+DEFORMATION_KERNEL_KINDS = ("deformation_plane", "deformed_rays", "deformed_fallback", "deformed_bend", "deformed_bend_scatter",
+                            "deformed_compact", "deformed_field", "deformed_scatter")
 
 
 def timing_enable(on: bool) -> None:
@@ -393,7 +409,7 @@ def timing_read(kinds=KERNEL_KINDS):
     KERNEL_KINDS + TC_KERNEL_KINDS, KERNEL_KINDS + TC_KERNEL_KINDS + VIEW_KERNEL_KINDS, that + VIEW_TRAIN_KERNEL_KINDS,
     that + DET_KERNEL_KINDS, that + HELD_OUT_KERNEL_KINDS, that + EVAL_KERNEL_KINDS, that + FRAME_IMAGE_KERNEL_KINDS, that + MESH_KERNEL_KINDS, that + LPIPS_KERNEL_KINDS, that + MATCH_KERNEL_KINDS, that
     + OCCUPANCY_KERNEL_KINDS, that + TERMINATION_KERNEL_KINDS, that + DEFORM_KERNEL_KINDS, that + NORMAL_KERNEL_KINDS,
-    that + LPIPS_MAP_KERNEL_KINDS or that + BAKED_KERNEL_KINDS."""
+    that + LPIPS_MAP_KERNEL_KINDS, that + BAKED_KERNEL_KINDS or that + DEFORMATION_KERNEL_KINDS."""
     n = len(kinds)
     ms = (C.c_double * n)()
     cnt = (C.c_int * n)()

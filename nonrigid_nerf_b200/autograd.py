@@ -730,14 +730,32 @@ def baked_check(net, latents, grid) -> None:
                            "torch.no_grad() (the grid carries no gradient)")
 
 
-def field_baked(net, rays, z_vals, latents, want_details, grid):
-    """field_rays that samples the radiance grid in place of the NeRF trunk for samples inside its box."""
+def deformation_check(net, deformation) -> None:
+    """Raise, before any launch, unless `deformation` is a geometry.FrameDeformation that a pass of `net` can read: the model
+    has a ray bender, and the grid is well formed and on the model's device."""
+    from .geometry import FrameDeformation
+    if not isinstance(deformation, FrameDeformation):
+        raise RuntimeError(f"nonrigid_nerf_b200: a baked deformation must be a geometry.FrameDeformation (DeformationGrid.frame(i)), got "
+                           f"{type(deformation).__name__}")
+    if net.ray_bender[0] is None:
+        raise RuntimeError("nonrigid_nerf_b200: a baked deformation needs a model with a ray bender (its rays that leave the grid are "
+                           "bent by it)")
+    deformation.c_struct(net.output_linear.weight.device)
+
+
+def field_baked(net, rays, z_vals, latents, want_details, grid, deformation=None):
+    """field_rays that samples the radiance grid in place of the NeRF trunk for samples inside its box; with `deformation`
+    (geometry.FrameDeformation) the bends of the rays inside its box come from that grid in place of the ray bender."""
     baked_check(net, latents, grid)
     bender = net.ray_bender[0]
     cutoff, scaling, removal = _knobs(net)
     nerf_pack = ops.pack_nerf(net)
     bender_pack = ops.pack_bender(bender) if bender is not None else None
     out_ch = net.output_linear.weight.shape[0]
+    if deformation is not None:
+        deformation_check(net, deformation)
+        return ops.field_forward_deformed(rays, z_vals, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details,
+                                          grid, deformation)
     return ops.field_forward_baked(rays, z_vals, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details, grid)
 
 

@@ -1,5 +1,6 @@
 // Baked canonical radiance grids (baked.cu, field_fwd.cu's field_baked_kernel): the fp16 store of a bake's planes and the
-// trilinear lookup a render pass runs in place of the NeRF trunk for samples inside the grid's box.
+// trilinear lookup a render pass runs in place of the NeRF trunk for samples inside the grid's box.  Baked per-frame
+// deformation grids store the ray bender's (offset, rigidity) the same way and are looked up by the same rule.
 //
 // A grid has n[0] x n[1] x n[2] vertices over [lo, hi]; vertex (i, j, k) holds the 4 raw channels of the canonical model at
 // the mesh grid's point (i, j, k) (mesh.cu's grid_coord), as fp16 at vox[(k * ny + j) * nx + i]: one 8-byte load per corner.
@@ -78,5 +79,54 @@ cudaError_t launch_baked_plane(const float* raw, long long n, int out_ch, uint2*
 // Without a bender: raw of every sample of rays x z inside the grid's box, at rays_o + rays_d * z (the field kernel's rounding)
 cudaError_t launch_baked_rays(const BakedGrid& g, const float* rays, const float* z_vals, int S, long long P, float* raw, int out_ch,
                               cudaStream_t st);
+
+// ---- baked per-frame deformation grids (c_abi.cu: nrn_field_forward_deformed) ----
+// One frame's grid is a BakedGrid whose 4 channels are the bender's unmasked offset o (0..2) and rigidity r (3), looked up
+// with baked_lookup.  A ray is DEFORMED when every one of its samples x = o + d z is finite and inside the grid's box; then
+// per sample r~ = (use_cutoff && r <= cutoff) ? 0 : r, m = fl(r~ o), m = fl(m s) with scaling, c = fl(x + m).  Any other ray
+// FALLS BACK: the bend pass bends it exactly, so its samples come out as the baked pass without a deformation grid.
+
+// The per-sample outputs of a deformed pass: the bend workspace (c, r~) as the bend pass writes it, raw of the samples whose
+// c the radiance grid looks up, and the details (each may be null)
+struct DeformOut {
+  float4* ws;
+  float* raw;
+  int out_ch;
+  float* d_init;
+  float* d_bent;
+  float* d_unmasked;
+  float* d_masked;
+  float* d_rigid;
+};
+
+struct DeformKnobs {
+  int use_cutoff, use_scaling, use_removal;
+  float cutoff, scaling, removal;
+};
+
+// The fallback rays, compacted in ascending order: their count K (device memory), their indices, and their rays [K][8],
+// depths [K][S] and latent rows [K][32] gathered for the bend pass
+struct DeformFallback {
+  uint8_t* flag;           // [n_rays] 1: the ray falls back
+  int32_t* block_counts;   // ceil(n_rays / kOccTile) + 1
+  int32_t* count;
+  int32_t* idx;
+  float* rays;
+  float* z_vals;
+  float* latents;
+};
+
+// plane [n] x 4 fp16 <- baked_half of (offsets [n][3], rigidity [n])
+cudaError_t launch_deform_plane(const float* offsets, const float* rigidity, long long n, uint2* plane, cudaStream_t st);
+// A warp per ray: the vote, and for a deformed ray every sample's c and r~ -> o.ws, the details, and raw where rg looks c up
+cudaError_t launch_deform_rays(const BakedGrid& dg, const BakedGrid& rg, const DeformKnobs& k, const float* rays, const float* z_vals,
+                               int n_rays, int S, const DeformOut& o, uint8_t* fallback, cudaStream_t st);
+// The fallback rays in ascending order (count, indices), and their rays, depths and latent rows gathered
+cudaError_t launch_deform_fallback(const DeformFallback& f, const float* rays, const float* z_vals, const float* latents,
+                                   long long latent_stride, int n_rays, int S, int num_sms, cudaStream_t st);
+// The bend pass's outputs over the gathered rays (bend workspace bw, details of `from`) back to the fallback rays' samples of
+// `to`, and raw where rg looks their bent points up (the object removal as the bend pass with the lookup applies it)
+cudaError_t launch_deform_scatter(const BakedGrid& rg, const DeformKnobs& k, const DeformFallback& f, const float4* bw, const DeformOut& from,
+                                  int n_rays, int S, const DeformOut& to, int num_sms, cudaStream_t st);
 
 }  // namespace nrn

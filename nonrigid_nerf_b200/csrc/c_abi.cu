@@ -39,6 +39,7 @@ cudaError_t launch_field_views_train(const FieldFwdParams& p, const ViewParams& 
 cudaError_t launch_field_bwd_views(const FieldBwdParams& p, const ViewBwdParams& v, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_fwd_kept(const FieldFwdParams& p, const int* kept, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_baked(const FieldFwdParams& p, const ViewParams& v, const BakedGrid& g, int num_sms, cudaStream_t stream);
+cudaError_t launch_field_bend_rays(const FieldFwdParams& p, const ViewParams& v, const int* n_rays, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_fwd_grad(const FieldFwdParams& p, bool has_bender, int num_sms, cudaStream_t stream);
 cudaError_t launch_field_bwd_grad(const FieldBwdParams& p, const PointGradParams& pg, bool has_bender, int num_sms, cudaStream_t stream);
 }
@@ -1694,6 +1695,9 @@ size_t nrn_baked_workspace_bytes(int n_rays, int n_samples, int out_ch, int has_
   return occ ? occ + align256(sizeof(uint32_t)) : 0;
 }
 
+static int baked_others(const NrnFieldArgs* a, const nrn::BakedGrid& bg, const nrn::FieldFwdParams& p0, const float4* ws, uint8_t* w,
+                        DeviceState* ds, int kind, cudaStream_t st);
+
 int nrn_field_forward_baked(const NrnFieldArgs* a, const NrnRadianceGrid* grid, void* workspace, size_t workspace_bytes) {
   const char* who = "nrn_field_forward_baked";
   long long P;
@@ -1716,18 +1720,10 @@ int nrn_field_forward_baked(const NrnFieldArgs* a, const NrnRadianceGrid* grid, 
   rc = device_state(&ds);
   if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(a->stream);
-  const size_t p = static_cast<size_t>(P);
   uint8_t* w = static_cast<uint8_t*>(workspace);
   float4* ws = nullptr;
-  if (bend) { ws = reinterpret_cast<float4*>(w); w += align256(p * sizeof(float4)); }
-  float* kept_xyz = reinterpret_cast<float*>(w); w += align256(p * 3 * sizeof(float));
-  int32_t* kept_idx = reinterpret_cast<int32_t*>(w); w += align256(p * sizeof(int32_t));
-  float* craw = reinterpret_cast<float*>(w); w += align256(p * a->out_ch * sizeof(float));
-  int32_t* count = reinterpret_cast<int32_t*>(w); w += align256(sizeof(int32_t));
-  int32_t* block_counts = reinterpret_cast<int32_t*>(w); w += occ_block_count_bytes(P);
-  uint32_t* empty = reinterpret_cast<uint32_t*>(w);
-
-  nrn::FieldFwdParams p0 = field_fwd_params(a, P, tiles, ds->err_word);
+  if (bend) { ws = reinterpret_cast<float4*>(w); w += align256(static_cast<size_t>(P) * sizeof(float4)); }
+  const nrn::FieldFwdParams p0 = field_fwd_params(a, P, tiles, ds->err_word);
   // a. raw of the samples inside the grid's box: with a bender from the bend pass's epilogue (which also writes the bent
   //    points and rigidities to ws, and the details), without one at rays_o + rays_d * z
   if (bend) {
@@ -1740,6 +1736,22 @@ int nrn_field_forward_baked(const NrnFieldArgs* a, const NrnRadianceGrid* grid, 
     });
   }
   if (rc) return rc;
+  return baked_others(a, bg, p0, ws, w, ds, 47, st);
+}
+
+// Steps b to d of a baked pass, after the samples inside the radiance grid's box have their raw: the other samples (their
+// points in ws, or without one at rays_o + rays_d * z) through the trunk, timed as kinds kind .. kind + 2.  w: the
+// workspace past ws, in nrn_baked_workspace_bytes's layout.
+static int baked_others(const NrnFieldArgs* a, const nrn::BakedGrid& bg, const nrn::FieldFwdParams& p0, const float4* ws, uint8_t* w,
+                        DeviceState* ds, int kind, cudaStream_t st) {
+  const long long P = p0.P;
+  const size_t p = static_cast<size_t>(P);
+  float* kept_xyz = reinterpret_cast<float*>(w); w += align256(p * 3 * sizeof(float));
+  int32_t* kept_idx = reinterpret_cast<int32_t*>(w); w += align256(p * sizeof(int32_t));
+  float* craw = reinterpret_cast<float*>(w); w += align256(p * a->out_ch * sizeof(float));
+  int32_t* count = reinterpret_cast<int32_t*>(w); w += align256(sizeof(int32_t));
+  int32_t* block_counts = reinterpret_cast<int32_t*>(w); w += occ_block_count_bytes(P);
+  uint32_t* empty = reinterpret_cast<uint32_t*>(w);
   // b. the samples outside the box or not finite, compacted in order: exactly those an occupancy grid of one empty cell
   //    over the same box keeps (without a bender this step also writes the details)
   nrn::OccGrid og{};
@@ -1749,23 +1761,148 @@ int nrn_field_forward_baked(const NrnFieldArgs* a, const NrnRadianceGrid* grid, 
   s.ws = ws; s.rays = a->rays; s.z_vals = a->z_vals; s.S = a->n_samples; s.P = P;
   nrn::OccCompact c{};
   c.kept_xyz = kept_xyz; c.kept_idx = kept_idx; c.count = count; c.block_counts = block_counts;
-  if (!bend) { c.d_init = a->initial_input_pts; c.d_bent = a->input_pts; }
-  rc = timed(47, st, "occupancy_compact", [&] {
+  if (!ws) { c.d_init = a->initial_input_pts; c.d_bent = a->input_pts; }
+  int rc = timed(kind, st, "occupancy_compact", [&] {
     const cudaError_t e = cudaMemsetAsync(empty, 0, sizeof(uint32_t), st);
     return e != cudaSuccess ? e : nrn::launch_occupancy_compact(og, s, c, st);
   });
   if (rc) return rc;
   // c. the point-mode trunk on them, their count read on the device
   nrn::FieldFwdParams q{};
-  q.pts = kept_xyz; q.pts_stride = 3; q.n_rays = static_cast<int>(P); q.S = 1; q.P = P; q.n_tiles = tiles;
+  q.pts = kept_xyz; q.pts_stride = 3; q.n_rays = static_cast<int>(P); q.S = 1; q.P = P; q.n_tiles = p0.n_tiles;
   q.nerf_w = p0.nerf_w; q.nerf_bias = p0.nerf_bias; q.out_ch = a->out_ch; q.raw = craw; q.err = ds->err_word;
-  rc = timed(48, st, "field_fwd_kept_kernel", [&] { return nrn::launch_field_fwd_kept(q, count, ds->num_sms, st); });
+  rc = timed(kind + 1, st, "field_fwd_kept_kernel", [&] { return nrn::launch_field_fwd_kept(q, count, ds->num_sms, st); });
   if (rc) return rc;
   // d. their raw into the pass's output (with the object removal), beside the grid's
-  return timed(49, st, "occ_scatter_kernel", [&] {
+  return timed(kind + 2, st, "occ_scatter_kernel", [&] {
     return nrn::launch_termination_scatter(craw, kept_idx, count, P, a->out_ch, ws, a->use_removal, a->removal_threshold, a->raw,
                                            ds->num_sms, st);
   });
+}
+
+// ---- baked per-frame deformation grids: the bake's plane store, and the render pass that looks each sample's bend up ----
+int nrn_deformation_plane_f16(const float* offsets, const float* rigidity, long long n, void* plane, void* stream) {
+  const char* who = "nrn_deformation_plane_f16";
+  if (n < 0 || n > (1LL << 40)) return fail(NRN_E_INVALID, "%s: bad size n=%lld", who, n);
+  if (n == 0) return NRN_OK;
+  if (!offsets || !rigidity || !plane) return fail(NRN_E_INVALID, "%s: null argument", who);
+  if (!aligned4(offsets) || !aligned4(rigidity) || (reinterpret_cast<uintptr_t>(plane) & 7u))
+    return fail(NRN_E_INVALID, "%s: offsets and rigidity must be 4-byte and plane 8-byte aligned", who);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return timed(50, st, "deform_plane_kernel", [&] {
+    return nrn::launch_deform_plane(offsets, rigidity, n, static_cast<uint2*>(plane), st);
+  });
+}
+
+// Frame `frame`'s grid as the kernels read it; NRN_E_INVALID for a malformed grid or a frame out of range
+static int deform_grid(const NrnDeformGrid* g, const char* who, nrn::BakedGrid* out) {
+  if (!g) return fail(NRN_E_INVALID, "%s: null", who);
+  if (g->n_frames < 1 || g->frame < 0 || g->frame >= g->n_frames)
+    return fail(NRN_E_INVALID, "%s: frame %d out of range (%d frames)", who, g->frame, g->n_frames);
+  NrnRadianceGrid r{};
+  r.values = g->values; r.nx = g->nx; r.ny = g->ny; r.nz = g->nz;
+  for (int d = 0; d < 3; ++d) { r.min_point[d] = g->min_point[d]; r.max_point[d] = g->max_point[d]; }
+  const int rc = baked_grid(&r, who, out);
+  if (rc) return rc;
+  out->vox += static_cast<long long>(g->frame) * g->nx * g->ny * g->nz;   // frame f's slab
+  return NRN_OK;
+}
+
+// nrn_baked_workspace_bytes's layout with a bender, then the fallback rays' flags, block counts, count, indices, rays,
+// latent rows and depths, the bend workspace over them and, with_details, their details
+size_t nrn_deformed_workspace_bytes(int n_rays, int n_samples, int out_ch, int with_details) {
+  const size_t baked = nrn_baked_workspace_bytes(n_rays, n_samples, out_ch, 1);
+  if (!baked) return 0;
+  const size_t n = static_cast<size_t>(n_rays), p = n * static_cast<size_t>(n_samples);
+  return baked + align256(n) + occ_block_count_bytes(n_rays) + align256(sizeof(int32_t)) + align256(n * sizeof(int32_t)) +
+         align256(n * 8 * sizeof(float)) + align256(n * nrn::kLatent * sizeof(float)) + align256(p * sizeof(float)) +
+         align256(p * sizeof(float4)) + (with_details ? 4 * align256(p * 3 * sizeof(float)) + align256(p * sizeof(float)) : 0);
+}
+
+int nrn_field_forward_deformed(const NrnFieldArgs* a, const NrnRadianceGrid* grid, const NrnDeformGrid* deform, void* workspace,
+                               size_t workspace_bytes) {
+  const char* who = "nrn_field_forward_deformed";
+  long long P;
+  int tiles;
+  int rc = check_field_args(a, who, &P, &tiles);
+  if (rc) return rc;
+  if (a->stash || a->relu_mask) return fail(NRN_E_INVALID, "%s: inference only (stash / relu_mask must be NULL)", who);
+  if (a->points) return fail(NRN_E_INVALID, "%s: needs ray mode (rays and z_vals; points must be NULL)", who);
+  nrn::BakedGrid bg, dg;
+  rc = baked_grid(grid, who, &bg);
+  if (rc) return rc;
+  rc = deform_grid(deform, "nrn_field_forward_deformed: deformation grid", &dg);
+  if (rc) return rc;
+  if (P > nrn::kOccMaxPoints) return fail(NRN_E_INVALID, "%s: %lld points in one pass (at most 2^31 - 1)", who, P);
+  if (P == 0) return NRN_OK;
+  if (!a->bender_packed) return fail(NRN_E_INVALID, "%s: a deformation grid needs the ray bender (bender_packed, for the rays that fall back)", who);
+  if (!a->raw) return fail(NRN_E_INVALID, "%s: null raw", who);
+  if (!aligned4(a->rays) || !aligned4(a->z_vals) || !aligned4(a->latents) || !aligned4(a->raw))
+    return fail(NRN_E_INVALID, "%s: rays, z_vals, latents and raw must be 4-byte aligned", who);
+  const bool det = a->initial_input_pts || a->input_pts || a->unmasked_offsets || a->masked_offsets || a->rigidity_mask;
+  const size_t need = nrn_deformed_workspace_bytes(a->n_rays, a->n_samples, a->out_ch, det);
+  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255u) || workspace_bytes < need)
+    return fail(NRN_E_INVALID, "%s: workspace null, not 256-byte aligned or smaller than nrn_deformed_workspace_bytes (%zu)", who, need);
+  DeviceState* ds;
+  rc = device_state(&ds);
+  if (rc) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  const int n = a->n_rays, S = a->n_samples;
+  const size_t p = static_cast<size_t>(P);
+  uint8_t* w = static_cast<uint8_t*>(workspace);
+  float4* ws = reinterpret_cast<float4*>(w);
+  uint8_t* rest = w + align256(p * sizeof(float4));   // baked_others' part
+  w += nrn_baked_workspace_bytes(n, S, a->out_ch, 1);
+  nrn::DeformFallback f{};
+  f.flag = w; w += align256(static_cast<size_t>(n));
+  f.block_counts = reinterpret_cast<int32_t*>(w); w += occ_block_count_bytes(n);
+  f.count = reinterpret_cast<int32_t*>(w); w += align256(sizeof(int32_t));
+  f.idx = reinterpret_cast<int32_t*>(w); w += align256(static_cast<size_t>(n) * sizeof(int32_t));
+  f.rays = reinterpret_cast<float*>(w); w += align256(static_cast<size_t>(n) * 8 * sizeof(float));
+  f.latents = reinterpret_cast<float*>(w); w += align256(static_cast<size_t>(n) * nrn::kLatent * sizeof(float));
+  f.z_vals = reinterpret_cast<float*>(w); w += align256(p * sizeof(float));
+  float4* bw = reinterpret_cast<float4*>(w); w += align256(p * sizeof(float4));
+  nrn::DeformOut out{ws, a->raw, a->out_ch, a->initial_input_pts, a->input_pts, a->unmasked_offsets, a->masked_offsets, a->rigidity_mask};
+  nrn::DeformOut gathered{bw, nullptr, a->out_ch, nullptr, nullptr, nullptr, nullptr, nullptr};   // the bend pass's, per gathered sample
+  float** gd[4] = {&gathered.d_init, &gathered.d_bent, &gathered.d_unmasked, &gathered.d_masked};
+  float* const od[4] = {out.d_init, out.d_bent, out.d_unmasked, out.d_masked};
+  for (int i = 0; i < 4; ++i) {
+    if (det && od[i]) *gd[i] = reinterpret_cast<float*>(w);
+    if (det) w += align256(p * 3 * sizeof(float));
+  }
+  if (det && out.d_rigid) gathered.d_rigid = reinterpret_cast<float*>(w);
+  nrn::DeformKnobs k{};
+  k.use_cutoff = a->use_cutoff; k.cutoff = a->rigidity_cutoff; k.use_scaling = a->use_scaling; k.scaling = a->scaling;
+  k.use_removal = a->use_removal; k.removal = a->removal_threshold;
+
+  const nrn::FieldFwdParams p0 = field_fwd_params(a, P, tiles, ds->err_word);
+  // a. per ray: inside the deformation grid's box, every sample's bend from the grid (-> ws, details, raw where the
+  //    radiance grid looks its point up); otherwise flagged
+  rc = timed(51, st, "deform_rays_kernel", [&] {
+    return nrn::launch_deform_rays(dg, bg, k, a->rays, a->z_vals, n, S, out, f.flag, st);
+  });
+  if (rc) return rc;
+  // b. the flagged rays compacted in ascending order, their count on the device, and their rays, depths and latents gathered
+  rc = timed(52, st, "deform_fallback", [&] {
+    return nrn::launch_deform_fallback(f, a->rays, a->z_vals, a->latents, a->latent_stride, n, S, ds->num_sms, st);
+  });
+  if (rc) return rc;
+  // c. the exact bend pass on them
+  nrn::FieldFwdParams b = p0;
+  b.rays = f.rays; b.z_vals = f.z_vals; b.latents = f.latents; b.latent_stride = nrn::kLatent;
+  b.raw = nullptr; b.d_init = gathered.d_init; b.d_bent = gathered.d_bent; b.d_unmasked = gathered.d_unmasked;
+  b.d_masked = gathered.d_masked; b.d_rigid = gathered.d_rigid;
+  nrn::ViewParams vp{};
+  vp.ws = bw;
+  rc = timed(53, st, "field_bend_rays_kernel", [&] { return nrn::launch_field_bend_rays(b, vp, f.count, ds->num_sms, st); });
+  if (rc) return rc;
+  // d. its outputs back to their samples, and raw where the radiance grid looks their bent points up
+  rc = timed(54, st, "deform_scatter_kernel", [&] {
+    return nrn::launch_deform_scatter(bg, k, f, bw, gathered, n, S, out, ds->num_sms, st);
+  });
+  if (rc) return rc;
+  // e. the samples outside the radiance grid's box through the trunk, as the baked pass runs them
+  return baked_others(a, bg, p0, ws, rest, ds, 55, st);
 }
 
 // ---- the inverse of the ray bender ----

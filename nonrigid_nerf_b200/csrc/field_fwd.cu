@@ -29,7 +29,9 @@
 //            stash (direction encoding, feature, hv) and hv's mask bits for field_bwd_views_kernel.
 //
 // Baked radiance grid (render(..., baked=)): the bend pass that also looks every bent point up in the grid (baked.cuh)
-// and writes raw of the points inside its box; the trunk runs afterwards on the others alone (c_abi.cu).
+// and writes raw of the points inside its box; the trunk runs afterwards on the others alone (c_abi.cu).  With a baked
+// deformation grid as well, the bend pass runs only on the rays that fall back to the exact bender, gathered, with their
+// count read on the device.
 #include "baked.cuh"
 #include "field_mma.cuh"
 
@@ -516,6 +518,14 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_kept_kernel(FieldFwd
   p.n_tiles = static_cast<int>((p.P + kTileM - 1) / kTileM);
   field_fwd_body<false, false, false>(p);
 }
+// The bend pass over rays whose count is read from device memory (the fallback rays of a pass with a baked deformation
+// grid, baked.cu): no host synchronisation, so such a pass can be captured in a CUDA graph
+__global__ void __launch_bounds__(kFwdThreads, 1) field_bend_rays_kernel(FieldFwdParams p, const ViewParams v, const int* __restrict__ n_rays) {
+  p.n_rays = *n_rays;
+  p.P = static_cast<long long>(p.n_rays) * p.S;
+  p.n_tiles = static_cast<int>((p.P + kTileM - 1) / kTileM);
+  field_fwd_body<true, false, false, kBend>(p, v);
+}
 __global__ void __launch_bounds__(kFwdThreads, 1) field_views_train_kernel(const FieldFwdParams p, const ViewParams v, const ViewTrainParams t) {
   field_fwd_body<false, true, false, kViews>(p, v, t);
 }
@@ -576,6 +586,11 @@ cudaError_t launch_field_bend(const FieldFwdParams& p, const ViewParams& v, int 
 // The bend pass with the baked grid's lookup: v.ws as launch_field_bend writes it, and p.raw of the points inside g's box
 cudaError_t launch_field_baked(const FieldFwdParams& p, const ViewParams& v, const BakedGrid& g, int num_sms, cudaStream_t stream) {
   return launch_field(field_baked_kernel, p, num_sms, field_fwd_smem_bytes(), stream, v, g);
+}
+
+// p.n_rays (and p.P, p.n_tiles) bound the ray count: they size the grid; the kernel takes the count itself from `n_rays`
+cudaError_t launch_field_bend_rays(const FieldFwdParams& p, const ViewParams& v, const int* n_rays, int num_sms, cudaStream_t stream) {
+  return launch_field(field_bend_rays_kernel, p, num_sms, field_fwd_smem_bytes(), stream, v, n_rays);
 }
 
 cudaError_t launch_field_views(const FieldFwdParams& p, const ViewParams& v, int num_sms, cudaStream_t stream) {

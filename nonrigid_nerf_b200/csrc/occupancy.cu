@@ -284,6 +284,11 @@ cudaError_t launch_occupancy_scatter(const float* compact_raw, const int32_t* ke
   return launch_termination_scatter(compact_raw, kept_idx, count, P, out_ch, ws, use_removal, removal, raw, num_sms, st);
 }
 
+cudaError_t launch_occupancy_scan(int32_t* counts, int n, int32_t* count, cudaStream_t st) {
+  occ_scan_kernel<<<1, kOccTile, 0, st>>>(counts, n, count);
+  return cudaGetLastError();
+}
+
 cudaError_t launch_termination_init(const TermPass& t, cudaStream_t st) {
   term_init_kernel<<<blocks_for(t.n, kOccThreads), kOccThreads, 0, st>>>(t);
   return cudaGetLastError();

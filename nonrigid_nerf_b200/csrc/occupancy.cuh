@@ -83,6 +83,9 @@ cudaError_t launch_occupancy_compact(const OccGrid& g, const OccPoints& pts, con
 // the point's rigidity >= removal (the fused kernel's test-time object removal)
 cudaError_t launch_occupancy_scatter(const float* compact_raw, const int32_t* kept_idx, const int32_t* count, long long P, int out_ch,
                                      const float4* ws, int use_removal, float removal, float* raw, int num_sms, cudaStream_t st);
+// The exclusive scan of n per-block counts in place (one block), the total -> counts[n] and *count: the middle step of the
+// compaction above, for other per-block counts (baked.cu's fallback rays)
+cudaError_t launch_occupancy_scan(int32_t* counts, int n, int32_t* count, cudaStream_t st);
 
 // Early termination (nrn_field_forward_terminate).  init: T = 1 and term = S for every ray.  compact: the lookup and
 // compaction of one segment's slots (kept indices are the samples' indices in the pass, so the scatter takes them as they

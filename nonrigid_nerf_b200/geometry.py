@@ -365,20 +365,82 @@ class RadianceGrid:
 
 
 @dataclasses.dataclass(frozen=True, eq=False)
+class DeformationGrid:
+    """The ray bender baked per frame by bake_deformation: F frames of nx * ny * nz vertices over [min_point, max_point];
+    values[f, k, j, i] holds, as fp16, the bender's unmasked offset (channels 0..2) and rigidity (channel 3) at
+    density_grid's point (i, j, k) with latent code latents[f], every test-time knob off.  frame(i) is what a render of
+    frame i reads (BakedScene.deformation)."""
+    values: torch.Tensor               # [F, nz, ny, nx, 4] fp16 on the bender's device
+    min_point: np.ndarray              # [3] float32
+    max_point: np.ndarray              # [3] float32
+    resolution: Tuple[int, int, int]   # (nx, ny, nz) vertices
+    latents: torch.Tensor              # [F, 32] fp32: the latent code of each frame
+
+    @property
+    def n_frames(self) -> int:
+        return int(self.values.shape[0])
+
+    def frame(self, i: int) -> "FrameDeformation":
+        return FrameDeformation(self, i)
+
+
+@dataclasses.dataclass(frozen=True, eq=False)
+class FrameDeformation:
+    """Frame `index` of a DeformationGrid, for render(..., baked=BakedScene(..., deformation=grid.frame(index))).  A ray whose
+    every sample is finite and inside the grid's box takes its bends from the grid (trilinear lookup of offset and rigidity,
+    then the bender's test-time knobs: nrnerf_b200.h gives the fp32 rule); any other ray is bent by the ray bender with its
+    own latent, exactly as without the grid.  Render with frame `index`'s latent code as the rays' latents."""
+    grid: DeformationGrid
+    index: int
+
+    def __post_init__(self):
+        if not isinstance(self.grid, DeformationGrid):
+            raise RuntimeError(f"nonrigid_nerf_b200: a FrameDeformation needs a geometry.DeformationGrid, got {type(self.grid).__name__}")
+        v = self.grid.values
+        if not (isinstance(v, torch.Tensor) and v.dim() == 5):   # before the index: F is values.shape[0]
+            raise RuntimeError("nonrigid_nerf_b200: deformation grid values must be a contiguous [F, nz, ny, nx, 4] float16 tensor, "
+                               f"got {type(v).__name__}" + (f" of shape {list(v.shape)}" if isinstance(v, torch.Tensor) else ""))
+        i, n = self.index, self.grid.n_frames
+        if not isinstance(i, (int, np.integer)) or isinstance(i, bool) or not 0 <= i < n:
+            raise RuntimeError(f"nonrigid_nerf_b200: deformation frame {i!r} out of range ({n} frames)")
+
+    def c_struct(self, device) -> "_lib.NrnDeformGrid":
+        """The grid as the C ABI reads it; raises unless the values are a contiguous [F, nz, ny, nx, 4] fp16 tensor on
+        `device`, the resolution is 2..1024 vertices per axis and the box has max > min."""
+        g = self.grid
+        nx, ny, nz = _vertices(g.resolution, "deformation grid")
+        lo, hi = _extent(g.min_point, g.max_point)
+        v = g.values
+        if not (isinstance(v, torch.Tensor) and v.dtype == torch.float16 and v.dim() == 5 and tuple(v.shape[1:]) == (nz, ny, nx, 4)
+                and v.is_contiguous()):
+            raise RuntimeError(f"nonrigid_nerf_b200: deformation grid values must be a contiguous [F, {nz}, {ny}, {nx}, 4] float16 "
+                               f"tensor for resolution {g.resolution}")
+        if v.device != torch.device(device):
+            raise RuntimeError(f"nonrigid_nerf_b200: the deformation grid is on {v.device}, the rays on {device}")
+        c = _lib.NrnDeformGrid()
+        c.values, c.nx, c.ny, c.nz, c.n_frames, c.frame = v.data_ptr(), nx, ny, nz, int(v.shape[0]), int(self.index)
+        c.min_point[:] = [float(x) for x in lo]
+        c.max_point[:] = [float(x) for x in hi]
+        return c
+
+
+@dataclasses.dataclass(frozen=True, eq=False)
 class BakedScene:
     """The grids render(..., baked=scene) samples: `coarse` for the coarse pass, `fine` for the fine pass (needed when
-    N_importance > 0; bake the model that pass runs).  Not a tuple, so the ray-sharded render wrapper hands it to every
-    rank as it is."""
+    N_importance > 0; bake the model that pass runs), and optionally one frame's `deformation` (DeformationGrid.frame(i)),
+    whose bends both passes look up in place of the ray bender.  Not a tuple, so the ray-sharded render wrapper hands it
+    to every rank as it is."""
     coarse: RadianceGrid
     fine: Optional[RadianceGrid] = None
+    deformation: Optional[FrameDeformation] = None
 
 
-def _vertices(resolution):
+def _vertices(resolution, what="radiance grid"):
     r = (resolution,) * 3 if isinstance(resolution, (int, np.integer)) else resolution
     if not isinstance(r, (tuple, list)) or len(r) != 3 or any(not isinstance(n, (int, np.integer)) or isinstance(n, bool) for n in r):
         raise RuntimeError(f"nonrigid_nerf_b200: resolution must be an int or (nx, ny, nz) vertices, got {resolution!r}")
     if any(n < 2 or n > 1024 for n in r):
-        raise RuntimeError(f"nonrigid_nerf_b200: radiance grid resolution must be 2..1024 vertices on every axis, got {r}")
+        raise RuntimeError(f"nonrigid_nerf_b200: {what} resolution must be 2..1024 vertices on every axis, got {r}")
     return tuple(int(n) for n in r)
 
 
@@ -413,6 +475,48 @@ def bake_radiance(network_fn, min_point, max_point, resolution) -> RadianceGrid:
             _lib.check(lib.nrn_radiance_plane_f16(raw.data_ptr(), nx * ny, field.out_ch, values[k].data_ptr(), _stream()),
                        "radiance_plane_f16")
     return RadianceGrid(values, lo, hi, (nx, ny, nz))
+
+
+def bake_deformation(ray_bender, latents, min_point, max_point, resolution) -> DeformationGrid:
+    """The ray bender's unmasked offset and rigidity per frame, on resolution = n or (nx, ny, nz) vertices (2..1024 per
+    axis) over min_point .. max_point (density_grid's points), for render(..., baked=BakedScene(..., deformation=
+    grid.frame(i))).  latents: [F, 32] (or [32] for one frame) on the bender's device.  The bend pass of the field kernel
+    runs in point mode, one z-plane and one frame at a time, with every test-time knob off (cut-off, scaling and object
+    removal act at lookup, so one bake serves every setting); the values are stored as fp16 with round to nearest, finite
+    values saturated to +-65504 and non-finite ones kept.  Takes 8 F nx ny nz bytes of device memory."""
+    nx, ny, nz = _vertices(resolution, "deformation grid")
+    lo, hi = _extent(min_point, max_point)
+    params = list(ray_bender.parameters())
+    dev = params[0].device if params else torch.device("cpu")
+    if dev.type != "cuda":
+        raise RuntimeError("nonrigid_nerf_b200: the ray bender must be on a CUDA device (there is no CPU path)")
+    lat = latents.detach() if isinstance(latents, torch.Tensor) else torch.as_tensor(latents)
+    if lat.dim() == 1:
+        lat = lat.reshape(1, -1)
+    if lat.dim() != 2 or lat.shape[1] != ops.LATENT or lat.shape[0] < 1:
+        raise RuntimeError(f"nonrigid_nerf_b200: latents must be [F, {ops.LATENT}] or [{ops.LATENT}], got {list(lat.shape)}")
+    if lat.device != dev:
+        raise RuntimeError(f"nonrigid_nerf_b200: the latents are on {lat.device}, the ray bender on {dev}")
+    lat = lat.to(torch.float32).contiguous().clone()
+    lib = _lib.load()
+    n_frames, n = lat.shape[0], nx * ny
+    with torch.cuda.device(dev), torch.no_grad():
+        bender_pack = ops.pack_bender(ray_bender)
+        # ops.bend_points runs the bend pass alone, which reads no NeRF weights: a zero buffer stands in for the packed NeRF
+        nerf_pack = torch.zeros(lib.nrn_packed_nerf_bytes(), dtype=torch.uint8, device=dev)
+        values = torch.empty(n_frames, nz, ny, nx, 4, dtype=torch.float16, device=dev)
+        points = torch.empty(n, 3, dtype=torch.float32, device=dev)
+        offsets = torch.empty(n, 3, dtype=torch.float32, device=dev)
+        rigidity = torch.empty(n, dtype=torch.float32, device=dev)
+        workspace = torch.empty(lib.nrn_views_workspace_bytes(n, 1), dtype=torch.uint8, device=dev)
+        for k in range(nz):
+            _lib.check(lib.nrn_mesh_grid_points(lo.ctypes.data, hi.ctypes.data, nx, ny, nz, k, points.data_ptr(), _stream()),
+                       "mesh_grid_points")
+            for f in range(n_frames):
+                ops.bend_points(points, lat[f:f + 1], bender_pack, nerf_pack, offsets, rigidity, workspace)
+                _lib.check(lib.nrn_deformation_plane_f16(offsets.data_ptr(), rigidity.data_ptr(), n, values[f, k].data_ptr(), _stream()),
+                           "deformation_plane_f16")
+    return DeformationGrid(values, lo, hi, (nx, ny, nz), lat)
 
 
 # ---- host-side writers --------------------------------------------------------------------------------------------------

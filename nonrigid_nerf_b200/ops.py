@@ -360,6 +360,26 @@ def field_forward_baked(rays: torch.Tensor, z_vals: torch.Tensor, latents: Optio
     return raw, details
 
 
+def field_forward_deformed(rays: torch.Tensor, z_vals: torch.Tensor, latents: torch.Tensor, nerf_pack: torch.Tensor, bender_pack: torch.Tensor,
+                           out_ch: int, cutoff=None, scaling=None, removal=None, want_details: bool = False, grid=None,
+                           deformation=None) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
+    """field_forward_baked whose bends come from one frame of a baked deformation grid (geometry.FrameDeformation) for every
+    ray whose samples all lie inside its box; the other rays are bent by the bender with their latents and equal
+    field_forward_baked's bit for bit.  raw [N, S, out_ch] and the details for every sample."""
+    if latents is None:
+        raise RuntimeError("nonrigid_nerf_b200: ray bending needs latents")
+    a, raw, details, keep = _field_args(rays, z_vals, None, 1, latents, nerf_pack, bender_pack, out_ch, (cutoff, scaling, removal), True,
+                                        want_details)
+    dev = keep[0].device
+    g, d = grid.c_struct(dev), deformation.c_struct(dev)
+    lib = _lib.load()
+    nbytes = lib.nrn_deformed_workspace_bytes(a.n_rays, a.n_samples, out_ch, int(want_details))
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.nrn_field_forward_deformed(C.byref(a), C.byref(g), C.byref(d), _ptr(ws), nbytes), "field_forward_deformed")
+    return raw, details
+
+
 def field_forward_terminate(rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[torch.Tensor], nerf_pack: torch.Tensor,
                             bender_pack: Optional[torch.Tensor], out_ch: int, cutoff=None, scaling=None, removal=None,
                             want_details: bool = False, threshold: float = 0.0, grid=None, noise: Optional[torch.Tensor] = None
@@ -420,6 +440,27 @@ def field_forward_views(rays: Optional[torch.Tensor], z_vals: Optional[torch.Ten
     with torch.cuda.device(dev):
         _lib.check(lib.nrn_field_forward_views(C.byref(a), C.byref(v)), "field_forward_views")
     return raw, details
+
+
+def bend_points(points: torch.Tensor, latent: torch.Tensor, bender_pack: torch.Tensor, nerf_pack: torch.Tensor, offsets: torch.Tensor,
+                rigidity: torch.Tensor, workspace: torch.Tensor) -> None:
+    """The ray bender alone, knobs off, at points [P, 3] (contiguous fp32) with one latent row [1, 32]: its unmasked offsets
+    into offsets [P, 3] and its rigidity into rigidity [P] (both contiguous fp32, preallocated so that a caller looping over
+    planes allocates nothing per call).  workspace: nrn_views_workspace_bytes(P, 1) bytes.  This is the bend pass of
+    nrn_field_forward_views in point mode with raw NULL, so the view head does not run; the bend pass reads no NeRF
+    weights, but the argument block names a packed NeRF, so nerf_pack is any 16-byte aligned buffer of
+    nrn_packed_nerf_bytes() bytes."""
+    n = points.shape[0]
+    a = _lib.NrnFieldArgs()
+    a.points, a.points_stride = points.data_ptr(), 3
+    a.n_rays, a.n_samples, a.out_ch = n, 1, 4
+    a.nerf_packed, a.bender_packed = nerf_pack.data_ptr(), bender_pack.data_ptr()
+    a.latents, a.latent_stride = latent.data_ptr(), 0   # one row for every point
+    a.unmasked_offsets, a.rigidity_mask = offsets.data_ptr(), rigidity.data_ptr()
+    a.stream = torch.cuda.current_stream().cuda_stream
+    v = _lib.NrnViewArgs()
+    v.workspace = workspace.data_ptr()
+    _lib.check(_lib.load().nrn_field_forward_views(C.byref(a), C.byref(v)), "bend_points")
 
 
 def field_forward_views_train(rays: torch.Tensor, z_vals: torch.Tensor, viewdirs: torch.Tensor, nerf_pack: torch.Tensor,

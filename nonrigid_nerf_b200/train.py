@@ -105,8 +105,11 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     baked (geometry.BakedScene, under torch.no_grad() only; the reference has no such option): the coarse pass samples
     baked.coarse and the fine pass baked.fine (required when N_importance > 0) in place of the NeRF trunk for every sample
     whose bent point is finite and inside the grid's box: raw is the grid's trilinear lookup there (raw[..., 4] = 0, the
-    object removal applied) and the trunk's raw elsewhere, so a box that holds no sample renders as without it.  Not
-    combined with occupancy or early_termination.  None: the trunk evaluates every sample.
+    object removal applied) and the trunk's raw elsewhere, so a box that holds no sample renders as without it.  With
+    baked.deformation (geometry.FrameDeformation, a model with a ray bender) both passes take the bends of every ray whose
+    samples all lie inside that grid's box from it (trilinear offset and rigidity, then the test-time knobs) instead of
+    the bender; any other ray is bent by the bender exactly as without it.  Pass that frame's latent code as the rays'
+    latents.  Not combined with occupancy or early_termination.  None: the trunk evaluates every sample.
     surface_normals=True (with surface_output=True) adds ret["surface_normals"] [N, 3]: the world-space unit normal
     geometry.normals_from_gradient(geometry.density_gradient(...)) of the pass's model, with the ray's latent code, at
     the frame-space point of the median-visibility sample (the point surface_pts and surface_rigidity are taken at).
@@ -138,7 +141,7 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
 
     def field(net, z, noise, key):
         if baked is not None:
-            return _ag.field_baked(net, rays, z, latents, detailed_output, baked.coarse if key == "coarse" else baked.fine)
+            return _ag.field_baked(net, rays, z, latents, detailed_output, baked.coarse if key == "coarse" else baked.fine, baked.deformation)
         if early_termination is not None:
             raw, det, term_index[key] = _ag.field_terminate(net, rays, z, latents, detailed_output, early_termination, occupancy, noise)
             return raw, det
@@ -279,7 +282,8 @@ def _check_termination(early_termination, network_fn, network_fine, latents) -> 
 
 def _check_baked(baked, network_fn, network_fine, n_importance, latents, occupancy, early_termination):
     """Before any launch: render(..., baked=scene) is refused for what it does not support (_ag.baked_check), with occupancy
-    or early_termination, and without a fine grid when N_importance > 0."""
+    or early_termination, without a fine grid when N_importance > 0, and for a deformation that a pass's model cannot read
+    (_ag.deformation_check)."""
     from .geometry import BakedScene
     if not isinstance(baked, BakedScene):
         raise RuntimeError(f"nonrigid_nerf_b200: baked must be a geometry.BakedScene, got {type(baked).__name__}")
@@ -291,6 +295,10 @@ def _check_baked(baked, network_fn, network_fine, n_importance, latents, occupan
         if baked.fine is None:
             raise RuntimeError("nonrigid_nerf_b200: N_importance > 0 needs a fine grid (BakedScene(coarse, fine))")
         _ag.baked_check(network_fn if network_fine is None else network_fine, latents, baked.fine)
+    if baked.deformation is not None:
+        _ag.deformation_check(network_fn, baked.deformation)
+        if n_importance > 0:
+            _ag.deformation_check(network_fn if network_fine is None else network_fine, baked.deformation)
 
 
 # ---- batchify_rays / render (train.py:108-137, :326-416) --------------------------------------------
