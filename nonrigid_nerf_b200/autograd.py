@@ -31,6 +31,17 @@ def _knobs(net):
     return cutoff, scaling, removal
 
 
+def _packs(net):
+    """(cutoff, scaling, removal, nerf_pack, bender_pack, out_ch) of an inference call on `net`; the view-dependent head
+    (use_viewdirs=True, no output_linear) writes 4 channels."""
+    bender = net.ray_bender[0]
+    cutoff, scaling, removal = _knobs(net)
+    nerf_pack = ops.pack_nerf(net)
+    bender_pack = ops.pack_bender(bender) if bender is not None else None
+    out_ch = 4 if getattr(net, "use_viewdirs", False) else net.output_linear.weight.shape[0]
+    return cutoff, scaling, removal, nerf_pack, bender_pack, out_ch
+
+
 def _tc_net(net):
     """The NeRF itself when it is a time-conditioned baseline (its latents enter L0 / L5 as per-ray biases), else None.
     Like train.py:574-576 the baseline runs without ray bending."""
@@ -649,12 +660,9 @@ def field_views(net, rays, z_vals, points, latents, viewdirs, want_details, bend
     if _needs_grad(net, latents):
         raise RuntimeError("nonrigid_nerf_b200: the point-wise NeRF.forward / run_network entry is inference-only; "
                            "differentiable rendering goes through render() / render_rays()")
-    bender = net.ray_bender[0]
-    cutoff, scaling, removal = _knobs(net)
-    nerf_pack = ops.pack_nerf(net)
-    bender_pack = ops.pack_bender(bender) if bender is not None else None
+    cutoff, scaling, removal, nerf_pack, bender_pack, _ = _packs(net)
     views_pack = None if bend_only else ops.pack_views(net)
-    s = net.num_ray_samples if (points is not None and bender is not None and not bend_only) else 1
+    s = net.num_ray_samples if (points is not None and bender_pack is not None and not bend_only) else 1
     return ops.field_forward_views(rays, z_vals, points, s, latents, viewdirs, nerf_pack, bender_pack, views_pack, cutoff,
                                    scaling, removal, want_details)
 
@@ -691,29 +699,30 @@ def field(net, rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[torch
     return raw, (details if want_details else {})
 
 
+def _skip_check(net, latents, what: str, why: str) -> None:
+    """Raise for what a render pass that skips samples (`what`: "with an occupancy grid", ...) does not support: the
+    view-dependent head, the time-conditioned baseline and differentiable calls (`why` the skipped samples get no gradient)."""
+    if getattr(net, "use_viewdirs", False):
+        raise RuntimeError(f"nonrigid_nerf_b200: rendering {what} is not implemented for use_viewdirs=True")
+    if getattr(net, "time_conditioned_baseline", False):
+        raise RuntimeError(f"nonrigid_nerf_b200: rendering {what} is not implemented for time_conditioned_baseline=True")
+    if _needs_grad(net, latents):
+        raise RuntimeError(f"nonrigid_nerf_b200: rendering {what} is inference only; call render() under torch.no_grad() ({why})")
+
+
 def occupancy_check(net, latents, grid) -> None:
     """Raise, before any launch, for what render(..., occupancy=grid) does not support: the view-dependent head, the
     time-conditioned baseline and differentiable calls."""
     from .geometry import OccupancyGrid
     if not isinstance(grid, OccupancyGrid):
         raise RuntimeError(f"nonrigid_nerf_b200: occupancy must be a geometry.OccupancyGrid, got {type(grid).__name__}")
-    if getattr(net, "use_viewdirs", False):
-        raise RuntimeError("nonrigid_nerf_b200: rendering with an occupancy grid is not implemented for use_viewdirs=True")
-    if getattr(net, "time_conditioned_baseline", False):
-        raise RuntimeError("nonrigid_nerf_b200: rendering with an occupancy grid is not implemented for time_conditioned_baseline=True")
-    if _needs_grad(net, latents):
-        raise RuntimeError("nonrigid_nerf_b200: rendering with an occupancy grid is inference only; call render() under "
-                           "torch.no_grad() (skipped samples would get no gradient)")
+    _skip_check(net, latents, "with an occupancy grid", "skipped samples would get no gradient")
 
 
 def field_occupancy(net, rays, z_vals, latents, want_details, grid):
     """field_rays that evaluates the NeRF trunk only on the samples the occupancy grid keeps; raw is 0 for the others."""
     occupancy_check(net, latents, grid)
-    bender = net.ray_bender[0]
-    cutoff, scaling, removal = _knobs(net)
-    nerf_pack = ops.pack_nerf(net)
-    bender_pack = ops.pack_bender(bender) if bender is not None else None
-    out_ch = net.output_linear.weight.shape[0]
+    cutoff, scaling, removal, nerf_pack, bender_pack, out_ch = _packs(net)
     return ops.field_forward_occupancy(rays, z_vals, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details,
                                        grid)
 
@@ -747,11 +756,7 @@ def field_baked(net, rays, z_vals, latents, want_details, grid, deformation=None
     """field_rays that samples the radiance grid in place of the NeRF trunk for samples inside its box; with `deformation`
     (geometry.FrameDeformation) the bends of the rays inside its box come from that grid in place of the ray bender."""
     baked_check(net, latents, grid)
-    bender = net.ray_bender[0]
-    cutoff, scaling, removal = _knobs(net)
-    nerf_pack = ops.pack_nerf(net)
-    bender_pack = ops.pack_bender(bender) if bender is not None else None
-    out_ch = net.output_linear.weight.shape[0]
+    cutoff, scaling, removal, nerf_pack, bender_pack, out_ch = _packs(net)
     if deformation is not None:
         deformation_check(net, deformation)
         return ops.field_forward_deformed(rays, z_vals, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details,
@@ -774,13 +779,7 @@ def termination_check(net, latents, threshold) -> float:
     """Raise, before any launch, for what render(..., early_termination=t) does not support: a threshold that is not a
     finite real in [0, 1], the view-dependent head, the time-conditioned baseline and differentiable calls.  Returns t."""
     t = termination_threshold(threshold)
-    if getattr(net, "use_viewdirs", False):
-        raise RuntimeError("nonrigid_nerf_b200: rendering with early_termination is not implemented for use_viewdirs=True")
-    if getattr(net, "time_conditioned_baseline", False):
-        raise RuntimeError("nonrigid_nerf_b200: rendering with early_termination is not implemented for time_conditioned_baseline=True")
-    if _needs_grad(net, latents):
-        raise RuntimeError("nonrigid_nerf_b200: rendering with early_termination is inference only; call render() under "
-                           "torch.no_grad() (samples that are not evaluated would get no gradient)")
+    _skip_check(net, latents, "with early_termination", "samples that are not evaluated would get no gradient")
     return t
 
 
@@ -790,22 +789,14 @@ def field_terminate(net, rays, z_vals, latents, want_details, threshold, grid=No
     t = termination_check(net, latents, threshold)
     if grid is not None:
         occupancy_check(net, latents, grid)
-    bender = net.ray_bender[0]
-    cutoff, scaling, removal = _knobs(net)
-    nerf_pack = ops.pack_nerf(net)
-    bender_pack = ops.pack_bender(bender) if bender is not None else None
-    out_ch = net.output_linear.weight.shape[0]
+    cutoff, scaling, removal, nerf_pack, bender_pack, out_ch = _packs(net)
     return ops.field_forward_terminate(rays, z_vals, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details, t,
                                        grid, noise)
 
 
 def field_rays(net, rays, z_vals, latents, want_details):
     """Inference path (no stash)."""
-    bender = net.ray_bender[0]
-    cutoff, scaling, removal = _knobs(net)
-    nerf_pack = ops.pack_nerf(net)
-    bender_pack = ops.pack_bender(bender) if bender is not None else None
-    out_ch = net.output_linear.weight.shape[0]
+    cutoff, scaling, removal, nerf_pack, bender_pack, out_ch = _packs(net)
     return ops.field_forward(rays, z_vals, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details,
                              tc_net=_tc_net(net))
 
@@ -818,11 +809,7 @@ def field_points(net, pts, latents, want_details):
     if _needs_grad(net, latents):
         raise RuntimeError("nonrigid_nerf_b200: the point-wise NeRF.forward / run_network entry is inference-only; "
                            "differentiable rendering goes through render() / render_rays()")
-    bender = net.ray_bender[0]
-    cutoff, scaling, removal = _knobs(net)
-    nerf_pack = ops.pack_nerf(net)
-    bender_pack = ops.pack_bender(bender) if bender is not None else None
-    out_ch = net.output_linear.weight.shape[0]
+    cutoff, scaling, removal, nerf_pack, bender_pack, out_ch = _packs(net)
     return ops.field_forward_points(pts, latents, nerf_pack, bender_pack, out_ch, cutoff, scaling, removal, want_details,
                                     tc_net=_tc_net(net))
 

@@ -1405,6 +1405,28 @@ static bool occ_sides_ok(int nx, int ny, int nz) {
 }
 static size_t occ_block_count_bytes(long long P) { return align256(sizeof(int32_t) * ((P + nrn::kOccTile - 1) / nrn::kOccTile + 1)); }
 
+// The next `bytes` of a workspace, rounded up to 256, as a T*; w moves past them
+extern "C++" template <typename T>
+T* bump(uint8_t*& w, size_t bytes) {
+  T* p = reinterpret_cast<T*>(w);
+  w += align256(bytes);
+  return p;
+}
+
+// A grid's box as the kernels read it: lo, hi and scale = n / (hi - lo) per axis for n[d] intervals; NRN_E_INVALID unless
+// the box and its scale are finite with max > min
+static int grid_box(const float* min_point, const float* max_point, const int n[3], const char* who, float* lo, float* hi, float* scale) {
+  for (int d = 0; d < 3; ++d) {
+    const float l = min_point[d], h = max_point[d];
+    if (!(std::isfinite(l) && std::isfinite(h) && h > l)) return fail(NRN_E_INVALID, "%s: grid box must be finite with max > min on every axis", who);
+    const float ext = h - l;
+    const float sc = static_cast<float>(n[d]) / ext;
+    if (!(std::isfinite(ext) && std::isfinite(sc) && sc > 0.f)) return fail(NRN_E_INVALID, "%s: grid box extent out of fp32 range", who);
+    lo[d] = l; hi[d] = h; scale[d] = sc;
+  }
+  return NRN_OK;
+}
+
 // The grid as the kernels read it; NRN_E_INVALID for a malformed one
 static int occ_grid(const NrnOccupancyGrid* g, const char* who, nrn::OccGrid* out) {
   if (!g) return fail(NRN_E_INVALID, "%s: null grid", who);
@@ -1414,16 +1436,93 @@ static int occ_grid(const NrnOccupancyGrid* g, const char* who, nrn::OccGrid* ou
   nrn::OccGrid o{};
   o.bits = g->bits; o.nx = g->nx; o.ny = g->ny; o.nz = g->nz;
   const int n[3] = {g->nx, g->ny, g->nz};
-  for (int d = 0; d < 3; ++d) {
-    const float lo = g->min_point[d], hi = g->max_point[d];
-    if (!(std::isfinite(lo) && std::isfinite(hi) && hi > lo)) return fail(NRN_E_INVALID, "%s: grid box must be finite with max > min on every axis", who);
-    const float ext = hi - lo;
-    const float sc = static_cast<float>(n[d]) / ext;
-    if (!(std::isfinite(ext) && std::isfinite(sc) && sc > 0.f)) return fail(NRN_E_INVALID, "%s: grid box extent out of fp32 range", who);
-    o.lo[d] = lo; o.hi[d] = hi; o.scale[d] = sc;
-  }
+  const int rc = grid_box(g->min_point, g->max_point, n, who, o.lo, o.hi, o.scale);
+  if (rc) return rc;
   *out = o;
   return NRN_OK;
+}
+
+// ---- the render passes that run the trunk on some samples only: their shared refusals, buffers and trunk step ----
+// The checks every such pass makes first: check_field_args, inference only, ray mode
+static int check_fast_args(const NrnFieldArgs* a, const char* who, long long* P, int* tiles) {
+  const int rc = check_field_args(a, who, P, tiles);
+  if (rc) return rc;
+  if (a->stash || a->relu_mask) return fail(NRN_E_INVALID, "%s: inference only (stash / relu_mask must be NULL)", who);
+  if (a->points) return fail(NRN_E_INVALID, "%s: needs ray mode (rays and z_vals; points must be NULL)", who);
+  return NRN_OK;
+}
+
+// The checks after the pass's grids: at most kOccMaxPoints points and, unless the batch is empty (nothing to launch), raw
+// and a 256-byte aligned workspace of at least `need` bytes, the result of the entry's size function `sizer`
+static int check_fast_buffers(const NrnFieldArgs* a, long long P, const void* workspace, size_t workspace_bytes, size_t need,
+                              const char* sizer, const char* who) {
+  if (P > nrn::kOccMaxPoints) return fail(NRN_E_INVALID, "%s: %lld points in one pass (at most 2^31 - 1)", who, P);
+  if (P == 0) return NRN_OK;
+  if (!a->raw) return fail(NRN_E_INVALID, "%s: null raw", who);
+  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255u) || workspace_bytes < need)
+    return fail(NRN_E_INVALID, "%s: workspace null, not 256-byte aligned or smaller than %s (%zu)", who, sizer, need);
+  return NRN_OK;
+}
+
+// The buffers of the samples a pass keeps for the trunk, over `slots` lookup slots: their xyz, indices and raw, their
+// count and the compaction's block counts
+struct KeptBuffers {
+  long long slots;
+  float* xyz;
+  int32_t* idx;
+  float* raw;
+  int32_t* count;
+  int32_t* block_counts;
+};
+static size_t kept_bytes(long long slots, int out_ch) {
+  const size_t k = static_cast<size_t>(slots);
+  return align256(k * 3 * sizeof(float)) + align256(k * sizeof(int32_t)) + align256(k * out_ch * sizeof(float)) + align256(sizeof(int32_t)) +
+         occ_block_count_bytes(slots);
+}
+static KeptBuffers carve_kept(uint8_t*& w, long long slots, int out_ch) {
+  const size_t k = static_cast<size_t>(slots);
+  KeptBuffers b;
+  b.slots = slots;
+  b.xyz = bump<float>(w, k * 3 * sizeof(float));
+  b.idx = bump<int32_t>(w, k * sizeof(int32_t));
+  b.raw = bump<float>(w, k * out_ch * sizeof(float));
+  b.count = bump<int32_t>(w, sizeof(int32_t));
+  b.block_counts = bump<int32_t>(w, occ_block_count_bytes(slots));
+  return b;
+}
+
+// The lookup of a pass's samples into the kept buffers: their points in ws (from the bend pass), or without a bender from
+// the rays and depths, the compaction then also writing the details
+struct KeptLookup {
+  nrn::OccPoints s;
+  nrn::OccCompact c;
+};
+static KeptLookup kept_lookup(const NrnFieldArgs* a, long long P, const float4* ws, const KeptBuffers& k) {
+  KeptLookup l{};
+  l.s.ws = ws; l.s.rays = a->rays; l.s.z_vals = a->z_vals; l.s.S = a->n_samples; l.s.P = P;
+  l.c.kept_xyz = k.xyz; l.c.kept_idx = k.idx; l.c.count = k.count; l.c.block_counts = k.block_counts;
+  if (!ws) { l.c.d_init = a->initial_input_pts; l.c.d_bent = a->input_pts; }
+  return l;
+}
+
+// The point-mode trunk on the kept points (their count read on the device, the slots sizing its grid), timed as field_kind,
+// then their raw into the pass's output (with the object removal), timed as scatter_kind, max_kept bounding the count for
+// the scatter's grid; zero_raw: the pass's raw zeroed first, in the scatter's timing
+static int kept_trunk(const NrnFieldArgs* a, const nrn::FieldFwdParams& p0, const KeptBuffers& k, long long max_kept, const float4* ws,
+                      bool zero_raw, DeviceState* ds, int field_kind, int scatter_kind, cudaStream_t st) {
+  nrn::FieldFwdParams q{};
+  q.pts = k.xyz; q.pts_stride = 3; q.n_rays = static_cast<int>(k.slots); q.S = 1; q.P = k.slots; q.n_tiles = static_cast<int>(tile_count(k.slots));
+  q.nerf_w = p0.nerf_w; q.nerf_bias = p0.nerf_bias; q.out_ch = a->out_ch; q.raw = k.raw; q.err = ds->err_word;
+  int rc = timed(field_kind, st, "field_fwd_kept_kernel", [&] { return nrn::launch_field_fwd_kept(q, k.count, ds->num_sms, st); });
+  if (rc) return rc;
+  return timed(scatter_kind, st, "occ_scatter_kernel", [&] {
+    if (zero_raw) {
+      const cudaError_t e = cudaMemsetAsync(a->raw, 0, static_cast<size_t>(p0.P) * a->out_ch * sizeof(float), st);
+      if (e != cudaSuccess) return e;
+    }
+    return nrn::launch_occupancy_scatter(k.raw, k.idx, k.count, max_kept, a->out_ch, ws, a->use_removal, a->removal_threshold, a->raw,
+                                         ds->num_sms, st);
+  });
 }
 
 size_t nrn_occupancy_words(int nx, int ny, int nz) {
@@ -1477,42 +1576,29 @@ size_t nrn_occupancy_workspace_bytes(int n_rays, int n_samples, int out_ch, int 
   if (n_rays < 0 || n_samples < 1 || out_ch < 4 || out_ch > 5) return 0;
   const long long P = static_cast<long long>(n_rays) * n_samples;
   if (P > nrn::kOccMaxPoints) return 0;
-  const size_t p = static_cast<size_t>(P);
-  return (has_bender ? align256(p * sizeof(float4)) : 0) + align256(p * 3 * sizeof(float)) + align256(p * sizeof(int32_t)) +
-         align256(p * out_ch * sizeof(float)) + align256(sizeof(int32_t)) + occ_block_count_bytes(P);
+  return (has_bender ? align256(static_cast<size_t>(P) * sizeof(float4)) : 0) + kept_bytes(P, out_ch);
 }
 
 int nrn_field_forward_occupancy(const NrnFieldArgs* a, const NrnOccupancyGrid* grid, void* workspace, size_t workspace_bytes) {
   const char* who = "nrn_field_forward_occupancy";
   long long P;
   int tiles;
-  int rc = check_field_args(a, who, &P, &tiles);
+  int rc = check_fast_args(a, who, &P, &tiles);
   if (rc) return rc;
-  if (a->stash || a->relu_mask) return fail(NRN_E_INVALID, "%s: inference only (stash / relu_mask must be NULL)", who);
-  if (a->points) return fail(NRN_E_INVALID, "%s: needs ray mode (rays and z_vals; points must be NULL)", who);
   nrn::OccGrid g;
   rc = occ_grid(grid, who, &g);
   if (rc) return rc;
-  if (P > nrn::kOccMaxPoints) return fail(NRN_E_INVALID, "%s: %lld points in one pass (at most 2^31 - 1)", who, P);
-  if (P == 0) return NRN_OK;
   const bool bend = a->bender_packed != nullptr;
-  if (!a->raw) return fail(NRN_E_INVALID, "%s: null raw", who);
-  const size_t need = nrn_occupancy_workspace_bytes(a->n_rays, a->n_samples, a->out_ch, bend);
-  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255u) || workspace_bytes < need)
-    return fail(NRN_E_INVALID, "%s: workspace null, not 256-byte aligned or smaller than nrn_occupancy_workspace_bytes (%zu)", who, need);
+  rc = check_fast_buffers(a, P, workspace, workspace_bytes, nrn_occupancy_workspace_bytes(a->n_rays, a->n_samples, a->out_ch, bend),
+                          "nrn_occupancy_workspace_bytes", who);
+  if (rc || P == 0) return rc;
   DeviceState* ds;
   rc = device_state(&ds);
   if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(a->stream);
-  const size_t p = static_cast<size_t>(P);
   uint8_t* w = static_cast<uint8_t*>(workspace);
-  float4* ws = nullptr;
-  if (bend) { ws = reinterpret_cast<float4*>(w); w += align256(p * sizeof(float4)); }
-  float* kept_xyz = reinterpret_cast<float*>(w); w += align256(p * 3 * sizeof(float));
-  int32_t* kept_idx = reinterpret_cast<int32_t*>(w); w += align256(p * sizeof(int32_t));
-  float* craw = reinterpret_cast<float*>(w); w += align256(p * a->out_ch * sizeof(float));
-  int32_t* count = reinterpret_cast<int32_t*>(w); w += align256(sizeof(int32_t));
-  int32_t* block_counts = reinterpret_cast<int32_t*>(w);
+  float4* ws = bend ? bump<float4>(w, static_cast<size_t>(P) * sizeof(float4)) : nullptr;
+  const KeptBuffers k = carve_kept(w, P, a->out_ch);
 
   nrn::FieldFwdParams p0 = field_fwd_params(a, P, tiles, ds->err_word);
   // a. the bend pass: bent points and rigidities -> ws, and the details
@@ -1523,23 +1609,11 @@ int nrn_field_forward_occupancy(const NrnFieldArgs* a, const NrnOccupancyGrid* g
     if (rc) return rc;
   }
   // b. lookup and compaction (without a bender the points come from the rays and depths, with their details)
-  nrn::OccPoints s{};
-  s.ws = ws; s.rays = a->rays; s.z_vals = a->z_vals; s.S = a->n_samples; s.P = P;
-  nrn::OccCompact c{};
-  c.kept_xyz = kept_xyz; c.kept_idx = kept_idx; c.count = count; c.block_counts = block_counts;
-  if (!bend) { c.d_init = a->initial_input_pts; c.d_bent = a->input_pts; }
-  rc = timed(33, st, "occupancy_compact", [&] { return nrn::launch_occupancy_compact(g, s, c, st); });
+  const KeptLookup l = kept_lookup(a, P, ws, k);
+  rc = timed(33, st, "occupancy_compact", [&] { return nrn::launch_occupancy_compact(g, l.s, l.c, st); });
   if (rc) return rc;
-  // c. the point-mode trunk on the kept points, their count read on the device
-  nrn::FieldFwdParams q{};
-  q.pts = kept_xyz; q.pts_stride = 3; q.n_rays = static_cast<int>(P); q.S = 1; q.P = P; q.n_tiles = tiles;
-  q.nerf_w = p0.nerf_w; q.nerf_bias = p0.nerf_bias; q.out_ch = a->out_ch; q.raw = craw; q.err = ds->err_word;
-  rc = timed(34, st, "field_fwd_kept_kernel", [&] { return nrn::launch_field_fwd_kept(q, count, ds->num_sms, st); });
-  if (rc) return rc;
-  // d. raw of every sample: the trunk's where kept (with the object removal), zero elsewhere
-  return timed(35, st, "occupancy_scatter", [&] {
-    return nrn::launch_occupancy_scatter(craw, kept_idx, count, P, a->out_ch, ws, a->use_removal, a->removal_threshold, a->raw, ds->num_sms, st);
-  });
+  // c, d. the trunk on the kept points; raw of every sample: the trunk's where kept (with the object removal), zero elsewhere
+  return kept_trunk(a, p0, k, P, ws, true, ds, 34, 35, st);
 }
 
 // ---- early ray termination: a render pass in depth-ordered rounds over segments of nrn_termination_segment() samples ----
@@ -1549,11 +1623,8 @@ size_t nrn_termination_workspace_bytes(int n_rays, int n_samples, int out_ch, in
   if (n_rays < 0 || n_samples < 1 || out_ch < 4 || out_ch > 5) return 0;
   const long long P = static_cast<long long>(n_rays) * n_samples;
   if (P > nrn::kOccMaxPoints) return 0;
-  const size_t p = static_cast<size_t>(P);
   const long long Pk = static_cast<long long>(n_rays) * std::min(nrn::kTermSegment, n_samples);   // the slots of one round
-  const size_t pk = static_cast<size_t>(Pk);
-  return (has_bender ? align256(p * sizeof(float4)) : 0) + align256(pk * 3 * sizeof(float)) + align256(pk * sizeof(int32_t)) +
-         align256(pk * out_ch * sizeof(float)) + align256(sizeof(int32_t)) + occ_block_count_bytes(Pk) +
+  return (has_bender ? align256(static_cast<size_t>(P) * sizeof(float4)) : 0) + kept_bytes(Pk, out_ch) +
          align256(static_cast<size_t>(n_rays) * sizeof(float));
 }
 
@@ -1562,10 +1633,8 @@ int nrn_field_forward_terminate(const NrnFieldArgs* a, const NrnOccupancyGrid* g
   const char* who = "nrn_field_forward_terminate";
   long long P;
   int tiles;
-  int rc = check_field_args(a, who, &P, &tiles);
+  int rc = check_fast_args(a, who, &P, &tiles);
   if (rc) return rc;
-  if (a->stash || a->relu_mask) return fail(NRN_E_INVALID, "%s: inference only (stash / relu_mask must be NULL)", who);
-  if (a->points) return fail(NRN_E_INVALID, "%s: needs ray mode (rays and z_vals; points must be NULL)", who);
   if (!term) return fail(NRN_E_INVALID, "%s: null termination args", who);
   if (!(term->threshold >= 0.f && term->threshold <= 1.f))
     return fail(NRN_E_INVALID, "%s: early-termination threshold %g outside [0, 1]", who, static_cast<double>(term->threshold));
@@ -1574,14 +1643,11 @@ int nrn_field_forward_terminate(const NrnFieldArgs* a, const NrnOccupancyGrid* g
     rc = occ_grid(grid, who, &g);
     if (rc) return rc;
   }
-  if (P > nrn::kOccMaxPoints) return fail(NRN_E_INVALID, "%s: %lld points in one pass (at most 2^31 - 1)", who, P);
-  if (P == 0) return NRN_OK;
   const bool bend = a->bender_packed != nullptr;
-  if (!a->raw) return fail(NRN_E_INVALID, "%s: null raw", who);
+  rc = check_fast_buffers(a, P, workspace, workspace_bytes, nrn_termination_workspace_bytes(a->n_rays, a->n_samples, a->out_ch, bend),
+                          "nrn_termination_workspace_bytes", who);
+  if (rc || P == 0) return rc;
   if (!term->termination_index) return fail(NRN_E_INVALID, "%s: null termination_index", who);
-  const size_t need = nrn_termination_workspace_bytes(a->n_rays, a->n_samples, a->out_ch, bend);
-  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255u) || workspace_bytes < need)
-    return fail(NRN_E_INVALID, "%s: workspace null, not 256-byte aligned or smaller than nrn_termination_workspace_bytes (%zu)", who, need);
   DeviceState* ds;
   rc = device_state(&ds);
   if (rc) return rc;
@@ -1589,16 +1655,10 @@ int nrn_field_forward_terminate(const NrnFieldArgs* a, const NrnOccupancyGrid* g
   const int S = a->n_samples, K = std::min(nrn::kTermSegment, S);
   const size_t p = static_cast<size_t>(P);
   const long long Pk = static_cast<long long>(a->n_rays) * K;
-  const size_t pk = static_cast<size_t>(Pk);
   uint8_t* w = static_cast<uint8_t*>(workspace);
-  float4* ws = nullptr;
-  if (bend) { ws = reinterpret_cast<float4*>(w); w += align256(p * sizeof(float4)); }
-  float* kept_xyz = reinterpret_cast<float*>(w); w += align256(pk * 3 * sizeof(float));
-  int32_t* kept_idx = reinterpret_cast<int32_t*>(w); w += align256(pk * sizeof(int32_t));
-  float* craw = reinterpret_cast<float*>(w); w += align256(pk * a->out_ch * sizeof(float));
-  int32_t* count = reinterpret_cast<int32_t*>(w); w += align256(sizeof(int32_t));
-  int32_t* block_counts = reinterpret_cast<int32_t*>(w); w += occ_block_count_bytes(Pk);
-  float* T = reinterpret_cast<float*>(w);
+  float4* ws = bend ? bump<float4>(w, p * sizeof(float4)) : nullptr;
+  const KeptBuffers k = carve_kept(w, Pk, a->out_ch);
+  float* T = bump<float>(w, static_cast<size_t>(a->n_rays) * sizeof(float));
 
   nrn::FieldFwdParams p0 = field_fwd_params(a, P, tiles, ds->err_word);
   // the bend pass over every sample: bent points and rigidities -> ws, and the details
@@ -1617,30 +1677,17 @@ int nrn_field_forward_terminate(const NrnFieldArgs* a, const NrnOccupancyGrid* g
   if (rc) return rc;
   rc = timed(40, st, "term_init_kernel", [&] { return nrn::launch_termination_init(t, st); });
   if (rc) return rc;
-  nrn::OccPoints s{};
-  s.ws = ws; s.rays = a->rays; s.z_vals = a->z_vals; s.S = S; s.P = P;
-  nrn::OccCompact c{};
-  c.kept_xyz = kept_xyz; c.kept_idx = kept_idx; c.count = count; c.block_counts = block_counts;
-  if (!bend) { c.d_init = a->initial_input_pts; c.d_bent = a->input_pts; }
-  nrn::FieldFwdParams q{};
-  q.pts = kept_xyz; q.pts_stride = 3; q.n_rays = static_cast<int>(Pk); q.S = 1; q.P = Pk; q.n_tiles = static_cast<int>(tile_count(Pk));
-  q.nerf_w = p0.nerf_w; q.nerf_bias = p0.nerf_bias; q.out_ch = a->out_ch; q.raw = craw; q.err = ds->err_word;
+  const KeptLookup l = kept_lookup(a, P, ws, k);
   for (int s0 = 0; s0 < S; s0 += K) {
     const int len = std::min(K, S - s0);
     nrn::OccSegment seg{};
     seg.s0 = s0; seg.len = len; seg.P = static_cast<long long>(a->n_rays) * len; seg.term = term->termination_index;
     seg.use_grid = grid != nullptr;
     // 1. the lookup of this segment's samples: the ray alive (and the grid keeping the point), compacted in order
-    rc = timed(37, st, "termination_compact", [&] { return nrn::launch_termination_compact(g, s, seg, c, st); });
+    rc = timed(37, st, "termination_compact", [&] { return nrn::launch_termination_compact(g, l.s, seg, l.c, st); });
     if (rc) return rc;
-    // 2. the point-mode trunk on the kept points, their count read on the device
-    rc = timed(38, st, "field_fwd_kept_kernel", [&] { return nrn::launch_field_fwd_kept(q, count, ds->num_sms, st); });
-    if (rc) return rc;
-    // 3. their raw into the pass's output (with the object removal)
-    rc = timed(39, st, "occ_scatter_kernel", [&] {
-      return nrn::launch_termination_scatter(craw, kept_idx, count, seg.P, a->out_ch, ws, a->use_removal, a->removal_threshold, a->raw,
-                                             ds->num_sms, st);
-    });
+    // 2, 3. the trunk on the kept points, and their raw into the pass's output (with the object removal)
+    rc = kept_trunk(a, p0, k, seg.P, ws, false, ds, 38, 39, st);
     if (rc) return rc;
     // 4. the transmittance over the segment; rays below the threshold die
     rc = timed(40, st, "term_transmittance_kernel", [&] { return nrn::launch_termination_transmittance(t, s0, len, st); });
@@ -1667,14 +1714,9 @@ static int baked_grid(const NrnRadianceGrid* g, const char* who, nrn::BakedGrid*
   nrn::BakedGrid o{};
   o.vox = static_cast<const uint2*>(g->values);
   o.n[0] = g->nx; o.n[1] = g->ny; o.n[2] = g->nz;
-  for (int d = 0; d < 3; ++d) {
-    const float lo = g->min_point[d], hi = g->max_point[d];
-    if (!(std::isfinite(lo) && std::isfinite(hi) && hi > lo)) return fail(NRN_E_INVALID, "%s: grid box must be finite with max > min on every axis", who);
-    const float ext = hi - lo;
-    const float sc = static_cast<float>(o.n[d] - 1) / ext;
-    if (!(std::isfinite(ext) && std::isfinite(sc) && sc > 0.f)) return fail(NRN_E_INVALID, "%s: grid box extent out of fp32 range", who);
-    o.lo[d] = lo; o.hi[d] = hi; o.scale[d] = sc;
-  }
+  const int cells[3] = {g->nx - 1, g->ny - 1, g->nz - 1};
+  const int rc = grid_box(g->min_point, g->max_point, cells, who, o.lo, o.hi, o.scale);
+  if (rc) return rc;
   *out = o;
   return NRN_OK;
 }
@@ -1702,27 +1744,21 @@ int nrn_field_forward_baked(const NrnFieldArgs* a, const NrnRadianceGrid* grid, 
   const char* who = "nrn_field_forward_baked";
   long long P;
   int tiles;
-  int rc = check_field_args(a, who, &P, &tiles);
+  int rc = check_fast_args(a, who, &P, &tiles);
   if (rc) return rc;
-  if (a->stash || a->relu_mask) return fail(NRN_E_INVALID, "%s: inference only (stash / relu_mask must be NULL)", who);
-  if (a->points) return fail(NRN_E_INVALID, "%s: needs ray mode (rays and z_vals; points must be NULL)", who);
   nrn::BakedGrid bg;
   rc = baked_grid(grid, who, &bg);
   if (rc) return rc;
-  if (P > nrn::kOccMaxPoints) return fail(NRN_E_INVALID, "%s: %lld points in one pass (at most 2^31 - 1)", who, P);
-  if (P == 0) return NRN_OK;
   const bool bend = a->bender_packed != nullptr;
-  if (!a->raw) return fail(NRN_E_INVALID, "%s: null raw", who);
-  const size_t need = nrn_baked_workspace_bytes(a->n_rays, a->n_samples, a->out_ch, bend);
-  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255u) || workspace_bytes < need)
-    return fail(NRN_E_INVALID, "%s: workspace null, not 256-byte aligned or smaller than nrn_baked_workspace_bytes (%zu)", who, need);
+  rc = check_fast_buffers(a, P, workspace, workspace_bytes, nrn_baked_workspace_bytes(a->n_rays, a->n_samples, a->out_ch, bend),
+                          "nrn_baked_workspace_bytes", who);
+  if (rc || P == 0) return rc;
   DeviceState* ds;
   rc = device_state(&ds);
   if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(a->stream);
   uint8_t* w = static_cast<uint8_t*>(workspace);
-  float4* ws = nullptr;
-  if (bend) { ws = reinterpret_cast<float4*>(w); w += align256(static_cast<size_t>(P) * sizeof(float4)); }
+  float4* ws = bend ? bump<float4>(w, static_cast<size_t>(P) * sizeof(float4)) : nullptr;
   const nrn::FieldFwdParams p0 = field_fwd_params(a, P, tiles, ds->err_word);
   // a. raw of the samples inside the grid's box: with a bender from the bend pass's epilogue (which also writes the bent
   //    points and rigidities to ws, and the details), without one at rays_o + rays_d * z
@@ -1739,45 +1775,32 @@ int nrn_field_forward_baked(const NrnFieldArgs* a, const NrnRadianceGrid* grid, 
   return baked_others(a, bg, p0, ws, w, ds, 47, st);
 }
 
+// An occupancy grid of one empty cell (its word at `bits`) over the radiance grid's box: it keeps exactly the samples
+// outside the box or not finite
+static nrn::OccGrid empty_cell_grid(const nrn::BakedGrid& bg, const uint32_t* bits) {
+  nrn::OccGrid og{};
+  og.bits = bits; og.nx = og.ny = og.nz = 1;
+  for (int d = 0; d < 3; ++d) { og.lo[d] = bg.lo[d]; og.hi[d] = bg.hi[d]; og.scale[d] = 1.f / (bg.hi[d] - bg.lo[d]); }
+  return og;
+}
+
 // Steps b to d of a baked pass, after the samples inside the radiance grid's box have their raw: the other samples (their
 // points in ws, or without one at rays_o + rays_d * z) through the trunk, timed as kinds kind .. kind + 2.  w: the
 // workspace past ws, in nrn_baked_workspace_bytes's layout.
 static int baked_others(const NrnFieldArgs* a, const nrn::BakedGrid& bg, const nrn::FieldFwdParams& p0, const float4* ws, uint8_t* w,
                         DeviceState* ds, int kind, cudaStream_t st) {
-  const long long P = p0.P;
-  const size_t p = static_cast<size_t>(P);
-  float* kept_xyz = reinterpret_cast<float*>(w); w += align256(p * 3 * sizeof(float));
-  int32_t* kept_idx = reinterpret_cast<int32_t*>(w); w += align256(p * sizeof(int32_t));
-  float* craw = reinterpret_cast<float*>(w); w += align256(p * a->out_ch * sizeof(float));
-  int32_t* count = reinterpret_cast<int32_t*>(w); w += align256(sizeof(int32_t));
-  int32_t* block_counts = reinterpret_cast<int32_t*>(w); w += occ_block_count_bytes(P);
-  uint32_t* empty = reinterpret_cast<uint32_t*>(w);
-  // b. the samples outside the box or not finite, compacted in order: exactly those an occupancy grid of one empty cell
-  //    over the same box keeps (without a bender this step also writes the details)
-  nrn::OccGrid og{};
-  og.bits = empty; og.nx = og.ny = og.nz = 1;
-  for (int d = 0; d < 3; ++d) { og.lo[d] = bg.lo[d]; og.hi[d] = bg.hi[d]; og.scale[d] = 1.f / (bg.hi[d] - bg.lo[d]); }
-  nrn::OccPoints s{};
-  s.ws = ws; s.rays = a->rays; s.z_vals = a->z_vals; s.S = a->n_samples; s.P = P;
-  nrn::OccCompact c{};
-  c.kept_xyz = kept_xyz; c.kept_idx = kept_idx; c.count = count; c.block_counts = block_counts;
-  if (!ws) { c.d_init = a->initial_input_pts; c.d_bent = a->input_pts; }
+  const KeptBuffers k = carve_kept(w, p0.P, a->out_ch);
+  uint32_t* empty = bump<uint32_t>(w, sizeof(uint32_t));
+  // b. the samples outside the box or not finite, compacted in order (without a bender this step also writes the details)
+  const nrn::OccGrid og = empty_cell_grid(bg, empty);
+  const KeptLookup l = kept_lookup(a, p0.P, ws, k);
   int rc = timed(kind, st, "occupancy_compact", [&] {
     const cudaError_t e = cudaMemsetAsync(empty, 0, sizeof(uint32_t), st);
-    return e != cudaSuccess ? e : nrn::launch_occupancy_compact(og, s, c, st);
+    return e != cudaSuccess ? e : nrn::launch_occupancy_compact(og, l.s, l.c, st);
   });
   if (rc) return rc;
-  // c. the point-mode trunk on them, their count read on the device
-  nrn::FieldFwdParams q{};
-  q.pts = kept_xyz; q.pts_stride = 3; q.n_rays = static_cast<int>(P); q.S = 1; q.P = P; q.n_tiles = p0.n_tiles;
-  q.nerf_w = p0.nerf_w; q.nerf_bias = p0.nerf_bias; q.out_ch = a->out_ch; q.raw = craw; q.err = ds->err_word;
-  rc = timed(kind + 1, st, "field_fwd_kept_kernel", [&] { return nrn::launch_field_fwd_kept(q, count, ds->num_sms, st); });
-  if (rc) return rc;
-  // d. their raw into the pass's output (with the object removal), beside the grid's
-  return timed(kind + 2, st, "occ_scatter_kernel", [&] {
-    return nrn::launch_termination_scatter(craw, kept_idx, count, P, a->out_ch, ws, a->use_removal, a->removal_threshold, a->raw,
-                                           ds->num_sms, st);
-  });
+  // c, d. the trunk on them, and their raw into the pass's output (with the object removal), beside the grid's
+  return kept_trunk(a, p0, k, p0.P, ws, false, ds, kind + 1, kind + 2, st);
 }
 
 // ---- baked per-frame deformation grids: the bake's plane store, and the render pass that looks each sample's bend up ----
@@ -1824,25 +1847,20 @@ int nrn_field_forward_deformed(const NrnFieldArgs* a, const NrnRadianceGrid* gri
   const char* who = "nrn_field_forward_deformed";
   long long P;
   int tiles;
-  int rc = check_field_args(a, who, &P, &tiles);
+  int rc = check_fast_args(a, who, &P, &tiles);
   if (rc) return rc;
-  if (a->stash || a->relu_mask) return fail(NRN_E_INVALID, "%s: inference only (stash / relu_mask must be NULL)", who);
-  if (a->points) return fail(NRN_E_INVALID, "%s: needs ray mode (rays and z_vals; points must be NULL)", who);
   nrn::BakedGrid bg, dg;
   rc = baked_grid(grid, who, &bg);
   if (rc) return rc;
   rc = deform_grid(deform, "nrn_field_forward_deformed: deformation grid", &dg);
   if (rc) return rc;
-  if (P > nrn::kOccMaxPoints) return fail(NRN_E_INVALID, "%s: %lld points in one pass (at most 2^31 - 1)", who, P);
-  if (P == 0) return NRN_OK;
+  const bool det = a->initial_input_pts || a->input_pts || a->unmasked_offsets || a->masked_offsets || a->rigidity_mask;
+  rc = check_fast_buffers(a, P, workspace, workspace_bytes, nrn_deformed_workspace_bytes(a->n_rays, a->n_samples, a->out_ch, det),
+                          "nrn_deformed_workspace_bytes", who);
+  if (rc || P == 0) return rc;
   if (!a->bender_packed) return fail(NRN_E_INVALID, "%s: a deformation grid needs the ray bender (bender_packed, for the rays that fall back)", who);
-  if (!a->raw) return fail(NRN_E_INVALID, "%s: null raw", who);
   if (!aligned4(a->rays) || !aligned4(a->z_vals) || !aligned4(a->latents) || !aligned4(a->raw))
     return fail(NRN_E_INVALID, "%s: rays, z_vals, latents and raw must be 4-byte aligned", who);
-  const bool det = a->initial_input_pts || a->input_pts || a->unmasked_offsets || a->masked_offsets || a->rigidity_mask;
-  const size_t need = nrn_deformed_workspace_bytes(a->n_rays, a->n_samples, a->out_ch, det);
-  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255u) || workspace_bytes < need)
-    return fail(NRN_E_INVALID, "%s: workspace null, not 256-byte aligned or smaller than nrn_deformed_workspace_bytes (%zu)", who, need);
   DeviceState* ds;
   rc = device_state(&ds);
   if (rc) return rc;
@@ -1850,27 +1868,29 @@ int nrn_field_forward_deformed(const NrnFieldArgs* a, const NrnRadianceGrid* gri
   const int n = a->n_rays, S = a->n_samples;
   const size_t p = static_cast<size_t>(P);
   uint8_t* w = static_cast<uint8_t*>(workspace);
-  float4* ws = reinterpret_cast<float4*>(w);
-  uint8_t* rest = w + align256(p * sizeof(float4));   // baked_others' part
-  w += nrn_baked_workspace_bytes(n, S, a->out_ch, 1);
+  float4* ws = bump<float4>(w, p * sizeof(float4));
+  uint8_t* rest = w;   // baked_others' part
+  w = static_cast<uint8_t*>(workspace) + nrn_baked_workspace_bytes(n, S, a->out_ch, 1);
   nrn::DeformFallback f{};
-  f.flag = w; w += align256(static_cast<size_t>(n));
-  f.block_counts = reinterpret_cast<int32_t*>(w); w += occ_block_count_bytes(n);
-  f.count = reinterpret_cast<int32_t*>(w); w += align256(sizeof(int32_t));
-  f.idx = reinterpret_cast<int32_t*>(w); w += align256(static_cast<size_t>(n) * sizeof(int32_t));
-  f.rays = reinterpret_cast<float*>(w); w += align256(static_cast<size_t>(n) * 8 * sizeof(float));
-  f.latents = reinterpret_cast<float*>(w); w += align256(static_cast<size_t>(n) * nrn::kLatent * sizeof(float));
-  f.z_vals = reinterpret_cast<float*>(w); w += align256(p * sizeof(float));
-  float4* bw = reinterpret_cast<float4*>(w); w += align256(p * sizeof(float4));
+  f.flag = bump<uint8_t>(w, static_cast<size_t>(n));
+  f.block_counts = bump<int32_t>(w, occ_block_count_bytes(n));
+  f.count = bump<int32_t>(w, sizeof(int32_t));
+  f.idx = bump<int32_t>(w, static_cast<size_t>(n) * sizeof(int32_t));
+  f.rays = bump<float>(w, static_cast<size_t>(n) * 8 * sizeof(float));
+  f.latents = bump<float>(w, static_cast<size_t>(n) * nrn::kLatent * sizeof(float));
+  f.z_vals = bump<float>(w, p * sizeof(float));
+  float4* bw = bump<float4>(w, p * sizeof(float4));
   nrn::DeformOut out{ws, a->raw, a->out_ch, a->initial_input_pts, a->input_pts, a->unmasked_offsets, a->masked_offsets, a->rigidity_mask};
   nrn::DeformOut gathered{bw, nullptr, a->out_ch, nullptr, nullptr, nullptr, nullptr, nullptr};   // the bend pass's, per gathered sample
   float** gd[4] = {&gathered.d_init, &gathered.d_bent, &gathered.d_unmasked, &gathered.d_masked};
   float* const od[4] = {out.d_init, out.d_bent, out.d_unmasked, out.d_masked};
-  for (int i = 0; i < 4; ++i) {
-    if (det && od[i]) *gd[i] = reinterpret_cast<float*>(w);
-    if (det) w += align256(p * 3 * sizeof(float));
+  if (det) {
+    for (int i = 0; i < 4; ++i) {
+      float* d = bump<float>(w, p * 3 * sizeof(float));
+      if (od[i]) *gd[i] = d;
+    }
+    if (out.d_rigid) gathered.d_rigid = bump<float>(w, p * sizeof(float));
   }
-  if (det && out.d_rigid) gathered.d_rigid = reinterpret_cast<float*>(w);
   nrn::DeformKnobs k{};
   k.use_cutoff = a->use_cutoff; k.cutoff = a->rigidity_cutoff; k.use_scaling = a->use_scaling; k.scaling = a->scaling;
   k.use_removal = a->use_removal; k.removal = a->removal_threshold;

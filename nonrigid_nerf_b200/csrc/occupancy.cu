@@ -277,11 +277,14 @@ cudaError_t launch_occupancy_compact(const OccGrid& g, const OccPoints& pts, con
   return cudaGetLastError();
 }
 
-cudaError_t launch_occupancy_scatter(const float* compact_raw, const int32_t* kept_idx, const int32_t* count, long long P, int out_ch,
+// max_kept bounds the count the kernel reads from device memory: it sizes the grid
+cudaError_t launch_occupancy_scatter(const float* compact_raw, const int32_t* kept_idx, const int32_t* count, long long max_kept, int out_ch,
                                      const float4* ws, int use_removal, float removal, float* raw, int num_sms, cudaStream_t st) {
-  cudaError_t e = cudaMemsetAsync(raw, 0, static_cast<size_t>(P) * out_ch * sizeof(float), st);
-  if (e != cudaSuccess) return e;
-  return launch_termination_scatter(compact_raw, kept_idx, count, P, out_ch, ws, use_removal, removal, raw, num_sms, st);
+  const long long cap = static_cast<long long>(num_sms) * 16;
+  const long long nb = blocks_for(max_kept, kOccThreads);
+  occ_scatter_kernel<<<static_cast<unsigned>(nb < cap ? nb : cap), kOccThreads, 0, st>>>(compact_raw, kept_idx, count, out_ch, ws, use_removal,
+                                                                                        removal, raw);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_occupancy_scan(int32_t* counts, int n, int32_t* count, cudaStream_t st) {
@@ -299,16 +302,6 @@ cudaError_t launch_termination_compact(const OccGrid& g, const OccPoints& pts, c
   if (nb > 0) occ_count_seg_kernel<<<nb, kOccTile, 0, st>>>(g, pts, seg, c.block_counts);
   occ_scan_kernel<<<1, kOccTile, 0, st>>>(c.block_counts, static_cast<int>(nb), c.count);
   if (nb > 0) occ_write_seg_kernel<<<nb, kOccTile, 0, st>>>(g, pts, seg, c);
-  return cudaGetLastError();
-}
-
-// max_kept bounds the count the kernel reads from device memory: it sizes the grid
-cudaError_t launch_termination_scatter(const float* compact_raw, const int32_t* kept_idx, const int32_t* count, long long max_kept, int out_ch,
-                                       const float4* ws, int use_removal, float removal, float* raw, int num_sms, cudaStream_t st) {
-  const long long cap = static_cast<long long>(num_sms) * 16;
-  const long long nb = blocks_for(max_kept, kOccThreads);
-  occ_scatter_kernel<<<static_cast<unsigned>(nb < cap ? nb : cap), kOccThreads, 0, st>>>(compact_raw, kept_idx, count, out_ch, ws, use_removal,
-                                                                                          removal, raw);
   return cudaGetLastError();
 }
 

@@ -79,23 +79,21 @@ struct TermPass {
 cudaError_t launch_occupancy_build(const float* sigma, int nx, int ny, int nz, float threshold, int dilation, uint8_t* ws,
                                    uint32_t* bits, cudaStream_t st);
 cudaError_t launch_occupancy_compact(const OccGrid& g, const OccPoints& pts, const OccCompact& c, cudaStream_t st);
-// raw [P][out_ch] (zeroed first) <- compact_raw [K][out_ch] at the kept indices; with ws and use_removal, alpha *= 0 where
-// the point's rigidity >= removal (the fused kernel's test-time object removal)
-cudaError_t launch_occupancy_scatter(const float* compact_raw, const int32_t* kept_idx, const int32_t* count, long long P, int out_ch,
+// raw[kept_idx[k]] <- compact_raw [k][out_ch] for k < K = *count <= max_kept; raw elsewhere is left as it is (a pass zeroes
+// it first).  With ws and use_removal, alpha *= 0 where the point's rigidity >= removal (the fused kernel's test-time object
+// removal).
+cudaError_t launch_occupancy_scatter(const float* compact_raw, const int32_t* kept_idx, const int32_t* count, long long max_kept, int out_ch,
                                      const float4* ws, int use_removal, float removal, float* raw, int num_sms, cudaStream_t st);
 // The exclusive scan of n per-block counts in place (one block), the total -> counts[n] and *count: the middle step of the
 // compaction above, for other per-block counts (baked.cu's fallback rays)
 cudaError_t launch_occupancy_scan(int32_t* counts, int n, int32_t* count, cudaStream_t st);
 
 // Early termination (nrn_field_forward_terminate).  init: T = 1 and term = S for every ray.  compact: the lookup and
-// compaction of one segment's slots (kept indices are the samples' indices in the pass, so the scatter takes them as they
-// are).  scatter: launch_occupancy_scatter without zeroing raw first (the pass zeroes it once).  transmittance: every
-// alive ray multiplies T by (1 - alpha + 1e-10) over samples [s0, s0 + len), in order, and dies (term = s0 + len) when
-// T < threshold.
+// compaction of one segment's slots (kept indices are the samples' indices in the pass, so launch_occupancy_scatter takes
+// them as they are).  transmittance: every alive ray multiplies T by (1 - alpha + 1e-10) over samples [s0, s0 + len), in
+// order, and dies (term = s0 + len) when T < threshold.
 cudaError_t launch_termination_init(const TermPass& t, cudaStream_t st);
 cudaError_t launch_termination_compact(const OccGrid& g, const OccPoints& pts, const OccSegment& seg, const OccCompact& c, cudaStream_t st);
-cudaError_t launch_termination_scatter(const float* compact_raw, const int32_t* kept_idx, const int32_t* count, long long max_kept, int out_ch,
-                                       const float4* ws, int use_removal, float removal, float* raw, int num_sms, cudaStream_t st);
 cudaError_t launch_termination_transmittance(const TermPass& t, int s0, int len, cudaStream_t st);
 
 }  // namespace nrn

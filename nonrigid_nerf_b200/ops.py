@@ -321,23 +321,32 @@ def field_forward_points(points: torch.Tensor, latents: Optional[torch.Tensor], 
                   tc_net=tc_net)
 
 
+def _fast_pass(entry: str, sizer: str, size_flag: int, rays, z_vals, latents, nerf_pack, bender_pack, out_ch, knobs, want_details,
+               structs, needs_latents: bool = False):
+    """Run the render pass `entry` (nrn_field_forward_<entry>) with the workspace nrn_<sizer>_workspace_bytes(n, S, out_ch,
+    size_flag) asks for: latents are passed with a bender, or always when needs_latents.  structs(a, dev): the C structs
+    (or None) that follow NrnFieldArgs.  Returns (raw, details)."""
+    if latents is None and (needs_latents or bender_pack is not None):
+        raise RuntimeError("nonrigid_nerf_b200: ray bending needs latents")
+    a, raw, details, keep = _field_args(rays, z_vals, None, 1, latents if needs_latents or bender_pack is not None else None, nerf_pack,
+                                        bender_pack, out_ch, knobs, True, want_details)
+    dev = keep[0].device
+    args = [C.byref(x) if x is not None else None for x in structs(a, dev)]
+    lib = _lib.load()
+    nbytes = getattr(lib, f"nrn_{sizer}_workspace_bytes")(a.n_rays, a.n_samples, out_ch, size_flag)
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(getattr(lib, f"nrn_field_forward_{entry}")(C.byref(a), *args, _ptr(ws), nbytes), f"field_forward_{entry}")
+    return raw, details
+
+
 def field_forward_occupancy(rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[torch.Tensor], nerf_pack: torch.Tensor,
                             bender_pack: Optional[torch.Tensor], out_ch: int, cutoff=None, scaling=None, removal=None,
                             want_details: bool = False, grid=None) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
     """field_forward (inference) that runs the NeRF trunk only on samples the occupancy grid keeps (geometry.OccupancyGrid):
     raw [N, S, out_ch] equal to field_forward's where kept and 0 elsewhere; the details for every sample."""
-    if bender_pack is not None and latents is None:
-        raise RuntimeError("nonrigid_nerf_b200: ray bending needs latents")
-    a, raw, details, keep = _field_args(rays, z_vals, None, 1, latents if bender_pack is not None else None, nerf_pack, bender_pack,
-                                        out_ch, (cutoff, scaling, removal), True, want_details)
-    dev = keep[0].device
-    g = grid.c_struct(dev)
-    lib = _lib.load()
-    nbytes = lib.nrn_occupancy_workspace_bytes(a.n_rays, a.n_samples, out_ch, int(bender_pack is not None))
-    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.nrn_field_forward_occupancy(C.byref(a), C.byref(g), _ptr(ws), nbytes), "field_forward_occupancy")
-    return raw, details
+    return _fast_pass("occupancy", "occupancy", int(bender_pack is not None), rays, z_vals, latents, nerf_pack, bender_pack,
+                      out_ch, (cutoff, scaling, removal), want_details, lambda a, dev: [grid.c_struct(dev)])
 
 
 def field_forward_baked(rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[torch.Tensor], nerf_pack: torch.Tensor,
@@ -346,18 +355,8 @@ def field_forward_baked(rays: torch.Tensor, z_vals: torch.Tensor, latents: Optio
     """field_forward (inference) that samples the radiance grid (geometry.RadianceGrid) in place of the NeRF trunk for
     samples whose (bent) point lies inside its box: raw [N, S, out_ch] from the lookup there (raw[..., 4] = 0), equal to
     field_forward's elsewhere; the details for every sample."""
-    if bender_pack is not None and latents is None:
-        raise RuntimeError("nonrigid_nerf_b200: ray bending needs latents")
-    a, raw, details, keep = _field_args(rays, z_vals, None, 1, latents if bender_pack is not None else None, nerf_pack, bender_pack,
-                                        out_ch, (cutoff, scaling, removal), True, want_details)
-    dev = keep[0].device
-    g = grid.c_struct(dev)
-    lib = _lib.load()
-    nbytes = lib.nrn_baked_workspace_bytes(a.n_rays, a.n_samples, out_ch, int(bender_pack is not None))
-    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.nrn_field_forward_baked(C.byref(a), C.byref(g), _ptr(ws), nbytes), "field_forward_baked")
-    return raw, details
+    return _fast_pass("baked", "baked", int(bender_pack is not None), rays, z_vals, latents, nerf_pack, bender_pack, out_ch,
+                      (cutoff, scaling, removal), want_details, lambda a, dev: [grid.c_struct(dev)])
 
 
 def field_forward_deformed(rays: torch.Tensor, z_vals: torch.Tensor, latents: torch.Tensor, nerf_pack: torch.Tensor, bender_pack: torch.Tensor,
@@ -366,18 +365,9 @@ def field_forward_deformed(rays: torch.Tensor, z_vals: torch.Tensor, latents: to
     """field_forward_baked whose bends come from one frame of a baked deformation grid (geometry.FrameDeformation) for every
     ray whose samples all lie inside its box; the other rays are bent by the bender with their latents and equal
     field_forward_baked's bit for bit.  raw [N, S, out_ch] and the details for every sample."""
-    if latents is None:
-        raise RuntimeError("nonrigid_nerf_b200: ray bending needs latents")
-    a, raw, details, keep = _field_args(rays, z_vals, None, 1, latents, nerf_pack, bender_pack, out_ch, (cutoff, scaling, removal), True,
-                                        want_details)
-    dev = keep[0].device
-    g, d = grid.c_struct(dev), deformation.c_struct(dev)
-    lib = _lib.load()
-    nbytes = lib.nrn_deformed_workspace_bytes(a.n_rays, a.n_samples, out_ch, int(want_details))
-    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.nrn_field_forward_deformed(C.byref(a), C.byref(g), C.byref(d), _ptr(ws), nbytes), "field_forward_deformed")
-    return raw, details
+    return _fast_pass("deformed", "deformed", int(want_details), rays, z_vals, latents, nerf_pack, bender_pack, out_ch,
+                      (cutoff, scaling, removal), want_details, lambda a, dev: [grid.c_struct(dev), deformation.c_struct(dev)],
+                      needs_latents=True)
 
 
 def field_forward_terminate(rays: torch.Tensor, z_vals: torch.Tensor, latents: Optional[torch.Tensor], nerf_pack: torch.Tensor,
@@ -389,27 +379,24 @@ def field_forward_terminate(rays: torch.Tensor, z_vals: torch.Tensor, latents: O
     `threshold`; with `grid` (geometry.OccupancyGrid) a sample is also skipped where the grid would skip it.  noise [N, S]:
     the sigma noise compositing will add (already scaled), or None.  Returns raw [N, S, out_ch] (field_forward's where
     evaluated, 0 elsewhere), the details for every sample, and termination_index [N] int32."""
-    if bender_pack is not None and latents is None:
-        raise RuntimeError("nonrigid_nerf_b200: ray bending needs latents")
-    a, raw, details, keep = _field_args(rays, z_vals, None, 1, latents if bender_pack is not None else None, nerf_pack, bender_pack,
-                                        out_ch, (cutoff, scaling, removal), True, want_details)
-    dev = keep[0].device
-    g = grid.c_struct(dev) if grid is not None else None
-    t = _lib.NrnTerminationArgs()
-    t.threshold = float(threshold)
-    if noise is not None:
-        noise = _f32c(noise, "noise")
-        if tuple(noise.shape) != (a.n_rays, a.n_samples):
-            raise RuntimeError(f"nonrigid_nerf_b200: noise must be [{a.n_rays}, {a.n_samples}], got {list(noise.shape)}")
-        t.noise = noise.data_ptr()
-    term = torch.empty(a.n_rays, dtype=torch.int32, device=dev)
-    t.termination_index = term.data_ptr()
-    lib = _lib.load()
-    nbytes = lib.nrn_termination_workspace_bytes(a.n_rays, a.n_samples, out_ch, int(bender_pack is not None))
-    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.nrn_field_forward_terminate(C.byref(a), C.byref(g) if g is not None else None, C.byref(t), _ptr(ws), nbytes),
-                   "field_forward_terminate")
+    term = noise_rows = None
+
+    def structs(a, dev):
+        nonlocal term, noise_rows
+        g = grid.c_struct(dev) if grid is not None else None
+        t = _lib.NrnTerminationArgs()
+        t.threshold = float(threshold)
+        if noise is not None:
+            noise_rows = _f32c(noise, "noise")
+            if tuple(noise_rows.shape) != (a.n_rays, a.n_samples):
+                raise RuntimeError(f"nonrigid_nerf_b200: noise must be [{a.n_rays}, {a.n_samples}], got {list(noise_rows.shape)}")
+            t.noise = noise_rows.data_ptr()
+        term = torch.empty(a.n_rays, dtype=torch.int32, device=dev)
+        t.termination_index = term.data_ptr()
+        return [g, t]
+
+    raw, details = _fast_pass("terminate", "termination", int(bender_pack is not None), rays, z_vals, latents, nerf_pack, bender_pack,
+                              out_ch, (cutoff, scaling, removal), want_details, structs)
     return raw, details, term
 
 

@@ -131,12 +131,7 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     latents = None
     if network_fn.ray_bender[0] is not None or getattr(network_fn, "time_conditioned_baseline", False):
         latents = additional_pixel_information["ray_bending_latents"]
-    if baked is not None:
-        _check_baked(baked, network_fn, network_fine, N_importance, latents, occupancy, early_termination)
-    if occupancy is not None:
-        _check_occupancy(occupancy, network_fn, network_fine if N_importance > 0 else None, latents)
-    if early_termination is not None:
-        early_termination = _check_termination(early_termination, network_fn, network_fine if N_importance > 0 else None, latents)
+    early_termination = _check_fast_paths(occupancy, early_termination, baked, network_fn, network_fine, N_importance, latents)
     term_index = {}
 
     def field(net, z, noise, key):
@@ -263,20 +258,21 @@ def _check_views(batch_has_viewdirs, network_fn, network_fine, additional_pixel_
         _ag.views_check(net, info.get("ray_bending_latents"))
 
 
-def _check_occupancy(occupancy, network_fn, network_fine, latents):
-    """Before any launch: render(..., occupancy=grid) is refused for what it does not support (_ag.occupancy_check)."""
-    for net in (network_fn, network_fine):
-        if net is not None:
+def _check_fast_paths(occupancy, early_termination, baked, network_fn, network_fine, n_importance, latents):
+    """Before any launch: render(..., occupancy=, early_termination=, baked=) is refused for what they do not support
+    (_check_baked, _ag.occupancy_check, _ag.termination_check); returns the early-termination threshold as a float, or
+    None."""
+    if baked is not None:
+        _check_baked(baked, network_fn, network_fine, n_importance, latents, occupancy, early_termination)
+    nets = [net for net in (network_fn, network_fine if n_importance > 0 else None) if net is not None]
+    if occupancy is not None:
+        for net in nets:
             _ag.occupancy_check(net, latents, occupancy)
-
-
-def _check_termination(early_termination, network_fn, network_fine, latents) -> float:
-    """Before any launch: render(..., early_termination=t) is refused for what it does not support
-    (_ag.termination_check); returns t as a float."""
+    if early_termination is None:
+        return None
     t = _ag.termination_threshold(early_termination)
-    for net in (network_fn, network_fine):
-        if net is not None:
-            _ag.termination_check(net, latents, t)
+    for net in nets:
+        _ag.termination_check(net, latents, t)
     return t
 
 
@@ -321,21 +317,13 @@ def render(rays_o, rays_d, chunk=1024 * 32, ndc=True, near=0.0, far=1.0, use_vie
     """Render rays.  Returns [rgb_map, disp_map, acc_map, extras] (train.py:326-416).  Keyword held_out [N] (one entry
     per ray of the flattened batch), keyword occupancy (a geometry.OccupancyGrid), keyword early_termination (a float
     in [0, 1]) and keyword baked (a geometry.BakedScene): see render_rays."""
-    if kwargs.get("network_fn") is not None and kwargs.get("baked") is not None:
-        _check_baked(kwargs["baked"], kwargs["network_fn"], kwargs.get("network_fine"), kwargs.get("N_importance", 0),
-                     (additional_pixel_information or {}).get("ray_bending_latents"), kwargs.get("occupancy"),
-                     kwargs.get("early_termination"))
-    if kwargs.get("early_termination") is not None:
-        t = _ag.termination_threshold(kwargs["early_termination"])
-        if kwargs.get("network_fn") is not None:
-            _check_termination(t, kwargs["network_fn"], kwargs.get("network_fine") if kwargs.get("N_importance", 0) > 0 else None,
-                               (additional_pixel_information or {}).get("ray_bending_latents"))
-    if kwargs.get("network_fn") is not None and kwargs.get("occupancy") is not None:
-        _check_occupancy(kwargs["occupancy"], kwargs["network_fn"], kwargs.get("network_fine") if kwargs.get("N_importance", 0) > 0 else None,
-                         (additional_pixel_information or {}).get("ray_bending_latents"))
     if kwargs.get("network_fn") is not None:
+        _check_fast_paths(kwargs.get("occupancy"), kwargs.get("early_termination"), kwargs.get("baked"), kwargs["network_fn"],
+                          kwargs.get("network_fine"), kwargs.get("N_importance", 0), (additional_pixel_information or {}).get("ray_bending_latents"))
         _check_views(bool(use_viewdirs), kwargs["network_fn"], kwargs.get("network_fine") if kwargs.get("N_importance", 0) > 0 else None,
                      additional_pixel_information)
+    elif kwargs.get("early_termination") is not None:
+        _ag.termination_threshold(kwargs["early_termination"])
     viewdirs = None
     if use_viewdirs:   # provide ray directions as input (train.py:364-381)
         if c2w_staticcam is not None:
