@@ -19,82 +19,11 @@
 // max|d_raw| (no host sync); WGRAD and the latent reduction divide it out again in fp32.
 // field_bwd_views_kernel (view-dependent head, no bender): Rgb^T, ViewsF^T and Feature^T + head^T in front of L7^T.
 // field_bwd_held_kernel (bender, held-out rays): the same chain; the gradient-stash rows of held-out rays' points are zero.
-#include "field_mma.cuh"
+#include "field_epilogue.cuh"
 
 namespace nrn {
 
 namespace {
-
-constexpr int kBwdStageLd = 66;   // floats per staged row (64 used)
-// Gradient images in shared memory: only the bender chain's (A operands of B4^T..B0^T, at most 96 columns).  The trunk's
-// 256-wide gradients stay in registers (epi_grad_frag), so the rest of shared memory goes to the weight ring.
-constexpr int kBwdActBytes = kGsYb1.chunks * kChunkBytes;   // 24 KB
-static_assert(kGsYb4.chunks <= kGsYb1.chunks && kGsYb3.chunks <= kGsYb1.chunks && kGsYb2.chunks <= kGsYb1.chunks &&
-              kGsYb0.chunks <= kGsYb1.chunks, "bender gradient images fit act");
-constexpr int kBwdRingStages = 5;
-constexpr size_t kBwdSmemBytes = kBwdActBytes + kBwdRingStages * kRingStageBytes + 2 * kWgRows * kBwdStageLd * sizeof(float) +
-                                 sizeof(RingShared<kBwdRingStages>) + 64;
-static_assert(kBwdSmemBytes <= 227 * 1024, "DGRAD kernel: dynamic shared memory per block");
-
-static_assert(dgrad::step(dgrad::L6T) == dgrad::step(dgrad::L7T) && dgrad::step(dgrad::L5hT) == dgrad::step(dgrad::L7T) &&
-              dgrad::step(dgrad::L4T) == dgrad::step(dgrad::L7T) && dgrad::step(dgrad::L3T) == dgrad::step(dgrad::L7T) &&
-              dgrad::step(dgrad::L2T) == dgrad::step(dgrad::L7T) && dgrad::step(dgrad::L1T) == dgrad::step(dgrad::L7T),
-              "step_at: one default shape; the consumers run L5h^T .. L1^T as one loop");
-constexpr uint32_t kSlabA = 2 * dgrad::step(dgrad::L4T).k16 * kChunkBytes;   // A operand bytes of one weight slab
-
-// step -> shape for a run-time step index: a switch over immediate table entries (no table in memory)
-__device__ __forceinline__ Step step_at(int step) {
-  switch (step) {
-    case dgrad::HeadT: return step_imm<dgrad::HeadT>();
-    case dgrad::L5eT: return step_imm<dgrad::L5eT>();
-    case dgrad::L0T: return step_imm<dgrad::L0T>();
-    case dgrad::B4T: return step_imm<dgrad::B4T>();
-    case dgrad::B3T: return step_imm<dgrad::B3T>();
-    case dgrad::B2T: return step_imm<dgrad::B2T>();
-    case dgrad::B1T: return step_imm<dgrad::B1T>();
-    case dgrad::B0T: return step_imm<dgrad::B0T>();
-    default: return step_imm<dgrad::L7T>();   // L7^T, L6^T, L5h^T, L4^T .. L1^T
-  }
-}
-
-__device__ __forceinline__ float clamp_h(float v) { return fminf(fmaxf(v, -65504.f), 65504.f); }
-
-// dY = dh * [h > 0]: accumulator columns [0, NCOLS), masked with the forward's ReLU mask bits `m` (loaded before the
-// step's MMAs), written as fp16 to this warpgroup's rows of the next A operand `img`; the whole image then goes to the
-// gradient stash with bulk TMA stores.
-template <int NCOLS, int NR>
-__device__ __forceinline__ void epi_mask_store(const float (&acc)[NR], const ReluMask<NCOLS>& m, uint8_t* img, int g) {
-  const int r0 = g * kWgRows + acc_r0(), q = acc_q();
-#pragma unroll
-  for (int j = 0; j < NCOLS / 8; ++j) {
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      // saturating convert, then multiply by the 0/1 mask on packed halves
-      const uint32_t g2 = pack_h2_sat(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-      *reinterpret_cast<uint32_t*>(img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = m.apply(i, j, g2);
-    }
-  }
-}
-
-// The same for a gradient that stays in registers: NCOLS accumulator columns as fp16 (MASK: dY = dh * [h > 0] with the
-// forward's ReLU mask bits `m`) -> the next step's A fragments `a` (wg_gemm_rs), and the same fp16 pairs straight to this
-// warpgroup's rows of the tile's gradient-stash image `gs_img` (a warp's 32 words of one column group and row half are one
-// contiguous 128-byte line of the chunk-major image).
-template <int NCOLS, bool MASK, int NR>
-__device__ __forceinline__ void epi_grad_frag(const float (&acc)[NR], const ReluMask<NCOLS>& m, uint32_t (&a)[NCOLS / 16][4],
-                                              uint8_t* gs_img, int g) {
-  const int r0 = g * kWgRows + acc_r0(), q = acc_q();
-#pragma unroll
-  for (int j = 0; j < NCOLS / 8; ++j) {
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      uint32_t g2 = pack_h2_sat(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-      if constexpr (MASK) g2 = m.apply(i, j, g2);
-      frag_pair(a, j, i) = g2;
-      *reinterpret_cast<uint32_t*>(gs_img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = g2;
-    }
-  }
-}
 
 // A = d_raw [4 channels, 0 ...] (K = 16) of this warpgroup's rows, times the loss scale and clamped to fp16: one register
 // fragment built from global memory (lanes q < 2 hold columns 2q, 2q + 1 of rows r0, r0 + 8; every other word is zero,
@@ -165,29 +94,6 @@ __device__ __forceinline__ void store_row_held(uint8_t* gs, Image im, const uint
   }
 }
 
-// Backward of the positional encoding: dx_d += dE[d] + sum_k 2^k (dE[sin_kd] cos_kd - dE[cos_kd] sin_kd)
-// de: this row's 64 staged accumulator columns; sin/cos: the forward embedding stashed as fp16.
-__device__ __forceinline__ void pe_backward(const float* de, const uint8_t* __restrict__ e_row, float (&dx)[3]) {
-  float e[64];
-#pragma unroll
-  for (int c = 0; c < 8; ++c) {
-    const uint4 w = __ldg(reinterpret_cast<const uint4*>(e_row + c * kChunkBytes));
-    e[c * 8 + 0] = h_lo(w.x); e[c * 8 + 1] = h_hi(w.x); e[c * 8 + 2] = h_lo(w.y); e[c * 8 + 3] = h_hi(w.y);
-    e[c * 8 + 4] = h_lo(w.z); e[c * 8 + 5] = h_hi(w.z); e[c * 8 + 6] = h_lo(w.w); e[c * 8 + 7] = h_hi(w.w);
-  }
-#pragma unroll
-  for (int d = 0; d < 3; ++d) {
-    float acc = de[d];
-#pragma unroll
-    for (int k = 0; k < 10; ++k) {
-      const float f = static_cast<float>(1 << k);
-      const float s = e[3 + 6 * k + d], c = e[3 + 6 * k + 3 + d];
-      acc += f * (de[3 + 6 * k + d] * c - de[3 + 6 * k + 3 + d] * s);
-    }
-    dx[d] += acc;
-  }
-}
-
 // step -> shape in the view-head DGRAD's streaming order Rgb^T, ViewsF^T, Feature^T, head^T, L7^T, L6^T, L5h^T .. L1^T
 static_assert(vdgrad::step(vdgrad::FeatureT) == dgrad::step(dgrad::L7T), "step_at_views: Feature^T has the trunk's shape");
 __device__ __forceinline__ Step step_at_views(int step) {
@@ -229,7 +135,7 @@ __device__ __forceinline__ void field_bwd_body(const FieldBwdParams& p, float* l
   if (warp >= 8) {
     setmaxnreg_dec<kProducerRegs>();
     // ===================== weight producer (W^T images) =====================
-    if (warp == 8 && lane == 0) produce(p.nerf_wT, p.bend_wT, p.n_tiles, 0, HAS_BENDER ? dgrad::kCount : dgrad::B4T, dgrad::B4T, step_at, ring, W);
+    if (warp == 8 && lane == 0) produce(p.nerf_wT, p.bend_wT, p.n_tiles, 0, HAS_BENDER ? dgrad::kCount : dgrad::B4T, dgrad::B4T, dgrad_step_at, ring, W);
     return;
   }
 

@@ -33,143 +33,11 @@
 // deformation grid as well, the bend pass runs only on the rays that fall back to the exact bender, gathered, with their
 // count read on the device.
 #include "baked.cuh"
-#include "field_mma.cuh"
+#include "field_epilogue.cuh"
 
 namespace nrn {
 
 namespace {
-
-constexpr int kFwdStageLd = 12;   // floats per staged row (8 used)
-// Activations in shared memory: the bender's hidden images (A operands of B1..B4, at most 96 columns) and E.  The trunk's
-// 256-wide activations stay in registers (epi_bias_frag), so the rest of shared memory goes to the weight ring.
-constexpr int kFwdHBytes = kStHb1.chunks * kChunkBytes;   // 24 KB
-static_assert(kStHb2.chunks <= kStHb1.chunks && kStHb3.chunks <= kStHb1.chunks && kStHb4.chunks <= kStHb1.chunks, "bender images fit H");
-constexpr int kFwdRingStages = 5;
-constexpr size_t kFwdSmemBytes = kFwdHBytes + kEBytes + kFwdRingStages * kRingStageBytes + 2 * kWgRows * kFwdStageLd * sizeof(float) +
-                                 sizeof(RingShared<kFwdRingStages>) + 64;
-static_assert(kFwdSmemBytes <= 227 * 1024, "forward kernel: dynamic shared memory per block");
-
-static_assert(fwd::step(fwd::L2) == fwd::step(fwd::L1) && fwd::step(fwd::L3) == fwd::step(fwd::L1) &&
-              fwd::step(fwd::L4) == fwd::step(fwd::L1) && fwd::step(fwd::L6) == fwd::step(fwd::L1) &&
-              fwd::step(fwd::L7) == fwd::step(fwd::L1), "step_at: one default shape");
-// step -> shape for a run-time step index: a switch over immediate table entries (no table in memory)
-__device__ __forceinline__ Step step_at(int step) {
-  switch (step) {
-    case fwd::B0: return step_imm<fwd::B0>();
-    case fwd::B1: return step_imm<fwd::B1>();
-    case fwd::B2: return step_imm<fwd::B2>();
-    case fwd::B3: return step_imm<fwd::B3>();
-    case fwd::B4: return step_imm<fwd::B4>();
-    case fwd::L0: return step_imm<fwd::L0>();
-    case fwd::L5: return step_imm<fwd::L5>();
-    case fwd::Head: return step_imm<fwd::Head>();
-    default: return step_imm<fwd::L1>();   // L1-L4, L6, L7: one shape
-  }
-}
-// Accumulator columns [0, NCOLS) + bias, ReLU, fp16 -> this warpgroup's rows of the chunk-major image `img`.  MASK
-// (training kernel): also the ReLU mask bits of those elements -> this thread's words of the tile's mask image at
-// byte `mask_off` of `mask_tile`.
-template <int NCOLS, bool MASK, int NR>
-__device__ __forceinline__ void epi_bias_relu_store(const float (&acc)[NR], const float* __restrict__ bias, uint8_t* img, int g,
-                                                    uint8_t* mask_tile, int mask_off) {
-  const int r0 = g * kWgRows + acc_r0(), q = acc_q();
-  ReluMask<NCOLS> m;
-  if constexpr (MASK) m.clear();
-#pragma unroll
-  for (int j = 0; j < NCOLS / 8; ++j) {
-    const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * q));
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      // one cvt.rn.relu.satfinite.f16x2 per two outputs: ReLU, clamp to fp16 range and pack in a single instruction
-      const uint32_t h2 = pack_h2_relu_sat(acc[4 * j + 2 * i] + b.x, acc[4 * j + 2 * i + 1] + b.y);
-      *reinterpret_cast<uint32_t*>(img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = h2;
-      if constexpr (MASK) m.pack(i, j, h2);
-    }
-  }
-  if constexpr (MASK) m.store(mask_tile + mask_off, g);
-}
-
-// The same for a layer whose output stays in registers: accumulator columns [0, NCOLS) + bias (RELU: then ReLU), fp16
-// with saturation -> the next step's A fragments `a`.  TRAIN: also the fp16 pairs straight to this warpgroup's rows of the
-// tile's stash image `st_img` (a warp's 32 words of one column group and row half are one contiguous 128-byte line of the
-// chunk-major image), and with RELU the mask bits of those elements -> this thread's words of the tile's mask image
-// `mask_img`.  ROW_BIAS (time-conditioned L0 / L5): accumulator rows r0 and r0 + 8 take their biases from their own rows
-// `bias` and `bias8` (their rays' ray-bias rows) instead of one vector.
-template <int NCOLS, bool RELU, bool TRAIN, bool ROW_BIAS = false>
-__device__ __forceinline__ void epi_bias_frag(const float (&acc)[NCOLS / 2], const float* __restrict__ bias, uint32_t (&a)[NCOLS / 16][4],
-                                              uint8_t* st_img, int g, uint8_t* mask_img = nullptr,
-                                              const float* __restrict__ bias8 = nullptr) {
-  const int r0 = g * kWgRows + acc_r0(), q = acc_q();
-  ReluMask<NCOLS> m;
-  if constexpr (TRAIN && RELU) m.clear();
-#pragma unroll
-  for (int j = 0; j < NCOLS / 8; ++j) {
-    const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * q));
-    float2 b8 = b;
-    if constexpr (ROW_BIAS) b8 = __ldg(reinterpret_cast<const float2*>(bias8 + 8 * j + 2 * q));
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const float2 bi = i ? b8 : b;
-      const float u = acc[4 * j + 2 * i] + bi.x, v = acc[4 * j + 2 * i + 1] + bi.y;
-      const uint32_t h2 = RELU ? pack_h2_relu_sat(u, v) : pack_h2_sat(u, v);
-      frag_pair(a, j, i) = h2;
-      if constexpr (TRAIN) {
-        if constexpr (RELU) m.pack(i, j, h2);
-        *reinterpret_cast<uint32_t*>(st_img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = h2;
-      }
-    }
-  }
-  if constexpr (TRAIN && RELU) m.store(mask_img, g);
-}
-
-// The floats f as fp16 -> chunks 0 .. NF / 8 - 1 of a chunk-major image row
-template <int NF>
-__device__ __forceinline__ void pack_row(const float (&f)[NF], uint8_t* dst_row) {
-  static_assert(NF % 8 == 0, "whole 8-column chunks");
-#pragma unroll
-  for (int c = 0; c < NF / 8; ++c) {
-    uint4 pk;
-    pk.x = pack_h2(f[c * 8 + 0], f[c * 8 + 1]);
-    pk.y = pack_h2(f[c * 8 + 2], f[c * 8 + 3]);
-    pk.z = pack_h2(f[c * 8 + 4], f[c * 8 + 5]);
-    pk.w = pack_h2(f[c * 8 + 6], f[c * 8 + 7]);
-    *reinterpret_cast<uint4*>(dst_row + c * kChunkBytes) = pk;
-  }
-}
-
-// Positional encoding of one point (Embedder.embed, run_nerf_helpers.py:149-150 with the settings of
-// get_embedder :157-164: raw xyz first, then per octave sin(2^k xyz), cos(2^k xyz); k = 0..9).
-// Written as fp16 chunks 0..7 of the row (63 features + one zero pad column).
-// sin/cos: the argument 2^k * x is reduced EXACTLY to [-0.5, 0.5) turns (x / 2pi carried as a
-// two-float value), then evaluated with MUFU (abs err ~4e-7), well below fp16 resolution.
-// The encoding of NF octaves, [x, sin(2^k x), cos(2^k x)] for k < NF, as floats f[0, 3 + 6 NF).
-template <int NF, int NR>
-__device__ __forceinline__ void encode_octaves(const float (&x)[3], float (&f)[NR]) {
-  f[0] = x[0]; f[1] = x[1]; f[2] = x[2];
-  const float kInv2PiHi = 0.15915494f;      // fl(1/2pi)
-  const float kInv2PiLo = 6.4206199e-09f;   // 1/2pi - fl(1/2pi)
-#pragma unroll
-  for (int d = 0; d < 3; ++d) {
-    const float thi = x[d] * kInv2PiHi;
-    const float tlo = fmaf(x[d], kInv2PiLo, fmaf(x[d], kInv2PiHi, -thi));
-#pragma unroll
-    for (int k = 0; k < NF; ++k) {
-      const float sc = static_cast<float>(1 << k);
-      const float a = thi * sc;
-      const float ph = (a - rintf(a)) + tlo * sc;
-      const float ang = ph * 6.2831853071795865f;
-      f[3 + 6 * k + d] = __sinf(ang);
-      f[3 + 6 * k + 3 + d] = __cosf(ang);
-    }
-  }
-}
-
-__device__ __forceinline__ void write_pe(const float (&x)[3], uint8_t* dst_row) {
-  float f[64];
-  encode_octaves<10>(x, f);
-  f[63] = 1.f;  // pad column: its weight column is zero (forward unaffected); WGRAD reads it as the bias input
-  pack_row(f, dst_row);
-}
 
 // Direction encoding of the view-dependent head (embeddirs_fn, get_embedder(multires_views = 4): d, then sin(2^k d),
 // cos(2^k d) for k = 0..3, the same turn reduction as write_pe) as fp16 chunks 0..3 of the row: 27 columns + 5 zero.
@@ -235,7 +103,7 @@ __device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p, const Vi
     if (warp == 8 && lane == 0) {
       if constexpr (PART == kViews) produce(p.nerf_w, v.w, p.n_tiles, fwd::L0, views::kEnd, views::Feature, step_at_views, ring, W);
       else produce(p.bend_w, p.nerf_w, p.n_tiles, HAS_BENDER ? fwd::B0 : fwd::L0, PART == kBend || PART == kBaked ? fwd::L0 : fwd::kCount, fwd::L0,
-                   step_at, ring, W);
+                   fwd_step_at, ring, W);
     }
     return;
   }
@@ -301,21 +169,7 @@ __device__ __forceinline__ void field_fwd_body(const FieldFwdParams& p, const Vi
     if (HAS_BENDER) {
       // ---- bender input row: [xyz_hi(3) xyz_lo(3) latent(32) 0(10)] fp16, chunks 0..5 of E ----
       sw.begin();
-      if (row_thread) {
-        float in[48];
-#pragma unroll
-        for (int d = 0; d < 3; ++d) {
-          const float hi = __half2float(__float2half_rn(x[d]));
-          in[d] = hi;
-          in[3 + d] = x[d] - hi;
-        }
-        const float* lat = p.latents + ray * p.latent_stride;
-#pragma unroll
-        for (int i = 0; i < kLatent; ++i) in[6 + i] = valid ? __ldg(lat + i) : 0.f;
-#pragma unroll
-        for (int i = 38; i < 48; ++i) in[i] = 0.f;
-        pack_row(in, e_row);
-      }
+      if (row_thread) write_bender_input(x, p.latents + ray * p.latent_stride, valid, e_row);
       sw.ready(kStBin, Es);
       // ---- B0, B1: 96 hidden units (64 offset | 32 rigidity) ----
       {

@@ -10,189 +10,13 @@
 //                          B4^T .. B0^T, whose xyz columns add (d bent / d x)^T dx.  No gradient stash, no WGRAD, no latent
 //                          reduction.
 // The kernels are their own bodies rather than flags of field_fwd_body / field_bwd_body, so that the training and
-// inference kernels keep their machine code.  The shared helpers below are those of field_fwd.cu and field_bwd.cu
-// restricted to what these kernels use.
-#include "field_mma.cuh"
+// inference kernels keep their machine code.  They share those bodies' layouts, step tables, encodings and epilogues
+// (field_epilogue.cuh), so their mask bits and E are the training forward's.
+#include "field_epilogue.cuh"
 
 namespace nrn {
 
 namespace {
-
-// ---- forward (field_fwd.cu's shared-memory layout) ----
-constexpr int kFwdStageLd = 12;
-constexpr int kFwdHBytes = kStHb1.chunks * kChunkBytes;   // bender images
-constexpr int kFwdRingStages = 5;
-constexpr size_t kFwdSmemBytes = kFwdHBytes + kEBytes + kFwdRingStages * kRingStageBytes + 2 * kWgRows * kFwdStageLd * sizeof(float) +
-                                 sizeof(RingShared<kFwdRingStages>) + 64;
-static_assert(kFwdSmemBytes <= 227 * 1024, "point-gradient forward: dynamic shared memory per block");
-
-__device__ __forceinline__ Step fwd_step_at(int step) {
-  switch (step) {
-    case fwd::B0: return step_imm<fwd::B0>();
-    case fwd::B1: return step_imm<fwd::B1>();
-    case fwd::B2: return step_imm<fwd::B2>();
-    case fwd::B3: return step_imm<fwd::B3>();
-    case fwd::B4: return step_imm<fwd::B4>();
-    case fwd::L0: return step_imm<fwd::L0>();
-    case fwd::L5: return step_imm<fwd::L5>();
-    default: return step_imm<fwd::L1>();   // L1-L4, L6, L7: one shape
-  }
-}
-
-// Accumulator columns [0, NCOLS) + bias, ReLU, fp16 -> this warpgroup's rows of the chunk-major image `img`, and the ReLU
-// mask bits of those elements -> the tile's mask image at byte `mask_off` of `mask_tile`
-template <int NCOLS, int NR>
-__device__ __forceinline__ void epi_bias_relu_mask(const float (&acc)[NR], const float* __restrict__ bias, uint8_t* img, int g,
-                                                   uint8_t* mask_tile, int mask_off) {
-  const int r0 = g * kWgRows + acc_r0(), q = acc_q();
-  ReluMask<NCOLS> m;
-  m.clear();
-#pragma unroll
-  for (int j = 0; j < NCOLS / 8; ++j) {
-    const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * q));
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const uint32_t h2 = pack_h2_relu_sat(acc[4 * j + 2 * i] + b.x, acc[4 * j + 2 * i + 1] + b.y);
-      *reinterpret_cast<uint32_t*>(img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = h2;
-      m.pack(i, j, h2);
-    }
-  }
-  m.store(mask_tile + mask_off, g);
-}
-
-// A trunk layer whose output stays in registers: columns + bias (rows r0 / r0 + 8 from `bias` / `bias8`), ReLU, fp16 ->
-// the next step's A fragments `a`, and the mask bits -> `mask_img`
-template <int NCOLS>
-__device__ __forceinline__ void epi_bias_relu_frag(const float (&acc)[NCOLS / 2], const float* __restrict__ bias,
-                                                   const float* __restrict__ bias8, uint32_t (&a)[NCOLS / 16][4], int g,
-                                                   uint8_t* mask_img) {
-  const int q = acc_q();
-  ReluMask<NCOLS> m;
-  m.clear();
-#pragma unroll
-  for (int j = 0; j < NCOLS / 8; ++j) {
-    const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * q));
-    const float2 b8 = __ldg(reinterpret_cast<const float2*>(bias8 + 8 * j + 2 * q));
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const float2 bi = i ? b8 : b;
-      const uint32_t h2 = pack_h2_relu_sat(acc[4 * j + 2 * i] + bi.x, acc[4 * j + 2 * i + 1] + bi.y);
-      frag_pair(a, j, i) = h2;
-      m.pack(i, j, h2);
-    }
-  }
-  m.store(mask_img, g);
-}
-
-template <int NF>
-__device__ __forceinline__ void pack_row(const float (&f)[NF], uint8_t* dst_row) {
-  static_assert(NF % 8 == 0, "whole 8-column chunks");
-#pragma unroll
-  for (int c = 0; c < NF / 8; ++c) {
-    uint4 pk;
-    pk.x = pack_h2(f[c * 8 + 0], f[c * 8 + 1]);
-    pk.y = pack_h2(f[c * 8 + 2], f[c * 8 + 3]);
-    pk.z = pack_h2(f[c * 8 + 4], f[c * 8 + 5]);
-    pk.w = pack_h2(f[c * 8 + 6], f[c * 8 + 7]);
-    *reinterpret_cast<uint4*>(dst_row + c * kChunkBytes) = pk;
-  }
-}
-
-// The positional encoding exactly as field_fwd.cu's write_pe computes it (the same turn reduction and MUFU sin / cos),
-// so that E, and with it every mask bit, is the forward kernel's
-__device__ __forceinline__ void write_pe(const float (&x)[3], uint8_t* dst_row) {
-  float f[64];
-  f[0] = x[0]; f[1] = x[1]; f[2] = x[2];
-  const float kInv2PiHi = 0.15915494f;
-  const float kInv2PiLo = 6.4206199e-09f;
-#pragma unroll
-  for (int d = 0; d < 3; ++d) {
-    const float thi = x[d] * kInv2PiHi;
-    const float tlo = fmaf(x[d], kInv2PiLo, fmaf(x[d], kInv2PiHi, -thi));
-#pragma unroll
-    for (int k = 0; k < 10; ++k) {
-      const float sc = static_cast<float>(1 << k);
-      const float a = thi * sc;
-      const float ph = (a - rintf(a)) + tlo * sc;
-      const float ang = ph * 6.2831853071795865f;
-      f[3 + 6 * k + d] = __sinf(ang);
-      f[3 + 6 * k + 3 + d] = __cosf(ang);
-    }
-  }
-  f[63] = 1.f;
-  pack_row(f, dst_row);
-}
-
-// ---- DGRAD (field_bwd.cu's shared-memory layout) ----
-constexpr int kBwdStageLd = 66;
-constexpr int kBwdActBytes = kGsYb1.chunks * kChunkBytes;
-constexpr int kBwdRingStages = 5;
-constexpr size_t kBwdSmemBytes = kBwdActBytes + kBwdRingStages * kRingStageBytes + 2 * kWgRows * kBwdStageLd * sizeof(float) +
-                                 sizeof(RingShared<kBwdRingStages>) + 64;
-static_assert(kBwdSmemBytes <= 227 * 1024, "point-gradient DGRAD: dynamic shared memory per block");
-constexpr uint32_t kSlabA = 2 * dgrad::step(dgrad::L4T).k16 * kChunkBytes;
-
-__device__ __forceinline__ Step bwd_step_at(int step) {
-  switch (step) {
-    case dgrad::HeadT: return step_imm<dgrad::HeadT>();
-    case dgrad::L5eT: return step_imm<dgrad::L5eT>();
-    case dgrad::L0T: return step_imm<dgrad::L0T>();
-    case dgrad::B4T: return step_imm<dgrad::B4T>();
-    case dgrad::B3T: return step_imm<dgrad::B3T>();
-    case dgrad::B2T: return step_imm<dgrad::B2T>();
-    case dgrad::B1T: return step_imm<dgrad::B1T>();
-    case dgrad::B0T: return step_imm<dgrad::B0T>();
-    default: return step_imm<dgrad::L7T>();
-  }
-}
-
-__device__ __forceinline__ float clamp_h(float v) { return fminf(fmaxf(v, -65504.f), 65504.f); }
-
-// dY = dh * [h > 0] with the forward's mask bits -> this warpgroup's rows of the next A operand `img` (bender steps)
-template <int NCOLS, int NR>
-__device__ __forceinline__ void epi_mask_store(const float (&acc)[NR], const ReluMask<NCOLS>& m, uint8_t* img, int g) {
-  const int r0 = g * kWgRows + acc_r0(), q = acc_q();
-#pragma unroll
-  for (int j = 0; j < NCOLS / 8; ++j) {
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const uint32_t g2 = pack_h2_sat(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-      *reinterpret_cast<uint32_t*>(img + j * kChunkBytes + (r0 + 8 * i) * 16 + 4 * q) = m.apply(i, j, g2);
-    }
-  }
-}
-
-// The same for a trunk gradient that stays in registers: -> the next step's A fragments `a`
-template <int NR>
-__device__ __forceinline__ void epi_mask_frag(const float (&acc)[NR], const ReluMask<kMaskHCols>& m, uint32_t (&a)[kMaskHCols / 16][4]) {
-#pragma unroll
-  for (int j = 0; j < kMaskHCols / 8; ++j) {
-#pragma unroll
-    for (int i = 0; i < 2; ++i) frag_pair(a, j, i) = m.apply(i, j, pack_h2_sat(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]));
-  }
-}
-
-// Backward of the positional encoding (field_bwd.cu): dx_d += dE[d] + sum_k 2^k (dE[sin_kd] cos_kd - dE[cos_kd] sin_kd)
-__device__ __forceinline__ void pe_backward(const float* de, const uint8_t* __restrict__ e_row, float (&dx)[3]) {
-  float e[64];
-#pragma unroll
-  for (int c = 0; c < 8; ++c) {
-    const uint4 w = __ldg(reinterpret_cast<const uint4*>(e_row + c * kChunkBytes));
-    e[c * 8 + 0] = h_lo(w.x); e[c * 8 + 1] = h_hi(w.x); e[c * 8 + 2] = h_lo(w.y); e[c * 8 + 3] = h_hi(w.y);
-    e[c * 8 + 4] = h_lo(w.z); e[c * 8 + 5] = h_hi(w.z); e[c * 8 + 6] = h_lo(w.w); e[c * 8 + 7] = h_hi(w.w);
-  }
-#pragma unroll
-  for (int d = 0; d < 3; ++d) {
-    float acc = de[d];
-#pragma unroll
-    for (int k = 0; k < 10; ++k) {
-      const float f = static_cast<float>(1 << k);
-      const float s = e[3 + 6 * k + d], c = e[3 + 6 * k + 3 + d];
-      acc += f * (de[3 + 6 * k + d] * c - de[3 + 6 * k + 3 + d] * s);
-    }
-    dx[d] += acc;
-  }
-}
 
 // head^T's A operand: d raw = e_3 times the loss scale for every point of the tile, rows past P zero (lanes q = 1 hold
 // columns 2, 3 of rows r0, r0 + 8)
@@ -280,39 +104,25 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_grad_kernel(const Fi
     if constexpr (HAS_BENDER) {
       // ---- bender input row [xyz_hi(3) xyz_lo(3) latent(32) 0(10)] -> E ----
       sw.begin();
-      if (row_thread) {
-        float in[48];
-#pragma unroll
-        for (int d = 0; d < 3; ++d) {
-          const float hi = __half2float(__float2half_rn(x[d]));
-          in[d] = hi;
-          in[3 + d] = x[d] - hi;
-        }
-        const float* lat = p.latents + pt * p.latent_stride;
-#pragma unroll
-        for (int i = 0; i < kLatent; ++i) in[6 + i] = valid ? __ldg(lat + i) : 0.f;
-#pragma unroll
-        for (int i = 38; i < 48; ++i) in[i] = 0.f;
-        pack_row(in, e_row);
-      }
+      if (row_thread) write_bender_input(x, p.latents + pt * p.latent_stride, valid, e_row);
       sw.ready(kNone, Es);
       float rigidity = 0.f;
       {
         Acc<fwd::B0> acc;
         wg_gemm_step<fwd::B0>(acc, ring, [&](uint32_t) { return a_e; }, W, 401);
         sw.begin();
-        epi_bias_relu_mask<kMkHb1.cols>(acc, p.bend_bias + fwd::b_off(fwd::B0), Hs, g, mk, kMkHb1.off);
+        epi_bias_relu_store<kMkHb1.cols, true>(acc, p.bend_bias + fwd::b_off(fwd::B0), Hs, g, mk, kMkHb1.off);
         sw.ready(kNone, Hs);
         wg_gemm_step<fwd::B1>(acc, ring, [&](uint32_t) { return a_h; }, W, 402);
         sw.begin();
-        epi_bias_relu_mask<kMkHb2.cols>(acc, p.bend_bias + fwd::b_off(fwd::B1), Hs, g, mk, kMkHb2.off);
+        epi_bias_relu_store<kMkHb2.cols, true>(acc, p.bend_bias + fwd::b_off(fwd::B1), Hs, g, mk, kMkHb2.off);
         sw.ready(kNone, Hs);
       }
       {
         Acc<fwd::B2> acc;
         wg_gemm_step<fwd::B2>(acc, ring, [&](uint32_t) { return a_h; }, W, 403);
         sw.begin();
-        epi_bias_relu_mask<kMkHb3.cols>(acc, p.bend_bias + fwd::b_off(fwd::B2), Hs, g, mk, kMkHb3.off);
+        epi_bias_relu_store<kMkHb3.cols, true>(acc, p.bend_bias + fwd::b_off(fwd::B2), Hs, g, mk, kMkHb3.off);
         if (acc_q() == 0) {
           stg[acc_r0() * kFwdStageLd] = acc[32];
           stg[(acc_r0() + 8) * kFwdStageLd] = acc[34];
@@ -328,7 +138,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_grad_kernel(const Fi
         Acc<fwd::B3> acc;
         wg_gemm_step<fwd::B3>(acc, ring, [&](uint32_t) { return a_h; }, W, 404);
         sw.begin();
-        epi_bias_relu_mask<kMkHb4.cols>(acc, p.bend_bias + fwd::b_off(fwd::B3), Hs, g, mk, kMkHb4.off);
+        epi_bias_relu_store<kMkHb4.cols, true>(acc, p.bend_bias + fwd::b_off(fwd::B3), Hs, g, mk, kMkHb4.off);
         sw.ready(kNone, Hs);
       }
       {   // ---- B4: offsets; bend = x + rigidity * unmasked (* scaling), rounded as field_fwd.cu does ----
@@ -377,7 +187,9 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_fwd_grad_kernel(const Fi
         b = rb + ray_r0 * p.ray_bias_stride;
         b8 = rb + ray_r8 * p.ray_bias_stride;
       }
-      epi_bias_relu_frag<kMaskHCols>(acc, b, b8, h, g, mk + kMkH + L * kMaskHBytes);
+      // the mask bits and no stash; one epilogue for every layer, with b8 = b outside LATENT_BIAS's L0 / L5
+      epi_bias_frag<kMaskHCols, /*RELU*/ true, /*TRAIN*/ true, /*ROW_BIAS*/ true, /*STASH*/ false>(acc, b, h, nullptr, g,
+                                                                                                mk + kMkH + L * kMaskHBytes, b8);
     }
   }
   if (wg_leader) tma_bulk_wait<0>();   // the E stores complete before the CTA exits
@@ -406,7 +218,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_grad_kernel(const Fi
 
   if (warp >= 8) {
     setmaxnreg_dec<kProducerRegs>();
-    if (warp == 8 && lane == 0) produce(p.nerf_wT, p.bend_wT, p.n_tiles, 0, HAS_BENDER ? dgrad::kCount : dgrad::B4T, dgrad::B4T, bwd_step_at, ring, W);
+    if (warp == 8 && lane == 0) produce(p.nerf_wT, p.bend_wT, p.n_tiles, 0, HAS_BENDER ? dgrad::kCount : dgrad::B4T, dgrad::B4T, dgrad_step_at, ring, W);
     return;
   }
 
@@ -441,7 +253,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_grad_kernel(const Fi
       ReluMask<kMaskHCols> m;
       m.load(mk + kMkH + 7 * kMaskHBytes, g);
       wg_gemm_rs<kTrunk.N, 1>(acc, a, ring, false, 0u, W, 500);
-      epi_mask_frag(acc, m, h);
+      epi_grad_frag<kMaskHCols, true, /*STASH*/ false>(acc, m, h, nullptr, g);
     }
     float dx[3] = {0.f, 0.f, 0.f};
 #pragma unroll 1
@@ -450,7 +262,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_grad_kernel(const Fi
       ReluMask<kMaskHCols> m;
       m.load(mk + kMkH + (6 - s) * kMaskHBytes, g);
       wg_gemm_rs<kTrunk.N, kTrunk.k16>(acc, h, ring, false, 0u, W, 501 + s);
-      epi_mask_frag(acc, m, h);
+      epi_grad_frag<kMaskHCols, true, /*STASH*/ false>(acc, m, h, nullptr, g);
     }
     {   // ---- L5e^T: gradient into the skip-connected embedding ----
       Acc<dgrad::L5eT> acc;
@@ -466,7 +278,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) field_bwd_grad_kernel(const Fi
       ReluMask<kMaskHCols> m;
       m.load(mk + kMkH + (4 - s) * kMaskHBytes, g);
       wg_gemm_rs<kTrunk.N, kTrunk.k16>(acc, h, ring, false, 0u, W, 504 + s);
-      epi_mask_frag(acc, m, h);
+      epi_grad_frag<kMaskHCols, true, /*STASH*/ false>(acc, m, h, nullptr, g);
     }
     {   // ---- L0^T: gradient into the embedding ----
       Acc<dgrad::L0T> acc;

@@ -160,7 +160,7 @@ def test_against_fp64_on_the_kernels_masks(kind):
 @pytest.mark.parametrize("kind", KINDS)
 def test_forward_matches_the_training_forward(kind):
     """field_fwd_grad_kernel's mask bits, encoding E, offsets and rigidity equal the training forward's (field_fwd.cu)
-    for the same points, bit for bit: the encoding and mask epilogues field_grad.cu restates stay those of field_fwd.cu."""
+    for the same points, bit for bit: the encoding and mask epilogues field_grad.cu shares stay those of field_fwd.cu."""
     net = _model(kind)
     n = 1000
     x, z = _points(n), _latent(kind)
